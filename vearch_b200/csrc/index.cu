@@ -1403,7 +1403,7 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
     GB_ALLOC(d_out, unsigned long long, nout, s);
     GB_CUDA(cudaMemsetAsync(d_tau, 0xFF, sizeof(unsigned long long) * nq, st));
     GB_CUDA(cudaMemsetAsync(d_out, 0xFF, sizeof(unsigned long long) * nout, st));
-    GB_CUDA(launch_lmk_group(probe_ids, npairs, dir, nseg, d_cnt, d_start, d_cursor, d_item_start, d_grp_start, d_totals,
+    GB_CUDA(launch_lmk_group(probe_ids, npairs, dir, nseg, 128, d_cnt, d_start, d_cursor, d_item_start, d_grp_start, d_totals,
                              d_pair_j, d_items, st));
     const int k16 = (int)round_up(dpad_, 16);
     const int64_t max_groups = npairs / 128 + nlist_;
@@ -2041,7 +2041,8 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
 
   // ---- phase B: group the remaining pairs by list, stage the operand tiles, filter ----
   const int nseg = (int)std::min<int64_t>(64, std::max<int64_t>(1, (lists_->max_len() + kLmkSegRows - 1) / kLmkSegRows));
-  const int64_t max_groups = npairs / 128 + nlist_;
+  const int pq_group = 256;  // pairs per group: two 128-row operand tiles that share every decoded entry tile
+  const int64_t max_groups = npairs / pq_group + nlist_;
   const int64_t max_items = max_groups * nseg;
   if (max_items > INT32_MAX) return 1;
   GB_ALLOC(d_cnt, int32_t, nlist_, s);
@@ -2054,8 +2055,8 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   GB_ALLOC(d_items, LmTile, max_items, s);
   GB_ALLOC(d_cand_cnt, int, nq, s);
   const size_t tile_bytes = (size_t)(d_ / 8) * 2048;
-  const size_t a_bytes = (size_t)max_groups * tile_bytes;
-  const size_t meta_bytes = (size_t)max_groups * 128 * pqtc_pair_meta_bytes();
+  const size_t a_bytes = (size_t)max_groups * 2 * tile_bytes;
+  const size_t meta_bytes = (size_t)max_groups * pq_group * pqtc_pair_meta_bytes();
   const size_t cand_bytes = (size_t)nq * cap * 8;
   unsigned char* big = static_cast<unsigned char*>(big_acquire(a_bytes + meta_bytes + cand_bytes, st));
   if (!big) return -1;
@@ -2066,7 +2067,7 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   unsigned long long* cand = reinterpret_cast<unsigned long long*>(big + a_bytes + meta_bytes);
   stage_begin("pq_group_and_stage_pairs", st);
   GB_CUDA(cudaMemsetAsync(d_cand_cnt, 0, sizeof(int) * nq, st));
-  GB_CUDA(launch_lmk_group(d_probes_b, npairs, dir, nseg, d_cnt, d_start, d_cursor, d_item_start, d_grp_start, d_totals,
+  GB_CUDA(launch_lmk_group(d_probes_b, npairs, dir, nseg, pq_group, d_cnt, d_start, d_cursor, d_item_start, d_grp_start, d_totals,
                            d_pair_j, d_items, st));
   GB_CUDA(launch_pq_stage_pairs(xq, dpad_, d_, d_centroids_, dpad_, d_items, (int)max_items, d_totals, d_pair_j, nprobe,
                                 coarse_dis, keysA, kk, kk, d_cbnrm_ + (size_t)M_ * 256, f, metric, pqtc_eps_scale(), a_scratch,
@@ -2135,10 +2136,10 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
       pair_rows += (long long)t.npairs * t.nrows;
       rows += t.nrows;
     }
-    fprintf(stderr, "[pqtc] nq=%d k'=%d pa_max=%d cap=%d: candidates mean %.1f max %lld, overflowed queries %lld, dbg counters %llu %llu; "
-            "items %lld groups %lld tiles(128x128) %lld rows decoded %lld pair-rows %lld (tile fill %.3f)\n",
+    fprintf(stderr, "[pqtc] nq=%d k'=%d pa_max=%d cap=%d: candidates mean %.1f max %lld, overflowed queries %lld, stale code words %llu, rare-path warp tiles (32x128) %llu; "
+            "items %lld groups %lld tiles(%dx128) %lld rows decoded %lld pair-rows %lld (tile fill %.3f)\n",
             nq, kk, pa_max, cap, nq > over ? (double)tot / (nq - over) : 0.0, mx, over, dc[0], dc[1], (long long)ht[1], (long long)ht[0],
-            tiles, rows, pair_rows, tiles ? (double)pair_rows / ((double)tiles * 128 * 128) : 0.0);
+            pq_group, tiles, rows, pair_rows, tiles ? (double)pair_rows / ((double)tiles * pq_group * 128) : 0.0);
   }
   return 0;
 }

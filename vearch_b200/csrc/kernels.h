@@ -96,8 +96,9 @@ cudaError_t launch_seg_select(const float* scores, const int64_t* seg_off, const
 // out[(j * nseg_max + seg) * k + i], j = q * nprobe + p; unused slots must be pre-set to the sentinel.
 constexpr int kLmkMaxK = 64;
 constexpr int kLmkSegRows = 2048;
-// grouping: cnt/start/cursor/item_start/grp_start: [nlist] ints; totals = {groups, items, pairs} (device side)
-cudaError_t launch_lmk_group(const int32_t* probe_ids, int64_t npairs, ListDirectory dir, int nseg_max, int32_t* cnt,
+// grouping: cnt/start/cursor/item_start/grp_start: [nlist] ints; totals = {groups, items, pairs} (device side);
+// a list's pairs are split evenly over ceil(pairs / gsize) groups
+cudaError_t launch_lmk_group(const int32_t* probe_ids, int64_t npairs, ListDirectory dir, int nseg_max, int gsize, int32_t* cnt,
                              int32_t* start, int32_t* cursor, int32_t* item_start, int32_t* grp_start, int64_t* totals,
                              int64_t* pair_j, LmTile* items, cudaStream_t st);
 // TMA-fed variant (kernels_tc.cu, "mirror"): the lists are kept a second time pre-split (TF32 head +

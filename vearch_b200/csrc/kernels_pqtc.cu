@@ -20,7 +20,8 @@
 //            fp16 operand tile of sa * (x - c_list) rows staged once (pq_stage_pairs_kernel), then a
 //            persistent warp-specialised kernel (pqtc_scan_kernel) decodes 128 entries at a time
 //            from their codes into the second operand (codebook in shared memory, pre-scaled by -2),
-//            multiplies 128 pairs x 128 entries x d on the tensor core and compares
+//            multiplies up to 256 pairs x 128 entries x d on the tensor core (two consumer warpgroups of 128
+//            pairs share each decoded tile) and compares
 //            acc + |r_e|^2 against  B_q - dis0 + eps(pair).  eps bounds |approximate - reference fp32|
 //            rigorously (fp16 rounding of both operands: 2^-10 |a||r| ; fp32 noise of both evaluations),
 //            so every entry whose reference score is <= B_q passes.  |r_e|^2 comes from a per-entry cache
@@ -37,7 +38,7 @@
 // centroid IS one 16-byte core-matrix row: decoding an entry is M x (LDS.128 from the codebook,
 // STS.128 into the tile), conflict-free on the store side (consecutive entries -> consecutive rows).
 //
-// Algorithmic bytes: (M + 8) per scanned entry per 128-pair group instead of per pair.
+// Algorithmic bytes: (M + 8) per scanned entry per 256-pair group instead of per pair.
 #include <float.h>
 #include <math.h>
 #include <stdio.h>
@@ -51,15 +52,21 @@ namespace gb {
 
 namespace {
 
-constexpr int PT_M = 128;          // pairs per group  (MMA M: two m64 halves, one warpgroup)
+constexpr int PT_M = 128;          // pairs per warpgroup (MMA M: two m64 halves) = rows of one A operand tile
+constexpr int PT_G = 2 * PT_M;     // pairs per group: two consumer warpgroups share each decoded B tile
 constexpr int PT_N = 128;          // entries per tile (MMA N, accumulator columns)
-constexpr int PT_NT = 320;         // warps 0-3 MMA + epilogue, 4-7 decode, 8 TMA producer, 9 candidate drain
+// warpgroups 0-1 MMA + epilogue (pairs 0-127 / 128-255 of the group), 2 decode, 3: warp 12 TMA producer,
+// warp 13 candidate drain, warps 14-15 idle (setmaxnreg works per warpgroup)
+constexpr int PT_NT = 512;
+constexpr int PT_REG_MMA = 192, PT_REG_OTHER = 64;  // 2 x 128 x (192 + 64) = the 64 K registers of the SM
 constexpr int PT_RQ = 512;         // records of the CTA's candidate queue (shared memory)
 constexpr unsigned long long kRecEmpty = ~0ull;
 constexpr int PT_CS = 4;           // code stages
 constexpr int PT_KSUB = 256;
 
-__device__ unsigned long long g_pqtc_dbg[4];  // debugging counters (GB_PQTC_DBG & 4): [0] stale code words seen by decode
+// debugging counters: [0] stale code words seen by decode (GB_PQTC_DBG & 4), [1] warp tiles (32 pairs x 128 entries) of
+// the epilogue with at least one candidate (the rare path)
+__device__ unsigned long long g_pqtc_dbg[4];
 
 struct PtShared {
   uint64_t code_full[PT_CS], code_empty[PT_CS];
@@ -164,8 +171,11 @@ struct PairMeta {
   int lim;    // rows [0, lim) of this pair's list were scored exactly by phase A: never candidates
 };
 
+// A group of up to PT_G pairs is staged as two stacked 128-row tiles, one per consumer warpgroup; its pairs are split
+// evenly over the two (the first ceil(n / 2) in tile 0), so neither runs a mostly empty remainder.  Thread r = row r % 128
+// of tile r / 128; meta[grp * PT_G + r] is that row's pair.
 template <int METRIC>
-__global__ void __launch_bounds__(PT_M)
+__global__ void __launch_bounds__(PT_G)
     pq_stage_pairs_kernel(const float* __restrict__ xq, int64_t ldq, int d, const float* __restrict__ coarse, int64_t ldc,
                           const LmTile* __restrict__ items, const int64_t* __restrict__ totals,
                           const int64_t* __restrict__ pair_j, int nprobe, const float* __restrict__ coarse_dis,
@@ -176,14 +186,15 @@ __global__ void __launch_bounds__(PT_M)
   if ((int64_t)blockIdx.x >= totals[1]) return;
   const LmTile t = items[blockIdx.x];
   if (t.seg != 0) return;  // one staging per pair group: the first item of the group owns the slot
-  const int r = threadIdx.x;
+  const int h = threadIdx.x / PT_M, r = threadIdx.x % PT_M;
+  const int n0 = (t.npairs + 1) / 2;  // pairs of tile 0
   const int kc_n = d / 8;
-  unsigned char* tile = a_scratch + (int64_t)t.grp * ((int64_t)kc_n * 2048);
+  unsigned char* tile = a_scratch + ((int64_t)t.grp * 2 + h) * ((int64_t)kc_n * 2048);
   PairMeta pm{-INFINITY, INFINITY, 1.0f, -1, 0, 0};
   const float* x = nullptr;
   const float* c = nullptr;
-  if (r < t.npairs) {
-    const int64_t j = pair_j[t.pair0 + r];
+  if (r < (h ? t.npairs - n0 : n0)) {
+    const int64_t j = pair_j[t.pair0 + h * n0 + r];
     pm.q = (int)(j / nprobe);
     pm.p = (int)(j - (int64_t)pm.q * nprobe);
     x = xq + (int64_t)pm.q * ldq;
@@ -259,45 +270,88 @@ __global__ void __launch_bounds__(PT_M)
       pm.lo = lo * pm.c;
     }
   }
-  meta[(int64_t)t.grp * PT_M + r] = pm;
+  meta[(int64_t)t.grp * PT_G + threadIdx.x] = pm;
 }
 
 // ---- the scan ---------------------------------------------------------------------------------------
-// rare path of the epilogue: the 32 columns of one pair contain at least one candidate.
-// Called by the whole warp; `active` = this lane's pair has a candidate among the 32 columns.  The
-// columns are read from the slab again here: handing the caller's register block over by reference
-// would force a local-memory copy of every accumulator block in the hot loop.
-__device__ __noinline__ void pt_push_hits(const float* slab, const float* ne32, float c, float thr, float lo, int q, int p,
-                                          uint32_t pos0, int lim, PtShared* sh, bool active) {
-  uint32_t v[32];
-  slab_row(slab, v);
-  uint32_t mask = 0;
-  if (active) {
+// Accumulator fragments of a consumer thread: fragment index 4 j + 2 r8 + e of half u = row 64 u + 16 w + l / 4 + 8 r8,
+// column 8 j + 2 (l % 4) + e (w = warp of the warpgroup, l = lane).  Its four rows f4 = 2 u + r8:
+__device__ __forceinline__ int pt_frag_row(int f4, int t) { return (f4 >> 1) * 64 + (t >> 5) * 16 + ((t & 31) >> 2) + (f4 & 1) * 8; }
+
+// rare path of the epilogue, called by a whole warp when one of its lanes has a candidate in the tile: each lane tests
+// its own fragments again (the same fmaf as the fast path, now with the score window's lower side and the phase-A row
+// limit) and the warp appends the hits to the CTA's queue with one shared-memory atomic.  Inlined: the fragments are
+// registers, and handing them over by reference would force a local-memory copy of the accumulator in the hot loop.
+__device__ __forceinline__ void pt_push_frag_hits(const float (&acc)[2][64], const float* ne, const float (&fthr)[4],
+                                                  const float (&fc)[4], const PairMeta* gm, uint32_t pos0,
+                                                  PtShared* sh) {
+  const int t = threadIdx.x & 127, lane = t & 31;
+  float lo[4];
+  int lim[4];
+  uint32_t mask[4];
 #pragma unroll
-    for (int j = 0; j < 32; j++) {
-      const float s = fmaf(ne32[j], c, __uint_as_float(v[j]));
-      if (s <= thr && s >= lo) mask |= 1u << j;
-    }
-    // rows phase A has scored exactly stay out
-    if ((int)pos0 < lim) mask = (int)pos0 + 32 <= lim ? 0u : mask & ~((1u << (lim - (int)pos0)) - 1u);
+  for (int f4 = 0; f4 < 4; f4++) {
+    const PairMeta* m = gm + pt_frag_row(f4, t);
+    lo[f4] = __ldg(&m->lo);
+    lim[f4] = __ldg(&m->lim);
+    mask[f4] = 0;
   }
-  if (mask) {
-    unsigned int idx = atomicAdd(&sh->q_head, (unsigned int)__popc(mask));
-    const unsigned long long hi = ((unsigned long long)(uint32_t)q << 48) | ((unsigned long long)(uint32_t)p << 32);
-    while (mask) {
-      const int j = __ffs(mask) - 1;
-      mask &= mask - 1;
+  // column-outer: each |r_e|^2 is loaded once for the four rows, so only the accumulator stays live in registers
+#pragma unroll
+  for (int j = 0; j < PT_N / 8; j++) {
+    const float2 n2 = *reinterpret_cast<const float2*>(&ne[8 * j + 2 * (lane & 3)]);
+#pragma unroll
+    for (int e = 0; e < 2; e++) {
+      const int col = 8 * j + 2 * (lane & 3) + e;
+#pragma unroll
+      for (int f4 = 0; f4 < 4; f4++) {
+        // ns = -(acc + c * ne) exactly (fma rounds symmetrically).  Written as the fast path's fmaf, ptxas would keep
+        // all 128 sums of the fast path alive for this rarely taken path and spill them
+        const float ns = fmaf(-(e ? n2.y : n2.x), fc[f4], -acc[f4 >> 1][4 * j + 2 * (f4 & 1) + e]);
+        // rows phase A has scored exactly stay out
+        if (ns >= -fthr[f4] && ns <= -lo[f4] && (int)(pos0 + col) >= lim[f4]) mask[f4] |= 1u << (2 * j + e);
+      }
+    }
+  }
+  const int n = __popc(mask[0]) + __popc(mask[1]) + __popc(mask[2]) + __popc(mask[3]);
+  int incl = n;  // warp-inclusive prefix sum of the hit counts
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  const int total = __shfl_sync(0xffffffffu, incl, 31);
+  unsigned int base = 0;
+  if (lane == 31 && total) base = atomicAdd(&sh->q_head, (unsigned int)total);
+  unsigned int idx = __shfl_sync(0xffffffffu, base, 31) + (unsigned int)(incl - n);
+#pragma unroll
+  for (int f4 = 0; f4 < 4; f4++) {
+    uint32_t mk = mask[f4];
+    if (!mk) continue;
+    const PairMeta* m = gm + pt_frag_row(f4, t);
+    const unsigned long long hi = ((unsigned long long)(uint32_t)__ldg(&m->q) << 48) | ((unsigned long long)(uint32_t)__ldg(&m->p) << 32);
+    while (mk) {
+      const int b = __ffs(mk) - 1;
+      mk &= mk - 1;
+      const uint32_t col = 8 * (b >> 1) + 2 * (lane & 3) + (b & 1);
       // the slot's previous occupant (idx - PT_RQ) has been consumed once the tail has passed it
       while (idx - *reinterpret_cast<volatile unsigned int*>(&sh->q_tail) >= (unsigned int)PT_RQ) __nanosleep(32);
-      *reinterpret_cast<volatile unsigned long long*>(&sh->q_rec[idx % PT_RQ]) = hi | (unsigned long long)(pos0 + (uint32_t)j);
+      *reinterpret_cast<volatile unsigned long long*>(&sh->q_rec[idx % PT_RQ]) = hi | (unsigned long long)(pos0 + col);
       idx++;
     }
   }
   __syncwarp();
 }
 
+__device__ __forceinline__ void bar_sync_256(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void bar_arrive_256(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // EAGER: tombstones and the docid predicate are resolved in the decode warps (one id + bitmap lookup per entry per
-// 128 pairs) -- needed when a deletion / filter bitmap is present, because the bound B_q was taken over valid entries
+// 256 pairs) -- needed when a deletion / filter bitmap is present, because the bound B_q was taken over valid entries
 // only and a selective filter would otherwise flood the candidate lists.  Without bitmaps the ids are not touched
 // here at all (their DRAM latency sits on the decode warps' critical path);
 // tombstoned entries that pass the filter are dropped by pq_rescore_kernel, which reads the id anyway.
@@ -322,14 +376,13 @@ __global__ void __launch_bounds__(PT_NT, 1)
   __shared__ PtShared sh;
   unsigned char* cb = smem;
   float* nstage = reinterpret_cast<float*>(smem + CB_BYTES);  // [PT_CS][PT_N] norms of the staged tiles
-  // [codebook][norms][A tile][B tiles x 2][code stages][slabs]; the operand tiles start on 4 KiB boundaries
+  // [codebook][norms][A tiles x 2][B tiles x 2][code stages]; the operand tiles start on 4 KiB boundaries
   // (GB_PQTC_DBG bit 5 + bits 8.. place them at a chosen offset instead, for debugging)
   unsigned char* a_buf = smem + CB_BYTES + NRM_BYTES;
   if (!(dbg & 32)) a_buf += (4096u - (smem_u32(a_buf) & 4095u)) & 4095u;
   else a_buf += (dbg >> 8) & 0xFFF0;  // debugging: place the tiles at a chosen (mis)alignment
-  unsigned char* b_buf = a_buf + tile_stride;
+  unsigned char* b_buf = a_buf + 2 * tile_stride;
   unsigned char* code_buf = b_buf + 2 * tile_stride;
-  float* slabs = reinterpret_cast<float*>(code_buf + PT_CS * CODE_STAGE);
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int64_t n_items = totals[1];
@@ -341,11 +394,11 @@ __global__ void __launch_bounds__(PT_NT, 1)
     }
     for (int b = 0; b < 2; b++) {
       mbar_init(&sh.b_full[b], PT_N);       // every decode thread has written its row
-      mbar_init(&sh.b_empty[b], PT_M);      // every MMA thread, once its MMAs are complete
-      mbar_init(&sh.acc_empty[b], PT_M);    // every epilogue thread
+      mbar_init(&sh.b_empty[b], PT_G);      // every MMA thread of both warpgroups, once its MMAs are complete
+      mbar_init(&sh.acc_empty[b], PT_G);    // every epilogue thread of both warpgroups
     }
-    mbar_init(&sh.a_full, 1);               // bulk copy
-    mbar_init(&sh.a_empty, PT_M);           // every MMA thread, after the item's last tile
+    mbar_init(&sh.a_full, 1);               // bulk copies
+    mbar_init(&sh.a_empty, PT_G);           // every MMA thread, after the item's last tile
     mbar_fence_init();
     sh.q_head = 0, sh.q_tail = 0, sh.q_done = 0;
   }
@@ -355,29 +408,36 @@ __global__ void __launch_bounds__(PT_NT, 1)
     reinterpret_cast<uint4*>(cb)[i] = __ldg(reinterpret_cast<const uint4*>(cb_g) + i);
   __syncthreads();
 
-  if (warp < 4) {
-    // ======================= MMA + epilogue: thread = pair =======================
-    const uint32_t a_base = smem_u32(a_buf), b_base = smem_u32(b_buf);
+  if (warp < 8) {
+    // ======================= MMA + epilogue: warpgroup h = pairs [128 h, 128 h + 128) of the group =======================
+    // Both warpgroups multiply the same B tile and take turns on the tensor pipe (named barriers 2 and 3): warpgroup 1
+    // issues tile i while warpgroup 0 tests tile i, warpgroup 0 issues tile i + 1 while warpgroup 1 tests tile i.
+    setmaxnreg_inc<PT_REG_MMA>();
+    const int h = warp >> 2, t = tid & 127;
+    const uint32_t a_base = smem_u32(a_buf) + (uint32_t)(h * tile_stride), b_base = smem_u32(b_buf);
     uint32_t an = 0, bn = 0;
+    bool turns = false;  // warpgroup 0 has issued a tile: from then on it waits for warpgroup 1's turn
     float acc[2][64];
     for (int64_t it = blockIdx.x; it < n_items; it += gridDim.x) {
-      const LmTile t = items[it];
-      if (t.nrows <= 0) continue;  // every role skips empty segments the same way
-      PairMeta pm = meta[(int64_t)t.grp * PT_M + tid];
-      // thresholds of the four pairs (rows) whose accumulator fragments this thread holds: fragment index
-      // 4 j + 2 r8 + e of half h = row 64 h + 16 w + l / 4 + 8 r8, column 8 j + 2 (l % 4) + e
+      const LmTile tl = items[it];
+      if (tl.nrows <= 0) continue;  // every role skips empty segments the same way
+      const PairMeta* gm = meta + (int64_t)tl.grp * PT_G + h * PT_M;
+      // thresholds of the four pairs (rows) whose accumulator fragments this thread holds
       float fthr[4], fc[4];
 #pragma unroll
       for (int f4 = 0; f4 < 4; f4++) {
-        const int row = (f4 >> 1) * 64 + (tid >> 5) * 16 + ((tid & 31) >> 2) + (f4 & 1) * 8;
-        const PairMeta* m = meta + (int64_t)t.grp * PT_M + row;
+        const PairMeta* m = gm + pt_frag_row(f4, t);
         fthr[f4] = __ldg(&m->thr), fc[f4] = __ldg(&m->c);
       }
       mbar_wait(&sh.a_full, an & 1);
-      const int ntiles = (t.nrows + PT_N - 1) / PT_N;
+      const int ntiles = (tl.nrows + PT_N - 1) / PT_N;
       for (int i = 0; i < ntiles; i++, bn++) {
         const int b = bn & 1;
         mbar_wait(&sh.b_full[b], (bn >> 1) & 1);
+        if (h) bar_sync_256(3);
+        else if (turns) bar_sync_256(2);
+        // every warpgroup runs both m64 halves of every tile, empty rows included (their thresholds are -inf): a
+        // branch around the MMAs or the wait makes ptxas serialise every wgmma of the kernel
         const uint64_t da = lt_desc(a_base), db = lt_desc(b_base + (uint32_t)(b * tile_stride));
         wg_fence();
 #pragma unroll
@@ -387,61 +447,46 @@ __global__ void __launch_bounds__(PT_NT, 1)
           wg_mma_f16(acc[1], da + adv + kDescHalfM, db + adv, kk != 0);
         }
         wg_commit();
+        bar_arrive_256(h ? 2 : 3);
+        turns = true;
         wg_wait<0>();
         wg_fence_acc(acc);
         mbar_arrive(&sh.b_empty[b]);
         if (i == ntiles - 1) mbar_arrive(&sh.a_empty);
         if (dbg & 16) __nanosleep(1000);
-        // Fast path: the same test (acc + c * ne <= thr, same fmaf / fminf) on the fragments themselves; only a
-        // tile where some pair has a candidate goes through the row-per-thread exchange below, which redoes the
-        // test per 32-column block and pushes the hits.
+        // Fast path: min over the tile of acc + c * ne per pair, on the fragments themselves.  A warp where some pair
+        // has a candidate redoes the test per entry and pushes the hits (pt_push_frag_hits).
+        float mn[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
+#pragma unroll
+        for (int j = 0; j < PT_N / 8; j++) {
+          const float2 n2 = *reinterpret_cast<const float2*>(&sh.ne[b][8 * j + 2 * (t & 3)]);
+#pragma unroll
+          for (int f4 = 0; f4 < 4; f4++) {
+            const float* a2 = &acc[f4 >> 1][4 * j + 2 * (f4 & 1)];
+            mn[f4] = fminf(mn[f4], fminf(fmaf(n2.x, fc[f4], a2[0]), fmaf(n2.y, fc[f4], a2[1])));
+          }
+        }
         bool hit = false;
-        {
-          float mn[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
 #pragma unroll
-          for (int j = 0; j < PT_N / 8; j++) {
-            const float2 n2 = *reinterpret_cast<const float2*>(&sh.ne[b][8 * j + 2 * (tid & 3)]);
-#pragma unroll
-            for (int f4 = 0; f4 < 4; f4++) {
-              const float* a2 = &acc[f4 >> 1][4 * j + 2 * (f4 & 1)];
-              mn[f4] = fminf(mn[f4], fminf(fmaf(n2.x, fc[f4], a2[0]), fmaf(n2.y, fc[f4], a2[1])));
-            }
-          }
-#pragma unroll
-          for (int f4 = 0; f4 < 4; f4++) hit |= mn[f4] <= fthr[f4];
-        }
-        if (wg0_any(hit)) {
-#pragma unroll
-        for (int c0 = 0; c0 < PT_N; c0 += 32) {
-          uint32_t v[32];
-          acc_cols(acc, c0, slabs, v);
-          const float* ne0 = &sh.ne[b][c0];
-          float mn = INFINITY;
-#pragma unroll
-          for (int j4 = 0; j4 < 32; j4 += 4) {
-            const float4 n4 = *reinterpret_cast<const float4*>(ne0 + j4);
-            const float s0 = fmaf(n4.x, pm.c, __uint_as_float(v[j4])), s1 = fmaf(n4.y, pm.c, __uint_as_float(v[j4 + 1]));
-            const float s2 = fmaf(n4.z, pm.c, __uint_as_float(v[j4 + 2])), s3 = fmaf(n4.w, pm.c, __uint_as_float(v[j4 + 3]));
-            mn = fminf(mn, fminf(fminf(s0, s1), fminf(s2, s3)));
-          }
-          const uint32_t pos = (uint32_t)(t.row0 + i * PT_N + c0);
-          const bool h = mn <= pm.thr;
-          if (__any_sync(0xffffffffu, h))
-            pt_push_hits(slabs + ((c0 >> 5) & 1) * kSlabFloats, ne0, pm.c, pm.thr, pm.lo, pm.q, pm.p, pos, pm.lim, &sh, h);
-        }
+        for (int f4 = 0; f4 < 4; f4++) hit |= mn[f4] <= fthr[f4];
+        if (__any_sync(0xffffffffu, hit)) {
+          if ((t & 31) == 0) atomicAdd(&g_pqtc_dbg[1], 1ull);
+          pt_push_frag_hits(acc, sh.ne[b], fthr, fc, gm, (uint32_t)(tl.row0 + i * PT_N), &sh);
         }
         mbar_arrive(&sh.acc_empty[b]);
       }
       an++;
     }
+    if (h == 0 && turns) bar_sync_256(2);  // warpgroup 1's arrival after its last tile
     __syncwarp();
     if ((tid & 31) == 0) {
       __threadfence_block();
       atomicAdd(&sh.q_done, 1);  // this warp's records are all in the queue
     }
-  } else if (warp < 8) {
+  } else if (warp < 12) {
     // ======================= decode: thread = entry of the tile =======================
-    const int e = tid - 4 * 32;
+    setmaxnreg_dec<PT_REG_OTHER>();
+    const int e = tid - 8 * 32;
     uint32_t cn = 0, bn = 0;
     for (int64_t it = blockIdx.x; it < n_items; it += gridDim.x) {
       const LmTile t = items[it];
@@ -485,7 +530,7 @@ __global__ void __launch_bounds__(PT_NT, 1)
         mbar_arrive(&sh.code_empty[s]);
         // entries past the end of the segment decode whatever bytes the stage holds: finite values,
         // masked by ne = +inf.  Tombstones (gamma_index_ivfpq.h:930) and the docid predicate
-        // (IsValid, :934-939) are resolved here, once per entry per 128 pairs.
+        // (IsValid, :934-939) are resolved here, once per entry per 256 pairs.
         const int row = t.row0 + i * PT_N + e;
         bool valid = row < row_end;
         if (EAGER && valid) {
@@ -519,71 +564,75 @@ __global__ void __launch_bounds__(PT_NT, 1)
         mbar_arrive(&sh.b_full[b]);
       }
     }
-  } else if (warp == 8) {
-    // ======================= TMA producer (whole warp loops, one elected lane issues) =======================
-    uint32_t an = 0, cn = 0;
-    for (int64_t it = blockIdx.x; it < n_items; it += gridDim.x) {
-      const LmTile t = items[it];
-      if (t.nrows <= 0) continue;  // every role skips empty segments the same way
-      mbar_wait(&sh.a_empty, (an & 1) ^ 1);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&sh.a_full, TILE);
-        bulk_g2s(a_buf, a_scratch + (int64_t)t.grp * TILE, TILE, &sh.a_full);
-      }
-      __syncwarp();
-      const unsigned char* lcodes = dir.codes[t.list];
-      const float* lnorms = HAS_NORM ? pqnorm + pqnorm_off[t.list] : nullptr;  // list segments start 128-byte aligned
-      const int ntiles = (t.nrows + PT_N - 1) / PT_N;
-      for (int i = 0; i < ntiles; i++, cn++) {
-        const int s = cn % PT_CS;
-        mbar_wait(&sh.code_empty[s], ((cn / PT_CS) & 1) ^ 1);
+  } else {
+    setmaxnreg_dec<PT_REG_OTHER>();  // warpgroup 3: warps 14 and 15 have no role and exit here
+    if (warp == 12) {
+      // ======================= TMA producer (whole warp loops, one elected lane issues) =======================
+      uint32_t an = 0, cn = 0;
+      for (int64_t it = blockIdx.x; it < n_items; it += gridDim.x) {
+        const LmTile t = items[it];
+        if (t.nrows <= 0) continue;  // every role skips empty segments the same way
+        mbar_wait(&sh.a_empty, (an & 1) ^ 1);
         if (elect_one()) {
-          const int n_e = min(PT_N, t.nrows - i * PT_N);
-          const uint32_t bytes = ((uint32_t)n_e * M + 15u) & ~15u;
-          const uint32_t nbytes = HAS_NORM ? ((uint32_t)n_e * 4u + 15u) & ~15u : 0u;
-          mbar_arrive_expect_tx(&sh.code_full[s], bytes + nbytes);
-          bulk_g2s(code_buf + s * CODE_STAGE, lcodes + (int64_t)(t.row0 + i * PT_N) * M, bytes, &sh.code_full[s]);
-          if (HAS_NORM) bulk_g2s(nstage + s * PT_N, lnorms + (t.row0 + i * PT_N), nbytes, &sh.code_full[s]);
+          mbar_arrive_expect_tx(&sh.a_full, 2 * TILE);
+          for (int h = 0; h < 2; h++)
+            bulk_g2s(a_buf + h * tile_stride, a_scratch + ((int64_t)t.grp * 2 + h) * TILE, TILE, &sh.a_full);
         }
         __syncwarp();
-      }
-      an++;
-    }
-  } else {
-    // ======================= candidate drain: shared queue -> global per-query lists =======================
-    const int lane = tid & 31;
-    unsigned int t = 0;
-    for (;;) {
-      unsigned long long r[4];
-      int n = 0;
-      bool open = true;
-#pragma unroll
-      for (int u = 0; u < 4; u++) {
-        r[u] = *reinterpret_cast<volatile unsigned long long*>(&sh.q_rec[(t + (unsigned)(lane + 32 * u)) % PT_RQ]);
-        const unsigned int m = __ballot_sync(0xffffffffu, r[u] != kRecEmpty);
-        if (open) {  // records are consumed as a contiguous prefix, so the tail stays a single counter
-          if (m == 0xffffffffu) n += 32;
-          else n += __ffs(~m) - 1, open = false;
+        const unsigned char* lcodes = dir.codes[t.list];
+        const float* lnorms = HAS_NORM ? pqnorm + pqnorm_off[t.list] : nullptr;  // list segments start 128-byte aligned
+        const int ntiles = (t.nrows + PT_N - 1) / PT_N;
+        for (int i = 0; i < ntiles; i++, cn++) {
+          const int s = cn % PT_CS;
+          mbar_wait(&sh.code_empty[s], ((cn / PT_CS) & 1) ^ 1);
+          if (elect_one()) {
+            const int n_e = min(PT_N, t.nrows - i * PT_N);
+            const uint32_t bytes = ((uint32_t)n_e * M + 15u) & ~15u;
+            const uint32_t nbytes = HAS_NORM ? ((uint32_t)n_e * 4u + 15u) & ~15u : 0u;
+            mbar_arrive_expect_tx(&sh.code_full[s], bytes + nbytes);
+            bulk_g2s(code_buf + s * CODE_STAGE, lcodes + (int64_t)(t.row0 + i * PT_N) * M, bytes, &sh.code_full[s]);
+            if (HAS_NORM) bulk_g2s(nstage + s * PT_N, lnorms + (t.row0 + i * PT_N), nbytes, &sh.code_full[s]);
+          }
+          __syncwarp();
         }
+        an++;
       }
-      if (n == 0) {
-        if (*reinterpret_cast<volatile int*>(&sh.q_done) == 4 && *reinterpret_cast<volatile unsigned int*>(&sh.q_head) == t) break;
-        __nanosleep(64);
-        continue;
-      }
+    } else if (warp == 13) {
+      // ======================= candidate drain: shared queue -> global per-query lists =======================
+      const int lane = tid & 31;
+      unsigned int t = 0;
+      for (;;) {
+        unsigned long long r[4];
+        int n = 0;
+        bool open = true;
 #pragma unroll
-      for (int u = 0; u < 4; u++) {
-        if (lane + 32 * u < n) {
-          const int q = (int)(r[u] >> 48), p = (int)((r[u] >> 32) & 0xFFFFu);
-          const int slot = atomicAdd(cand_cnt + q, 1);  // a count above cap flags the query for the exact kernel
-          if (slot < cap) cand[(int64_t)q * cap + slot] = ((unsigned long long)(uint32_t)p << 32) | (r[u] & 0xFFFFFFFFull);
-          *reinterpret_cast<volatile unsigned long long*>(&sh.q_rec[(t + (unsigned)(lane + 32 * u)) % PT_RQ]) = kRecEmpty;
+        for (int u = 0; u < 4; u++) {
+          r[u] = *reinterpret_cast<volatile unsigned long long*>(&sh.q_rec[(t + (unsigned)(lane + 32 * u)) % PT_RQ]);
+          const unsigned int m = __ballot_sync(0xffffffffu, r[u] != kRecEmpty);
+          if (open) {  // records are consumed as a contiguous prefix, so the tail stays a single counter
+            if (m == 0xffffffffu) n += 32;
+            else n += __ffs(~m) - 1, open = false;
+          }
         }
+        if (n == 0) {
+          if (*reinterpret_cast<volatile int*>(&sh.q_done) == 8 && *reinterpret_cast<volatile unsigned int*>(&sh.q_head) == t) break;
+          __nanosleep(64);
+          continue;
+        }
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+          if (lane + 32 * u < n) {
+            const int q = (int)(r[u] >> 48), p = (int)((r[u] >> 32) & 0xFFFFu);
+            const int slot = atomicAdd(cand_cnt + q, 1);  // a count above cap flags the query for the exact kernel
+            if (slot < cap) cand[(int64_t)q * cap + slot] = ((unsigned long long)(uint32_t)p << 32) | (r[u] & 0xFFFFFFFFull);
+            *reinterpret_cast<volatile unsigned long long*>(&sh.q_rec[(t + (unsigned)(lane + 32 * u)) % PT_RQ]) = kRecEmpty;
+          }
+        }
+        __threadfence_block();
+        __syncwarp();
+        t += (unsigned int)n;
+        if (lane == 0) *reinterpret_cast<volatile unsigned int*>(&sh.q_tail) = t;
       }
-      __threadfence_block();
-      __syncwarp();
-      t += (unsigned int)n;
-      if (lane == 0) *reinterpret_cast<volatile unsigned int*>(&sh.q_tail) = t;
     }
   }
 }
@@ -675,7 +724,7 @@ cudaError_t launch_scan_shape(const unsigned char* a_scratch, const PairMeta* me
   int tile_stride = (D / 8) * 2048, dbg = 0;
   if (const char* ev = getenv("GB_PQTC_DBG")) dbg = atoi(ev);
   if (dbg & 2) tile_stride = next_pow2(tile_stride);
-  const size_t base = (size_t)M * PT_KSUB * DSUB * 2 + 3 * (size_t)tile_stride + (size_t)PT_CS * PT_N * M + 4096 + kSlabBytes;
+  const size_t base = (size_t)M * PT_KSUB * DSUB * 2 + 4 * (size_t)tile_stride + (size_t)PT_CS * PT_N * M + 4096;
   const bool l2 = metric == kMetricL2;
   const bool eager = f.del_bits != nullptr || f.filter_bits != nullptr;
   if (l2 && (!pqnorm || !pqnorm_off)) return cudaErrorInvalidValue;
@@ -774,12 +823,12 @@ cudaError_t launch_pq_stage_pairs(const float* xq, int64_t ldq, int d, const flo
   if (max_items <= 0) return cudaSuccess;
   if (d % 16) return cudaErrorInvalidValue;
   if (metric == kMetricL2)
-    pq_stage_pairs_kernel<kMetricL2><<<max_items, PT_M, 0, st>>>(xq, ldq, d, coarse, ldc, items, totals, pair_j, nprobe,
+    pq_stage_pairs_kernel<kMetricL2><<<max_items, PT_G, 0, st>>>(xq, ldq, d, coarse, ldc, items, totals, pair_j, nprobe,
                                                                 coarse_dis, bound_keys, bound_stride, kprime, rmax2,
                                                                 f.min_score, f.max_score, eps_scale, a_scratch,
                                                                 static_cast<PairMeta*>(meta), cand_cnt, cap, row_limit);
   else
-    pq_stage_pairs_kernel<kMetricIP><<<max_items, PT_M, 0, st>>>(xq, ldq, d, coarse, ldc, items, totals, pair_j, nprobe,
+    pq_stage_pairs_kernel<kMetricIP><<<max_items, PT_G, 0, st>>>(xq, ldq, d, coarse, ldc, items, totals, pair_j, nprobe,
                                                                 coarse_dis, bound_keys, bound_stride, kprime, rmax2,
                                                                 f.min_score, f.max_score, eps_scale, a_scratch,
                                                                 static_cast<PairMeta*>(meta), cand_cnt, cap, row_limit);

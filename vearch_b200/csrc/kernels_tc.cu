@@ -781,7 +781,7 @@ __device__ __forceinline__ int lmk_nseg(int len, int nseg_max) {
 }
 
 __global__ void __launch_bounds__(1024)
-    lmk_scan_kernel(const int32_t* __restrict__ cnt, ListDirectory dir, int nseg_max, int32_t* __restrict__ start,
+    lmk_scan_kernel(const int32_t* __restrict__ cnt, ListDirectory dir, int nseg_max, int gsize, int32_t* __restrict__ start,
                     int32_t* __restrict__ item_start, int32_t* __restrict__ grp_start, int64_t* __restrict__ totals) {
   __shared__ long long s_pairs[1024], s_items[1024], s_grps[1024];
   __shared__ long long carry[3];
@@ -795,7 +795,7 @@ __global__ void __launch_bounds__(1024)
       c = cnt[l];
       const int len = dir.len[l];
       if (c > 0 && len > 0) {
-        g = (c + TC_M - 1) / TC_M;
+        g = (c + gsize - 1) / gsize;
         it = g * lmk_nseg(len, nseg_max);
       }
     }
@@ -832,22 +832,26 @@ __global__ void lmk_assign_kernel(const int32_t* __restrict__ probe_ids, int64_t
 
 __global__ void lmk_items_kernel(const int32_t* __restrict__ cnt, const int32_t* __restrict__ start,
                                  const int32_t* __restrict__ item_start, const int32_t* __restrict__ grp_start,
-                                 ListDirectory dir, int nseg_max, LmTile* __restrict__ items) {
+                                 ListDirectory dir, int nseg_max, int gsize, LmTile* __restrict__ items) {
   const int l = blockIdx.x * blockDim.x + threadIdx.x;
   if (l >= dir.nlist) return;
   const int c = cnt[l], len = dir.len[l];
   if (c <= 0 || len <= 0) return;
   const int nseg = lmk_nseg(len, nseg_max);
   const int seglen = (((len + nseg - 1) / nseg) + TC_N - 1) / TC_N * TC_N;
+  // the list's pairs are split evenly over its ceil(c / gsize) groups: no group is a mostly empty remainder
+  const int ng = (c + gsize - 1) / gsize;
   int it = item_start[l];
-  for (int p0 = 0; p0 < c; p0 += TC_M)
+  for (int g = 0; g < ng; g++) {
+    const int p0 = (int)((int64_t)g * c / ng), p1 = (int)((int64_t)(g + 1) * c / ng);
     for (int sg = 0; sg < nseg; sg++) {
       LmTile tl;
-      tl.list = l, tl.pair0 = start[l] + p0, tl.npairs = min(TC_M, c - p0);
+      tl.list = l, tl.pair0 = start[l] + p0, tl.npairs = p1 - p0;
       tl.row0 = sg * seglen, tl.nrows = max(0, min(seglen, len - tl.row0)), tl.seg = sg;
-      tl.grp = grp_start[l] + p0 / TC_M;
+      tl.grp = grp_start[l] + g;
       items[it++] = tl;
     }
+  }
 }
 
 // ---- segment select: per query, stream its P score segments, filter, keep the top-k ---------
@@ -1085,7 +1089,7 @@ cudaError_t launch_lm_assign_tiles(const int32_t* probe_ids, int64_t npairs, int
   return cudaGetLastError();
 }
 
-cudaError_t launch_lmk_group(const int32_t* probe_ids, int64_t npairs, ListDirectory dir, int nseg_max, int32_t* cnt,
+cudaError_t launch_lmk_group(const int32_t* probe_ids, int64_t npairs, ListDirectory dir, int nseg_max, int gsize, int32_t* cnt,
                              int32_t* start, int32_t* cursor, int32_t* item_start, int32_t* grp_start, int64_t* totals,
                              int64_t* pair_j, LmTile* items, cudaStream_t st) {
   if (npairs <= 0) return cudaSuccess;
@@ -1096,11 +1100,11 @@ cudaError_t launch_lmk_group(const int32_t* probe_ids, int64_t npairs, ListDirec
   const unsigned nb = (unsigned)((npairs + 255) / 256);
   lm_count_kernel<<<nb, 256, 0, st>>>(probe_ids, npairs, dir, cnt);
   note_launch();
-  lmk_scan_kernel<<<1, 1024, 0, st>>>(cnt, dir, nseg_max, start, item_start, grp_start, totals);
+  lmk_scan_kernel<<<1, 1024, 0, st>>>(cnt, dir, nseg_max, gsize, start, item_start, grp_start, totals);
   note_launch();
   lmk_assign_kernel<<<nb, 256, 0, st>>>(probe_ids, npairs, dir, start, cursor, pair_j);
   note_launch();
-  lmk_items_kernel<<<(dir.nlist + 255) / 256, 256, 0, st>>>(cnt, start, item_start, grp_start, dir, nseg_max, items);
+  lmk_items_kernel<<<(dir.nlist + 255) / 256, 256, 0, st>>>(cnt, start, item_start, grp_start, dir, nseg_max, gsize, items);
   note_launch();
   return cudaGetLastError();
 }
