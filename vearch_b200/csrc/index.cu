@@ -1052,11 +1052,23 @@ IVFFlatIndex::IVFFlatIndex(int d, const ModelParams& mp, int device, int seg_shi
     : Index(type, d, mp, device, seg_shift), nlist_(mp.ncentroids) {
   cudaMalloc(&d_centroids_, (size_t)nlist_ * dpad_ * 4);
   cudaMemset(d_centroids_, 0, (size_t)nlist_ * dpad_ * 4);
+  const int64_t ctiles = (nlist_ + 127) / 128;
+  cudaMalloc(&d_cent_tiles_, (size_t)ctiles * tc_mirror_tile_floats((int)round_up(dpad_, 16)) * 4);
+  cudaMalloc(&d_cent_norms_, (size_t)ctiles * 128 * 4);
+  rebuild_centroid_tiles(0);
+  cudaStreamSynchronize(0);
 }
 IVFFlatIndex::~IVFFlatIndex() {
   if (mirror_.base) cudaFree(mirror_.base);
   if (mirror_.norms) cudaFree(mirror_.norms);
-  if (mirror_.d_tile0) cudaFree(mirror_.d_tile0); cudaFree(d_centroids_); }
+  if (mirror_.d_tile0) cudaFree(mirror_.d_tile0); cudaFree(d_centroids_);
+  cudaFree(d_cent_tiles_);
+  cudaFree(d_cent_norms_);
+}
+int IVFFlatIndex::rebuild_centroid_tiles(cudaStream_t st) {
+  GB_CUDA(launch_tc_stage_rows(d_centroids_, dpad_, nlist_, dpad_, (int)round_up(dpad_, 16), d_cent_tiles_, d_cent_norms_, st));
+  return 0;
+}
 
 int IVFFlatIndex::training_threshold() const {
   // gamma_index_ivfflat.cc:239: default nlist * 200 ; Indexing() clamps to [39, 256] * nlist (:350-375)
@@ -1068,8 +1080,10 @@ int IVFFlatIndex::training_threshold() const {
   return (int)t;
 }
 int64_t IVFFlatIndex::index_mem_bytes() const {
-  const int64_t mirror = mirror_.cap_tiles * (tc_mirror_tile_floats((int)round_up(dpad_, 16)) * 4 + 512);
-  return (int64_t)nlist_ * dpad_ * 4 + (lists_ ? lists_->mem_bytes() : 0) + mirror;
+  const int64_t tile_bytes = tc_mirror_tile_floats((int)round_up(dpad_, 16)) * 4 + 512;
+  const int64_t mirror = mirror_.cap_tiles * tile_bytes;
+  const int64_t cent_tiles = (nlist_ + 127) / 128 * tile_bytes;
+  return (int64_t)nlist_ * dpad_ * 4 + cent_tiles + (lists_ ? lists_->mem_bytes() : 0) + mirror;
 }
 int IVFFlatIndex::set_centroids(const float* host, int nlist) {
   if (nlist != nlist_) {
@@ -1082,6 +1096,8 @@ int IVFFlatIndex::set_centroids(const float* host, int nlist) {
   GB_CUDA(cudaMemset(d_centroids_, 0, (size_t)nlist_ * dpad_ * 4));
   GB_CUDA(cudaMemcpy2D(d_centroids_, (size_t)dpad_ * 4, host, (size_t)d_ * 4, (size_t)d_ * 4, nlist_,
                        cudaMemcpyHostToDevice));
+  if (rebuild_centroid_tiles(0)) return -1;
+  GB_CUDA(cudaStreamSynchronize(0));  // searches run on other (non-blocking) streams
   if (!lists_) lists_.reset(new IvfLists(nlist_, code_bytes()));
   trained_ = true;
   return 0;
@@ -1116,6 +1132,7 @@ int IVFFlatIndex::train() {
   xt = train_transform(xt, num, s);  // OPQ: learn the rotation, continue on the rotated slab
   if (!xt) return -1;
   if (kmeans_device(xt, dpad_, num, d_, nlist_, kp, d_centroids_, dpad_, st, nullptr)) return -1;
+  if (rebuild_centroid_tiles(st)) return -1;
   if (train_extra(xt, num, s)) return -1;
   GB_CUDA(cudaStreamSynchronize(st));
   if (!lists_) lists_.reset(new IvfLists(nlist_, code_bytes()));
@@ -1260,15 +1277,56 @@ int IVFFlatIndex::resolve_nprobe(const SearchContext& ctx) const {
   return nprobe;
 }
 
+// GB_COARSE_FUSED=0: always write the query x centroid score matrix and select from it (A/B runs; the reference of the
+// fused path's tests).  Read per call: tests flip it between searches of one process.
+static bool coarse_fused_enabled() {
+  const char* e = getenv("GB_COARSE_FUSED");
+  return e ? atoi(e) != 0 : true;
+}
+
+// centroid tiles per segment of the fused coarse quantiser: fewest (waves of one CTA per SM) x (tiles per item + 1),
+// the + 1 standing for an item's fixed cost (pipeline fill, a fresh key set); ties go to fewer segments
+static int coarse_seg_tiles(int nqt, int ntc, int nsm) {
+  int best = ntc;
+  int64_t best_cost = INT64_MAX;
+  for (int t = ntc; t >= 1; t--) {
+    const int nseg = (ntc + t - 1) / t;
+    if (nseg > 16) break;  // bounds the per-query keys the merge reads
+    const int64_t cost = ((int64_t)nqt * nseg + nsm - 1) / nsm * (t + 1);
+    if (cost < best_cost) best_cost = cost, best = t;
+  }
+  return best;
+}
+
 // quantizer->search (gamma_index_ivfflat.cc:568 / gamma_index_ivfpq.cc:595)
 int IVFFlatIndex::coarse_dev(int nq, const float* xq, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis,
                              Scratch& s) {
   cudaStream_t st = s.stream();
+  GB_ALLOC(keys, unsigned long long, (size_t)nq * nprobe, s);
+  const bool tc = tc_enabled() && nlist_ >= 64 && nq >= 32;
+  const int k16 = (int)round_up(dpad_, 16);
+  if (tc && coarse_fused_enabled() && nprobe <= kCoarseMaxK && k16 > 16) {
+    // fused: per (query tile, centroid segment) the best nprobe keys, merged per query; no score matrix
+    const int nqt = (nq + 127) / 128, ntc = (nlist_ + 127) / 128;
+    const int seg_tiles = coarse_seg_tiles(nqt, ntc, sm_count(device_));
+    const int nseg = (ntc + seg_tiles - 1) / seg_tiles;
+    GB_ALLOC(a_tiles, float, (size_t)nqt * tc_mirror_tile_floats(k16), s);
+    GB_ALLOC(a_norms, float, (size_t)nqt * 128, s);
+    GB_ALLOC(tau, unsigned long long, nq, s);
+    GB_ALLOC(part, unsigned long long, (size_t)nq * nseg * nprobe, s);
+    StageScope stage(this, "coarse_quantizer", st);
+    GB_CUDA(cudaMemsetAsync(tau, 0xFF, sizeof(unsigned long long) * nq, st));
+    GB_CUDA(launch_tc_stage_rows(xq, dpad_, nq, dpad_, k16, a_tiles, a_norms, st));
+    GB_CUDA(launch_coarse_topk(a_tiles, a_norms, nq, d_cent_tiles_, d_cent_norms_, nlist_, k16, seg_tiles, metric, nprobe, tau,
+                               part, st));
+    GB_CUDA(launch_select_keys(part, (int64_t)nseg * nprobe, nq, nseg * nprobe, nprobe, keys, nprobe, st));
+    GB_CUDA(launch_split_keys(keys, (int64_t)nq * nprobe, metric, coarse_dis, probe_ids, st));
+    return 0;
+  }
   int64_t ldo = round_up(nlist_, 4);
   GB_ALLOC(scores, float, (size_t)nq * ldo, s);
-  GB_ALLOC(keys, unsigned long long, (size_t)nq * nprobe, s);
   StageScope stage(this, "coarse_quantizer", st);
-  if (tc_enabled() && nlist_ >= 64 && nq >= 32) {
+  if (tc) {
     GB_CUDA(launch_dist_matrix_tc(xq, dpad_, nq, d_centroids_, dpad_, nlist_, dpad_, metric, scores, ldo, st));
   } else {
     GB_CUDA(launch_dist_matrix(xq, dpad_, nq, d_centroids_, dpad_, nlist_, dpad_, metric, scores, ldo, st));

@@ -384,6 +384,11 @@ class IVFFlatIndex : public Index {
 
   int nlist_;
   float* d_centroids_ = nullptr;  // [nlist][dpad]
+  // the centroids once more as tensor-core operand tiles (launch_tc_stage_rows) for the fused coarse quantiser, and
+  // |c|^2 per row; rebuilt by every change of d_centroids_ (rebuild_centroid_tiles)
+  float* d_cent_tiles_ = nullptr;
+  float* d_cent_norms_ = nullptr;
+  int rebuild_centroid_tiles(cudaStream_t st);
   std::unique_ptr<IvfLists> lists_;
   std::vector<uint64_t> vid2pos_;  // vid -> (list << 32 | pos), ~0 = not in a list (vid_bucket_no_pos_)
 

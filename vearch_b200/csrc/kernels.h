@@ -36,6 +36,19 @@ cudaError_t launch_dist_matrix_tc(const float* X, int64_t ldx, int n, const floa
                                   int metric, float* out, int64_t ldo, cudaStream_t st);
 cudaError_t launch_dist_argmin_tc(const float* X, int64_t ldx, int n, const float* C, int64_t ldc, int m, int d,
                                   int metric, unsigned long long* best, cudaStream_t st);
+// rows of x (n x d, stride ldx) -> 128-row operand tiles in the canonical tensor-core layout (per K = 16 chunk a
+// TF32 head and an fp32 remainder, tc_mirror_tile_floats(k16) floats per tile) and norms[row] = |x_row|^2; rows
+// past n are zero
+cudaError_t launch_tc_stage_rows(const float* x, int64_t ldx, int64_t n, int d, int k16, float* tiles, float* norms,
+                                 cudaStream_t st);
+// fused coarse quantiser (3xTF32 scores, bit-equal to launch_dist_matrix_tc): for every query q and centroid segment
+// s (seg_tiles 128-centroid tiles, nseg = ceil(ceil(nlist / 128) / seg_tiles)) the k best keys of the segment, in
+// any order, sentinel padded: out[(q * nseg + s) * k + i].  a_* / c_*: launch_tc_stage_rows of the queries and the
+// centroids; tau_g[nq] pre-set to the sentinel.
+constexpr int kCoarseMaxK = 64;
+cudaError_t launch_coarse_topk(const float* a_tiles, const float* a_norms, int nq, const float* c_tiles, const float* c_norms,
+                               int nlist, int k16, int seg_tiles, int metric, int k, unsigned long long* tau_g,
+                               unsigned long long* out, cudaStream_t st);
 
 // ---- K7: top-k selection / merge ----------------------------------------------------------
 // Per row r: select the k best of m candidates.  Input is either scores (fp32, vid = id_base+col)

@@ -4,6 +4,8 @@
 //    gamma_index_ivfpq.cc:595) and point x centroid (k-means assign, faiss Clustering via
 //    gamma_index_ivfflat.cc:407 / gamma_index_ivfpq.cc:372).  faiss itself evaluates this
 //    contraction as sgemm + norms (IndexFlat, >= 20 queries).
+//  * K2 fused  coarse_topk_kernel: the coarse quantiser's top-nprobe without a score matrix (TMA-fed, the
+//    same MMAs as dist_tc_kernel, per-query key sets in the epilogue).
 //  * K3 list-major: when many queries of a batch probe the same list the IVF-Flat scan
 //    (gamma_index_ivfflat.cc:579-787) IS a dense contraction.  The (query, probe) pairs are grouped by
 //    list on the device (lm_count / lmk_scan / lmk_assign / lmk_items); a work item multiplies a group
@@ -762,16 +764,172 @@ __global__ void tc_mirror_append_kernel(const float* __restrict__ x, int64_t ldx
   norms[gt * TC_N + p % TC_N] = tc_split_row(x + i * ldx, d, k16, p % TC_N, mirror + gt * ((int64_t)TC_N * k16 * 2));
 }
 
+// Stages 128-row operand tiles (canonical layout, hi + lo per K chunk) and their row norms.  With items: tile = pair
+// group, row r = the query of the group's pair r.  Without (items == nullptr): tile b = rows [128 b, 128 b + 128) of
+// x, rows past nrows zero (the coarse quantiser's query tiles and the centroid copy).
 __global__ void __launch_bounds__(TC_M)
     lm_stage_queries_kernel(const float* __restrict__ xq, int64_t ldq, int d, int k16, const LmTile* __restrict__ items,
-                            const int64_t* __restrict__ totals, const int64_t* __restrict__ pair_j, int nprobe,
+                            const int64_t* __restrict__ totals, const int64_t* __restrict__ pair_j, int nprobe, int64_t nrows,
                             float* __restrict__ a_scratch, float* __restrict__ a_norms) {
-  if ((int64_t)blockIdx.x >= totals[1]) return;
-  const LmTile t = items[blockIdx.x];
-  if (t.seg != 0) return;  // one staging per pair group: the first item of the group owns the slot
   const int r = threadIdx.x;
-  const float* src = r < t.npairs ? xq + (pair_j[t.pair0 + r] / nprobe) * ldq : nullptr;
-  a_norms[(int64_t)t.grp * TC_M + r] = tc_split_row(src, d, k16, r, a_scratch + (int64_t)t.grp * ((int64_t)TC_M * k16 * 2));
+  int64_t grp = blockIdx.x;
+  const float* src = nullptr;
+  if (items) {
+    if ((int64_t)blockIdx.x >= totals[1]) return;
+    const LmTile t = items[blockIdx.x];
+    if (t.seg != 0) return;  // one staging per pair group: the first item of the group owns the slot
+    grp = t.grp;
+    if (r < t.npairs) src = xq + (pair_j[t.pair0 + r] / nprobe) * ldq;
+  } else if (grp * TC_M + r < nrows) {
+    src = xq + (grp * TC_M + r) * ldq;
+  }
+  a_norms[grp * TC_M + r] = tc_split_row(src, d, k16, r, a_scratch + grp * ((int64_t)TC_M * k16 * 2));
+}
+
+// ---- K2 fused: the coarse quantiser's top-nprobe on the tensor cores ----------------------------
+// The coarse quantiser's key set: the same admission rule and the same kept set as lmk_consider, but once full the
+// k keys form a max-heap, so a replacement costs one sift-down (log2 k levels of two independent shared loads)
+// instead of a scan of all k slots.  Nearly every key a query admits past the first k replaces one, and these
+// dependent shared-memory chains are what the epilogue waits on.
+__device__ __forceinline__ void ck_sift_down(unsigned long long* hk, int k, int i, unsigned long long key) {
+  for (;;) {
+    const int l = 2 * i + 1;
+    if (l >= k) break;
+    const unsigned long long vl = hk[l * TC_NT], vr = l + 1 < k ? hk[(l + 1) * TC_NT] : 0ull;
+    const int c = vr > vl ? l + 1 : l;
+    const unsigned long long vc = vr > vl ? vr : vl;
+    if (vc <= key) break;
+    hk[i * TC_NT] = vc;
+    i = c;
+  }
+  hk[i * TC_NT] = key;
+}
+
+template <int METRIC>
+__device__ __noinline__ LmkState ck_consider(unsigned long long* hk, int k, uint32_t vid, float sc, LmkState st) {
+  // the score window of select_rows_kernel: non-finite scores never enter
+  if (vid == kLmkNoVid || !(sc <= FLT_MAX && sc >= -FLT_MAX)) return st;
+  const unsigned long long key = make_key(score2ord<METRIC>(sc), vid);
+  if (key >= st.tau) return st;
+  if (st.n < k) {
+    hk[st.n * TC_NT] = key;
+    if (++st.n < k) return st;
+    for (int i = k / 2 - 1; i >= 0; i--) ck_sift_down(hk, k, i, hk[i * TC_NT]);  // the set is full: heapify
+  } else {
+    ck_sift_down(hk, k, 0, key);  // key < st.tau <= the largest key: it replaces the top
+  }
+  const unsigned long long mx = hk[0];
+  if (mx < st.tau) st.tau = mx;
+  return st;
+}
+
+// Work item = (128-query tile, segment of consecutive 128-centroid tiles).  Both operands sit in global memory in
+// the canonical operand layout (queries staged per call, centroids whenever they change), so the CTA is fed as
+// ivf_listmajor_tma_kernel is: warp 4 issues cp.async.bulk copies into a ring, warpgroup 0 runs the wgmma sequence of
+// dist_tc_kernel (the same chunks, MMAs and order, so every score is bit-equal to the matrix that kernel writes) and
+// thread t keeps query t's k best keys of the segment.  Segments of one query share their bound through tau_g.
+// A column leaves the hot loop only if it beats the thread's bound; each lane then walks its OWN hits, re-reading
+// the dot product from the slab, so a warp iterates as often as its busiest lane and not once per column that any
+// lane hit (early in a segment nearly every column is a hit somewhere in the warp).
+template <int METRIC>
+__global__ void __launch_bounds__(LT_NT, 1)
+    coarse_topk_kernel(const float* __restrict__ a_tiles, const float* __restrict__ a_norms, int nq,
+                       const float* __restrict__ c_tiles, const float* __restrict__ c_norms, int nlist, int k16,
+                       int seg_tiles, int nseg, int k, unsigned long long* tau_g, unsigned long long* __restrict__ out) {
+  extern __shared__ __align__(1024) unsigned char smem[];  // [ring: NST * STAGE] [slabs] [key sets: k * 1 KiB]
+  __shared__ LtShared sh;
+  constexpr int NST = LT_STAGES;
+  constexpr int STAGE = TC_STAGE_BYTES;
+  const int tid = threadIdx.x, warp = tid >> 5;
+  const int qt = blockIdx.x / nseg, sg = blockIdx.x - qt * nseg;
+  const int ct0 = sg * seg_tiles;
+  const int ntiles = min(seg_tiles, (nlist + TC_N - 1) / TC_N - ct0);
+  const int nk = k16 / TC_BK;
+  unsigned char* ring = smem;
+
+  if (tid == 0) {
+    for (int s = 0; s < NST; s++) {
+      mbar_init(&sh.full[s], 1);      // the producer's arrive.expect_tx; the copies complete the phase
+      mbar_init(&sh.empty[s], TC_M);  // every MMA thread arrives
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ======================= MMA + epilogue =======================
+    unsigned long long* hk = reinterpret_cast<unsigned long long*>(ring + (size_t)NST * STAGE + kSlabBytes) + tid;
+    float* slabs = reinterpret_cast<float*>(ring + (size_t)NST * STAGE);
+    const int q = qt * TC_M + tid;
+    const bool valid = q < nq;
+    LmkState st{valid ? __ldcg(tau_g + q) : 0ull, 0};  // bound 0: padding rows admit nothing
+    float bound = key_bound<METRIC>(st.tau);
+    const float xn = a_norms[q];
+    float acc[2][64];
+    for (int i = 0; i < ntiles; i++) {
+      const int b = i & 1, ct = ct0 + i;
+      const float cn = c_norms[ct * TC_N + tid];  // issued before the MMAs, stored after them
+      ring_tile_mma<NST, STAGE>(acc, smem_u32(ring), sh.full, sh.empty, i * nk, nk, TC_TILE_BYTES, LT_HALF,
+                                LT_HALF + TC_TILE_BYTES);
+      sh.cn[b][tid] = cn;  // buffer b was last read in tile i - 2, before tile i - 1's exchange barriers
+      sh.vid[b][tid] = ct * TC_N + tid < nlist ? (uint32_t)(ct * TC_N + tid) : kLmkNoVid;
+#pragma unroll
+      for (int c0 = 0; c0 < TC_N; c0 += 32) {
+        uint32_t v[32];
+        acc_cols(acc, c0, slabs, v);
+        uint32_t hit = 0;
+#pragma unroll
+        for (int j4 = 0; j4 < 32; j4 += 4) {
+          const float4 c4 = *reinterpret_cast<const float4*>(&sh.cn[b][c0 + j4]);
+          const float cc[4] = {c4.x, c4.y, c4.z, c4.w};
+#pragma unroll
+          for (int u = 0; u < 4; u++) {
+            const float sc = tc_score<METRIC>(__uint_as_float(v[j4 + u]), xn, cc[u]);
+            hit |= (METRIC == kMetricL2 ? sc <= bound : sc >= bound) ? (1u << (j4 + u)) : 0u;
+          }
+        }
+        const float* srow = slabs + ((c0 >> 5) & 1) * kSlabFloats + tid * 32;  // this thread's row (acc_cols layout)
+        while (hit) {
+          const int jj = __ffs(hit) - 1;
+          hit &= hit - 1;
+          const float sc = tc_score<METRIC>(srow[(((jj >> 2) ^ (tid & 7)) << 2) | (jj & 3)], xn, sh.cn[b][c0 + jj]);
+          st = ck_consider<METRIC>(hk, k, sh.vid[b][c0 + jj], sc, st);
+        }
+        bound = key_bound<METRIC>(st.tau);
+      }
+      if (valid) {  // exchange bounds with the other segments of this query
+        const unsigned long long tg = __ldcg(tau_g + q);
+        if (tg < st.tau) {
+          st.tau = tg;
+          bound = key_bound<METRIC>(st.tau);
+        } else if (st.tau < tg) {
+          atomicMin(tau_g + q, st.tau);
+        }
+      }
+    }
+    if (valid) {
+      unsigned long long* o = out + ((int64_t)q * nseg + sg) * k;
+      for (int i = 0; i < k; i++) o[i] = i < st.n ? hk[i * TC_NT] : kKeySentinel;
+    }
+  } else {
+    // ======================= TMA producer (whole warp loops, one elected lane issues) =======================
+    const char* asrc = reinterpret_cast<const char*>(a_tiles) + (int64_t)qt * nk * LT_HALF;
+    const char* bsrc = reinterpret_cast<const char*>(c_tiles) + (int64_t)ct0 * nk * LT_HALF;
+    int n = 0;
+    for (int i = 0; i < ntiles; i++) {
+      for (int kc = 0; kc < nk; kc++, n++) {
+        const int s = n % NST;
+        mbar_wait(&sh.empty[s], (uint32_t)(((n / NST) & 1) ^ 1));
+        if (elect_one()) {
+          unsigned char* stage = ring + (size_t)s * STAGE;
+          mbar_arrive_expect_tx(&sh.full[s], STAGE);
+          bulk_g2s(stage, asrc + (int64_t)kc * LT_HALF, LT_HALF, &sh.full[s]);
+          bulk_g2s(stage + LT_HALF, bsrc + ((int64_t)i * nk + kc) * LT_HALF, LT_HALF, &sh.full[s]);
+        }
+        __syncwarp();
+      }
+    }
+  }
 }
 
 // ---- grouping for the fused kernel: histogram (lm_count_kernel) -> scan -> slots -> items ----
@@ -1130,9 +1288,46 @@ cudaError_t launch_lm_stage_queries(const float* xq, int64_t ldq, int d, int k16
                                     const int64_t* totals, const int64_t* pair_j, int nprobe, float* a_scratch,
                                     float* a_norms, cudaStream_t st) {
   if (max_items <= 0) return cudaSuccess;
-  lm_stage_queries_kernel<<<max_items, TC_M, 0, st>>>(xq, ldq, d, k16, items, totals, pair_j, nprobe, a_scratch, a_norms);
+  lm_stage_queries_kernel<<<max_items, TC_M, 0, st>>>(xq, ldq, d, k16, items, totals, pair_j, nprobe, 0, a_scratch, a_norms);
   note_launch();
   return cudaGetLastError();
+}
+
+cudaError_t launch_tc_stage_rows(const float* x, int64_t ldx, int64_t n, int d, int k16, float* tiles, float* norms,
+                                 cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
+  if ((d & 3) || (ldx & 3) || (k16 % TC_BK) || k16 < d) return cudaErrorInvalidValue;
+  lm_stage_queries_kernel<<<(unsigned)((n + TC_M - 1) / TC_M), TC_M, 0, st>>>(x, ldx, d, k16, nullptr, nullptr, nullptr, 1, n,
+                                                                              tiles, norms);
+  note_launch();
+  return cudaGetLastError();
+}
+
+template <int METRIC>
+static cudaError_t launch_coarse_topk_t(const float* a_tiles, const float* a_norms, int nq, const float* c_tiles,
+                                        const float* c_norms, int nlist, int k16, int seg_tiles, int nseg, int k,
+                                        unsigned long long* tau_g, unsigned long long* out, cudaStream_t st) {
+  const size_t smem = (size_t)LT_RING + kSlabBytes + (size_t)k * TC_NT * 8;
+  cudaError_t e = cudaFuncSetAttribute(coarse_topk_kernel<METRIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  const int64_t grid = (int64_t)((nq + TC_M - 1) / TC_M) * nseg;
+  coarse_topk_kernel<METRIC><<<(unsigned)grid, LT_NT, smem, st>>>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16,
+                                                                  seg_tiles, nseg, k, tau_g, out);
+  note_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_coarse_topk(const float* a_tiles, const float* a_norms, int nq, const float* c_tiles, const float* c_norms,
+                               int nlist, int k16, int seg_tiles, int metric, int k, unsigned long long* tau_g,
+                               unsigned long long* out, cudaStream_t st) {
+  const int ntc = (nlist + TC_N - 1) / TC_N;
+  if (k <= 0 || k > kCoarseMaxK || k16 <= TC_BK || (k16 % TC_BK) || seg_tiles <= 0) return cudaErrorInvalidValue;
+  if (nq <= 0 || nlist <= 0) return cudaSuccess;
+  const int nseg = (ntc + seg_tiles - 1) / seg_tiles;
+  if ((int64_t)((nq + TC_M - 1) / TC_M) * nseg > INT32_MAX) return cudaErrorInvalidValue;
+  return metric == kMetricL2
+             ? launch_coarse_topk_t<kMetricL2>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16, seg_tiles, nseg, k, tau_g, out, st)
+             : launch_coarse_topk_t<kMetricIP>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16, seg_tiles, nseg, k, tau_g, out, st);
 }
 
 template <int METRIC>
