@@ -580,13 +580,14 @@ def test_request_coalescing_matches_direct_search(ivf_state, ivfflat_index):
     (16, 10, 64, "ivf_listmajor_tma_kernel"),   # TMA-fed pipeline over the pre-tiled mirror
     (6, 10, 64, "ivf_listmajor_tma_kernel"),    # lists > 2048 rows: row segments
     (16, 10, 72, "ivf_listmajor_tma_kernel"),   # d not a multiple of the K chunk: zero-padded tail
-    (16, 64, 64, "ivf_listmajor_topk_kernel"),  # 32 < k <= 64: register-staged pipeline
-    (16, 10, 16, "ivf_listmajor_topk_kernel"),  # a single K chunk per tile: the plain fused kernel
+    (16, 64, 64, "ivf_listmajor_pipe_kernel"),  # 32 < k <= 64: register-staged pipeline
+    (16, 10, 16, "ivf_listmajor_pipe_kernel"),  # d <= 16: one K chunk of data, padded to two
     (16, 100, 64, "ivf_listmajor_tc_kernel+seg_select_kernel")])
 def test_ivfflat_listmajor_tensor_core_scan_matches_oracle(metric, nlist, k, d, kernel):
     """Many queries per list => the list-major grouped-GEMM scan (kernels_tc.cu) is selected: fused
-    top-k epilogue for k <= 64 (fed by TMA from the mirror for k <= 32), dense score segments +
-    segment select above.  Integer data: scores bit-equal to the oracle; filters and tombstones honoured."""
+    top-k epilogue for k <= 64 (fed by TMA from the mirror for k <= 32 and d > 16, else the
+    register-staged pipeline), dense score segments + segment select above.  Integer data: scores
+    bit-equal to the oracle; filters and tombstones honoured."""
     n, nq, nprobe = 30000, 700, 6
     db = synth.sift_like(n, d, seed=95)
     xq = synth.sift_like(nq, d, seed=96)

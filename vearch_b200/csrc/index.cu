@@ -1341,18 +1341,10 @@ int IVFFlatIndex::coarse_dev(int nq, const float* xq, int nprobe, int metric, in
 // Host side: group the (query, probe) pairs by list (stable counting sort), give every pair a
 // score segment of len(list) floats, cut (list, 128 pairs, 128 rows) tiles; device side: grouped
 // GEMM on wgmma + segment select.
-// GB_LISTMAJOR: 0 = off, 1 = on (fused top-k epilogue when k allows), 2 = on, always the dense-score variant
-static int listmajor_mode() {  // read per call: tests flip it between searches of one process
+// GB_LISTMAJOR=0: never list-major.  Read per call: tests flip it between searches of one process.
+static bool listmajor_enabled() {
   const char* e = getenv("GB_LISTMAJOR");
-  return e ? atoi(e) : 1;
-}
-static bool listmajor_enabled() { return listmajor_mode() != 0; }
-static bool tma_enabled() {  // GB_TC_MIRROR=0: never build the pre-tiled mirror (register-staged kernel)
-  static int v = [] {
-    const char* e = getenv("GB_TC_MIRROR");
-    return e ? atoi(e) : 1;
-  }();
-  return v != 0;
+  return e ? atoi(e) != 0 : true;
 }
 
 // called from index_batch with mu_ held exclusively: no search is inside ensure_mirror.  Kernels of an
@@ -1440,10 +1432,10 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
                                      const int32_t* probe_ids, int nprobe, unsigned long long* out_keys, Scratch& s) {
   if (!tc_enabled() || !listmajor_enabled()) return 1;
   const int64_t npairs = (int64_t)nq * nprobe;
-  if (npairs < (int64_t)nlist_ * 32 && !getenv("GB_LISTMAJOR_FORCE")) return 1;  // < 32 queries per list on average
+  if (npairs < (int64_t)nlist_ * 32) return 1;  // < 32 queries per list on average
   cudaStream_t st = s.stream();
   ListDirectory dir = lists_->directory();
-  if (k <= kLmkMaxK && listmajor_mode() != 2) {
+  if (k <= kLmkMaxK) {
     // fused top-k epilogue: no score round trip through HBM, no host synchronisation
     const int nseg = (int)std::min<int64_t>(8, std::max<int64_t>(1, (lists_->max_len() + kLmkSegRows - 1) / kLmkSegRows));
     const int64_t max_items = (npairs / 128 + nlist_) * nseg;
@@ -1467,7 +1459,8 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
     const int64_t max_groups = npairs / 128 + nlist_;
     const size_t slot_bytes = (size_t)128 * k16 * 8, a_bytes = (size_t)max_groups * (slot_bytes + 128 * 4);
     std::shared_lock<std::shared_mutex> mlk(mirror_rw_, std::defer_lock);
-    bool tma = tma_enabled() && k <= 32 && k16 > 16 && a_bytes <= ((size_t)8 << 30) && ensure_mirror(mlk, st) == 0;
+    // TMA-fed from the mirror when it applies and fits, else the register-staged pipeline over the lists themselves
+    bool tma = k <= 32 && k16 > 16 && a_bytes <= ((size_t)8 << 30) && ensure_mirror(mlk, st) == 0;
     if (tma) {
       float* a_scratch = static_cast<float*>(big_acquire(a_bytes, st));
       if (!a_scratch) return -1;
@@ -1483,9 +1476,9 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
                                        nseg, metric, f, d_tau, d_out, st));
       scan_timer_end(st);
     } else {
-      last_scan_kernel_ = "ivf_listmajor_topk_kernel";
+      last_scan_kernel_ = "ivf_listmajor_pipe_kernel";
       scan_timer_begin(st);
-      GB_CUDA(launch_ivf_listmajor_topk(xq, dpad_, dpad_, d_items, (int)max_items, d_totals, d_pair_j, nprobe, dir, k, nseg,
+      GB_CUDA(launch_ivf_listmajor_pipe(xq, dpad_, dpad_, d_items, (int)max_items, d_totals, d_pair_j, nprobe, dir, k, nseg,
                                         metric, f, d_tau, d_out, st));
       scan_timer_end(st);
     }

@@ -137,7 +137,8 @@ cudaError_t launch_ivf_listmajor_tma(const float* a_scratch, const float* a_norm
                                      int max_items, const int64_t* totals, const int64_t* pair_j, int nprobe,
                                      ListDirectory dir, int k, int nseg_max, int metric, FilterArgs f,
                                      unsigned long long* tau_g, unsigned long long* out, cudaStream_t st);
-cudaError_t launch_ivf_listmajor_topk(const float* xq, int64_t ldq, int d, const LmTile* items, int max_items,
+// register-staged variant: reads the lists themselves (no mirror), any d
+cudaError_t launch_ivf_listmajor_pipe(const float* xq, int64_t ldq, int d, const LmTile* items, int max_items,
                                       const int64_t* totals, const int64_t* pair_j, int nprobe, ListDirectory dir, int k,
                                       int nseg_max, int metric, FilterArgs f, unsigned long long* tau_g,
                                       unsigned long long* out, cudaStream_t st);

@@ -6,17 +6,17 @@
 //     skip if ids[j] & kDelIdxMask, skip if !IsValid(vid), dis = L2sqr/IP(x, vec_j),
 //     keep if IsSimilarScoreValid(dis) and better than the current k-th best.
 //
-// One CTA per (query, probed list, list split).  The list's rows stream HBM -> shared memory
-// through a 4-stage ring of TMA 1-D bulk copies (cp.async.bulk + mbarrier complete_tx), so the
-// copy engine keeps 4 x 16 KB in flight per CTA with no register staging.  LPR lanes share one
-// row (float4 chunks, rotated start so both the row and the query reads are bank-conflict-free),
-// partial sums meet through warp shuffles, and candidates that beat the running k-th best go to
-// the CandQueue (common.cuh).  List ids are only read for candidates that beat the threshold.
+// Two kernels.  ivfflat_scan_warp_kernel serves every d with a compile-time geometry (dispatch_warp);
+// ivfflat_scan_kernel, the generic one, any other d: one CTA per (query, probed list, list split).
+// The list's rows stream HBM -> shared memory through a 4-stage ring of TMA 1-D bulk copies
+// (cp.async.bulk + mbarrier complete_tx), so the copy engine keeps 4 x 16 KB in flight per CTA with
+// no register staging.  LPR lanes share one row (float4 chunks, rotated start so both the row and
+// the query reads are bank-conflict-free), partial sums meet through warp shuffles, and candidates
+// that beat the running k-th best go to the CandQueue (common.cuh).  List ids are only read for
+// candidates that beat the threshold.
 //
 // Algorithmic bytes: (4*d + 8) per scanned entry (SURVEY.md 8d); roofline: HBM.
 #include <float.h>
-#include <stdlib.h>
-#include <string.h>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -172,220 +172,18 @@ void ivf_cq_geometry(int k, int T, int* KP, int* SORTN) {
   *SORTN = next_pow2(*KP + 2 * T);
 }
 
-// ---- fast path: compile-time geometry ---------------------------------------------------
-// LPR >= 8 lanes share a row, lane p owns float4 chunks {p + LPR*j, j < J} (S = LPR*J).  A
-// quarter-warp then reads 8 consecutive float4 of ONE row, so shared-memory reads are
-// conflict-free without rotation and the query chunks sit in registers (4*J floats per lane).
-// One __syncthreads_count per tile both releases the stage and gives every thread the same
-// upper bound on the queue fill, so the flush decision needs no second barrier.
-constexpr int IVF_MAX_PG = 32;  // work items (probe, split) per CTA
-
-template <int METRIC, int LPR, int J>
-__global__ void __launch_bounds__(IVF_NT)
-    ivfflat_scan_fast_kernel(const float* __restrict__ xq, int64_t ldq, const int32_t* __restrict__ probe_ids,
-                             int nprobe, int nsplit, int pg, ListDirectory dir, int R, int nst, int k, int KP, int SORTN,
-                             FilterArgs f, unsigned long long* __restrict__ partial) {
-  constexpr int S = LPR * J;        // float4 per row
-  constexpr int G = IVF_NT / LPR;   // rows per round
-  constexpr int ROW_BYTES = S * 16;
-  const int T = G * R;
-  const int stage_bytes = T * ROW_BYTES;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  unsigned long long* buf = reinterpret_cast<unsigned long long*>(smem_raw + (size_t)nst * stage_bytes);
-  __shared__ __align__(8) uint64_t full_bar[8];
-  __shared__ int s_cnt;
-  __shared__ unsigned long long s_tau;
-  __shared__ int g_list[IVF_MAX_PG], g_r0[IVF_MAX_PG], g_r1[IVF_MAX_PG], g_tile0[IVF_MAX_PG + 1];
-
-  const int tid = threadIdx.x;
-  const int q = blockIdx.y, grp_id = blockIdx.x;
-  unsigned long long* out = partial + ((int64_t)q * gridDim.x + grp_id) * k;
-  const int nitems = nprobe * nsplit;
-  const int i0 = grp_id * pg;
-  const int ni = min(pg, nitems - i0);
-
-  if (tid == 0) {
-    int acc = 0;
-    for (int i = 0; i < ni; i++) {
-      const int item = i0 + i;
-      const int probe = item / nsplit, split = item - probe * nsplit;
-      const int list = probe_ids[(int64_t)q * nprobe + probe];
-      int len = 0;
-      if (list >= 0 && list < dir.nlist) len = dir.len[list];  // key < 0: "not enough centroids" (ivfflat.cc:653)
-      const int r0 = split * IVF_CHUNK_ROWS;
-      const int r1 = min(len, r0 + IVF_CHUNK_ROWS);
-      g_list[i] = list;
-      g_r0[i] = r0;
-      g_r1[i] = r1 > r0 ? r1 : r0;
-      g_tile0[i] = acc;
-      acc += r1 > r0 ? (r1 - r0 + T - 1) / T : 0;
-    }
-    g_tile0[ni > 0 ? ni : 0] = acc;
-    for (int s = 0; s < nst; s++) mbar_init(&full_bar[s], 1);
-    mbar_fence_init();
-  }
-  CandQueue cq{buf, &s_cnt, &s_tau, k, KP, SORTN};
-  cq.init();  // __syncthreads inside
-  const int total_tiles = ni > 0 ? g_tile0[ni] : 0;
-  if (total_tiles == 0) {
-    for (int i = tid; i < k; i += IVF_NT) out[i] = kKeySentinel;
-    return;
-  }
-
-  const int grp = tid / LPR, p = tid % LPR;
-  float4 qreg[J];
-  {
-    const float4* q4 = reinterpret_cast<const float4*>(xq + (int64_t)q * ldq);
-#pragma unroll
-    for (int j = 0; j < J; j++) qreg[j] = __ldg(q4 + p + LPR * j);
-  }
-
-  // producer (thread 0): walks the same (item, tile) sequence NST tiles ahead of the consumers,
-  // so the ring keeps streaming across list boundaries
-  int pr_pi = 0;
-  auto issue = [&](int gt) {
-    while (gt >= g_tile0[pr_pi + 1]) pr_pi++;
-    const int ti = gt - g_tile0[pr_pi];
-    const int row0 = g_r0[pr_pi] + ti * T;
-    const int rows = min(T, g_r1[pr_pi] - row0);
-    const uint32_t bytes = (uint32_t)rows * ROW_BYTES;
-    const int s = gt % nst;
-    mbar_arrive_expect_tx(&full_bar[s], bytes);
-    bulk_g2s(smem_raw + (size_t)s * stage_bytes, dir.vecs[g_list[pr_pi]] + (int64_t)row0 * (S * 4), bytes, &full_bar[s]);
-  };
-  if (tid == 0)
-    for (int gt = 0; gt < nst && gt < total_tiles; gt++) issue(gt);
-
-  int pi = 0;
-  const int64_t* __restrict__ lids = nullptr;
-  int cur = -1;
-  int est = 0;  // upper bound of the queue fill, identical in every thread
-  for (int gt = 0; gt < total_tiles; gt++) {
-    while (gt >= g_tile0[pi + 1]) pi++;
-    if (pi != cur) {
-      cur = pi;
-      lids = dir.ids[g_list[pi]];
-    }
-    const int ti = gt - g_tile0[pi];
-    const int row0 = g_r0[pi] + ti * T;
-    const int tile_rows = min(T, g_r1[pi] - row0);
-    const int s = gt % nst;
-    mbar_wait(&full_bar[s], (gt / nst) & 1);
-    const unsigned long long tau = s_tau;
-    const uint32_t tau_hi = (uint32_t)(tau >> 32);
-    const float4* st4 = reinterpret_cast<const float4*>(smem_raw + (size_t)s * stage_bytes);
-    int pushed = 0;
-    for (int r = 0; r < R; r++) {
-      const int rit = r * G + grp;
-      const bool valid = rit < tile_rows;
-      float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-      if (valid) {
-        const float4* rowp = st4 + (size_t)rit * S + p;
-#pragma unroll
-        for (int j = 0; j < J; j++) {
-          float4 v = rowp[LPR * j];
-          float4 w = qreg[j];
-          if (METRIC == kMetricL2) {
-            float t0 = v.x - w.x, t1 = v.y - w.y, t2 = v.z - w.z, t3 = v.w - w.w;
-            a0 = fmaf(t0, t0, a0), a1 = fmaf(t1, t1, a1), a2 = fmaf(t2, t2, a2), a3 = fmaf(t3, t3, a3);
-          } else {
-            a0 = fmaf(v.x, w.x, a0), a1 = fmaf(v.y, w.y, a1), a2 = fmaf(v.z, w.z, a2), a3 = fmaf(v.w, w.w, a3);
-          }
-        }
-      }
-      float dis = (a0 + a1) + (a2 + a3);
-#pragma unroll
-      for (int off = LPR >> 1; off > 0; off >>= 1) dis += __shfl_xor_sync(0xffffffffu, dis, off);
-
-      bool pred = valid && p == 0 && dis <= f.max_score && dis >= f.min_score;
-      unsigned long long key = kKeySentinel;
-      if (pred) {
-        uint32_t ord = score2ord<METRIC>(dis);
-        pred = ord <= tau_hi;
-        if (pred) {
-          int64_t raw = lids[row0 + rit];
-          pred = raw >= 0;  // top bit set => tombstone (gamma_index_ivfflat.h:72)
-          uint32_t vid = (uint32_t)raw;
-          if (pred) pred = ctx_is_valid(f.del_bits, f.filter_bits, vid);
-          key = make_key(ord, vid);
-          pred = pred && key < tau;
-        }
-      }
-      cq.push_warp(pred, key);
-      pushed |= pred ? 1 : 0;
-    }
-    // stage s consumed + pushes done; the count is the same value in every thread
-    est += __syncthreads_count(pushed) * R;
-    if (tid == 0 && gt + nst < total_tiles) issue(gt + nst);
-    if (gt + 1 < total_tiles && est + T > cq.cap()) {
-      cq.flush();
-      est = 0;
-    }
-  }
-  __syncthreads();
-  cq.flush(true);
-  for (int i = tid; i < k; i += IVF_NT) out[i] = buf[i];
-}
-
-struct FastCfg {
-  int pg, nst, stage_bytes;
-  int warp_mode;  // 1: warp-autonomous kernel (per-warp TMA rings), 0: block-synchronous ring
-};
-inline FastCfg fast_cfg(int nprobe, int nsplit, int avg_len) {
-  FastCfg c;
-  // resident CTAs matter more than ring depth, so the rings stay shallow: by default the
-  // warp-autonomous kernel with 4 KiB per warp per ring slot and 2 slots; GB_IVF_MODE /
-  // GB_IVF_STAGE_KB / GB_IVF_NST / GB_IVF_PG override the choice for sweeps
-  c.stage_bytes = 16 * 1024;
-  c.nst = 2;
-  c.warp_mode = 1;
-  if (const char* e = getenv("GB_IVF_MODE")) c.warp_mode = !strcmp(e, "warp");
-  if (!c.warp_mode) c.stage_bytes = 8 * 1024;
-  // ~16k rows of work per CTA: enough tiles to amortise start-up, enough CTAs to balance
-  int per = avg_len > 0 ? 16384 / avg_len : 1;
-  c.pg = per < 1 ? 1 : (per > IVF_MAX_PG ? IVF_MAX_PG : per);
-  if (nsplit > 1) c.pg = 1;
-  if (const char* e = getenv("GB_IVF_STAGE_KB")) c.stage_bytes = atoi(e) * 1024;
-  if (const char* e = getenv("GB_IVF_NST")) c.nst = atoi(e);
-  if (const char* e = getenv("GB_IVF_PG")) c.pg = atoi(e);
-  if (c.nst < 2) c.nst = 2;
-  if (c.nst > 8) c.nst = 8;
-  if (c.pg < 1) c.pg = 1;
-  if (c.pg > IVF_MAX_PG) c.pg = IVF_MAX_PG;
-  if (c.pg > nprobe * nsplit) c.pg = nprobe * nsplit;
-  return c;
-}
-
-template <int METRIC, int LPR, int J>
-cudaError_t launch_fast(const float* xq, int64_t ldq, int nq, const int32_t* probe_ids, int nprobe, int nsplit,
-                        FastCfg c, ListDirectory dir, int k, FilterArgs f, unsigned long long* partial,
-                        cudaStream_t st) {
-  constexpr int S = LPR * J, G = IVF_NT / LPR, ROW_BYTES = S * 16;
-  int R = c.stage_bytes / (G * ROW_BYTES);
-  if (R < 1) R = 1;
-  const int T = G * R;
-  int KP, SORTN;
-  ivf_cq_geometry(k, T, &KP, &SORTN);
-  size_t smem = (size_t)c.nst * T * ROW_BYTES + (size_t)SORTN * 8;
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;
-  cudaError_t e = cudaFuncSetAttribute(ivfflat_scan_fast_kernel<METRIC, LPR, J>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  const int nitems = nprobe * nsplit;
-  dim3 grid((nitems + c.pg - 1) / c.pg, nq);
-  ivfflat_scan_fast_kernel<METRIC, LPR, J><<<grid, IVF_NT, smem, st>>>(xq, ldq, probe_ids, nprobe, nsplit, c.pg, dir, R,
-                                                                       c.nst, k, KP, SORTN, f, partial);
-  note_launch();
-  return cudaGetLastError();
-}
-
-// ---- warp-autonomous variant ---------------------------------------------------------------
-// Same work decomposition as the fast kernel (one CTA per query x group of (probe, split) items,
-// flat tile sequence), but every WARP owns its slice of the tile sequence (tiles w, w+4, ...), its
+// ---- fixed-geometry kernel (dimensions with an instantiation) --------------------------------
+// One CTA per query x group of pg (probe, split) work items; the group's rows form one flat tile
+// sequence across list boundaries.  Every WARP owns its slice of that sequence (tiles w, w+4, ...), its
 // own ring of TMA bulk copies with its own mbarriers (lane 0 produces), its own threshold and its
 // own candidate queue (count and tau live in registers, pushes are ballot-compacted, flushes are
 // warp-level bitonic sorts).  No block-wide barrier exists until the final 4-way merge, so a warp
 // never waits for another warp's memory latency.
+// LPR >= 8 lanes share a row, lane p owns float4 chunks {p + LPR*j, j < J} (S = LPR*J).  A
+// quarter-warp then reads 8 consecutive float4 of ONE row, so shared-memory reads are
+// conflict-free without rotation and the query chunks sit in registers (4*J floats per lane).
+constexpr int IVF_MAX_PG = 32;  // work items (probe, split) per CTA
+
 __device__ __forceinline__ void warp_bitonic_sort(unsigned long long* a, int n, int lane) {
   for (int k = 2; k <= n; k <<= 1) {
     for (int j = k >> 1; j > 0; j >>= 1) {
@@ -407,6 +205,11 @@ __device__ __forceinline__ void warp_bitonic_sort(unsigned long long* a, int n, 
 
 constexpr int IVF_NWARP = IVF_NT / 32;
 constexpr int IVF_MAX_NST = 8;
+// ring geometry, a sweep result: resident CTAs matter more than ring depth, so the rings stay shallow --
+// 16 KiB per CTA per ring slot (4 KiB per warp) and 2 slots
+constexpr int IVF_WARP_STAGE_BYTES = 16 * 1024;
+constexpr int IVF_WARP_NST = 2;
+static_assert(IVF_WARP_NST <= IVF_MAX_NST, "the kernel holds at most IVF_MAX_NST mbarriers per warp");
 
 template <int METRIC, int LPR, int J>
 __global__ void __launch_bounds__(IVF_NT)
@@ -566,56 +369,63 @@ __global__ void __launch_bounds__(IVF_NT)
   for (int i = tid; i < k; i += IVF_NT) out[i] = fin[i];
 }
 
+// work items (probe, split) per CTA: ~16k rows of work per CTA, enough tiles to amortise start-up, enough CTAs to
+// balance; one item per CTA when lists are split
+inline int warp_pg(int nprobe, int nsplit, int avg_len) {
+  const int per = avg_len > 0 ? 16384 / avg_len : 1;
+  int pg = per < 1 ? 1 : (per > IVF_MAX_PG ? IVF_MAX_PG : per);
+  if (nsplit > 1) pg = 1;
+  return pg > nprobe * nsplit ? nprobe * nsplit : pg;
+}
+
 template <int METRIC, int LPR, int J>
-cudaError_t launch_warp(const float* xq, int64_t ldq, int nq, const int32_t* probe_ids, int nprobe, int nsplit,
-                        FastCfg c, ListDirectory dir, int k, FilterArgs f, unsigned long long* partial,
-                        cudaStream_t st) {
+cudaError_t launch_warp(const float* xq, int64_t ldq, int nq, const int32_t* probe_ids, int nprobe, int nsplit, int pg,
+                        ListDirectory dir, int k, FilterArgs f, unsigned long long* partial, cudaStream_t st) {
   constexpr int S = LPR * J, RPW = 32 / LPR, ROW_BYTES = S * 16;
-  int R = c.stage_bytes / IVF_NWARP / (RPW * ROW_BYTES);  // stage_bytes = per-CTA bytes per ring slot
+  int R = IVF_WARP_STAGE_BYTES / IVF_NWARP / (RPW * ROW_BYTES);
   if (R < 1) R = 1;
   const int TW = RPW * R;
   const int KP = next_pow2(k < 16 ? 16 : k);
   const int SORTNW = next_pow2(KP + 2 * RPW + TW);
-  size_t smem = (size_t)IVF_NWARP * c.nst * TW * ROW_BYTES + (size_t)IVF_NWARP * SORTNW * 8 + (size_t)IVF_NWARP * KP * 8;
+  size_t smem =
+      (size_t)IVF_NWARP * IVF_WARP_NST * TW * ROW_BYTES + (size_t)IVF_NWARP * SORTNW * 8 + (size_t)IVF_NWARP * KP * 8;
   if (smem > 227 * 1024) return cudaErrorInvalidValue;
   cudaError_t e = cudaFuncSetAttribute(ivfflat_scan_warp_kernel<METRIC, LPR, J>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   const int nitems = nprobe * nsplit;
-  dim3 grid((nitems + c.pg - 1) / c.pg, nq);
-  ivfflat_scan_warp_kernel<METRIC, LPR, J><<<grid, IVF_NT, smem, st>>>(xq, ldq, probe_ids, nprobe, nsplit, c.pg, dir, R,
-                                                                       c.nst, k, KP, SORTNW, f, partial);
+  dim3 grid((nitems + pg - 1) / pg, nq);
+  ivfflat_scan_warp_kernel<METRIC, LPR, J><<<grid, IVF_NT, smem, st>>>(xq, ldq, probe_ids, nprobe, nsplit, pg, dir, R,
+                                                                       IVF_WARP_NST, k, KP, SORTNW, f, partial);
   note_launch();
   return cudaGetLastError();
 }
 
 // returns cudaErrorNotSupported when no instantiation fits (caller falls back to the generic kernel)
 template <int METRIC>
-cudaError_t dispatch_fast(int S, const float* xq, int64_t ldq, int nq, const int32_t* probe_ids, int nprobe,
-                          int nsplit, FastCfg c, ListDirectory dir, int k, FilterArgs f, unsigned long long* partial,
+cudaError_t dispatch_warp(int S, const float* xq, int64_t ldq, int nq, const int32_t* probe_ids, int nprobe,
+                          int nsplit, int pg, ListDirectory dir, int k, FilterArgs f, unsigned long long* partial,
                           cudaStream_t st) {
-#define GB_FAST(LPR, J)                                                                                              \
-  if (S == (LPR) * (J))                                                                                            \
-    return c.warp_mode ? launch_warp<METRIC, LPR, J>(xq, ldq, nq, probe_ids, nprobe, nsplit, c, dir, k, f, partial, st) \
-                       : launch_fast<METRIC, LPR, J>(xq, ldq, nq, probe_ids, nprobe, nsplit, c, dir, k, f, partial, st)
-  GB_FAST(8, 1);   // d = 32
-  GB_FAST(8, 2);   // d = 64
-  GB_FAST(8, 3);   // d = 96
-  GB_FAST(8, 4);   // d = 128
-  GB_FAST(8, 5);
-  GB_FAST(8, 6);   // d = 192
-  GB_FAST(8, 7);
-  GB_FAST(8, 8);   // d = 256
-  GB_FAST(16, 5);
-  GB_FAST(16, 6);  // d = 384
-  GB_FAST(16, 7);
-  GB_FAST(16, 8);  // d = 512
-  GB_FAST(32, 5);
-  GB_FAST(32, 6);  // d = 768
-  GB_FAST(32, 7);
-  GB_FAST(32, 8);  // d = 1024
-  GB_FAST(32, 12); // d = 1536
-#undef GB_FAST
+#define GB_WARP(LPR, J) \
+  if (S == (LPR) * (J)) return launch_warp<METRIC, LPR, J>(xq, ldq, nq, probe_ids, nprobe, nsplit, pg, dir, k, f, partial, st)
+  GB_WARP(8, 1);   // d = 32
+  GB_WARP(8, 2);   // d = 64
+  GB_WARP(8, 3);   // d = 96
+  GB_WARP(8, 4);   // d = 128
+  GB_WARP(8, 5);
+  GB_WARP(8, 6);   // d = 192
+  GB_WARP(8, 7);
+  GB_WARP(8, 8);   // d = 256
+  GB_WARP(16, 5);
+  GB_WARP(16, 6);  // d = 384
+  GB_WARP(16, 7);
+  GB_WARP(16, 8);  // d = 512
+  GB_WARP(32, 5);
+  GB_WARP(32, 6);  // d = 768
+  GB_WARP(32, 7);
+  GB_WARP(32, 8);  // d = 1024
+  GB_WARP(32, 12); // d = 1536
+#undef GB_WARP
   return cudaErrorNotSupported;
 }
 
@@ -636,14 +446,14 @@ cudaError_t launch_ivfflat_scan(const float* xq, int64_t ldq, int nq, int d, con
   int nparts = ivfflat_scan_nparts(nprobe, max_list_len);
   int nsplit = nparts / nprobe;
   if (nparts_out) *nparts_out = nparts;
-  if (ldq % 4 == 0 && !getenv("GB_IVF_GENERIC")) {
-    FastCfg c = fast_cfg(nprobe, nsplit, avg_list_len);
-    cudaError_t fe = metric == kMetricL2 ? dispatch_fast<kMetricL2>(d >> 2, xq, ldq, nq, probe_ids, nprobe, nsplit, c,
+  if (ldq % 4 == 0) {
+    const int pg = warp_pg(nprobe, nsplit, avg_list_len);
+    cudaError_t fe = metric == kMetricL2 ? dispatch_warp<kMetricL2>(d >> 2, xq, ldq, nq, probe_ids, nprobe, nsplit, pg,
                                                                     dir, k, f, partial, st)
-                                         : dispatch_fast<kMetricIP>(d >> 2, xq, ldq, nq, probe_ids, nprobe, nsplit, c,
+                                         : dispatch_warp<kMetricIP>(d >> 2, xq, ldq, nq, probe_ids, nprobe, nsplit, pg,
                                                                     dir, k, f, partial, st);
     if (fe != cudaErrorNotSupported) {
-      if (nparts_out) *nparts_out = (nparts + c.pg - 1) / c.pg;  // partial[q][group][k]
+      if (nparts_out) *nparts_out = (nparts + pg - 1) / pg;  // partial[q][group][k]
       return fe;
     }
   }

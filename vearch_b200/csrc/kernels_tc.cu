@@ -11,10 +11,9 @@
 //    list on the device (lm_count / lmk_scan / lmk_assign / lmk_items); a work item multiplies a group
 //    of <= 128 pairs by the 128-row tiles of a row segment of the list, so the list is read once per
 //    128 queries instead of once per query, and tombstones / bitmaps / score window / top-k are
-//    applied as scan_codes does (gamma_index_ivfflat.h:63-91).  Four kernels, one algorithm:
-//      ivf_listmajor_tma_kernel   operands arrive by cp.async.bulk from the pre-tiled mirror (default)
-//      ivf_listmajor_pipe_kernel  warp-specialised, operands staged through registers (no mirror)
-//      ivf_listmajor_topk_kernel  the same without warp specialisation (single-chunk rows)
+//    applied as scan_codes does (gamma_index_ivfflat.h:63-91).  Three kernels, one algorithm:
+//      ivf_listmajor_tma_kernel   operands arrive by cp.async.bulk from the pre-tiled mirror (k <= 32, d > 16)
+//      ivf_listmajor_pipe_kernel  warp-specialised, operands staged through registers (no mirror, d <= 16 or k <= 64)
 //      ivf_listmajor_tc_kernel + seg_select_kernel   dense scores + segment select (k > 64)
 //
 // Precision: every operand is split x = hi + lo, hi = the TF32-representable head (low 13 mantissa
@@ -33,7 +32,6 @@
 // and |y_t|^2.  TMA kernel: the same tiles already exist in global memory (tc_mirror_build_kernel,
 // lm_stage_queries_kernel) and arrive as 16 KiB bulk copies.
 #include <float.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -78,8 +76,7 @@ __device__ __forceinline__ void tc_chunk_mma(float (&acc)[2][64], uint32_t a_hi,
 // loads issued two chunks ahead) and write them into the other stage, so neither the global-load
 // latency nor the MMA latency sits on the critical path.
 struct TcShared {
-  alignas(16) float cn[TC_N];  // |y|^2 of the tile's rows (read as float4 by the fused epilogues)
-  uint32_t vid[TC_N];          // ids of the tile's rows (fused top-k epilogue)
+  alignas(16) float cn[TC_N];  // |y|^2 of the tile's rows (aligned: the epilogues' reads vectorise)
 };
 
 __device__ __forceinline__ void tc_tile_run(unsigned char* smem, TcShared* sh, const float* __restrict__ arow,
@@ -323,69 +320,6 @@ __device__ __forceinline__ void lmk_scan_block(uint32_t (&v)[32], float xn, cons
   }
 }
 
-template <int METRIC>
-__global__ void __launch_bounds__(TC_NT)
-    ivf_listmajor_topk_kernel(const float* __restrict__ xq, int64_t ldq, int d, const LmTile* __restrict__ items,
-                              const int64_t* __restrict__ totals, const int64_t* __restrict__ pair_j, int nprobe,
-                              ListDirectory dir, int k, int nseg_max, FilterArgs f, unsigned long long* tau_g,
-                              unsigned long long* __restrict__ out) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ TcShared sh;
-  if ((int64_t)blockIdx.x >= totals[1]) return;
-  const int tid = threadIdx.x;
-  const LmTile t = items[blockIdx.x];
-  unsigned long long* hk = reinterpret_cast<unsigned long long*>(smem + TC_SMEM) + tid;
-  float* slabs = reinterpret_cast<float*>(smem);  // the operand stages are idle during the epilogue
-  const bool valid = tid < t.npairs;
-  int64_t j = 0;
-  int q = 0;
-  const float* arow = nullptr;
-  LmkState st{0ull, 0};
-  if (valid) {
-    j = pair_j[t.pair0 + tid];
-    q = (int)(j / nprobe);
-    arow = xq + (int64_t)q * ldq;
-    st.tau = __ldcg(tau_g + q);
-  }
-  const float* lvecs = dir.vecs[t.list];
-  const int64_t* __restrict__ lids = dir.ids[t.list];
-  const int row_end = t.row0 + t.nrows;
-  float bound = key_bound<METRIC>(st.tau);
-  float acc[2][64];
-  for (int r0 = t.row0; r0 < row_end; r0 += TC_N) {
-    const float* brow = nullptr;
-    uint32_t myvid = kLmkNoVid;  // validity of row r0 + tid, resolved while the tile is being multiplied
-    if (r0 + tid < row_end) {
-      brow = lvecs + (int64_t)(r0 + tid) * d;
-      const int64_t raw = lids[r0 + tid];
-      if (raw >= 0 && ctx_is_valid(f.del_bits, f.filter_bits, (uint32_t)raw)) myvid = (uint32_t)raw;  // tombstone: ivfflat.h:72
-    }
-    float xn;
-    tc_tile_run(smem, &sh, arow, brow, d, acc, &xn);
-    sh.vid[tid] = myvid;  // visible after the first exchange's barrier
-#pragma unroll
-    for (int c0 = 0; c0 < TC_N; c0 += 32) {
-      uint32_t v[32];
-      acc_cols(acc, c0, slabs, v);
-      lmk_scan_block<METRIC>(v, xn, &sh.cn[c0], &sh.vid[c0], hk, k, f.min_score, f.max_score, st, bound);
-    }
-    if (valid) {  // exchange bounds with the other CTAs working on this query
-      const unsigned long long tg = __ldcg(tau_g + q);
-      if (tg < st.tau) {
-        st.tau = tg;
-        bound = key_bound<METRIC>(st.tau);
-      } else if (st.tau < tg) {
-        atomicMin(tau_g + q, st.tau);
-      }
-    }
-    __syncthreads();  // the slabs, cn and vid are overwritten by the next tile
-  }
-  if (valid) {
-    unsigned long long* o = out + ((int64_t)j * nseg_max + t.seg) * k;
-    for (int i = 0; i < k; i++) o[i] = i < st.n ? hk[i * TC_NT] : kKeySentinel;
-  }
-}
-
 // MMAs of one 128 x 128 tile from a ring of operand stages (warpgroup 0).  Chunk n of the CTA's
 // sequence sits in stage n % NST once full[s] completes its phase; every thread arrives on empty[s]
 // once its warp's MMAs of that chunk are done (one commit group stays in flight).
@@ -411,9 +345,37 @@ __device__ __forceinline__ void ring_tile_mma(float (&acc)[2][64], uint32_t r_ba
   mbar_arrive(&empty[prev]);
 }
 
-// ---- K3 list-major, warp-specialised pipeline -------------------------------------------------
-// Same work item and the same results as ivf_listmajor_topk_kernel, but staging runs concurrently
-// with the MMAs and the epilogue, synchronised by mbarriers only:
+// Thread 0: the mbarriers of a ring of nst stages.  A full phase completes after full_count arrivals (and, for a
+// TMA-fed ring, the transaction bytes of the stage's copies); an empty phase once every MMA thread has arrived.
+__device__ __forceinline__ void ring_init(uint64_t* full, uint64_t* empty, int nst, uint32_t full_count) {
+  for (int s = 0; s < nst; s++) {
+    mbar_init(&full[s], full_count);
+    mbar_init(&empty[s], TC_M);
+  }
+  mbar_fence_init();
+}
+
+// After a tile: exchange bounds with the other CTAs working on the same query (tau_q = its slot of tau_g) --
+// adopt a tighter published bound, or publish this thread's own.
+template <int METRIC>
+__device__ __forceinline__ void lmk_exchange_bound(unsigned long long* tau_q, LmkState& st, float& bound) {
+  const unsigned long long tg = __ldcg(tau_q);
+  if (tg < st.tau) {
+    st.tau = tg;
+    bound = key_bound<METRIC>(st.tau);
+  } else if (st.tau < tg) {
+    atomicMin(tau_q, st.tau);
+  }
+}
+
+// the thread's key set (n keys, slot-major in shared memory) -> o[0, k), sentinel padded
+__device__ __forceinline__ void lmk_write_keys(unsigned long long* o, const unsigned long long* hk, int k, int n) {
+  for (int i = 0; i < k; i++) o[i] = i < n ? hk[i * TC_NT] : kKeySentinel;
+}
+
+// ---- K3 list-major, register-staged pipeline ---------------------------------------------------
+// The fused top-k kernel that needs no mirror.  Staging runs concurrently with the MMAs and the
+// epilogue, synchronised by mbarriers only:
 //   warps 4-7  producers: thread p stages row p of the query group and of the list tile, one K = 16
 //              chunk at a time, into a ring of LW_STAGES operand stages (hi/lo TF32 split, canonical
 //              K-major layout), two chunks of global loads in flight per thread;
@@ -445,15 +407,13 @@ __global__ void __launch_bounds__(LW_NT, 1)
   const LmTile t = items[blockIdx.x];
   const int row_end = t.row0 + t.nrows;
   const int ntiles = (t.nrows + TC_N - 1) / TC_N;
-  const int nk = (d + TC_BK - 1) / TC_BK;
+  // at least two K chunks per tile, which the ring's phase arithmetic assumes (d <= 16: the loads zero-fill
+  // columns >= d, so the second chunk adds exact zeros)
+  const int nk = max(2, (d + TC_BK - 1) / TC_BK);
 
   if (tid == 0) {
-    for (int s = 0; s < LW_STAGES; s++) {
-      mbar_init(&sh.full[s], TC_M);   // every producer thread arrives
-      mbar_init(&sh.empty[s], TC_M);  // every MMA thread arrives
-    }
     for (int b = 0; b < 2; b++) mbar_init(&sh.acc_empty[b], TC_M);  // every epilogue thread arrives
-    mbar_fence_init();
+    ring_init(sh.full, sh.empty, LW_STAGES, TC_M);                   // every producer thread arrives
   }
   __syncthreads();
   const uint32_t LBO = TC_M * 16, SBO = 128;
@@ -486,20 +446,9 @@ __global__ void __launch_bounds__(LW_NT, 1)
         lmk_scan_block<METRIC>(v, xn, &sh.cn[b][c0], &sh.vid[b][c0], hk, k, f.min_score, f.max_score, st, bound);
       }
       mbar_arrive(&sh.acc_empty[b]);  // cn[b], vid[b] may be overwritten
-      if (valid) {                    // exchange bounds with the other CTAs working on this query
-        const unsigned long long tg = __ldcg(tau_g + q);
-        if (tg < st.tau) {
-          st.tau = tg;
-          bound = key_bound<METRIC>(st.tau);
-        } else if (st.tau < tg) {
-          atomicMin(tau_g + q, st.tau);
-        }
-      }
+      if (valid) lmk_exchange_bound<METRIC>(tau_g + q, st, bound);
     }
-    if (valid) {
-      unsigned long long* o = out + ((int64_t)j * nseg_max + t.seg) * k;
-      for (int i = 0; i < k; i++) o[i] = i < st.n ? hk[i * TC_NT] : kKeySentinel;
-    }
+    if (valid) lmk_write_keys(out + ((int64_t)j * nseg_max + t.seg) * k, hk, k, st.n);
   } else {
     // ======================= producers =======================
     const int p = tid - TC_M;
@@ -604,6 +553,27 @@ struct LtShared {
   uint64_t full[LT_STAGES], empty[LT_STAGES];
 };
 
+// TMA producer of an LT_STAGES ring (the whole warp loops, one elected lane issues): for each of ntiles tiles and
+// each of its nk K chunks, chunk kc of the A operand (a_chunks, the same for every tile) and chunk (tile, kc) of the
+// B operand (b_chunks), 16 KiB each, into the next stage
+__device__ __forceinline__ void ring_tma_produce(unsigned char* ring, uint64_t* full, uint64_t* empty, const char* a_chunks,
+                                                 const char* b_chunks, int ntiles, int nk) {
+  int n = 0;
+  for (int i = 0; i < ntiles; i++) {
+    for (int kc = 0; kc < nk; kc++, n++) {
+      const int s = n % LT_STAGES;
+      mbar_wait(&empty[s], (uint32_t)(((n / LT_STAGES) & 1) ^ 1));
+      if (elect_one()) {
+        unsigned char* stage = ring + (size_t)s * TC_STAGE_BYTES;
+        mbar_arrive_expect_tx(&full[s], TC_STAGE_BYTES);
+        bulk_g2s(stage, a_chunks + (int64_t)kc * LT_HALF, LT_HALF, &full[s]);
+        bulk_g2s(stage + LT_HALF, b_chunks + ((int64_t)i * nk + kc) * LT_HALF, LT_HALF, &full[s]);
+      }
+      __syncwarp();
+    }
+  }
+}
+
 
 
 template <int METRIC>
@@ -624,13 +594,7 @@ __global__ void __launch_bounds__(LT_NT, 1)
   const int nk = mv.k16 / TC_BK;
   unsigned char* ring = smem;  // [ring: NST * STAGE] [slabs] [key sets: k * 1 KiB]
 
-  if (tid == 0) {
-    for (int s = 0; s < NST; s++) {
-      mbar_init(&sh.full[s], 1);      // the producer's arrive.expect_tx; the copies complete the phase
-      mbar_init(&sh.empty[s], TC_M);  // every MMA thread arrives
-    }
-    mbar_fence_init();
-  }
+  if (tid == 0) ring_init(sh.full, sh.empty, NST, 1);  // the producer's arrive.expect_tx; the copies complete the phase
   __syncthreads();
   const int64_t tile_floats = (int64_t)TC_N * mv.k16 * 2;
   const int64_t ltile0 = mv.tile0[t.list] + t.row0 / TC_N;  // first mirror tile of this item
@@ -674,38 +638,13 @@ __global__ void __launch_bounds__(LT_NT, 1)
         acc_cols(acc, c0, slabs, v);
         lmk_scan_block<METRIC>(v, xn, &sh.cn[b][c0], &sh.vid[b][c0], hk, k, f.min_score, f.max_score, st, bound);
       }
-      if (valid) {
-        const unsigned long long tg = __ldcg(tau_g + q);
-        if (tg < st.tau) {
-          st.tau = tg;
-          bound = key_bound<METRIC>(st.tau);
-        } else if (st.tau < tg) {
-          atomicMin(tau_g + q, st.tau);
-        }
-      }
+      if (valid) lmk_exchange_bound<METRIC>(tau_g + q, st, bound);
     }
-    if (valid) {
-      unsigned long long* o = out + ((int64_t)j * nseg_max + t.seg) * k;
-      for (int i = 0; i < k; i++) o[i] = i < st.n ? hk[i * TC_NT] : kKeySentinel;
-    }
+    if (valid) lmk_write_keys(out + ((int64_t)j * nseg_max + t.seg) * k, hk, k, st.n);
   } else {
-    // ======================= TMA producer (whole warp loops, one elected lane issues) =======================
-    const char* asrc = reinterpret_cast<const char*>(a_scratch) + (int64_t)t.grp * nk * LT_HALF;
-    const char* bsrc = reinterpret_cast<const char*>(mv.base + ltile0 * tile_floats);
-    int n = 0;
-    for (int i = 0; i < ntiles; i++) {
-      for (int kc = 0; kc < nk; kc++, n++) {
-        const int s = n % NST;
-        mbar_wait(&sh.empty[s], (uint32_t)(((n / NST) & 1) ^ 1));
-        if (elect_one()) {
-          unsigned char* stage = ring + (size_t)s * STAGE;
-          mbar_arrive_expect_tx(&sh.full[s], STAGE);
-          bulk_g2s(stage, asrc + (int64_t)kc * LT_HALF, LT_HALF, &sh.full[s]);
-          bulk_g2s(stage + LT_HALF, bsrc + ((int64_t)i * nk + kc) * LT_HALF, LT_HALF, &sh.full[s]);
-        }
-        __syncwarp();
-      }
-    }
+    // ======================= TMA producer =======================
+    ring_tma_produce(ring, sh.full, sh.empty, reinterpret_cast<const char*>(a_scratch) + (int64_t)t.grp * nk * LT_HALF,
+                     reinterpret_cast<const char*>(mv.base + ltile0 * tile_floats), ntiles, nk);
   }
 }
 
@@ -847,13 +786,7 @@ __global__ void __launch_bounds__(LT_NT, 1)
   const int nk = k16 / TC_BK;
   unsigned char* ring = smem;
 
-  if (tid == 0) {
-    for (int s = 0; s < NST; s++) {
-      mbar_init(&sh.full[s], 1);      // the producer's arrive.expect_tx; the copies complete the phase
-      mbar_init(&sh.empty[s], TC_M);  // every MMA thread arrives
-    }
-    mbar_fence_init();
-  }
+  if (tid == 0) ring_init(sh.full, sh.empty, NST, 1);  // the producer's arrive.expect_tx; the copies complete the phase
   __syncthreads();
 
   if (warp < 4) {
@@ -897,38 +830,13 @@ __global__ void __launch_bounds__(LT_NT, 1)
         }
         bound = key_bound<METRIC>(st.tau);
       }
-      if (valid) {  // exchange bounds with the other segments of this query
-        const unsigned long long tg = __ldcg(tau_g + q);
-        if (tg < st.tau) {
-          st.tau = tg;
-          bound = key_bound<METRIC>(st.tau);
-        } else if (st.tau < tg) {
-          atomicMin(tau_g + q, st.tau);
-        }
-      }
+      if (valid) lmk_exchange_bound<METRIC>(tau_g + q, st, bound);  // with the other segments of this query
     }
-    if (valid) {
-      unsigned long long* o = out + ((int64_t)q * nseg + sg) * k;
-      for (int i = 0; i < k; i++) o[i] = i < st.n ? hk[i * TC_NT] : kKeySentinel;
-    }
+    if (valid) lmk_write_keys(out + ((int64_t)q * nseg + sg) * k, hk, k, st.n);
   } else {
-    // ======================= TMA producer (whole warp loops, one elected lane issues) =======================
-    const char* asrc = reinterpret_cast<const char*>(a_tiles) + (int64_t)qt * nk * LT_HALF;
-    const char* bsrc = reinterpret_cast<const char*>(c_tiles) + (int64_t)ct0 * nk * LT_HALF;
-    int n = 0;
-    for (int i = 0; i < ntiles; i++) {
-      for (int kc = 0; kc < nk; kc++, n++) {
-        const int s = n % NST;
-        mbar_wait(&sh.empty[s], (uint32_t)(((n / NST) & 1) ^ 1));
-        if (elect_one()) {
-          unsigned char* stage = ring + (size_t)s * STAGE;
-          mbar_arrive_expect_tx(&sh.full[s], STAGE);
-          bulk_g2s(stage, asrc + (int64_t)kc * LT_HALF, LT_HALF, &sh.full[s]);
-          bulk_g2s(stage + LT_HALF, bsrc + ((int64_t)i * nk + kc) * LT_HALF, LT_HALF, &sh.full[s]);
-        }
-        __syncwarp();
-      }
-    }
+    // ======================= TMA producer =======================
+    ring_tma_produce(ring, sh.full, sh.empty, reinterpret_cast<const char*>(a_tiles) + (int64_t)qt * nk * LT_HALF,
+                     reinterpret_cast<const char*>(c_tiles) + (int64_t)ct0 * nk * LT_HALF, ntiles, nk);
   }
 }
 
@@ -1358,44 +1266,23 @@ cudaError_t launch_ivf_listmajor_tma(const float* a_scratch, const float* a_norm
                                  out, st);
 }
 
-cudaError_t launch_ivf_listmajor_topk(const float* xq, int64_t ldq, int d, const LmTile* items, int max_items,
+cudaError_t launch_ivf_listmajor_pipe(const float* xq, int64_t ldq, int d, const LmTile* items, int max_items,
                                       const int64_t* totals, const int64_t* pair_j, int nprobe, ListDirectory dir, int k,
                                       int nseg_max, int metric, FilterArgs f, unsigned long long* tau_g,
                                       unsigned long long* out, cudaStream_t st) {
   if ((d & 3) || (ldq & 3) || k <= 0 || k > kLmkMaxK) return cudaErrorInvalidValue;
   if (max_items <= 0) return cudaSuccess;
-  static const int pipe = [] {
-    const char* e = getenv("GB_LM_PIPE");
-    return e ? atoi(e) : 1;
-  }();
-  if (pipe && d > TC_BK) {  // the ring's phase arithmetic assumes >= 2 chunks per tile
-    const size_t smem = (size_t)LW_RING + kSlabBytes + (size_t)k * TC_NT * 8;
-    cudaError_t e;
-    if (metric == kMetricL2) {
-      e = cudaFuncSetAttribute(ivf_listmajor_pipe_kernel<kMetricL2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return e;
-      ivf_listmajor_pipe_kernel<kMetricL2><<<max_items, LW_NT, smem, st>>>(xq, ldq, d, items, totals, pair_j, nprobe, dir,
-                                                                          k, nseg_max, f, tau_g, out);
-    } else {
-      e = cudaFuncSetAttribute(ivf_listmajor_pipe_kernel<kMetricIP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return e;
-      ivf_listmajor_pipe_kernel<kMetricIP><<<max_items, LW_NT, smem, st>>>(xq, ldq, d, items, totals, pair_j, nprobe, dir,
-                                                                          k, nseg_max, f, tau_g, out);
-    }
-    note_launch();
-    return cudaGetLastError();
-  }
-  const size_t smem = (size_t)TC_SMEM + (size_t)k * TC_NT * 8;
+  const size_t smem = (size_t)LW_RING + kSlabBytes + (size_t)k * TC_NT * 8;
   cudaError_t e;
   if (metric == kMetricL2) {
-    e = cudaFuncSetAttribute(ivf_listmajor_topk_kernel<kMetricL2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    e = cudaFuncSetAttribute(ivf_listmajor_pipe_kernel<kMetricL2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    ivf_listmajor_topk_kernel<kMetricL2><<<max_items, TC_NT, smem, st>>>(xq, ldq, d, items, totals, pair_j, nprobe, dir, k,
+    ivf_listmajor_pipe_kernel<kMetricL2><<<max_items, LW_NT, smem, st>>>(xq, ldq, d, items, totals, pair_j, nprobe, dir, k,
                                                                         nseg_max, f, tau_g, out);
   } else {
-    e = cudaFuncSetAttribute(ivf_listmajor_topk_kernel<kMetricIP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    e = cudaFuncSetAttribute(ivf_listmajor_pipe_kernel<kMetricIP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    ivf_listmajor_topk_kernel<kMetricIP><<<max_items, TC_NT, smem, st>>>(xq, ldq, d, items, totals, pair_j, nprobe, dir, k,
+    ivf_listmajor_pipe_kernel<kMetricIP><<<max_items, LW_NT, smem, st>>>(xq, ldq, d, items, totals, pair_j, nprobe, dir, k,
                                                                         nseg_max, f, tau_g, out);
   }
   note_launch();
