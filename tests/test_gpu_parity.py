@@ -808,15 +808,13 @@ def test_ivfpq_opq_rotation_train_apply_search_and_file(tmp_path):
 # ----------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("path", ["query_major", "list_major"])
 @pytest.mark.parametrize("data", ["int", "float"])
-def test_baseline_shape_ivfflat_d128_nlist1024_nprobe32(path, data, monkeypatch):
+def test_baseline_shape_ivfflat_d128_nlist1024_nprobe32(path, data):
     d, n, nlist, nprobe, k = 128, 200_000, 1024, 32, 10
     nq = 1100 if path == "list_major" else 200  # >= 32 (query, probe) pairs per list selects the list-major scan
     if data == "int":
         db, xq = synth.sift_like(n, d, seed=301), synth.sift_like(nq, d, seed=302)
     else:
         db, xq = synth.sift_like(n, d, seed=303, rounded=False), synth.sift_like(nq, d, seed=304, rounded=False)
-    if path == "query_major":
-        monkeypatch.setenv("GB_LISTMAJOR", "0")
     idx = gi().GammaIndex("IVFFLAT", d, {"ncentroids": nlist, "nprobe": nprobe, "metric_type": "L2",
                                          "training_threshold": nlist * 39})
     idx.add_vectors(db)

@@ -21,17 +21,6 @@ const char* last_error() { return g_last_error.c_str(); }
 
 static inline int64_t round_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
-// tensor-core (wgmma 3xTF32) path for the dense query x centroid contraction: coarse search and
-// the k-means assign step.  GB_TC=0 selects the exact CUDA-core kernel everywhere.  List assignment
-// at add time always uses the exact kernel so list membership is deterministic against the oracle.
-static bool tc_enabled() {
-  static int v = [] {
-    const char* e = getenv("GB_TC");
-    return e ? atoi(e) : 1;
-  }();
-  return v != 0;
-}
-
 // SM count of a device, queried once (grids of the persistent kernels, work-splitting heuristics)
 static int sm_count(int device) {
   static std::mutex mu;
@@ -979,7 +968,7 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
   std::vector<int32_t> h_off(k + 1), h_perm(n), cursor(k);
   std::vector<float> hassign(k), h_cent;
   const int metric = kp.spherical ? kMetricIP : kMetricL2;  // gamma's quantizer is IndexFlat(d, metric)
-  const bool use_tc = tc_enabled() && k >= 64;
+  const bool use_tc = k >= 64;  // tensor-core (wgmma 3xTF32) distance tiles
   for (int it = 0; it < kp.niter; it++) {
     GB_CUDA(launch_fill_u64(best, n, kKeySentinel, st));
     if (use_tc) {
@@ -1144,6 +1133,7 @@ int IVFFlatIndex::assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* ou
   cudaStream_t st = s.stream();
   GB_ALLOC(best, unsigned long long, n, s);
   GB_CUDA(launch_fill_u64(best, n, kKeySentinel, st));
+  // always the exact CUDA-core kernel, never the tensor-core tiles: list membership stays deterministic against the oracle
   GB_CUDA(launch_dist_argmin(x, ldx, (int)n, d_centroids_, dpad_, nlist_, dpad_, mp_.metric, best, 0, st));
   GB_CUDA(launch_split_keys(best, n, mp_.metric, nullptr, out, st));
   return 0;
@@ -1303,7 +1293,7 @@ int IVFFlatIndex::coarse_dev(int nq, const float* xq, int nprobe, int metric, in
                              Scratch& s) {
   cudaStream_t st = s.stream();
   GB_ALLOC(keys, unsigned long long, (size_t)nq * nprobe, s);
-  const bool tc = tc_enabled() && nlist_ >= 64 && nq >= 32;
+  const bool tc = nlist_ >= 64 && nq >= 32;
   const int k16 = (int)round_up(dpad_, 16);
   if (tc && coarse_fused_enabled() && nprobe <= kCoarseMaxK && k16 > 16) {
     // fused: per (query tile, centroid segment) the best nprobe keys, merged per query; no score matrix
@@ -1341,11 +1331,6 @@ int IVFFlatIndex::coarse_dev(int nq, const float* xq, int nprobe, int metric, in
 // Host side: group the (query, probe) pairs by list (stable counting sort), give every pair a
 // score segment of len(list) floats, cut (list, 128 pairs, 128 rows) tiles; device side: grouped
 // GEMM on wgmma + segment select.
-// GB_LISTMAJOR=0: never list-major.  Read per call: tests flip it between searches of one process.
-static bool listmajor_enabled() {
-  const char* e = getenv("GB_LISTMAJOR");
-  return e ? atoi(e) != 0 : true;
-}
 
 // called from index_batch with mu_ held exclusively: no search is inside ensure_mirror.  Kernels of an
 // earlier search_device may still be running, but they only look at rows below the lengths they were
@@ -1430,7 +1415,6 @@ int IVFFlatIndex::ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStr
 
 int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, const float* xq, int k,
                                      const int32_t* probe_ids, int nprobe, unsigned long long* out_keys, Scratch& s) {
-  if (!tc_enabled() || !listmajor_enabled()) return 1;
   const int64_t npairs = (int64_t)nq * nprobe;
   if (npairs < (int64_t)nlist_ * 32) return 1;  // < 32 queries per list on average
   cudaStream_t st = s.stream();
@@ -2023,29 +2007,16 @@ int IVFPQIndex::ensure_pq_norms(cudaStream_t st) {
   return 0;
 }
 
-// GB_PQTC=0: never use the tensor-core filter (exact LUT kernel for every probe); GB_PQTC=2: use it
-// whenever the shape allows, whatever the batch size (tests)
-static int pqtc_mode() {  // read per call: tests flip it between searches of one process
-  const char* e = getenv("GB_PQTC");
-  return e ? atoi(e) : 1;
-}
-// test hook: scales the filter's error margin (1 = the rigorous bound, 0 = no margin at all)
-static float pqtc_eps_scale() {
-  const char* e = getenv("GB_PQTC_EPS");
-  return e ? (float)atof(e) : 1.0f;
-}
-
 // List-major IVF-PQ scan (kernels_pqtc.cu): exact scan of the first pa probes -> per-query bound ->
 // tensor-core filter over the remaining probes -> exact re-score of the candidates.  Returns 1 when
 // the batch / shape does not qualify (caller runs the exact kernel over all probes).
 int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const float* xq, int kk, const float* ip,
                                   const int32_t* probe_ids, const float* coarse_dis, int nprobe,
                                   unsigned long long* adc_out, bool need_sorted, Scratch& s) {
-  const int mode = pqtc_mode();
-  if (!mode || !tc_enabled() || !d_cb16_ || !pqtc_supported(M_, dsub_) || dpad_ != d_) return 1;
+  if (!d_cb16_ || !pqtc_supported(M_, dsub_) || dpad_ != d_) return 1;
   if (kk > 2048 || nprobe < 2 || nprobe > 65535 || nq > 65535) return 1;  // (query, probe) travel as 16-bit fields of a candidate record
   const int64_t npairs = (int64_t)nq * nprobe;
-  if (mode != 2 && npairs < (int64_t)nlist_ * 32) return 1;  // < 32 queries per list on average
+  if (npairs < (int64_t)nlist_ * 32) return 1;  // < 32 queries per list on average
   if (metric == kMetricL2) {
     const int nr = ensure_pq_norms(s.stream());
     if (nr) return nr;
@@ -2053,20 +2024,14 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   cudaStream_t st = s.stream();
   ListDirectory dir = lists_->directory();
   // phase A, per query: its first probes in full -- the fewest whose lists hold >= 4 k' entries together (so that its
-  // k'-th exact score is a tight bound B_q), at most pa_max; phase B filters the other probes.  GB_PQTC_PA=n: the
-  // first n probes of every query; GB_PQTC_TARGET=t: t k' entries instead of 4 k'.
-  int pa_max = std::min(nprobe - 1, 8);
-  long long pa_target = 4 * (long long)kk;
-  if (const char* e = getenv("GB_PQTC_PA")) {
-    pa_max = std::max(1, std::min(nprobe - 1, atoi(e)));
-    pa_target = LLONG_MAX;
-  }
-  if (const char* e = getenv("GB_PQTC_TARGET")) pa_target = std::max(1LL, atoll(e)) * kk;
+  // k'-th exact score is a tight bound B_q), at most pa_max; phase B filters the other probes.
+  const int pa_max = std::min(nprobe - 1, 8);
+  const long long pa_target = 4 * (long long)kk;
   const int cap = std::max(2048, std::min(8192, next_pow2(8 * kk)));
   const int nsm = sm_count(device_);
   snprintf(last_scan_info_, sizeof(last_scan_info_),
            "{\"phase_a_max_probes\": %d, \"phase_a_target_entries\": %lld, \"candidate_cap\": %d, \"kprime\": %d}", pa_max,
-           pa_target == LLONG_MAX ? -1LL : pa_target, cap, kk);
+           pa_target, cap, kk);
   GB_ALLOC(d_probes_a, int32_t, npairs, s);
   GB_ALLOC(d_probes_b, int32_t, npairs, s);
   GB_ALLOC(d_row_limit, int, npairs, s);
@@ -2121,7 +2086,7 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   GB_CUDA(launch_lmk_group(d_probes_b, npairs, dir, nseg, pq_group, d_cnt, d_start, d_cursor, d_item_start, d_grp_start, d_totals,
                            d_pair_j, d_items, st));
   GB_CUDA(launch_pq_stage_pairs(xq, dpad_, d_, d_centroids_, dpad_, d_items, (int)max_items, d_totals, d_pair_j, nprobe,
-                                coarse_dis, keysA, kk, kk, d_cbnrm_ + (size_t)M_ * 256, f, metric, pqtc_eps_scale(), a_scratch,
+                                coarse_dis, keysA, kk, kk, d_cbnrm_ + (size_t)M_ * 256, f, metric, a_scratch,
                                 meta, d_cand_cnt, cap, d_row_limit, st));
   stage_end(st);
   scan_timer_begin(st);  // the dominant kernel: the roofline in bench.py is this launch alone
@@ -2142,56 +2107,6 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
                             d_cand_cnt, cap));
   GB_CUDA(launch_pq_fallback_merge(d_cand_cnt, cap, nq, partF, ngF, kk, adc_out, st));
   stage_end(st);
-  if (const char* dump = getenv("GB_PQTC_DUMP")) {  // debugging aid: candidate lists + phase A keys to a file
-    std::vector<int> h(nq);
-    std::vector<unsigned long long> hc((size_t)nq * cap), hk((size_t)nq * kk);
-    GB_CUDA(cudaMemcpyAsync(h.data(), d_cand_cnt, sizeof(int) * nq, cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaMemcpyAsync(hc.data(), cand, hc.size() * 8, cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaMemcpyAsync(hk.data(), keysA, hk.size() * 8, cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
-    int64_t ht[3];
-    GB_CUDA(cudaMemcpy(ht, d_totals, sizeof(ht), cudaMemcpyDeviceToHost));
-    std::vector<int64_t> hpj((size_t)npairs);
-    std::vector<LmTile> hit((size_t)ht[1]);
-    GB_CUDA(cudaMemcpy(hpj.data(), d_pair_j, hpj.size() * 8, cudaMemcpyDeviceToHost));
-    GB_CUDA(cudaMemcpy(hit.data(), d_items, hit.size() * sizeof(LmTile), cudaMemcpyDeviceToHost));
-    if (FILE* fp = fopen(dump, "wb")) {
-      const int hdr[8] = {nq, cap, kk, pa_max, (int)ht[1], (int)npairs, (int)sizeof(LmTile), (int)ht[2]};
-      fwrite(hdr, 4, 8, fp);
-      fwrite(h.data(), 4, h.size(), fp);
-      fwrite(hc.data(), 8, hc.size(), fp);
-      fwrite(hk.data(), 8, hk.size(), fp);
-      fwrite(hpj.data(), 8, hpj.size(), fp);
-      fwrite(hit.data(), sizeof(LmTile), hit.size(), fp);
-      fclose(fp);
-    }
-  }
-  if (getenv("GB_PQTC_STATS")) {  // diagnostics: candidates per query, overflowed queries
-    std::vector<int> h(nq);
-    GB_CUDA(cudaMemcpyAsync(h.data(), d_cand_cnt, sizeof(int) * nq, cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
-    long long tot = 0, over = 0, mx = 0;
-    for (int v : h) {
-      if (v > cap) over++;
-      else tot += v, mx = std::max<long long>(mx, v);
-    }
-    unsigned long long dc[4];
-    pqtc_debug_counters(dc, true);
-    int64_t ht[3];
-    GB_CUDA(cudaMemcpy(ht, d_totals, sizeof(ht), cudaMemcpyDeviceToHost));
-    std::vector<LmTile> hit((size_t)ht[1]);
-    GB_CUDA(cudaMemcpy(hit.data(), d_items, hit.size() * sizeof(LmTile), cudaMemcpyDeviceToHost));
-    long long tiles = 0, pair_rows = 0, rows = 0;
-    for (const LmTile& t : hit) {
-      tiles += (t.nrows + 127) / 128;
-      pair_rows += (long long)t.npairs * t.nrows;
-      rows += t.nrows;
-    }
-    fprintf(stderr, "[pqtc] nq=%d k'=%d pa_max=%d cap=%d: candidates mean %.1f max %lld, overflowed queries %lld, stale code words %llu, rare-path warp tiles (32x128) %llu; "
-            "items %lld groups %lld tiles(%dx128) %lld rows decoded %lld pair-rows %lld (tile fill %.3f)\n",
-            nq, kk, pa_max, cap, nq > over ? (double)tot / (nq - over) : 0.0, mx, over, dc[0], dc[1], (long long)ht[1], (long long)ht[0],
-            pq_group, tiles, rows, pair_rows, tiles ? (double)pair_rows / ((double)tiles * pq_group * 128) : 0.0);
-  }
   return 0;
 }
 

@@ -171,7 +171,6 @@ cudaError_t launch_ivfpq_scan(const float* ip_table, int nq, const int32_t* prob
 
 // ---- K5 list-major: tensor-core filter + exact re-score (kernels_pqtc.cu) ---------------------------
 bool pqtc_supported(int M, int dsub);
-void pqtc_debug_counters(unsigned long long out[4], bool reset);  // GB_PQTC_DBG diagnostics
 size_t pqtc_pair_meta_bytes();
 // cb[m][c][.] = fp16(-2 sb pq) (L2) / fp16(-sb pq) (IP), sb = rmax2[1] a power of two; nrm[m][c] = |pq[m][c]|^2; rmax2[0] = sum_m max_c nrm
 cudaError_t launch_pqtc_tables(const float* pq, int M, int dsub, int metric, uint16_t* cb, float* nrm, float* rmax2,
@@ -186,8 +185,8 @@ cudaError_t launch_pqtc_plan_phase_a(const int32_t* probe_ids, int64_t npairs, i
 cudaError_t launch_pq_stage_pairs(const float* xq, int64_t ldq, int d, const float* coarse, int64_t ldc, const LmTile* items,
                                   int max_items, const int64_t* totals, const int64_t* pair_j, int nprobe,
                                   const float* coarse_dis, const unsigned long long* bound_keys, int64_t bound_stride,
-                                  int kprime, const float* rmax2, FilterArgs f, int metric, float eps_scale,
-                                  unsigned char* a_scratch, void* meta, int* cand_cnt, int cap, const int* row_limit, cudaStream_t st);
+                                  int kprime, const float* rmax2, FilterArgs f, int metric, unsigned char* a_scratch,
+                                  void* meta, int* cand_cnt, int cap, const int* row_limit, cudaStream_t st);
 // persistent kernel, one CTA per SM: candidates (probe << 32 | position) appended to cand[q][cap]
 cudaError_t launch_pqtc_scan(const unsigned char* a_scratch, const void* meta, const uint16_t* cb, const float* pqnorm, const int64_t* pqnorm_off,
                              const LmTile* items, int max_items, const int64_t* totals, ListDirectory dir, int M, int dsub,

@@ -41,8 +41,6 @@
 // Algorithmic bytes: (M + 8) per scanned entry per 256-pair group instead of per pair.
 #include <float.h>
 #include <math.h>
-#include <stdio.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -63,10 +61,6 @@ constexpr int PT_RQ = 512;         // records of the CTA's candidate queue (shar
 constexpr unsigned long long kRecEmpty = ~0ull;
 constexpr int PT_CS = 4;           // code stages
 constexpr int PT_KSUB = 256;
-
-// debugging counters: [0] stale code words seen by decode (GB_PQTC_DBG & 4), [1] warp tiles (32 pairs x 128 entries) of
-// the epilogue with at least one candidate (the rare path)
-__device__ unsigned long long g_pqtc_dbg[4];
 
 struct PtShared {
   uint64_t code_full[PT_CS], code_empty[PT_CS];
@@ -180,7 +174,7 @@ __global__ void __launch_bounds__(PT_G)
                           const LmTile* __restrict__ items, const int64_t* __restrict__ totals,
                           const int64_t* __restrict__ pair_j, int nprobe, const float* __restrict__ coarse_dis,
                           const unsigned long long* __restrict__ bound_keys, int64_t bound_stride, int kprime,
-                          const float* __restrict__ rmax2, float min_score, float max_score, float eps_scale,
+                          const float* __restrict__ rmax2, float min_score, float max_score,
                           unsigned char* __restrict__ a_scratch, PairMeta* __restrict__ meta, int* __restrict__ cand_cnt,
                           int cap, const int* __restrict__ row_limit) {
   if ((int64_t)blockIdx.x >= totals[1]) return;
@@ -255,13 +249,13 @@ __global__ void __launch_bounds__(PT_G)
         //   (<= 2^-15 |a| |r| for d <= 4096 even if every add truncated)
         //   + fp32 noise of the reference evaluation, bounded by 2^-17 of the magnitudes that enter it
         const float Z = fabsf(dis0) + R2 + 2.f * (sqrtf(nx2) + sqrtf(nc2)) * R;
-        const float eps = eps_scale * (1.05f * 0.0009765625f * sqrtf(na2) * R + 7.62939453125e-6f * Z);
+        const float eps = 1.05f * 0.0009765625f * sqrtf(na2) * R + 7.62939453125e-6f * Z;
         thr = fminf(B, max_score) - dis0 + eps;
         lo = min_score - dis0 - eps;
       } else {
         // score = dis0 - acc / c (the codebook is staged negated); better = larger
         const float Z = fabsf(dis0) + sqrtf(na2) * R;
-        const float eps = eps_scale * (1.05f * 0.00048828125f * sqrtf(na2) * R + 7.62939453125e-6f * Z);
+        const float eps = 1.05f * 0.00048828125f * sqrtf(na2) * R + 7.62939453125e-6f * Z;
         thr = dis0 - fmaxf(B, min_score) + eps;
         lo = dis0 - max_score - eps;
       }
@@ -361,7 +355,7 @@ __global__ void __launch_bounds__(PT_NT, 1)
                      const uint16_t* __restrict__ cb_g, const float* __restrict__ pqnorm,
                      const int64_t* __restrict__ pqnorm_off, const LmTile* __restrict__ items,
                      const int64_t* __restrict__ totals, ListDirectory dir, FilterArgs f, int* __restrict__ cand_cnt,
-                     unsigned long long* __restrict__ cand, int cap, int tile_stride, int dbg) {
+                     unsigned long long* __restrict__ cand, int cap) {
   constexpr int D = M * DSUB;
   constexpr int KC = D / 8;                // core matrices along K
   constexpr int TILE = KC * 2048;          // one 128-row operand tile, bytes
@@ -377,12 +371,10 @@ __global__ void __launch_bounds__(PT_NT, 1)
   unsigned char* cb = smem;
   float* nstage = reinterpret_cast<float*>(smem + CB_BYTES);  // [PT_CS][PT_N] norms of the staged tiles
   // [codebook][norms][A tiles x 2][B tiles x 2][code stages]; the operand tiles start on 4 KiB boundaries
-  // (GB_PQTC_DBG bit 5 + bits 8.. place them at a chosen offset instead, for debugging)
   unsigned char* a_buf = smem + CB_BYTES + NRM_BYTES;
-  if (!(dbg & 32)) a_buf += (4096u - (smem_u32(a_buf) & 4095u)) & 4095u;
-  else a_buf += (dbg >> 8) & 0xFFF0;  // debugging: place the tiles at a chosen (mis)alignment
-  unsigned char* b_buf = a_buf + 2 * tile_stride;
-  unsigned char* code_buf = b_buf + 2 * tile_stride;
+  a_buf += (4096u - (smem_u32(a_buf) & 4095u)) & 4095u;
+  unsigned char* b_buf = a_buf + 2 * TILE;
+  unsigned char* code_buf = b_buf + 2 * TILE;
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int64_t n_items = totals[1];
@@ -414,7 +406,7 @@ __global__ void __launch_bounds__(PT_NT, 1)
     // issues tile i while warpgroup 0 tests tile i, warpgroup 0 issues tile i + 1 while warpgroup 1 tests tile i.
     setmaxnreg_inc<PT_REG_MMA>();
     const int h = warp >> 2, t = tid & 127;
-    const uint32_t a_base = smem_u32(a_buf) + (uint32_t)(h * tile_stride), b_base = smem_u32(b_buf);
+    const uint32_t a_base = smem_u32(a_buf) + (uint32_t)(h * TILE), b_base = smem_u32(b_buf);
     uint32_t an = 0, bn = 0;
     bool turns = false;  // warpgroup 0 has issued a tile: from then on it waits for warpgroup 1's turn
     float acc[2][64];
@@ -438,7 +430,7 @@ __global__ void __launch_bounds__(PT_NT, 1)
         else if (turns) bar_sync_256(2);
         // every warpgroup runs both m64 halves of every tile, empty rows included (their thresholds are -inf): a
         // branch around the MMAs or the wait makes ptxas serialise every wgmma of the kernel
-        const uint64_t da = lt_desc(a_base), db = lt_desc(b_base + (uint32_t)(b * tile_stride));
+        const uint64_t da = lt_desc(a_base), db = lt_desc(b_base + (uint32_t)(b * TILE));
         wg_fence();
 #pragma unroll
         for (int kk = 0; kk < KC / 2; kk++) {  // K = 16 per instruction: two core matrices = 4096 bytes further
@@ -453,7 +445,6 @@ __global__ void __launch_bounds__(PT_NT, 1)
         wg_fence_acc(acc);
         mbar_arrive(&sh.b_empty[b]);
         if (i == ntiles - 1) mbar_arrive(&sh.a_empty);
-        if (dbg & 16) __nanosleep(1000);
         // Fast path: min over the tile of acc + c * ne per pair, on the fragments themselves.  A warp where some pair
         // has a candidate redoes the test per entry and pushes the hits (pt_push_frag_hits).
         float mn[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
@@ -469,10 +460,7 @@ __global__ void __launch_bounds__(PT_NT, 1)
         bool hit = false;
 #pragma unroll
         for (int f4 = 0; f4 < 4; f4++) hit |= mn[f4] <= fthr[f4];
-        if (__any_sync(0xffffffffu, hit)) {
-          if ((t & 31) == 0) atomicAdd(&g_pqtc_dbg[1], 1ull);
-          pt_push_frag_hits(acc, sh.ne[b], fthr, fc, gm, (uint32_t)(tl.row0 + i * PT_N), &sh);
-        }
+        if (__any_sync(0xffffffffu, hit)) pt_push_frag_hits(acc, sh.ne[b], fthr, fc, gm, (uint32_t)(tl.row0 + i * PT_N), &sh);
         mbar_arrive(&sh.acc_empty[b]);
       }
       an++;
@@ -516,16 +504,6 @@ __global__ void __launch_bounds__(PT_NT, 1)
             for (int u = 0; u < M / 4; u++) w[u] = reinterpret_cast<const uint32_t*>(cp)[u];
           }
         }
-        if (dbg & 4) {  // compare what the stage held with the list in global memory
-          const int rowc = t.row0 + i * PT_N + e;
-          if (rowc < t.row0 + t.nrows) {
-            const uint32_t* g = reinterpret_cast<const uint32_t*>(dir.codes[t.list] + (int64_t)rowc * M);
-            bool bad = false;
-#pragma unroll
-            for (int u = 0; u < M / 4; u++) bad |= (w[u] != g[u]);
-            if (bad) atomicAdd(&g_pqtc_dbg[0], 1ull);
-          }
-        }
         const float nstaged = HAS_NORM ? nstage[s * PT_N + e] : 0.f;
         mbar_arrive(&sh.code_empty[s]);
         // entries past the end of the segment decode whatever bytes the stage holds: finite values,
@@ -539,8 +517,7 @@ __global__ void __launch_bounds__(PT_NT, 1)
         }
         const int b = bn & 1;
         mbar_wait(&sh.b_empty[b], ((bn >> 1) & 1) ^ 1);
-        if (dbg & 1) __nanosleep(3000);
-        unsigned char* brow = b_buf + b * tile_stride + e * 16;
+        unsigned char* brow = b_buf + b * TILE + e * 16;
         const float nsum = nstaged;
 #pragma unroll
         for (int m = 0; m < M; m++) {
@@ -576,7 +553,7 @@ __global__ void __launch_bounds__(PT_NT, 1)
         if (elect_one()) {
           mbar_arrive_expect_tx(&sh.a_full, 2 * TILE);
           for (int h = 0; h < 2; h++)
-            bulk_g2s(a_buf + h * tile_stride, a_scratch + ((int64_t)t.grp * 2 + h) * TILE, TILE, &sh.a_full);
+            bulk_g2s(a_buf + h * TILE, a_scratch + ((int64_t)t.grp * 2 + h) * TILE, TILE, &sh.a_full);
         }
         __syncwarp();
         const unsigned char* lcodes = dir.codes[t.list];
@@ -720,11 +697,8 @@ cudaError_t launch_scan_shape(const unsigned char* a_scratch, const PairMeta* me
                               const int64_t* pqnorm_off,
                               const LmTile* items, const int64_t* totals, ListDirectory dir, FilterArgs f, int metric,
                               int* cand_cnt, unsigned long long* cand, int cap, int grid, cudaStream_t st) {
-  constexpr int D = M * DSUB;
-  int tile_stride = (D / 8) * 2048, dbg = 0;
-  if (const char* ev = getenv("GB_PQTC_DBG")) dbg = atoi(ev);
-  if (dbg & 2) tile_stride = next_pow2(tile_stride);
-  const size_t base = (size_t)M * PT_KSUB * DSUB * 2 + 4 * (size_t)tile_stride + (size_t)PT_CS * PT_N * M + 4096;
+  constexpr int TILE = (M * DSUB / 8) * 2048;
+  const size_t base = (size_t)M * PT_KSUB * DSUB * 2 + 4 * (size_t)TILE + (size_t)PT_CS * PT_N * M + 4096;
   const bool l2 = metric == kMetricL2;
   const bool eager = f.del_bits != nullptr || f.filter_bits != nullptr;
   if (l2 && (!pqnorm || !pqnorm_off)) return cudaErrorInvalidValue;
@@ -732,7 +706,7 @@ cudaError_t launch_scan_shape(const unsigned char* a_scratch, const PairMeta* me
   auto go = [&](auto kern) -> cudaError_t {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    kern<<<grid, PT_NT, smem, st>>>(a_scratch, meta, cb, pqnorm, pqnorm_off, items, totals, dir, f, cand_cnt, cand, cap, tile_stride, dbg);
+    kern<<<grid, PT_NT, smem, st>>>(a_scratch, meta, cb, pqnorm, pqnorm_off, items, totals, dir, f, cand_cnt, cand, cap);
     note_launch();
     return cudaGetLastError();
   };
@@ -779,14 +753,6 @@ cudaError_t launch_pq_entry_norms(ListDirectory dir, int nlist, int max_len, int
   return cudaGetLastError();
 }
 
-void pqtc_debug_counters(unsigned long long out[4], bool reset) {
-  cudaMemcpyFromSymbol(out, g_pqtc_dbg, sizeof(unsigned long long) * 4);
-  if (reset) {
-    const unsigned long long z[4] = {0, 0, 0, 0};
-    cudaMemcpyToSymbol(g_pqtc_dbg, z, sizeof(z));
-  }
-}
-
 bool pqtc_supported(int M, int dsub) {
   // power-of-two shapes only.  (M = 12, dsub = 8 -- 1536-byte code tiles, 24 KiB operand tiles -- compiled and ran, but
   // intermittently (about 1 search in 100, on some boxes more) lost the rows of one decode warp of a tile; the cause
@@ -817,20 +783,19 @@ cudaError_t launch_pqtc_plan_phase_a(const int32_t* probe_ids, int64_t npairs, i
 cudaError_t launch_pq_stage_pairs(const float* xq, int64_t ldq, int d, const float* coarse, int64_t ldc, const LmTile* items,
                                   int max_items, const int64_t* totals, const int64_t* pair_j, int nprobe,
                                   const float* coarse_dis, const unsigned long long* bound_keys, int64_t bound_stride,
-                                  int kprime, const float* rmax2, FilterArgs f, int metric, float eps_scale,
-                                  unsigned char* a_scratch, void* meta, int* cand_cnt, int cap, const int* row_limit,
-                                  cudaStream_t st) {
+                                  int kprime, const float* rmax2, FilterArgs f, int metric, unsigned char* a_scratch,
+                                  void* meta, int* cand_cnt, int cap, const int* row_limit, cudaStream_t st) {
   if (max_items <= 0) return cudaSuccess;
   if (d % 16) return cudaErrorInvalidValue;
   if (metric == kMetricL2)
     pq_stage_pairs_kernel<kMetricL2><<<max_items, PT_G, 0, st>>>(xq, ldq, d, coarse, ldc, items, totals, pair_j, nprobe,
                                                                 coarse_dis, bound_keys, bound_stride, kprime, rmax2,
-                                                                f.min_score, f.max_score, eps_scale, a_scratch,
+                                                                f.min_score, f.max_score, a_scratch,
                                                                 static_cast<PairMeta*>(meta), cand_cnt, cap, row_limit);
   else
     pq_stage_pairs_kernel<kMetricIP><<<max_items, PT_G, 0, st>>>(xq, ldq, d, coarse, ldc, items, totals, pair_j, nprobe,
                                                                 coarse_dis, bound_keys, bound_stride, kprime, rmax2,
-                                                                f.min_score, f.max_score, eps_scale, a_scratch,
+                                                                f.min_score, f.max_score, a_scratch,
                                                                 static_cast<PairMeta*>(meta), cand_cnt, cap, row_limit);
   note_launch();
   return cudaGetLastError();
