@@ -97,7 +97,8 @@ int gb_index_nlist(gb_index *index);
 int gb_index_set_centroids(gb_index *index, const float *centroids, int nlist); /* marks trained */
 int gb_index_get_centroids(gb_index *index, float *centroids);
 int gb_index_pq_m(gb_index *index);
-int gb_index_set_pq_centroids(gb_index *index, const float *pq); /* [M][256][dsub] */
+int gb_index_pq_ksub(gb_index *index); /* centroids per sub-quantiser: 256 (IVFPQ), 16 (IVFPQFastScan) */
+int gb_index_set_pq_centroids(gb_index *index, const float *pq); /* [M][ksub][dsub] */
 int gb_index_get_pq_centroids(gb_index *index, float *pq);
 int gb_index_get_precomputed_table(gb_index *index, float *table); /* [nlist][M][256] */
 /* OPQ rotation of an IVFPQ index created with "opq": {"nsubvector": M} (gamma_index_ivfpq.cc:168-178):
@@ -136,6 +137,10 @@ int gb_index_search_preassigned(gb_index *index, int nq, const float *x, int k, 
                                 float min_score, float max_score, float *out_scores, int64_t *out_ids);
 /* pq.compute_codes on residuals (gamma_index_ivfpq.cc:489-494) */
 int gb_index_pq_encode(gb_index *index, int64_t n, const float *x, const int64_t *assign, uint8_t *codes);
+/* IVFPQFastScan encodes raw vectors (assign is ignored, may be NULL): codes = n x ceil(M/2) bytes, sub-quantiser 2j in
+   the low nibble of byte j.  The uint8 look-up tables of a query batch: lut8 = nq x M x 16, ab = nq x (a, b), the
+   score of an entry being accu * (1/a) + b; metric -1 = the index metric. */
+int gb_index_pqfs_lut(gb_index *index, int nq, const float *x, int metric, uint8_t *lut8, float *ab);
 
 /* ---- standalone kernels exposed for tests / bench ---- */
 /* faiss Clustering restated (k-means), host in/out; obj (niter floats) may be NULL */

@@ -66,6 +66,8 @@ def _declare(l):
     l.gb_index_set_centroids.argtypes = [vp, vp, i32]
     l.gb_index_get_centroids.argtypes = [vp, vp]
     l.gb_index_pq_m.argtypes = [vp]
+    l.gb_index_pq_ksub.argtypes = [vp]
+    l.gb_index_pqfs_lut.argtypes = [vp, i32, vp, i32, vp, vp]
     l.gb_index_set_pq_centroids.argtypes = [vp, vp]
     l.gb_index_get_pq_centroids.argtypes = [vp, vp]
     l.gb_index_get_precomputed_table.argtypes = [vp, vp]

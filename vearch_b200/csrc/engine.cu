@@ -317,7 +317,8 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     training_threshold_ = mp.training_threshold;  // table.cc:143-150
   if (training_threshold_ > 0) mp.training_threshold = training_threshold_;
   Index* idx = create_index(index_type_, dim_, mp, device_, 20);
-  if (!idx) return Status::Make(index_type_ == "FLAT" || index_type_ == "IVFFLAT" || index_type_ == "IVFPQ"
+  if (!idx) return Status::Make(index_type_ == "FLAT" || index_type_ == "IVFFLAT" || index_type_ == "IVFPQ" ||
+                                        index_type_ == "IVFPQFastScan"
                                     ? kInvalidArgument
                                     : kNotSupported,
                                 last_error());
@@ -1319,7 +1320,8 @@ int Engine::Dump() {
   f.write(reinterpret_cast<const char*>(rows.data()), (std::streamsize)(rows.size() * 4));
   int trained = index_->trained() ? 1 : 0;
   wr<int32_t>(f, trained);
-  IVFFlatIndex* ivf = dynamic_cast<IVFFlatIndex*>(index_.get());
+  // an index whose trained state does not persist (IVFPQFastScan) is trained again by Load
+  IVFFlatIndex* ivf = index_->persists_trained_state() ? dynamic_cast<IVFFlatIndex*>(index_.get()) : nullptr;
   IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(index_.get());
   if (trained && ivf) {
     std::vector<float> c((size_t)ivf->nlist() * dim_);
@@ -1405,7 +1407,7 @@ int Engine::Load() {
     int64_t eload = 0;
     if (eivf) eivf->load_gamma(dir, e.name + ".000", &eload);  // trained state + lists; absent: trained again later
   }
-  IVFFlatIndex* ivf = dynamic_cast<IVFFlatIndex*>(index_.get());
+  IVFFlatIndex* ivf = index_->persists_trained_state() ? dynamic_cast<IVFFlatIndex*>(index_.get()) : nullptr;
   IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(index_.get());
   if (trained && ivf) {
     std::vector<float> c((size_t)ivf->nlist() * dim_);

@@ -967,7 +967,7 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
   std::vector<unsigned long long> h_best(n);
   std::vector<int32_t> h_off(k + 1), h_perm(n), cursor(k);
   std::vector<float> hassign(k), h_cent;
-  const int metric = kp.spherical ? kMetricIP : kMetricL2;  // gamma's quantizer is IndexFlat(d, metric)
+  const int metric = kp.spherical && !kp.l2_assign ? kMetricIP : kMetricL2;  // gamma's quantizer is IndexFlat(d, metric)
   const bool use_tc = k >= 64;  // tensor-core (wgmma 3xTF32) distance tiles
   for (int it = 0; it < kp.niter; it++) {
     GB_CUDA(launch_fill_u64(best, n, kKeySentinel, st));
@@ -1118,6 +1118,10 @@ int IVFFlatIndex::train() {
   const bool is_pq = (type_ == "IVFPQ");
   kp.niter = is_pq ? 10 : 25;                              // gamma_index_ivfpq.cc:188
   kp.spherical = is_pq && mp_.metric == kMetricIP;          // gamma_index_ivfpq.cc:189-191
+  if (type_ == "IVFPQFastScan") {  // gamma_index_ivfpqfs.cc:95-104: IndexFlatL2 quantiser, spherical for IP, niter kept
+    kp.spherical = mp_.metric == kMetricIP;
+    kp.l2_assign = true;
+  }
   xt = train_transform(xt, num, s);  // OPQ: learn the rotation, continue on the rotated slab
   if (!xt) return -1;
   if (kmeans_device(xt, dpad_, num, d_, nlist_, kp, d_centroids_, dpad_, st, nullptr)) return -1;
@@ -1134,8 +1138,9 @@ int IVFFlatIndex::assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* ou
   GB_ALLOC(best, unsigned long long, n, s);
   GB_CUDA(launch_fill_u64(best, n, kKeySentinel, st));
   // always the exact CUDA-core kernel, never the tensor-core tiles: list membership stays deterministic against the oracle
-  GB_CUDA(launch_dist_argmin(x, ldx, (int)n, d_centroids_, dpad_, nlist_, dpad_, mp_.metric, best, 0, st));
-  GB_CUDA(launch_split_keys(best, n, mp_.metric, nullptr, out, st));
+  const int metric = coarse_metric(mp_.metric);
+  GB_CUDA(launch_dist_argmin(x, ldx, (int)n, d_centroids_, dpad_, nlist_, dpad_, metric, best, 0, st));
+  GB_CUDA(launch_split_keys(best, n, metric, nullptr, out, st));
   return 0;
 }
 
@@ -1560,7 +1565,7 @@ int IVFFlatIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f,
     Scratch sb(s.stream());
     GB_ALLOC(probe_ids, int32_t, (size_t)qb * nprobe, sb);
     GB_ALLOC(coarse_dis, float, (size_t)qb * nprobe, sb);
-    if (coarse_dev(qb, xq + (int64_t)q0 * dpad_, nprobe, metric, probe_ids, coarse_dis, sb)) return -1;
+    if (coarse_dev(qb, xq + (int64_t)q0 * dpad_, nprobe, coarse_metric(metric), probe_ids, coarse_dis, sb)) return -1;
     if (scan_dev(ctx, f, metric, qb, xq + (int64_t)q0 * dpad_, k, probe_ids, coarse_dis, nprobe,
                  out_keys + (int64_t)q0 * k, sb))
       return -1;
@@ -1579,7 +1584,7 @@ int IVFFlatIndex::coarse_search_host(int nq, const float* x, int nprobe, float* 
   GB_ALLOC(ids, int32_t, (size_t)nq * nprobe, s);
   GB_ALLOC(dis, float, (size_t)nq * nprobe, s);
   const float* dqt = transform_dev(dq, nq, s);
-  if (!dqt || coarse_dev(nq, dqt, nprobe, mp_.metric, ids, dis, s)) return -1;
+  if (!dqt || coarse_dev(nq, dqt, nprobe, coarse_metric(mp_.metric), ids, dis, s)) return -1;
   std::vector<int32_t> h((size_t)nq * nprobe);
   GB_CUDA(cudaMemcpyAsync(h.data(), ids, h.size() * 4, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaMemcpyAsync(out_dis, dis, h.size() * 4, cudaMemcpyDeviceToHost, st));
@@ -2176,6 +2181,172 @@ int IVFPQIndex::search_preassigned_host(const SearchContext& ctx, int nq, const 
 }
 
 // ------------------------------------------------------------------------------------------
+IVFPQFastScanIndex::IVFPQFastScanIndex(int d, const ModelParams& mp, int device, int seg_shift)
+    : IVFFlatIndex(d, mp, device, seg_shift, "IVFPQFastScan"), M_(mp.nsubvector), dsub_(d / mp.nsubvector) {
+  cudaMalloc(&d_pq_, (size_t)M_ * kKsub * dsub_ * 4);
+  cudaMemset(d_pq_, 0, (size_t)M_ * kKsub * dsub_ * 4);
+}
+IVFPQFastScanIndex::~IVFPQFastScanIndex() { cudaFree(d_pq_); }
+int IVFPQFastScanIndex::training_threshold() const {
+  // gamma_index_ivfpqfs.cc: default nlist * 39; Indexing() clamps to [39, 256] * nlist like IVFPQ
+  int64_t t = mp_.training_threshold ? mp_.training_threshold : (int64_t)nlist_ * 39;
+  if (t < nlist_)
+    t = (int64_t)nlist_ * 39;
+  else if (t > (int64_t)nlist_ * 256)
+    t = (int64_t)nlist_ * 256;
+  return (int)t;
+}
+int64_t IVFPQFastScanIndex::index_mem_bytes() const { return IVFFlatIndex::index_mem_bytes() + (int64_t)M_ * kKsub * dsub_ * 4; }
+int IVFPQFastScanIndex::set_pq_centroids(const float* host) {
+  cudaSetDevice(device_);
+  std::unique_lock<std::shared_mutex> lk(mu_);
+  drain_searches();
+  GB_CUDA(cudaMemcpy(d_pq_, host, (size_t)M_ * kKsub * dsub_ * 4, cudaMemcpyHostToDevice));
+  return 0;
+}
+int IVFPQFastScanIndex::get_pq_centroids(float* host) const {
+  cudaSetDevice(device_);
+  GB_CUDA(cudaMemcpy(host, d_pq_, (size_t)M_ * kKsub * dsub_ * 4, cudaMemcpyDeviceToHost));
+  return 0;
+}
+int IVFPQFastScanIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
+  (void)dir;
+  (void)abs_name;
+  return 0;
+}
+int IVFPQFastScanIndex::load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) {
+  (void)dir;
+  (void)abs_name;
+  *load_num = 0;
+  return 0;
+}
+
+// faiss ProductQuantizer::train with ksub = 16 on the raw training vectors (by_residual = false): the same
+// sub-sampling rule as the 256-centroid IVFPQ codebook (at most 256 * ksub points), then M independent 16-means.
+int IVFPQFastScanIndex::train_extra(const float* xtrain, int64_t n, Scratch& s) {
+  cudaStream_t st = s.stream();
+  const int64_t npq = std::min<int64_t>(n, 256 * kKsub);
+  const float* xs = xtrain;
+  if (npq < n) {
+    std::vector<int32_t> perm;
+    rand_perm_mt(perm, n, 1234);
+    GB_ALLOC(d_idx, int32_t, npq, s);
+    GB_CUDA(cudaMemcpyAsync(d_idx, perm.data(), (size_t)npq * 4, cudaMemcpyHostToDevice, st));
+    GB_ALLOC(sub, float, (size_t)npq * dpad_, s);
+    GB_CUDA(launch_gather_rows(xtrain, dpad_, d_idx, npq, dpad_, sub, dpad_, st));
+    GB_CUDA(cudaStreamSynchronize(st));
+    xs = sub;
+  }
+  const int dsp = (int)round_up(dsub_, 4);
+  GB_ALLOC(slice, float, (size_t)npq * dsp, s);
+  GB_ALLOC(cent, float, (size_t)kKsub * dsp, s);
+  KMeansParams kp;  // ClusteringParameters defaults: niter 25, seed 1234, max 256 points per centroid
+  for (int m = 0; m < M_; m++) {
+    GB_CUDA(launch_slice_cols(xs, dpad_, npq, m * dsub_, dsub_, slice, dsp, st));
+    if (kmeans_device(slice, dsp, npq, dsub_, kKsub, kp, cent, dsp, st, nullptr)) return -1;
+    GB_CUDA(cudaMemcpy2DAsync(d_pq_ + (size_t)m * kKsub * dsub_, (size_t)dsub_ * 4, cent, (size_t)dsp * 4, (size_t)dsub_ * 4,
+                              kKsub, cudaMemcpyDeviceToDevice, st));
+  }
+  return 0;
+}
+
+int IVFPQFastScanIndex::append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                                     const int32_t* d_assign, Scratch& s) {
+  (void)d_assign;
+  cudaStream_t st = s.stream();
+  const int cb = code_bytes();
+  GB_ALLOC(codes, uint8_t, (size_t)n * cb, s);
+  GB_CUDA(launch_pqfs_encode(x, dpad_, n, d_pq_, M_, dsub_, codes, st));
+  GB_CUDA(launch_ivf_append_codes(codes, n, cb, d_list, d_pos, reinterpret_cast<uint8_t* const*>(lists_->d_data()),
+                                  lists_->d_ids(), vid0, st));
+  return 0;
+}
+
+int IVFPQFastScanIndex::encode_host(const float* x, int64_t n, uint8_t* codes_out) {
+  cudaSetDevice(device_);
+  cudaStream_t st = thread_stream(device_);
+  Scratch s(st);
+  const int cb = code_bytes();
+  GB_ALLOC(dx, float, (size_t)n * dpad_, s);
+  GB_CUDA(cudaMemsetAsync(dx, 0, (size_t)n * dpad_ * 4, st));
+  GB_CUDA(cudaMemcpy2DAsync(dx, (size_t)dpad_ * 4, x, (size_t)d_ * 4, (size_t)d_ * 4, n, cudaMemcpyHostToDevice, st));
+  GB_ALLOC(codes, uint8_t, (size_t)n * cb, s);
+  GB_CUDA(launch_pqfs_encode(dx, dpad_, n, d_pq_, M_, dsub_, codes, st));
+  GB_CUDA(cudaMemcpyAsync(codes_out, codes, (size_t)n * cb, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int IVFPQFastScanIndex::lut_host(int nq, const float* x, int metric, uint8_t* lut8_out, float* ab_out) {
+  cudaSetDevice(device_);
+  cudaStream_t st = thread_stream(device_);
+  Scratch s(st);
+  GB_ALLOC(dx, float, (size_t)nq * dpad_, s);
+  GB_CUDA(cudaMemsetAsync(dx, 0, (size_t)nq * dpad_ * 4, st));
+  GB_CUDA(cudaMemcpy2DAsync(dx, (size_t)dpad_ * 4, x, (size_t)d_ * 4, (size_t)d_ * 4, nq, cudaMemcpyHostToDevice, st));
+  GB_ALLOC(lut, uint8_t, (size_t)nq * M_ * kKsub, s);
+  GB_ALLOC(ab, float, (size_t)nq * 2, s);
+  GB_CUDA(launch_pqfs_lut(dx, dpad_, nq, d_pq_, M_, dsub_, metric >= 0 ? metric : mp_.metric, lut, ab, st));
+  GB_CUDA(cudaMemcpyAsync(lut8_out, lut, (size_t)nq * M_ * kKsub, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaMemcpyAsync(ab_out, ab, (size_t)nq * 8, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// IndexIVFFastScan::search_preassigned restated over this engine's lists, filters applied before selection;
+// recall_num > 0 re-ranks the recall_num best exactly from the raw vectors, as IVFPQ does
+int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
+                                 const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
+                                 Scratch& s) {
+  (void)coarse_dis;  // no residual: the list's coarse distance takes no part in the score
+  cudaStream_t st = s.stream();
+  if (metric != mp_.metric) {
+    set_last_error("IVFPQFastScan: per-request metric must equal the trained metric");
+    return -1;
+  }
+  const bool rerank = ctx.params.recall_num > 0;
+  int kk = k;
+  if (ctx.params.recall_num > k) kk = ctx.params.recall_num;
+  if (kk > 4096) {
+    set_last_error("IVFPQFastScan: recall_num / topn above 4096 is not supported");
+    return -1;
+  }
+  GB_ALLOC(lut, uint8_t, (size_t)nq * M_ * kKsub, s);
+  GB_ALLOC(ab, float, (size_t)nq * 2, s);
+  {
+    StageScope stage(this, "pqfs_lut_kernel", st);
+    GB_CUDA(launch_pqfs_lut(xq, dpad_, nq, d_pq_, M_, dsub_, metric, lut, ab, st));
+  }
+  unsigned long long* fs = out_keys;
+  if (rerank) {
+    fs = s.alloc_n<unsigned long long>((size_t)nq * kk);
+    if (!fs) return -1;
+  }
+  const int nsm = sm_count(device_);
+  const int pg = (int)std::min<int64_t>(32, std::max<int64_t>(1, (int64_t)nprobe * nq / ((int64_t)nsm * 32)));
+  const int ngroups = (nprobe + pg - 1) / pg;
+  GB_ALLOC(partial, unsigned long long, (size_t)nq * ngroups * kk, s);
+  last_scan_kernel_ = "ivfpqfs_scan_kernel";
+  snprintf(last_scan_info_, sizeof(last_scan_info_), "{\"probes_per_cta\": %d}", pg);
+  scan_timer_begin(st);
+  stage_begin("ivfpqfs_scan_kernel", st);
+  GB_CUDA(launch_ivfpqfs_scan(lut, ab, nq, probe_ids, nprobe, pg, lists_->directory(), M_, kk, metric, f, partial, st));
+  stage_end(st);
+  scan_timer_end(st);
+  if (ngroups > 1) {
+    GB_CUDA(launch_select_keys(partial, (int64_t)ngroups * kk, nq, ngroups * kk, kk, fs, kk, st));
+  } else {
+    GB_CUDA(cudaMemcpyAsync(fs, partial, (size_t)nq * kk * 8, cudaMemcpyDeviceToDevice, st));
+  }
+  if (rerank) {
+    StageScope stage(this, "rerank_kernel", st);
+    GB_CUDA(launch_rerank(fs, kk, nq, xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_, k, metric, f, out_keys,
+                          st));
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
 Index* create_index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
@@ -2214,6 +2385,35 @@ Index* create_index(const std::string& type, int d, const ModelParams& mp, int d
       return nullptr;
     }
     return new IVFPQIndex(d, mp, device, seg_shift);
+  }
+  if (type == "IVFPQFastScan") {  // IVFPQFastScanModelParams::Validate (gamma_index_ivfpqfs.h:231-245)
+    if (mp.nsubvector <= 0 || d % mp.nsubvector != 0) {
+      set_last_error("Dimension [" + std::to_string(d) + "] cannot divide by nsubvector [" + std::to_string(mp.nsubvector) +
+                     "].");
+      return nullptr;
+    }
+    if (mp.nsubvector > IVFPQFastScanIndex::kMaxM) {
+      set_last_error("IVFPQFastScan: nsubvector [" + std::to_string(mp.nsubvector) + "] above " +
+                     std::to_string(IVFPQFastScanIndex::kMaxM) + " is not supported by this engine");
+      return nullptr;
+    }
+    if (mp.bbs < -1) {
+      set_last_error("invalid bbs =" + std::to_string(mp.bbs));
+      return nullptr;
+    }
+    if (mp.bbs > 0 && mp.bbs % 32 != 0) {
+      set_last_error("bbs only supports the case where 32 can be divided evenly, bbs=" + std::to_string(mp.bbs));
+      return nullptr;
+    }
+    if (mp.has_opq) {
+      set_last_error("IVFPQFastScan: opq is not supported by this engine");
+      return nullptr;
+    }
+    if (mp.ncentroids <= 0 || mp.nprobe > mp.ncentroids) {
+      set_last_error("nprobe should be less than ncentroids");
+      return nullptr;
+    }
+    return new IVFPQFastScanIndex(d, mp, device, seg_shift);
   }
   set_last_error("unsupported index type " + type);
   return nullptr;

@@ -153,6 +153,8 @@ struct ModelParams {  // index/impl/gamma_index_ivfpq.h:1031-1257, gamma_index_i
   int bucket_init_size = 1000;
   int bucket_max_size = 1280000;
   int opq_nsubvector = 0;       // > 0: OPQ rotation in front of the IVFPQ index (gamma_index_ivfpq.h:1202-1216)
+  bool has_opq = false;         // an "opq" object was given (IVFPQFastScan refuses it)
+  int bbs = 32;                 // IVFPQFastScan block size as given (gamma_index_ivfpqfs.h:126-133; <= 0 => 32)
 };
 
 struct RetrievalParams {  // gamma_index_ivfpq.cc:233-294, gamma_index_ivfflat.cc:293-340
@@ -185,6 +187,8 @@ class Index {
   int64_t indexed_count() const { return indexed_count_; }
   bool trained() const { return trained_; }
   virtual int training_threshold() const { return 0; }
+  // whether Engine::Dump saves the trained state (centroids, codebook) for Load to restore; false: Load trains again
+  virtual bool persists_trained_state() const { return true; }
 
   // AddToStore (vector_manager.cc:455): append raw vectors, host rows n x d
   int add_vectors(const float* x, int64_t n);
@@ -321,6 +325,7 @@ struct KMeansParams {
   bool spherical = false;
   int max_points_per_centroid = 256;
   bool hot_start = false;  // keep the centroids passed in as the initial state (ProductQuantizer::Train_hot_start)
+  bool l2_assign = false;  // spherical, but assign by L2 (quantiser IndexFlatL2, as IVFPQFastScan has under IP)
 };
 int kmeans_device(const float* x, int64_t ldx, int64_t n, int d, int k, const KMeansParams& kp, float* centroids,
                   int64_t ldc, cudaStream_t st, std::vector<float>* obj);
@@ -351,8 +356,8 @@ class IVFFlatIndex : public Index {
   // a bulk add_pending when more than half of the slab space is dead
   int compact_lists();
   int mirror_builds() const { return mirror_.builds; }  // test hook
-  int dump_gamma(const std::string& dir, const std::string& abs_name);
-  int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num);
+  virtual int dump_gamma(const std::string& dir, const std::string& abs_name);
+  virtual int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num);
 
  protected:
   virtual const char* gamma_file_name() const;
@@ -369,6 +374,8 @@ class IVFFlatIndex : public Index {
                          int nprobe, unsigned long long* out_keys, Scratch& s);
   int assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* assign_dev_out, Scratch& s);
   int resolve_nprobe(const SearchContext& ctx) const;
+  // metric of the coarse quantiser (list assignment and probe choice) for a search under `metric`
+  virtual int coarse_metric(int metric) const { return metric; }
   virtual int code_bytes() const { return dpad_ * 4; }
   virtual int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
                            const int32_t* d_assign, Scratch& s);
@@ -484,6 +491,44 @@ class IVFPQIndex : public IVFFlatIndex {
   int set_opq(const float* host_A);        // d x d row-major; marks the rotation trained
   int get_opq(float* host_A) const;
   int apply_opq_host(const float* x, int64_t n, float* out);  // test hook: y = A x through the device path
+};
+
+// GammaIVFPQFastScanIndex (index/impl/gamma_index_ivfpqfs.{h,cc}): faiss::IndexIVFPQFastScan with by_residual = false.
+// The lists hold 4-bit codes of the raw vectors (16-centroid PQ, two codes per byte); a search quantises each query's
+// M x 16 table to uint8 and sums it in integers.  The coarse quantiser is IndexFlatL2 under either metric.
+class IVFPQFastScanIndex : public IVFFlatIndex {
+ public:
+  static constexpr int kKsub = 16;
+  IVFPQFastScanIndex(int d, const ModelParams& mp, int device, int seg_shift);
+  ~IVFPQFastScanIndex() override;
+  int training_threshold() const override;
+  int64_t index_mem_bytes() const override;
+  int M() const { return M_; }
+  int dsub() const { return dsub_; }
+  // M above this: faiss's 16-bit table sums could wrap (255 * 257 < 2^16), and the byte-pair table grows past what
+  // the scan's shared memory holds beside its stages and queue
+  static constexpr int kMaxM = 256;
+  bool persists_trained_state() const override { return false; }
+  int set_pq_centroids(const float* host);  // [M][16][dsub]
+  int get_pq_centroids(float* host) const;
+  int encode_host(const float* x, int64_t n, uint8_t* codes_out);  // n x ceil(M/2) packed codes
+  // uint8 tables [nq][M][16] and (a, b) [nq][2] of a query batch under `metric` (-1: the index metric)
+  int lut_host(int nq, const float* x, int metric, uint8_t* lut8_out, float* ab_out);
+  // the reference dumps no index file: a loaded table trains and fills this index again from its raw vectors
+  int dump_gamma(const std::string& dir, const std::string& abs_name) override;
+  int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) override;
+
+ protected:
+  int coarse_metric(int metric) const override { (void)metric; return kMetricL2; }
+  int code_bytes() const override { return (M_ + 1) / 2; }
+  int train_extra(const float* xtrain, int64_t n, Scratch& s) override;
+  int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                   const int32_t* d_assign, Scratch& s) override;
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
+               const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
+               Scratch& s) override;
+  int M_, dsub_;
+  float* d_pq_ = nullptr;  // [M][16][dsub]
 };
 
 // reflector (index/reflector.h:68-80): type name -> index object

@@ -54,6 +54,7 @@ bool parse_model_params(const std::string& text, ModelParams* mp, std::string* e
     if (v > 0) mp->nsubvector = v;
   }
   if (const JsonValue* opq = jv.get("opq")) {  // gamma_index_ivfpq.h:1202-1216
+    mp->has_opq = opq->type == JsonValue::Object;
     if (opq->type == JsonValue::Object && opq->get_int("nsubvector", &v)) {
       if (v < -1) {
         *err = "invalid opq_nsubvector = " + std::to_string(v);
@@ -83,6 +84,9 @@ bool parse_model_params(const std::string& text, ModelParams* mp, std::string* e
     }
     if (v > 0) mp->bucket_max_size = v;
   }
+  // IVFPQFastScan only (validated by create_index): the reference's bbs-blocked list layout never leaves its process, so
+  // the block size has no effect here beyond being checked
+  if (jv.get_int("bbs", &v)) mp->bbs = v;
   if (jv.get_int("training_threshold", &v) && v > 0) mp->training_threshold = v;
   std::string mt;
   if (jv.get_string("metric_type", &mt)) {
@@ -281,6 +285,10 @@ static IVFPQIndex* as_pq(gb_index* index) {
   if (!index || !index->impl) return nullptr;
   return dynamic_cast<IVFPQIndex*>(index->impl);
 }
+static IVFPQFastScanIndex* as_pqfs(gb_index* index) {
+  if (!index || !index->impl) return nullptr;
+  return dynamic_cast<IVFPQFastScanIndex*>(index->impl);
+}
 #define IVF_OR_FAIL(v, index)                \
   IVFFlatIndex* v = as_ivf(index);           \
   if (!v) {                                  \
@@ -307,16 +315,32 @@ int gb_index_get_centroids(gb_index* index, float* centroids) {
   return ivf->get_centroids(centroids);
 }
 int gb_index_pq_m(gb_index* index) {
+  if (IVFPQFastScanIndex* fs = as_pqfs(index)) return fs->M();
   PQ_OR_FAIL(pq, index);
   return pq->M();
 }
+int gb_index_pq_ksub(gb_index* index) {
+  if (as_pqfs(index)) return IVFPQFastScanIndex::kKsub;
+  PQ_OR_FAIL(pq, index);
+  return 256;
+}
 int gb_index_set_pq_centroids(gb_index* index, const float* pqc) {
+  if (IVFPQFastScanIndex* fs = as_pqfs(index)) return fs->set_pq_centroids(pqc);
   PQ_OR_FAIL(pq, index);
   return pq->set_pq_centroids(pqc);
 }
 int gb_index_get_pq_centroids(gb_index* index, float* pqc) {
+  if (IVFPQFastScanIndex* fs = as_pqfs(index)) return fs->get_pq_centroids(pqc);
   PQ_OR_FAIL(pq, index);
   return pq->get_pq_centroids(pqc);
+}
+int gb_index_pqfs_lut(gb_index* index, int nq, const float* x, int metric, uint8_t* lut8, float* ab) {
+  IVFPQFastScanIndex* fs = as_pqfs(index);
+  if (!fs) {
+    set_last_error("not an IVFPQFastScan index");
+    return -1;
+  }
+  return fs->lut_host(nq, x, metric, lut8, ab);
 }
 int gb_index_get_precomputed_table(gb_index* index, float* table) {
   PQ_OR_FAIL(pq, index);
@@ -372,6 +396,7 @@ int gb_index_list_len(gb_index* index, int list) {
 int gb_index_code_size(gb_index* index) {
   IVF_OR_FAIL(ivf, index);
   IVFPQIndex* pq = as_pq(index);
+  if (IVFPQFastScanIndex* fs = as_pqfs(index)) return (fs->M() + 1) / 2;
   return pq ? pq->M() : ((ivf->d() + 3) / 4 * 4) * 4;
 }
 int gb_index_get_list(gb_index* index, int list, uint8_t* codes, int64_t* ids) {
@@ -405,6 +430,7 @@ int gb_index_search_preassigned(gb_index* index, int nq, const float* x, int k, 
   return ivf->search_preassigned_host(ctx, nq, x, k, keys, coarse_dis, nprobe, out_scores, out_ids);
 }
 int gb_index_pq_encode(gb_index* index, int64_t n, const float* x, const int64_t* assign, uint8_t* codes) {
+  if (IVFPQFastScanIndex* fs = as_pqfs(index)) return fs->encode_host(x, n, codes);
   PQ_OR_FAIL(pq, index);
   return pq->encode_host(x, n, assign, codes);
 }

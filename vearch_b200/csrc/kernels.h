@@ -208,6 +208,19 @@ cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq
                           const float* const* raw_segments, int seg_shift, int64_t ld_raw, int k, int metric,
                           FilterArgs f, unsigned long long* out_keys, cudaStream_t st);
 
+// ---- K11: IVFPQFastScan (kernels_pqfs.cu): 16-centroid PQ on raw vectors, 4-bit codes, uint8 tables -------------
+// codes[i][j] = code(2j) | code(2j + 1) << 4, code(m) = argmin_c |x_i|m - pq_m[c]|^2; pq_centroids [M][16][dsub]
+cudaError_t launch_pqfs_encode(const float* x, int64_t ldx, int64_t n, const float* pq_centroids, int M, int dsub, uint8_t* codes,
+                               cudaStream_t st);
+// per query the M x 16 float table (L2 distance / inner product per sub-vector), quantised per sub-quantiser:
+// lut8[q][m][c] = floor((v - min_m) a + 0.5), a = 255 / max_m span_m (1 if every span is 0), ab[q] = (a, sum_m min_m)
+cudaError_t launch_pqfs_lut(const float* xq, int64_t ldq, int nq, const float* pq_centroids, int M, int dsub, int metric,
+                            uint8_t* lut8, float* ab, cudaStream_t st);
+// partial[q][group][k] sorted, group = ceil(nprobe / pg) CTAs per query; score = accu * (1 / a) + b
+cudaError_t launch_ivfpqfs_scan(const uint8_t* lut8, const float* ab, int nq, const int32_t* probe_ids, int nprobe, int pg,
+                                ListDirectory dir, int M, int k, int metric, FilterArgs f, unsigned long long* partial,
+                                cudaStream_t st);
+
 // ---- K6/K8: build-side kernels ------------------------------------------------------------
 // centroids[c] = (sum of x[perm[off[c]..off[c+1])] in that order) * (1/count); empty => zeros
 cudaError_t launch_segment_mean(const float* x, int64_t ldx, int d, const int32_t* perm, const int32_t* off, int k,

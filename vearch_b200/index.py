@@ -43,7 +43,8 @@ class GammaIndex:
     """One vector field's raw store + index model on one GPU."""
 
     def __init__(self, index_type, d, params=None, device=0):
-        self.index_type = index_type.upper()
+        t = index_type.upper()
+        self.index_type = "IVFPQFastScan" if t == "IVFPQFASTSCAN" else t  # gamma's spelling of the registered name
         self.d = int(d)
         self.device = device
         pj = json.dumps(params or {}).encode()
@@ -218,14 +219,19 @@ class GammaIndex:
     def pq_m(self):
         return int(_lib.lib().gb_index_pq_m(self._h))
 
+    @property
+    def pq_ksub(self):
+        """Centroids per sub-quantiser: 256 (IVFPQ), 16 (IVFPQFastScan)."""
+        return int(_lib.lib().gb_index_pq_ksub(self._h))
+
     def set_pq_centroids(self, pq):
         pq = _f32(pq)
-        assert pq.shape == (self.pq_m, 256, self.d // self.pq_m)
+        assert pq.shape == (self.pq_m, self.pq_ksub, self.d // self.pq_m)
         _check(_lib.lib().gb_index_set_pq_centroids(self._h, _ptr(pq)), "set_pq_centroids")
 
     def get_pq_centroids(self):
         m = self.pq_m
-        out = np.empty((m, 256, self.d // m), np.float32)
+        out = np.empty((m, self.pq_ksub, self.d // m), np.float32)
         _check(_lib.lib().gb_index_get_pq_centroids(self._h, _ptr(out)), "get_pq_centroids")
         return out
 
@@ -327,12 +333,24 @@ class GammaIndex:
         _check(rc, "search_preassigned")
         return dis, ids
 
-    def pq_encode(self, x, assign):
+    def pq_encode(self, x, assign=None):
+        """IVFPQ: codes of the residuals w.r.t. the assigned lists.  IVFPQFastScan: packed 4-bit codes of the raw
+        vectors (no assign), ceil(M/2) bytes each, sub-quantiser 2j in the low nibble of byte j."""
         x = _f32(x)
-        assign = np.ascontiguousarray(assign, np.int64)
-        codes = np.empty((x.shape[0], self.pq_m), np.uint8)
+        assign = None if assign is None else np.ascontiguousarray(assign, np.int64)
+        codes = np.empty((x.shape[0], self.code_size), np.uint8)
         _check(_lib.lib().gb_index_pq_encode(self._h, x.shape[0], _ptr(x), _ptr(assign), _ptr(codes)), "pq_encode")
         return codes
+
+    def pqfs_lut(self, x, metric=-1):
+        """IVFPQFastScan: the uint8 tables [nq, M, 16] of a query batch and (a, b) [nq, 2]; an entry scores
+        accu * (1 / a) + b, accu the sum of its M table entries."""
+        x = _f32(x)
+        nq = x.shape[0]
+        lut = np.empty((nq, self.pq_m, 16), np.uint8)
+        ab = np.empty((nq, 2), np.float32)
+        _check(_lib.lib().gb_index_pqfs_lut(self._h, nq, _ptr(x), metric, _ptr(lut), _ptr(ab)), "pqfs_lut")
+        return lut, ab
 
 
 def index_factory(d, description, metric=METRIC_L2, device=0, **extra):
