@@ -38,7 +38,7 @@ def shared_state_index(db, d, M, nlist, metric, seed=0):
 
 
 @pytest.mark.parametrize("metric", [L2, IP])
-@pytest.mark.parametrize("d,M", [(128, 64), (128, 32), (64, 16), (30, 15), (24, 12)])
+@pytest.mark.parametrize("d,M", [(128, 64), (128, 32), (64, 16), (32, 8), (30, 15), (24, 12)])
 @pytest.mark.parametrize("data", ["int", "float"])
 def test_shared_state_bit_exact(metric, d, M, data):
     n, nq, nlist = 20000, 40, 64

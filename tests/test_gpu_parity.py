@@ -428,7 +428,8 @@ def test_ivfpq_train_on_device_recall():
 
 @pytest.mark.parametrize("metric", [L2, IP])
 @pytest.mark.parametrize("d,M,data", [(128, 16, "float"), (128, 16, "int"), (64, 8, "float"), (64, 16, "float"),
-                                      (128, 8, "float"), (32, 4, "float"), (96, 12, "float")])
+                                      (128, 8, "float"), (32, 4, "float"), (96, 12, "float"), (128, 32, "float"),
+                                      (128, 64, "float")])
 def test_ivfpq_listmajor_tensor_core_filter_matches_oracle(metric, d, M, data):
     """Many queries per list => the IVF-PQ scan runs list-major (kernels_pqtc.cu): exact LUT scan of the
     first probes -> per-query bound -> fp16 wgmma FILTER over the other probes -> candidates re-scored
@@ -464,7 +465,7 @@ def test_ivfpq_listmajor_tensor_core_filter_matches_oracle(metric, d, M, data):
     ids2[0] |= orc.DEL_MASK
     for kk, kw in [(10, {}), (400, {}), (10, {"del_bitmap": delb}), (100, {"del_bitmap": delb})]:
         dg, ig = idx.search_preassigned(xq, kk, keys, cd, **kw)
-        # shapes outside the filter's list (M = 12) take the LUT kernel for every probe; same answers either way
+        # shapes outside the filter's list (M = 12, 32, 64) take the LUT kernel for every probe; same answers either way
         assert idx.last_scan_kernel == ("pqtc_scan_kernel" if M in (4, 8, 16) else "ivfpq_scan_kernel")
         do, io = orc.ivfpq_search_preassigned(off, codes, ids2, cent, pqc, T, xq, kk, keys, cd, metric, **kw)
         assert_same_results(dg, ig, do, io)

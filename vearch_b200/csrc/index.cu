@@ -2115,64 +2115,81 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   return 0;
 }
 
+// Metric check, ADC depth, query-major list scan + merge of its CTA groups, exact re-rank
+int IVFFlatIndex::scan_pq_dev(const char* type, const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric,
+                              int nq, const float* rerank_xq, int k, int nprobe, unsigned long long* out_keys, Scratch& s,
+                              const std::function<int(int, unsigned long long*, bool)>& prepare,
+                              const std::function<cudaError_t(int, int, unsigned long long*)>& launch) {
+  cudaStream_t st = s.stream();
+  if (metric != mp_.metric) {
+    set_last_error(std::string(type) + ": per-request metric must equal the trained metric");
+    return -1;
+  }
+  // recall_num / re-rank semantics: gamma_index_ivfpq.cc:764-770
+  const bool rerank = ctx.params.recall_num > 0;
+  const int kk = std::max(k, ctx.params.recall_num);
+  if (kk > 4096) {
+    set_last_error(std::string(type) + ": recall_num / topn above 4096 is not supported");
+    return -1;
+  }
+  unsigned long long* keys = out_keys;
+  if (rerank) {
+    keys = s.alloc_n<unsigned long long>((size_t)nq * kk);
+    if (!keys) return -1;
+  }
+  // the exact re-rank takes its candidates in any order; without it the keys are the result and must be sorted
+  const int rc = prepare(kk, keys, !rerank);
+  if (rc < 0) return -1;
+  if (rc == 1) {
+    const int nsm = sm_count(device_);
+    const int pg = (int)std::min<int64_t>(32, std::max<int64_t>(1, (int64_t)nprobe * nq / ((int64_t)nsm * 32)));
+    const int ngroups = (nprobe + pg - 1) / pg;
+    GB_ALLOC(partial, unsigned long long, (size_t)nq * ngroups * kk, s);
+    last_scan_kernel_ = kernel;
+    snprintf(last_scan_info_, sizeof(last_scan_info_), "{\"probes_per_cta\": %d}", pg);
+    scan_timer_begin(st);
+    stage_begin(kernel, st);
+    GB_CUDA(launch(kk, pg, partial));
+    stage_end(st);
+    scan_timer_end(st);
+    if (ngroups > 1) {
+      GB_CUDA(launch_select_keys(partial, (int64_t)ngroups * kk, nq, ngroups * kk, kk, keys, kk, st));
+    } else {
+      GB_CUDA(cudaMemcpyAsync(keys, partial, (size_t)nq * kk * 8, cudaMemcpyDeviceToDevice, st));
+    }
+  }
+  if (rerank) {
+    StageScope stage(this, "rerank_kernel", st);
+    GB_CUDA(launch_rerank(keys, kk, nq, rerank_xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_, k, metric, f,
+                          out_keys, st));
+  }
+  return 0;
+}
+
 // GammaIVFPQIndex::search_preassigned (gamma_index_ivfpq.cc:730-947)
 int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
                          const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
                          Scratch& s) {
   cudaStream_t st = s.stream();
-  if (metric != mp_.metric) {
-    set_last_error("IVFPQ: per-request metric must equal the trained metric");
-    return -1;
-  }
-  // recall_num / re-rank semantics: gamma_index_ivfpq.cc:764-770
-  const bool rerank = ctx.params.recall_num > 0;
-  int kk = k;
-  if (ctx.params.recall_num > k) kk = ctx.params.recall_num;
-  if (kk > 4096) {
-    set_last_error("IVFPQ: recall_num / topn above 4096 is not supported");
-    return -1;
-  }
-  GB_ALLOC(ip, float, (size_t)nq * M_ * 256, s);
-  {
-    StageScope stage(this, "pq_ip_table", st);
-    GB_CUDA(launch_pq_ip_table(xq, dpad_, nq, d_pq_, M_, dsub_, ip, st));
-  }
-  unsigned long long* adc = out_keys;
-  if (rerank) {
-    adc = s.alloc_n<unsigned long long>((size_t)nq * kk);
-    if (!adc) return -1;
-  }
-  // the exact re-rank takes its candidates in any order; without it the ADC keys are the result and must be sorted
-  int lm = scan_listmajor_pq(f, metric, nq, xq, kk, ip, probe_ids, coarse_dis, nprobe, adc, !rerank, s);
-  if (lm < 0) return -1;
-  if (lm == 0) {
-    last_scan_kernel_ = "pqtc_scan_kernel";
-  } else {
-    snprintf(last_scan_info_, sizeof(last_scan_info_), "{}");
-    const int nsm = sm_count(device_);
-    int pg = (int)std::min<int64_t>(32, std::max<int64_t>(1, (int64_t)nprobe * nq / ((int64_t)nsm * 32)));
-    int ngroups = (nprobe + pg - 1) / pg;
-    GB_ALLOC(partial, unsigned long long, (size_t)nq * ngroups * kk, s);
-    last_scan_kernel_ = "ivfpq_scan_kernel";
-    scan_timer_begin(st);
-    stage_begin("ivfpq_scan_kernel", st);
-    GB_CUDA(launch_ivfpq_scan(ip, nq, probe_ids, coarse_dis, nprobe, pg, lists_->directory(), M_, d_table_, kk, metric, f,
-                              partial, st));
-    stage_end(st);
-    scan_timer_end(st);
-    if (ngroups > 1) {
-      GB_CUDA(launch_select_keys(partial, (int64_t)ngroups * kk, nq, ngroups * kk, kk, adc, kk, st));
-    } else {
-      GB_CUDA(cudaMemcpyAsync(adc, partial, (size_t)nq * kk * 8, cudaMemcpyDeviceToDevice, st));
+  float* ip = nullptr;
+  auto prepare = [&](int kk, unsigned long long* keys, bool need_sorted) {
+    ip = s.alloc_n<float>((size_t)nq * M_ * 256);
+    if (!ip) return -1;
+    {
+      StageScope stage(this, "pq_ip_table", st);
+      GB_CUDA(launch_pq_ip_table(xq, dpad_, nq, d_pq_, M_, dsub_, ip, st));
     }
-  }
-  if (rerank) {
-    // "for opq, rerank need raw vector" (gamma_index_ivfpq.cc:735): original queries against the raw store
-    StageScope stage(this, "rerank_kernel", st);
-    GB_CUDA(launch_rerank(adc, kk, nq, raw_queries_for(xq), dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_, k,
-                          metric, f, out_keys, st));
-  }
-  return 0;
+    const int lm = scan_listmajor_pq(f, metric, nq, xq, kk, ip, probe_ids, coarse_dis, nprobe, keys, need_sorted, s);
+    if (lm == 0) last_scan_kernel_ = "pqtc_scan_kernel";
+    return lm;
+  };
+  auto launch = [&](int kk, int pg, unsigned long long* partial) {
+    return launch_ivfpq_scan(ip, nq, probe_ids, coarse_dis, nprobe, pg, lists_->directory(), M_, d_table_, kk, metric, f,
+                             partial, st);
+  };
+  // "for opq, rerank need raw vector" (gamma_index_ivfpq.cc:735): original queries against the raw store
+  return scan_pq_dev("IVFPQ", "ivfpq_scan_kernel", ctx, f, metric, nq, raw_queries_for(xq), k, nprobe, out_keys, s, prepare,
+                     launch);
 }
 
 int IVFPQIndex::search_preassigned_host(const SearchContext& ctx, int nq, const float* x, int k, const int64_t* keys,
@@ -2300,50 +2317,20 @@ int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, 
                                  Scratch& s) {
   (void)coarse_dis;  // no residual: the list's coarse distance takes no part in the score
   cudaStream_t st = s.stream();
-  if (metric != mp_.metric) {
-    set_last_error("IVFPQFastScan: per-request metric must equal the trained metric");
-    return -1;
-  }
-  const bool rerank = ctx.params.recall_num > 0;
-  int kk = k;
-  if (ctx.params.recall_num > k) kk = ctx.params.recall_num;
-  if (kk > 4096) {
-    set_last_error("IVFPQFastScan: recall_num / topn above 4096 is not supported");
-    return -1;
-  }
-  GB_ALLOC(lut, uint8_t, (size_t)nq * M_ * kKsub, s);
-  GB_ALLOC(ab, float, (size_t)nq * 2, s);
-  {
+  uint8_t* lut = nullptr;
+  float* ab = nullptr;
+  auto prepare = [&](int, unsigned long long*, bool) {
+    lut = s.alloc_n<uint8_t>((size_t)nq * M_ * kKsub);
+    ab = s.alloc_n<float>((size_t)nq * 2);
+    if (!lut || !ab) return -1;
     StageScope stage(this, "pqfs_lut_kernel", st);
     GB_CUDA(launch_pqfs_lut(xq, dpad_, nq, d_pq_, M_, dsub_, metric, lut, ab, st));
-  }
-  unsigned long long* fs = out_keys;
-  if (rerank) {
-    fs = s.alloc_n<unsigned long long>((size_t)nq * kk);
-    if (!fs) return -1;
-  }
-  const int nsm = sm_count(device_);
-  const int pg = (int)std::min<int64_t>(32, std::max<int64_t>(1, (int64_t)nprobe * nq / ((int64_t)nsm * 32)));
-  const int ngroups = (nprobe + pg - 1) / pg;
-  GB_ALLOC(partial, unsigned long long, (size_t)nq * ngroups * kk, s);
-  last_scan_kernel_ = "ivfpqfs_scan_kernel";
-  snprintf(last_scan_info_, sizeof(last_scan_info_), "{\"probes_per_cta\": %d}", pg);
-  scan_timer_begin(st);
-  stage_begin("ivfpqfs_scan_kernel", st);
-  GB_CUDA(launch_ivfpqfs_scan(lut, ab, nq, probe_ids, nprobe, pg, lists_->directory(), M_, kk, metric, f, partial, st));
-  stage_end(st);
-  scan_timer_end(st);
-  if (ngroups > 1) {
-    GB_CUDA(launch_select_keys(partial, (int64_t)ngroups * kk, nq, ngroups * kk, kk, fs, kk, st));
-  } else {
-    GB_CUDA(cudaMemcpyAsync(fs, partial, (size_t)nq * kk * 8, cudaMemcpyDeviceToDevice, st));
-  }
-  if (rerank) {
-    StageScope stage(this, "rerank_kernel", st);
-    GB_CUDA(launch_rerank(fs, kk, nq, xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_, k, metric, f, out_keys,
-                          st));
-  }
-  return 0;
+    return 1;
+  };
+  auto launch = [&](int kk, int pg, unsigned long long* partial) {
+    return launch_ivfpqfs_scan(lut, ab, nq, probe_ids, nprobe, pg, lists_->directory(), M_, kk, metric, f, partial, st);
+  };
+  return scan_pq_dev("IVFPQFastScan", "ivfpqfs_scan_kernel", ctx, f, metric, nq, xq, k, nprobe, out_keys, s, prepare, launch);
 }
 
 // ------------------------------------------------------------------------------------------

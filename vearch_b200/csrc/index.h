@@ -10,6 +10,7 @@
 #include <stdint.h>
 
 #include <condition_variable>
+#include <functional>
 #include <memory>
 #include <atomic>
 #include <mutex>
@@ -369,6 +370,13 @@ class IVFFlatIndex : public Index {
   virtual int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
                        const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
                        Scratch& s);
+  // scan_dev of the PQ-coded indexes (IVFPQ, IVFPQFastScan) through the query-major list scan: `prepare(kk, keys,
+  // need_sorted)` builds the per-query tables and may serve the scan another way (0 = served, 1 = not, < 0 = error);
+  // `launch(kk, pg, partial)` launches the scan kernel, named `kernel`, over pg probes per CTA
+  int scan_pq_dev(const char* type, const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric, int nq,
+                  const float* rerank_xq, int k, int nprobe, unsigned long long* out_keys, Scratch& s,
+                  const std::function<int(int, unsigned long long*, bool)>& prepare,
+                  const std::function<cudaError_t(int, int, unsigned long long*)>& launch);
   // list-major IVF-Flat scan on the tensor cores (kernels_tc.cu); returns 1 if not applicable
   int scan_listmajor_dev(const FilterArgs& f, int metric, int nq, const float* xq, int k, const int32_t* probe_ids,
                          int nprobe, unsigned long long* out_keys, Scratch& s);

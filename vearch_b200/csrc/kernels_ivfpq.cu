@@ -20,6 +20,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "list_scan.cuh"
 
 namespace gb {
 
@@ -73,11 +74,7 @@ __global__ void __launch_bounds__(KSUB)
   }
 }
 
-// ---------------- ADC scan ------------------------------------------------------------------
-constexpr int PQ_NT = 256;
-constexpr int PQ_NST = 2;
-constexpr int PQ_MAX_PG = 32;  // probes per CTA
-
+// ---------------- ADC scan: the IVF-PQ codec of the list scan (list_scan.cuh) -------------------
 // entries per thread per tile for the vector-load code layouts (MW = M / 4 code words per entry): per-tile
 // bookkeeping (barrier, tau reload, fill estimate, refill) is paid once per PT entries, while LUT + queue +
 // two code stages must stay within ~52 KiB so that four CTAs share an SM (M = 16: 2 x 256 entries, 8 KiB;
@@ -85,240 +82,63 @@ constexpr int PQ_MAX_PG = 32;  // probes per CTA
 __host__ __device__ constexpr int pq_pt(int MW) { return MW == 2 ? 4 : (MW == 4 ? 2 : (MW == 8 ? 2 : 1)); }
 
 __host__ __device__ inline int pq_tile_entries(int M) {
-  if (M == 8 || M == 16 || M == 32 || M == 64) return pq_pt(M / 4) * PQ_NT;
+  if (M == 8 || M == 16 || M == 32 || M == 64) return pq_pt(M / 4) * LS_NT;
   int e = 16384 / M;
-  e = (e / PQ_NT) * PQ_NT;
-  if (e < PQ_NT) e = PQ_NT;
+  e = (e / LS_NT) * LS_NT;
+  if (e < LS_NT) e = LS_NT;
   if (e > 1024) e = 1024;
   return e;
 }
 
-template <int MW>
-__device__ __forceinline__ float adc_distance(const unsigned char* __restrict__ code, const float* __restrict__ lut,
-                                              float dis0, int M) {
-  float dis = dis0;
-  if (MW > 0) {
-    uint32_t w[MW > 0 ? MW : 1];
-    if (MW % 4 == 0) {
-#pragma unroll
-      for (int i = 0; i < MW / 4; i++) {
-        uint4 v = reinterpret_cast<const uint4*>(code)[i];
-        w[4 * i] = v.x, w[4 * i + 1] = v.y, w[4 * i + 2] = v.z, w[4 * i + 3] = v.w;
-      }
-    } else if (MW % 2 == 0) {
-#pragma unroll
-      for (int i = 0; i < MW / 2; i++) {
-        uint2 v = reinterpret_cast<const uint2*>(code)[i];
-        w[2 * i] = v.x, w[2 * i + 1] = v.y;
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < MW; i++) w[i] = reinterpret_cast<const uint32_t*>(code)[i];
+// Per list the CTA builds the LUT  T[list] + (-2) ip  (precompute_list_tables); under IP the per-query inner-product
+// table (L2-resident) IS the LUT and is copied once.  dis = dis0; dis += lut[m][code[m]] for m = 0..M-1.
+struct IvfpqCodec {
+  using Entry = float;
+  static constexpr bool kDis0 = true;
+  static constexpr int kMinCtasPerSm = 0;  // shared memory, not registers, sets its CTAs per SM
+  const float* ip_table;  // [nq][M][256]
+  const float* T;         // [nlist][M][256], L2 only
+  int M;
+  const float4* ipq4;  // this CTA's query in ip_table
+
+  __host__ __device__ int code_bytes() const { return M; }
+  int tile_entries() const { return pq_tile_entries(M); }
+  __host__ __device__ static constexpr int pt(int MW) { return pq_pt(MW); }
+
+  __device__ __forceinline__ void cta_begin(float* lut, int q, int metric) {
+    ipq4 = reinterpret_cast<const float4*>(ip_table + (int64_t)q * M * KSUB);
+    if (metric != kMetricL2) {
+      float4* dst = reinterpret_cast<float4*>(lut);
+      for (int i = threadIdx.x; i < M * KSUB / 4; i += LS_NT) dst[i] = __ldg(ipq4 + i);
+      __syncthreads();
     }
-#pragma unroll
-    for (int i = 0; i < MW; i++) {
-      uint32_t x = w[i];
-      dis += lut[(4 * i + 0) * KSUB + (x & 0xffu)];
-      dis += lut[(4 * i + 1) * KSUB + ((x >> 8) & 0xffu)];
-      dis += lut[(4 * i + 2) * KSUB + ((x >> 16) & 0xffu)];
-      dis += lut[(4 * i + 3) * KSUB + (x >> 24)];
-    }
-  } else {
-    for (int m = 0; m < M; m++) dis += lut[m * KSUB + code[m]];
   }
-  return dis;
-}
-
-template <int METRIC, int MW>
-__global__ void __launch_bounds__(PQ_NT)
-    ivfpq_scan_kernel(const float* __restrict__ ip_table, const int32_t* __restrict__ probe_ids,
-                      const float* __restrict__ coarse_dis, int nprobe, int ld_probe, int pg, ListDirectory dir, int M,
-                      const float* __restrict__ T, int tile_e, int k, int KP, int SORTN, FilterArgs f,
-                      const int* __restrict__ gate_cnt, int gate_cap, const int* __restrict__ row_limit, int sorted_out,
-                      unsigned long long* __restrict__ partial) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  const int tile_bytes = tile_e * M;
-  // the LUT sits at the start of the dynamic window: its shared address is a link-time constant, so
-  // every gather is  LDS [byte_offset + imm]  with no base add
-  float* lut = reinterpret_cast<float*>(smem_raw);
-  unsigned long long* buf = reinterpret_cast<unsigned long long*>(lut + M * KSUB);
-  unsigned char* stages = reinterpret_cast<unsigned char*>(buf + SORTN);
-  __shared__ __align__(8) uint64_t full_bar[PQ_NST];
-  __shared__ int s_cnt;
-  __shared__ unsigned long long s_tau;
-  __shared__ int g_list[PQ_MAX_PG], g_len[PQ_MAX_PG], g_tile0[PQ_MAX_PG + 1];
-  __shared__ float g_dis0[PQ_MAX_PG];
-
-  const int tid = threadIdx.x;
-  const int q = blockIdx.y, grp = blockIdx.x;
-  // flag-gated launch (fallback of the tensor-core filter, kernels_pqtc.cu): only queries whose
-  // candidate list overflowed are scanned
-  if (gate_cnt && gate_cnt[q] <= gate_cap) return;
-  unsigned long long* out = partial + ((int64_t)q * gridDim.x + grp) * k;
-  const int p0 = grp * pg;
-  const int np = min(pg, nprobe - p0);
-
-  if (tid == 0) {
-    int acc = 0;
-    for (int i = 0; i < np; i++) {
-      int l = probe_ids[(int64_t)q * ld_probe + p0 + i];
-      int len = (l >= 0 && l < dir.nlist) ? dir.len[l] : 0;  // key < 0: "not enough centroids" (ivfpq.cc:640)
-      // phase A of the tensor-core filter scans only a prefix of its lists (kernels_pqtc.cu)
-      if (row_limit) len = min(len, row_limit[(int64_t)q * ld_probe + p0 + i]);
-      g_list[i] = l;
-      g_len[i] = len;
-      g_dis0[i] = coarse_dis[(int64_t)q * ld_probe + p0 + i];
-      g_tile0[i] = acc;
-      acc += (len + tile_e - 1) / tile_e;
-    }
-    g_tile0[np > 0 ? np : 0] = acc;
-    for (int s = 0; s < PQ_NST; s++) mbar_init(&full_bar[s], 1);
-    mbar_fence_init();
-  }
-  CandQueue cq{buf, &s_cnt, &s_tau, k, KP, SORTN};
-  cq.init();  // __syncthreads inside: g_* and barriers visible
-  const int total_tiles = np > 0 ? g_tile0[np] : 0;
-  if (total_tiles == 0) {
-    for (int i = tid; i < k; i += PQ_NT) out[i] = kKeySentinel;
-    return;
-  }
-
-  // per-query inner-product table (L2-resident): IP => it IS the LUT (dis0 = <x, centroid>);
-  // L2 => combined with the list's precomputed row when a new list starts
-  const float4* ipq4 = reinterpret_cast<const float4*>(ip_table + (int64_t)q * M * KSUB);
-  if (METRIC != kMetricL2) {
-    float4* dst = reinterpret_cast<float4*>(lut);
-    for (int i = tid; i < M * KSUB / 4; i += PQ_NT) dst[i] = __ldg(ipq4 + i);
-  }
-
-  // producer cursor (thread 0 only)
-  int pr_pi = 0;
-  auto issue = [&](int gt) {
-    while (gt >= g_tile0[pr_pi + 1]) pr_pi++;
-    int ti = gt - g_tile0[pr_pi];
-    int n_e = min(tile_e, g_len[pr_pi] - ti * tile_e);
-    uint32_t bytes = ((uint32_t)n_e * M + 15u) & ~15u;
-    int s = gt % PQ_NST;
-    mbar_arrive_expect_tx(&full_bar[s], bytes);
-    bulk_g2s(stages + (size_t)s * tile_bytes, dir.codes[g_list[pr_pi]] + (int64_t)ti * tile_e * M, bytes,
-             &full_bar[s]);
-  };
-  if (tid == 0)
-    for (int gt = 0; gt < PQ_NST && gt < total_tiles; gt++) issue(gt);
-
-  int pi = -1;  // consumer cursor
-  float dis0 = 0.f;
-  const int64_t* __restrict__ lids = nullptr;
-  // entries per thread per tile: compile-time for the vector-load code layouts (gives the
-  // compiler PT independent ADC chains to interleave), runtime for the generic layout
-  constexpr int PT = pq_pt(MW);
-  const int per_thread = MW > 0 ? PT : tile_e / PQ_NT;
-  int est = 0;  // upper bound of the queue fill, identical in every thread
-
-  for (int gt = 0; gt < total_tiles; gt++) {
-    int npi = pi < 0 ? 0 : pi;
-    while (gt >= g_tile0[npi + 1]) npi++;
-    if (npi != pi) {  // first tile of a new list: build its LUT (precompute_list_tables)
-      pi = npi;
-      dis0 = g_dis0[pi];
-      lids = dir.ids[g_list[pi]];
-      if (METRIC == kMetricL2) {
-        const float4* Tl = reinterpret_cast<const float4*>(T + (int64_t)g_list[pi] * M * KSUB);
-        float4* lut4 = reinterpret_cast<float4*>(lut);
-        for (int i = tid; i < M * KSUB / 4; i += PQ_NT) {
-          float4 t = __ldg(Tl + i), a = __ldg(ipq4 + i);
-          lut4[i] = make_float4(fmaf(-2.0f, a.x, t.x), fmaf(-2.0f, a.y, t.y), fmaf(-2.0f, a.z, t.z),
-                                fmaf(-2.0f, a.w, t.w));
-        }
+  __device__ __forceinline__ void list_begin(float* lut, int list, int metric) const {
+    if (metric == kMetricL2) {
+      const float4* Tl = reinterpret_cast<const float4*>(T + (int64_t)list * M * KSUB);
+      float4* lut4 = reinterpret_cast<float4*>(lut);
+      for (int i = threadIdx.x; i < M * KSUB / 4; i += LS_NT) {
+        float4 t = __ldg(Tl + i), a = __ldg(ipq4 + i);
+        lut4[i] = make_float4(fmaf(-2.0f, a.x, t.x), fmaf(-2.0f, a.y, t.y), fmaf(-2.0f, a.z, t.z),
+                              fmaf(-2.0f, a.w, t.w));
       }
       __syncthreads();
     }
-    const int ti = gt - g_tile0[pi];
-    const int n_e = min(tile_e, g_len[pi] - ti * tile_e);
-    const int s = gt % PQ_NST;
-    mbar_wait(&full_bar[s], (gt / PQ_NST) & 1);
-    const unsigned long long tau = s_tau;
-    // score window and the queue's bound folded into one float interval: two compares per entry, the
-    // order-preserving key is only built for entries inside it
-    const float tb = key_bound<METRIC>(tau);
-    const float lo_b = METRIC == kMetricL2 ? f.min_score : fmaxf(tb, f.min_score);
-    const float hi_b = METRIC == kMetricL2 ? fminf(tb, f.max_score) : f.max_score;
-    const unsigned char* st = stages + (size_t)s * tile_bytes;
-    int pushed = 0;
+  }
+  using Acc = float;
+  __device__ __forceinline__ float start(float dis0) const { return dis0; }
+  __device__ __forceinline__ float finish(float dis) const { return dis; }
+};
 
-    auto consider = [&](int e, float dis) {
-      bool pred = e < n_e && dis <= hi_b && dis >= lo_b;
-      unsigned long long key = kKeySentinel;
-      if (pred) {
-        int64_t raw = lids[(int64_t)ti * tile_e + e];
-        pred = raw >= 0;  // tombstone (gamma_index_ivfpq.h:930)
-        uint32_t vid = (uint32_t)raw;
-        if (pred) pred = ctx_is_valid(f.del_bits, f.filter_bits, vid);
-        key = make_key(score2ord<METRIC>(dis), vid);
-        pred = pred && key < tau;
-      }
-      cq.push_warp(pred, key);
-      pushed |= pred ? 1 : 0;
-    };
-    if (MW > 0) {
-      float dis[PT];
-#pragma unroll
-      for (int u = 0; u < PT; u++) {
-        const int e = u * PQ_NT + tid;
-        // entries past n_e read stale-but-in-bounds stage bytes; they are masked in consider()
-        dis[u] = adc_distance<MW>(st + (size_t)e * M, lut, dis0, M);
-      }
-#pragma unroll
-      for (int u = 0; u < PT; u++) consider(u * PQ_NT + tid, dis[u]);
-    } else {
-      for (int u = 0; u < per_thread; u++) {
-        const int e = u * PQ_NT + tid;
-        float dis = e < n_e ? adc_distance<MW>(st + (size_t)e * M, lut, dis0, M) : 0.f;
-        consider(e, dis);
-      }
-    }
-    // stage consumed + pushes done; the count is identical in every thread (no 2nd barrier needed)
-    est += __syncthreads_count(pushed) * per_thread;
-    if (tid == 0 && gt + PQ_NST < total_tiles) issue(gt + PQ_NST);
-    if (gt + 1 < total_tiles && est + tile_e > cq.cap()) {
-      cq.flush();
-      est = 0;
-    }
+template <int METRIC>
+cudaError_t launch_scan_m(const IvfpqCodec& c, int nq, const ListScanArgs& a, cudaStream_t st) {
+  switch (c.M) {
+    case 8: return launch_list_scan<IvfpqCodec, METRIC, 2>(c, nq, a, st);
+    case 16: return launch_list_scan<IvfpqCodec, METRIC, 4>(c, nq, a, st);
+    case 32: return launch_list_scan<IvfpqCodec, METRIC, 8>(c, nq, a, st);
+    case 64: return launch_list_scan<IvfpqCodec, METRIC, 16>(c, nq, a, st);
+    default: return launch_list_scan<IvfpqCodec, METRIC, 0>(c, nq, a, st);
   }
-  __syncthreads();
-  if (sorted_out) {
-    cq.flush(true);
-  } else {
-    // The caller wants the k best and their bound, not their order (phase A of the tensor-core filter): exact radix
-    // select, no sort; the largest key -- the sentinel when fewer than k entries qualified -- goes to slot k - 1.
-    cq.flush(false, true);
-    __shared__ unsigned long long s_wmax[PQ_NT / 32];
-    __shared__ int s_wpos[PQ_NT / 32];
-    unsigned long long mx = 0;
-    int pos = -1;
-    for (int i = tid; i < k; i += PQ_NT) {
-      const unsigned long long v = buf[i];
-      if (pos < 0 || v > mx) mx = v, pos = i;
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      const unsigned long long om = __shfl_xor_sync(0xffffffffu, mx, off);
-      const int op = __shfl_xor_sync(0xffffffffu, pos, off);
-      if (op >= 0 && (pos < 0 || om > mx || (om == mx && op > pos))) mx = om, pos = op;
-    }
-    if ((tid & 31) == 0) s_wmax[tid >> 5] = mx, s_wpos[tid >> 5] = pos;
-    __syncthreads();
-    if (tid == 0) {
-      for (int w = 1; w < PQ_NT / 32; w++)
-        if (s_wpos[w] >= 0 && (pos < 0 || s_wmax[w] > mx || (s_wmax[w] == mx && s_wpos[w] > pos))) mx = s_wmax[w], pos = s_wpos[w];
-      if (pos >= 0 && pos != k - 1) {
-        buf[pos] = buf[k - 1];
-        buf[k - 1] = mx;
-      }
-    }
-    __syncthreads();
-  }
-  for (int i = tid; i < k; i += PQ_NT) out[i] = buf[i];
 }
 
 // ---------------- exact re-rank -------------------------------------------------------------
@@ -425,50 +245,6 @@ __global__ void __launch_bounds__(ENC_NT)
   codes[i * M + m] = (uint8_t)bi;
 }
 
-void pq_cq_geometry(int k, int tile_e, int* KP, int* SORTN) {
-  *KP = next_pow2(k < 16 ? 16 : k);
-  *SORTN = next_pow2(*KP + tile_e + tile_e / 2);  // cap >= tile_e: one tile always fits after a flush
-}
-
-template <int METRIC, int MW>
-cudaError_t launch_scan_t(const float* ip_table, int nq, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
-                          int ld_probe, int pg, ListDirectory dir, int M, const float* T, int k, FilterArgs f,
-                          const int* gate_cnt, int gate_cap, const int* row_limit, int sorted_out, unsigned long long* partial,
-                          cudaStream_t st) {
-  int tile_e = pq_tile_entries(M);
-  int KP, SORTN;
-  pq_cq_geometry(k, tile_e, &KP, &SORTN);
-  size_t smem = (size_t)PQ_NST * tile_e * M + (size_t)M * KSUB * 4 + (size_t)SORTN * 8;
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;
-  cudaError_t e = cudaFuncSetAttribute(ivfpq_scan_kernel<METRIC, MW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)smem);
-  if (e != cudaSuccess) return e;
-  int ngroups = (nprobe + pg - 1) / pg;
-  dim3 grid(ngroups, nq);
-  ivfpq_scan_kernel<METRIC, MW><<<grid, PQ_NT, smem, st>>>(ip_table, probe_ids, coarse_dis, nprobe, ld_probe, pg, dir, M, T,
-                                                          tile_e, k, KP, SORTN, f, gate_cnt, gate_cap, row_limit, sorted_out, partial);
-                                                          note_launch();
-  return cudaGetLastError();
-}
-
-template <int METRIC>
-cudaError_t launch_scan_m(const float* ip_table, int nq, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
-                          int ld_probe, int pg, ListDirectory dir, int M, const float* T, int k, FilterArgs f,
-                          const int* gate_cnt, int gate_cap, const int* row_limit, int sorted_out, unsigned long long* partial,
-                          cudaStream_t st) {
-#define GB_SCAN(MW) \
-  return launch_scan_t<METRIC, MW>(ip_table, nq, probe_ids, coarse_dis, nprobe, ld_probe, pg, dir, M, T, k, f, gate_cnt, \
-                                   gate_cap, row_limit, sorted_out, partial, st)
-  switch (M) {
-    case 8: GB_SCAN(2);
-    case 16: GB_SCAN(4);
-    case 32: GB_SCAN(8);
-    case 64: GB_SCAN(16);
-    default: GB_SCAN(0);
-  }
-#undef GB_SCAN
-}
-
 }  // namespace
 
 cudaError_t launch_pq_ip_table(const float* xq, int64_t ldq, int nq, const float* pq_centroids, int M, int dsub,
@@ -497,14 +273,12 @@ cudaError_t launch_ivfpq_scan(const float* ip_table, int nq, const int32_t* prob
                               int nprobe, int pg, ListDirectory dir, int M, const float* T, int k, int metric,
                               FilterArgs f, unsigned long long* partial, cudaStream_t st, int ld_probe,
                               const int* gate_cnt, int gate_cap, const int* row_limit, bool sorted_out) {
-  if (nq <= 0 || nprobe <= 0) return cudaSuccess;
-  if (ld_probe <= 0) ld_probe = nprobe;
-  if (k <= 0 || k > 4096 || nq > 65535 || pg < 1 || pg > PQ_MAX_PG) return cudaErrorInvalidValue;
-  if (metric == kMetricL2) {
-    if (!T) return cudaErrorInvalidValue;
-    return launch_scan_m<kMetricL2>(ip_table, nq, probe_ids, coarse_dis, nprobe, ld_probe, pg, dir, M, T, k, f, gate_cnt, gate_cap, row_limit, sorted_out ? 1 : 0, partial, st);
-  }
-  return launch_scan_m<kMetricIP>(ip_table, nq, probe_ids, coarse_dis, nprobe, ld_probe, pg, dir, M, T, k, f, gate_cnt, gate_cap, row_limit, sorted_out ? 1 : 0, partial, st);
+  if (metric == kMetricL2 && !T) return cudaErrorInvalidValue;
+  const IvfpqCodec c{ip_table, T, M, nullptr};
+  const ListScanArgs a{probe_ids, coarse_dis, nprobe, ld_probe > 0 ? ld_probe : nprobe, pg, dir, k, f,
+                       gate_cnt, gate_cap, row_limit, sorted_out, partial};
+  if (metric == kMetricL2) return launch_scan_m<kMetricL2>(c, nq, a, st);
+  return launch_scan_m<kMetricIP>(c, nq, a, st);
 }
 
 cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq, const float* xq, int64_t ldq, int d,

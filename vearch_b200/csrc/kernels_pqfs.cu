@@ -14,6 +14,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "list_scan.cuh"
 
 namespace gb {
 
@@ -110,214 +111,59 @@ __global__ void __launch_bounds__(LUT_NT)
   }
 }
 
-// ---------------- scan ---------------------------------------------------------------------------------------
-constexpr int FS_NT = 256;
-constexpr int FS_NST = 2;
-constexpr int FS_MAX_PG = 32;  // probes per CTA
-
-// entries per tile: 16 KiB of codes, between 256 and 1024 entries (a multiple of FS_NT)
+// ---------------- scan: the IVFPQFastScan codec of the list scan (list_scan.cuh) ---------------------------
+// entries per tile: 16 KiB of codes, between 256 and 1024 entries (a multiple of LS_NT)
 __host__ __device__ constexpr int pqfs_tile_entries(int MB) {
-  const int e = 16384 / MB / FS_NT * FS_NT;
-  return e < FS_NT ? FS_NT : (e > 1024 ? 1024 : e);
+  const int e = 16384 / MB / LS_NT * LS_NT;
+  return e < LS_NT ? LS_NT : (e > 1024 ? 1024 : e);
 }
 
-// accu = sum_j T[j][code byte j].  uint16 pair entries summed in 32 bits: faiss sums 16-bit, which wraps only above
-// 257 sub-quantisers (255 * 257 < 2^16); the index accepts M <= 256 (IVFPQFastScanIndex::kMaxM), so both are equal.
-template <int MW>
-__device__ __forceinline__ uint32_t pqfs_accu(const unsigned char* __restrict__ code, const uint16_t* __restrict__ T, int MB) {
-  uint32_t accu = 0;
-  if (MW > 0) {
-    uint32_t w[MW > 0 ? MW : 1];
-    if (MW % 4 == 0) {
-#pragma unroll
-      for (int i = 0; i < MW / 4; i++) {
-        const uint4 v = reinterpret_cast<const uint4*>(code)[i];
-        w[4 * i] = v.x, w[4 * i + 1] = v.y, w[4 * i + 2] = v.z, w[4 * i + 3] = v.w;
-      }
-    } else if (MW % 2 == 0) {
-#pragma unroll
-      for (int i = 0; i < MW / 2; i++) {
-        const uint2 v = reinterpret_cast<const uint2*>(code)[i];
-        w[2 * i] = v.x, w[2 * i + 1] = v.y;
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < MW; i++) w[i] = reinterpret_cast<const uint32_t*>(code)[i];
+// The table does not depend on the list (no residual), so the CTA builds the byte-pair table
+// T[j][byte] = lut8[2j][lo] + lut8[2j+1][hi] once.  accu = sum_j T[j][code byte j]: uint16 pair entries summed in 32 bits;
+// faiss sums 16-bit, which wraps only above 257 sub-quantisers (255 * 257 < 2^16); the index accepts M <= 256
+// (IVFPQFastScanIndex::kMaxM), so both are equal.  Score accu * (1 / a) + b.
+struct IvfpqfsCodec {
+  using Entry = uint16_t;
+  static constexpr bool kDis0 = false;
+  // 40 registers: for M <= 12 shared memory admits 6 or 7 CTAs per SM
+  static constexpr int kMinCtasPerSm = 6;
+  const uint8_t* lut8;  // [nq][M][16]
+  const float* ab;      // [nq][2]
+  int M;
+  float one_a, b;  // this CTA's query
+
+  __host__ __device__ int code_bytes() const { return (M + 1) / 2; }
+  int tile_entries() const { return pqfs_tile_entries(code_bytes()); }
+  __host__ __device__ static constexpr int pt(int MW) { return pqfs_tile_entries(4 * MW) / LS_NT; }
+
+  __device__ __forceinline__ void cta_begin(uint16_t* T, int q, int metric) {
+    (void)metric;
+    const uint8_t* lq = lut8 + (int64_t)q * M * FS_KSUB;
+    for (int i = threadIdx.x; i < code_bytes() * 256; i += LS_NT) {
+      const int j = i >> 8, lo = i & 15, hi = (i >> 4) & 15;
+      T[i] = (uint16_t)(lq[2 * j * FS_KSUB + lo] + (2 * j + 1 < M ? lq[(2 * j + 1) * FS_KSUB + hi] : 0));
     }
-#pragma unroll
-    for (int i = 0; i < MW; i++) {
-      const uint32_t x = w[i];
-      accu += T[(4 * i + 0) * 256 + (x & 0xffu)];
-      accu += T[(4 * i + 1) * 256 + ((x >> 8) & 0xffu)];
-      accu += T[(4 * i + 2) * 256 + ((x >> 16) & 0xffu)];
-      accu += T[(4 * i + 3) * 256 + (x >> 24)];
-    }
-  } else {
-    for (int j = 0; j < MB; j++) accu += T[j * 256 + code[j]];
+    one_a = __fdiv_rn(1.f, ab[2 * q]);
+    b = ab[2 * q + 1];
+    __syncthreads();
   }
-  return accu;
-}
-
-// One CTA per (query, group of pg probes): a TMA bulk ring over the flat (list, tile) sequence of its probes.  The table
-// does not depend on the list (no residual), so the byte-pair table T[j][byte] = lut8[2j][lo] + lut8[2j+1][hi] is built
-// once per CTA.
-template <int METRIC, int MW>
-__global__ void __launch_bounds__(FS_NT)
-    ivfpqfs_scan_kernel(const uint8_t* __restrict__ lut8, const float* __restrict__ ab, const int32_t* __restrict__ probe_ids,
-                        int nprobe, int pg, ListDirectory dir, int M, int MB, int tile_e, int k, int KP, int SORTN, FilterArgs f,
-                        unsigned long long* __restrict__ partial) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  const int tile_bytes = tile_e * MB;
-  uint16_t* T = reinterpret_cast<uint16_t*>(smem_raw);  // [MB][256]
-  unsigned long long* buf = reinterpret_cast<unsigned long long*>(smem_raw + (size_t)MB * 512);
-  unsigned char* stages = reinterpret_cast<unsigned char*>(buf + SORTN);
-  __shared__ __align__(8) uint64_t full_bar[FS_NST];
-  __shared__ int s_cnt;
-  __shared__ unsigned long long s_tau;
-  __shared__ int g_list[FS_MAX_PG], g_len[FS_MAX_PG], g_tile0[FS_MAX_PG + 1];
-
-  const int tid = threadIdx.x;
-  const int q = blockIdx.y, grp = blockIdx.x;
-  unsigned long long* out = partial + ((int64_t)q * gridDim.x + grp) * k;
-  const int p0 = grp * pg;
-  const int np = min(pg, nprobe - p0);
-
-  if (tid == 0) {
-    int acc = 0;
-    for (int i = 0; i < np; i++) {
-      const int l = probe_ids[(int64_t)q * nprobe + p0 + i];
-      const int len = (l >= 0 && l < dir.nlist) ? dir.len[l] : 0;
-      g_list[i] = l;
-      g_len[i] = len;
-      g_tile0[i] = acc;
-      acc += (len + tile_e - 1) / tile_e;
-    }
-    g_tile0[np > 0 ? np : 0] = acc;
-    for (int s = 0; s < FS_NST; s++) mbar_init(&full_bar[s], 1);
-    mbar_fence_init();
+  __device__ __forceinline__ void list_begin(uint16_t* T, int list, int metric) const {
+    (void)T, (void)list, (void)metric;
   }
-  CandQueue cq{buf, &s_cnt, &s_tau, k, KP, SORTN};
-  cq.init();  // __syncthreads inside: g_* and barriers visible
-  const int total_tiles = np > 0 ? g_tile0[np] : 0;
-  if (total_tiles == 0) {
-    for (int i = tid; i < k; i += FS_NT) out[i] = kKeySentinel;
-    return;
-  }
-
-  int pr_pi = 0;  // producer cursor (thread 0 only)
-  auto issue = [&](int gt) {
-    while (gt >= g_tile0[pr_pi + 1]) pr_pi++;
-    const int ti = gt - g_tile0[pr_pi];
-    const int n_e = min(tile_e, g_len[pr_pi] - ti * tile_e);
-    const uint32_t bytes = ((uint32_t)n_e * MB + 15u) & ~15u;
-    const int s = gt % FS_NST;
-    mbar_arrive_expect_tx(&full_bar[s], bytes);
-    bulk_g2s(stages + (size_t)s * tile_bytes, dir.codes[g_list[pr_pi]] + (int64_t)ti * tile_e * MB, bytes, &full_bar[s]);
-  };
-  if (tid == 0)
-    for (int gt = 0; gt < FS_NST && gt < total_tiles; gt++) issue(gt);
-
-  const uint8_t* lq = lut8 + (int64_t)q * M * FS_KSUB;
-  for (int i = tid; i < MB * 256; i += FS_NT) {
-    const int j = i >> 8, lo = i & 15, hi = (i >> 4) & 15;
-    T[i] = (uint16_t)(lq[2 * j * FS_KSUB + lo] + (2 * j + 1 < M ? lq[(2 * j + 1) * FS_KSUB + hi] : 0));
-  }
-  const float one_a = __fdiv_rn(1.f, ab[2 * q]), b = ab[2 * q + 1];
-  __syncthreads();
-
-  int pi = -1;  // consumer cursor
-  const int64_t* __restrict__ lids = nullptr;
-  constexpr int PT = MW > 0 ? pqfs_tile_entries(4 * MW) / FS_NT : 1;
-  const int per_thread = MW > 0 ? PT : tile_e / FS_NT;
-  int est = 0;  // upper bound of the queue fill, identical in every thread
-
-  for (int gt = 0; gt < total_tiles; gt++) {
-    int npi = pi < 0 ? 0 : pi;
-    while (gt >= g_tile0[npi + 1]) npi++;
-    if (npi != pi) {
-      pi = npi;
-      lids = dir.ids[g_list[pi]];
-    }
-    const int ti = gt - g_tile0[pi];
-    const int n_e = min(tile_e, g_len[pi] - ti * tile_e);
-    const int s = gt % FS_NST;
-    mbar_wait(&full_bar[s], (gt / FS_NST) & 1);
-    const unsigned long long tau = s_tau;
-    const float tb = key_bound<METRIC>(tau);
-    const float lo_b = METRIC == kMetricL2 ? f.min_score : fmaxf(tb, f.min_score);
-    const float hi_b = METRIC == kMetricL2 ? fminf(tb, f.max_score) : f.max_score;
-    const unsigned char* st = stages + (size_t)s * tile_bytes;
-    int pushed = 0;
-
-    auto consider = [&](int e, float dis) {
-      bool pred = e < n_e && dis <= hi_b && dis >= lo_b;
-      unsigned long long key = kKeySentinel;
-      if (pred) {
-        const int64_t raw = lids[(int64_t)ti * tile_e + e];
-        pred = raw >= 0;  // tombstone
-        const uint32_t vid = (uint32_t)raw;
-        if (pred) pred = ctx_is_valid(f.del_bits, f.filter_bits, vid);
-        key = make_key(score2ord<METRIC>(dis), vid);
-        pred = pred && key < tau;
-      }
-      cq.push_warp(pred, key);
-      pushed |= pred ? 1 : 0;
-    };
-    auto score = [&](uint32_t accu) { return __fadd_rn(__fmul_rn((float)accu, one_a), b); };
-    if (MW > 0) {
-      uint32_t accu[PT];
-#pragma unroll
-      for (int u = 0; u < PT; u++) accu[u] = pqfs_accu<MW>(st + (size_t)(u * FS_NT + tid) * MB, T, MB);  // stale bytes past n_e are masked
-#pragma unroll
-      for (int u = 0; u < PT; u++) consider(u * FS_NT + tid, score(accu[u]));
-    } else {
-      for (int u = 0; u < per_thread; u++) {
-        const int e = u * FS_NT + tid;
-        consider(e, e < n_e ? score(pqfs_accu<0>(st + (size_t)e * MB, T, MB)) : 0.f);
-      }
-    }
-    est += __syncthreads_count(pushed) * per_thread;  // stage consumed + pushes done
-    if (tid == 0 && gt + FS_NST < total_tiles) issue(gt + FS_NST);
-    if (gt + 1 < total_tiles && est + tile_e > cq.cap()) {
-      cq.flush();
-      est = 0;
-    }
-  }
-  __syncthreads();
-  cq.flush(true);
-  for (int i = tid; i < k; i += FS_NT) out[i] = buf[i];
-}
-
-template <int METRIC, int MW>
-cudaError_t launch_scan_t(const uint8_t* lut8, const float* ab, int nq, const int32_t* probe_ids, int nprobe, int pg,
-                          ListDirectory dir, int M, int k, FilterArgs f, unsigned long long* partial, cudaStream_t st) {
-  const int MB = (M + 1) / 2;
-  const int tile_e = pqfs_tile_entries(MB);
-  const int KP = next_pow2(k < 16 ? 16 : k);
-  const int SORTN = next_pow2(KP + tile_e + tile_e / 2);  // cap >= tile_e: one tile always fits after a flush
-  const size_t smem = (size_t)MB * 512 + (size_t)SORTN * 8 + (size_t)FS_NST * tile_e * MB;
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;
-  cudaError_t e = cudaFuncSetAttribute(ivfpqfs_scan_kernel<METRIC, MW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  dim3 grid((nprobe + pg - 1) / pg, nq);
-  ivfpqfs_scan_kernel<METRIC, MW><<<grid, FS_NT, smem, st>>>(lut8, ab, probe_ids, nprobe, pg, dir, M, MB, tile_e, k, KP, SORTN,
-                                                             f, partial);
-  note_launch();
-  return cudaGetLastError();
-}
+  using Acc = uint32_t;
+  __device__ __forceinline__ uint32_t start(float dis0) const { (void)dis0; return 0u; }
+  __device__ __forceinline__ float finish(uint32_t accu) const { return __fadd_rn(__fmul_rn((float)accu, one_a), b); }
+};
 
 template <int METRIC>
-cudaError_t launch_scan_m(const uint8_t* lut8, const float* ab, int nq, const int32_t* probe_ids, int nprobe, int pg,
-                          ListDirectory dir, int M, int k, FilterArgs f, unsigned long long* partial, cudaStream_t st) {
-#define GB_FS(MW) return launch_scan_t<METRIC, MW>(lut8, ab, nq, probe_ids, nprobe, pg, dir, M, k, f, partial, st)
-  switch ((M + 1) / 2) {  // code bytes
-    case 4: GB_FS(1);
-    case 8: GB_FS(2);
-    case 16: GB_FS(4);
-    case 32: GB_FS(8);
-    default: GB_FS(0);
+cudaError_t launch_scan_m(const IvfpqfsCodec& c, int nq, const ListScanArgs& a, cudaStream_t st) {
+  switch (c.code_bytes()) {
+    case 4: return launch_list_scan<IvfpqfsCodec, METRIC, 1>(c, nq, a, st);
+    case 8: return launch_list_scan<IvfpqfsCodec, METRIC, 2>(c, nq, a, st);
+    case 16: return launch_list_scan<IvfpqfsCodec, METRIC, 4>(c, nq, a, st);
+    case 32: return launch_list_scan<IvfpqfsCodec, METRIC, 8>(c, nq, a, st);
+    default: return launch_list_scan<IvfpqfsCodec, METRIC, 0>(c, nq, a, st);
   }
-#undef GB_FS
 }
 
 }  // namespace
@@ -347,10 +193,10 @@ cudaError_t launch_pqfs_lut(const float* xq, int64_t ldq, int nq, const float* p
 cudaError_t launch_ivfpqfs_scan(const uint8_t* lut8, const float* ab, int nq, const int32_t* probe_ids, int nprobe, int pg,
                                 ListDirectory dir, int M, int k, int metric, FilterArgs f, unsigned long long* partial,
                                 cudaStream_t st) {
-  if (nq <= 0 || nprobe <= 0) return cudaSuccess;
-  if (k <= 0 || k > 4096 || nq > 65535 || pg < 1 || pg > FS_MAX_PG) return cudaErrorInvalidValue;
-  if (metric == kMetricL2) return launch_scan_m<kMetricL2>(lut8, ab, nq, probe_ids, nprobe, pg, dir, M, k, f, partial, st);
-  return launch_scan_m<kMetricIP>(lut8, ab, nq, probe_ids, nprobe, pg, dir, M, k, f, partial, st);
+  const IvfpqfsCodec c{lut8, ab, M, 0.f, 0.f};
+  const ListScanArgs a{probe_ids, nullptr, nprobe, nprobe, pg, dir, k, f, nullptr, 0, nullptr, true, partial};
+  if (metric == kMetricL2) return launch_scan_m<kMetricL2>(c, nq, a, st);
+  return launch_scan_m<kMetricIP>(c, nq, a, st);
 }
 
 }  // namespace gb

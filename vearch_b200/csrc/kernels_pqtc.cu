@@ -4,7 +4,7 @@
 // driven by search_preassigned (gamma_index_ivfpq.cc:730-947): per (query, probed list, entry)
 //     dis = dis0 + sum_m tab[m][code[m]],   tab = T[list] - 2 ip[query]   (L2, precomputed-table form)
 //     dis = <x, centroid> + sum_m ip[query][m][code[m]]                    (inner product)
-// and the k' best (k' = recall_num or k) survive.  ivfpq_scan_kernel (kernels_ivfpq.cu) evaluates that
+// and the k' best (k' = recall_num or k) survive.  The query-major list scan (list_scan.cuh) evaluates that
 // sum literally, 16 shared-memory gathers per (query, entry): it is bound by instruction issue and
 // LDS wavefronts, not by HBM.  When every list is probed by dozens of queries of the same batch the
 // same numbers are a dense contraction:
@@ -661,7 +661,7 @@ __global__ void __launch_bounds__(RS_NT)
     float dis = coarse_dis[(int64_t)q * nprobe + p];
     const unsigned char* code = dir.codes[l] + (int64_t)pos * M;
     const float* Tl = METRIC == kMetricL2 ? T + (int64_t)l * M * PT_KSUB : nullptr;
-    // the reference's order: dis = dis0; dis += tab[m][code[m]], tab = T - 2 ip as ivfpq_scan_kernel builds it
+    // the reference's order: dis = dis0; dis += tab[m][code[m]], tab = T - 2 ip as the list scan's IVF-PQ codec builds it
     for (int m = 0; m < M; m++) {
       const int c = code[m];
       const float a = staged ? ips[m * PT_KSUB + c] : __ldg(ipq + m * PT_KSUB + c);
