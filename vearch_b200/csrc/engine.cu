@@ -1321,7 +1321,7 @@ int Engine::Dump() {
   int trained = index_->trained() ? 1 : 0;
   wr<int32_t>(f, trained);
   // an index whose trained state does not persist (IVFPQFastScan) is trained again by Load
-  IVFFlatIndex* ivf = index_->persists_trained_state() ? dynamic_cast<IVFFlatIndex*>(index_.get()) : nullptr;
+  IvfIndex* ivf = index_->persists_trained_state() ? dynamic_cast<IvfIndex*>(index_.get()) : nullptr;
   IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(index_.get());
   if (trained && ivf) {
     std::vector<float> c((size_t)ivf->nlist() * dim_);
@@ -1345,7 +1345,7 @@ int Engine::Dump() {
     wr<int32_t>(ef, e.dim);
     ef.write(reinterpret_cast<const char*>(erows.data()), (std::streamsize)(erows.size() * 4));
     if (ef.fail()) return -1;
-    IVFFlatIndex* eivf = dynamic_cast<IVFFlatIndex*>(e.index.get());
+    IvfIndex* eivf = dynamic_cast<IvfIndex*>(e.index.get());
     if (eivf && eivf->trained() && eivf->dump_gamma(dir, e.name + ".000")) return -1;
   }
   std::ofstream done(dir + "/dump.done");
@@ -1403,11 +1403,11 @@ int Engine::Load() {
     std::vector<float> erows((size_t)maxd * e.dim);
     if (maxd && !ef.read(reinterpret_cast<char*>(erows.data()), (std::streamsize)(erows.size() * 4))) return -1;
     if (maxd && e.index->add_vectors(erows.data(), maxd)) return -1;
-    IVFFlatIndex* eivf = dynamic_cast<IVFFlatIndex*>(e.index.get());
+    IvfIndex* eivf = dynamic_cast<IvfIndex*>(e.index.get());
     int64_t eload = 0;
     if (eivf) eivf->load_gamma(dir, e.name + ".000", &eload);  // trained state + lists; absent: trained again later
   }
-  IVFFlatIndex* ivf = index_->persists_trained_state() ? dynamic_cast<IVFFlatIndex*>(index_.get()) : nullptr;
+  IvfIndex* ivf = index_->persists_trained_state() ? dynamic_cast<IvfIndex*>(index_.get()) : nullptr;
   IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(index_.get());
   if (trained && ivf) {
     std::vector<float> c((size_t)ivf->nlist() * dim_);

@@ -64,6 +64,14 @@ void* Scratch::alloc(size_t bytes) {
   T* var = (s).alloc_n<T>((size_t)(n));       \
   if (!var) return -1
 
+cudaError_t upload_rows_padded(float* dst, const float* src, int64_t n, int d, int dpad, cudaStream_t st) {
+  if (dpad != d) {
+    const cudaError_t e = cudaMemsetAsync(dst, 0, (size_t)n * dpad * 4, st);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaMemcpy2DAsync(dst, (size_t)dpad * 4, src, (size_t)d * 4, (size_t)d * 4, n, cudaMemcpyHostToDevice, st);
+}
+
 // ------------------------------------------------------------------------------------------
 // Segments are VIRTUAL address ranges of seg_rows rows; physical HBM is mapped into them in chunks as rows
 // arrive (CUDA virtual memory management: cuMemAddressReserve / cuMemCreate / cuMemMap, reached through
@@ -839,10 +847,7 @@ int Index::search_direct(const SearchContext& ctx, int nq, const float* x, int k
     if (cudaMallocAsync(&dq, (size_t)nq * dpad_ * 4, st) != cudaSuccess) break;
     if (cudaMallocAsync(&dd, (size_t)nq * k * 4, st) != cudaSuccess) break;
     if (cudaMallocAsync(&di, (size_t)nq * k * 8, st) != cudaSuccess) break;
-    if (d_ != dpad_ && cudaMemsetAsync(dq, 0, (size_t)nq * dpad_ * 4, st) != cudaSuccess) break;
-    if (cudaMemcpy2DAsync(dq, (size_t)dpad_ * 4, x, (size_t)d_ * 4, (size_t)d_ * 4, nq, cudaMemcpyHostToDevice, st) !=
-        cudaSuccess)
-      break;
+    if (upload_rows_padded(dq, x, nq, d_, dpad_, st) != cudaSuccess) break;
     rc = search_device(ctx, nq, dq, dpad_, k, dd, di, st);
     if (rc) break;
     rc = -1;
@@ -924,6 +929,23 @@ static void rand_perm_mt(std::vector<int32_t>& perm, int64_t n, int64_t seed) {
     int64_t i2 = i + (int64_t)(mt() % (uint32_t)(n - i));
     std::swap(perm[i], perm[i2]);
   }
+}
+
+// faiss's max_train_points rule: the first n_out rows of a seeded permutation (seed 1234) of the n rows of x (stride
+// dpad), or x itself when n_out == n
+static int subsample_rows(const float* x, int64_t n, int64_t n_out, int dpad, const float** out, Scratch& s) {
+  *out = x;
+  if (n_out >= n) return 0;
+  cudaStream_t st = s.stream();
+  std::vector<int32_t> perm;
+  rand_perm_mt(perm, n, 1234);
+  GB_ALLOC(d_idx, int32_t, n_out, s);
+  GB_CUDA(cudaMemcpyAsync(d_idx, perm.data(), (size_t)n_out * 4, cudaMemcpyHostToDevice, st));
+  GB_ALLOC(sub, float, (size_t)n_out * dpad, s);
+  GB_CUDA(launch_gather_rows(x, dpad, d_idx, n_out, dpad, sub, dpad, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  *out = sub;
+  return 0;
 }
 
 int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k, const KMeansParams& kp,
@@ -1037,7 +1059,7 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
 }
 
 // ------------------------------------------------------------------------------------------
-IVFFlatIndex::IVFFlatIndex(int d, const ModelParams& mp, int device, int seg_shift, const std::string& type)
+IvfIndex::IvfIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift)
     : Index(type, d, mp, device, seg_shift), nlist_(mp.ncentroids) {
   cudaMalloc(&d_centroids_, (size_t)nlist_ * dpad_ * 4);
   cudaMemset(d_centroids_, 0, (size_t)nlist_ * dpad_ * 4);
@@ -1047,34 +1069,37 @@ IVFFlatIndex::IVFFlatIndex(int d, const ModelParams& mp, int device, int seg_shi
   rebuild_centroid_tiles(0);
   cudaStreamSynchronize(0);
 }
-IVFFlatIndex::~IVFFlatIndex() {
-  if (mirror_.base) cudaFree(mirror_.base);
-  if (mirror_.norms) cudaFree(mirror_.norms);
-  if (mirror_.d_tile0) cudaFree(mirror_.d_tile0); cudaFree(d_centroids_);
+IvfIndex::~IvfIndex() {
+  cudaFree(d_centroids_);
   cudaFree(d_cent_tiles_);
   cudaFree(d_cent_norms_);
 }
-int IVFFlatIndex::rebuild_centroid_tiles(cudaStream_t st) {
+IVFFlatIndex::~IVFFlatIndex() {
+  if (mirror_.base) cudaFree(mirror_.base);
+  if (mirror_.norms) cudaFree(mirror_.norms);
+  if (mirror_.d_tile0) cudaFree(mirror_.d_tile0);
+}
+int IvfIndex::rebuild_centroid_tiles(cudaStream_t st) {
   GB_CUDA(launch_tc_stage_rows(d_centroids_, dpad_, nlist_, dpad_, (int)round_up(dpad_, 16), d_cent_tiles_, d_cent_norms_, st));
   return 0;
 }
 
-int IVFFlatIndex::training_threshold() const {
-  // gamma_index_ivfflat.cc:239: default nlist * 200 ; Indexing() clamps to [39, 256] * nlist (:350-375)
-  int64_t t = mp_.training_threshold ? mp_.training_threshold : (int64_t)nlist_ * 200;
+int IvfIndex::training_threshold() const {
+  // Indexing() clamps to [39, 256] * nlist (gamma_index_ivfflat.cc:350-375, gamma_index_ivfpq.cc:304-329)
+  int64_t t = mp_.training_threshold ? mp_.training_threshold : default_training_threshold();
   if (t < nlist_)
     t = (int64_t)nlist_ * 39;
   else if (t > (int64_t)nlist_ * 256)
     t = (int64_t)nlist_ * 256;
   return (int)t;
 }
-int64_t IVFFlatIndex::index_mem_bytes() const {
-  const int64_t tile_bytes = tc_mirror_tile_floats((int)round_up(dpad_, 16)) * 4 + 512;
-  const int64_t mirror = mirror_.cap_tiles * tile_bytes;
-  const int64_t cent_tiles = (nlist_ + 127) / 128 * tile_bytes;
-  return (int64_t)nlist_ * dpad_ * 4 + cent_tiles + (lists_ ? lists_->mem_bytes() : 0) + mirror;
+static int64_t tc_tile_bytes(int dpad) { return tc_mirror_tile_floats((int)round_up(dpad, 16)) * 4 + 512; }
+int64_t IvfIndex::index_mem_bytes() const {
+  const int64_t cent_tiles = (nlist_ + 127) / 128 * tc_tile_bytes(dpad_);
+  return (int64_t)nlist_ * dpad_ * 4 + cent_tiles + (lists_ ? lists_->mem_bytes() : 0);
 }
-int IVFFlatIndex::set_centroids(const float* host, int nlist) {
+int64_t IVFFlatIndex::index_mem_bytes() const { return IvfIndex::index_mem_bytes() + mirror_.cap_tiles * tc_tile_bytes(dpad_); }
+int IvfIndex::set_centroids(const float* host, int nlist) {
   if (nlist != nlist_) {
     set_last_error("set_centroids: nlist mismatch");
     return -1;
@@ -1091,7 +1116,7 @@ int IVFFlatIndex::set_centroids(const float* host, int nlist) {
   trained_ = true;
   return 0;
 }
-int IVFFlatIndex::get_centroids(float* host) const {
+int IvfIndex::get_centroids(float* host) const {
   cudaSetDevice(device_);
   GB_CUDA(cudaMemcpy2D(host, (size_t)d_ * 4, d_centroids_, (size_t)dpad_ * 4, (size_t)d_ * 4, nlist_,
                        cudaMemcpyDeviceToHost));
@@ -1099,7 +1124,7 @@ int IVFFlatIndex::get_centroids(float* host) const {
 }
 
 // GammaIVFFlatIndex::Indexing (gamma_index_ivfflat.cc:342-411): train on the FIRST num vectors.
-int IVFFlatIndex::train() {
+int IvfIndex::train() {
   std::lock_guard<std::mutex> bg(build_mu_);
   if (trained_) return 0;
   cudaSetDevice(device_);
@@ -1114,17 +1139,9 @@ int IVFFlatIndex::train() {
   Scratch s(st);
   const float* xt = store_->contiguous(num, s);
   if (!xt) return -1;
-  KMeansParams kp;
-  const bool is_pq = (type_ == "IVFPQ");
-  kp.niter = is_pq ? 10 : 25;                              // gamma_index_ivfpq.cc:188
-  kp.spherical = is_pq && mp_.metric == kMetricIP;          // gamma_index_ivfpq.cc:189-191
-  if (type_ == "IVFPQFastScan") {  // gamma_index_ivfpqfs.cc:95-104: IndexFlatL2 quantiser, spherical for IP, niter kept
-    kp.spherical = mp_.metric == kMetricIP;
-    kp.l2_assign = true;
-  }
   xt = train_transform(xt, num, s);  // OPQ: learn the rotation, continue on the rotated slab
   if (!xt) return -1;
-  if (kmeans_device(xt, dpad_, num, d_, nlist_, kp, d_centroids_, dpad_, st, nullptr)) return -1;
+  if (kmeans_device(xt, dpad_, num, d_, nlist_, coarse_kmeans_params(), d_centroids_, dpad_, st, nullptr)) return -1;
   if (rebuild_centroid_tiles(st)) return -1;
   if (train_extra(xt, num, s)) return -1;
   GB_CUDA(cudaStreamSynchronize(st));
@@ -1133,7 +1150,7 @@ int IVFFlatIndex::train() {
   return 0;
 }
 
-int IVFFlatIndex::assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* out, Scratch& s) {
+int IvfIndex::assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* out, Scratch& s) {
   cudaStream_t st = s.stream();
   GB_ALLOC(best, unsigned long long, n, s);
   GB_CUDA(launch_fill_u64(best, n, kKeySentinel, st));
@@ -1145,16 +1162,16 @@ int IVFFlatIndex::assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* ou
 }
 
 int IVFFlatIndex::append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
-                               const int32_t* d_assign, Scratch& s) {
-  (void)d_assign;
+                               const std::vector<int>& add, Scratch& s) {
   GB_CUDA(launch_ivf_append_vecs(x, dpad_, n, dpad_, d_list, d_pos, reinterpret_cast<float* const*>(lists_->d_data()),
                                  lists_->d_ids(), vid0, s.stream()));
-  return 0;
+  // the tensor-core mirror's rows after the list data, before the new lengths are committed
+  return mirror_append(x, n, d_list, d_pos, add, s.stream());
 }
 
 // GammaIVFFlatIndex::Add (gamma_index_ivfflat.cc:413-474) driven like
 // VectorManager::AddRTVecsToIndex (vector_manager.cc:572-702), in large device batches.
-int IVFFlatIndex::index_batch(const float* x, int64_t n, int64_t vid0, const uint8_t* del_bitmap) {
+int IvfIndex::index_batch(const float* x, int64_t n, int64_t vid0, const uint8_t* del_bitmap) {
   cudaStream_t st = build_stream_;
   Scratch s(st);
   x = transform_dev(x, n, s);  // OPQ rotation; the raw store keeps the original rows
@@ -1187,15 +1204,14 @@ int IVFFlatIndex::index_batch(const float* x, int64_t n, int64_t vid0, const uin
   std::unique_lock<std::shared_mutex> lk(mu_);
   drain_searches();  // kernels of earlier searches read lengths and base pointers at run time
   if (lists_->reserve(add, st)) return -1;
-  if (append_batch(x, n, vid0, d_list, d_pos, d_assign, s)) return -1;
-  // data (lists AND their tensor-core mirror) first, the new lengths last (realtime_mem_data.cc:292-293)
-  if (type_ == "IVFFLAT" && mirror_append(x, n, d_list, d_pos, add, st)) return -1;
+  // data first, the new lengths last (realtime_mem_data.cc:292-293)
+  if (append_batch(x, n, vid0, d_list, d_pos, add, s)) return -1;
   if (lists_->commit(add, st)) return -1;
   GB_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
 
-int IVFFlatIndex::add_pending(const uint8_t* del_bitmap) {
+int IvfIndex::add_pending(const uint8_t* del_bitmap) {
   std::lock_guard<std::mutex> bg(build_mu_);
   if (!trained_) return 0;
   cudaSetDevice(device_);
@@ -1222,21 +1238,25 @@ int IVFFlatIndex::add_pending(const uint8_t* del_bitmap) {
   return 0;
 }
 
-int IVFFlatIndex::reset_index() {
+int IvfIndex::reset_index() {
   std::lock_guard<std::mutex> bg(build_mu_);
   cudaSetDevice(device_);
   std::unique_lock<std::shared_mutex> lk(mu_);
-  std::unique_lock<std::shared_mutex> ml(mirror_rw_);
   cudaDeviceSynchronize();  // kernels of earlier device-resident searches may still read the lists
   lists_.reset();
   vid2pos_.clear();
-  mirror_.lens.clear();
+  reset_codec();
   indexed_count_ = 0;
   trained_ = false;
   return 0;
 }
 
-int IVFFlatIndex::compact_lists() {
+void IVFFlatIndex::reset_codec() {
+  std::unique_lock<std::shared_mutex> ml(mirror_rw_);
+  mirror_.lens.clear();
+}
+
+int IvfIndex::compact_lists() {
   std::lock_guard<std::mutex> bg(build_mu_);
   if (!lists_) return 0;
   cudaSetDevice(device_);
@@ -1252,7 +1272,7 @@ int Index::update_vector(int64_t vid, const float* x) {
 
 // GammaIVFFlatIndex::Update / GammaIVFPQIndex::Update (gamma_index_ivfflat.cc:476-522,
 // gamma_index_ivfpq.cc:402-453): tombstone the old entry, append the new vector to its list.
-int IVFFlatIndex::update_vector(int64_t vid, const float* x) {
+int IvfIndex::update_vector(int64_t vid, const float* x) {
   std::lock_guard<std::mutex> bg(build_mu_);
   if (Index::update_vector(vid, x)) return -1;
   if (!trained_ || vid >= indexed_count_) return 0;  // not indexed yet: the add path will pick it up
@@ -1264,7 +1284,7 @@ int IVFFlatIndex::update_vector(int64_t vid, const float* x) {
   return index_batch(store_->seg((int)si) + off * dpad_, 1, vid, nullptr);
 }
 
-int IVFFlatIndex::resolve_nprobe(const SearchContext& ctx) const {
+int IvfIndex::resolve_nprobe(const SearchContext& ctx) const {
   int nprobe = mp_.nprobe;
   if (ctx.params.nprobe > 0 && ctx.params.nprobe <= nlist_) nprobe = ctx.params.nprobe;  // ivfflat.cc:551-559
   if (nprobe > nlist_) nprobe = nlist_;
@@ -1294,8 +1314,8 @@ static int coarse_seg_tiles(int nqt, int ntc, int nsm) {
 }
 
 // quantizer->search (gamma_index_ivfflat.cc:568 / gamma_index_ivfpq.cc:595)
-int IVFFlatIndex::coarse_dev(int nq, const float* xq, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis,
-                             Scratch& s) {
+int IvfIndex::coarse_dev(int nq, const float* xq, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis,
+                         Scratch& s) {
   cudaStream_t st = s.stream();
   GB_ALLOC(keys, unsigned long long, (size_t)nq * nprobe, s);
   const bool tc = nlist_ >= 64 && nq >= 32;
@@ -1337,6 +1357,22 @@ int IVFFlatIndex::coarse_dev(int nq, const float* xq, int nprobe, int metric, in
 // score segment of len(list) floats, cut (list, 128 pairs, 128 rows) tiles; device side: grouped
 // GEMM on wgmma + segment select.
 
+int IvfIndex::group_pairs_by_list(const int32_t* probe_ids, int64_t npairs, int nseg, int group, int64_t max_items,
+                                  LmGrouping* g, Scratch& s) {
+  GB_ALLOC(d_cnt, int32_t, nlist_, s);
+  GB_ALLOC(d_start, int32_t, nlist_, s);
+  GB_ALLOC(d_cursor, int32_t, nlist_, s);
+  GB_ALLOC(d_item_start, int32_t, nlist_, s);
+  GB_ALLOC(d_grp_start, int32_t, nlist_, s);
+  GB_ALLOC(totals, int64_t, 3, s);
+  GB_ALLOC(pair_j, int64_t, npairs, s);
+  GB_ALLOC(items, LmTile, max_items, s);
+  GB_CUDA(launch_lmk_group(probe_ids, npairs, lists_->directory(), nseg, group, d_cnt, d_start, d_cursor, d_item_start,
+                           d_grp_start, totals, pair_j, items, s.stream()));
+  *g = {totals, pair_j, items};
+  return 0;
+}
+
 // called from index_batch with mu_ held exclusively: no search is inside ensure_mirror.  Kernels of an
 // earlier search_device may still be running, but they only look at rows below the lengths they were
 // launched with, and the rows written here lie above those.
@@ -1358,7 +1394,7 @@ int IVFFlatIndex::mirror_append(const float* x, int64_t n, const int32_t* d_list
 }
 
 int IVFFlatIndex::ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStream_t st) {
-  if (type_ != "IVFFLAT" || !lists_) return 1;
+  if (!lists_) return 1;
   lk.lock();
   if (mirror_.disabled) return 1;
   if (mirror_.base && mirror_.lens == lists_->lens()) return 0;
@@ -1429,21 +1465,13 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
     const int nseg = (int)std::min<int64_t>(8, std::max<int64_t>(1, (lists_->max_len() + kLmkSegRows - 1) / kLmkSegRows));
     const int64_t max_items = (npairs / 128 + nlist_) * nseg;
     if (max_items > INT32_MAX) return 1;
-    GB_ALLOC(d_cnt, int32_t, nlist_, s);
-    GB_ALLOC(d_start, int32_t, nlist_, s);
-    GB_ALLOC(d_cursor, int32_t, nlist_, s);
-    GB_ALLOC(d_item_start, int32_t, nlist_, s);
-    GB_ALLOC(d_grp_start, int32_t, nlist_, s);
-    GB_ALLOC(d_totals, int64_t, 3, s);
-    GB_ALLOC(d_pair_j, int64_t, npairs, s);
-    GB_ALLOC(d_items, LmTile, max_items, s);
     GB_ALLOC(d_tau, unsigned long long, nq, s);
     const size_t nout = (size_t)npairs * nseg * k;
     GB_ALLOC(d_out, unsigned long long, nout, s);
     GB_CUDA(cudaMemsetAsync(d_tau, 0xFF, sizeof(unsigned long long) * nq, st));
     GB_CUDA(cudaMemsetAsync(d_out, 0xFF, sizeof(unsigned long long) * nout, st));
-    GB_CUDA(launch_lmk_group(probe_ids, npairs, dir, nseg, 128, d_cnt, d_start, d_cursor, d_item_start, d_grp_start, d_totals,
-                             d_pair_j, d_items, st));
+    LmGrouping g;
+    if (group_pairs_by_list(probe_ids, npairs, nseg, 128, max_items, &g, s)) return -1;
     const int k16 = (int)round_up(dpad_, 16);
     const int64_t max_groups = npairs / 128 + nlist_;
     const size_t slot_bytes = (size_t)128 * k16 * 8, a_bytes = (size_t)max_groups * (slot_bytes + 128 * 4);
@@ -1451,23 +1479,22 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
     // TMA-fed from the mirror when it applies and fits, else the register-staged pipeline over the lists themselves
     bool tma = k <= 32 && k16 > 16 && a_bytes <= ((size_t)8 << 30) && ensure_mirror(mlk, st) == 0;
     if (tma) {
-      float* a_scratch = static_cast<float*>(big_acquire(a_bytes, st));
-      if (!a_scratch) return -1;
-      auto rel_fn = [this, a_scratch, st](void*) { big_release(a_scratch, st); };
-      std::unique_ptr<void, decltype(rel_fn)> rel(a_scratch, rel_fn);
+      BigScope big(this, a_bytes, st);
+      if (!big.p) return -1;
+      float* a_scratch = static_cast<float*>(big.p);
       float* a_norms = reinterpret_cast<float*>(reinterpret_cast<char*>(a_scratch) + (size_t)max_groups * slot_bytes);
       TcMirrorView mv{mirror_.base, mirror_.d_tile0, mirror_.norms, k16};
       last_scan_kernel_ = "ivf_listmajor_tma_kernel";
       scan_timer_begin(st);
-      GB_CUDA(launch_lm_stage_queries(xq, dpad_, dpad_, k16, d_items, (int)max_items, d_totals, d_pair_j, nprobe, a_scratch,
+      GB_CUDA(launch_lm_stage_queries(xq, dpad_, dpad_, k16, g.items, (int)max_items, g.totals, g.pair_j, nprobe, a_scratch,
                                       a_norms, st));
-      GB_CUDA(launch_ivf_listmajor_tma(a_scratch, a_norms, mv, d_items, (int)max_items, d_totals, d_pair_j, nprobe, dir, k,
+      GB_CUDA(launch_ivf_listmajor_tma(a_scratch, a_norms, mv, g.items, (int)max_items, g.totals, g.pair_j, nprobe, dir, k,
                                        nseg, metric, f, d_tau, d_out, st));
       scan_timer_end(st);
     } else {
       last_scan_kernel_ = "ivf_listmajor_pipe_kernel";
       scan_timer_begin(st);
-      GB_CUDA(launch_ivf_listmajor_pipe(xq, dpad_, dpad_, d_items, (int)max_items, d_totals, d_pair_j, nprobe, dir, k, nseg,
+      GB_CUDA(launch_ivf_listmajor_pipe(xq, dpad_, dpad_, g.items, (int)max_items, g.totals, g.pair_j, nprobe, dir, k, nseg,
                                         metric, f, d_tau, d_out, st));
       scan_timer_end(st);
     }
@@ -1491,10 +1518,9 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
   GB_ALLOC(d_pair_off, int64_t, npairs, s);
   GB_ALLOC(d_seg_off, int64_t, npairs, s);
   GB_ALLOC(d_tiles, LmTile, std::max<int64_t>(ntiles, 1), s);
-  float* scores = static_cast<float*>(big_acquire((size_t)std::max<int64_t>(total, 1) * 4, st));
-  if (!scores) return -1;
-  auto rel_fn = [this, scores, st](void*) { big_release(scores, st); };
-  std::unique_ptr<void, decltype(rel_fn)> rel(scores, rel_fn);  // released (event-stamped) on every exit path
+  BigScope big(this, (size_t)std::max<int64_t>(total, 1) * 4, st);
+  if (!big.p) return -1;
+  float* scores = static_cast<float*>(big.p);
   GB_CUDA(launch_lm_assign_tiles(probe_ids, npairs, nprobe, dir, d_cnt, d_start, d_cursor, d_base_off, d_tile_start,
                                  d_pair_q, d_pair_off, d_seg_off, d_tiles, st));
   last_scan_kernel_ = "ivf_listmajor_tc_kernel+seg_select_kernel";
@@ -1505,29 +1531,28 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
   return 0;
 }
 
-int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
-                           const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
-                           Scratch& s) {
+int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq,
+                           const float* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
+                           unsigned long long* out_keys, Scratch& s) {
   (void)ctx;
+  (void)xq_raw;  // no transform: xq is the raw queries
   (void)coarse_dis;
   cudaStream_t st = s.stream();
-  if (type_ == "IVFFLAT") {
-    // The list-major scan selects on 3xTF32 tensor-core scores (|x|^2 + |y|^2 - 2 x.y for L2: on SIFT-like float data,
-    // |x|^2 ~ 40 d^2, the cancellation leaves ~1e-4 relative).  Its k winners are re-scored with the direct fp32 form
-    // from the raw vectors and re-sorted (rerank_kernel, k rows per query), so every distance that leaves the index is
-    // the exact-kernel value; on integer-valued data both forms are exact and nothing changes.
-    GB_ALLOC(lm_keys, unsigned long long, (size_t)nq * k, s);
-    int lm = scan_listmajor_dev(f, metric, nq, xq, k, probe_ids, nprobe, lm_keys, s);
-    if (lm < 0) return lm;
-    if (lm == 0) {
-      if ((dpad_ & 3) == 0 && k <= 8192) {
-        GB_CUDA(launch_rerank(lm_keys, k, nq, xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_, k, metric, f,
-                              out_keys, st));
-      } else {
-        GB_CUDA(cudaMemcpyAsync(out_keys, lm_keys, (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, st));
-      }
-      return 0;
+  // The list-major scan selects on 3xTF32 tensor-core scores (|x|^2 + |y|^2 - 2 x.y for L2: on SIFT-like float data,
+  // |x|^2 ~ 40 d^2, the cancellation leaves ~1e-4 relative).  Its k winners are re-scored with the direct fp32 form
+  // from the raw vectors and re-sorted (rerank_kernel, k rows per query), so every distance that leaves the index is
+  // the exact-kernel value; on integer-valued data both forms are exact and nothing changes.
+  GB_ALLOC(lm_keys, unsigned long long, (size_t)nq * k, s);
+  int lm = scan_listmajor_dev(f, metric, nq, xq, k, probe_ids, nprobe, lm_keys, s);
+  if (lm < 0) return lm;
+  if (lm == 0) {
+    if ((dpad_ & 3) == 0 && k <= 8192) {
+      GB_CUDA(launch_rerank(lm_keys, k, nq, xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_, k, metric, f,
+                            out_keys, st));
+    } else {
+      GB_CUDA(cudaMemcpyAsync(out_keys, lm_keys, (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, st));
     }
+    return 0;
   }
   int nparts = ivfflat_scan_nparts(nprobe, lists_->max_len());
   GB_ALLOC(partial, unsigned long long, (size_t)nq * nparts * k, s);
@@ -1541,23 +1566,11 @@ int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int me
   return 0;
 }
 
-// When a transform sits in front of the index the scan works on transformed queries while the exact re-rank
-// needs the original ones: the search entry points leave both base pointers here for scan_dev (same thread).
-static thread_local const float* tls_xq_transformed = nullptr;
-static thread_local const float* tls_xq_raw = nullptr;
-static const float* raw_queries_for(const float* xq) {
-  return tls_xq_transformed && tls_xq_raw ? tls_xq_raw + (xq - tls_xq_transformed) : xq;
-}
-
 // GammaIVFFlatIndex::Search (gamma_index_ivfflat.cc:524-577)
-int IVFFlatIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq_in,
-                                  int k, unsigned long long* out_keys, Scratch& s) {
+int IvfIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq_in, int k,
+                              unsigned long long* out_keys, Scratch& s) {
   const float* xq = transform_dev(xq_in, nq, s);
   if (!xq) return -1;
-  struct TlsGuard {
-    TlsGuard(const float* t, const float* r) { tls_xq_transformed = t == r ? nullptr : t, tls_xq_raw = r; }
-    ~TlsGuard() { tls_xq_transformed = tls_xq_raw = nullptr; }
-  } guard(xq, xq_in);
   const int nprobe = resolve_nprobe(ctx);
   const int QB = 16384;
   for (int q0 = 0; q0 < nq; q0 += QB) {
@@ -1566,21 +1579,20 @@ int IVFFlatIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f,
     GB_ALLOC(probe_ids, int32_t, (size_t)qb * nprobe, sb);
     GB_ALLOC(coarse_dis, float, (size_t)qb * nprobe, sb);
     if (coarse_dev(qb, xq + (int64_t)q0 * dpad_, nprobe, coarse_metric(metric), probe_ids, coarse_dis, sb)) return -1;
-    if (scan_dev(ctx, f, metric, qb, xq + (int64_t)q0 * dpad_, k, probe_ids, coarse_dis, nprobe,
+    if (scan_dev(ctx, f, metric, qb, xq + (int64_t)q0 * dpad_, xq_in + (int64_t)q0 * dpad_, k, probe_ids, coarse_dis, nprobe,
                  out_keys + (int64_t)q0 * k, sb))
       return -1;
   }
   return 0;
 }
 
-int IVFFlatIndex::coarse_search_host(int nq, const float* x, int nprobe, float* out_dis, int64_t* out_ids) {
+int IvfIndex::coarse_search_host(int nq, const float* x, int nprobe, float* out_dis, int64_t* out_ids) {
   cudaSetDevice(device_);
   cudaStream_t st = thread_stream(device_);
   std::shared_lock<std::shared_mutex> lk(mu_);
   Scratch s(st);
   GB_ALLOC(dq, float, (size_t)nq * dpad_, s);
-  GB_CUDA(cudaMemsetAsync(dq, 0, (size_t)nq * dpad_ * 4, st));
-  GB_CUDA(cudaMemcpy2DAsync(dq, (size_t)dpad_ * 4, x, (size_t)d_ * 4, (size_t)d_ * 4, nq, cudaMemcpyHostToDevice, st));
+  GB_CUDA(upload_rows_padded(dq, x, nq, d_, dpad_, st));
   GB_ALLOC(ids, int32_t, (size_t)nq * nprobe, s);
   GB_ALLOC(dis, float, (size_t)nq * nprobe, s);
   const float* dqt = transform_dev(dq, nq, s);
@@ -1593,8 +1605,8 @@ int IVFFlatIndex::coarse_search_host(int nq, const float* x, int nprobe, float* 
   return 0;
 }
 
-int IVFFlatIndex::search_preassigned_host(const SearchContext& ctx, int nq, const float* x, int k, const int64_t* keys,
-                                          const float* coarse_dis, int nprobe, float* out_dis, int64_t* out_ids) {
+int IvfIndex::search_preassigned_host(const SearchContext& ctx, int nq, const float* x, int k, const int64_t* keys,
+                                      const float* coarse_dis, int nprobe, float* out_dis, int64_t* out_ids) {
   if (!trained_ || !lists_) {
     set_last_error("index not trained");
     return -1;
@@ -1604,8 +1616,7 @@ int IVFFlatIndex::search_preassigned_host(const SearchContext& ctx, int nq, cons
   std::shared_lock<std::shared_mutex> lk(mu_);
   Scratch s(st);
   GB_ALLOC(dq, float, (size_t)nq * dpad_, s);
-  GB_CUDA(cudaMemsetAsync(dq, 0, (size_t)nq * dpad_ * 4, st));
-  GB_CUDA(cudaMemcpy2DAsync(dq, (size_t)dpad_ * 4, x, (size_t)d_ * 4, (size_t)d_ * 4, nq, cudaMemcpyHostToDevice, st));
+  GB_CUDA(upload_rows_padded(dq, x, nq, d_, dpad_, st));
   std::vector<int32_t> h((size_t)nq * nprobe);
   for (size_t i = 0; i < h.size(); i++) h[i] = (int32_t)keys[i];
   GB_ALLOC(ids, int32_t, h.size(), s);
@@ -1618,10 +1629,7 @@ int IVFFlatIndex::search_preassigned_host(const SearchContext& ctx, int nq, cons
   GB_ALLOC(okeys, unsigned long long, (size_t)nq * k, s);
   const float* dqt = transform_dev(dq, nq, s);
   if (!dqt) return -1;
-  tls_xq_transformed = dqt == dq ? nullptr : dqt, tls_xq_raw = dq;
-  const int src = scan_dev(ctx, f, metric, nq, dqt, k, ids, dis, nprobe, okeys, s);
-  tls_xq_transformed = tls_xq_raw = nullptr;
-  if (src) return -1;
+  if (scan_dev(ctx, f, metric, nq, dqt, dq, k, ids, dis, nprobe, okeys, s)) return -1;
   GB_ALLOC(dd, float, (size_t)nq * k, s);
   GB_ALLOC(di, int64_t, (size_t)nq * k, s);
   GB_CUDA(launch_decode_keys(okeys, k, nq, k, metric, dd, di, 0, st));
@@ -1632,13 +1640,81 @@ int IVFFlatIndex::search_preassigned_host(const SearchContext& ctx, int nq, cons
 }
 
 // ------------------------------------------------------------------------------------------
+IvfPqBase::IvfPqBase(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int M, int ksub)
+    : IvfIndex(type, d, mp, device, seg_shift), M_(M), dsub_(d / M), ksub_(ksub) {
+  cudaMalloc(&d_pq_, (size_t)M_ * ksub_ * dsub_ * 4);
+  cudaMemset(d_pq_, 0, (size_t)M_ * ksub_ * dsub_ * 4);
+}
+IvfPqBase::~IvfPqBase() { cudaFree(d_pq_); }
+int64_t IvfPqBase::index_mem_bytes() const { return IvfIndex::index_mem_bytes() + (int64_t)M_ * ksub_ * dsub_ * 4; }
+int IvfPqBase::set_pq_centroids(const float* host) {
+  cudaSetDevice(device_);
+  std::unique_lock<std::shared_mutex> lk(mu_);
+  drain_searches();
+  GB_CUDA(cudaMemcpy(d_pq_, host, (size_t)M_ * ksub_ * dsub_ * 4, cudaMemcpyHostToDevice));
+  if (codebook_changed(build_stream_)) return -1;
+  GB_CUDA(cudaStreamSynchronize(build_stream_));
+  return 0;
+}
+int IvfPqBase::get_pq_centroids(float* host) const {
+  cudaSetDevice(device_);
+  GB_CUDA(cudaMemcpy(host, d_pq_, (size_t)M_ * ksub_ * dsub_ * 4, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int IvfPqBase::train_codebook(const float* x, int64_t n, Scratch& s) {
+  cudaStream_t st = s.stream();
+  const int dsp = (int)round_up(dsub_, 4);
+  GB_ALLOC(slice, float, (size_t)n * dsp, s);
+  GB_ALLOC(cent, float, (size_t)ksub_ * dsp, s);
+  KMeansParams kp;  // ClusteringParameters defaults: niter 25, seed 1234, max 256 points per centroid
+  for (int m = 0; m < M_; m++) {
+    GB_CUDA(launch_slice_cols(x, dpad_, n, m * dsub_, dsub_, slice, dsp, st));
+    if (kmeans_device(slice, dsp, n, dsub_, ksub_, kp, cent, dsp, st, nullptr)) return -1;
+    GB_CUDA(cudaMemcpy2DAsync(d_pq_ + (size_t)m * ksub_ * dsub_, (size_t)dsub_ * 4, cent, (size_t)dsp * 4, (size_t)dsub_ * 4,
+                              ksub_, cudaMemcpyDeviceToDevice, st));
+  }
+  return codebook_changed(st);
+}
+
+int IvfPqBase::append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                            const std::vector<int>& add, Scratch& s) {
+  (void)add;
+  cudaStream_t st = s.stream();
+  const int cb = code_bytes();
+  GB_ALLOC(codes, uint8_t, (size_t)n * cb, s);
+  GB_CUDA(encode_dev(x, n, d_list, codes, st));  // residual codecs: w.r.t. the assigned list
+  GB_CUDA(launch_ivf_append_codes(codes, n, cb, d_list, d_pos, reinterpret_cast<uint8_t* const*>(lists_->d_data()),
+                                  lists_->d_ids(), vid0, st));
+  return 0;
+}
+
+int IvfPqBase::encode_host(const float* x, int64_t n, const int64_t* assign, uint8_t* codes_out) {
+  cudaSetDevice(device_);
+  cudaStream_t st = thread_stream(device_);
+  Scratch s(st);
+  const int cb = code_bytes();
+  GB_ALLOC(dx, float, (size_t)n * dpad_, s);
+  GB_CUDA(upload_rows_padded(dx, x, n, d_, dpad_, st));
+  int32_t* da = nullptr;
+  std::vector<int32_t> h;
+  if (assign) {
+    h.assign(assign, assign + n);
+    da = s.alloc_n<int32_t>(n);
+    if (!da) return -1;
+    GB_CUDA(cudaMemcpyAsync(da, h.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  }
+  GB_ALLOC(codes, uint8_t, (size_t)n * cb, s);
+  GB_CUDA(encode_dev(dx, n, da, codes, st));
+  GB_CUDA(cudaMemcpyAsync(codes_out, codes, (size_t)n * cb, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// gamma_index_ivfpq.cc:122-124: nsubvector defaults to d / 2
 IVFPQIndex::IVFPQIndex(int d, const ModelParams& mp, int device, int seg_shift)
-    : IVFFlatIndex(d, mp, device, seg_shift, "IVFPQ") {
-  M_ = mp.nsubvector > 0 ? mp.nsubvector : d / 2;  // gamma_index_ivfpq.cc:122-124
-  if (M_ < 1) M_ = 1;
-  dsub_ = d / M_;
-  cudaMalloc(&d_pq_, (size_t)M_ * 256 * dsub_ * 4);
-  cudaMemset(d_pq_, 0, (size_t)M_ * 256 * dsub_ * 4);
+    : IvfPqBase("IVFPQ", d, mp, device, seg_shift, std::max(1, mp.nsubvector > 0 ? mp.nsubvector : d / 2), 256) {
   if (mp.opq_nsubvector > 0) {  // faiss::OPQMatrix(d, opq_nsubvector, d) (gamma_index_ivfpq.cc:168-178)
     cudaMalloc(&d_opq_, (size_t)d * dpad_ * 4);
     cudaMemset(d_opq_, 0, (size_t)d * dpad_ * 4);
@@ -1739,8 +1815,7 @@ int IVFPQIndex::apply_opq_host(const float* x, int64_t n, float* out) {
   std::shared_lock<std::shared_mutex> lk(mu_);
   Scratch s(st);
   GB_ALLOC(dx, float, (size_t)n * dpad_, s);
-  GB_CUDA(cudaMemsetAsync(dx, 0, (size_t)n * dpad_ * 4, st));
-  GB_CUDA(cudaMemcpy2DAsync(dx, (size_t)dpad_ * 4, x, (size_t)d_ * 4, (size_t)d_ * 4, n, cudaMemcpyHostToDevice, st));
+  GB_CUDA(upload_rows_padded(dx, x, n, d_, dpad_, st));
   const float* y = transform_dev(dx, n, s);
   if (!y) return -1;
   GB_CUDA(cudaMemcpy2DAsync(out, (size_t)d_ * 4, y, (size_t)dpad_ * 4, (size_t)d_ * 4, n, cudaMemcpyDeviceToHost, st));
@@ -1753,20 +1828,9 @@ const float* IVFPQIndex::train_transform(const float* xt, int64_t n_in, Scratch&
   if (opq_trained_) return transform_dev(xt, n_in, s);
   cudaStream_t st = s.stream();
   const int d = d_, Mo = mp_.opq_nsubvector, dso = d / Mo, dsp = (int)round_up(dso, 4);
-  int64_t n = std::min<int64_t>(n_in, 256 * 256);  // max_train_points
-  const float* xs = xt;
-  if (n < n_in) {
-    std::vector<int32_t> perm;
-    rand_perm_mt(perm, n_in, 1234);
-    int32_t* d_idx = s.alloc_n<int32_t>(n);
-    float* sub = s.alloc_n<float>((size_t)n * dpad_);
-    if (!d_idx || !sub) return nullptr;
-    if (cudaMemcpyAsync(d_idx, perm.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        launch_gather_rows(xt, dpad_, d_idx, n, dpad_, sub, dpad_, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess)
-      return nullptr;
-    xs = sub;
-  }
+  const int64_t n = std::min<int64_t>(n_in, 256 * 256);  // max_train_points
+  const float* xs;
+  if (subsample_rows(xt, n_in, n, dpad_, &xs, s)) return nullptr;
   const int64_t ldn = round_up(n, 4);
   float* xc = s.alloc_n<float>((size_t)n * dpad_);      // centred training set
   float* xproj = s.alloc_n<float>((size_t)n * dpad_);
@@ -1807,9 +1871,7 @@ const float* IVFPQIndex::train_transform(const float* xt, int64_t n_in, Scratch&
   const int niter = 50, niter_pq_0 = 40, niter_pq = 4;
   for (int it = 0; it < niter; it++) {
     for (size_t i = 0; i < R.size(); i++) Rf[i] = (float)R[i];
-    if (!ck(cudaMemsetAsync(d_opq_, 0, (size_t)d * dpad_ * 4, st)) ||
-        !ck(cudaMemcpy2DAsync(d_opq_, (size_t)dpad_ * 4, Rf.data(), (size_t)d * 4, (size_t)d * 4, d, cudaMemcpyHostToDevice, st)) ||
-        !ck(cudaMemsetAsync(xproj, 0, (size_t)n * dpad_ * 4, st)) ||
+    if (!ck(upload_rows_padded(d_opq_, Rf.data(), d, d, dpad_, st)) || !ck(cudaMemsetAsync(xproj, 0, (size_t)n * dpad_ * 4, st)) ||
         !ck(launch_dist_matrix(xc, dpad_, (int)n, d_opq_, dpad_, d, dpad_, kMetricIP, xproj, dpad_, st)))
       return nullptr;
     KMeansParams kp;
@@ -1841,9 +1903,7 @@ const float* IVFPQIndex::train_transform(const float* xt, int64_t n_in, Scratch&
       }
   }
   for (size_t i = 0; i < R.size(); i++) Rf[i] = (float)R[i];
-  if (!ck(cudaMemsetAsync(d_opq_, 0, (size_t)d * dpad_ * 4, st)) ||
-      !ck(cudaMemcpy2DAsync(d_opq_, (size_t)dpad_ * 4, Rf.data(), (size_t)d * 4, (size_t)d * 4, d, cudaMemcpyHostToDevice, st)) ||
-      !ck(cudaStreamSynchronize(st)))
+  if (!ck(upload_rows_padded(d_opq_, Rf.data(), d, d, dpad_, st)) || !ck(cudaStreamSynchronize(st)))
     return nullptr;
   opq_trained_ = true;
   return transform_dev(xt, n_in, s);
@@ -1851,27 +1911,24 @@ const float* IVFPQIndex::train_transform(const float* xt, int64_t n_in, Scratch&
 
 IVFPQIndex::~IVFPQIndex() {
   if (d_opq_) cudaFree(d_opq_);
-  cudaFree(d_pq_);
   cudaFree(d_table_);
   cudaFree(d_cb16_);
   cudaFree(d_cbnrm_);
   if (pqn_.base) cudaFree(pqn_.base);
   if (pqn_.d_off) cudaFree(pqn_.d_off);
 }
-int IVFPQIndex::training_threshold() const {
-  // gamma_index_ivfpq.cc:139-144: default max(nlist*200, 256); Indexing() clamps like IVFFLAT (:304-329)
-  int64_t t = mp_.training_threshold ? mp_.training_threshold : std::max<int64_t>((int64_t)nlist_ * 200, 256);
-  if (t < nlist_)
-    t = (int64_t)nlist_ * 39;
-  else if (t > (int64_t)nlist_ * 256)
-    t = (int64_t)nlist_ * 256;
-  return (int)t;
+// gamma_index_ivfpq.cc:139-144
+int64_t IVFPQIndex::default_training_threshold() const { return std::max<int64_t>((int64_t)nlist_ * 200, 256); }
+KMeansParams IVFPQIndex::coarse_kmeans_params() const {
+  KMeansParams kp;
+  kp.niter = 10;                            // gamma_index_ivfpq.cc:188
+  kp.spherical = mp_.metric == kMetricIP;  // gamma_index_ivfpq.cc:189-191
+  return kp;
 }
 int64_t IVFPQIndex::index_mem_bytes() const {
-  return IVFFlatIndex::index_mem_bytes() + (int64_t)M_ * 256 * dsub_ * 4 +
-         (d_table_ ? (int64_t)nlist_ * M_ * 256 * 4 : 0);
+  return IvfPqBase::index_mem_bytes() + (d_table_ ? (int64_t)nlist_ * M_ * 256 * 4 : 0);
 }
-int IVFPQIndex::rebuild_table(cudaStream_t st) {
+int IVFPQIndex::codebook_changed(cudaStream_t st) {
   pq_gen_++;  // the per-entry norm cache belongs to the previous codebook
   // tables of the tensor-core filter (kernels_pqtc.cu): fp16 codebook pre-scaled by -2 sb (L2) / -sb (IP), sb a power of two,
   // centroid norms, and the bound on |r| its error margin uses
@@ -1883,20 +1940,6 @@ int IVFPQIndex::rebuild_table(cudaStream_t st) {
   if (mp_.metric != kMetricL2) return 0;  // IP: tab = ip table, dis0 = <x, centroid>
   if (!d_table_) GB_CUDA(cudaMalloc(&d_table_, (size_t)nlist_ * M_ * 256 * 4));
   GB_CUDA(launch_pq_precompute_table(d_centroids_, dpad_, nlist_, d_pq_, M_, dsub_, d_table_, st));
-  return 0;
-}
-int IVFPQIndex::set_pq_centroids(const float* host) {
-  cudaSetDevice(device_);
-  std::unique_lock<std::shared_mutex> lk(mu_);
-  drain_searches();
-  GB_CUDA(cudaMemcpy(d_pq_, host, (size_t)M_ * 256 * dsub_ * 4, cudaMemcpyHostToDevice));
-  if (rebuild_table(build_stream_)) return -1;
-  GB_CUDA(cudaStreamSynchronize(build_stream_));
-  return 0;
-}
-int IVFPQIndex::get_pq_centroids(float* host) const {
-  cudaSetDevice(device_);
-  GB_CUDA(cudaMemcpy(host, d_pq_, (size_t)M_ * 256 * dsub_ * 4, cudaMemcpyDeviceToHost));
   return 0;
 }
 int IVFPQIndex::get_precomputed_table(float* host) const {
@@ -1912,69 +1955,24 @@ int IVFPQIndex::get_precomputed_table(float* host) const {
 // faiss IndexIVFPQ::train_residual restated: residuals of (a subsample of <= 256*ksub) training
 // vectors -> ProductQuantizer::train = M independent 256-means on the dsub-wide slices.
 int IVFPQIndex::train_extra(const float* xtrain, int64_t n, Scratch& s) {
-  cudaStream_t st = s.stream();
   if (d_ % M_ != 0) {
     set_last_error("dimension not divisible by nsubvector");
     return -1;
   }
-  int64_t npq = std::min<int64_t>(n, 256 * 256);
-  const float* xs = xtrain;
-  if (npq < n) {
-    std::vector<int32_t> perm;
-    rand_perm_mt(perm, n, 1234);
-    GB_ALLOC(d_idx, int32_t, npq, s);
-    GB_CUDA(cudaMemcpyAsync(d_idx, perm.data(), (size_t)npq * 4, cudaMemcpyHostToDevice, st));
-    GB_ALLOC(sub, float, (size_t)npq * dpad_, s);
-    GB_CUDA(launch_gather_rows(xtrain, dpad_, d_idx, npq, dpad_, sub, dpad_, st));
-    GB_CUDA(cudaStreamSynchronize(st));
-    xs = sub;
-  }
+  const int64_t npq = std::min<int64_t>(n, 256 * 256);
+  const float* xs;
+  if (subsample_rows(xtrain, n, npq, dpad_, &xs, s)) return -1;
   GB_ALLOC(assign, int32_t, npq, s);
   if (assign_dev(xs, dpad_, npq, assign, s)) return -1;
   GB_ALLOC(resid, float, (size_t)npq * dpad_, s);
-  GB_CUDA(launch_residual(xs, dpad_, npq, d_, d_centroids_, dpad_, assign, resid, dpad_, st));
-  const int dsp = (int)round_up(dsub_, 4);
-  GB_ALLOC(slice, float, (size_t)npq * dsp, s);
-  GB_ALLOC(cent, float, (size_t)256 * dsp, s);
-  KMeansParams kp;  // ClusteringParameters defaults: niter 25, seed 1234, max 256 points per centroid
-  for (int m = 0; m < M_; m++) {
-    GB_CUDA(launch_slice_cols(resid, dpad_, npq, m * dsub_, dsub_, slice, dsp, st));
-    if (kmeans_device(slice, dsp, npq, dsub_, 256, kp, cent, dsp, st, nullptr)) return -1;
-    GB_CUDA(cudaMemcpy2DAsync(d_pq_ + (size_t)m * 256 * dsub_, (size_t)dsub_ * 4, cent, (size_t)dsp * 4,
-                              (size_t)dsub_ * 4, 256, cudaMemcpyDeviceToDevice, st));
-  }
-  return rebuild_table(st);
+  GB_CUDA(launch_residual(xs, dpad_, npq, d_, d_centroids_, dpad_, assign, resid, dpad_, s.stream()));
+  return train_codebook(resid, npq, s);
 }
 
 // GammaIVFPQIndex::Add (gamma_index_ivfpq.cc:455-540): residual -> pq.compute_codes -> AddKeys
-int IVFPQIndex::append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
-                             const int32_t* d_assign, Scratch& s) {
-  cudaStream_t st = s.stream();
-  GB_ALLOC(codes, uint8_t, (size_t)n * M_, s);
-  // residual is taken w.r.t. the assigned list (d_list == d_assign except for skipped rows)
-  (void)d_assign;
-  GB_CUDA(launch_pq_encode(x, dpad_, n, d_centroids_, dpad_, d_list, d_pq_, M_, dsub_, codes, st));
-  GB_CUDA(launch_ivf_append_codes(codes, n, M_, d_list, d_pos, reinterpret_cast<uint8_t* const*>(lists_->d_data()),
-                                  lists_->d_ids(), vid0, st));
-  return 0;
-}
-
-int IVFPQIndex::encode_host(const float* x, int64_t n, const int64_t* assign, uint8_t* codes_out) {
-  cudaSetDevice(device_);
-  cudaStream_t st = thread_stream(device_);
-  Scratch s(st);
-  GB_ALLOC(dx, float, (size_t)n * dpad_, s);
-  GB_CUDA(cudaMemsetAsync(dx, 0, (size_t)n * dpad_ * 4, st));
-  GB_CUDA(cudaMemcpy2DAsync(dx, (size_t)dpad_ * 4, x, (size_t)d_ * 4, (size_t)d_ * 4, n, cudaMemcpyHostToDevice, st));
-  std::vector<int32_t> h(n);
-  for (int64_t i = 0; i < n; i++) h[i] = (int32_t)assign[i];
-  GB_ALLOC(da, int32_t, n, s);
-  GB_CUDA(cudaMemcpyAsync(da, h.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  GB_ALLOC(codes, uint8_t, (size_t)n * M_, s);
-  GB_CUDA(launch_pq_encode(dx, dpad_, n, d_centroids_, dpad_, da, d_pq_, M_, dsub_, codes, st));
-  GB_CUDA(cudaMemcpyAsync(codes_out, codes, (size_t)n * M_, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  return 0;
+cudaError_t IVFPQIndex::encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st) {
+  if (!lists) return cudaErrorInvalidValue;  // residual codes need each row's list
+  return launch_pq_encode(x, dpad_, n, d_centroids_, dpad_, lists, d_pq_, M_, dsub_, codes, st);
 }
 
 // Cache of |r_e|^2 per list entry for the tensor-core filter.  Searches hold mu_ shared, appends hold it exclusively and
@@ -2066,38 +2064,28 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   const int64_t max_groups = npairs / pq_group + nlist_;
   const int64_t max_items = max_groups * nseg;
   if (max_items > INT32_MAX) return 1;
-  GB_ALLOC(d_cnt, int32_t, nlist_, s);
-  GB_ALLOC(d_start, int32_t, nlist_, s);
-  GB_ALLOC(d_cursor, int32_t, nlist_, s);
-  GB_ALLOC(d_item_start, int32_t, nlist_, s);
-  GB_ALLOC(d_grp_start, int32_t, nlist_, s);
-  GB_ALLOC(d_totals, int64_t, 3, s);
-  GB_ALLOC(d_pair_j, int64_t, npairs, s);
-  GB_ALLOC(d_items, LmTile, max_items, s);
   GB_ALLOC(d_cand_cnt, int, nq, s);
   const size_t tile_bytes = (size_t)(d_ / 8) * 2048;
   const size_t a_bytes = (size_t)max_groups * 2 * tile_bytes;
   const size_t meta_bytes = (size_t)max_groups * pq_group * pqtc_pair_meta_bytes();
   const size_t cand_bytes = (size_t)nq * cap * 8;
-  unsigned char* big = static_cast<unsigned char*>(big_acquire(a_bytes + meta_bytes + cand_bytes, st));
-  if (!big) return -1;
-  auto rel_fn = [this, big, st](void*) { big_release(big, st); };
-  std::unique_ptr<void, decltype(rel_fn)> rel(big, rel_fn);
-  unsigned char* a_scratch = big;
-  void* meta = big + a_bytes;
-  unsigned long long* cand = reinterpret_cast<unsigned long long*>(big + a_bytes + meta_bytes);
+  BigScope big(this, a_bytes + meta_bytes + cand_bytes, st);
+  if (!big.p) return -1;
+  unsigned char* a_scratch = static_cast<unsigned char*>(big.p);
+  void* meta = a_scratch + a_bytes;
+  unsigned long long* cand = reinterpret_cast<unsigned long long*>(a_scratch + a_bytes + meta_bytes);
   stage_begin("pq_group_and_stage_pairs", st);
   GB_CUDA(cudaMemsetAsync(d_cand_cnt, 0, sizeof(int) * nq, st));
-  GB_CUDA(launch_lmk_group(d_probes_b, npairs, dir, nseg, pq_group, d_cnt, d_start, d_cursor, d_item_start, d_grp_start, d_totals,
-                           d_pair_j, d_items, st));
-  GB_CUDA(launch_pq_stage_pairs(xq, dpad_, d_, d_centroids_, dpad_, d_items, (int)max_items, d_totals, d_pair_j, nprobe,
+  LmGrouping g;
+  if (group_pairs_by_list(d_probes_b, npairs, nseg, pq_group, max_items, &g, s)) return -1;
+  GB_CUDA(launch_pq_stage_pairs(xq, dpad_, d_, d_centroids_, dpad_, g.items, (int)max_items, g.totals, g.pair_j, nprobe,
                                 coarse_dis, keysA, kk, kk, d_cbnrm_ + (size_t)M_ * 256, f, metric, a_scratch,
                                 meta, d_cand_cnt, cap, d_row_limit, st));
   stage_end(st);
   scan_timer_begin(st);  // the dominant kernel: the roofline in bench.py is this launch alone
   stage_begin("pqtc_scan_kernel", st);
-  GB_CUDA(launch_pqtc_scan(a_scratch, meta, d_cb16_, pqn_.base, pqn_.d_off, d_items, (int)max_items, d_totals, dir, M_, dsub_, f, metric,
-                           d_cand_cnt, cand, cap, nsm, st));
+  GB_CUDA(launch_pqtc_scan(a_scratch, meta, d_cb16_, pqn_.base, pqn_.d_off, g.items, (int)max_items, g.totals, dir, M_, dsub_, f,
+                           metric, d_cand_cnt, cand, cap, nsm, st));
   stage_end(st);
   scan_timer_end(st);
   stage_begin("pq_rescore_and_fallback", st);
@@ -2116,20 +2104,20 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
 }
 
 // Metric check, ADC depth, query-major list scan + merge of its CTA groups, exact re-rank
-int IVFFlatIndex::scan_pq_dev(const char* type, const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric,
-                              int nq, const float* rerank_xq, int k, int nprobe, unsigned long long* out_keys, Scratch& s,
-                              const std::function<int(int, unsigned long long*, bool)>& prepare,
-                              const std::function<cudaError_t(int, int, unsigned long long*)>& launch) {
+int IvfPqBase::scan_pq_dev(const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric, int nq,
+                           const float* rerank_xq, int k, int nprobe, unsigned long long* out_keys, Scratch& s,
+                           const std::function<int(int, unsigned long long*, bool)>& prepare,
+                           const std::function<cudaError_t(int, int, unsigned long long*)>& launch) {
   cudaStream_t st = s.stream();
   if (metric != mp_.metric) {
-    set_last_error(std::string(type) + ": per-request metric must equal the trained metric");
+    set_last_error(type_ + ": per-request metric must equal the trained metric");
     return -1;
   }
   // recall_num / re-rank semantics: gamma_index_ivfpq.cc:764-770
   const bool rerank = ctx.params.recall_num > 0;
   const int kk = std::max(k, ctx.params.recall_num);
   if (kk > 4096) {
-    set_last_error(std::string(type) + ": recall_num / topn above 4096 is not supported");
+    set_last_error(type_ + ": recall_num / topn above 4096 is not supported");
     return -1;
   }
   unsigned long long* keys = out_keys;
@@ -2167,9 +2155,9 @@ int IVFFlatIndex::scan_pq_dev(const char* type, const char* kernel, const Search
 }
 
 // GammaIVFPQIndex::search_preassigned (gamma_index_ivfpq.cc:730-947)
-int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
-                         const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
-                         Scratch& s) {
+int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq,
+                         const float* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
+                         unsigned long long* out_keys, Scratch& s) {
   cudaStream_t st = s.stream();
   float* ip = nullptr;
   auto prepare = [&](int kk, unsigned long long* keys, bool need_sorted) {
@@ -2188,110 +2176,30 @@ int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metr
                              partial, st);
   };
   // "for opq, rerank need raw vector" (gamma_index_ivfpq.cc:735): original queries against the raw store
-  return scan_pq_dev("IVFPQ", "ivfpq_scan_kernel", ctx, f, metric, nq, raw_queries_for(xq), k, nprobe, out_keys, s, prepare,
-                     launch);
-}
-
-int IVFPQIndex::search_preassigned_host(const SearchContext& ctx, int nq, const float* x, int k, const int64_t* keys,
-                                        const float* coarse_dis, int nprobe, float* out_dis, int64_t* out_ids) {
-  return IVFFlatIndex::search_preassigned_host(ctx, nq, x, k, keys, coarse_dis, nprobe, out_dis, out_ids);
+  return scan_pq_dev("ivfpq_scan_kernel", ctx, f, metric, nq, xq_raw, k, nprobe, out_keys, s, prepare, launch);
 }
 
 // ------------------------------------------------------------------------------------------
-IVFPQFastScanIndex::IVFPQFastScanIndex(int d, const ModelParams& mp, int device, int seg_shift)
-    : IVFFlatIndex(d, mp, device, seg_shift, "IVFPQFastScan"), M_(mp.nsubvector), dsub_(d / mp.nsubvector) {
-  cudaMalloc(&d_pq_, (size_t)M_ * kKsub * dsub_ * 4);
-  cudaMemset(d_pq_, 0, (size_t)M_ * kKsub * dsub_ * 4);
-}
-IVFPQFastScanIndex::~IVFPQFastScanIndex() { cudaFree(d_pq_); }
-int IVFPQFastScanIndex::training_threshold() const {
-  // gamma_index_ivfpqfs.cc: default nlist * 39; Indexing() clamps to [39, 256] * nlist like IVFPQ
-  int64_t t = mp_.training_threshold ? mp_.training_threshold : (int64_t)nlist_ * 39;
-  if (t < nlist_)
-    t = (int64_t)nlist_ * 39;
-  else if (t > (int64_t)nlist_ * 256)
-    t = (int64_t)nlist_ * 256;
-  return (int)t;
-}
-int64_t IVFPQFastScanIndex::index_mem_bytes() const { return IVFFlatIndex::index_mem_bytes() + (int64_t)M_ * kKsub * dsub_ * 4; }
-int IVFPQFastScanIndex::set_pq_centroids(const float* host) {
-  cudaSetDevice(device_);
-  std::unique_lock<std::shared_mutex> lk(mu_);
-  drain_searches();
-  GB_CUDA(cudaMemcpy(d_pq_, host, (size_t)M_ * kKsub * dsub_ * 4, cudaMemcpyHostToDevice));
-  return 0;
-}
-int IVFPQFastScanIndex::get_pq_centroids(float* host) const {
-  cudaSetDevice(device_);
-  GB_CUDA(cudaMemcpy(host, d_pq_, (size_t)M_ * kKsub * dsub_ * 4, cudaMemcpyDeviceToHost));
-  return 0;
-}
-int IVFPQFastScanIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
-  (void)dir;
-  (void)abs_name;
-  return 0;
-}
-int IVFPQFastScanIndex::load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) {
-  (void)dir;
-  (void)abs_name;
-  *load_num = 0;
-  return 0;
+// gamma_index_ivfpqfs.cc:95-104: IndexFlatL2 quantiser, spherical for IP, niter kept
+KMeansParams IVFPQFastScanIndex::coarse_kmeans_params() const {
+  KMeansParams kp;
+  kp.spherical = mp_.metric == kMetricIP;
+  kp.l2_assign = true;
+  return kp;
 }
 
 // faiss ProductQuantizer::train with ksub = 16 on the raw training vectors (by_residual = false): the same
 // sub-sampling rule as the 256-centroid IVFPQ codebook (at most 256 * ksub points), then M independent 16-means.
 int IVFPQFastScanIndex::train_extra(const float* xtrain, int64_t n, Scratch& s) {
-  cudaStream_t st = s.stream();
   const int64_t npq = std::min<int64_t>(n, 256 * kKsub);
-  const float* xs = xtrain;
-  if (npq < n) {
-    std::vector<int32_t> perm;
-    rand_perm_mt(perm, n, 1234);
-    GB_ALLOC(d_idx, int32_t, npq, s);
-    GB_CUDA(cudaMemcpyAsync(d_idx, perm.data(), (size_t)npq * 4, cudaMemcpyHostToDevice, st));
-    GB_ALLOC(sub, float, (size_t)npq * dpad_, s);
-    GB_CUDA(launch_gather_rows(xtrain, dpad_, d_idx, npq, dpad_, sub, dpad_, st));
-    GB_CUDA(cudaStreamSynchronize(st));
-    xs = sub;
-  }
-  const int dsp = (int)round_up(dsub_, 4);
-  GB_ALLOC(slice, float, (size_t)npq * dsp, s);
-  GB_ALLOC(cent, float, (size_t)kKsub * dsp, s);
-  KMeansParams kp;  // ClusteringParameters defaults: niter 25, seed 1234, max 256 points per centroid
-  for (int m = 0; m < M_; m++) {
-    GB_CUDA(launch_slice_cols(xs, dpad_, npq, m * dsub_, dsub_, slice, dsp, st));
-    if (kmeans_device(slice, dsp, npq, dsub_, kKsub, kp, cent, dsp, st, nullptr)) return -1;
-    GB_CUDA(cudaMemcpy2DAsync(d_pq_ + (size_t)m * kKsub * dsub_, (size_t)dsub_ * 4, cent, (size_t)dsp * 4, (size_t)dsub_ * 4,
-                              kKsub, cudaMemcpyDeviceToDevice, st));
-  }
-  return 0;
+  const float* xs;
+  if (subsample_rows(xtrain, n, npq, dpad_, &xs, s)) return -1;
+  return train_codebook(xs, npq, s);
 }
 
-int IVFPQFastScanIndex::append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
-                                     const int32_t* d_assign, Scratch& s) {
-  (void)d_assign;
-  cudaStream_t st = s.stream();
-  const int cb = code_bytes();
-  GB_ALLOC(codes, uint8_t, (size_t)n * cb, s);
-  GB_CUDA(launch_pqfs_encode(x, dpad_, n, d_pq_, M_, dsub_, codes, st));
-  GB_CUDA(launch_ivf_append_codes(codes, n, cb, d_list, d_pos, reinterpret_cast<uint8_t* const*>(lists_->d_data()),
-                                  lists_->d_ids(), vid0, st));
-  return 0;
-}
-
-int IVFPQFastScanIndex::encode_host(const float* x, int64_t n, uint8_t* codes_out) {
-  cudaSetDevice(device_);
-  cudaStream_t st = thread_stream(device_);
-  Scratch s(st);
-  const int cb = code_bytes();
-  GB_ALLOC(dx, float, (size_t)n * dpad_, s);
-  GB_CUDA(cudaMemsetAsync(dx, 0, (size_t)n * dpad_ * 4, st));
-  GB_CUDA(cudaMemcpy2DAsync(dx, (size_t)dpad_ * 4, x, (size_t)d_ * 4, (size_t)d_ * 4, n, cudaMemcpyHostToDevice, st));
-  GB_ALLOC(codes, uint8_t, (size_t)n * cb, s);
-  GB_CUDA(launch_pqfs_encode(dx, dpad_, n, d_pq_, M_, dsub_, codes, st));
-  GB_CUDA(cudaMemcpyAsync(codes_out, codes, (size_t)n * cb, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  return 0;
+cudaError_t IVFPQFastScanIndex::encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st) {
+  (void)lists;  // codes of the raw vectors
+  return launch_pqfs_encode(x, dpad_, n, d_pq_, M_, dsub_, codes, st);
 }
 
 int IVFPQFastScanIndex::lut_host(int nq, const float* x, int metric, uint8_t* lut8_out, float* ab_out) {
@@ -2299,8 +2207,7 @@ int IVFPQFastScanIndex::lut_host(int nq, const float* x, int metric, uint8_t* lu
   cudaStream_t st = thread_stream(device_);
   Scratch s(st);
   GB_ALLOC(dx, float, (size_t)nq * dpad_, s);
-  GB_CUDA(cudaMemsetAsync(dx, 0, (size_t)nq * dpad_ * 4, st));
-  GB_CUDA(cudaMemcpy2DAsync(dx, (size_t)dpad_ * 4, x, (size_t)d_ * 4, (size_t)d_ * 4, nq, cudaMemcpyHostToDevice, st));
+  GB_CUDA(upload_rows_padded(dx, x, nq, d_, dpad_, st));
   GB_ALLOC(lut, uint8_t, (size_t)nq * M_ * kKsub, s);
   GB_ALLOC(ab, float, (size_t)nq * 2, s);
   GB_CUDA(launch_pqfs_lut(dx, dpad_, nq, d_pq_, M_, dsub_, metric >= 0 ? metric : mp_.metric, lut, ab, st));
@@ -2312,9 +2219,9 @@ int IVFPQFastScanIndex::lut_host(int nq, const float* x, int metric, uint8_t* lu
 
 // IndexIVFFastScan::search_preassigned restated over this engine's lists, filters applied before selection;
 // recall_num > 0 re-ranks the recall_num best exactly from the raw vectors, as IVFPQ does
-int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
-                                 const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
-                                 Scratch& s) {
+int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq,
+                                 const float* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
+                                 unsigned long long* out_keys, Scratch& s) {
   (void)coarse_dis;  // no residual: the list's coarse distance takes no part in the score
   cudaStream_t st = s.stream();
   uint8_t* lut = nullptr;
@@ -2330,7 +2237,7 @@ int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, 
   auto launch = [&](int kk, int pg, unsigned long long* partial) {
     return launch_ivfpqfs_scan(lut, ab, nq, probe_ids, nprobe, pg, lists_->directory(), M_, kk, metric, f, partial, st);
   };
-  return scan_pq_dev("IVFPQFastScan", "ivfpqfs_scan_kernel", ctx, f, metric, nq, xq, k, nprobe, out_keys, s, prepare, launch);
+  return scan_pq_dev("ivfpqfs_scan_kernel", ctx, f, metric, nq, xq_raw, k, nprobe, out_keys, s, prepare, launch);
 }
 
 // ------------------------------------------------------------------------------------------

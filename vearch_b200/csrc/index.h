@@ -284,6 +284,15 @@ class Index {
   };
   std::mutex big_mu_;
   std::vector<BigBuf> big_;
+  struct BigScope {  // a big_acquire'd buffer (p, nullptr on failure), released event-stamped on every exit path
+    Index* ix;
+    cudaStream_t st;
+    void* p;
+    BigScope(Index* i, size_t bytes, cudaStream_t s) : ix(i), st(s), p(i->big_acquire(bytes, s)) {}
+    ~BigScope() {
+      if (p) ix->big_release(p, st);
+    }
+  };
   void scan_timer_begin(cudaStream_t st);
   void scan_timer_end(cudaStream_t st);
   // per-stage device times (bench breakdown): CUDA events on the launching stream around each stage of a
@@ -331,10 +340,21 @@ struct KMeansParams {
 int kmeans_device(const float* x, int64_t ldx, int64_t n, int d, int k, const KMeansParams& kp, float* centroids,
                   int64_t ldc, cudaStream_t st, std::vector<float>* obj);
 
-class IVFFlatIndex : public Index {
+// What an IVF index's codec puts into gamma's index file (index_io.cu)
+struct GammaFileFormat {
+  const char* file = nullptr;  // <dir>/<abs_name>/<file>; nullptr: the reference writes no index file for this type
+  uint32_t magic = 0;          // faiss fourcc of the index
+  uint64_t code_size = 0;      // bytes per list entry on disk (in memory: code_bytes(), rows padded when they differ)
+  bool indexed_count = false;  // an i32 indexed_count follows the lists
+};
+
+// The inverted-file skeleton shared by every IVF type: coarse centroids, inverted lists, train / add / update / reset /
+// compact, coarse search, and the gamma index-file skeleton.  A codec derived from it says how vectors become list
+// entries (append_batch, code_bytes) and how a query scans the probed lists (scan_dev).
+class IvfIndex : public Index {
  public:
-  IVFFlatIndex(int d, const ModelParams& mp, int device, int seg_shift, const std::string& type = "IVFFLAT");
-  ~IVFFlatIndex() override;
+  IvfIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift);
+  ~IvfIndex() override;
   int training_threshold() const override;
   int train() override;
   int add_pending(const uint8_t* del_bitmap) override;
@@ -342,6 +362,7 @@ class IVFFlatIndex : public Index {
   int reset_index() override;
   int64_t index_mem_bytes() const override;
   int nlist() const { return nlist_; }
+  virtual int code_bytes() const = 0;  // bytes per list entry
   // parity hooks: exchange index state with the oracle
   int set_centroids(const float* host, int nlist);  // marks trained
   int get_centroids(float* host) const;
@@ -349,45 +370,51 @@ class IVFFlatIndex : public Index {
   // quantizer->search (ivfflat.cc:568): top-nprobe lists per query
   int coarse_search_host(int nq, const float* x, int nprobe, float* out_dis, int64_t* out_ids);
   // search_preassigned with caller-provided (keys, coarse_dis): host in/out
-  virtual int search_preassigned_host(const SearchContext& ctx, int nq, const float* x, int k, const int64_t* keys,
-                                      const float* coarse_dis, int nprobe, float* out_dis, int64_t* out_ids);
-  // gamma's own index files (index_io.cu): <dir>/<abs_name>/{ivfflat,ivfpq}.index.  load: the vector
-  // store must already hold the vectors the file indexes; *load_num = IndexModel::Load's load_num
+  int search_preassigned_host(const SearchContext& ctx, int nq, const float* x, int k, const int64_t* keys,
+                              const float* coarse_dis, int nprobe, float* out_dis, int64_t* out_ids);
   // re-pack the inverted lists into one tight slab (IvfLists::compact); also done automatically after
   // a bulk add_pending when more than half of the slab space is dead
   int compact_lists();
-  int mirror_builds() const { return mirror_.builds; }  // test hook
-  virtual int dump_gamma(const std::string& dir, const std::string& abs_name);
-  virtual int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num);
+  // gamma's own index files (index_io.cu): <dir>/<abs_name>/<gamma_format().file>.  load: the vector
+  // store must already hold the vectors the file indexes; *load_num = IndexModel::Load's load_num
+  int dump_gamma(const std::string& dir, const std::string& abs_name);
+  int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num);
 
  protected:
-  virtual const char* gamma_file_name() const;
+  virtual GammaFileFormat gamma_format() const = 0;
+  // codec blocks after the coarse quantiser (product quantizer, OPQ)
   virtual int dump_gamma_extra(FILE* f) { (void)f; return 0; }
   virtual int load_gamma_extra(FILE* f) { (void)f; return 0; }
+  // the reference's default training_threshold of the type; training_threshold() clamps it to [39, 256] * nlist
+  virtual int64_t default_training_threshold() const = 0;
+  // k-means of the coarse centroids (default: faiss ClusteringParameters)
+  virtual KMeansParams coarse_kmeans_params() const { return KMeansParams(); }
   int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
                       unsigned long long* out_keys, Scratch& s) override;
   int coarse_dev(int nq, const float* xq, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis, Scratch& s);
-  virtual int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
-                       const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
-                       Scratch& s);
-  // scan_dev of the PQ-coded indexes (IVFPQ, IVFPQFastScan) through the query-major list scan: `prepare(kk, keys,
-  // need_sorted)` builds the per-query tables and may serve the scan another way (0 = served, 1 = not, < 0 = error);
-  // `launch(kk, pg, partial)` launches the scan kernel, named `kernel`, over pg probes per CTA
-  int scan_pq_dev(const char* type, const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric, int nq,
-                  const float* rerank_xq, int k, int nprobe, unsigned long long* out_keys, Scratch& s,
-                  const std::function<int(int, unsigned long long*, bool)>& prepare,
-                  const std::function<cudaError_t(int, int, unsigned long long*)>& launch);
-  // list-major IVF-Flat scan on the tensor cores (kernels_tc.cu); returns 1 if not applicable
-  int scan_listmajor_dev(const FilterArgs& f, int metric, int nq, const float* xq, int k, const int32_t* probe_ids,
-                         int nprobe, unsigned long long* out_keys, Scratch& s);
+  // xq: the queries after transform_dev; xq_raw: the same queries untransformed (the exact re-rank reads the raw store)
+  virtual int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq,
+                       const float* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
+                       unsigned long long* out_keys, Scratch& s) = 0;
+  // List-major pair grouping (launch_lmk_group): the (query, probe) pairs grouped by list, `group` pairs per group, each
+  // group cut into nseg row segments.  Items, pair order and totals are left in `s` for the list-major kernels.
+  struct LmGrouping {
+    int64_t* totals;
+    int64_t* pair_j;
+    LmTile* items;
+  };
+  int group_pairs_by_list(const int32_t* probe_ids, int64_t npairs, int nseg, int group, int64_t max_items, LmGrouping* g,
+                          Scratch& s);
   int assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* assign_dev_out, Scratch& s);
   int resolve_nprobe(const SearchContext& ctx) const;
   // metric of the coarse quantiser (list assignment and probe choice) for a search under `metric`
   virtual int coarse_metric(int metric) const { return metric; }
-  virtual int code_bytes() const { return dpad_ * 4; }
+  // write rows x [vid0, vid0+n) into the lists at (d_list, d_pos), after reserve and before commit; add[l] = rows for list l
   virtual int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
-                           const int32_t* d_assign, Scratch& s);
+                           const std::vector<int>& add, Scratch& s) = 0;
   virtual int train_extra(const float* xtrain, int64_t n, Scratch& s) { (void)xtrain; (void)n; (void)s; return 0; }
+  // codec state dropped by reset_index, with build_mu_ and mu_ held exclusively
+  virtual void reset_codec() {}
   // vector transform in front of the index (OPQ, gamma_index_ivfpq.cc:362-364, 422, 470, 585-590): applied to the
   // training slab (which also trains it), to vectors on their way into the lists and to queries; the raw store
   // and the exact re-rank keep the original vectors.  Default: identity (returns x).
@@ -406,8 +433,31 @@ class IVFFlatIndex : public Index {
   int rebuild_centroid_tiles(cudaStream_t st);
   std::unique_ptr<IvfLists> lists_;
   std::vector<uint64_t> vid2pos_;  // vid -> (list << 32 | pos), ~0 = not in a list (vid_bucket_no_pos_)
+};
 
-  // Tensor-core mirror of the lists (IVFFLAT only; kernels_tc.cu): every list once more, pre-split and
+// GammaIVFFlatIndex (index/impl/gamma_index_ivfflat.{h,cc}): the lists hold the raw fp32 rows
+class IVFFlatIndex : public IvfIndex {
+ public:
+  IVFFlatIndex(int d, const ModelParams& mp, int device, int seg_shift) : IvfIndex("IVFFLAT", d, mp, device, seg_shift) {}
+  ~IVFFlatIndex() override;
+  int64_t index_mem_bytes() const override;
+  int code_bytes() const override { return dpad_ * 4; }
+  int mirror_builds() const { return mirror_.builds; }  // test hook
+
+ protected:
+  GammaFileFormat gamma_format() const override;
+  int64_t default_training_threshold() const override { return (int64_t)nlist_ * 200; }  // gamma_index_ivfflat.cc:239
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, const float* xq_raw, int k,
+               const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
+               Scratch& s) override;
+  // list-major IVF-Flat scan on the tensor cores (kernels_tc.cu); returns 1 if not applicable
+  int scan_listmajor_dev(const FilterArgs& f, int metric, int nq, const float* xq, int k, const int32_t* probe_ids,
+                         int nprobe, unsigned long long* out_keys, Scratch& s);
+  int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                   const std::vector<int>& add, Scratch& s) override;
+  void reset_codec() override;
+
+  // Tensor-core mirror of the lists (kernels_tc.cu): every list once more, pre-split and
   // pre-tiled in the shared-memory operand layout so the list-major kernel is fed by cp.async.bulk.
   // Built by the first list-major search, kept current in place by appends that fit its reserve,
   // rebuilt when a list outgrows it; users hold mirror_rw_ shared from the freshness check until their
@@ -427,45 +477,67 @@ class IVFFlatIndex : public Index {
   // next list-major search rebuilds it
   int mirror_append(const float* x, int64_t n, const int32_t* d_list, const int32_t* d_pos, const std::vector<int>& add,
                     cudaStream_t st);
-  std::shared_mutex mirror_rw_;
+  std::shared_mutex mirror_rw_;  // taken after mu_
   int ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStream_t st);  // 0 = usable and current
 };
 
-class IVFPQIndex : public IVFFlatIndex {
+// Product-quantiser base of IVFPQ and IVFPQFastScan: M sub-quantisers of ksub centroids each over dsub-wide slices, the
+// codebook [M][ksub][dsub], its training, the encode path into the lists and the query-major list-scan search path.
+class IvfPqBase : public IvfIndex {
  public:
-  IVFPQIndex(int d, const ModelParams& mp, int device, int seg_shift);
-  ~IVFPQIndex() override;
-  int training_threshold() const override;
+  IvfPqBase(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int M, int ksub);
+  ~IvfPqBase() override;
   int64_t index_mem_bytes() const override;
   int M() const { return M_; }
   int dsub() const { return dsub_; }
-  int set_pq_centroids(const float* host);  // [M][256][dsub]; rebuilds the precomputed table
+  int ksub() const { return ksub_; }
+  int set_pq_centroids(const float* host);  // [M][ksub][dsub]; runs codebook_changed
   int get_pq_centroids(float* host) const;
-  int get_precomputed_table(float* host) const;
+  // list codes of n host rows; assign: each row's list (residual codecs), may be null otherwise
   int encode_host(const float* x, int64_t n, const int64_t* assign, uint8_t* codes_out);
-  int search_preassigned_host(const SearchContext& ctx, int nq, const float* x, int k, const int64_t* keys,
-                              const float* coarse_dis, int nprobe, float* out_dis, int64_t* out_ids) override;
 
  protected:
-  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
+  // codes of n device rows (stride dpad) into codes [n][code_bytes()]; lists: each row's list (residual codecs)
+  virtual cudaError_t encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st) = 0;
+  // tables derived from the codebook, rebuilt after every change of it
+  virtual int codebook_changed(cudaStream_t st) { (void)st; return 0; }
+  int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                   const std::vector<int>& add, Scratch& s) override;
+  // faiss ProductQuantizer::train on n rows (stride dpad): M independent ksub-means on the dsub-wide slices
+  int train_codebook(const float* x, int64_t n, Scratch& s);
+  // scan_dev of the PQ-coded indexes through the query-major list scan: `prepare(kk, keys, need_sorted)` builds the
+  // per-query tables and may serve the scan another way (0 = served, 1 = not, < 0 = error); `launch(kk, pg, partial)`
+  // launches the scan kernel, named `kernel`, over pg probes per CTA
+  int scan_pq_dev(const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* rerank_xq,
+                  int k, int nprobe, unsigned long long* out_keys, Scratch& s,
+                  const std::function<int(int, unsigned long long*, bool)>& prepare,
+                  const std::function<cudaError_t(int, int, unsigned long long*)>& launch);
+
+  int M_, dsub_, ksub_;
+  float* d_pq_ = nullptr;  // [M][ksub][dsub]
+};
+
+class IVFPQIndex : public IvfPqBase {
+ public:
+  IVFPQIndex(int d, const ModelParams& mp, int device, int seg_shift);
+  ~IVFPQIndex() override;
+  int64_t index_mem_bytes() const override;
+  int code_bytes() const override { return M_; }
+  int get_precomputed_table(float* host) const;
+
+ protected:
+  GammaFileFormat gamma_format() const override;
+  int64_t default_training_threshold() const override;
+  KMeansParams coarse_kmeans_params() const override;
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, const float* xq_raw, int k,
                const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
                Scratch& s) override;
-  int code_bytes() const override { return M_; }
-  const char* gamma_file_name() const override;
-
- public:
-  int reset_index() override {
-    opq_trained_ = false;
-    return IVFFlatIndex::reset_index();
-  }
-
- protected:
+  void reset_codec() override { opq_trained_ = false; }
   int dump_gamma_extra(FILE* f) override;
   int load_gamma_extra(FILE* f) override;
-  int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
-                   const int32_t* d_assign, Scratch& s) override;
+  cudaError_t encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st) override;
   int train_extra(const float* xtrain, int64_t n, Scratch& s) override;
-  int rebuild_table(cudaStream_t st);
+  int codebook_changed(cudaStream_t st) override;
   // list-major scan through the tensor-core filter (kernels_pqtc.cu); 1 = not applicable
   int scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const float* xq, int kk, const float* ip,
                         const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* adc_out,
@@ -474,8 +546,6 @@ class IVFPQIndex : public IVFFlatIndex {
   const float* train_transform(const float* xt, int64_t n, Scratch& s) override;
   const float* transform_dev(const float* x, int64_t n, Scratch& s) override;
 
-  int M_, dsub_;
-  float* d_pq_ = nullptr;     // [M][256][dsub]
   float* d_table_ = nullptr;  // [nlist][M][256] (L2 only)
   uint16_t* d_cb16_ = nullptr;  // [M][256][dsub] fp16, pre-scaled (tensor-core filter)
   float* d_cbnrm_ = nullptr;    // [M][256] |pq|^2, then rmax2, sb
@@ -504,40 +574,34 @@ class IVFPQIndex : public IVFFlatIndex {
 // GammaIVFPQFastScanIndex (index/impl/gamma_index_ivfpqfs.{h,cc}): faiss::IndexIVFPQFastScan with by_residual = false.
 // The lists hold 4-bit codes of the raw vectors (16-centroid PQ, two codes per byte); a search quantises each query's
 // M x 16 table to uint8 and sums it in integers.  The coarse quantiser is IndexFlatL2 under either metric.
-class IVFPQFastScanIndex : public IVFFlatIndex {
+class IVFPQFastScanIndex : public IvfPqBase {
  public:
   static constexpr int kKsub = 16;
-  IVFPQFastScanIndex(int d, const ModelParams& mp, int device, int seg_shift);
-  ~IVFPQFastScanIndex() override;
-  int training_threshold() const override;
-  int64_t index_mem_bytes() const override;
-  int M() const { return M_; }
-  int dsub() const { return dsub_; }
+  IVFPQFastScanIndex(int d, const ModelParams& mp, int device, int seg_shift)
+      : IvfPqBase("IVFPQFastScan", d, mp, device, seg_shift, mp.nsubvector, kKsub) {}
+  int code_bytes() const override { return (M_ + 1) / 2; }
   // M above this: faiss's 16-bit table sums could wrap (255 * 257 < 2^16), and the byte-pair table grows past what
   // the scan's shared memory holds beside its stages and queue
   static constexpr int kMaxM = 256;
   bool persists_trained_state() const override { return false; }
-  int set_pq_centroids(const float* host);  // [M][16][dsub]
-  int get_pq_centroids(float* host) const;
-  int encode_host(const float* x, int64_t n, uint8_t* codes_out);  // n x ceil(M/2) packed codes
   // uint8 tables [nq][M][16] and (a, b) [nq][2] of a query batch under `metric` (-1: the index metric)
   int lut_host(int nq, const float* x, int metric, uint8_t* lut8_out, float* ab_out);
-  // the reference dumps no index file: a loaded table trains and fills this index again from its raw vectors
-  int dump_gamma(const std::string& dir, const std::string& abs_name) override;
-  int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) override;
 
  protected:
+  // the reference dumps no index file: a loaded table trains and fills this index again from its raw vectors
+  GammaFileFormat gamma_format() const override { return GammaFileFormat(); }
+  int64_t default_training_threshold() const override { return (int64_t)nlist_ * 39; }  // gamma_index_ivfpqfs.cc
+  KMeansParams coarse_kmeans_params() const override;
   int coarse_metric(int metric) const override { (void)metric; return kMetricL2; }
-  int code_bytes() const override { return (M_ + 1) / 2; }
+  cudaError_t encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st) override;
   int train_extra(const float* xtrain, int64_t n, Scratch& s) override;
-  int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
-                   const int32_t* d_assign, Scratch& s) override;
-  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, const float* xq_raw, int k,
                const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
                Scratch& s) override;
-  int M_, dsub_;
-  float* d_pq_ = nullptr;  // [M][16][dsub]
 };
+
+// host rows n x d (stride d) -> device rows n x dpad, the padding columns zeroed
+cudaError_t upload_rows_padded(float* dst, const float* src, int64_t n, int d, int dpad, cudaStream_t st);
 
 // reflector (index/reflector.h:68-80): type name -> index object
 Index* create_index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift);

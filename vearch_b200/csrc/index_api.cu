@@ -141,6 +141,11 @@ static int fill_ctx(SearchContext* ctx, const char* rp_json, int brute_force, co
     return -1;                           \
   }
 
+template <class T>
+static T* as(gb_index* index) {
+  return index && index->impl ? dynamic_cast<T*>(index->impl) : nullptr;
+}
+
 extern "C" {
 
 const char* gb_last_error(void) { return last_error(); }
@@ -277,30 +282,14 @@ const char* gb_index_last_scan_kernel(gb_index* index) {
 const char* gb_index_last_scan_info(gb_index* index) { return index && index->impl ? index->impl->last_scan_info() : "{}"; }
 float gb_index_last_scan_ms(gb_index* index) { return index && index->impl ? index->impl->last_scan_ms() : 0.f; }
 
-static IVFFlatIndex* as_ivf(gb_index* index) {
-  if (!index || !index->impl) return nullptr;
-  return dynamic_cast<IVFFlatIndex*>(index->impl);
-}
-static IVFPQIndex* as_pq(gb_index* index) {
-  if (!index || !index->impl) return nullptr;
-  return dynamic_cast<IVFPQIndex*>(index->impl);
-}
-static IVFPQFastScanIndex* as_pqfs(gb_index* index) {
-  if (!index || !index->impl) return nullptr;
-  return dynamic_cast<IVFPQFastScanIndex*>(index->impl);
-}
-#define IVF_OR_FAIL(v, index)                \
-  IVFFlatIndex* v = as_ivf(index);           \
-  if (!v) {                                  \
-    set_last_error("not an IVF index");      \
-    return -1;                               \
+#define AS_OR_FAIL(T, v, index, what)          \
+  T* v = as<T>(index);                         \
+  if (!v) {                                    \
+    set_last_error("not an " what " index");   \
+    return -1;                                 \
   }
-#define PQ_OR_FAIL(v, index)                 \
-  IVFPQIndex* v = as_pq(index);              \
-  if (!v) {                                  \
-    set_last_error("not an IVFPQ index");    \
-    return -1;                               \
-  }
+#define IVF_OR_FAIL(v, index) AS_OR_FAIL(IvfIndex, v, index, "IVF")
+#define PQ_OR_FAIL(v, index) AS_OR_FAIL(IvfPqBase, v, index, "IVFPQ")
 
 int gb_index_nlist(gb_index* index) {
   IVF_OR_FAIL(ivf, index);
@@ -315,77 +304,69 @@ int gb_index_get_centroids(gb_index* index, float* centroids) {
   return ivf->get_centroids(centroids);
 }
 int gb_index_pq_m(gb_index* index) {
-  if (IVFPQFastScanIndex* fs = as_pqfs(index)) return fs->M();
   PQ_OR_FAIL(pq, index);
   return pq->M();
 }
 int gb_index_pq_ksub(gb_index* index) {
-  if (as_pqfs(index)) return IVFPQFastScanIndex::kKsub;
   PQ_OR_FAIL(pq, index);
-  return 256;
+  return pq->ksub();
 }
 int gb_index_set_pq_centroids(gb_index* index, const float* pqc) {
-  if (IVFPQFastScanIndex* fs = as_pqfs(index)) return fs->set_pq_centroids(pqc);
   PQ_OR_FAIL(pq, index);
   return pq->set_pq_centroids(pqc);
 }
 int gb_index_get_pq_centroids(gb_index* index, float* pqc) {
-  if (IVFPQFastScanIndex* fs = as_pqfs(index)) return fs->get_pq_centroids(pqc);
   PQ_OR_FAIL(pq, index);
   return pq->get_pq_centroids(pqc);
 }
 int gb_index_pqfs_lut(gb_index* index, int nq, const float* x, int metric, uint8_t* lut8, float* ab) {
-  IVFPQFastScanIndex* fs = as_pqfs(index);
-  if (!fs) {
-    set_last_error("not an IVFPQFastScan index");
-    return -1;
-  }
+  AS_OR_FAIL(IVFPQFastScanIndex, fs, index, "IVFPQFastScan");
   return fs->lut_host(nq, x, metric, lut8, ab);
 }
 int gb_index_get_precomputed_table(gb_index* index, float* table) {
-  PQ_OR_FAIL(pq, index);
+  AS_OR_FAIL(IVFPQIndex, pq, index, "IVFPQ");
   return pq->get_precomputed_table(table);
 }
 int gb_index_has_opq(gb_index* index) {
-  IVFPQIndex* pq = index && index->impl ? dynamic_cast<IVFPQIndex*>(index->impl) : nullptr;
+  IVFPQIndex* pq = as<IVFPQIndex>(index);
   return pq && pq->has_opq() ? 1 : 0;
 }
 int gb_index_set_opq(gb_index* index, const float* A) {
   IDX_OR_FAIL(index);
-  IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(index->impl);
+  IVFPQIndex* pq = as<IVFPQIndex>(index);
   return pq ? pq->set_opq(A) : -1;
 }
 int gb_index_get_opq(gb_index* index, float* A) {
   IDX_OR_FAIL(index);
-  IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(index->impl);
+  IVFPQIndex* pq = as<IVFPQIndex>(index);
   return pq ? pq->get_opq(A) : -1;
 }
 int gb_index_apply_opq(gb_index* index, int64_t n, const float* x, float* out) {
   IDX_OR_FAIL(index);
-  IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(index->impl);
+  IVFPQIndex* pq = as<IVFPQIndex>(index);
   return pq ? pq->apply_opq_host(x, n, out) : -1;
 }
 int gb_index_mirror_builds(gb_index* index) {
   if (!index || !index->impl) return -1;
-  IVFFlatIndex* ivf = dynamic_cast<IVFFlatIndex*>(index->impl);
+  IVFFlatIndex* ivf = as<IVFFlatIndex>(index);
   return ivf ? ivf->mirror_builds() : 0;
 }
 int gb_index_compact(gb_index* index) {
   IDX_OR_FAIL(index);
-  IVFFlatIndex* ivf = dynamic_cast<IVFFlatIndex*>(index->impl);
+  IvfIndex* ivf = as<IvfIndex>(index);
   return ivf ? ivf->compact_lists() : 0;
 }
 int gb_index_dump(gb_index* index, const char* dir, const char* abs_name) {
   IDX_OR_FAIL(index);
   if (!dir || !abs_name) return -1;
-  IVFFlatIndex* ivf = dynamic_cast<IVFFlatIndex*>(index->impl);
+  IvfIndex* ivf = as<IvfIndex>(index);
   return ivf ? ivf->dump_gamma(dir, abs_name) : 0;
 }
 int gb_index_load(gb_index* index, const char* dir, const char* abs_name, int64_t* load_num) {
   IDX_OR_FAIL(index);
   if (!dir || !abs_name || !load_num) return -1;
   *load_num = 0;
-  IVFFlatIndex* ivf = dynamic_cast<IVFFlatIndex*>(index->impl);
+  IvfIndex* ivf = as<IvfIndex>(index);
   return ivf ? ivf->load_gamma(dir, abs_name, load_num) : 0;
 }
 int gb_index_list_len(gb_index* index, int list) {
@@ -395,9 +376,7 @@ int gb_index_list_len(gb_index* index, int list) {
 }
 int gb_index_code_size(gb_index* index) {
   IVF_OR_FAIL(ivf, index);
-  IVFPQIndex* pq = as_pq(index);
-  if (IVFPQFastScanIndex* fs = as_pqfs(index)) return (fs->M() + 1) / 2;
-  return pq ? pq->M() : ((ivf->d() + 3) / 4 * 4) * 4;
+  return ivf->code_bytes();
 }
 int gb_index_get_list(gb_index* index, int list, uint8_t* codes, int64_t* ids) {
   IVF_OR_FAIL(ivf, index);
@@ -430,7 +409,6 @@ int gb_index_search_preassigned(gb_index* index, int nq, const float* x, int k, 
   return ivf->search_preassigned_host(ctx, nq, x, k, keys, coarse_dis, nprobe, out_scores, out_ids);
 }
 int gb_index_pq_encode(gb_index* index, int64_t n, const float* x, const int64_t* assign, uint8_t* codes) {
-  if (IVFPQFastScanIndex* fs = as_pqfs(index)) return fs->encode_host(x, n, codes);
   PQ_OR_FAIL(pq, index);
   return pq->encode_host(x, n, assign, codes);
 }
@@ -449,10 +427,8 @@ int gb_kmeans(int device, const float* x, int64_t n, int d, int k, int niter, in
     const int dpad = (d + 3) / 4 * 4;
     float* dx = s.alloc_n<float>((size_t)n * dpad);
     float* dc = s.alloc_n<float>((size_t)k * dpad);
-    if (dx && dc && cudaMemsetAsync(dx, 0, (size_t)n * dpad * 4, st) == cudaSuccess &&
-        cudaMemsetAsync(dc, 0, (size_t)k * dpad * 4, st) == cudaSuccess &&
-        cudaMemcpy2DAsync(dx, (size_t)dpad * 4, x, (size_t)d * 4, (size_t)d * 4, n, cudaMemcpyHostToDevice, st) ==
-            cudaSuccess) {
+    if (dx && dc && cudaMemsetAsync(dc, 0, (size_t)k * dpad * 4, st) == cudaSuccess &&
+        upload_rows_padded(dx, x, n, d, dpad, st) == cudaSuccess) {
       KMeansParams kp;
       kp.niter = niter;
       kp.seed = seed;
@@ -495,8 +471,7 @@ int gb_kmeans_update(int device, const float* x, int64_t n, int d, int k, const 
     cur[c] = off[c];
   }
   for (int64_t i = 0; i < n; i++) perm[cur[assign[i]]++] = (int32_t)i;
-  GB_CUDA(cudaMemsetAsync(dx, 0, (size_t)n * dpad * 4, st));
-  GB_CUDA(cudaMemcpy2DAsync(dx, (size_t)dpad * 4, x, (size_t)d * 4, (size_t)d * 4, n, cudaMemcpyHostToDevice, st));
+  GB_CUDA(upload_rows_padded(dx, x, n, d, dpad, st));
   GB_CUDA(cudaMemcpyAsync(dperm, perm.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemcpyAsync(doff, off.data(), (size_t)(k + 1) * 4, cudaMemcpyHostToDevice, st));
   GB_CUDA(launch_segment_mean(dx, dpad, d, dperm, doff, k, dc, dpad, st));
@@ -520,10 +495,8 @@ int gb_debug_dist_matrix(int device, const float* x, int n, const float* c, int 
   float* dc = s.alloc_n<float>((size_t)m * dpad);
   float* dout = s.alloc_n<float>((size_t)n * ldo);
   if (!dx || !dc || !dout) return -1;
-  GB_CUDA(cudaMemsetAsync(dx, 0, (size_t)n * dpad * 4, st));
-  GB_CUDA(cudaMemsetAsync(dc, 0, (size_t)m * dpad * 4, st));
-  GB_CUDA(cudaMemcpy2DAsync(dx, (size_t)dpad * 4, x, (size_t)d * 4, (size_t)d * 4, n, cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemcpy2DAsync(dc, (size_t)dpad * 4, c, (size_t)d * 4, (size_t)d * 4, m, cudaMemcpyHostToDevice, st));
+  GB_CUDA(upload_rows_padded(dx, x, n, d, dpad, st));
+  GB_CUDA(upload_rows_padded(dc, c, m, d, dpad, st));
   if (use_tc) {
     GB_CUDA(launch_dist_matrix_tc(dx, dpad, n, dc, dpad, m, dpad, metric, dout, ldo, st));
   } else {

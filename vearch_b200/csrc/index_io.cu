@@ -86,23 +86,24 @@ int fail(const std::string& msg) {
 
 }  // namespace
 
-const char* IVFFlatIndex::gamma_file_name() const { return "ivfflat.index"; }
-const char* IVFPQIndex::gamma_file_name() const { return "ivfpq.index"; }
+// IVF-Flat rows are padded to a multiple of 4 floats here; gamma's are not
+GammaFileFormat IVFFlatIndex::gamma_format() const { return {"ivfflat.index", fourcc("IvFl"), (uint64_t)d_ * 4, true}; }
+GammaFileFormat IVFPQIndex::gamma_format() const { return {"ivfpq.index", fourcc("IwPQ"), (uint64_t)code_bytes(), false}; }
 
 // ---- Dump -----------------------------------------------------------------------------------
-int IVFFlatIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
-  if (!trained_) return 0;  // "gamma index is not trained, skip dumping" (ivfflat.cc:808-811)
+int IvfIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
+  const GammaFileFormat gf = gamma_format();
+  if (!trained_ || !gf.file) return 0;  // "gamma index is not trained, skip dumping" (ivfflat.cc:808-811)
   std::lock_guard<std::mutex> bg(build_mu_);  // no list mutation while the lists are copied out
   cudaSetDevice(device_);
   const std::string index_dir = dir + "/" + abs_name;
   mkdir(dir.c_str(), 0755);
   if (mkdir(index_dir.c_str(), 0755) && errno != EEXIST) return fail("mkdir error, index dir=" + index_dir);
-  const std::string path = index_dir + "/" + gamma_file_name();
+  const std::string path = index_dir + "/" + gf.file;
   FilePtr fp(fopen(path.c_str(), "wb"));
   FILE* f = fp.get();
   if (!f) return fail("cannot open " + path);
-  const bool is_pq = type_ != "IVFFLAT";
-  bool ok = wr<uint32_t>(f, is_pq ? fourcc("IwPQ") : fourcc("IvFl"));
+  bool ok = wr<uint32_t>(f, gf.magic);
   // write_ivf_header (index_io.cc:41-47)
   ok = ok && wr_index_header(f, d_, indexed_count_, mp_.metric);
   ok = ok && wr<uint64_t>(f, (uint64_t)nlist_) && wr<uint64_t>(f, (uint64_t)mp_.nprobe);
@@ -115,7 +116,7 @@ int IVFFlatIndex::dump_gamma(const std::string& dir, const std::string& abs_name
   if (!ok) return fail("write error in " + path);
   if (dump_gamma_extra(f)) return fail("write error in " + path);
   // WriteInvertedLists (index_io.cc:108-141)
-  const uint64_t cb = is_pq ? (uint64_t)code_bytes() : (uint64_t)d_ * 4;
+  const uint64_t cb = gf.code_size;
   ok = wr<uint32_t>(f, fourcc("ilar")) && wr<uint64_t>(f, (uint64_t)nlist_) && wr<uint64_t>(f, cb) &&
        wr<uint32_t>(f, fourcc("full")) && wr<uint64_t>(f, (uint64_t)nlist_);
   const std::vector<int> lens = lists_->lens();
@@ -128,14 +129,14 @@ int IVFFlatIndex::dump_gamma(const std::string& dir, const std::string& abs_name
     const size_t n = (size_t)lens[l];
     if (ids.size() < n) return fail("list shrank during dump");
     const uint8_t* src = codes.data();
-    if (!is_pq && dpad_ != d_) {  // our rows are padded to a multiple of 4 floats; gamma's are not
+    if (cb != (uint64_t)code_bytes()) {  // padded rows in memory
       packed.resize(n * cb);
-      for (size_t r = 0; r < n; r++) memcpy(packed.data() + r * cb, codes.data() + r * (size_t)dpad_ * 4, cb);
+      for (size_t r = 0; r < n; r++) memcpy(packed.data() + r * cb, codes.data() + r * (size_t)code_bytes(), cb);
       src = packed.data();
     }
     ok = wr_bytes(f, src, n * cb) && wr_bytes(f, ids.data(), n * 8);
   }
-  if (ok && !is_pq) ok = wr<int32_t>(f, (int32_t)indexed_count_);  // ivfflat.cc:835
+  if (ok && gf.indexed_count) ok = wr<int32_t>(f, (int32_t)indexed_count_);  // ivfflat.cc:835
   if (!ok || fflush(f)) return fail("write error in " + path);
   return 0;
 }
@@ -158,18 +159,19 @@ int IVFPQIndex::dump_gamma_extra(FILE* f) {
 }
 
 // ---- Load -----------------------------------------------------------------------------------
-int IVFFlatIndex::load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) {
+int IvfIndex::load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) {
   *load_num = 0;
-  const std::string path = dir + "/" + abs_name + "/" + gamma_file_name();
+  const GammaFileFormat gf = gamma_format();
+  if (!gf.file) return 0;
+  const std::string path = dir + "/" + abs_name + "/" + gf.file;
   FilePtr fp(fopen(path.c_str(), "rb"));
   FILE* f = fp.get();
   if (!f) return 0;  // "isn't existed, skip loading": it should train again after load (ivfflat.cc:846-850)
   std::lock_guard<std::mutex> bg(build_mu_);
   cudaSetDevice(device_);
   if (lists_ && lists_->total() > 0) return fail("load into a non-empty index");
-  const bool is_pq = type_ != "IVFFLAT";
   uint32_t h = 0;
-  if (!rd(f, &h) || h != (is_pq ? fourcc("IwPQ") : fourcc("IvFl"))) return fail("bad magic in " + path);
+  if (!rd(f, &h) || h != gf.magic) return fail("bad magic in " + path);
   IndexHeader ih, qh;
   uint64_t nlist = 0, nprobe = 0, n = 0;
   if (!rd_index_header(f, &ih) || !rd(f, &nlist) || !rd(f, &nprobe)) return fail("truncated ivf header in " + path);
@@ -208,8 +210,7 @@ int IVFFlatIndex::load_gamma(const std::string& dir, const std::string& abs_name
   uint64_t nb = 0, cb = 0, ns = 0;
   if (!rd(f, &h) || !rd(f, &nb) || !rd(f, &cb) || !rd(f, &lt) || h != fourcc("ilar") || lt != fourcc("full"))
     return fail("bad inverted-list header in " + path);
-  const uint64_t want_cb = is_pq ? (uint64_t)code_bytes() : (uint64_t)d_ * 4;
-  if (nb != (uint64_t)nlist_ || cb != want_cb) {
+  if (nb != (uint64_t)nlist_ || cb != gf.code_size) {
     // kIndexError: "unsupported inverted list format, it need rebuilding!" (ivfflat.cc:866-869)
     indexed_count_ = 0;
     return 0;
@@ -239,7 +240,7 @@ int IVFFlatIndex::load_gamma(const std::string& dir, const std::string& abs_name
     ids.resize(len);
     if (!rd_bytes(f, codes.data(), codes.size()) || !rd_bytes(f, ids.data(), len * 8)) return fail("truncated list in " + path);
     const uint8_t* src = codes.data();
-    if (my_cb != cb) {  // IVF-Flat with d % 4 != 0: pad rows to our stride
+    if (my_cb != cb) {  // padded rows in memory
       padded.assign(len * my_cb, 0);
       for (size_t r = 0; r < len; r++) memcpy(padded.data() + r * my_cb, codes.data() + r * cb, cb);
       src = padded.data();
@@ -257,7 +258,7 @@ int IVFFlatIndex::load_gamma(const std::string& dir, const std::string& abs_name
     }
   }
   int64_t indexed = live;  // IwPQ: ReadInvertedLists' running count (total - tombstones)
-  if (!is_pq) {
+  if (gf.indexed_count) {
     int32_t cnt = 0;
     if (!rd(f, &cnt) || cnt < 0) return fail("invalid indexed count in " + path);  // ivfflat.cc:871-878
     indexed = cnt;
