@@ -34,7 +34,7 @@ long long gb_launch_count(void);
  * (index/reflector.h:68-80, vector/vector_manager.cc:171; gamma_index_ivfflat.cc:215-291,
  * gamma_index_ivfpq.cc:112-231).  index_type: "FLAT" | "IVFFLAT" | "IVFPQ".
  * model_params_json keys: ncentroids, nprobe, metric_type ("L2"|"InnerProduct"), nsubvector,
- * nbits_per_idx, training_threshold, bucket_init_size, bucket_max_size (may be NULL/""). */
+ * nbits_per_idx (IVFPQ: 1..8), training_threshold, bucket_init_size, bucket_max_size (may be NULL/""). */
 gb_index *gb_index_create(const char *index_type, int dimension, const char *model_params_json, int device);
 void gb_index_destroy(gb_index *index);
 
@@ -97,10 +97,10 @@ int gb_index_nlist(gb_index *index);
 int gb_index_set_centroids(gb_index *index, const float *centroids, int nlist); /* marks trained */
 int gb_index_get_centroids(gb_index *index, float *centroids);
 int gb_index_pq_m(gb_index *index);
-int gb_index_pq_ksub(gb_index *index); /* centroids per sub-quantiser: 256 (IVFPQ), 16 (IVFPQFastScan) */
+int gb_index_pq_ksub(gb_index *index); /* centroids per sub-quantiser: 2^nbits_per_idx (IVFPQ), 16 (IVFPQFastScan) */
 int gb_index_set_pq_centroids(gb_index *index, const float *pq); /* [M][ksub][dsub] */
 int gb_index_get_pq_centroids(gb_index *index, float *pq);
-int gb_index_get_precomputed_table(gb_index *index, float *table); /* [nlist][M][256] */
+int gb_index_get_precomputed_table(gb_index *index, float *table); /* [nlist][M][ksub] */
 /* OPQ rotation of an IVFPQ index created with "opq": {"nsubvector": M} (gamma_index_ivfpq.cc:168-178):
  * A is d x d row-major, y = A x; apply runs the device path the index itself uses */
 int gb_index_has_opq(gb_index *index);
@@ -135,7 +135,8 @@ int gb_index_search_preassigned(gb_index *index, int nq, const float *x, int k, 
                                 const float *coarse_dis, int nprobe, const char *retrieval_params_json,
                                 const uint8_t *del_bitmap, const uint8_t *filter_bitmap, int64_t bitmap_bits,
                                 float min_score, float max_score, float *out_scores, int64_t *out_ids);
-/* pq.compute_codes on residuals (gamma_index_ivfpq.cc:489-494) */
+/* pq.compute_codes on residuals (gamma_index_ivfpq.cc:489-494): codes = n x code_size bytes, bit-packed below
+   nbits_per_idx = 8 (code m at bits [m nbits, (m + 1) nbits) of the row, LSB-first) */
 int gb_index_pq_encode(gb_index *index, int64_t n, const float *x, const int64_t *assign, uint8_t *codes);
 /* IVFPQFastScan encodes raw vectors (assign is ignored, may be NULL): codes = n x ceil(M/2) bytes, sub-quantiser 2j in
    the low nibble of byte j.  The uint8 look-up tables of a query batch: lut8 = nq x M x 16, ab = nq x (a, b), the

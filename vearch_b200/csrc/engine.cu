@@ -1328,7 +1328,7 @@ int Engine::Dump() {
     if (ivf->get_centroids(c.data())) return -1;
     f.write(reinterpret_cast<const char*>(c.data()), (std::streamsize)(c.size() * 4));
     if (pq) {
-      std::vector<float> p((size_t)pq->M() * 256 * pq->dsub());
+      std::vector<float> p((size_t)pq->M() * pq->ksub() * pq->dsub());
       if (pq->get_pq_centroids(p.data())) return -1;
       f.write(reinterpret_cast<const char*>(p.data()), (std::streamsize)(p.size() * 4));
     }
@@ -1414,7 +1414,7 @@ int Engine::Load() {
     if (!f.read(reinterpret_cast<char*>(c.data()), (std::streamsize)(c.size() * 4))) return -1;
     if (ivf->set_centroids(c.data(), ivf->nlist())) return -1;
     if (pq) {
-      std::vector<float> p((size_t)pq->M() * 256 * pq->dsub());
+      std::vector<float> p((size_t)pq->M() * pq->ksub() * pq->dsub());
       if (!f.read(reinterpret_cast<char*>(p.data()), (std::streamsize)(p.size() * 4))) return -1;
       if (pq->set_pq_centroids(p.data())) return -1;
     }

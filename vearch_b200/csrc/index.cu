@@ -1714,7 +1714,8 @@ int IvfPqBase::encode_host(const float* x, int64_t n, const int64_t* assign, uin
 // ------------------------------------------------------------------------------------------
 // gamma_index_ivfpq.cc:122-124: nsubvector defaults to d / 2
 IVFPQIndex::IVFPQIndex(int d, const ModelParams& mp, int device, int seg_shift)
-    : IvfPqBase("IVFPQ", d, mp, device, seg_shift, std::max(1, mp.nsubvector > 0 ? mp.nsubvector : d / 2), 256) {
+    : IvfPqBase("IVFPQ", d, mp, device, seg_shift, std::max(1, mp.nsubvector > 0 ? mp.nsubvector : d / 2), 1 << mp.nbits),
+      nbits_(mp.nbits) {
   if (mp.opq_nsubvector > 0) {  // faiss::OPQMatrix(d, opq_nsubvector, d) (gamma_index_ivfpq.cc:168-178)
     cudaMalloc(&d_opq_, (size_t)d * dpad_ * 4);
     cudaMemset(d_opq_, 0, (size_t)d * dpad_ * 4);
@@ -1926,20 +1927,20 @@ KMeansParams IVFPQIndex::coarse_kmeans_params() const {
   return kp;
 }
 int64_t IVFPQIndex::index_mem_bytes() const {
-  return IvfPqBase::index_mem_bytes() + (d_table_ ? (int64_t)nlist_ * M_ * 256 * 4 : 0);
+  return IvfPqBase::index_mem_bytes() + (d_table_ ? (int64_t)nlist_ * M_ * ksub_ * 4 : 0);
 }
 int IVFPQIndex::codebook_changed(cudaStream_t st) {
   pq_gen_++;  // the per-entry norm cache belongs to the previous codebook
   // tables of the tensor-core filter (kernels_pqtc.cu): fp16 codebook pre-scaled by -2 sb (L2) / -sb (IP), sb a power of two,
   // centroid norms, and the bound on |r| its error margin uses
-  if (pqtc_supported(M_, dsub_)) {
+  if (ksub_ == 256 && pqtc_supported(M_, dsub_)) {
     if (!d_cb16_) GB_CUDA(cudaMalloc(&d_cb16_, (size_t)M_ * 256 * dsub_ * 2));
     if (!d_cbnrm_) GB_CUDA(cudaMalloc(&d_cbnrm_, ((size_t)M_ * 256 + 4) * 4));
     GB_CUDA(launch_pqtc_tables(d_pq_, M_, dsub_, mp_.metric, d_cb16_, d_cbnrm_, d_cbnrm_ + (size_t)M_ * 256, st));
   }
   if (mp_.metric != kMetricL2) return 0;  // IP: tab = ip table, dis0 = <x, centroid>
-  if (!d_table_) GB_CUDA(cudaMalloc(&d_table_, (size_t)nlist_ * M_ * 256 * 4));
-  GB_CUDA(launch_pq_precompute_table(d_centroids_, dpad_, nlist_, d_pq_, M_, dsub_, d_table_, st));
+  if (!d_table_) GB_CUDA(cudaMalloc(&d_table_, (size_t)nlist_ * M_ * ksub_ * 4));
+  GB_CUDA(launch_pq_precompute_table(d_centroids_, dpad_, nlist_, d_pq_, M_, dsub_, d_table_, st, ksub_));
   return 0;
 }
 int IVFPQIndex::get_precomputed_table(float* host) const {
@@ -1948,18 +1949,18 @@ int IVFPQIndex::get_precomputed_table(float* host) const {
     return -1;
   }
   cudaSetDevice(device_);
-  GB_CUDA(cudaMemcpy(host, d_table_, (size_t)nlist_ * M_ * 256 * 4, cudaMemcpyDeviceToHost));
+  GB_CUDA(cudaMemcpy(host, d_table_, (size_t)nlist_ * M_ * ksub_ * 4, cudaMemcpyDeviceToHost));
   return 0;
 }
 
-// faiss IndexIVFPQ::train_residual restated: residuals of (a subsample of <= 256*ksub) training
-// vectors -> ProductQuantizer::train = M independent 256-means on the dsub-wide slices.
+// faiss IndexIVFPQ::train_residual restated: residuals of (a subsample of <= 256*ksub, max_points_per_centroid * ksub)
+// training vectors -> ProductQuantizer::train = M independent ksub-means on the dsub-wide slices.
 int IVFPQIndex::train_extra(const float* xtrain, int64_t n, Scratch& s) {
   if (d_ % M_ != 0) {
     set_last_error("dimension not divisible by nsubvector");
     return -1;
   }
-  const int64_t npq = std::min<int64_t>(n, 256 * 256);
+  const int64_t npq = std::min<int64_t>(n, (int64_t)256 * ksub_);
   const float* xs;
   if (subsample_rows(xtrain, n, npq, dpad_, &xs, s)) return -1;
   GB_ALLOC(assign, int32_t, npq, s);
@@ -1969,10 +1970,18 @@ int IVFPQIndex::train_extra(const float* xtrain, int64_t n, Scratch& s) {
   return train_codebook(resid, npq, s);
 }
 
-// GammaIVFPQIndex::Add (gamma_index_ivfpq.cc:455-540): residual -> pq.compute_codes -> AddKeys
+// GammaIVFPQIndex::Add (gamma_index_ivfpq.cc:455-540): residual -> pq.compute_codes -> AddKeys.  Below 8 bits the
+// per-(row, sub-quantiser) encoder writes one byte per code to scratch and one thread per row packs them (threads of
+// the encoder would share output bytes).
 cudaError_t IVFPQIndex::encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st) {
   if (!lists) return cudaErrorInvalidValue;  // residual codes need each row's list
-  return launch_pq_encode(x, dpad_, n, d_centroids_, dpad_, lists, d_pq_, M_, dsub_, codes, st);
+  if (nbits_ == 8) return launch_pq_encode(x, dpad_, n, d_centroids_, dpad_, lists, d_pq_, M_, dsub_, codes, st);
+  Scratch s(st);
+  uint8_t* raw = s.alloc_n<uint8_t>((size_t)n * M_);
+  if (!raw) return cudaErrorMemoryAllocation;
+  const cudaError_t e = launch_pq_encode(x, dpad_, n, d_centroids_, dpad_, lists, d_pq_, M_, dsub_, raw, st, ksub_);
+  if (e != cudaSuccess) return e;
+  return launch_pq_pack_codes(raw, n, M_, nbits_, codes, st);
 }
 
 // Cache of |r_e|^2 per list entry for the tensor-core filter.  Searches hold mu_ shared, appends hold it exclusively and
@@ -2016,7 +2025,7 @@ int IVFPQIndex::ensure_pq_norms(cudaStream_t st) {
 int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const float* xq, int kk, const float* ip,
                                   const int32_t* probe_ids, const float* coarse_dis, int nprobe,
                                   unsigned long long* adc_out, bool need_sorted, Scratch& s) {
-  if (!d_cb16_ || !pqtc_supported(M_, dsub_) || dpad_ != d_) return 1;
+  if (ksub_ != 256 || !d_cb16_ || !pqtc_supported(M_, dsub_) || dpad_ != d_) return 1;  // the filter reads 8-bit codes
   if (kk > 2048 || nprobe < 2 || nprobe > 65535 || nq > 65535) return 1;  // (query, probe) travel as 16-bit fields of a candidate record
   const int64_t npairs = (int64_t)nq * nprobe;
   if (npairs < (int64_t)nlist_ * 32) return 1;  // < 32 queries per list on average
@@ -2161,22 +2170,26 @@ int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metr
   cudaStream_t st = s.stream();
   float* ip = nullptr;
   auto prepare = [&](int kk, unsigned long long* keys, bool need_sorted) {
-    ip = s.alloc_n<float>((size_t)nq * M_ * 256);
+    ip = s.alloc_n<float>((size_t)nq * M_ * ksub_);
     if (!ip) return -1;
     {
       StageScope stage(this, "pq_ip_table", st);
-      GB_CUDA(launch_pq_ip_table(xq, dpad_, nq, d_pq_, M_, dsub_, ip, st));
+      GB_CUDA(launch_pq_ip_table(xq, dpad_, nq, d_pq_, M_, dsub_, ip, st, ksub_));
     }
     const int lm = scan_listmajor_pq(f, metric, nq, xq, kk, ip, probe_ids, coarse_dis, nprobe, keys, need_sorted, s);
     if (lm == 0) last_scan_kernel_ = "pqtc_scan_kernel";
     return lm;
   };
   auto launch = [&](int kk, int pg, unsigned long long* partial) {
+    if (nbits_ < 8)
+      return launch_ivfpq_packed_scan(ip, nq, probe_ids, coarse_dis, nprobe, pg, lists_->directory(), M_, nbits_, d_table_,
+                                      kk, metric, f, partial, st);
     return launch_ivfpq_scan(ip, nq, probe_ids, coarse_dis, nprobe, pg, lists_->directory(), M_, d_table_, kk, metric, f,
                              partial, st);
   };
   // "for opq, rerank need raw vector" (gamma_index_ivfpq.cc:735): original queries against the raw store
-  return scan_pq_dev("ivfpq_scan_kernel", ctx, f, metric, nq, xq_raw, k, nprobe, out_keys, s, prepare, launch);
+  return scan_pq_dev(nbits_ < 8 ? "ivfpq_packed_scan_kernel" : "ivfpq_scan_kernel", ctx, f, metric, nq, xq_raw, k, nprobe,
+                     out_keys, s, prepare, launch);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2265,8 +2278,14 @@ Index* create_index(const std::string& type, int d, const ModelParams& mp, int d
       set_last_error("Dimension [" + std::to_string(d) + "] cannot divide by nsubvector [" + std::to_string(M) + "].");
       return nullptr;
     }
-    if (mp.nbits != 8) {
-      set_last_error("only nbits_per_idx = 8 is supported");
+    // gamma_index_ivfpq.cc:182 takes any nbits; 1..8 here (IVFPQIndex::kMaxNbits)
+    if (mp.nbits < 1) {
+      set_last_error("invalid nbits_per_idx =" + std::to_string(mp.nbits));
+      return nullptr;
+    }
+    if (mp.nbits > IVFPQIndex::kMaxNbits) {
+      set_last_error("IVFPQ: nbits_per_idx [" + std::to_string(mp.nbits) + "] above " +
+                     std::to_string(IVFPQIndex::kMaxNbits) + " is not supported by this engine");
       return nullptr;
     }
     if (mp.opq_nsubvector > 0 && d % mp.opq_nsubvector != 0) {  // gamma_index_ivfpq.cc:169-176

@@ -517,13 +517,19 @@ class IvfPqBase : public IvfIndex {
   float* d_pq_ = nullptr;  // [M][ksub][dsub]
 };
 
+// GammaIVFPQIndex (index/impl/gamma_index_ivfpq.{h,cc}) at nbits_per_idx 1..8: ksub = 2^nbits centroids per
+// sub-quantiser; list entries hold the residual codes bit-packed in ceil(M nbits / 8) bytes (faiss PQEncoderGeneric:
+// code m at bits [m nbits, (m + 1) nbits), LSB-first), one byte per code at nbits = 8.
 class IVFPQIndex : public IvfPqBase {
  public:
+  // nbits_per_idx above this: faiss's 16-bit codes (PQDecoder16), whose [M][65536] fp32 table no scan keeps in shared memory
+  static constexpr int kMaxNbits = 8;
   IVFPQIndex(int d, const ModelParams& mp, int device, int seg_shift);
   ~IVFPQIndex() override;
   int64_t index_mem_bytes() const override;
-  int code_bytes() const override { return M_; }
-  int get_precomputed_table(float* host) const;
+  int nbits() const { return nbits_; }
+  int code_bytes() const override { return (M_ * nbits_ + 7) / 8; }
+  int get_precomputed_table(float* host) const;  // [nlist][M][ksub]
 
  protected:
   GammaFileFormat gamma_format() const override;
@@ -546,7 +552,9 @@ class IVFPQIndex : public IvfPqBase {
   const float* train_transform(const float* xt, int64_t n, Scratch& s) override;
   const float* transform_dev(const float* x, int64_t n, Scratch& s) override;
 
-  float* d_table_ = nullptr;  // [nlist][M][256] (L2 only)
+  int nbits_;
+  float* d_table_ = nullptr;  // [nlist][M][ksub] (L2 only)
+  // the tensor-core filter and its tables exist at nbits = 8 only; packed codes are scanned query-major
   uint16_t* d_cb16_ = nullptr;  // [M][256][dsub] fp16, pre-scaled (tensor-core filter)
   float* d_cbnrm_ = nullptr;    // [M][256] |pq|^2, then rmax2, sb
   // |r_e|^2 of every list entry (L2), flat with 32-entry aligned list segments: built by the first list-major search

@@ -14,6 +14,7 @@
 //                quantizer = u32 "IxF2" | "IxFI", index header (ntotal = nlist), u64 nlist*d, nlist*d fp32
 //                direct map = u8 type (0 = none), u64 0
 //   IwPQ only  : u8 by_residual, u64 code_size, u64 d, u64 M, u64 nbits, u64 M*ksub*dsub, fp32 centroids [M][ksub][dsub]
+//                (ksub = 2^nbits, code_size = ceil(M nbits / 8): the list codes bit-packed as faiss PQEncoderGeneric)
 //   lists      : u32 "ilar", u64 nlist, u64 code_bytes, u32 "full", u64 nlist, u64 sizes[nlist],
 //                per non-empty list: codes[size * code_bytes], i64 ids[size] (top bit = tombstone)
 //   IvFl only  : i32 indexed_count
@@ -142,11 +143,11 @@ int IvfIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
 }
 
 int IVFPQIndex::dump_gamma_extra(FILE* f) {
-  std::vector<float> pq((size_t)M_ * 256 * dsub_);
+  std::vector<float> pq((size_t)M_ * ksub_ * dsub_);
   if (get_pq_centroids(pq.data())) return -1;
   // by_residual, code_size, write_product_quantizer (ivfpq.cc:1037-1039, index_io.cc:92-98)
-  bool ok = wr<uint8_t>(f, 1) && wr<uint64_t>(f, (uint64_t)M_) && wr<uint64_t>(f, (uint64_t)d_) &&
-            wr<uint64_t>(f, (uint64_t)M_) && wr<uint64_t>(f, 8) && wr<uint64_t>(f, (uint64_t)pq.size()) &&
+  bool ok = wr<uint8_t>(f, 1) && wr<uint64_t>(f, (uint64_t)code_bytes()) && wr<uint64_t>(f, (uint64_t)d_) &&
+            wr<uint64_t>(f, (uint64_t)M_) && wr<uint64_t>(f, (uint64_t)nbits_) && wr<uint64_t>(f, (uint64_t)pq.size()) &&
             wr_bytes(f, pq.data(), pq.size() * 4);
   if (ok && has_opq()) {  // write_opq (index_io.cc:230-246): "LTra", have_bias, A, b, d_in, d_out, is_trained
     std::vector<float> A((size_t)d_ * d_);
@@ -283,9 +284,12 @@ int IVFPQIndex::load_gamma_extra(FILE* f) {
   if (!rd(f, &by_residual) || !rd(f, &code_size) || !rd(f, &d) || !rd(f, &M) || !rd(f, &nbits) || !rd(f, &n))
     return fail("truncated product quantizer");
   if (!by_residual) return fail("by_residual = false is not supported");
-  if (d != (uint64_t)d_ || M != (uint64_t)M_ || nbits != 8 || code_size != (uint64_t)M_ || n != (uint64_t)M_ * 256 * dsub_)
+  if (d != (uint64_t)d_ || M != (uint64_t)M_ || nbits != (uint64_t)nbits_ || code_size != (uint64_t)code_bytes() ||
+      n != (uint64_t)M_ * ksub_ * dsub_)
     return fail("product quantizer does not match the table: d=" + std::to_string(d) + " M=" + std::to_string(M) +
-                " nbits=" + std::to_string(nbits));
+                " nbits=" + std::to_string(nbits) + " code_size=" + std::to_string(code_size) + " centroids=" +
+                std::to_string(n) + " (table: d=" + std::to_string(d_) + " M=" + std::to_string(M_) + " nbits=" +
+                std::to_string(nbits_) + " code_size=" + std::to_string(code_bytes()) + ")");
   std::vector<float> pq((size_t)n);
   if (!rd_bytes(f, pq.data(), pq.size() * 4)) return fail("truncated product quantizer");
   if (has_opq()) {  // read_opq (index_io.cc:248-270); whether the block is there is decided by the table's params

@@ -153,12 +153,12 @@ cudaError_t launch_pq_decode(const uint8_t* codes, int64_t n, const float* pq_ce
                              int64_t ldr, cudaStream_t st);
 
 // ---- K4/K5: IVF-PQ look-up tables + ADC scan --------------------------------------------
-// ip[q][m][c] = <x_q|m, pq_m[c]>   (pq.compute_inner_prod_table)
+// ip[q][m][c] = <x_q|m, pq_m[c]>   (pq.compute_inner_prod_table); ksub = 2^nbits centroids per sub-quantiser
 cudaError_t launch_pq_ip_table(const float* xq, int64_t ldq, int nq, const float* pq_centroids, int M, int dsub,
-                               float* ip, cudaStream_t st);
-// T[l][m][c] = |pq_m[c]|^2 + 2 <centroid_l|m, pq_m[c]>  (IndexIVFPQ::precompute_table)
+                               float* ip, cudaStream_t st, int ksub = 256);
+// T[l][m][c] = |pq_m[c]|^2 + 2 <centroid_l|m, pq_m[c]>  (IndexIVFPQ::precompute_table), [nlist][M][ksub]
 cudaError_t launch_pq_precompute_table(const float* coarse, int64_t ldc, int nlist, const float* pq_centroids, int M,
-                                       int dsub, float* T, cudaStream_t st);
+                                       int dsub, float* T, cudaStream_t st, int ksub = 256);
 // partial[q][group][k], group = ceil(nprobe/pg) CTAs per query, each scanning pg (<= 32) probed lists.
 // coarse_dis = dis0 per (q, probe).  T nullable for IP.
 // ld_probe: row stride of probe_ids / coarse_dis (0 = nprobe; > nprobe scans the first nprobe probes of
@@ -168,6 +168,11 @@ cudaError_t launch_ivfpq_scan(const float* ip_table, int nq, const int32_t* prob
                               FilterArgs f, unsigned long long* partial, cudaStream_t st, int ld_probe = 0,
                               const int* gate_cnt = nullptr, int gate_cap = 0, const int* row_limit = nullptr,
                               bool sorted_out = true);  // false: partial[..][k - 1] = the largest key, the others in any order
+// the same scan over bit-packed codes, nbits_per_idx 1..7 (ceil(M nbits / 8) bytes per entry, code m at bits
+// [m nbits, (m + 1) nbits), LSB-first); ip_table [nq][M][2^nbits], T [nlist][M][2^nbits]; sorted partials
+cudaError_t launch_ivfpq_packed_scan(const float* ip_table, int nq, const int32_t* probe_ids, const float* coarse_dis,
+                                     int nprobe, int pg, ListDirectory dir, int M, int nbits, const float* T, int k,
+                                     int metric, FilterArgs f, unsigned long long* partial, cudaStream_t st);
 
 // ---- K5 list-major: tensor-core filter + exact re-score (kernels_pqtc.cu) ---------------------------
 bool pqtc_supported(int M, int dsub);
@@ -228,10 +233,13 @@ cudaError_t launch_segment_mean(const float* x, int64_t ldx, int d, const int32_
 // out = x - centroids[assign]
 cudaError_t launch_residual(const float* x, int64_t ldx, int64_t n, int d, const float* centroids, int64_t ldc,
                             const int32_t* assign, float* out, int64_t ldo, cudaStream_t st);
-// codes[i][m] = argmin_c |(x_i - coarse[assign_i])|m - pq_m[c]|^2 (coarse nullable => no residual)
+// codes[i][m] = argmin_c |(x_i - coarse[assign_i])|m - pq_m[c]|^2 over c < ksub, first minimum (coarse nullable =>
+// no residual); one byte per code
 cudaError_t launch_pq_encode(const float* x, int64_t ldx, int64_t n, const float* coarse, int64_t ldc,
                              const int32_t* assign, const float* pq_centroids, int M, int dsub, uint8_t* codes,
-                             cudaStream_t st);
+                             cudaStream_t st, int ksub = 256);
+// [n][M] codes < 2^nbits -> [n][ceil(M nbits / 8)] rows, code m at bits [m nbits, (m + 1) nbits) LSB-first, high bits 0
+cudaError_t launch_pq_pack_codes(const uint8_t* codes, int64_t n, int M, int nbits, uint8_t* packed, cudaStream_t st);
 // copy a column slice [col0, col0+w) of x into a dense n x ldo buffer (zero padded to ldo)
 cudaError_t launch_slice_cols(const float* x, int64_t ldx, int64_t n, int col0, int w, float* out, int64_t ldo,
                               cudaStream_t st);

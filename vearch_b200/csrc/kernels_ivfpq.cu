@@ -16,6 +16,11 @@
 // are bit-equal to the oracle's.
 //
 // Algorithmic bytes of the scan: (M + 8) per entry + M*256*4 per (query, list) for the T row.
+//
+// nbits_per_idx < 8 (ksub = 2^nbits): the table kernels and the encoder run over ksub centroids with the same
+// arithmetic, the encoder's [n][M] codes are bit-packed by pq_pack_codes (faiss PQEncoderGeneric: code m at bits
+// [m nbits, (m + 1) nbits) of the entry, LSB-first), and IvfpqPackedCodec scans them (code_size + 8 bytes per entry,
+// M*ksub*4 per (query, list)).
 #include <float.h>
 
 #include "common.cuh"
@@ -26,51 +31,54 @@ namespace gb {
 
 namespace {
 
-constexpr int KSUB = 256;
+constexpr int KSUB = 256;  // ksub at nbits = 8, and the threads of the table kernels
 
 // ---------------- per-query inner-product table ------------------------------------------
 constexpr int IPT_QB = 32;
 
+// one CTA per (sub-quantiser, IPT_QB queries); thread t computes centroid t % ksub of every (KSUB / ksub)-th query
 __global__ void __launch_bounds__(KSUB)
     pq_ip_table_kernel(const float* __restrict__ xq, int64_t ldq, int nq, const float* __restrict__ pq, int M, int dsub,
-                       float* __restrict__ ip) {
+                       int ksub, float* __restrict__ ip) {
   extern __shared__ float sm[];
-  float* ps = sm;                // [dsub][256]
-  float* xs = sm + dsub * KSUB;  // [IPT_QB][dsub]
+  float* ps = sm;                // [dsub][ksub]
+  float* xs = sm + dsub * ksub;  // [IPT_QB][dsub]
   const int m = blockIdx.x;
   const int q0 = blockIdx.y * IPT_QB;
-  const int c = threadIdx.x;
-  for (int idx = threadIdx.x; idx < dsub * KSUB; idx += KSUB) {
+  const int c = threadIdx.x % ksub, qstep = KSUB / ksub;
+  for (int idx = threadIdx.x; idx < dsub * ksub; idx += KSUB) {
     int cc = idx / dsub, j = idx - cc * dsub;
-    ps[j * KSUB + cc] = pq[((int64_t)m * KSUB) * dsub + idx];
+    ps[j * ksub + cc] = pq[((int64_t)m * ksub) * dsub + idx];
   }
   for (int idx = threadIdx.x; idx < IPT_QB * dsub; idx += KSUB) {
     int qq = idx / dsub, j = idx - qq * dsub;
     xs[idx] = (q0 + qq < nq) ? xq[(int64_t)(q0 + qq) * ldq + m * dsub + j] : 0.f;
   }
   __syncthreads();
-  for (int qq = 0; qq < IPT_QB && q0 + qq < nq; qq++) {
+  for (int qq = threadIdx.x / ksub; qq < IPT_QB && q0 + qq < nq; qq += qstep) {
     float acc = 0.f;
-    for (int j = 0; j < dsub; j++) acc = __fadd_rn(acc, __fmul_rn(xs[qq * dsub + j], ps[j * KSUB + c]));
-    ip[((int64_t)(q0 + qq) * M + m) * KSUB + c] = acc;
+    for (int j = 0; j < dsub; j++) acc = __fadd_rn(acc, __fmul_rn(xs[qq * dsub + j], ps[j * ksub + c]));
+    ip[((int64_t)(q0 + qq) * M + m) * ksub + c] = acc;
   }
 }
 
 // ---------------- precomputed table T[l][m][c] --------------------------------------------
+// one CTA per list; thread t computes the entries t, t + KSUB, ... of the list's [M][ksub] row
 __global__ void __launch_bounds__(KSUB)
     pq_precompute_table_kernel(const float* __restrict__ coarse, int64_t ldc, const float* __restrict__ pq, int M,
-                               int dsub, float* __restrict__ T) {
-  const int l = blockIdx.x, c = threadIdx.x;
-  for (int m = 0; m < M; m++) {
+                               int dsub, int ksub, float* __restrict__ T) {
+  const int l = blockIdx.x;
+  for (int i = threadIdx.x; i < M * ksub; i += KSUB) {
+    const int m = i / ksub;
     const float* cl = coarse + (int64_t)l * ldc + m * dsub;
-    const float* p = pq + ((int64_t)m * KSUB + c) * dsub;
+    const float* p = pq + (int64_t)i * dsub;
     float nrm = 0.f, ipv = 0.f;
     for (int j = 0; j < dsub; j++) {
       float pj = p[j];
       nrm = __fadd_rn(nrm, __fmul_rn(pj, pj));
       ipv = __fadd_rn(ipv, __fmul_rn(__ldg(cl + j), pj));
     }
-    T[((int64_t)l * M + m) * KSUB + c] = __fadd_rn(nrm, __fmul_rn(2.0f, ipv));
+    T[(int64_t)l * M * ksub + i] = __fadd_rn(nrm, __fmul_rn(2.0f, ipv));
   }
 }
 
@@ -140,6 +148,72 @@ cudaError_t launch_scan_m(const IvfpqCodec& c, int nq, const ListScanArgs& a, cu
     default: return launch_list_scan<IvfpqCodec, METRIC, 0>(c, nq, a, st);
   }
 }
+
+// ---------------- ADC scan over bit-packed codes (nbits_per_idx < 8) ------------------------------
+// Code m of an entry sits at bits [m nbits, (m + 1) nbits) of its code_size = ceil(M nbits / 8) bytes, LSB-first.  The
+// table is [M][ksub] fp32, built per list exactly as IvfpqCodec's [M][256] one; an entry's score is dis0, then
+// += lut[m][code m] for m = 0..M-1, one fp32 add at a time (PQDecoder order, gamma_index_ivfpq.h:532-536).  Rows are
+// code_size bytes apart in the stage, so they start at any byte: the codes are read as the aligned 32-bit words that
+// hold them, through a 64-bit bit buffer.
+__host__ __device__ inline int pq_packed_tile_entries(int code_size) {  // ~16 KiB of codes, 256..1024 entries
+  int e = 16384 / code_size;
+  e = (e / LS_NT) * LS_NT;
+  return e < LS_NT ? LS_NT : (e > 1024 ? 1024 : e);
+}
+
+struct IvfpqPackedCodec {
+  using Entry = float;
+  static constexpr bool kDis0 = true;
+  static constexpr bool kCodeSum = true;
+  static constexpr int kMinCtasPerSm = 0;
+  const float* ip_table;  // [nq][M][ksub]
+  const float* T;         // [nlist][M][ksub], L2 only
+  int M, nbits;
+  const float* ipq;  // this CTA's query in ip_table
+
+  __host__ __device__ int ksub() const { return 1 << nbits; }
+  __host__ __device__ int code_bytes() const { return (M * nbits + 7) / 8; }
+  __host__ __device__ int table_entries() const { return (M * ksub() + 3) & ~3; }
+  int tile_entries() const { return pq_packed_tile_entries(code_bytes()); }
+  __host__ __device__ static constexpr int pt(int) { return 1; }  // not used: MW = 0 only
+
+  __device__ __forceinline__ void cta_begin(float* lut, int q, int metric) {
+    ipq = ip_table + (int64_t)q * M * ksub();
+    if (metric != kMetricL2) {
+      for (int i = threadIdx.x; i < M * ksub(); i += LS_NT) lut[i] = __ldg(ipq + i);
+      __syncthreads();
+    }
+  }
+  __device__ __forceinline__ void list_begin(float* lut, int list, int metric) const {
+    if (metric == kMetricL2) {
+      const float* Tl = T + (int64_t)list * M * ksub();
+      for (int i = threadIdx.x; i < M * ksub(); i += LS_NT) lut[i] = fmaf(-2.0f, __ldg(ipq + i), __ldg(Tl + i));
+      __syncthreads();
+    }
+  }
+  using Acc = float;
+  __device__ __forceinline__ float start(float dis0) const { return dis0; }
+  __device__ __forceinline__ float finish(float dis) const { return dis; }
+  __device__ __forceinline__ float code_sum(const unsigned char* code, const float* __restrict__ tab, float acc) const {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(code);
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(a & ~(uintptr_t)3);
+    const int skip = (int)(a & 3) * 8;
+    uint64_t bits = w[0] >> skip;  // >= 8 valid bits: the first code (nbits <= 7) needs no refill
+    int nb = 32 - skip;
+    const uint32_t mask = (1u << nbits) - 1u;
+    const int ks = ksub();
+    for (int m = 0; m < M; m++, tab += ks) {
+      if (nb < nbits) {
+        bits |= (uint64_t)(*++w) << nb;
+        nb += 32;
+      }
+      acc += tab[(uint32_t)bits & mask];
+      bits >>= nbits;
+      nb -= nbits;
+    }
+    return acc;
+  }
+};
 
 // ---------------- exact re-rank -------------------------------------------------------------
 constexpr int RR_NT = 256;
@@ -214,13 +288,13 @@ constexpr int ENC_MAX_DSUB = 128;
 template <int DSUB>
 __global__ void __launch_bounds__(ENC_NT)
     pq_encode_kernel(const float* __restrict__ x, int64_t ldx, int64_t n, const float* __restrict__ coarse, int64_t ldc,
-                     const int32_t* __restrict__ assign, const float* __restrict__ pq, int M, int dsub_rt,
+                     const int32_t* __restrict__ assign, const float* __restrict__ pq, int M, int dsub_rt, int ksub,
                      uint8_t* __restrict__ codes) {
-  extern __shared__ float ps[];  // [256][dsub]
+  extern __shared__ float ps[];  // [ksub][dsub]
   const int dsub = DSUB > 0 ? DSUB : dsub_rt;
   const int m = blockIdx.y;
   const int64_t i = (int64_t)blockIdx.x * ENC_NT + threadIdx.x;
-  for (int idx = threadIdx.x; idx < KSUB * dsub; idx += ENC_NT) ps[idx] = pq[(int64_t)m * KSUB * dsub + idx];
+  for (int idx = threadIdx.x; idx < ksub * dsub; idx += ENC_NT) ps[idx] = pq[(int64_t)m * ksub * dsub + idx];
   __syncthreads();
   if (i >= n) return;
   float r[DSUB > 0 ? DSUB : ENC_MAX_DSUB];
@@ -230,7 +304,7 @@ __global__ void __launch_bounds__(ENC_NT)
   for (int j = 0; j < dsub; j++) r[j] = ci ? __fsub_rn(xi[j], ci[j]) : xi[j];
   float best = FLT_MAX;
   int bi = 0;
-  for (int c = 0; c < KSUB; c++) {
+  for (int c = 0; c < ksub; c++) {
     float dis = 0.f;
 #pragma unroll
     for (int j = 0; j < dsub; j++) {
@@ -245,26 +319,50 @@ __global__ void __launch_bounds__(ENC_NT)
   codes[i * M + m] = (uint8_t)bi;
 }
 
+// one thread per row: [n][M] codes -> [n][ceil(M nbits / 8)] bit-packed rows (PQEncoderGeneric's layout)
+__global__ void pq_pack_codes_kernel(const uint8_t* __restrict__ codes, int64_t n, int M, int nbits,
+                                     uint8_t* __restrict__ packed) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint8_t* src = codes + i * M;
+  const int cs = (M * nbits + 7) / 8;
+  uint8_t* dst = packed + i * cs;
+  uint32_t bits = 0;
+  int nb = 0, o = 0;
+  for (int m = 0; m < M; m++) {
+    bits |= (uint32_t)src[m] << nb;
+    nb += nbits;
+    while (nb >= 8) {
+      dst[o++] = (uint8_t)bits;
+      bits >>= 8;
+      nb -= 8;
+    }
+  }
+  if (nb > 0) dst[o] = (uint8_t)bits;
+}
+
 }  // namespace
 
 cudaError_t launch_pq_ip_table(const float* xq, int64_t ldq, int nq, const float* pq_centroids, int M, int dsub,
-                               float* ip, cudaStream_t st) {
+                               float* ip, cudaStream_t st, int ksub) {
   if (nq <= 0) return cudaSuccess;
-  size_t smem = ((size_t)dsub * KSUB + (size_t)IPT_QB * dsub) * 4;
+  if (ksub < 2 || ksub > KSUB || (ksub & (ksub - 1))) return cudaErrorInvalidValue;
+  size_t smem = ((size_t)dsub * ksub + (size_t)IPT_QB * dsub) * 4;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(pq_ip_table_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
   dim3 grid(M, (nq + IPT_QB - 1) / IPT_QB);
-  pq_ip_table_kernel<<<grid, KSUB, smem, st>>>(xq, ldq, nq, pq_centroids, M, dsub, ip);
+  pq_ip_table_kernel<<<grid, KSUB, smem, st>>>(xq, ldq, nq, pq_centroids, M, dsub, ksub, ip);
   note_launch();
   return cudaGetLastError();
 }
 
 cudaError_t launch_pq_precompute_table(const float* coarse, int64_t ldc, int nlist, const float* pq_centroids, int M,
-                                       int dsub, float* T, cudaStream_t st) {
+                                       int dsub, float* T, cudaStream_t st, int ksub) {
   if (nlist <= 0) return cudaSuccess;
-  pq_precompute_table_kernel<<<nlist, KSUB, 0, st>>>(coarse, ldc, pq_centroids, M, dsub, T);
+  if (ksub < 1 || ksub > KSUB) return cudaErrorInvalidValue;
+  pq_precompute_table_kernel<<<nlist, KSUB, 0, st>>>(coarse, ldc, pq_centroids, M, dsub, ksub, T);
   note_launch();
   return cudaGetLastError();
 }
@@ -279,6 +377,16 @@ cudaError_t launch_ivfpq_scan(const float* ip_table, int nq, const int32_t* prob
                        gate_cnt, gate_cap, row_limit, sorted_out, partial};
   if (metric == kMetricL2) return launch_scan_m<kMetricL2>(c, nq, a, st);
   return launch_scan_m<kMetricIP>(c, nq, a, st);
+}
+
+cudaError_t launch_ivfpq_packed_scan(const float* ip_table, int nq, const int32_t* probe_ids, const float* coarse_dis,
+                                     int nprobe, int pg, ListDirectory dir, int M, int nbits, const float* T, int k,
+                                     int metric, FilterArgs f, unsigned long long* partial, cudaStream_t st) {
+  if ((metric == kMetricL2 && !T) || nbits < 1 || nbits > 7) return cudaErrorInvalidValue;
+  const IvfpqPackedCodec c{ip_table, T, M, nbits, nullptr};
+  const ListScanArgs a{probe_ids, coarse_dis, nprobe, nprobe, pg, dir, k, f, nullptr, 0, nullptr, true, partial};
+  if (metric == kMetricL2) return launch_list_scan<IvfpqPackedCodec, kMetricL2, 0>(c, nq, a, st);
+  return launch_list_scan<IvfpqPackedCodec, kMetricIP, 0>(c, nq, a, st);
 }
 
 cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq, const float* xq, int64_t ldq, int d,
@@ -300,10 +408,10 @@ cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq
 
 cudaError_t launch_pq_encode(const float* x, int64_t ldx, int64_t n, const float* coarse, int64_t ldc,
                              const int32_t* assign, const float* pq_centroids, int M, int dsub, uint8_t* codes,
-                             cudaStream_t st) {
+                             cudaStream_t st, int ksub) {
   if (n <= 0) return cudaSuccess;
-  if (dsub > ENC_MAX_DSUB) return cudaErrorInvalidValue;
-  size_t smem = (size_t)KSUB * dsub * 4;
+  if (dsub > ENC_MAX_DSUB || ksub < 1 || ksub > KSUB) return cudaErrorInvalidValue;
+  size_t smem = (size_t)ksub * dsub * 4;
   dim3 grid((unsigned)((n + ENC_NT - 1) / ENC_NT), M);
 #define GB_ENC(DS)                                                                                               \
   {                                                                                                              \
@@ -312,7 +420,7 @@ cudaError_t launch_pq_encode(const float* x, int64_t ldx, int64_t n, const float
           cudaFuncSetAttribute(pq_encode_kernel<DS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);     \
       if (e != cudaSuccess) return e;                                                                            \
     }                                                                                                            \
-    pq_encode_kernel<DS><<<grid, ENC_NT, smem, st>>>(x, ldx, n, coarse, ldc, assign, pq_centroids, M, dsub, codes); \
+    pq_encode_kernel<DS><<<grid, ENC_NT, smem, st>>>(x, ldx, n, coarse, ldc, assign, pq_centroids, M, dsub, ksub, codes); \
     note_launch(); \
   }
   switch (dsub) {
@@ -324,6 +432,14 @@ cudaError_t launch_pq_encode(const float* x, int64_t ldx, int64_t n, const float
     default: GB_ENC(0) break;
   }
 #undef GB_ENC
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pq_pack_codes(const uint8_t* codes, int64_t n, int M, int nbits, uint8_t* packed, cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
+  if (nbits < 1 || nbits > 8) return cudaErrorInvalidValue;
+  pq_pack_codes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(codes, n, M, nbits, packed);
+  note_launch();
   return cudaGetLastError();
 }
 

@@ -17,6 +17,14 @@
 //   list_begin(tab, list, METRIC)     when a list starts
 //   Acc, start(dis0), finish(acc)     an entry's score is finish(start(dis0) + its table entries, added in code order)
 // A hook that writes the table ends with the barrier that publishes it.
+//
+// A codec whose codes are not one per byte (bit-packed IVF-PQ) also declares kCodeSum = true and supplies
+//   table_entries()                   Entry elements of its table (a multiple of 4: the code stages behind it stay
+//                                     16-byte aligned)
+//   code_sum(code, tab, acc)          acc + the entry's table entries in code order; `code` is the entry's first byte in
+//                                     the stage, not 4-byte aligned in general; it may read the aligned 32-bit word
+//                                     holding the entry's last byte (the launcher pads the window by 16 bytes)
+// and is launched with MW = 0 only.  The other codecs keep the [code_bytes()][256] table and table_sum.
 #pragma once
 #include "common.cuh"
 
@@ -68,6 +76,37 @@ __device__ __forceinline__ Acc table_sum(const unsigned char* __restrict__ code,
   return acc;
 }
 
+// LsCodeSum<Codec>::value: the codec declares kCodeSum (and then supplies table_entries / code_sum)
+template <class Codec, class = void>
+struct LsCodeSum {
+  static constexpr bool value = false;
+};
+template <class Codec>
+struct LsCodeSum<Codec, decltype(void(Codec::kCodeSum))> {
+  static constexpr bool value = Codec::kCodeSum;
+};
+
+// Entry elements of the codec's table
+template <class Codec>
+__host__ __device__ __forceinline__ int ls_table_entries(const Codec& c) {
+  if constexpr (LsCodeSum<Codec>::value) {
+    return c.table_entries();
+  } else {
+    return c.code_bytes() * 256;
+  }
+}
+
+// an entry's sum over the table: the codec's own for kCodeSum codecs, table_sum otherwise
+template <int MW, class Codec, class Acc, class Entry>
+__device__ __forceinline__ Acc ls_entry_sum(const Codec& c, const unsigned char* code, const Entry* tab, Acc acc,
+                                            int nbytes) {
+  if constexpr (LsCodeSum<Codec>::value) {
+    return c.code_sum(code, tab, acc);
+  } else {
+    return table_sum<MW>(code, tab, acc, nbytes);
+  }
+}
+
 // the launcher's arguments; the kernel takes them one by one, with its pointers __restrict__ (passed as this struct,
 // two IVF-PQ instantiations spilled)
 struct ListScanArgs {
@@ -91,13 +130,14 @@ __global__ void __launch_bounds__(LS_NT, Codec::kMinCtasPerSm)
                      int gate_cap, const int* __restrict__ row_limit, bool sorted_out,
                      unsigned long long* __restrict__ partial, int tile_e, int KP, int SORTN) {
   using Entry = typename Codec::Entry;
+  static_assert(!LsCodeSum<Codec>::value || MW == 0, "a kCodeSum codec runs the generic layout only");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int cb = c.code_bytes();
   const int tile_bytes = tile_e * cb;
   // the table sits at the start of the dynamic window: its shared address is a link-time constant, so every gather is
   // LDS [byte_offset + imm]  with no base add
   Entry* tab = reinterpret_cast<Entry*>(smem_raw);
-  unsigned long long* buf = reinterpret_cast<unsigned long long*>(tab + cb * 256);
+  unsigned long long* buf = reinterpret_cast<unsigned long long*>(tab + ls_table_entries(c));
   unsigned char* stages = reinterpret_cast<unsigned char*>(buf + SORTN);
   __shared__ __align__(8) uint64_t full_bar[LS_NST];
   __shared__ int s_cnt;
@@ -214,7 +254,7 @@ __global__ void __launch_bounds__(LS_NT, Codec::kMinCtasPerSm)
     } else {
       for (int u = 0; u < per_thread; u++) {
         const int e = u * LS_NT + tid;
-        consider(e, e < n_e ? c.finish(table_sum<MW>(st + (size_t)e * cb, tab, c.start(dis0), cb)) : 0.f);
+        consider(e, e < n_e ? c.finish(ls_entry_sum<MW>(c, st + (size_t)e * cb, tab, c.start(dis0), cb)) : 0.f);
       }
     }
     // stage consumed + pushes done; the count is identical in every thread (no 2nd barrier needed)
@@ -269,8 +309,8 @@ cudaError_t launch_list_scan(const Codec& c, int nq, const ListScanArgs& a, cuda
   const int tile_e = c.tile_entries();
   const int KP = next_pow2(a.k < 16 ? 16 : a.k);
   const int SORTN = next_pow2(KP + tile_e + tile_e / 2);  // cap >= tile_e: one tile always fits after a flush
-  const size_t smem = (size_t)c.code_bytes() * 256 * sizeof(typename Codec::Entry) + (size_t)SORTN * 8 +
-                      (size_t)LS_NST * tile_e * c.code_bytes();
+  const size_t smem = (size_t)ls_table_entries(c) * sizeof(typename Codec::Entry) + (size_t)SORTN * 8 +
+                      (size_t)LS_NST * tile_e * c.code_bytes() + (LsCodeSum<Codec>::value ? 16 : 0);
   if (smem > 227 * 1024) return cudaErrorInvalidValue;
   cudaError_t e =
       cudaFuncSetAttribute(list_scan_kernel<Codec, METRIC, MW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -221,7 +221,7 @@ class GammaIndex:
 
     @property
     def pq_ksub(self):
-        """Centroids per sub-quantiser: 256 (IVFPQ), 16 (IVFPQFastScan)."""
+        """Centroids per sub-quantiser: 2^nbits_per_idx (IVFPQ; 256 at the default 8 bits), 16 (IVFPQFastScan)."""
         return int(_lib.lib().gb_index_pq_ksub(self._h))
 
     def set_pq_centroids(self, pq):
@@ -236,7 +236,8 @@ class GammaIndex:
         return out
 
     def get_precomputed_table(self):
-        out = np.empty((self.nlist, self.pq_m, 256), np.float32)
+        """IVFPQ under L2: T[l][m][c] = |pq_m[c]|^2 + 2 <centroid_l|m, pq_m[c]>, shape (nlist, M, pq_ksub)."""
+        out = np.empty((self.nlist, self.pq_m, self.pq_ksub), np.float32)
         _check(_lib.lib().gb_index_get_precomputed_table(self._h, _ptr(out)), "get_precomputed_table")
         return out
 
@@ -354,7 +355,7 @@ class GammaIndex:
 
 
 def index_factory(d, description, metric=METRIC_L2, device=0, **extra):
-    """index/index.h index_factory: "IVF1024,Flat" | "IVF4096,PQ16x8" | "Flat"."""
+    """index/index.h index_factory: "IVF1024,Flat" | "IVF4096,PQ16x8" | "IVF256,PQ32x4" (PQ<M>x<nbits>) | "Flat"."""
     parts = [p.strip() for p in description.split(",")]
     params = dict(extra)
     params["metric_type"] = "L2" if metric == METRIC_L2 else "InnerProduct"
