@@ -34,7 +34,8 @@ long long gb_launch_count(void);
  * (index/reflector.h:68-80, vector/vector_manager.cc:171; gamma_index_ivfflat.cc:215-291,
  * gamma_index_ivfpq.cc:112-231).  index_type: "FLAT" | "IVFFLAT" | "IVFPQ".
  * model_params_json keys: ncentroids, nprobe, metric_type ("L2"|"InnerProduct"), nsubvector,
- * nbits_per_idx (IVFPQ: 1..8), training_threshold, bucket_init_size, bucket_max_size (may be NULL/""). */
+ * nbits_per_idx (IVFPQ: 1..8), training_threshold, bucket_init_size, bucket_max_size, store_type ("RocksDB", any
+ * case: raw vectors in pinned host memory; anything else: in HBM) (may be NULL/""). */
 gb_index *gb_index_create(const char *index_type, int dimension, const char *model_params_json, int device);
 void gb_index_destroy(gb_index *index);
 
@@ -59,7 +60,7 @@ int64_t gb_index_ntotal(gb_index *index);        /* stored vectors */
 int64_t gb_index_indexed_count(gb_index *index); /* vectors present in the index */
 int gb_index_is_trained(gb_index *index);
 int gb_index_training_threshold(gb_index *index);
-int64_t gb_index_mem_bytes(gb_index *index, int which /* 0 = index, 1 = raw vectors */);
+int64_t gb_index_mem_bytes(gb_index *index, int which /* 0 = index, 1 = raw vectors in HBM, 2 = raw vectors in host memory */);
 
 /* IndexModel::Search (index_model.h:296-298) with the RetrievalContext flattened:
  * retrieval_params_json = the request's index_params (nprobe, metric_type, recall_num,

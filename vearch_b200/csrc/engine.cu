@@ -316,6 +316,7 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
   if (table_index_params.empty() && mp.training_threshold > training_threshold_)
     training_threshold_ = mp.training_threshold;  // table.cc:143-150
   if (training_threshold_ > 0) mp.training_threshold = training_threshold_;
+  mp.host_store = !strcasecmp(v.str(4).c_str(), "RocksDB");  // VectorInfo.store_type
   Index* idx = create_index(index_type_, dim_, mp, device_, 20);
   if (!idx) return Status::Make(index_type_ == "FLAT" || index_type_ == "IVFFLAT" || index_type_ == "IVFPQ" ||
                                         index_type_ == "IVFPQFastScan"
@@ -342,6 +343,7 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     ModelParams emp;
     if (!parse_model_params(vf.index_params, &emp, &err)) return Status::Make(kInvalidArgument, err);
     if (training_threshold_ > 0) emp.training_threshold = training_threshold_;
+    emp.host_store = !strcasecmp(ev.str(4).c_str(), "RocksDB");
     Index* eidx = create_index(vf.index_type, vf.dim, emp, device_, 20);
     if (!eidx) return Status::Make(kInvalidArgument, last_error());
     vf.index.reset(eidx);
@@ -1244,8 +1246,10 @@ std::string Engine::MemoryInfo() {  // search/engine.cc:1178-1200
   for (auto& col : values_)
     for (auto& v : col) table_mem += (long long)v.size() + (long long)sizeof(std::string);
   long long index_mem = index_ ? index_->index_mem_bytes() : 0;
-  long long vec_mem = index_ ? index_->store().mem_bytes() : 0;
-  for (auto& e : extra_) index_mem += e.index->index_mem_bytes(), vec_mem += e.index->store().mem_bytes();
+  // raw vectors wherever they are placed: HBM, or pinned host memory (store_type "RocksDB")
+  long long vec_mem = index_ ? index_->store().mem_bytes() + index_->store().host_bytes() : 0;
+  for (auto& e : extra_)
+    index_mem += e.index->index_mem_bytes(), vec_mem += e.index->store().mem_bytes() + e.index->store().host_bytes();
   char buf[256];
   snprintf(buf, sizeof buf,
            "{\"bitmap_mem\":%lld,\"field_range_mem\":0,\"index_mem\":%lld,\"table_mem\":%lld,\"vector_mem\":%lld}",

@@ -111,13 +111,18 @@ const VmmApi& vmm_api() {
 }
 }  // namespace
 
-RawStore::RawStore(int d, int seg_shift) : d_(d), dpad_((int)round_up(d, 4)), seg_shift_(seg_shift) {
+RawStore::RawStore(int d, int seg_shift, bool host)
+    : d_(d), dpad_((int)round_up(d, 4)), seg_shift_(host ? std::min(seg_shift, kHostSegShift) : seg_shift), host_(host) {
   cudaMalloc(&d_segs_, sizeof(float*) * kMaxSegs);
   cudaGetDevice(&device_);
 }
 RawStore::~RawStore() {
   const VmmApi& api = vmm_api();
   for (Seg& sg : segs_) {
+    if (host_) {
+      cudaFreeHost(sg.base);
+      continue;
+    }
     if (!sg.vmm) {
       cudaFree(sg.base);
       continue;
@@ -139,6 +144,22 @@ int RawStore::new_segment() {
   }
   Seg sg;
   const size_t bytes = (size_t)seg_rows() * dpad_ * 4;
+  if (host_) {  // pinned, mapped into every device's address space; kernels read it through the device pointer
+    GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&sg.base), bytes, cudaHostAllocMapped | cudaHostAllocPortable));
+    memset(sg.base, 0, bytes);  // pad columns must read as zero
+    float* dev = nullptr;
+    const cudaError_t e = cudaHostGetDevicePointer(reinterpret_cast<void**>(&dev), sg.base, 0);
+    if (e != cudaSuccess) {
+      cudaFreeHost(sg.base);
+      set_last_error(std::string("raw store: cudaHostGetDevicePointer: ") + cudaGetErrorString(e));
+      return -1;
+    }
+    sg.mapped = bytes;
+    host_bytes_ += (int64_t)bytes;
+    segs_.push_back(sg);
+    GB_CUDA(cudaMemcpy(d_segs_ + segs_.size() - 1, &dev, sizeof(float*), cudaMemcpyHostToDevice));
+    return 0;
+  }
   const VmmApi& api = vmm_api();
   if (api.ok) {
     CUmemAllocationProp prop = {};
@@ -211,6 +232,9 @@ int RawStore::ensure(int64_t n_total) {
   }
   return 0;
 }
+// Host placement: the segments are ordinary (pinned) host memory, so host rows move with memcpy and device rows with
+// device-to-host copies.  A search may still be reading a row when update_host overwrites it: the caller holds the
+// index lock exclusively and has drained in-flight searches first (Index::update_vector).
 int RawStore::append_host(const float* x, int64_t n, cudaStream_t st) {
   if (ensure(n_ + n)) return -1;
   int64_t done = 0;
@@ -218,8 +242,12 @@ int RawStore::append_host(const float* x, int64_t n, cudaStream_t st) {
     int64_t vid = n_ + done;
     int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
     int64_t cnt = std::min(n - done, seg_rows() - off);
-    GB_CUDA(cudaMemcpy2DAsync(segs_[si].base + off * dpad_, (size_t)dpad_ * 4, x + done * d_, (size_t)d_ * 4, (size_t)d_ * 4,
-                              (size_t)cnt, cudaMemcpyHostToDevice, st));
+    if (host_) {
+      for (int64_t i = 0; i < cnt; i++) memcpy(segs_[si].base + (off + i) * dpad_, x + (done + i) * d_, (size_t)d_ * 4);
+    } else {
+      GB_CUDA(cudaMemcpy2DAsync(segs_[si].base + off * dpad_, (size_t)dpad_ * 4, x + done * d_, (size_t)d_ * 4,
+                                (size_t)d_ * 4, (size_t)cnt, cudaMemcpyHostToDevice, st));
+    }
     done += cnt;
   }
   GB_CUDA(cudaStreamSynchronize(st));
@@ -234,7 +262,7 @@ int RawStore::append_device(const float* x, int64_t ld, int64_t n, cudaStream_t 
     int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
     int64_t cnt = std::min(n - done, seg_rows() - off);
     GB_CUDA(cudaMemcpy2DAsync(segs_[si].base + off * dpad_, (size_t)dpad_ * 4, x + done * ld, (size_t)ld * 4,
-                              (size_t)d_ * 4, (size_t)cnt, cudaMemcpyDeviceToDevice, st));
+                              (size_t)d_ * 4, (size_t)cnt, host_ ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, st));
     done += cnt;
   }
   GB_CUDA(cudaStreamSynchronize(st));
@@ -244,6 +272,10 @@ int RawStore::append_device(const float* x, int64_t ld, int64_t n, cudaStream_t 
 int RawStore::update_host(int64_t vid, const float* x, cudaStream_t st) {
   if (vid < 0 || vid >= n_) return -1;
   int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
+  if (host_) {
+    memcpy(segs_[si].base + off * dpad_, x, (size_t)d_ * 4);
+    return 0;
+  }
   GB_CUDA(cudaMemcpyAsync(segs_[si].base + off * dpad_, x, (size_t)d_ * 4, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaStreamSynchronize(st));
   return 0;
@@ -251,6 +283,10 @@ int RawStore::update_host(int64_t vid, const float* x, cudaStream_t st) {
 int RawStore::get_host(int64_t vid, float* out) const {
   if (vid < 0 || vid >= n_) return -1;
   int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
+  if (host_) {
+    memcpy(out, segs_[si].base + off * dpad_, (size_t)d_ * 4);
+    return 0;
+  }
   GB_CUDA(cudaMemcpy(out, segs_[si].base + off * dpad_, (size_t)d_ * 4, cudaMemcpyDeviceToHost));
   return 0;
 }
@@ -261,24 +297,37 @@ int RawStore::get_rows_host(int64_t start, int64_t n, float* out) const {
     int64_t vid = start + done;
     int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
     int64_t cnt = std::min(n - done, seg_rows() - off);
-    GB_CUDA(cudaMemcpy2D(out + done * d_, (size_t)d_ * 4, segs_[si].base + off * dpad_, (size_t)dpad_ * 4, (size_t)d_ * 4,
-                         (size_t)cnt, cudaMemcpyDeviceToHost));
+    if (host_) {
+      for (int64_t i = 0; i < cnt; i++) memcpy(out + (done + i) * d_, segs_[si].base + (off + i) * dpad_, (size_t)d_ * 4);
+    } else {
+      GB_CUDA(cudaMemcpy2D(out + done * d_, (size_t)d_ * 4, segs_[si].base + off * dpad_, (size_t)dpad_ * 4,
+                           (size_t)d_ * 4, (size_t)cnt, cudaMemcpyDeviceToHost));
+    }
     done += cnt;
   }
   return 0;
 }
-const float* RawStore::contiguous(int64_t n, Scratch& s) {
-  if (n <= seg_rows()) return segs_.empty() ? nullptr : segs_[0].base;
-  float* buf = s.alloc_n<float>((size_t)n * dpad_);
-  if (!buf) return nullptr;
+cudaError_t RawStore::copy_rows_to_device(int64_t start, int64_t n, float* dst, cudaStream_t st) const {
   int64_t done = 0;
   while (done < n) {
-    int64_t si = done >> seg_shift_;
-    int64_t cnt = std::min(n - done, seg_rows());
-    if (cudaMemcpyAsync(buf + done * dpad_, segs_[si].base, (size_t)cnt * dpad_ * 4, cudaMemcpyDeviceToDevice,
-                        s.stream()) != cudaSuccess)
-      return nullptr;
+    int64_t vid = start + done;
+    int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
+    int64_t cnt = std::min(n - done, seg_rows() - off);
+    const cudaError_t e = cudaMemcpyAsync(dst + done * dpad_, segs_[si].base + off * dpad_, (size_t)cnt * dpad_ * 4,
+                                          host_ ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st);
+    if (e != cudaSuccess) return e;
     done += cnt;
+  }
+  return cudaSuccess;
+}
+const float* RawStore::contiguous(int64_t n, Scratch& s) {
+  if (!host_ && n <= seg_rows()) return segs_.empty() ? nullptr : segs_[0].base;
+  float* buf = s.alloc_n<float>((size_t)n * dpad_);
+  if (!buf) return nullptr;
+  const cudaError_t e = copy_rows_to_device(0, n, buf, s.stream());
+  if (e != cudaSuccess) {
+    set_last_error(std::string("raw store: copy of the training rows: ") + cudaGetErrorString(e));
+    return nullptr;
   }
   return buf;
 }
@@ -478,7 +527,7 @@ Index::Index(const std::string& type, int d, const ModelParams& mp, int device, 
     (void)hooked;
     live_indexes().all.push_back(this);
   }
-  store_.reset(new RawStore(d, seg_shift));
+  store_.reset(new RawStore(d, seg_shift, mp.host_store));
   cudaStreamCreateWithFlags(&build_stream_, cudaStreamNonBlocking);
 }
 void Index::quiesce() {
@@ -639,6 +688,51 @@ int Index::add_vectors_device(const float* x, int64_t ld, int64_t n) {
   cudaSetDevice(device_);
   std::unique_lock<std::shared_mutex> lk(mu_);
   return store_->append_device(x, ld, n, build_stream_);
+}
+
+const float* Index::store_rows_dev(int64_t vid0, int64_t n, Scratch& s) {
+  const int64_t si = vid0 >> store_->seg_shift(), off = vid0 & (store_->seg_rows() - 1);
+  if (!store_->on_host()) return store_->seg((int)si) + off * dpad_;
+  float* buf = s.alloc_n<float>((size_t)n * dpad_);
+  if (!buf) return nullptr;
+  const cudaError_t e = store_->copy_rows_to_device(vid0, n, buf, s.stream());
+  if (e != cudaSuccess) {
+    set_last_error(std::string("raw store: copy of rows to the device: ") + cudaGetErrorString(e));
+    return nullptr;
+  }
+  return buf;
+}
+
+Index::CopyLane::~CopyLane() {
+  for (int b = 0; b < 2; b++) {
+    if (copied[b]) cudaEventDestroy(copied[b]);
+    if (reusable[b]) cudaEventDestroy(reusable[b]);
+  }
+  if (cs) cudaStreamDestroy(cs);
+}
+Index::CopyLane* Index::lane_acquire() {
+  std::lock_guard<std::mutex> g(lane_mu_);
+  if (!free_lanes_.empty()) {
+    CopyLane* l = free_lanes_.back();
+    free_lanes_.pop_back();
+    return l;
+  }
+  std::unique_ptr<CopyLane> l(new CopyLane);
+  cudaError_t e = cudaStreamCreateWithFlags(&l->cs, cudaStreamNonBlocking);
+  for (int b = 0; b < 2 && e == cudaSuccess; b++) {
+    e = cudaEventCreateWithFlags(&l->copied[b], cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&l->reusable[b], cudaEventDisableTiming);
+  }
+  if (e != cudaSuccess) {
+    set_last_error(std::string("copy stream for the host store: ") + cudaGetErrorString(e));
+    return nullptr;
+  }
+  lanes_.push_back(std::move(l));
+  return lanes_.back().get();
+}
+void Index::lane_release(CopyLane* l) {
+  std::lock_guard<std::mutex> g(lane_mu_);
+  free_lanes_.push_back(l);
 }
 
 int Index::upload_bitmaps(const SearchContext& ctx, FilterArgs* f, Scratch& s) {
@@ -897,6 +991,45 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
     if (!partial) return -1;
   }
   last_scan_kernel_ = "dist_tile_kernel+select_rows_kernel";
+  if (store_->on_host()) {
+    // Host placement: each chunk is copied once, on a copy stream, into one of two HBM staging buffers, so the copy of
+    // chunk c + 1 overlaps the distance and select kernels of chunk c.  The chunks, kernels and partial merge are those
+    // of the HBM store, so the keys are the same; the scan runs at PCIe speed, not at HBM speed.
+    struct LaneScope {  // the lane goes back to the pool on every exit path, once this search's copies are enqueued
+      Index* ix;
+      CopyLane* l;
+      ~LaneScope() {
+        if (l) ix->lane_release(l);
+      }
+    } lane{this, lane_acquire()};
+    if (!lane.l) return -1;
+    CopyLane& cl = *lane.l;
+    float* stage[2];
+    for (int b = 0; b < 2; b++) {
+      stage[b] = s.alloc_n<float>((size_t)CC * dpad_);
+      if (!stage[b]) return -1;
+      GB_CUDA(cudaEventRecord(cl.reusable[b], st));  // the buffers are allocated in stream order on st
+    }
+    scan_timer_begin(st);
+    for (int c = 0; c < nch; c++) {
+      const int b = c & 1;
+      GB_CUDA(cudaStreamWaitEvent(cl.cs, cl.reusable[b], 0));
+      GB_CUDA(cudaMemcpyAsync(stage[b], chunks[c].base, (size_t)chunks[c].cnt * dpad_ * 4, cudaMemcpyHostToDevice, cl.cs));
+      GB_CUDA(cudaEventRecord(cl.copied[b], cl.cs));
+      GB_CUDA(cudaStreamWaitEvent(st, cl.copied[b], 0));
+      for (int q0 = 0; q0 < nq; q0 += QB) {
+        int qb = std::min(QB, nq - q0);
+        GB_CUDA(launch_dist_matrix(xq + (int64_t)q0 * dpad_, dpad_, qb, stage[b], dpad_, chunks[c].cnt, dpad_, metric,
+                                   scores, ldo, st));
+        GB_CUDA(launch_select_scores(scores, ldo, qb, chunks[c].cnt, chunks[c].id0, k, metric, f,
+                                     partial + ((int64_t)q0 * nch + c) * k, (int64_t)nch * k, st));
+      }
+      GB_CUDA(cudaEventRecord(cl.reusable[b], st));
+    }
+    if (nch > 1) GB_CUDA(launch_select_keys(partial, (int64_t)nch * k, nq, nch * k, k, out_keys, k, st));
+    scan_timer_end(st);
+    return 0;
+  }
   scan_timer_begin(st);
   for (int q0 = 0; q0 < nq; q0 += QB) {
     int qb = std::min(QB, nq - q0);
@@ -1078,6 +1211,7 @@ IVFFlatIndex::~IVFFlatIndex() {
   if (mirror_.base) cudaFree(mirror_.base);
   if (mirror_.norms) cudaFree(mirror_.norms);
   if (mirror_.d_tile0) cudaFree(mirror_.d_tile0);
+  if (d_rowptr_) cudaFree(d_rowptr_);
 }
 int IvfIndex::rebuild_centroid_tiles(cudaStream_t st) {
   GB_CUDA(launch_tc_stage_rows(d_centroids_, dpad_, nlist_, dpad_, (int)round_up(dpad_, 16), d_cent_tiles_, d_cent_norms_, st));
@@ -1098,7 +1232,9 @@ int64_t IvfIndex::index_mem_bytes() const {
   const int64_t cent_tiles = (nlist_ + 127) / 128 * tc_tile_bytes(dpad_);
   return (int64_t)nlist_ * dpad_ * 4 + cent_tiles + (lists_ ? lists_->mem_bytes() : 0);
 }
-int64_t IVFFlatIndex::index_mem_bytes() const { return IvfIndex::index_mem_bytes() + mirror_.cap_tiles * tc_tile_bytes(dpad_); }
+int64_t IVFFlatIndex::index_mem_bytes() const {
+  return IvfIndex::index_mem_bytes() + mirror_.cap_tiles * tc_tile_bytes(dpad_) + rowptr_cap_ * (int64_t)sizeof(float*);
+}
 int IvfIndex::set_centroids(const float* host, int nlist) {
   if (nlist != nlist_) {
     set_last_error("set_centroids: nlist mismatch");
@@ -1207,6 +1343,7 @@ int IvfIndex::index_batch(const float* x, int64_t n, int64_t vid0, const uint8_t
   // data first, the new lengths last (realtime_mem_data.cc:292-293)
   if (append_batch(x, n, vid0, d_list, d_pos, add, s)) return -1;
   if (lists_->commit(add, st)) return -1;
+  if (lists_changed(st)) return -1;
   GB_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
@@ -1219,12 +1356,17 @@ int IvfIndex::add_pending(const uint8_t* del_bitmap) {
   for (;;) {
     int64_t vid0 = indexed_count_, n = 0;
     const float* x = nullptr;
+    Scratch s(build_stream_);
     {  // add_vectors (exclusive mu_) may append segments while we look: the segment table is read under the shared lock
       std::shared_lock<std::shared_mutex> lk(mu_);
       if (vid0 >= store_->size()) break;
-      int64_t si = vid0 >> store_->seg_shift(), off = vid0 & (store_->seg_rows() - 1);
-      n = std::min<int64_t>(std::min(store_->size() - vid0, store_->seg_rows() - off), BATCH);
-      x = store_->seg((int)si) + off * dpad_;
+      // HBM rows are indexed in place, so a batch ends at its segment's end.  Host rows are copied to HBM first, across
+      // segments: their batches end at the same BATCH-aligned rows, so both placements build the same list layout.
+      const int64_t span = store_->on_host() ? BATCH : store_->seg_rows();
+      int64_t off = vid0 & (span - 1);
+      n = std::min<int64_t>(std::min(store_->size() - vid0, span - off), BATCH);
+      x = store_rows_dev(vid0, n, s);
+      if (!x) return -1;
     }
     if (index_batch(x, n, vid0, del_bitmap)) return -1;
     indexed_count_ += n;
@@ -1233,7 +1375,7 @@ int IvfIndex::add_pending(const uint8_t* del_bitmap) {
   // waste is worth a copy (more than half of the live bytes and more than 1 GiB)
   if (lists_ && lists_->mem_bytes() - lists_->packed_bytes() > std::max<int64_t>((int64_t)1 << 30, lists_->packed_bytes() / 2)) {
     std::unique_lock<std::shared_mutex> lk(mu_);
-    if (lists_->compact(build_stream_)) return -1;
+    if (compact_locked()) return -1;
   }
   return 0;
 }
@@ -1261,12 +1403,40 @@ int IvfIndex::compact_lists() {
   if (!lists_) return 0;
   cudaSetDevice(device_);
   std::unique_lock<std::shared_mutex> lk(mu_);
-  return lists_->compact(build_stream_);
+  return compact_locked();
+}
+int IvfIndex::compact_locked() {
+  if (lists_->compact(build_stream_) || lists_changed(build_stream_)) return -1;
+  GB_CUDA(cudaStreamSynchronize(build_stream_));
+  return 0;
+}
+
+// Host placement: the winner re-score of the list-major scan reads the list rows, byte copies of the raw rows, through
+// a per-vid row-pointer table, so an IVF-Flat search never reads host memory.  Rebuilt whole after every change of the
+// lists (growth and compaction move them), with mu_ held exclusively and earlier searches drained.
+int IVFFlatIndex::lists_changed(cudaStream_t st) {
+  if (!store_->on_host() || !lists_) return 0;
+  drain_searches();  // no kernel of an earlier search reads the table while it is rewritten or freed
+  const int64_t need = (int64_t)vid2pos_.size();
+  if (need > rowptr_cap_) {
+    const int64_t cap = std::max<int64_t>(need, rowptr_cap_ + rowptr_cap_ / 2);
+    const float** p = nullptr;
+    GB_CUDA(cudaMalloc(&p, (size_t)cap * sizeof(float*)));
+    GB_CUDA(cudaMemsetAsync(p, 0, (size_t)cap * sizeof(float*), st));
+    if (d_rowptr_) GB_CUDA(cudaFree(d_rowptr_));
+    d_rowptr_ = p;
+    rowptr_cap_ = cap;
+  }
+  GB_CUDA(launch_ivf_rowptrs(lists_->directory(), dpad_, d_rowptr_, st));
+  return 0;
 }
 
 int Index::update_vector(int64_t vid, const float* x) {
   cudaSetDevice(device_);
   std::unique_lock<std::shared_mutex> lk(mu_);
+  // host rows are overwritten by the CPU at once, not in stream order: no kernel or copy of an earlier search may still
+  // read them
+  if (store_->on_host()) drain_searches();
   return store_->update_host(vid, x, build_stream_);
 }
 
@@ -1280,8 +1450,10 @@ int IvfIndex::update_vector(int64_t vid, const float* x) {
     std::unique_lock<std::shared_mutex> lk(mu_);
     if (lists_->tombstone((int)(vid2pos_[vid] >> 32), (int)(uint32_t)vid2pos_[vid], build_stream_)) return -1;
   }
-  int64_t si = vid >> store_->seg_shift(), off = vid & (store_->seg_rows() - 1);
-  return index_batch(store_->seg((int)si) + off * dpad_, 1, vid, nullptr);
+  Scratch s(build_stream_);
+  const float* x_dev = store_rows_dev(vid, 1, s);
+  if (!x_dev) return -1;
+  return index_batch(x_dev, 1, vid, nullptr);
 }
 
 int IvfIndex::resolve_nprobe(const SearchContext& ctx) const {
@@ -1547,8 +1719,16 @@ int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int me
   if (lm < 0) return lm;
   if (lm == 0) {
     if ((dpad_ & 3) == 0 && k <= 8192) {
-      GB_CUDA(launch_rerank(lm_keys, k, nq, xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_, k, metric, f,
-                            out_keys, st));
+      if (store_->on_host()) {  // the list rows, through the row-pointer table (lists_changed)
+        if (!d_rowptr_) {
+          set_last_error("IVFFLAT: the row-pointer table of the host store was not built");
+          return -1;
+        }
+        GB_CUDA(launch_rerank(lm_keys, k, nq, xq, dpad_, dpad_, d_rowptr_, 0, dpad_, false, k, metric, f, out_keys, st));
+      } else {
+        GB_CUDA(launch_rerank(lm_keys, k, nq, xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_, false, k,
+                              metric, f, out_keys, st));
+      }
     } else {
       GB_CUDA(cudaMemcpyAsync(out_keys, lm_keys, (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, st));
     }
@@ -2157,8 +2337,9 @@ int IvfPqBase::scan_pq_dev(const char* kernel, const SearchContext& ctx, const F
   }
   if (rerank) {
     StageScope stage(this, "rerank_kernel", st);
-    GB_CUDA(launch_rerank(keys, kk, nq, rerank_xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_, k, metric, f,
-                          out_keys, st));
+    // host placement: the candidate rows come over PCIe straight from the mapped segments
+    GB_CUDA(launch_rerank(keys, kk, nq, rerank_xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_,
+                          store_->on_host(), k, metric, f, out_keys, st));
   }
   return 0;
 }

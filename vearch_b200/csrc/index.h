@@ -53,18 +53,26 @@ class Scratch {
 };
 
 // MemoryRawVector on device (vector/memory_raw_vector.cc:152-240): append-only fp32 rows kept in
-// fixed-size HBM segments, row stride dpad (d rounded up to 4 floats, zero padded).
+// fixed-size segments, row stride dpad (d rounded up to 4 floats, zero padded).  The segments are in HBM, or, for a
+// field whose store_type is "RocksDB" (host placement), in pinned host memory mapped into the device's address space:
+// kernels then read rows over PCIe through the same segment table, and the partition's HBM holds only its index.
 class RawStore {
  public:
-  RawStore(int d, int seg_shift);
+  // host placement: segments of 2^kHostSegShift rows (32 MiB at d = 128), so a small partition pins little memory;
+  // kMaxSegs of them still cover 2^32 rows
+  static constexpr int kHostSegShift = 16;
+  RawStore(int d, int seg_shift, bool host);
   ~RawStore();
   int d() const { return d_; }
   int dpad() const { return dpad_; }
   int64_t size() const { return n_; }
+  bool on_host() const { return host_; }
   int seg_shift() const { return seg_shift_; }
   int64_t seg_rows() const { return (int64_t)1 << seg_shift_; }
   int nsegs() const { return (int)segs_.size(); }
+  // a segment's base: device memory, or (host placement) the pinned host rows, for copies
   const float* seg(int i) const { return segs_[i].base; }
+  // device-visible segment bases [kMaxSegs], what kernels index rows through
   const float* const* d_segs() const { return d_segs_; }
   // rows: n x d floats (stride d) on host, or n x dpad (stride ld) on device
   int append_host(const float* x, int64_t n, cudaStream_t st);
@@ -74,7 +82,10 @@ class RawStore {
   int get_rows_host(int64_t start, int64_t n, float* out) const;  // n x d, stride d
   // contiguous copy of rows [0, n) (training slab, GetVectorHeader): returns device ptr, owned by `s`
   const float* contiguous(int64_t n, Scratch& s);
-  int64_t mem_bytes() const { return phys_bytes_; }  // physical HBM behind the store
+  // rows [start, start + n) (n x dpad) into device memory at dst, ordered on st
+  cudaError_t copy_rows_to_device(int64_t start, int64_t n, float* dst, cudaStream_t st) const;
+  int64_t mem_bytes() const { return phys_bytes_; }  // physical HBM behind the store (0 for host placement)
+  int64_t host_bytes() const { return host_bytes_; }  // pinned host memory behind the store
 
  private:
   int ensure(int64_t n_total);
@@ -87,7 +98,8 @@ class RawStore {
     std::vector<std::pair<unsigned long long, size_t>> chunks;  // (CUmemGenericAllocationHandle, bytes), in address order
   };
   int d_, dpad_, seg_shift_, device_ = 0;
-  int64_t n_ = 0, phys_bytes_ = 0;
+  bool host_;
+  int64_t n_ = 0, phys_bytes_ = 0, host_bytes_ = 0;
   std::vector<Seg> segs_;
   float** d_segs_ = nullptr;  // device array [kMaxSegs]
   static constexpr int kMaxSegs = 65536;
@@ -156,6 +168,7 @@ struct ModelParams {  // index/impl/gamma_index_ivfpq.h:1031-1257, gamma_index_i
   int opq_nsubvector = 0;       // > 0: OPQ rotation in front of the IVFPQ index (gamma_index_ivfpq.h:1202-1216)
   bool has_opq = false;         // an "opq" object was given (IVFPQFastScan refuses it)
   int bbs = 32;                 // IVFPQFastScan block size as given (gamma_index_ivfpqfs.h:126-133; <= 0 => 32)
+  bool host_store = false;      // raw vectors in pinned host memory (store_type "RocksDB"); otherwise in HBM
 };
 
 struct RetrievalParams {  // gamma_index_ivfpq.cc:233-294, gamma_index_ivfflat.cc:293-340
@@ -232,6 +245,21 @@ class Index {
   virtual int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
                               unsigned long long* out_keys, Scratch& s) = 0;
   int upload_bitmaps(const SearchContext& ctx, FilterArgs* f, Scratch& s);
+  // rows [vid0, vid0 + n) as device rows (stride dpad): in HBM the segment itself (the rows must lie in one segment),
+  // for host placement a copy in `s`, ordered on its stream (any rows)
+  const float* store_rows_dev(int64_t vid0, int64_t n, Scratch& s);
+  // A copy stream and its events for the staged FLAT scan of a host store (flat_search_dev).  Created on first use and
+  // pooled: a search holds a lane while it enqueues its copies; what it enqueued keeps the events' records it waited on.
+  struct CopyLane {
+    cudaStream_t cs = nullptr;
+    cudaEvent_t copied[2] = {nullptr, nullptr}, reusable[2] = {nullptr, nullptr};
+    ~CopyLane();
+  };
+  CopyLane* lane_acquire();  // nullptr on failure (last_error set)
+  void lane_release(CopyLane* l);
+  std::mutex lane_mu_;
+  std::vector<std::unique_ptr<CopyLane>> lanes_;
+  std::vector<CopyLane*> free_lanes_;
 
   std::string type_;
   int d_, dpad_, device_;
@@ -423,6 +451,9 @@ class IvfIndex : public Index {
 
   // index rows [vid0, vid0+n) (device pointer x, stride dpad) into the lists
   int index_batch(const float* x, int64_t n, int64_t vid0, const uint8_t* del_bitmap);
+  // after every change of the lists (append, compaction), with mu_ held exclusively, ordered on st
+  virtual int lists_changed(cudaStream_t st) { (void)st; return 0; }
+  int compact_locked();  // lists_->compact + lists_changed, with mu_ held exclusively
 
   int nlist_;
   float* d_centroids_ = nullptr;  // [nlist][dpad]
@@ -456,6 +487,10 @@ class IVFFlatIndex : public IvfIndex {
   int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
                    const std::vector<int>& add, Scratch& s) override;
   void reset_codec() override;
+  int lists_changed(cudaStream_t st) override;
+  // host placement: rowptr[vid] = the list row holding vid, for the winner re-score (lists_changed)
+  const float** d_rowptr_ = nullptr;
+  int64_t rowptr_cap_ = 0;
 
   // Tensor-core mirror of the lists (kernels_tc.cu): every list once more, pre-split and
   // pre-tiled in the shared-memory operand layout so the list-major kernel is fed by cp.async.bulk.

@@ -88,6 +88,10 @@ bool parse_model_params(const std::string& text, ModelParams* mp, std::string* e
   // the block size has no effect here beyond being checked
   if (jv.get_int("bbs", &v)) mp->bbs = v;
   if (jv.get_int("training_threshold", &v) && v > 0) mp->training_threshold = v;
+  // placement of the raw vectors (VectorManager::DetermineVectorStorageType, vector_manager.cc:50-89): "RocksDB" keeps
+  // them out of HBM, in pinned host memory; every other value, and none, keeps them in HBM
+  std::string stt;
+  if (jv.get_string("store_type", &stt)) mp->host_store = !strcasecmp("RocksDB", stt.c_str());
   std::string mt;
   if (jv.get_string("metric_type", &mt)) {
     if (strcasecmp("L2", mt.c_str()) && strcasecmp("InnerProduct", mt.c_str())) {
@@ -220,7 +224,8 @@ int gb_index_training_threshold(gb_index* index) {
 }
 int64_t gb_index_mem_bytes(gb_index* index, int which) {
   if (!index || !index->impl) return -1;
-  return which == 0 ? index->impl->index_mem_bytes() : index->impl->store().mem_bytes();
+  if (which == 0) return index->impl->index_mem_bytes();
+  return which == 2 ? index->impl->store().host_bytes() : index->impl->store().mem_bytes();
 }
 
 int gb_index_search(gb_index* index, int nq, const float* x, int k, const char* retrieval_params_json, int brute_force,

@@ -270,9 +270,10 @@ int IvfIndex::load_gamma(const std::string& dir, const std::string& abs_name, in
   {  // publish: nothing above this point changed what a search can see
     std::unique_lock<std::shared_mutex> lk(mu_);
     if (lists_->commit(add, st)) return -1;
+    vid2pos_.swap(v2p);
+    if (lists_changed(st)) return -1;  // IVF-Flat on a host store: the row pointers into the loaded lists
+    GB_CUDA(cudaStreamSynchronize(st));
   }
-  GB_CUDA(cudaStreamSynchronize(st));
-  vid2pos_.swap(v2p);
   indexed_count_ = indexed;
   *load_num = indexed;
   return 0;

@@ -208,10 +208,14 @@ cudaError_t launch_pq_rescore(const float* ip_table, int nq, const int32_t* prob
 // queries with cand_cnt > cap: out[q] = best kprime of partial[q][ngroups][kprime]
 cudaError_t launch_pq_fallback_merge(const int* cand_cnt, int cap, int nq, const unsigned long long* partial, int ngroups,
                                      int kprime, unsigned long long* out, cudaStream_t st);
-// K5r exact re-rank of ADC candidates (gamma_index_ivfpq.cc:675-726)
+// K5r exact re-rank of ADC candidates (gamma_index_ivfpq.cc:675-726).  Row of vid: raw_segments[vid >> seg_shift] +
+// (vid & (2^seg_shift - 1)) * ld_raw; seg_shift 0 makes raw_segments a per-vid row-pointer table.  host_rows: the rows
+// are in mapped host memory (a variant with more rows in flight per warp for PCIe latency).
 cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq, const float* xq, int64_t ldq, int d,
-                          const float* const* raw_segments, int seg_shift, int64_t ld_raw, int k, int metric,
-                          FilterArgs f, unsigned long long* out_keys, cudaStream_t st);
+                          const float* const* raw_segments, int seg_shift, int64_t ld_raw, bool host_rows, int k,
+                          int metric, FilterArgs f, unsigned long long* out_keys, cudaStream_t st);
+// IVF-Flat row pointers: rowptr[vid] = the list row holding vid, for every live (not tombstoned) list entry
+cudaError_t launch_ivf_rowptrs(ListDirectory dir, int ld, const float** rowptr, cudaStream_t st);
 
 // ---- K11: IVFPQFastScan (kernels_pqfs.cu): 16-centroid PQ on raw vectors, 4-bit codes, uint8 tables -------------
 // codes[i][j] = code(2j) | code(2j + 1) << 4, code(m) = argmin_c |x_i|m - pq_m[c]|^2; pq_centroids [M][16][dsub]

@@ -255,6 +255,24 @@ cudaError_t launch_ivf_append_vecs(const float* x, int64_t ldx, int64_t n, int d
   return cudaGetLastError();
 }
 
+__global__ void ivf_rowptrs_kernel(ListDirectory dir, int ld, const float** rowptr) {
+  const int l = blockIdx.x;
+  const int len = dir.len[l];
+  const int64_t* ids = dir.ids[l];
+  const float* rows = dir.vecs[l];
+  for (int p = threadIdx.x; p < len; p += blockDim.x) {
+    const int64_t id = ids[p];
+    if (id >= 0) rowptr[id] = rows + (int64_t)p * ld;  // top bit set: tombstoned by Update
+  }
+}
+
+cudaError_t launch_ivf_rowptrs(ListDirectory dir, int ld, const float** rowptr, cudaStream_t st) {
+  if (dir.nlist <= 0) return cudaSuccess;
+  ivf_rowptrs_kernel<<<dir.nlist, 256, 0, st>>>(dir, ld, rowptr);
+  note_launch();
+  return cudaGetLastError();
+}
+
 cudaError_t launch_ivf_append_codes(const uint8_t* codes, int64_t n, int M, const int32_t* list, const int32_t* pos,
                                     uint8_t* const* list_codes, int64_t* const* list_ids, int64_t vid0,
                                     cudaStream_t st) {

@@ -218,6 +218,10 @@ struct IvfpqPackedCodec {
 // ---------------- exact re-rank -------------------------------------------------------------
 constexpr int RR_NT = 256;
 
+// RR_U: candidates a warp gathers per iteration.  Four keep 2 KiB of independent row loads in flight per warp, which
+// covers HBM latency (eight cost occupancy; the gather is pure latency: recall_num random 4d-byte rows per query).
+// Rows in mapped host memory come over PCIe, whose round trip is several times longer: eight per warp there.
+template <int RR_U>
 __global__ void __launch_bounds__(RR_NT)
     rerank_kernel(const unsigned long long* __restrict__ cand_keys, int ncand, int NP, const float* __restrict__ xq,
                   int64_t ldq, int d, const float* const* __restrict__ raw_segments, int seg_shift, int64_t ld_raw,
@@ -232,9 +236,6 @@ __global__ void __launch_bounds__(RR_NT)
   __syncthreads();
   const float4* q4 = reinterpret_cast<const float4*>(qs);
   const uint32_t seg_mask = (1u << seg_shift) - 1u;
-  // four candidates per warp iteration: 2 KiB of independent row loads in flight per warp (eight cost occupancy; the gather is pure HBM
-  // latency: recall_num random 4d-byte rows per query)
-  constexpr int RR_U = 4;
   for (int j0 = warp * RR_U; j0 < ncand; j0 += (RR_NT / 32) * RR_U) {
     uint32_t vid[RR_U];
     const float4* row[RR_U];
@@ -390,19 +391,20 @@ cudaError_t launch_ivfpq_packed_scan(const float* ip_table, int nq, const int32_
 }
 
 cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq, const float* xq, int64_t ldq, int d,
-                          const float* const* raw_segments, int seg_shift, int64_t ld_raw, int k, int metric,
-                          FilterArgs f, unsigned long long* out_keys, cudaStream_t st) {
+                          const float* const* raw_segments, int seg_shift, int64_t ld_raw, bool host_rows, int k,
+                          int metric, FilterArgs f, unsigned long long* out_keys, cudaStream_t st) {
   if (nq <= 0) return cudaSuccess;
   if (ncand <= 0 || ncand > 8192 || (d & 3)) return cudaErrorInvalidValue;
   int NP = next_pow2(ncand < 2 ? 2 : ncand);  // >= 16 bytes of keys: the query row behind them is read as float4
   size_t smem = (size_t)NP * 8 + (size_t)d * 4;
+  auto kern = host_rows ? rerank_kernel<8> : rerank_kernel<4>;
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(rerank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
-  rerank_kernel<<<nq, RR_NT, smem, st>>>(cand_keys, ncand, NP, xq, ldq, d, raw_segments, seg_shift, ld_raw, k, metric,
-                                         f, out_keys);
-                                         note_launch();
+  kern<<<nq, RR_NT, smem, st>>>(cand_keys, ncand, NP, xq, ldq, d, raw_segments, seg_shift, ld_raw, k, metric, f,
+                                out_keys);
+  note_launch();
   return cudaGetLastError();
 }
 

@@ -107,12 +107,14 @@ class GammaEngine:
             self._h = None
 
     def create_table(self, name, dim, index_type, index_params, vec_name="emb", fields=(("_id", wire.DT_STRING, False),),
-                     refresh_interval=100, extra_vectors=(), **kw):
-        """extra_vectors: further vector fields [(name, dim, index_type, index_params)] of a multi-vector table."""
+                     refresh_interval=100, extra_vectors=(), store_type="MemoryOnly", **kw):
+        """extra_vectors: further vector fields [(name, dim, index_type, index_params[, store_type])] of a multi-vector
+        table.  store_type "RocksDB" keeps a field's raw vectors in pinned host memory instead of HBM."""
         self.vec_name, self.dim = vec_name, dim
-        vectors = [(vec_name, dim, "MemoryOnly", "")] + [(n, d, "MemoryOnly", "") for n, d, _, _ in extra_vectors]
+        vectors = [(vec_name, dim, store_type, "")] + \
+                  [(e[0], e[1], e[4] if len(e) > 4 else "MemoryOnly", "") for e in extra_vectors]
         indexes = [("idx", index_type, vec_name, json.dumps(index_params))] + \
-                  [(f"idx_{n}", t, n, json.dumps(p)) for n, _, t, p in extra_vectors]
+                  [(f"idx_{e[0]}", e[2], e[0], json.dumps(e[3])) for e in extra_vectors]
         tb = wire.build_table(name, list(fields), vectors, indexes, refresh_interval=refresh_interval, **kw)
         _status(_api().CreateTable(self._h, tb, len(tb)))
 

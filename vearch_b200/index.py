@@ -42,12 +42,17 @@ def _bitmap(a):
 class GammaIndex:
     """One vector field's raw store + index model on one GPU."""
 
-    def __init__(self, index_type, d, params=None, device=0):
+    def __init__(self, index_type, d, params=None, device=0, store_type=None):
+        """store_type: where the raw vectors live, as a table's VectorInfo.store_type: "RocksDB" (any case) keeps them
+        in pinned host memory, read over PCIe, so HBM holds only the index; anything else keeps them in HBM."""
         t = index_type.upper()
         self.index_type = "IVFPQFastScan" if t == "IVFPQFASTSCAN" else t  # gamma's spelling of the registered name
         self.d = int(d)
         self.device = device
-        pj = json.dumps(params or {}).encode()
+        params = dict(params or {})
+        if store_type is not None:
+            params["store_type"] = store_type
+        pj = json.dumps(params).encode()
         self._h = _lib.lib().gb_index_create(self.index_type.encode(), self.d, pj, device)
         if not self._h:
             raise GammaError(f"create {index_type}: {_lib.last_error()}")
@@ -89,6 +94,7 @@ class GammaIndex:
         return int(_lib.lib().gb_index_code_size(self._h))
 
     def mem_bytes(self, which=0):
+        """0: the index's HBM; 1: the raw vectors' HBM; 2: the raw vectors' pinned host memory."""
         return int(_lib.lib().gb_index_mem_bytes(self._h, which))
 
     # ---- build --------------------------------------------------------------------------
