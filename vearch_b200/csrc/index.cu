@@ -1736,11 +1736,10 @@ int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int me
   }
   int nparts = ivfflat_scan_nparts(nprobe, lists_->max_len());
   GB_ALLOC(partial, unsigned long long, (size_t)nq * nparts * k, s);
-  last_scan_kernel_ = "ivfflat_scan_warp_kernel";
   scan_timer_begin(st);
   int avg_len = (int)(lists_->total() / std::max(1, nlist_));
   GB_CUDA(launch_ivfflat_scan(xq, dpad_, nq, dpad_, probe_ids, nprobe, lists_->directory(), lists_->max_len(), avg_len, k,
-                              metric, f, partial, &nparts, st));
+                              metric, f, partial, &nparts, &last_scan_kernel_, st));
   scan_timer_end(st);
   GB_CUDA(launch_select_keys(partial, (int64_t)nparts * k, nq, nparts * k, k, out_keys, k, st));
   return 0;
@@ -2294,7 +2293,7 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
 
 // Metric check, ADC depth, query-major list scan + merge of its CTA groups, exact re-rank
 int IvfPqBase::scan_pq_dev(const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric, int nq,
-                           const float* rerank_xq, int k, int nprobe, unsigned long long* out_keys, Scratch& s,
+                           const float* rerank_xq, int k, int nprobe, int max_kk, unsigned long long* out_keys, Scratch& s,
                            const std::function<int(int, unsigned long long*, bool)>& prepare,
                            const std::function<cudaError_t(int, int, unsigned long long*)>& launch) {
   cudaStream_t st = s.stream();
@@ -2305,8 +2304,9 @@ int IvfPqBase::scan_pq_dev(const char* kernel, const SearchContext& ctx, const F
   // recall_num / re-rank semantics: gamma_index_ivfpq.cc:764-770
   const bool rerank = ctx.params.recall_num > 0;
   const int kk = std::max(k, ctx.params.recall_num);
-  if (kk > 4096) {
-    set_last_error(type_ + ": recall_num / topn above 4096 is not supported");
+  if (kk > max_kk) {
+    set_last_error(type_ + ": recall_num / topn [" + std::to_string(kk) + "] above " + std::to_string(max_kk) +
+                   " is not supported by this engine at nsubvector " + std::to_string(M_));
     return -1;
   }
   unsigned long long* keys = out_keys;
@@ -2370,7 +2370,7 @@ int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metr
   };
   // "for opq, rerank need raw vector" (gamma_index_ivfpq.cc:735): original queries against the raw store
   return scan_pq_dev(nbits_ < 8 ? "ivfpq_packed_scan_kernel" : "ivfpq_scan_kernel", ctx, f, metric, nq, xq_raw, k, nprobe,
-                     out_keys, s, prepare, launch);
+                     ivfpq_scan_max_k(M_, nbits_), out_keys, s, prepare, launch);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2431,7 +2431,7 @@ int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, 
   auto launch = [&](int kk, int pg, unsigned long long* partial) {
     return launch_ivfpqfs_scan(lut, ab, nq, probe_ids, nprobe, pg, lists_->directory(), M_, kk, metric, f, partial, st);
   };
-  return scan_pq_dev("ivfpqfs_scan_kernel", ctx, f, metric, nq, xq_raw, k, nprobe, out_keys, s, prepare, launch);
+  return scan_pq_dev("ivfpqfs_scan_kernel", ctx, f, metric, nq, xq_raw, k, nprobe, 4096, out_keys, s, prepare, launch);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2467,6 +2467,15 @@ Index* create_index(const std::string& type, int d, const ModelParams& mp, int d
     if (mp.nbits > IVFPQIndex::kMaxNbits) {
       set_last_error("IVFPQ: nbits_per_idx [" + std::to_string(mp.nbits) + "] above " +
                      std::to_string(IVFPQIndex::kMaxNbits) + " is not supported by this engine");
+      return nullptr;
+    }
+    // the query-major scan holds the [M][2^nbits] fp32 table in one CTA's shared memory: an M it cannot search at all
+    // is refused here rather than at the first search (the reference has no such limit)
+    if (ivfpq_scan_max_k(M, mp.nbits) < 1) {
+      int max_m = M;
+      while (max_m > 1 && ivfpq_scan_max_k(max_m, mp.nbits) < 1) max_m--;
+      set_last_error("IVFPQ: nsubvector [" + std::to_string(M) + "] above " + std::to_string(max_m) + " at nbits_per_idx " +
+                     std::to_string(mp.nbits) + " is not supported by this engine");
       return nullptr;
     }
     if (mp.opq_nsubvector > 0 && d % mp.opq_nsubvector != 0) {  // gamma_index_ivfpq.cc:169-176

@@ -542,9 +542,9 @@ class IvfPqBase : public IvfIndex {
   int train_codebook(const float* x, int64_t n, Scratch& s);
   // scan_dev of the PQ-coded indexes through the query-major list scan: `prepare(kk, keys, need_sorted)` builds the
   // per-query tables and may serve the scan another way (0 = served, 1 = not, < 0 = error); `launch(kk, pg, partial)`
-  // launches the scan kernel, named `kernel`, over pg probes per CTA
+  // launches the scan kernel, named `kernel`, over pg probes per CTA; max_kk: the largest ADC depth it selects
   int scan_pq_dev(const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* rerank_xq,
-                  int k, int nprobe, unsigned long long* out_keys, Scratch& s,
+                  int k, int nprobe, int max_kk, unsigned long long* out_keys, Scratch& s,
                   const std::function<int(int, unsigned long long*, bool)>& prepare,
                   const std::function<cudaError_t(int, int, unsigned long long*)>& launch);
 

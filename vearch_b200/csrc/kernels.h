@@ -74,10 +74,10 @@ struct ListDirectory {            // device-resident mirror of RTInvertIndex (T1
   int nlist;
 };
 // partial[q][part][k]; *nparts_out (<= ivfflat_scan_nparts) = parts actually written per query.
-// One CTA per (query, group of (probe, split) work items).
+// One CTA per (query, group of (probe, split) work items).  *kernel_out = the name of the kernel launched.
 cudaError_t launch_ivfflat_scan(const float* xq, int64_t ldq, int nq, int d, const int32_t* probe_ids, int nprobe,
                                 ListDirectory dir, int max_list_len, int avg_list_len, int k, int metric, FilterArgs f,
-                                unsigned long long* partial, int* nparts_out, cudaStream_t st);
+                                unsigned long long* partial, int* nparts_out, const char** kernel_out, cudaStream_t st);
 int ivfflat_scan_nparts(int nprobe, int max_list_len);
 
 // K3 list-major (tensor cores): (query, probe) pairs grouped by list; tile = 128 pairs x 128 rows.
@@ -168,6 +168,9 @@ cudaError_t launch_ivfpq_scan(const float* ip_table, int nq, const int32_t* prob
                               FilterArgs f, unsigned long long* partial, cudaStream_t st, int ld_probe = 0,
                               const int* gate_cnt = nullptr, int gate_cap = 0, const int* row_limit = nullptr,
                               bool sorted_out = true);  // false: partial[..][k - 1] = the largest key, the others in any order
+// the largest k (<= 4096) launch_ivfpq_scan (nbits 8) / launch_ivfpq_packed_scan (1..7) can select for M sub-quantisers,
+// 0 if none: the [M][2^nbits] fp32 table, the queue and the code stages share one CTA's shared memory
+int ivfpq_scan_max_k(int M, int nbits);
 // the same scan over bit-packed codes, nbits_per_idx 1..7 (ceil(M nbits / 8) bytes per entry, code m at bits
 // [m nbits, (m + 1) nbits), LSB-first); ip_table [nq][M][2^nbits], T [nlist][M][2^nbits]; sorted partials
 cudaError_t launch_ivfpq_packed_scan(const float* ip_table, int nq, const int32_t* probe_ids, const float* coarse_dis,

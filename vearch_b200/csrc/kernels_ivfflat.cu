@@ -389,7 +389,9 @@ cudaError_t launch_warp(const float* xq, int64_t ldq, int nq, const int32_t* pro
   const int SORTNW = next_pow2(KP + 2 * RPW + TW);
   size_t smem =
       (size_t)IVF_NWARP * IVF_WARP_NST * TW * ROW_BYTES + (size_t)IVF_NWARP * SORTNW * 8 + (size_t)IVF_NWARP * KP * 8;
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;
+  // large k (KP = 4096 needs >= 416 KiB; at d 1536 k > 1024 already does not fit): the generic kernel, whose queue is
+  // one per CTA rather than one per warp, takes it
+  if (smem > 227 * 1024) return cudaErrorNotSupported;
   cudaError_t e = cudaFuncSetAttribute(ivfflat_scan_warp_kernel<METRIC, LPR, J>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
@@ -401,7 +403,8 @@ cudaError_t launch_warp(const float* xq, int64_t ldq, int nq, const int32_t* pro
   return cudaGetLastError();
 }
 
-// returns cudaErrorNotSupported when no instantiation fits (caller falls back to the generic kernel)
+// returns cudaErrorNotSupported when no instantiation serves d or its shared memory does not fit k (caller falls back to
+// the generic kernel)
 template <int METRIC>
 cudaError_t dispatch_warp(int S, const float* xq, int64_t ldq, int nq, const int32_t* probe_ids, int nprobe,
                           int nsplit, int pg, ListDirectory dir, int k, FilterArgs f, unsigned long long* partial,
@@ -439,7 +442,7 @@ int ivfflat_scan_nparts(int nprobe, int max_list_len) {
 
 cudaError_t launch_ivfflat_scan(const float* xq, int64_t ldq, int nq, int d, const int32_t* probe_ids, int nprobe,
                                 ListDirectory dir, int max_list_len, int avg_list_len, int k, int metric, FilterArgs f,
-                                unsigned long long* partial, int* nparts_out, cudaStream_t st) {
+                                unsigned long long* partial, int* nparts_out, const char** kernel_out, cudaStream_t st) {
   if (nq <= 0 || nprobe <= 0) return cudaSuccess;
   if ((d & 3) || k <= 0 || k > 4096 || nq > 65535) return cudaErrorInvalidValue;
   IvfGeom g = ivf_geom(d);
@@ -454,9 +457,11 @@ cudaError_t launch_ivfflat_scan(const float* xq, int64_t ldq, int nq, int d, con
                                                                     dir, k, f, partial, st);
     if (fe != cudaErrorNotSupported) {
       if (nparts_out) *nparts_out = (nparts + pg - 1) / pg;  // partial[q][group][k]
+      if (kernel_out) *kernel_out = "ivfflat_scan_warp_kernel";
       return fe;
     }
   }
+  if (kernel_out) *kernel_out = "ivfflat_scan_kernel";
   int KP, SORTN;
   ivf_cq_geometry(k, g.T, &KP, &SORTN);
   size_t smem = (size_t)IVF_NST * g.stage_bytes + (size_t)d * 4 + (size_t)SORTN * 8;

@@ -380,6 +380,12 @@ cudaError_t launch_ivfpq_scan(const float* ip_table, int nq, const int32_t* prob
   return launch_scan_m<kMetricIP>(c, nq, a, st);
 }
 
+int ivfpq_scan_max_k(int M, int nbits) {
+  if (M <= 0 || nbits < 1 || nbits > 8) return 0;
+  if (nbits == 8) return list_scan_max_k(IvfpqCodec{nullptr, nullptr, M, nullptr});
+  return list_scan_max_k(IvfpqPackedCodec{nullptr, nullptr, M, nbits, nullptr});
+}
+
 cudaError_t launch_ivfpq_packed_scan(const float* ip_table, int nq, const int32_t* probe_ids, const float* coarse_dis,
                                      int nprobe, int pg, ListDirectory dir, int M, int nbits, const float* T, int k,
                                      int metric, FilterArgs f, unsigned long long* partial, cudaStream_t st) {

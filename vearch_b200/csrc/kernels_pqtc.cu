@@ -677,18 +677,37 @@ __global__ void __launch_bounds__(RS_NT)
   for (int i = tid; i < kprime; i += RS_NT) out[(int64_t)q * kprime + i] = buf[i];
 }
 
-// overflowed queries: merge the exact kernel's per-group partials (sorted runs of k') into out[q]
+// overflowed queries: the k' best of the exact kernel's per-group partials (ngroups runs of k') into out[q], streamed
+// through a CandQueue in rounds of RS_NT * FM_ITEMS keys, so the shared memory depends on k' alone
+constexpr int FM_ITEMS = 4;
 __global__ void __launch_bounds__(RS_NT)
     pq_fallback_merge_kernel(const int* __restrict__ cand_cnt, int cap, const unsigned long long* __restrict__ partial,
-                             int ngroups, int kprime, int NP, unsigned long long* __restrict__ out) {
+                             int ngroups, int kprime, int KP, int SORTN, unsigned long long* __restrict__ out) {
   extern __shared__ __align__(16) unsigned char rs_smem[];
   unsigned long long* buf = reinterpret_cast<unsigned long long*>(rs_smem);
+  __shared__ int s_cnt;
+  __shared__ unsigned long long s_tau;
   const int q = blockIdx.x, tid = threadIdx.x;
   if (cand_cnt[q] <= cap) return;
-  const int n = ngroups * kprime;
-  for (int i = tid; i < NP; i += RS_NT) buf[i] = i < n ? partial[(int64_t)q * n + i] : kKeySentinel;
-  __syncthreads();
-  block_bitonic_sort(buf, NP);
+  const int64_t n = (int64_t)ngroups * kprime;
+  const unsigned long long* row = partial + (int64_t)q * n;
+  CandQueue cq{buf, &s_cnt, &s_tau, kprime, KP, SORTN};
+  cq.init();
+  const int per_round = RS_NT * FM_ITEMS;
+  for (int64_t base = 0; base < n; base += per_round) {
+    const unsigned long long tau = s_tau;
+#pragma unroll
+    for (int u = 0; u < FM_ITEMS; u++) {
+      const int64_t i = base + u * RS_NT + tid;
+      const unsigned long long key = i < n ? row[i] : kKeySentinel;
+      cq.push_warp(key < tau, key);
+    }
+    __syncthreads();
+    const int c_now = s_cnt;
+    __syncthreads();  // same snapshot in every thread before any warp pushes again
+    if (base + per_round < n && c_now + per_round > cq.cap()) cq.flush();
+  }
+  cq.flush(true);
   for (int i = tid; i < kprime; i += RS_NT) out[(int64_t)q * kprime + i] = buf[i];
 }
 
@@ -850,12 +869,13 @@ cudaError_t launch_pq_rescore(const float* ip_table, int nq, const int32_t* prob
 cudaError_t launch_pq_fallback_merge(const int* cand_cnt, int cap, int nq, const unsigned long long* partial, int ngroups,
                                      int kprime, unsigned long long* out, cudaStream_t st) {
   if (nq <= 0) return cudaSuccess;
-  const int NP = next_pow2(ngroups * kprime < 16 ? 16 : ngroups * kprime);
-  const size_t smem = (size_t)NP * 8;
-  if (smem > 200 * 1024) return cudaErrorInvalidValue;
+  if (kprime <= 0 || kprime > 4096 || ngroups <= 0) return cudaErrorInvalidValue;
+  const int KP = next_pow2(kprime < 16 ? 16 : kprime);
+  const int SORTN = next_pow2(KP + RS_NT * FM_ITEMS);  // at most 64 KiB at k' = 4096
+  const size_t smem = (size_t)SORTN * 8;
   cudaError_t e = cudaFuncSetAttribute(pq_fallback_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  pq_fallback_merge_kernel<<<nq, RS_NT, smem, st>>>(cand_cnt, cap, partial, ngroups, kprime, NP, out);
+  pq_fallback_merge_kernel<<<nq, RS_NT, smem, st>>>(cand_cnt, cap, partial, ngroups, kprime, KP, SORTN, out);
   note_launch();
   return cudaGetLastError();
 }

@@ -301,17 +301,36 @@ __global__ void __launch_bounds__(LS_NT, Codec::kMinCtasPerSm)
   for (int i = tid; i < k; i += LS_NT) out[i] = buf[i];
 }
 
+// queue geometry of a scan for k and the dynamic shared memory it needs: table, queue, code stages
+template <class Codec>
+size_t list_scan_smem(const Codec& c, int k, int* KP_out = nullptr, int* SORTN_out = nullptr) {
+  const int tile_e = c.tile_entries();
+  const int KP = next_pow2(k < 16 ? 16 : k);
+  const int SORTN = next_pow2(KP + tile_e + tile_e / 2);  // cap >= tile_e: one tile always fits after a flush
+  if (KP_out) *KP_out = KP;
+  if (SORTN_out) *SORTN_out = SORTN;
+  return (size_t)ls_table_entries(c) * sizeof(typename Codec::Entry) + (size_t)SORTN * 8 +
+         (size_t)LS_NST * tile_e * c.code_bytes() + (LsCodeSum<Codec>::value ? 16 : 0);
+}
+constexpr size_t kListScanMaxSmem = 227 * 1024;
+
+// the largest k (<= 4096) a codec's scan can select, 0 if none: the shared memory grows with k only through KP
+template <class Codec>
+int list_scan_max_k(const Codec& c) {
+  for (int k = 4096; k >= 16; k >>= 1)
+    if (list_scan_smem(c, k) <= kListScanMaxSmem) return k;
+  return 0;
+}
+
 // partial[q][group][k], one CTA per (query, group of pg probes); nq <= 65535, 1 <= k <= 4096, 1 <= pg <= LS_MAX_PG
 template <class Codec, int METRIC, int MW>
 cudaError_t launch_list_scan(const Codec& c, int nq, const ListScanArgs& a, cudaStream_t st) {
   if (nq <= 0 || a.nprobe <= 0) return cudaSuccess;
   if (a.k <= 0 || a.k > 4096 || nq > 65535 || a.pg < 1 || a.pg > LS_MAX_PG) return cudaErrorInvalidValue;
   const int tile_e = c.tile_entries();
-  const int KP = next_pow2(a.k < 16 ? 16 : a.k);
-  const int SORTN = next_pow2(KP + tile_e + tile_e / 2);  // cap >= tile_e: one tile always fits after a flush
-  const size_t smem = (size_t)ls_table_entries(c) * sizeof(typename Codec::Entry) + (size_t)SORTN * 8 +
-                      (size_t)LS_NST * tile_e * c.code_bytes() + (LsCodeSum<Codec>::value ? 16 : 0);
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;
+  int KP, SORTN;
+  const size_t smem = list_scan_smem(c, a.k, &KP, &SORTN);
+  if (smem > kListScanMaxSmem) return cudaErrorInvalidValue;
   cudaError_t e =
       cudaFuncSetAttribute(list_scan_kernel<Codec, METRIC, MW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
