@@ -136,6 +136,25 @@ int gb_index_search_preassigned(gb_index *index, int nq, const float *x, int k, 
                                 const float *coarse_dis, int nprobe, const char *retrieval_params_json,
                                 const uint8_t *del_bitmap, const uint8_t *filter_bitmap, int64_t bitmap_bits,
                                 float min_score, float max_score, float *out_scores, int64_t *out_ids);
+/* BINARYIVF (create with index_type "BINARYIVF" and the dimension in bits, a positive multiple of 8): rows, queries
+ * and centroids are packed binary vectors of d / 8 bytes, bit i at bit (i & 7) of byte i >> 3.  Scores are Hamming
+ * distances (integers as floats, smaller first).  The float entry points that take or return rows, queries or
+ * centroids (gb_index_add_vectors*, gb_index_update_vector, gb_index_get_vector(s), gb_index_search*,
+ * gb_index_coarse_search, gb_index_search_preassigned, gb_index_set/get_centroids) refuse it. */
+int gb_index_add_binary(gb_index *index, int64_t n, const uint8_t *x);
+int gb_index_update_binary(gb_index *index, int64_t vid, const uint8_t *x);
+int gb_index_get_binary(gb_index *index, int64_t start, int64_t n, uint8_t *out);
+int gb_index_search_binary(gb_index *index, int nq, const uint8_t *x, int k, const char *retrieval_params_json,
+                           int brute_force, const uint8_t *del_bitmap, const uint8_t *filter_bitmap, int64_t bitmap_bits,
+                           float min_score, float max_score, int search_unindexed_tail, float *out_scores, int64_t *out_ids);
+int gb_index_set_binary_centroids(gb_index *index, const uint8_t *centroids, int nlist);
+int gb_index_get_binary_centroids(gb_index *index, uint8_t *centroids);
+/* the float centroids of the +-1 k-means the packed centroids were taken from: nlist x d floats */
+int gb_index_get_real_centroids(gb_index *index, float *centroids);
+int gb_index_coarse_search_binary(gb_index *index, int nq, const uint8_t *x, int nprobe, float *out_dis, int64_t *out_ids);
+int gb_index_search_preassigned_binary(gb_index *index, int nq, const uint8_t *x, int k, const int64_t *keys, int nprobe,
+                                       const uint8_t *del_bitmap, const uint8_t *filter_bitmap, int64_t bitmap_bits,
+                                       float min_score, float max_score, float *out_scores, int64_t *out_ids);
 /* pq.compute_codes on residuals (gamma_index_ivfpq.cc:489-494): codes = n x code_size bytes, bit-packed below
    nbits_per_idx = 8 (code m at bits [m nbits, (m + 1) nbits) of the row, LSB-first) */
 int gb_index_pq_encode(gb_index *index, int64_t n, const float *x, const int64_t *assign, uint8_t *codes);

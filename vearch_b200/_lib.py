@@ -86,6 +86,15 @@ def _declare(l):
     l.gb_index_coarse_search.argtypes = [vp, i32, vp, i32, vp, vp]
     l.gb_index_search_preassigned.argtypes = [vp, i32, vp, i32, vp, vp, i32, cstr, vp, vp, i64, f32, f32, vp, vp]
     l.gb_index_pq_encode.argtypes = [vp, i64, vp, vp, vp]
+    l.gb_index_add_binary.argtypes = [vp, i64, vp]
+    l.gb_index_update_binary.argtypes = [vp, i64, vp]
+    l.gb_index_get_binary.argtypes = [vp, i64, i64, vp]
+    l.gb_index_search_binary.argtypes = [vp, i32, vp, i32, cstr, i32, vp, vp, i64, f32, f32, i32, vp, vp]
+    l.gb_index_set_binary_centroids.argtypes = [vp, vp, i32]
+    l.gb_index_get_binary_centroids.argtypes = [vp, vp]
+    l.gb_index_get_real_centroids.argtypes = [vp, vp]
+    l.gb_index_coarse_search_binary.argtypes = [vp, i32, vp, i32, vp, vp]
+    l.gb_index_search_preassigned_binary.argtypes = [vp, i32, vp, i32, vp, i32, vp, vp, i64, f32, f32, vp, vp]
     l.gb_kmeans.argtypes = [i32, vp, i64, i32, i32, i32, i64, i32, i32, vp, vp]
     l.gb_kmeans_update.argtypes = [i32, vp, i64, i32, i32, vp, vp]
     l.gb_merge_partitions_device.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, vp]

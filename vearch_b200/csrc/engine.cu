@@ -317,13 +317,18 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     training_threshold_ = mp.training_threshold;  // table.cc:143-150
   if (training_threshold_ > 0) mp.training_threshold = training_threshold_;
   mp.host_store = !strcasecmp(v.str(4).c_str(), "RocksDB");  // VectorInfo.store_type
+  // BINARYIVF: the field's values are packed bits, dimension / 8 bytes (vector_manager.cc:100-130); a table with more
+  // than one vector field cannot join Hamming and float scores here
+  if (index_type_ == "BINARYIVF" && nvec > 1)
+    return Status::Make(kNotSupported, vec_name_ + ": BINARYIVF is not supported in a multi-vector table");
   Index* idx = create_index(index_type_, dim_, mp, device_, 20);
   if (!idx) return Status::Make(index_type_ == "FLAT" || index_type_ == "IVFFLAT" || index_type_ == "IVFPQ" ||
-                                        index_type_ == "IVFPQFastScan"
+                                        index_type_ == "IVFPQFastScan" || index_type_ == "BINARYIVF"
                                     ? kInvalidArgument
                                     : kNotSupported,
                                 last_error());
   index_.reset(idx);
+  vbytes_ = (size_t)idx->store().row_bytes();
   extra_.clear();
   for (size_t vi = 1; vi < nvec; vi++) {  // the other vector fields: same rules, their own index each
     FbTable ev = t.vec_table(2, vi);
@@ -344,6 +349,8 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     if (!parse_model_params(vf.index_params, &emp, &err)) return Status::Make(kInvalidArgument, err);
     if (training_threshold_ > 0) emp.training_threshold = training_threshold_;
     emp.host_store = !strcasecmp(ev.str(4).c_str(), "RocksDB");
+    if (vf.index_type == "BINARYIVF")
+      return Status::Make(kNotSupported, vf.name + ": BINARYIVF is not supported in a multi-vector table");
     Index* eidx = create_index(vf.index_type, vf.dim, emp, device_, 20);
     if (!eidx) return Status::Make(kInvalidArgument, last_error());
     vf.index.reset(eidx);
@@ -445,9 +452,8 @@ int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
       scalar_index_put(fi, docid, f.value);
     }
     if (has_vec) {
-      if (vec_len != (size_t)dim_ * 4) return -1;
-      std::vector<float> x(dim_);
-      memcpy(x.data(), vec, vec_len);
+      if (vec_len != vbytes_) return -1;
+      std::vector<unsigned char> x(vec, vec + vec_len);
       if (flush_pending_locked()) return -1;
       if (index_->update_vector(docid, x.data())) return -1;
     }
@@ -463,8 +469,8 @@ int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
   } else if (docid >= max_docid_) {
     return -2;
   }
-  // CheckDoc (engine.cc:802-813): every vector field present with d*4 bytes
-  if (!has_vec || vec_len != (size_t)dim_ * 4) return -3;
+  // CheckDoc (engine.cc:802-813): every vector field present with d*4 bytes (BINARYIVF: d / 8)
+  if (!has_vec || vec_len != vbytes_) return -3;
   for (size_t ei = 0; ei < extra_.size(); ei++)
     if (!evec[ei].first || evec[ei].second != (size_t)extra_[ei].dim * 4) return -3;
   if (key.empty()) return -3;
@@ -475,8 +481,8 @@ int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
     if (fields_[fi].indexed) scalar_index_put((int)fi, max_docid_, values_[fi][max_docid_]);
   keys_.push_back(key);
   key2docid_[key] = max_docid_;
-  pending_.resize((size_t)(pending_n_ + 1) * dim_);
-  memcpy(pending_.data() + (size_t)pending_n_ * dim_, vec, vec_len);
+  pending_.resize((size_t)(pending_n_ + 1) * vbytes_);
+  memcpy(pending_.data() + (size_t)pending_n_ * vbytes_, vec, vec_len);
   for (size_t ei = 0; ei < extra_.size(); ei++) {
     auto& e = extra_[ei];
     e.pending.resize((size_t)(pending_n_ + 1) * e.dim);
@@ -524,16 +530,16 @@ void Engine::serialize_doc(int docid, bool with_docid, std::string* out) {
   if (docid >= 0) {
     for (size_t fi = 0; fi < fields_.size(); fi++) add_field(fields_[fi].name, values_[fi][docid], fields_[fi].data_type);
     if (with_docid) add_field("_docid", std::string(reinterpret_cast<const char*>(&docid), 4), DT_INT);
-    std::vector<float> x(dim_);
+    std::string x(vbytes_, '\0');
     bool got = false;
     int64_t stored = index_->store().size();
     if (docid < stored) {
-      got = index_->store().get_host(docid, x.data()) == 0;
+      got = index_->store().get_host(docid, &x[0]) == 0;
     } else if (docid - stored < pending_n_) {
-      memcpy(x.data(), pending_.data() + (size_t)(docid - stored) * dim_, (size_t)dim_ * 4);
+      memcpy(&x[0], pending_.data() + (size_t)(docid - stored) * vbytes_, vbytes_);
       got = true;
     }
-    if (got) add_field(vec_name_, std::string(reinterpret_cast<const char*>(x.data()), (size_t)dim_ * 4), DT_VECTOR);
+    if (got) add_field(vec_name_, x, DT_VECTOR);
     for (auto& e : extra_) {
       std::vector<float> ex(e.dim);
       bool egot = false;
@@ -799,7 +805,8 @@ Status Engine::Search(const SearchRequestPB& req, std::string* pb_out) {
   if (brute == 0 && index_status_.load() != 2 && max_docid_ > 100 && !enable_realtime_)
     return Status::Make(kIndexError, space_name_ + " index not trained, brute_force_search is 0, max_docid_ = " +
                                          std::to_string(max_docid_) + ", threshold = 100");
-  int n = (int)(vq.value.size() / ((size_t)qdim * 4));
+  const size_t qbytes = (size_t)qindex->store().row_bytes();  // d * 4, or BINARYIVF's d / 8
+  int n = (int)(vq.value.size() / qbytes);
   if (n <= 0) return Status::Make(kInvalidArgument, "Search n shouldn't less than 0!");
   if (IsKilled(req.request_id, req.partition_id)) return Status::Make(kMemoryExceeded, "");
   SearchContext ctx;
@@ -815,8 +822,6 @@ Status Engine::Search(const SearchRequestPB& req, std::string* pb_out) {
     ctx.max_score = FLT_MAX;
   }
   const int topN = req.topn + req.offset;
-  std::vector<float> x((size_t)n * qdim);
-  memcpy(x.data(), vq.value.data(), x.size() * 4);
   std::vector<float> dis((size_t)n * topN);
   std::vector<int64_t> ids((size_t)n * topN);
   std::vector<uint8_t> bm, fbm;
@@ -856,7 +861,14 @@ Status Engine::Search(const SearchRequestPB& req, std::string* pb_out) {
       ctx.bitmap_bits = max_docid_;
     }
   }
-  int rc = qindex->search(ctx, n, x.data(), topN, dis.data(), ids.data());
+  int rc;
+  if (BinaryIvfIndex* bq = dynamic_cast<BinaryIvfIndex*>(qindex)) {
+    rc = bq->search_codes(ctx, n, reinterpret_cast<const uint8_t*>(vq.value.data()), topN, dis.data(), ids.data());
+  } else {
+    std::vector<float> x((size_t)n * qdim);
+    memcpy(x.data(), vq.value.data(), x.size() * 4);
+    rc = qindex->search(ctx, n, x.data(), topN, dis.data(), ids.data());
+  }
   if (rc == -2 || IsKilled(req.request_id, req.partition_id)) return Status::Make(kMemoryExceeded, "");
   if (rc != 0) return Status::Make(kInvalidArgument, "faild search of query " + vq.name + ": " + last_error());
 
@@ -1047,11 +1059,11 @@ void Engine::put_doc_fields(int docid, const FieldSel& sel, PbWriter* item) {
   for (const auto& vn : sel.vecs) {
     int dim = 0;
     Index* ix = index_of(vn, &dim);
-    std::vector<float> vbuf(dim);
+    std::vector<unsigned char> vbuf(ix ? ix->store().row_bytes() : 0);
     if (ix && ix->store().get_host(docid, vbuf.data()) == 0) {
       PbWriter fld;
       fld.put_string(1, vn);
-      fld.put_bytes(3, vbuf.data(), (size_t)dim * 4);
+      fld.put_bytes(3, vbuf.data(), vbuf.size());
       item->put_message(2, fld.out);
     }
   }
@@ -1319,9 +1331,9 @@ int Engine::Dump() {
   for (size_t fi = 0; fi < fields_.size(); fi++)
     for (int d = 0; d < max_docid_; d++) wr_str(f, values_[fi][d]);
   wr_str(f, std::string(del_bitmap_.begin(), del_bitmap_.end()));
-  std::vector<float> rows((size_t)max_docid_ * dim_);
+  std::vector<unsigned char> rows((size_t)max_docid_ * vbytes_);
   if (max_docid_ && index_->store().get_rows_host(0, max_docid_, rows.data())) return -1;
-  f.write(reinterpret_cast<const char*>(rows.data()), (std::streamsize)(rows.size() * 4));
+  f.write(reinterpret_cast<const char*>(rows.data()), (std::streamsize)rows.size());
   int trained = index_->trained() ? 1 : 0;
   wr<int32_t>(f, trained);
   // an index whose trained state does not persist (IVFPQFastScan) is trained again by Load
@@ -1385,8 +1397,8 @@ int Engine::Load() {
   if (!rd_str(f, &bm)) return -1;
   del_bitmap_.assign(bm.begin(), bm.end());
   del_bitmap_.resize(std::max<size_t>(del_bitmap_.size(), (size_t)(maxd >> 3) + 4096), 0);
-  std::vector<float> rows((size_t)maxd * dim_);
-  if (maxd && !f.read(reinterpret_cast<char*>(rows.data()), (std::streamsize)(rows.size() * 4))) return -1;
+  std::vector<unsigned char> rows((size_t)maxd * vbytes_);
+  if (maxd && !f.read(reinterpret_cast<char*>(rows.data()), (std::streamsize)rows.size())) return -1;
   int32_t trained;
   if (!rdv(f, &trained)) return -1;
   for (size_t fi = 0; fi < fields_.size(); fi++)

@@ -192,7 +192,9 @@ class Engine {
   std::string vec_name_, index_type_, index_params_;
   int dim_ = 0;
   std::unique_ptr<Index> index_;
-  std::vector<float> pending_;  // rows accepted by AddOrUpdate, not yet uploaded to HBM
+  // rows accepted by AddOrUpdate, not yet uploaded to HBM: vbytes_ bytes each (d fp32 values, or BINARYIVF's d / 8 bytes)
+  std::vector<unsigned char> pending_;
+  size_t vbytes_ = 0;
   int pending_n_ = 0;
   // further vector fields of a multi-vector table (vector_manager.cc:343-453: one raw vector + one index
   // per field).  The first field keeps the members above; every document carries all of them.

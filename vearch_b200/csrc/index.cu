@@ -111,8 +111,8 @@ const VmmApi& vmm_api() {
 }
 }  // namespace
 
-RawStore::RawStore(int d, int seg_shift, bool host)
-    : d_(d), dpad_((int)round_up(d, 4)), seg_shift_(host ? std::min(seg_shift, kHostSegShift) : seg_shift), host_(host) {
+RawStore::RawStore(int row_bytes, int seg_shift, bool host)
+    : row_bytes_(row_bytes), stride_((int)round_up(row_bytes, 16)), seg_shift_(host ? std::min(seg_shift, kHostSegShift) : seg_shift), host_(host) {
   cudaMalloc(&d_segs_, sizeof(float*) * kMaxSegs);
   cudaGetDevice(&device_);
 }
@@ -143,11 +143,11 @@ int RawStore::new_segment() {
     return -1;
   }
   Seg sg;
-  const size_t bytes = (size_t)seg_rows() * dpad_ * 4;
+  const size_t bytes = (size_t)seg_rows() * stride_;
   if (host_) {  // pinned, mapped into every device's address space; kernels read it through the device pointer
     GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&sg.base), bytes, cudaHostAllocMapped | cudaHostAllocPortable));
     memset(sg.base, 0, bytes);  // pad columns must read as zero
-    float* dev = nullptr;
+    unsigned char* dev = nullptr;
     const cudaError_t e = cudaHostGetDevicePointer(reinterpret_cast<void**>(&dev), sg.base, 0);
     if (e != cudaSuccess) {
       cudaFreeHost(sg.base);
@@ -157,7 +157,7 @@ int RawStore::new_segment() {
     sg.mapped = bytes;
     host_bytes_ += (int64_t)bytes;
     segs_.push_back(sg);
-    GB_CUDA(cudaMemcpy(d_segs_ + segs_.size() - 1, &dev, sizeof(float*), cudaMemcpyHostToDevice));
+    GB_CUDA(cudaMemcpy(d_segs_ + segs_.size() - 1, &dev, sizeof(dev), cudaMemcpyHostToDevice));
     return 0;
   }
   const VmmApi& api = vmm_api();
@@ -172,7 +172,7 @@ int RawStore::new_segment() {
       sg.va_bytes = (size_t)round_up((int64_t)bytes, (int64_t)gran);
       CUdeviceptr p = 0;
       if (api.reserve(&p, sg.va_bytes, 0, 0, 0) == CUDA_SUCCESS) {
-        sg.base = reinterpret_cast<float*>(p);
+        sg.base = reinterpret_cast<unsigned char*>(p);
         sg.vmm = true;
       }
     }
@@ -184,13 +184,13 @@ int RawStore::new_segment() {
     phys_bytes_ += (int64_t)bytes;
   }
   segs_.push_back(sg);
-  GB_CUDA(cudaMemcpy(d_segs_ + segs_.size() - 1, &sg.base, sizeof(float*), cudaMemcpyHostToDevice));
+  GB_CUDA(cudaMemcpy(d_segs_ + segs_.size() - 1, &sg.base, sizeof(sg.base), cudaMemcpyHostToDevice));
   return 0;
 }
 // physical memory behind the first `rows` rows of segment si
 int RawStore::map_rows(int si, int64_t rows) {
   Seg& sg = segs_[si];
-  const size_t need = (size_t)rows * dpad_ * 4;
+  const size_t need = (size_t)rows * stride_;
   if (need <= sg.mapped) return 0;
   const VmmApi& api = vmm_api();
   while (sg.mapped < need) {
@@ -235,7 +235,8 @@ int RawStore::ensure(int64_t n_total) {
 // Host placement: the segments are ordinary (pinned) host memory, so host rows move with memcpy and device rows with
 // device-to-host copies.  A search may still be reading a row when update_host overwrites it: the caller holds the
 // index lock exclusively and has drained in-flight searches first (Index::update_vector).
-int RawStore::append_host(const float* x, int64_t n, cudaStream_t st) {
+int RawStore::append_host(const void* xv, int64_t n, cudaStream_t st) {
+  const unsigned char* x = static_cast<const unsigned char*>(xv);
   if (ensure(n_ + n)) return -1;
   int64_t done = 0;
   while (done < n) {
@@ -243,10 +244,10 @@ int RawStore::append_host(const float* x, int64_t n, cudaStream_t st) {
     int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
     int64_t cnt = std::min(n - done, seg_rows() - off);
     if (host_) {
-      for (int64_t i = 0; i < cnt; i++) memcpy(segs_[si].base + (off + i) * dpad_, x + (done + i) * d_, (size_t)d_ * 4);
+      for (int64_t i = 0; i < cnt; i++) memcpy(segs_[si].base + (off + i) * stride_, x + (done + i) * row_bytes_, row_bytes_);
     } else {
-      GB_CUDA(cudaMemcpy2DAsync(segs_[si].base + off * dpad_, (size_t)dpad_ * 4, x + done * d_, (size_t)d_ * 4,
-                                (size_t)d_ * 4, (size_t)cnt, cudaMemcpyHostToDevice, st));
+      GB_CUDA(cudaMemcpy2DAsync(segs_[si].base + off * stride_, stride_, x + done * row_bytes_, row_bytes_, row_bytes_,
+                                (size_t)cnt, cudaMemcpyHostToDevice, st));
     }
     done += cnt;
   }
@@ -254,43 +255,45 @@ int RawStore::append_host(const float* x, int64_t n, cudaStream_t st) {
   n_ += n;
   return 0;
 }
-int RawStore::append_device(const float* x, int64_t ld, int64_t n, cudaStream_t st) {
+int RawStore::append_device(const void* xv, int64_t ld_bytes, int64_t n, cudaStream_t st) {
+  const unsigned char* x = static_cast<const unsigned char*>(xv);
   if (ensure(n_ + n)) return -1;
   int64_t done = 0;
   while (done < n) {
     int64_t vid = n_ + done;
     int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
     int64_t cnt = std::min(n - done, seg_rows() - off);
-    GB_CUDA(cudaMemcpy2DAsync(segs_[si].base + off * dpad_, (size_t)dpad_ * 4, x + done * ld, (size_t)ld * 4,
-                              (size_t)d_ * 4, (size_t)cnt, host_ ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, st));
+    GB_CUDA(cudaMemcpy2DAsync(segs_[si].base + off * stride_, stride_, x + done * ld_bytes, (size_t)ld_bytes, row_bytes_,
+                              (size_t)cnt, host_ ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, st));
     done += cnt;
   }
   GB_CUDA(cudaStreamSynchronize(st));
   n_ += n;
   return 0;
 }
-int RawStore::update_host(int64_t vid, const float* x, cudaStream_t st) {
+int RawStore::update_host(int64_t vid, const void* x, cudaStream_t st) {
   if (vid < 0 || vid >= n_) return -1;
   int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
   if (host_) {
-    memcpy(segs_[si].base + off * dpad_, x, (size_t)d_ * 4);
+    memcpy(segs_[si].base + off * stride_, x, row_bytes_);
     return 0;
   }
-  GB_CUDA(cudaMemcpyAsync(segs_[si].base + off * dpad_, x, (size_t)d_ * 4, cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaMemcpyAsync(segs_[si].base + off * stride_, x, row_bytes_, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
-int RawStore::get_host(int64_t vid, float* out) const {
+int RawStore::get_host(int64_t vid, void* out) const {
   if (vid < 0 || vid >= n_) return -1;
   int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
   if (host_) {
-    memcpy(out, segs_[si].base + off * dpad_, (size_t)d_ * 4);
+    memcpy(out, segs_[si].base + off * stride_, row_bytes_);
     return 0;
   }
-  GB_CUDA(cudaMemcpy(out, segs_[si].base + off * dpad_, (size_t)d_ * 4, cudaMemcpyDeviceToHost));
+  GB_CUDA(cudaMemcpy(out, segs_[si].base + off * stride_, row_bytes_, cudaMemcpyDeviceToHost));
   return 0;
 }
-int RawStore::get_rows_host(int64_t start, int64_t n, float* out) const {
+int RawStore::get_rows_host(int64_t start, int64_t n, void* outv) const {
+  unsigned char* out = static_cast<unsigned char*>(outv);
   if (start < 0 || n < 0 || start + n > n_) return -1;
   int64_t done = 0;
   while (done < n) {
@@ -298,22 +301,23 @@ int RawStore::get_rows_host(int64_t start, int64_t n, float* out) const {
     int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
     int64_t cnt = std::min(n - done, seg_rows() - off);
     if (host_) {
-      for (int64_t i = 0; i < cnt; i++) memcpy(out + (done + i) * d_, segs_[si].base + (off + i) * dpad_, (size_t)d_ * 4);
+      for (int64_t i = 0; i < cnt; i++) memcpy(out + (done + i) * row_bytes_, segs_[si].base + (off + i) * stride_, row_bytes_);
     } else {
-      GB_CUDA(cudaMemcpy2D(out + done * d_, (size_t)d_ * 4, segs_[si].base + off * dpad_, (size_t)dpad_ * 4,
-                           (size_t)d_ * 4, (size_t)cnt, cudaMemcpyDeviceToHost));
+      GB_CUDA(cudaMemcpy2D(out + done * row_bytes_, row_bytes_, segs_[si].base + off * stride_, stride_, row_bytes_,
+                           (size_t)cnt, cudaMemcpyDeviceToHost));
     }
     done += cnt;
   }
   return 0;
 }
-cudaError_t RawStore::copy_rows_to_device(int64_t start, int64_t n, float* dst, cudaStream_t st) const {
+cudaError_t RawStore::copy_rows_to_device(int64_t start, int64_t n, void* dstv, cudaStream_t st) const {
+  unsigned char* dst = static_cast<unsigned char*>(dstv);
   int64_t done = 0;
   while (done < n) {
     int64_t vid = start + done;
     int64_t si = vid >> seg_shift_, off = vid & (seg_rows() - 1);
     int64_t cnt = std::min(n - done, seg_rows() - off);
-    const cudaError_t e = cudaMemcpyAsync(dst + done * dpad_, segs_[si].base + off * dpad_, (size_t)cnt * dpad_ * 4,
+    const cudaError_t e = cudaMemcpyAsync(dst + done * stride_, segs_[si].base + off * stride_, (size_t)cnt * stride_,
                                           host_ ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st);
     if (e != cudaSuccess) return e;
     done += cnt;
@@ -321,8 +325,8 @@ cudaError_t RawStore::copy_rows_to_device(int64_t start, int64_t n, float* dst, 
   return cudaSuccess;
 }
 const float* RawStore::contiguous(int64_t n, Scratch& s) {
-  if (!host_ && n <= seg_rows()) return segs_.empty() ? nullptr : segs_[0].base;
-  float* buf = s.alloc_n<float>((size_t)n * dpad_);
+  if (!host_ && n <= seg_rows()) return segs_.empty() ? nullptr : seg(0);
+  float* buf = s.alloc_n<float>((size_t)n * stride_ / 4);
   if (!buf) return nullptr;
   const cudaError_t e = copy_rows_to_device(0, n, buf, s.stream());
   if (e != cudaSuccess) {
@@ -513,7 +517,7 @@ void quiesce_all_indexes() {
 }
 }  // namespace
 
-Index::Index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift)
+Index::Index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int row_bytes)
     : type_(type), d_(d), dpad_((int)round_up(d, 4)), device_(device), mp_(mp) {
   cudaSetDevice(device_);
   cudaMemPool_t pool;
@@ -527,7 +531,7 @@ Index::Index(const std::string& type, int d, const ModelParams& mp, int device, 
     (void)hooked;
     live_indexes().all.push_back(this);
   }
-  store_.reset(new RawStore(d, seg_shift, mp.host_store));
+  store_.reset(new RawStore(row_bytes > 0 ? row_bytes : 4 * d, seg_shift, mp.host_store));
   cudaStreamCreateWithFlags(&build_stream_, cudaStreamNonBlocking);
 }
 void Index::quiesce() {
@@ -679,7 +683,7 @@ float Index::last_scan_ms() {
   scan_events_.clear();
   return total;
 }
-int Index::add_vectors(const float* x, int64_t n) {
+int Index::add_vectors(const void* x, int64_t n) {
   cudaSetDevice(device_);
   std::unique_lock<std::shared_mutex> lk(mu_);
   return store_->append_host(x, n, build_stream_);
@@ -687,13 +691,13 @@ int Index::add_vectors(const float* x, int64_t n) {
 int Index::add_vectors_device(const float* x, int64_t ld, int64_t n) {
   cudaSetDevice(device_);
   std::unique_lock<std::shared_mutex> lk(mu_);
-  return store_->append_device(x, ld, n, build_stream_);
+  return store_->append_device(x, ld * 4, n, build_stream_);
 }
 
-const float* Index::store_rows_dev(int64_t vid0, int64_t n, Scratch& s) {
+const void* Index::store_rows_dev(int64_t vid0, int64_t n, Scratch& s) {
   const int64_t si = vid0 >> store_->seg_shift(), off = vid0 & (store_->seg_rows() - 1);
-  if (!store_->on_host()) return store_->seg((int)si) + off * dpad_;
-  float* buf = s.alloc_n<float>((size_t)n * dpad_);
+  if (!store_->on_host()) return store_->seg_bytes((int)si) + off * store_->stride();
+  void* buf = s.alloc((size_t)n * store_->stride());
   if (!buf) return nullptr;
   const cudaError_t e = store_->copy_rows_to_device(vid0, n, buf, s.stream());
   if (e != cudaSuccess) {
@@ -765,6 +769,10 @@ int Index::search_device(const SearchContext& ctx, int nq, const float* x_dev, i
   if (nq <= 0) return 0;
   if (k <= 0 || k > 4096) {
     set_last_error("topK must be in [1, 4096]");
+    return -1;
+  }
+  if (store_->row_bytes() != 4 * d_) {  // BINARYIVF: packed queries only (BinaryIvfIndex::search_codes)
+    set_last_error(type_ + ": queries are packed binary rows, not floats");
     return -1;
   }
   cudaSetDevice(device_);
@@ -1192,8 +1200,8 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
 }
 
 // ------------------------------------------------------------------------------------------
-IvfIndex::IvfIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift)
-    : Index(type, d, mp, device, seg_shift), nlist_(mp.ncentroids) {
+IvfIndex::IvfIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int row_bytes)
+    : Index(type, d, mp, device, seg_shift, row_bytes), nlist_(mp.ncentroids) {
   cudaMalloc(&d_centroids_, (size_t)nlist_ * dpad_ * 4);
   cudaMemset(d_centroids_, 0, (size_t)nlist_ * dpad_ * 4);
   const int64_t ctiles = (nlist_ + 127) / 128;
@@ -1297,8 +1305,9 @@ int IvfIndex::assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* out, S
   return 0;
 }
 
-int IVFFlatIndex::append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+int IVFFlatIndex::append_batch(const void* xv, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
                                const std::vector<int>& add, Scratch& s) {
+  const float* x = static_cast<const float*>(xv);
   GB_CUDA(launch_ivf_append_vecs(x, dpad_, n, dpad_, d_list, d_pos, reinterpret_cast<float* const*>(lists_->d_data()),
                                  lists_->d_ids(), vid0, s.stream()));
   // the tensor-core mirror's rows after the list data, before the new lengths are committed
@@ -1307,13 +1316,18 @@ int IVFFlatIndex::append_batch(const float* x, int64_t n, int64_t vid0, const in
 
 // GammaIVFFlatIndex::Add (gamma_index_ivfflat.cc:413-474) driven like
 // VectorManager::AddRTVecsToIndex (vector_manager.cc:572-702), in large device batches.
-int IvfIndex::index_batch(const float* x, int64_t n, int64_t vid0, const uint8_t* del_bitmap) {
+int IvfIndex::assign_batch(const void* x, int64_t n, const void** xc, int32_t* out, Scratch& s) {
+  const float* xt = transform_dev(static_cast<const float*>(x), n, s);  // OPQ rotation; the raw store keeps the original rows
+  if (!xt) return -1;
+  *xc = xt;
+  return assign_dev(xt, dpad_, n, out, s);
+}
+
+int IvfIndex::index_batch(const void* x, int64_t n, int64_t vid0, const uint8_t* del_bitmap) {
   cudaStream_t st = build_stream_;
   Scratch s(st);
-  x = transform_dev(x, n, s);  // OPQ rotation; the raw store keeps the original rows
-  if (!x) return -1;
   GB_ALLOC(d_assign, int32_t, n, s);
-  if (assign_dev(x, dpad_, n, d_assign, s)) return -1;
+  if (assign_batch(x, n, &x, d_assign, s)) return -1;
   std::vector<int32_t> h_list(n), h_pos(n);
   GB_CUDA(cudaMemcpyAsync(h_list.data(), d_assign, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
@@ -1355,7 +1369,7 @@ int IvfIndex::add_pending(const uint8_t* del_bitmap) {
   const int64_t BATCH = 1 << 20;
   for (;;) {
     int64_t vid0 = indexed_count_, n = 0;
-    const float* x = nullptr;
+    const void* x = nullptr;
     Scratch s(build_stream_);
     {  // add_vectors (exclusive mu_) may append segments while we look: the segment table is read under the shared lock
       std::shared_lock<std::shared_mutex> lk(mu_);
@@ -1431,7 +1445,7 @@ int IVFFlatIndex::lists_changed(cudaStream_t st) {
   return 0;
 }
 
-int Index::update_vector(int64_t vid, const float* x) {
+int Index::update_vector(int64_t vid, const void* x) {
   cudaSetDevice(device_);
   std::unique_lock<std::shared_mutex> lk(mu_);
   // host rows are overwritten by the CPU at once, not in stream order: no kernel or copy of an earlier search may still
@@ -1442,7 +1456,7 @@ int Index::update_vector(int64_t vid, const float* x) {
 
 // GammaIVFFlatIndex::Update / GammaIVFPQIndex::Update (gamma_index_ivfflat.cc:476-522,
 // gamma_index_ivfpq.cc:402-453): tombstone the old entry, append the new vector to its list.
-int IvfIndex::update_vector(int64_t vid, const float* x) {
+int IvfIndex::update_vector(int64_t vid, const void* x) {
   std::lock_guard<std::mutex> bg(build_mu_);
   if (Index::update_vector(vid, x)) return -1;
   if (!trained_ || vid >= indexed_count_) return 0;  // not indexed yet: the add path will pick it up
@@ -1451,7 +1465,7 @@ int IvfIndex::update_vector(int64_t vid, const float* x) {
     if (lists_->tombstone((int)(vid2pos_[vid] >> 32), (int)(uint32_t)vid2pos_[vid], build_stream_)) return -1;
   }
   Scratch s(build_stream_);
-  const float* x_dev = store_rows_dev(vid, 1, s);
+  const void* x_dev = store_rows_dev(vid, 1, s);
   if (!x_dev) return -1;
   return index_batch(x_dev, 1, vid, nullptr);
 }
@@ -1856,9 +1870,10 @@ int IvfPqBase::train_codebook(const float* x, int64_t n, Scratch& s) {
   return codebook_changed(st);
 }
 
-int IvfPqBase::append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+int IvfPqBase::append_batch(const void* xv, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
                             const std::vector<int>& add, Scratch& s) {
   (void)add;
+  const float* x = static_cast<const float*>(xv);
   cudaStream_t st = s.stream();
   const int cb = code_bytes();
   GB_ALLOC(codes, uint8_t, (size_t)n * cb, s);
@@ -2435,6 +2450,294 @@ int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, 
 }
 
 // ------------------------------------------------------------------------------------------
+// GammaIndexBinaryIVF (gamma_index_binary_ivf.cc) over faiss::IndexBinaryIVF
+BinaryIvfIndex::BinaryIvfIndex(int d_bits, const ModelParams& mp, int device, int seg_shift)
+    : IvfIndex("BINARYIVF", d_bits, mp, device, seg_shift, d_bits / 8), cb_(d_bits / 8) {
+  ldw_ = store_->stride() / 4;
+  mp_.metric = kMetricL2;  // Hamming distances rank like L2: smaller first
+  cudaMalloc(&d_bcent_, (size_t)nlist_ * ldw_ * 4);
+  cudaMemset(d_bcent_, 0, (size_t)nlist_ * ldw_ * 4);
+}
+BinaryIvfIndex::~BinaryIvfIndex() { cudaFree(d_bcent_); }
+int64_t BinaryIvfIndex::index_mem_bytes() const { return IvfIndex::index_mem_bytes() + (int64_t)nlist_ * ldw_ * 4; }
+
+// GammaIndexBinaryIVF::Indexing (gamma_index_binary_ivf.cc:212-270) -> faiss IndexBinaryIVF::train: the first num rows
+// expanded to +-1 floats, faiss Clustering (niter 10, Init) with an IndexFlatL2, centroids packed by sign
+int BinaryIvfIndex::train() {
+  std::lock_guard<std::mutex> bg(build_mu_);
+  if (trained_) return 0;
+  cudaSetDevice(device_);
+  const int64_t num = training_threshold();
+  if (num > store_->size()) {
+    set_last_error("vector total count less than training_threshold");
+    return -1;
+  }
+  std::unique_lock<std::shared_mutex> lk(mu_);
+  drain_searches();
+  cudaStream_t st = build_stream_;
+  Scratch s(st);
+  GB_ALLOC(raw, uint8_t, (size_t)num * ldw_ * 4, s);
+  GB_CUDA(store_->copy_rows_to_device(0, num, raw, st));
+  GB_ALLOC(xf, float, (size_t)num * dpad_, s);
+  GB_CUDA(launch_binary_to_real(raw, ldw_ * 4, num, d_, xf, dpad_, st));
+  KMeansParams kp;
+  kp.niter = 10;  // gamma_index_binary_ivf.cc:97
+  if (kmeans_device(xf, dpad_, num, d_, nlist_, kp, d_centroids_, dpad_, st, nullptr)) return -1;
+  GB_CUDA(launch_real_to_binary(d_centroids_, dpad_, nlist_, d_, d_bcent_, ldw_ * 4, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  if (!lists_) lists_.reset(new IvfLists(nlist_, code_bytes()));
+  trained_ = true;
+  return 0;
+}
+
+int BinaryIvfIndex::set_binary_centroids(const uint8_t* host, int nlist) {
+  if (nlist != nlist_) {
+    set_last_error("set_centroids: nlist mismatch");
+    return -1;
+  }
+  cudaSetDevice(device_);
+  std::unique_lock<std::shared_mutex> lk(mu_);
+  drain_searches();
+  GB_CUDA(cudaMemset(d_bcent_, 0, (size_t)nlist_ * ldw_ * 4));
+  GB_CUDA(cudaMemcpy2D(d_bcent_, (size_t)ldw_ * 4, host, cb_, cb_, nlist_, cudaMemcpyHostToDevice));
+  if (!lists_) lists_.reset(new IvfLists(nlist_, code_bytes()));
+  trained_ = true;
+  return 0;
+}
+int BinaryIvfIndex::get_binary_centroids(uint8_t* host) const {
+  cudaSetDevice(device_);
+  GB_CUDA(cudaMemcpy2D(host, cb_, d_bcent_, (size_t)ldw_ * 4, cb_, nlist_, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int BinaryIvfIndex::hamming_topk(const uint32_t* xq, int64_t ldq, int nq, const uint32_t* rows, int64_t ldr, int m,
+                                 int64_t id_base, int k, const FilterArgs& f, unsigned long long* out_keys,
+                                 int64_t out_stride, Scratch& s) {
+  cudaStream_t st = s.stream();
+  const int64_t ldo = round_up(m, 4);
+  const int QB = (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)nq, ((int64_t)1 << 28) / ldo, 65536}));
+  GB_ALLOC(scores, float, (size_t)QB * ldo, s);
+  for (int q0 = 0; q0 < nq; q0 += QB) {
+    const int qb = std::min(QB, nq - q0);
+    GB_CUDA(launch_hamming_tile(xq + (int64_t)q0 * ldq, ldq, qb, rows, ldr, m, (cb_ + 3) / 4, scores, ldo, st));
+    GB_CUDA(launch_select_scores(scores, ldo, qb, m, id_base, k, kMetricL2, f, out_keys + (int64_t)q0 * out_stride,
+                                 out_stride, st));
+  }
+  return 0;
+}
+
+// IndexBinaryFlat::assign: the Hamming-nearest centroid, the smaller list id among equals
+int BinaryIvfIndex::assign_batch(const void* x, int64_t n, const void** xc, int32_t* out, Scratch& s) {
+  *xc = x;
+  GB_ALLOC(best, unsigned long long, n, s);
+  const FilterArgs none{nullptr, nullptr, -FLT_MAX, FLT_MAX};
+  for (int64_t i0 = 0; i0 < n; i0 += 65536) {
+    const int nb = (int)std::min<int64_t>(65536, n - i0);
+    if (hamming_topk(static_cast<const uint32_t*>(x) + i0 * ldw_, ldw_, nb, reinterpret_cast<const uint32_t*>(d_bcent_),
+                     ldw_, nlist_, 0, 1, none, best + i0, 1, s))
+      return -1;
+  }
+  GB_CUDA(launch_split_keys(best, n, kMetricL2, nullptr, out, s.stream()));
+  return 0;
+}
+
+// the list entry is the row's d / 8 bytes as they are (IndexBinaryIVF::add_core)
+int BinaryIvfIndex::append_batch(const void* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                                 const std::vector<int>& add, Scratch& s) {
+  (void)add;
+  cudaStream_t st = s.stream();
+  GB_ALLOC(codes, uint8_t, (size_t)n * cb_, s);
+  GB_CUDA(cudaMemcpy2DAsync(codes, cb_, x, (size_t)ldw_ * 4, cb_, n, cudaMemcpyDeviceToDevice, st));
+  GB_CUDA(launch_ivf_append_codes(codes, n, cb_, d_list, d_pos, reinterpret_cast<uint8_t* const*>(lists_->d_data()),
+                                  lists_->d_ids(), vid0, st));
+  return 0;
+}
+
+int BinaryIvfIndex::scan_dev(const SearchContext&, const FilterArgs&, int, int, const float*, const float*, int,
+                             const int32_t*, const float*, int, unsigned long long*, Scratch&) {
+  set_last_error(type_ + ": queries are packed binary rows, not floats");
+  return -1;
+}
+
+int BinaryIvfIndex::flat_codes(const FilterArgs& f, int nq, const uint32_t* xq, int k, int64_t row_begin, int64_t row_end,
+                               unsigned long long* out_keys, Scratch& s) {
+  cudaStream_t st = s.stream();
+  if (row_end <= row_begin) return launch_fill_u64(out_keys, (int64_t)nq * k, kKeySentinel, st) == cudaSuccess ? 0 : -1;
+  const int64_t CC = std::min<int64_t>(131072, store_->seg_rows());
+  std::vector<std::pair<int64_t, int>> chunks;  // (first row, rows), inside one segment
+  for (int64_t r = row_begin; r < row_end;) {
+    const int64_t off = r & (store_->seg_rows() - 1);
+    const int cnt = (int)std::min<int64_t>(std::min(row_end - r, store_->seg_rows() - off), CC);
+    chunks.emplace_back(r, cnt);
+    r += cnt;
+  }
+  const int nch = (int)chunks.size();
+  unsigned long long* partial = out_keys;
+  if (nch > 1) {
+    partial = s.alloc_n<unsigned long long>((size_t)nq * nch * k);
+    if (!partial) return -1;
+  }
+  last_scan_kernel_ = "hamming_tile_kernel+select_rows_kernel";
+  scan_timer_begin(st);
+  for (int c = 0; c < nch; c++) {
+    // host placement: the chunk is copied to HBM first, in stream order (the same chunks, so the same keys)
+    const uint32_t* rows = static_cast<const uint32_t*>(store_rows_dev(chunks[c].first, chunks[c].second, s));
+    if (!rows) return -1;
+    if (hamming_topk(xq, ldw_, nq, rows, ldw_, chunks[c].second, chunks[c].first, k, f, partial + (int64_t)c * k,
+                     (int64_t)nch * k, s))
+      return -1;
+  }
+  if (nch > 1) GB_CUDA(launch_select_keys(partial, (int64_t)nch * k, nq, nch * k, k, out_keys, k, st));
+  scan_timer_end(st);
+  return 0;
+}
+
+// quantizer->search: the nprobe Hamming-nearest centroids, the smaller list id among equals
+int BinaryIvfIndex::coarse_codes(int nq, const uint32_t* xq, int nprobe, int32_t* probe_ids, float* coarse_dis, Scratch& s) {
+  GB_ALLOC(keys, unsigned long long, (size_t)nq * nprobe, s);
+  const FilterArgs none{nullptr, nullptr, -FLT_MAX, FLT_MAX};
+  if (hamming_topk(xq, ldw_, nq, reinterpret_cast<const uint32_t*>(d_bcent_), ldw_, nlist_, 0, nprobe, none, keys, nprobe, s))
+    return -1;
+  GB_CUDA(launch_split_keys(keys, (int64_t)nq * nprobe, kMetricL2, coarse_dis, probe_ids, s.stream()));
+  return 0;
+}
+
+// search_knn_hamming_heap over the probed lists: the shared query-major list scan with the Hamming codec, then the merge
+// of its CTA groups
+int BinaryIvfIndex::scan_codes(const FilterArgs& f, int nq, const uint32_t* xq, int k, const int32_t* probe_ids, int nprobe,
+                               unsigned long long* out_keys, Scratch& s) {
+  cudaStream_t st = s.stream();
+  const int max_k = binary_scan_max_k(cb_);
+  if (k > max_k) {
+    set_last_error(type_ + ": topK [" + std::to_string(k) + "] above " + std::to_string(max_k) +
+                   " is not supported by this engine at " + std::to_string(d_) + " bits");
+    return -1;
+  }
+  const int nsm = sm_count(device_);
+  const int pg = (int)std::min<int64_t>(32, std::max<int64_t>(1, (int64_t)nprobe * nq / ((int64_t)nsm * 32)));
+  const int ngroups = (nprobe + pg - 1) / pg;
+  GB_ALLOC(partial, unsigned long long, (size_t)nq * ngroups * k, s);
+  last_scan_kernel_ = "binary_ivf_scan_kernel";
+  snprintf(last_scan_info_, sizeof(last_scan_info_), "{\"probes_per_cta\": %d}", pg);
+  scan_timer_begin(st);
+  GB_CUDA(launch_binary_ivf_scan(xq, ldw_, nq, probe_ids, nprobe, pg, lists_->directory(), cb_, k, f, partial, st));
+  scan_timer_end(st);
+  if (ngroups > 1) {
+    GB_CUDA(launch_select_keys(partial, (int64_t)ngroups * k, nq, ngroups * k, k, out_keys, k, st));
+  } else {
+    GB_CUDA(cudaMemcpyAsync(out_keys, partial, (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, st));
+  }
+  return 0;
+}
+
+const uint32_t* BinaryIvfIndex::upload_queries(int nq, const uint8_t* x, Scratch& s) {
+  uint32_t* dq = s.alloc_n<uint32_t>((size_t)nq * ldw_);
+  if (!dq) return nullptr;
+  if (cudaMemsetAsync(dq, 0, (size_t)nq * ldw_ * 4, s.stream()) != cudaSuccess ||
+      cudaMemcpy2DAsync(dq, (size_t)ldw_ * 4, x, cb_, cb_, nq, cudaMemcpyHostToDevice, s.stream()) != cudaSuccess) {
+    set_last_error("BINARYIVF: query upload failed");
+    return nullptr;
+  }
+  return dq;
+}
+
+int BinaryIvfIndex::finish_host(const unsigned long long* keys, int nq, int k, float* out_dis, int64_t* out_ids,
+                                cudaStream_t st) {
+  Scratch s(st);
+  GB_ALLOC(dd, float, (size_t)nq * k, s);
+  GB_ALLOC(di, int64_t, (size_t)nq * k, s);
+  GB_CUDA(launch_decode_keys(keys, k, nq, k, kMetricL2, dd, di, 0, st));
+  GB_CUDA(cudaMemcpyAsync(out_dis, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// GammaIndexBinaryIVF::Search (gamma_index_binary_ivf.cc:290-325) with this engine's brute-force and realtime-tail rules
+// (Index::search_device): brute_force or an untrained index scan every stored row exactly; search_unindexed_tail adds
+// the stored but not yet indexed rows, merged by distance
+int BinaryIvfIndex::search_codes(const SearchContext& ctx, int nq, const uint8_t* x, int k, float* out_dis, int64_t* out_ids) {
+  if (nq <= 0) return 0;
+  if (k <= 0 || k > 4096) {
+    set_last_error("topK must be in [1, 4096]");
+    return -1;
+  }
+  cudaSetDevice(device_);
+  cudaStream_t st = thread_stream(device_);
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  Scratch s(st);
+  const uint32_t* xq = upload_queries(nq, x, s);
+  if (!xq) return -1;
+  FilterArgs f;
+  if (upload_bitmaps(ctx, &f, s)) return -1;
+  GB_ALLOC(keys, unsigned long long, (size_t)nq * k, s);
+  if (ctx.params.brute_force || !trained_) {
+    if (flat_codes(f, nq, xq, k, 0, store_->size(), keys, s)) return -1;
+  } else {
+    const int nprobe = resolve_nprobe(ctx);
+    GB_ALLOC(probe_ids, int32_t, (size_t)nq * nprobe, s);
+    GB_ALLOC(coarse_dis, float, (size_t)nq * nprobe, s);
+    if (coarse_codes(nq, xq, nprobe, probe_ids, coarse_dis, s)) return -1;
+    if (scan_codes(f, nq, xq, k, probe_ids, nprobe, keys, s)) return -1;
+    const int64_t tail0 = indexed_count_, tail1 = store_->size();
+    if (ctx.search_unindexed_tail && tail1 > tail0) {
+      GB_ALLOC(both, unsigned long long, (size_t)nq * 2 * k, s);
+      GB_CUDA(cudaMemcpy2DAsync(both, (size_t)2 * k * 8, keys, (size_t)k * 8, (size_t)k * 8, nq, cudaMemcpyDeviceToDevice, st));
+      GB_ALLOC(tailk, unsigned long long, (size_t)nq * k, s);
+      if (flat_codes(f, nq, xq, k, tail0, tail1, tailk, s)) return -1;
+      GB_CUDA(cudaMemcpy2DAsync(both + k, (size_t)2 * k * 8, tailk, (size_t)k * 8, (size_t)k * 8, nq, cudaMemcpyDeviceToDevice,
+                                st));
+      GB_CUDA(launch_select_keys(both, (int64_t)2 * k, nq, 2 * k, k, keys, k, st));
+    }
+  }
+  return finish_host(keys, nq, k, out_dis, out_ids, st);
+}
+
+int BinaryIvfIndex::coarse_search_codes(int nq, const uint8_t* x, int nprobe, float* out_dis, int64_t* out_ids) {
+  if (nq <= 0) return 0;
+  if (!trained_ || nprobe <= 0 || nprobe > std::min(nlist_, 4096)) {
+    set_last_error("coarse_search: untrained index or nprobe out of range");
+    return -1;
+  }
+  cudaSetDevice(device_);
+  cudaStream_t st = thread_stream(device_);
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  Scratch s(st);
+  const uint32_t* xq = upload_queries(nq, x, s);
+  if (!xq) return -1;
+  GB_ALLOC(keys, unsigned long long, (size_t)nq * nprobe, s);
+  const FilterArgs none{nullptr, nullptr, -FLT_MAX, FLT_MAX};
+  if (hamming_topk(xq, ldw_, nq, reinterpret_cast<const uint32_t*>(d_bcent_), ldw_, nlist_, 0, nprobe, none, keys, nprobe, s))
+    return -1;
+  return finish_host(keys, nq, nprobe, out_dis, out_ids, st);
+}
+
+int BinaryIvfIndex::search_preassigned_codes(const SearchContext& ctx, int nq, const uint8_t* x, int k, const int64_t* keys,
+                                             int nprobe, float* out_dis, int64_t* out_ids) {
+  if (nq <= 0) return 0;
+  if (!lists_ || k <= 0 || k > 4096 || nprobe <= 0 || nprobe > 4096) {
+    set_last_error("search_preassigned: untrained index, topK or nprobe out of range");
+    return -1;
+  }
+  cudaSetDevice(device_);
+  cudaStream_t st = thread_stream(device_);
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  Scratch s(st);
+  const uint32_t* xq = upload_queries(nq, x, s);
+  if (!xq) return -1;
+  FilterArgs f;
+  if (upload_bitmaps(ctx, &f, s)) return -1;
+  std::vector<int32_t> h_ids((size_t)nq * nprobe);
+  for (size_t i = 0; i < h_ids.size(); i++) h_ids[i] = (int32_t)keys[i];
+  GB_ALLOC(probe_ids, int32_t, h_ids.size(), s);
+  GB_CUDA(cudaMemcpyAsync(probe_ids, h_ids.data(), h_ids.size() * 4, cudaMemcpyHostToDevice, st));
+  GB_ALLOC(okeys, unsigned long long, (size_t)nq * k, s);
+  if (scan_codes(f, nq, xq, k, probe_ids, nprobe, okeys, s)) return -1;
+  const int rc = finish_host(okeys, nq, k, out_dis, out_ids, st);  // synchronises before h_ids goes
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------
 Index* create_index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
@@ -2517,6 +2820,24 @@ Index* create_index(const std::string& type, int d, const ModelParams& mp, int d
       return nullptr;
     }
     return new IVFPQFastScanIndex(d, mp, device, seg_shift);
+  }
+  if (type == "BINARYIVF") {  // BinaryModelParams::Parse (gamma_index_binary_ivf.cc:33-50): only ncentroids is read
+    if (d % 8 != 0) {
+      set_last_error("BINARYIVF: dimension [" + std::to_string(d) + "] must be a multiple of 8 bits");
+      return nullptr;
+    }
+    if (mp.ncentroids_arg < -1) {
+      set_last_error("invalid ncentroids = " + std::to_string(mp.ncentroids_arg));
+      return nullptr;
+    }
+    ModelParams bmp = mp;
+    bmp.ncentroids = mp.ncentroids_arg > 0 ? mp.ncentroids_arg : BinaryIvfIndex::kDefaultNlist;
+    bmp.nprobe = BinaryIvfIndex::kDefaultNprobe;  // the reference ignores nprobe, metric_type and nsubvector
+    if (binary_scan_max_k(d / 8) < 1) {
+      set_last_error("BINARYIVF: dimension [" + std::to_string(d) + "] is too large for the list scan of this engine");
+      return nullptr;
+    }
+    return new BinaryIvfIndex(d, bmp, device, seg_shift);
   }
   set_last_error("unsupported index type " + type);
   return nullptr;

@@ -52,8 +52,9 @@ class Scratch {
   std::vector<void*> ptrs_;
 };
 
-// MemoryRawVector on device (vector/memory_raw_vector.cc:152-240): append-only fp32 rows kept in
-// fixed-size segments, row stride dpad (d rounded up to 4 floats, zero padded).  The segments are in HBM, or, for a
+// MemoryRawVector on device (vector/memory_raw_vector.cc:152-240): append-only rows of row_bytes bytes kept in
+// fixed-size segments, row stride row_bytes rounded up to 16 bytes, zero padded.  A row is d fp32 values (4 d bytes,
+// stride 4 dpad) for the float index types and d / 8 packed bytes for BINARYIVF: the store knows only its byte size.  The segments are in HBM, or, for a
 // field whose store_type is "RocksDB" (host placement), in pinned host memory mapped into the device's address space:
 // kernels then read rows over PCIe through the same segment table, and the partition's HBM holds only its index.
 class RawStore {
@@ -61,29 +62,30 @@ class RawStore {
   // host placement: segments of 2^kHostSegShift rows (32 MiB at d = 128), so a small partition pins little memory;
   // kMaxSegs of them still cover 2^32 rows
   static constexpr int kHostSegShift = 16;
-  RawStore(int d, int seg_shift, bool host);
+  RawStore(int row_bytes, int seg_shift, bool host);
   ~RawStore();
-  int d() const { return d_; }
-  int dpad() const { return dpad_; }
+  int row_bytes() const { return (int)row_bytes_; }
+  int64_t stride() const { return stride_; }  // bytes between rows
   int64_t size() const { return n_; }
   bool on_host() const { return host_; }
   int seg_shift() const { return seg_shift_; }
   int64_t seg_rows() const { return (int64_t)1 << seg_shift_; }
   int nsegs() const { return (int)segs_.size(); }
   // a segment's base: device memory, or (host placement) the pinned host rows, for copies
-  const float* seg(int i) const { return segs_[i].base; }
+  const unsigned char* seg_bytes(int i) const { return segs_[i].base; }
+  const float* seg(int i) const { return reinterpret_cast<const float*>(segs_[i].base); }  // float index types
   // device-visible segment bases [kMaxSegs], what kernels index rows through
-  const float* const* d_segs() const { return d_segs_; }
-  // rows: n x d floats (stride d) on host, or n x dpad (stride ld) on device
-  int append_host(const float* x, int64_t n, cudaStream_t st);
-  int append_device(const float* x, int64_t ld, int64_t n, cudaStream_t st);
-  int update_host(int64_t vid, const float* x, cudaStream_t st);
-  int get_host(int64_t vid, float* out) const;
-  int get_rows_host(int64_t start, int64_t n, float* out) const;  // n x d, stride d
-  // contiguous copy of rows [0, n) (training slab, GetVectorHeader): returns device ptr, owned by `s`
+  const float* const* d_segs() const { return reinterpret_cast<const float* const*>(d_segs_); }
+  // rows: n x row_bytes, packed, on host, or n rows ld_bytes apart on device
+  int append_host(const void* x, int64_t n, cudaStream_t st);
+  int append_device(const void* x, int64_t ld_bytes, int64_t n, cudaStream_t st);
+  int update_host(int64_t vid, const void* x, cudaStream_t st);
+  int get_host(int64_t vid, void* out) const;
+  int get_rows_host(int64_t start, int64_t n, void* out) const;  // n x row_bytes, packed
+  // contiguous copy of the fp32 rows [0, n) (training slab, GetVectorHeader): returns device ptr, owned by `s`
   const float* contiguous(int64_t n, Scratch& s);
-  // rows [start, start + n) (n x dpad) into device memory at dst, ordered on st
-  cudaError_t copy_rows_to_device(int64_t start, int64_t n, float* dst, cudaStream_t st) const;
+  // rows [start, start + n) (stride() bytes apart) into device memory at dst, ordered on st
+  cudaError_t copy_rows_to_device(int64_t start, int64_t n, void* dst, cudaStream_t st) const;
   int64_t mem_bytes() const { return phys_bytes_; }  // physical HBM behind the store (0 for host placement)
   int64_t host_bytes() const { return host_bytes_; }  // pinned host memory behind the store
 
@@ -92,16 +94,18 @@ class RawStore {
   int new_segment();
   int map_rows(int si, int64_t rows);
   struct Seg {
-    float* base = nullptr;
+    unsigned char* base = nullptr;
     bool vmm = false;
     size_t va_bytes = 0, mapped = 0, gran = 0;
     std::vector<std::pair<unsigned long long, size_t>> chunks;  // (CUmemGenericAllocationHandle, bytes), in address order
   };
-  int d_, dpad_, seg_shift_, device_ = 0;
+  size_t row_bytes_;
+  int64_t stride_;
+  int seg_shift_, device_ = 0;
   bool host_;
   int64_t n_ = 0, phys_bytes_ = 0, host_bytes_ = 0;
   std::vector<Seg> segs_;
-  float** d_segs_ = nullptr;  // device array [kMaxSegs]
+  unsigned char** d_segs_ = nullptr;  // device array [kMaxSegs]
   static constexpr int kMaxSegs = 65536;
 };
 
@@ -169,6 +173,7 @@ struct ModelParams {  // index/impl/gamma_index_ivfpq.h:1031-1257, gamma_index_i
   bool has_opq = false;         // an "opq" object was given (IVFPQFastScan refuses it)
   int bbs = 32;                 // IVFPQFastScan block size as given (gamma_index_ivfpqfs.h:126-133; <= 0 => 32)
   bool host_store = false;      // raw vectors in pinned host memory (store_type "RocksDB"); otherwise in HBM
+  int ncentroids_arg = 0;       // "ncentroids" as given, 0 if absent (BINARYIVF has its own default and range check)
 };
 
 struct RetrievalParams {  // gamma_index_ivfpq.cc:233-294, gamma_index_ivfflat.cc:293-340
@@ -190,7 +195,8 @@ struct SearchContext {  // RetrievalContext / SearchCondition (common/gamma_comm
 
 class Index {
  public:
-  Index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift);
+  // row_bytes: bytes of a stored row (0: 4 d, d fp32 values)
+  Index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int row_bytes = 0);
   virtual ~Index();
   const std::string& type() const { return type_; }
   int d() const { return d_; }
@@ -204,8 +210,8 @@ class Index {
   // whether Engine::Dump saves the trained state (centroids, codebook) for Load to restore; false: Load trains again
   virtual bool persists_trained_state() const { return true; }
 
-  // AddToStore (vector_manager.cc:455): append raw vectors, host rows n x d
-  int add_vectors(const float* x, int64_t n);
+  // AddToStore (vector_manager.cc:455): append raw vectors, host rows n x store().row_bytes() bytes
+  int add_vectors(const void* x, int64_t n);
   int add_vectors_device(const float* x, int64_t ld, int64_t n);
   // IndexModel::Indexing(): train on the first `num` stored vectors
   virtual int train() { trained_ = true; return 0; }
@@ -213,7 +219,7 @@ class Index {
   virtual int add_pending(const uint8_t* del_bitmap) { indexed_count_ = store_->size(); return 0; }
   // Engine::Update -> RawVector update + IndexModel::Update (search/engine.cc:774-850;
   // realtime_mem_data.cc:298-320: old entry tombstoned, vector re-appended to its new list)
-  virtual int update_vector(int64_t vid, const float* x);
+  virtual int update_vector(int64_t vid, const void* x);  // x: one row of store().row_bytes() bytes
   // IndexModel::Search (index_model.h:296): x = nq x d floats; out = nq x k, unfilled id -1.
   // Returns 0, -1 on error (last_error), -2 if killed.  x/out pointers are host unless *_dev.
   int search(const SearchContext& ctx, int nq, const float* x, int k, float* out_dis, int64_t* out_ids);
@@ -245,9 +251,9 @@ class Index {
   virtual int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
                               unsigned long long* out_keys, Scratch& s) = 0;
   int upload_bitmaps(const SearchContext& ctx, FilterArgs* f, Scratch& s);
-  // rows [vid0, vid0 + n) as device rows (stride dpad): in HBM the segment itself (the rows must lie in one segment),
-  // for host placement a copy in `s`, ordered on its stream (any rows)
-  const float* store_rows_dev(int64_t vid0, int64_t n, Scratch& s);
+  // rows [vid0, vid0 + n) as device rows (store().stride() bytes apart): in HBM the segment itself (the rows must lie in
+  // one segment), for host placement a copy in `s`, ordered on its stream (any rows)
+  const void* store_rows_dev(int64_t vid0, int64_t n, Scratch& s);
   // A copy stream and its events for the staged FLAT scan of a host store (flat_search_dev).  Created on first use and
   // pooled: a search holds a lane while it enqueues its copies; what it enqueued keeps the events' records it waited on.
   struct CopyLane {
@@ -381,12 +387,12 @@ struct GammaFileFormat {
 // entries (append_batch, code_bytes) and how a query scans the probed lists (scan_dev).
 class IvfIndex : public Index {
  public:
-  IvfIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift);
+  IvfIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int row_bytes = 0);
   ~IvfIndex() override;
   int training_threshold() const override;
   int train() override;
   int add_pending(const uint8_t* del_bitmap) override;
-  int update_vector(int64_t vid, const float* x) override;
+  int update_vector(int64_t vid, const void* x) override;
   int reset_index() override;
   int64_t index_mem_bytes() const override;
   int nlist() const { return nlist_; }
@@ -434,11 +440,15 @@ class IvfIndex : public Index {
   int group_pairs_by_list(const int32_t* probe_ids, int64_t npairs, int nseg, int group, int64_t max_items, LmGrouping* g,
                           Scratch& s);
   int assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* assign_dev_out, Scratch& s);
+  // the rows of a batch as the codec takes them (*xc) and each row's nearest list (out): fp32 rows (stride dpad) through
+  // transform_dev and assign_dev; BINARYIVF: the packed rows as they are, by Hamming distance
+  virtual int assign_batch(const void* x, int64_t n, const void** xc, int32_t* out, Scratch& s);
   int resolve_nprobe(const SearchContext& ctx) const;
   // metric of the coarse quantiser (list assignment and probe choice) for a search under `metric`
   virtual int coarse_metric(int metric) const { return metric; }
-  // write rows x [vid0, vid0+n) into the lists at (d_list, d_pos), after reserve and before commit; add[l] = rows for list l
-  virtual int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+  // write rows x [vid0, vid0+n) (as assign_batch left them) into the lists at (d_list, d_pos), after reserve and before
+  // commit; add[l] = rows for list l
+  virtual int append_batch(const void* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
                            const std::vector<int>& add, Scratch& s) = 0;
   virtual int train_extra(const float* xtrain, int64_t n, Scratch& s) { (void)xtrain; (void)n; (void)s; return 0; }
   // codec state dropped by reset_index, with build_mu_ and mu_ held exclusively
@@ -449,8 +459,8 @@ class IvfIndex : public Index {
   virtual const float* train_transform(const float* xt, int64_t n, Scratch& s) { (void)n; (void)s; return xt; }
   virtual const float* transform_dev(const float* x, int64_t n, Scratch& s) { (void)n; (void)s; return x; }
 
-  // index rows [vid0, vid0+n) (device pointer x, stride dpad) into the lists
-  int index_batch(const float* x, int64_t n, int64_t vid0, const uint8_t* del_bitmap);
+  // index rows [vid0, vid0+n) (device pointer x, store().stride() bytes apart) into the lists
+  int index_batch(const void* x, int64_t n, int64_t vid0, const uint8_t* del_bitmap);
   // after every change of the lists (append, compaction), with mu_ held exclusively, ordered on st
   virtual int lists_changed(cudaStream_t st) { (void)st; return 0; }
   int compact_locked();  // lists_->compact + lists_changed, with mu_ held exclusively
@@ -484,7 +494,7 @@ class IVFFlatIndex : public IvfIndex {
   // list-major IVF-Flat scan on the tensor cores (kernels_tc.cu); returns 1 if not applicable
   int scan_listmajor_dev(const FilterArgs& f, int metric, int nq, const float* xq, int k, const int32_t* probe_ids,
                          int nprobe, unsigned long long* out_keys, Scratch& s);
-  int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+  int append_batch(const void* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
                    const std::vector<int>& add, Scratch& s) override;
   void reset_codec() override;
   int lists_changed(cudaStream_t st) override;
@@ -536,7 +546,7 @@ class IvfPqBase : public IvfIndex {
   virtual cudaError_t encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st) = 0;
   // tables derived from the codebook, rebuilt after every change of it
   virtual int codebook_changed(cudaStream_t st) { (void)st; return 0; }
-  int append_batch(const float* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+  int append_batch(const void* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
                    const std::vector<int>& add, Scratch& s) override;
   // faiss ProductQuantizer::train on n rows (stride dpad): M independent ksub-means on the dsub-wide slices
   int train_codebook(const float* x, int64_t n, Scratch& s);
@@ -641,6 +651,58 @@ class IVFPQFastScanIndex : public IvfPqBase {
   int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, const float* xq_raw, int k,
                const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
                Scratch& s) override;
+};
+
+// GammaIndexBinaryIVF (index/impl/gamma_index_binary_ivf.{h,cc}): faiss::IndexBinaryIVF over packed binary rows of
+// d / 8 bytes (d in bits), compared by Hamming distance, smaller first.  The coarse centroids are trained by faiss
+// Clustering on the rows expanded to +-1 floats (binary_to_real), kept as floats in d_centroids_ and packed again
+// (real_to_binary) for the coarse quantiser; list entries are the raw d / 8 bytes.  Rows and queries cross this class
+// as packed bytes only: its float entry points (Index::search, coarse_search_host, ...) are refused.
+class BinaryIvfIndex : public IvfIndex {
+ public:
+  static constexpr int kDefaultNlist = 256;   // BinaryModelParams() (gamma_index_binary_ivf.cc:23)
+  static constexpr int kDefaultNprobe = 20;   // GammaIndexBinaryIVF::Init (gamma_index_binary_ivf.cc:114)
+  BinaryIvfIndex(int d_bits, const ModelParams& mp, int device, int seg_shift);
+  ~BinaryIvfIndex() override;
+  int code_bytes() const override { return cb_; }
+  bool persists_trained_state() const override { return false; }
+  int train() override;
+  int64_t index_mem_bytes() const override;
+  // x: nq x d / 8 bytes on host; out: nq x k, integer distances as floats, unfilled id -1
+  int search_codes(const SearchContext& ctx, int nq, const uint8_t* x, int k, float* out_dis, int64_t* out_ids);
+  // packed centroids [nlist][d / 8] (set_binary_centroids marks the index trained)
+  int set_binary_centroids(const uint8_t* host, int nlist);
+  int get_binary_centroids(uint8_t* host) const;
+  int coarse_search_codes(int nq, const uint8_t* x, int nprobe, float* out_dis, int64_t* out_ids);
+  int search_preassigned_codes(const SearchContext& ctx, int nq, const uint8_t* x, int k, const int64_t* keys, int nprobe,
+                               float* out_dis, int64_t* out_ids);
+
+ protected:
+  GammaFileFormat gamma_format() const override { return GammaFileFormat(); }  // Dump writes nothing
+  int64_t default_training_threshold() const override { return (int64_t)nlist_ * 39; }  // nlist * min_points_per_centroid
+  int assign_batch(const void* x, int64_t n, const void** xc, int32_t* out, Scratch& s) override;
+  int append_batch(const void* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                   const std::vector<int>& add, Scratch& s) override;
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, const float* xq_raw, int k,
+               const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
+               Scratch& s) override;
+
+ private:
+  // the k nearest of rows [0, m) (ldr words apart, ids id_base + row) for nq queries (ldq words apart), filtered:
+  // out_keys[q * out_stride ..], sorted
+  int hamming_topk(const uint32_t* xq, int64_t ldq, int nq, const uint32_t* rows, int64_t ldr, int m, int64_t id_base, int k,
+                   const FilterArgs& f, unsigned long long* out_keys, int64_t out_stride, Scratch& s);
+  // brute force over the stored rows [row_begin, row_end)
+  int flat_codes(const FilterArgs& f, int nq, const uint32_t* xq, int k, int64_t row_begin, int64_t row_end,
+                 unsigned long long* out_keys, Scratch& s);
+  int coarse_codes(int nq, const uint32_t* xq, int nprobe, int32_t* probe_ids, float* coarse_dis, Scratch& s);
+  int scan_codes(const FilterArgs& f, int nq, const uint32_t* xq, int k, const int32_t* probe_ids, int nprobe,
+                 unsigned long long* out_keys, Scratch& s);
+  const uint32_t* upload_queries(int nq, const uint8_t* x, Scratch& s);
+  int finish_host(const unsigned long long* keys, int nq, int k, float* out_dis, int64_t* out_ids, cudaStream_t st);
+  int cb_;             // bytes per row, d / 8
+  int64_t ldw_;        // words between device rows (the raw store's stride)
+  uint8_t* d_bcent_ = nullptr;  // [nlist][4 ldw_] packed centroids
 };
 
 // host rows n x d (stride d) -> device rows n x dpad, the padding columns zeroed

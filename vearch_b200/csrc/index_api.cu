@@ -34,6 +34,7 @@ bool parse_model_params(const std::string& text, ModelParams* mp, std::string* e
       return false;
     }
     if (v > 0) mp->ncentroids = v;
+    mp->ncentroids_arg = v;
   }
   if (jv.get_int("nprobe", &v)) {
     if (v < -1) {
@@ -187,24 +188,29 @@ void gb_index_destroy(gb_index* index) {
 
 int gb_index_add_vectors(gb_index* index, int64_t n, const float* x) {
   IDX_OR_FAIL(index);
+  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
   return index->impl->add_vectors(x, n);
 }
 int gb_index_add_vectors_device(gb_index* index, int64_t n, const float* x_dev, int64_t ld) {
   IDX_OR_FAIL(index);
+  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
   return index->impl->add_vectors_device(x_dev, ld, n);
 }
 int gb_index_update_vector(gb_index* index, int64_t vid, const float* x) {
   IDX_OR_FAIL(index);
+  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
   cudaSetDevice(index->impl->device());
   return index->impl->update_vector(vid, x);  // RawVector update + IndexModel::Update
 }
 int gb_index_get_vector(gb_index* index, int64_t vid, float* out) {
   IDX_OR_FAIL(index);
+  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
   cudaSetDevice(index->impl->device());
   return index->impl->store().get_host(vid, out);
 }
 int gb_index_get_vectors(gb_index* index, int64_t start, int64_t n, float* out) {
   IDX_OR_FAIL(index);
+  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
   cudaSetDevice(index->impl->device());
   return index->impl->store().get_rows_host(start, n, out);
 }
@@ -302,10 +308,12 @@ int gb_index_nlist(gb_index* index) {
 }
 int gb_index_set_centroids(gb_index* index, const float* centroids, int nlist) {
   IVF_OR_FAIL(ivf, index);
+  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
   return ivf->set_centroids(centroids, nlist);
 }
 int gb_index_get_centroids(gb_index* index, float* centroids) {
   IVF_OR_FAIL(ivf, index);
+  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
   return ivf->get_centroids(centroids);
 }
 int gb_index_pq_m(gb_index* index) {
@@ -402,6 +410,7 @@ int gb_index_tombstone(gb_index* index, int list, int pos) {
 }
 int gb_index_coarse_search(gb_index* index, int nq, const float* x, int nprobe, float* out_dis, int64_t* out_ids) {
   IVF_OR_FAIL(ivf, index);
+  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
   return ivf->coarse_search_host(nq, x, nprobe, out_dis, out_ids);
 }
 int gb_index_search_preassigned(gb_index* index, int nq, const float* x, int k, const int64_t* keys,
@@ -409,6 +418,7 @@ int gb_index_search_preassigned(gb_index* index, int nq, const float* x, int k, 
                                 const uint8_t* del_bitmap, const uint8_t* filter_bitmap, int64_t bitmap_bits,
                                 float min_score, float max_score, float* out_scores, int64_t* out_ids) {
   IVF_OR_FAIL(ivf, index);
+  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
   SearchContext ctx;
   if (fill_ctx(&ctx, retrieval_params_json, 0, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score)) return -1;
   return ivf->search_preassigned_host(ctx, nq, x, k, keys, coarse_dis, nprobe, out_scores, out_ids);
@@ -416,6 +426,56 @@ int gb_index_search_preassigned(gb_index* index, int nq, const float* x, int k, 
 int gb_index_pq_encode(gb_index* index, int64_t n, const float* x, const int64_t* assign, uint8_t* codes) {
   PQ_OR_FAIL(pq, index);
   return pq->encode_host(x, n, assign, codes);
+}
+
+#define BIN_OR_FAIL(v, index) AS_OR_FAIL(BinaryIvfIndex, v, index, "BINARYIVF")
+int gb_index_add_binary(gb_index* index, int64_t n, const uint8_t* x) {
+  BIN_OR_FAIL(b, index);
+  return b->add_vectors(x, n);
+}
+int gb_index_update_binary(gb_index* index, int64_t vid, const uint8_t* x) {
+  BIN_OR_FAIL(b, index);
+  cudaSetDevice(b->device());
+  return b->update_vector(vid, x);
+}
+int gb_index_get_binary(gb_index* index, int64_t start, int64_t n, uint8_t* out) {
+  BIN_OR_FAIL(b, index);
+  cudaSetDevice(b->device());
+  return b->store().get_rows_host(start, n, out);
+}
+int gb_index_search_binary(gb_index* index, int nq, const uint8_t* x, int k, const char* retrieval_params_json,
+                           int brute_force, const uint8_t* del_bitmap, const uint8_t* filter_bitmap, int64_t bitmap_bits,
+                           float min_score, float max_score, int search_unindexed_tail, float* out_scores, int64_t* out_ids) {
+  BIN_OR_FAIL(b, index);
+  SearchContext ctx;
+  if (fill_ctx(&ctx, retrieval_params_json, brute_force, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score))
+    return -1;
+  ctx.search_unindexed_tail = search_unindexed_tail != 0;
+  return b->search_codes(ctx, nq, x, k, out_scores, out_ids);
+}
+int gb_index_set_binary_centroids(gb_index* index, const uint8_t* centroids, int nlist) {
+  BIN_OR_FAIL(b, index);
+  return b->set_binary_centroids(centroids, nlist);
+}
+int gb_index_get_binary_centroids(gb_index* index, uint8_t* centroids) {
+  BIN_OR_FAIL(b, index);
+  return b->get_binary_centroids(centroids);
+}
+int gb_index_get_real_centroids(gb_index* index, float* centroids) {
+  BIN_OR_FAIL(b, index);
+  return b->get_centroids(centroids);
+}
+int gb_index_coarse_search_binary(gb_index* index, int nq, const uint8_t* x, int nprobe, float* out_dis, int64_t* out_ids) {
+  BIN_OR_FAIL(b, index);
+  return b->coarse_search_codes(nq, x, nprobe, out_dis, out_ids);
+}
+int gb_index_search_preassigned_binary(gb_index* index, int nq, const uint8_t* x, int k, const int64_t* keys, int nprobe,
+                                       const uint8_t* del_bitmap, const uint8_t* filter_bitmap, int64_t bitmap_bits,
+                                       float min_score, float max_score, float* out_scores, int64_t* out_ids) {
+  BIN_OR_FAIL(b, index);
+  SearchContext ctx;
+  if (fill_ctx(&ctx, "", 0, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score)) return -1;
+  return b->search_preassigned_codes(ctx, nq, x, k, keys, nprobe, out_scores, out_ids);
 }
 
 int gb_kmeans(int device, const float* x, int64_t n, int d, int k, int niter, int64_t seed, int spherical,

@@ -233,6 +233,21 @@ cudaError_t launch_ivfpqfs_scan(const uint8_t* lut8, const float* ab, int nq, co
                                 ListDirectory dir, int M, int k, int metric, FilterArgs f, unsigned long long* partial,
                                 cudaStream_t st);
 
+// ---- K12: BINARYIVF (kernels_binary.cu): packed binary rows, Hamming distance on the CUDA cores ---------------------
+// out[q][r] = popcount(Q_q ^ R_r) over `words` 32-bit words (rows zero padded to whole words; strides in words), exact
+// integers as fp32.  Used for every query x rows job: coarse search (rows = centroids), add-time assignment, brute force.
+cudaError_t launch_hamming_tile(const uint32_t* Q, int64_t ldq, int nq, const uint32_t* R, int64_t ldr, int m, int words,
+                                float* out, int64_t ldo, cudaStream_t st);
+// faiss binary_to_real / real_to_binary: bit j of a packed row (byte j >> 3, bit j & 7) <-> +1 / -1 (a float > 0 is 1)
+cudaError_t launch_binary_to_real(const uint8_t* x, int64_t ldx, int64_t n, int d, float* out, int64_t ldo, cudaStream_t st);
+cudaError_t launch_real_to_binary(const float* x, int64_t ldx, int64_t n, int d, uint8_t* out, int64_t ldo, cudaStream_t st);
+// query-major Hamming scan of the probed lists (code_size bytes per entry): partial[q][group][k] sorted, as
+// launch_ivfpq_scan; queries [nq][ldq] words, zero padded past code_size bytes
+cudaError_t launch_binary_ivf_scan(const uint32_t* queries, int64_t ldq, int nq, const int32_t* probe_ids, int nprobe, int pg,
+                                   ListDirectory dir, int code_size, int k, FilterArgs f, unsigned long long* partial,
+                                   cudaStream_t st);
+int binary_scan_max_k(int code_size);  // the largest k (<= 4096) the scan can select at this code size, 0 if none
+
 // ---- K6/K8: build-side kernels ------------------------------------------------------------
 // centroids[c] = (sum of x[perm[off[c]..off[c+1])] in that order) * (1/count); empty => zeros
 cudaError_t launch_segment_mean(const float* x, int64_t ldx, int d, const int32_t* perm, const int32_t* off, int k,

@@ -124,7 +124,9 @@ class GammaEngine:
         _status(_api().CreateTable(self._h, table_bytes, len(table_bytes)))
 
     def add_doc(self, key, vector, extra_fields=()):
-        v = np.ascontiguousarray(vector, np.float32).tobytes()
+        """vector: float32 values, or for a BINARYIVF table a uint8 array of dimension / 8 packed bytes"""
+        vector = np.asarray(vector)
+        v = (vector if vector.dtype == np.uint8 else vector.astype(np.float32)).tobytes()
         fields = [("_id", key.encode() if isinstance(key, str) else key, wire.DT_STRING)]
         fields += list(extra_fields)
         fields.append((self.vec_name, v, wire.DT_VECTOR))

@@ -360,6 +360,92 @@ class GammaIndex:
         return lut, ab
 
 
+class BinaryIVFIndex(GammaIndex):
+    """BINARYIVF (gamma_index_binary_ivf.cc): d is in bits, a multiple of 8; rows, queries and centroids are uint8 arrays
+    of shape [n, d / 8], bit i at bit (i & 7) of byte i >> 3 (numpy.packbits(..., bitorder="little")).  Scores are
+    Hamming distances as float32, smaller first."""
+
+    def __init__(self, d, params=None, device=0, store_type=None):
+        super().__init__("BINARYIVF", d, params, device, store_type)
+        self.code_bytes = self.d // 8
+
+    def _rows(self, x):
+        x = np.ascontiguousarray(x, dtype=np.uint8)
+        if x.ndim == 1:
+            x = x.reshape(1, -1)
+        assert x.ndim == 2 and x.shape[1] == self.code_bytes, f"expected uint8 rows of {self.code_bytes} bytes"
+        return x
+
+    def add_vectors(self, x):
+        x = self._rows(x)
+        _check(_lib.lib().gb_index_add_binary(self._h, x.shape[0], _ptr(x)), "add_binary")
+
+    def update_vector(self, vid, x):
+        x = self._rows(x)
+        _check(_lib.lib().gb_index_update_binary(self._h, vid, _ptr(x)), "update_binary")
+
+    def get_vectors(self, start, n):
+        out = np.empty((n, self.code_bytes), np.uint8)
+        _check(_lib.lib().gb_index_get_binary(self._h, start, n, _ptr(out)), "get_binary")
+        return out
+
+    def get_vector(self, vid):
+        return self.get_vectors(vid, 1)[0]
+
+    def search(self, x, k, params=None, brute_force=False, del_bitmap=None, filter_bitmap=None, min_score=-FLT_MAX,
+               max_score=FLT_MAX, search_unindexed_tail=False):
+        x = self._rows(x)
+        nq = x.shape[0]
+        dis = np.empty((nq, k), np.float32)
+        ids = np.empty((nq, k), np.int64)
+        pj = json.dumps(params).encode() if params else b""
+        db, fb = _bitmap(del_bitmap), _bitmap(filter_bitmap)
+        bits = max([b.size * 8 for b in (db, fb) if b is not None], default=0)
+        rc = _lib.lib().gb_index_search_binary(self._h, nq, _ptr(x), k, pj, int(brute_force), _ptr(db), _ptr(fb), bits,
+                                               C.c_float(min_score), C.c_float(max_score), int(search_unindexed_tail),
+                                               _ptr(dis), _ptr(ids))
+        _check(rc, "search_binary")
+        return dis, ids
+
+    def set_centroids(self, c):
+        c = self._rows(c)
+        _check(_lib.lib().gb_index_set_binary_centroids(self._h, _ptr(c), c.shape[0]), "set_binary_centroids")
+
+    def get_centroids(self):
+        out = np.empty((self.nlist, self.code_bytes), np.uint8)
+        _check(_lib.lib().gb_index_get_binary_centroids(self._h, _ptr(out)), "get_binary_centroids")
+        return out
+
+    def get_real_centroids(self):
+        """The float k-means centroids behind the packed ones (training's +-1 space)."""
+        out = np.empty((self.nlist, self.d), np.float32)
+        _check(_lib.lib().gb_index_get_real_centroids(self._h, _ptr(out)), "get_real_centroids")
+        return out
+
+    def coarse_search(self, x, nprobe):
+        x = self._rows(x)
+        dis = np.empty((x.shape[0], nprobe), np.float32)
+        ids = np.empty((x.shape[0], nprobe), np.int64)
+        _check(_lib.lib().gb_index_coarse_search_binary(self._h, x.shape[0], _ptr(x), nprobe, _ptr(dis), _ptr(ids)),
+               "coarse_search_binary")
+        return dis, ids
+
+    def search_preassigned(self, x, k, keys, del_bitmap=None, filter_bitmap=None, min_score=-FLT_MAX,
+                           max_score=FLT_MAX):
+        x = self._rows(x)
+        keys = np.ascontiguousarray(keys, dtype=np.int64)
+        nq, nprobe = keys.shape
+        dis = np.empty((nq, k), np.float32)
+        ids = np.empty((nq, k), np.int64)
+        db, fb = _bitmap(del_bitmap), _bitmap(filter_bitmap)
+        bits = max([b.size * 8 for b in (db, fb) if b is not None], default=0)
+        rc = _lib.lib().gb_index_search_preassigned_binary(self._h, nq, _ptr(x), k, _ptr(keys), nprobe, _ptr(db), _ptr(fb),
+                                                           bits, C.c_float(min_score), C.c_float(max_score), _ptr(dis),
+                                                           _ptr(ids))
+        _check(rc, "search_preassigned_binary")
+        return dis, ids
+
+
 def index_factory(d, description, metric=METRIC_L2, device=0, **extra):
     """index/index.h index_factory: "IVF1024,Flat" | "IVF4096,PQ16x8" | "IVF256,PQ32x4" (PQ<M>x<nbits>) | "Flat"."""
     parts = [p.strip() for p in description.split(",")]

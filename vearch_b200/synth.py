@@ -115,3 +115,34 @@ def sift_hard_torch(n, d, seed, device, latent=16, n_comp=64, centers_seed=99, c
         x = 100.0 + 3.0 * (z @ W.T) + 4.0 * torch.randn((e - s, d), generator=g, device=device)
         out[s:e] = torch.clamp(torch.round(x), 0, 218)
     return out
+
+
+def binary_clustered(n, d_bits, seed=1234, n_clusters=256, flip=0.1, centers_seed=99):
+    """[n, d_bits / 8] uint8 packed binary rows (bit i at bit i & 7 of byte i >> 3): random centre bit vectors, each row
+    a centre with every bit flipped independently at rate `flip`, so nearest neighbours share a centre and IVF recall
+    is meaningful"""
+    crng = np.random.default_rng(centers_seed)
+    centres = crng.integers(0, 2, size=(n_clusters, d_bits), dtype=np.uint8)
+    rng = np.random.default_rng(seed)
+    lab = rng.integers(0, n_clusters, size=n)
+    bits = centres[lab] ^ (rng.random((n, d_bits)) < flip).astype(np.uint8)
+    return np.packbits(bits, axis=1, bitorder="little")
+
+
+def binary_clustered_torch(n, d_bits, seed, device, n_clusters=4096, flip=0.1, centers_seed=99, chunk=1 << 20):
+    """binary_clustered generated on the device (another random stream): a torch uint8 [n, d_bits / 8] tensor"""
+    import torch
+    gc = torch.Generator(device=device)
+    gc.manual_seed(centers_seed)
+    centres = torch.randint(0, 2, (n_clusters, d_bits), generator=gc, device=device, dtype=torch.uint8)
+    g = torch.Generator(device=device)
+    g.manual_seed(seed)
+    weights = (2 ** torch.arange(8, device=device, dtype=torch.int32))
+    out = torch.empty((n, d_bits // 8), dtype=torch.uint8, device=device)
+    for s in range(0, n, chunk):
+        e = min(n, s + chunk)
+        lab = torch.randint(0, n_clusters, (e - s,), generator=g, device=device)
+        flips = (torch.rand((e - s, d_bits), generator=g, device=device) < flip).to(torch.uint8)
+        bits = (centres[lab] ^ flips).view(e - s, d_bits // 8, 8).to(torch.int32)
+        out[s:e] = (bits * weights).sum(2).to(torch.uint8)
+    return out

@@ -258,7 +258,9 @@ def encode_search_request(vec_name, queries, topn, index_params="", is_brute_sea
     extra_vec_queries: further (vector field, queries) pairs of a multi-vector search; ranker: WeightedRanker JSON;
     multi_vector_rank=1: order the joined documents by the combined score."""
     import numpy as np
-    q = np.ascontiguousarray(queries, dtype=np.float32)
+    q = np.ascontiguousarray(queries)  # uint8: packed binary queries of a BINARYIVF field, d / 8 bytes each
+    if q.dtype != np.uint8:
+        q = np.ascontiguousarray(q, dtype=np.float32)
     out = bytearray()
     params = {}
     if request_id:
