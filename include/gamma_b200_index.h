@@ -127,6 +127,13 @@ int gb_index_compact(gb_index *index);
 /* test hook: how often the tensor-core mirror of the lists (DESIGN.md section 2) was built in full; appends
  * that fit the reserved tiles update it in place and do not count */
 int gb_index_mirror_builds(gb_index *index);
+/* test hook (IVFFLAT): the list shifts s_l of the list-major L2 scan, nlist x d floats; its tensor-core operands are
+ * x - s_l and y - s_l.  s_l = round(c_l / g_l) * g_l with g_l the largest power of two <= rho_l / sqrt(d) and rho_l half
+ * the distance from centroid c_l to its nearest other centroid; s_l = c_l when rho_l = 0 */
+int gb_index_get_list_shifts(gb_index *index, float *out);
+/* test hook (IVF types): the kernel(s) of the last coarse search: "coarse_topk_kernel" (fused), or the score matrix of
+ * "dist_tc_kernel+select_rows_kernel" (>= 32 queries) or "dist_tile_kernel+select_rows_kernel" (exact) */
+const char *gb_index_last_coarse_kernel(gb_index *index);
 int gb_index_load(gb_index *index, const char *dir, const char *abs_name, int64_t *load_num);
 /* quantizer->search (gamma_index_ivfflat.cc:568) */
 int gb_index_coarse_search(gb_index *index, int nq, const float *x, int nprobe, float *out_dis, int64_t *out_ids);

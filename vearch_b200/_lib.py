@@ -82,6 +82,9 @@ def _declare(l):
     l.gb_index_dump.argtypes = [vp, cstr, cstr]
     l.gb_index_compact.argtypes = [vp]
     l.gb_index_mirror_builds.argtypes = [vp]
+    l.gb_index_get_list_shifts.argtypes = [vp, vp]
+    l.gb_index_last_coarse_kernel.argtypes = [vp]
+    l.gb_index_last_coarse_kernel.restype = cstr
     l.gb_index_load.argtypes = [vp, cstr, cstr, vp]
     l.gb_index_coarse_search.argtypes = [vp, i32, vp, i32, vp, vp]
     l.gb_index_search_preassigned.argtypes = [vp, i32, vp, i32, vp, vp, i32, cstr, vp, vp, i64, f32, f32, vp, vp]

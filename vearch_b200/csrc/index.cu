@@ -1215,7 +1215,15 @@ IvfIndex::~IvfIndex() {
   cudaFree(d_cent_tiles_);
   cudaFree(d_cent_norms_);
 }
+IVFFlatIndex::IVFFlatIndex(int d, const ModelParams& mp, int device, int seg_shift)
+    : IvfIndex("IVFFLAT", d, mp, device, seg_shift) {
+  if (metric() == kMetricL2) {  // inner products are scanned unshifted: no table
+    cudaMalloc(&d_shifts_, (size_t)nlist_ * dpad_ * 4);
+    cudaMemset(d_shifts_, 0, (size_t)nlist_ * dpad_ * 4);  // = the zero centroids of an untrained index
+  }
+}
 IVFFlatIndex::~IVFFlatIndex() {
+  if (d_shifts_) cudaFree(d_shifts_);
   if (mirror_.base) cudaFree(mirror_.base);
   if (mirror_.norms) cudaFree(mirror_.norms);
   if (mirror_.d_tile0) cudaFree(mirror_.d_tile0);
@@ -1223,6 +1231,22 @@ IVFFlatIndex::~IVFFlatIndex() {
 }
 int IvfIndex::rebuild_centroid_tiles(cudaStream_t st) {
   GB_CUDA(launch_tc_stage_rows(d_centroids_, dpad_, nlist_, dpad_, (int)round_up(dpad_, 16), d_cent_tiles_, d_cent_norms_, st));
+  return centroids_changed(st);
+}
+int IVFFlatIndex::centroids_changed(cudaStream_t st) {
+  if (!d_shifts_) return 0;  // inner product: the mirror holds the raw rows, whatever the centroids
+  GB_CUDA(launch_list_shifts(d_centroids_, dpad_, nlist_, d_, d_shifts_, st));
+  std::unique_lock<std::shared_mutex> ml(mirror_rw_);
+  mirror_.lens.clear();  // staged with the old shifts: rebuilt by the next list-major search
+  return 0;
+}
+int IVFFlatIndex::get_list_shifts(float* host) const {
+  if (!d_shifts_) {
+    set_last_error("IVFFLAT: list shifts exist only under L2");
+    return -1;
+  }
+  cudaSetDevice(device_);
+  GB_CUDA(cudaMemcpy2D(host, (size_t)d_ * 4, d_shifts_, (size_t)dpad_ * 4, (size_t)d_ * 4, nlist_, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1241,7 +1265,8 @@ int64_t IvfIndex::index_mem_bytes() const {
   return (int64_t)nlist_ * dpad_ * 4 + cent_tiles + (lists_ ? lists_->mem_bytes() : 0);
 }
 int64_t IVFFlatIndex::index_mem_bytes() const {
-  return IvfIndex::index_mem_bytes() + mirror_.cap_tiles * tc_tile_bytes(dpad_) + rowptr_cap_ * (int64_t)sizeof(float*);
+  return IvfIndex::index_mem_bytes() + (d_shifts_ ? (int64_t)nlist_ * dpad_ * 4 : 0) + mirror_.cap_tiles * tc_tile_bytes(dpad_) +
+         rowptr_cap_ * (int64_t)sizeof(float*);
 }
 int IvfIndex::set_centroids(const float* host, int nlist) {
   if (nlist != nlist_) {
@@ -1516,6 +1541,7 @@ int IvfIndex::coarse_dev(int nq, const float* xq, int nprobe, int metric, int32_
     GB_ALLOC(tau, unsigned long long, nq, s);
     GB_ALLOC(part, unsigned long long, (size_t)nq * nseg * nprobe, s);
     StageScope stage(this, "coarse_quantizer", st);
+    last_coarse_kernel_ = "coarse_topk_kernel";
     GB_CUDA(cudaMemsetAsync(tau, 0xFF, sizeof(unsigned long long) * nq, st));
     GB_CUDA(launch_tc_stage_rows(xq, dpad_, nq, dpad_, k16, a_tiles, a_norms, st));
     GB_CUDA(launch_coarse_topk(a_tiles, a_norms, nq, d_cent_tiles_, d_cent_norms_, nlist_, k16, seg_tiles, metric, nprobe, tau,
@@ -1527,6 +1553,7 @@ int IvfIndex::coarse_dev(int nq, const float* xq, int nprobe, int metric, int32_
   int64_t ldo = round_up(nlist_, 4);
   GB_ALLOC(scores, float, (size_t)nq * ldo, s);
   StageScope stage(this, "coarse_quantizer", st);
+  last_coarse_kernel_ = tc ? "dist_tc_kernel+select_rows_kernel" : "dist_tile_kernel+select_rows_kernel";
   if (tc) {
     GB_CUDA(launch_dist_matrix_tc(xq, dpad_, nq, d_centroids_, dpad_, nlist_, dpad_, metric, scores, ldo, st));
   } else {
@@ -1573,8 +1600,8 @@ int IVFFlatIndex::mirror_append(const float* x, int64_t n, const int32_t* d_list
     }
     lens[l] += add[l];
   }
-  GB_CUDA(launch_tc_mirror_append(x, dpad_, n, dpad_, (int)round_up(dpad_, 16), d_list, d_pos, mirror_.d_tile0, mirror_.base,
-                                  mirror_.norms, st));
+  GB_CUDA(launch_tc_mirror_append(x, dpad_, n, dpad_, (int)round_up(dpad_, 16), d_list, d_pos, mirror_.d_tile0,
+                                  d_shifts_, mirror_.base, mirror_.norms, st));
   mirror_.lens = lens;
   return 0;
 }
@@ -1626,8 +1653,8 @@ int IVFFlatIndex::ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStr
       if (!mirror_.disabled) {
         if (!mirror_.d_tile0 && cudaMalloc(&mirror_.d_tile0, sizeof(int64_t) * (nlist_ + 1)) != cudaSuccess) return -1;
         GB_CUDA(cudaMemcpyAsync(mirror_.d_tile0, tile0.data(), sizeof(int64_t) * (nlist_ + 1), cudaMemcpyHostToDevice, st));
-        GB_CUDA(launch_tc_mirror_build(lists_->directory(), dpad_, k16, mirror_.d_tile0, tiles, mirror_.base, mirror_.norms,
-                                       st));
+        GB_CUDA(launch_tc_mirror_build(lists_->directory(), dpad_, k16, mirror_.d_tile0, tiles,
+                                       d_shifts_, mirror_.base, mirror_.norms, st));
         GB_CUDA(cudaStreamSynchronize(st));  // tile0 is a stack vector; other streams may use the mirror next
         mirror_.tiles = tiles;
         mirror_.lens = lens;
@@ -1644,6 +1671,10 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
                                      const int32_t* probe_ids, int nprobe, unsigned long long* out_keys, Scratch& s) {
   const int64_t npairs = (int64_t)nq * nprobe;
   if (npairs < (int64_t)nlist_ * 32) return 1;  // < 32 queries per list on average
+  // the mirror is staged for the index's metric (shifted under L2), so a search under the other metric scans
+  // query-major
+  if (metric != this->metric()) return 1;
+  const float* shifts = d_shifts_;  // L2 index (the metrics agree): shifted; IP: nullptr
   cudaStream_t st = s.stream();
   ListDirectory dir = lists_->directory();
   if (k <= kLmkMaxK) {
@@ -1672,16 +1703,16 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
       TcMirrorView mv{mirror_.base, mirror_.d_tile0, mirror_.norms, k16};
       last_scan_kernel_ = "ivf_listmajor_tma_kernel";
       scan_timer_begin(st);
-      GB_CUDA(launch_lm_stage_queries(xq, dpad_, dpad_, k16, g.items, (int)max_items, g.totals, g.pair_j, nprobe, a_scratch,
-                                      a_norms, st));
+      GB_CUDA(launch_lm_stage_queries(xq, dpad_, dpad_, k16, g.items, (int)max_items, g.totals, g.pair_j, nprobe, shifts,
+                                      a_scratch, a_norms, st));
       GB_CUDA(launch_ivf_listmajor_tma(a_scratch, a_norms, mv, g.items, (int)max_items, g.totals, g.pair_j, nprobe, dir, k,
                                        nseg, metric, f, d_tau, d_out, st));
       scan_timer_end(st);
     } else {
       last_scan_kernel_ = "ivf_listmajor_pipe_kernel";
       scan_timer_begin(st);
-      GB_CUDA(launch_ivf_listmajor_pipe(xq, dpad_, dpad_, g.items, (int)max_items, g.totals, g.pair_j, nprobe, dir, k, nseg,
-                                        metric, f, d_tau, d_out, st));
+      GB_CUDA(launch_ivf_listmajor_pipe(xq, dpad_, dpad_, g.items, (int)max_items, g.totals, g.pair_j, nprobe, dir, shifts, k,
+                                        nseg, metric, f, d_tau, d_out, st));
       scan_timer_end(st);
     }
     if (mlk.owns_lock()) mlk.unlock();
@@ -1711,7 +1742,8 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
                                  d_pair_q, d_pair_off, d_seg_off, d_tiles, st));
   last_scan_kernel_ = "ivf_listmajor_tc_kernel+seg_select_kernel";
   scan_timer_begin(st);
-  GB_CUDA(launch_ivf_listmajor_tc(xq, dpad_, dpad_, d_tiles, (int)ntiles, d_pair_q, d_pair_off, dir, metric, scores, st));
+  GB_CUDA(launch_ivf_listmajor_tc(xq, dpad_, dpad_, d_tiles, (int)ntiles, d_pair_q, d_pair_off, dir, shifts, metric, scores,
+                                  st));
   GB_CUDA(launch_seg_select(scores, d_seg_off, probe_ids, nq, nprobe, dir, k, metric, f, out_keys, st));
   scan_timer_end(st);
   return 0;
@@ -1724,10 +1756,13 @@ int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int me
   (void)xq_raw;  // no transform: xq is the raw queries
   (void)coarse_dis;
   cudaStream_t st = s.stream();
-  // The list-major scan selects on 3xTF32 tensor-core scores (|x|^2 + |y|^2 - 2 x.y for L2: on SIFT-like float data,
-  // |x|^2 ~ 40 d^2, the cancellation leaves ~1e-4 relative).  Its k winners are re-scored with the direct fp32 form
-  // from the raw vectors and re-sorted (rerank_kernel, k rows per query), so every distance that leaves the index is
-  // the exact-kernel value; on integer-valued data both forms are exact and nothing changes.
+  // The list-major scan selects on 3xTF32 tensor-core scores.  Under L2 it evaluates |x - s|^2 + |y - s|^2 -
+  // 2 (x - s).(y - s) with s = s_l, the shift of the probed list (d_shifts_, near its centroid), so the cancellation
+  // error scales with the residual norms: on raw vectors with a common offset (|x|^2 ~ 1e8 at offset 1000, d = 128) the
+  // rounding of |x|^2 + |y|^2 alone would exceed the gaps between neighbours.  The k winners are re-scored with the
+  // direct fp32 form from the raw vectors and re-sorted (rerank_kernel, k rows per query), so every distance that
+  // leaves the index is the exact-kernel value; on integer-valued data with integer shifts both forms are exact and
+  // nothing changes.
   GB_ALLOC(lm_keys, unsigned long long, (size_t)nq * k, s);
   int lm = scan_listmajor_dev(f, metric, nq, xq, k, probe_ids, nprobe, lm_keys, s);
   if (lm < 0) return lm;

@@ -400,6 +400,7 @@ class IvfIndex : public Index {
   // parity hooks: exchange index state with the oracle
   int set_centroids(const float* host, int nlist);  // marks trained
   int get_centroids(float* host) const;
+  const char* last_coarse_kernel() const { return last_coarse_kernel_; }  // test hook: which coarse path ran last
   IvfLists* lists() { return lists_.get(); }
   // quantizer->search (ivfflat.cc:568): top-nprobe lists per query
   int coarse_search_host(int nq, const float* x, int nprobe, float* out_dis, int64_t* out_ids);
@@ -466,12 +467,15 @@ class IvfIndex : public Index {
   int compact_locked();  // lists_->compact + lists_changed, with mu_ held exclusively
 
   int nlist_;
+  const char* last_coarse_kernel_ = "";
   float* d_centroids_ = nullptr;  // [nlist][dpad]
   // the centroids once more as tensor-core operand tiles (launch_tc_stage_rows) for the fused coarse quantiser, and
   // |c|^2 per row; rebuilt by every change of d_centroids_ (rebuild_centroid_tiles)
   float* d_cent_tiles_ = nullptr;
   float* d_cent_norms_ = nullptr;
   int rebuild_centroid_tiles(cudaStream_t st);
+  // after every change of d_centroids_ (the end of rebuild_centroid_tiles), with mu_ held exclusively, ordered on st
+  virtual int centroids_changed(cudaStream_t st) { (void)st; return 0; }
   std::unique_ptr<IvfLists> lists_;
   std::vector<uint64_t> vid2pos_;  // vid -> (list << 32 | pos), ~0 = not in a list (vid_bucket_no_pos_)
 };
@@ -479,11 +483,12 @@ class IvfIndex : public Index {
 // GammaIVFFlatIndex (index/impl/gamma_index_ivfflat.{h,cc}): the lists hold the raw fp32 rows
 class IVFFlatIndex : public IvfIndex {
  public:
-  IVFFlatIndex(int d, const ModelParams& mp, int device, int seg_shift) : IvfIndex("IVFFLAT", d, mp, device, seg_shift) {}
+  IVFFlatIndex(int d, const ModelParams& mp, int device, int seg_shift);
   ~IVFFlatIndex() override;
   int64_t index_mem_bytes() const override;
   int code_bytes() const override { return dpad_ * 4; }
   int mirror_builds() const { return mirror_.builds; }  // test hook
+  int get_list_shifts(float* host) const;               // test hook: d_shifts_ as [nlist][d] (L2 indexes only)
 
  protected:
   GammaFileFormat gamma_format() const override;
@@ -498,6 +503,10 @@ class IVFFlatIndex : public IvfIndex {
                    const std::vector<int>& add, Scratch& s) override;
   void reset_codec() override;
   int lists_changed(cudaStream_t st) override;
+  int centroids_changed(cudaStream_t st) override;  // new list shifts; the mirror goes stale
+  // The list shifts s_l [nlist][dpad] of the list-major scan of an L2 index (nullptr under IP) (launch_list_shifts): its tensor-core operands are
+  // x - s_l and y - s_l, so the rounding of the expanded form scales with the residual norms, not the raw ones.
+  float* d_shifts_ = nullptr;
   // host placement: rowptr[vid] = the list row holding vid, for the winner re-score (lists_changed)
   const float** d_rowptr_ = nullptr;
   int64_t rowptr_cap_ = 0;

@@ -364,6 +364,14 @@ int gb_index_mirror_builds(gb_index* index) {
   IVFFlatIndex* ivf = as<IVFFlatIndex>(index);
   return ivf ? ivf->mirror_builds() : 0;
 }
+int gb_index_get_list_shifts(gb_index* index, float* out) {
+  AS_OR_FAIL(IVFFlatIndex, ivf, index, "IVFFLAT");
+  return ivf->get_list_shifts(out);
+}
+const char* gb_index_last_coarse_kernel(gb_index* index) {
+  IvfIndex* ivf = as<IvfIndex>(index);
+  return ivf ? ivf->last_coarse_kernel() : "";
+}
 int gb_index_compact(gb_index* index) {
   IDX_OR_FAIL(index);
   IvfIndex* ivf = as<IvfIndex>(index);

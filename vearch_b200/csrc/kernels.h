@@ -85,10 +85,15 @@ struct LmTile {
   int list, pair0, npairs, row0, nrows, seg;
   int grp;  // ordinal of this (list, pair group): its slot in the staged-query scratch
 };
+// List shifts (L2 only): every list-major operand is staged as x - s_l, s_l the row of its list in shifts [nlist][ldq]
+// (the pair's list for queries), so the expanded form |x - s|^2 + |y - s|^2 - 2 (x - s).(y - s) works on residual-sized
+// norms; nullptr = unshifted.  launch_list_shifts writes s_l = round(c_l / g_l) * g_l, g_l the largest power of two
+// <= rho_l / sqrt(d), rho_l half the distance from c_l to its nearest other centroid (s_l = c_l when rho_l = 0).
+cudaError_t launch_list_shifts(const float* cent, int64_t ldc, int nlist, int d, float* shifts, cudaStream_t st);
 // scores[pair_off[j] + r] = score(query pair_q[j], row r of its list)
 cudaError_t launch_ivf_listmajor_tc(const float* xq, int64_t ldq, int d, const LmTile* tiles, int ntiles,
-                                    const int32_t* pair_q, const int64_t* pair_off, ListDirectory dir, int metric,
-                                    float* scores, cudaStream_t st);
+                                    const int32_t* pair_q, const int64_t* pair_off, ListDirectory dir,
+                                    const float* shifts, int metric, float* scores, cudaStream_t st);
 // device-side grouping of the (query, probe) pairs by list: histogram + scans (totals[0..2] = score
 // floats, tiles, valid pairs), then slot assignment and the tile table
 cudaError_t launch_lm_count_scan(const int32_t* probe_ids, int64_t npairs, ListDirectory dir, int32_t* cnt,
@@ -126,22 +131,23 @@ struct TcMirrorView {
 inline int64_t tc_mirror_tile_floats(int k16) { return (int64_t)128 * k16 * 2; }
 // rows just appended to the lists (row i of x -> position pos[i] of list list[i], list < 0: skipped)
 cudaError_t launch_tc_mirror_append(const float* x, int64_t ldx, int64_t n, int d, int k16, const int32_t* list,
-                                    const int32_t* pos, const int64_t* tile0, float* mirror, float* norms, cudaStream_t st);
+                                    const int32_t* pos, const int64_t* tile0, const float* shifts, float* mirror,
+                                    float* norms, cudaStream_t st);
 cudaError_t launch_tc_mirror_build(ListDirectory dir, int d, int k16, const int64_t* tile0, int64_t total_tiles,
-                                   float* mirror, float* norms, cudaStream_t st);
+                                   const float* shifts, float* mirror, float* norms, cudaStream_t st);
 // a_scratch: per pair group nk chunks of 16 KiB (hi, lo) of the group's 128 queries; a_norms: [group][128]
 cudaError_t launch_lm_stage_queries(const float* xq, int64_t ldq, int d, int k16, const LmTile* items, int max_items,
-                                    const int64_t* totals, const int64_t* pair_j, int nprobe, float* a_scratch,
-                                    float* a_norms, cudaStream_t st);
+                                    const int64_t* totals, const int64_t* pair_j, int nprobe, const float* shifts,
+                                    float* a_scratch, float* a_norms, cudaStream_t st);
 cudaError_t launch_ivf_listmajor_tma(const float* a_scratch, const float* a_norms, TcMirrorView mv, const LmTile* items,
                                      int max_items, const int64_t* totals, const int64_t* pair_j, int nprobe,
                                      ListDirectory dir, int k, int nseg_max, int metric, FilterArgs f,
                                      unsigned long long* tau_g, unsigned long long* out, cudaStream_t st);
 // register-staged variant: reads the lists themselves (no mirror), any d
 cudaError_t launch_ivf_listmajor_pipe(const float* xq, int64_t ldq, int d, const LmTile* items, int max_items,
-                                      const int64_t* totals, const int64_t* pair_j, int nprobe, ListDirectory dir, int k,
-                                      int nseg_max, int metric, FilterArgs f, unsigned long long* tau_g,
-                                      unsigned long long* out, cudaStream_t st);
+                                      const int64_t* totals, const int64_t* pair_j, int nprobe, ListDirectory dir,
+                                      const float* shifts, int k, int nseg_max, int metric, FilterArgs f,
+                                      unsigned long long* tau_g, unsigned long long* out, cudaStream_t st);
 
 // ---- OPQ training helpers (kernels_build.cu) ---------------------------------------------------
 // out[i][j] = x[i][j] - mean_j (columns >= d zeroed up to ldo); mean computed on device

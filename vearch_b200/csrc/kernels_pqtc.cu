@@ -236,8 +236,11 @@ __global__ void __launch_bounds__(PT_G)
     const unsigned long long bk = bound_keys[(int64_t)pm.q * bound_stride + kprime - 1];
     const float R2 = rmax2[0], R = sqrtf(R2);
     pm.c = sa * rmax2[1];
-    if (bk == kKeySentinel) {
-      // phase A found fewer than k' entries: no bound -> the exact kernel redoes this query
+    // eps below has relative terms only.  Near fp32's subnormal range (|a|^2 or the codebook's largest |r|^2 below
+    // 2^-96) the roundings of the exact table evaluation are absolute (2^-149 each) and can exceed it: no filter there
+    const bool tiny = (amax > 0.f && na2 < 0x1p-96f) || (R2 > 0.f && R2 < 0x1p-96f);
+    if (bk == kKeySentinel || tiny) {
+      // phase A found fewer than k' entries (no bound), or the bound would not hold -> the exact kernel redoes this query
       atomicMax(cand_cnt + pm.q, cap + 1);
     } else {
       const float B = ord2score((uint32_t)(bk >> 32), METRIC);

@@ -21,7 +21,8 @@
 // "3xTF32", relative error ~2^-21).  Integer-valued operands below 2^11 have lo == 0 and every
 // product and partial sum is exact, so on the SIFT-shaped parity data scores are bit-equal to the
 // exact fp32 kernels.  L2 uses |x|^2 + |y|^2 - 2 x.y with both norms accumulated in-kernel from the
-// staged operands (faiss clamps the expanded form at 0; so do we).
+// staged operands (faiss clamps the expanded form at 0; so do we).  The K3 kernels stage x - s_l and y - s_l
+// under L2, s_l the shift of the probed list (launch_list_shifts), so that rounding scales with the residuals.
 //
 // Operand layout: canonical no-swizzle K-major tiles (8-row x 16-byte core matrices; LBO = stride
 // between the two K core matrices of one MMA, SBO = stride between 8-row groups).  One warpgroup
@@ -47,6 +48,8 @@ constexpr int TC_STAGE_BYTES = 4 * TC_TILE_BYTES;        // a_hi, a_lo, b_hi, b_
 constexpr int TC_SMEM = TC_STAGES * TC_STAGE_BYTES;      // 64 KiB
 static_assert(kSlabBytes <= TC_SMEM / 2, "the accumulator slabs reuse the first operand stage");
 static_assert(TC_M * 16 == 2048, "lt_desc assumes LBO = 2048");
+
+__device__ __forceinline__ float4 f4_sub(float4 a, float4 b) { return make_float4(a.x - b.x, a.y - b.y, a.z - b.z, a.w - b.w); }
 
 // The 3xTF32 MMAs of one K = 16 chunk whose four 128 x 16 tiles sit at a_hi, a_lo, b_hi, b_lo.
 // Issued by every thread of warpgroup 0; the caller fences before and commits after.
@@ -79,8 +82,11 @@ struct TcShared {
   alignas(16) float cn[TC_N];  // |y|^2 of the tile's rows (aligned: the epilogues' reads vectorise)
 };
 
+// shift: nullptr, or a row subtracted from both operands' rows before the split (the list shift of K3; see
+// tc_split_row)
 __device__ __forceinline__ void tc_tile_run(unsigned char* smem, TcShared* sh, const float* __restrict__ arow,
-                                            const float* __restrict__ brow, int d, float (&acc)[2][64], float* an) {
+                                            const float* __restrict__ brow, const float* __restrict__ shift, int d,
+                                            float (&acc)[2][64], float* an) {
   const int tid = threadIdx.x;
   // canonical layout: element (r, k) of a 128 x 16 tile lives at (k/4)*(128*16) + (r/8)*128 + (r%8)*16 + (k%4)*4
   const uint32_t LBO = TC_M * 16, SBO = 128;
@@ -98,6 +104,11 @@ __device__ __forceinline__ void tc_tile_run(unsigned char* smem, TcShared* sh, c
       pb[kb] = pa[kb];
       if (arow && gk < d) pa[kb] = __ldg(reinterpret_cast<const float4*>(arow + gk));
       if (brow && gk < d) pb[kb] = __ldg(reinterpret_cast<const float4*>(brow + gk));
+      if (shift && gk < d) {
+        const float4 s4 = __ldg(reinterpret_cast<const float4*>(shift + gk));
+        if (arow) pa[kb] = f4_sub(pa[kb], s4);
+        if (brow) pb[kb] = f4_sub(pb[kb], s4);
+      }
     }
   };
   auto chunk = [&](int kc, float4 (&pa)[NV], float4 (&pb)[NV]) {
@@ -169,7 +180,7 @@ __global__ void __launch_bounds__(TC_NT)
   const float* brow = col0 + tid < m ? C + (int64_t)(col0 + tid) * ldc : nullptr;
   float acc[2][64];
   float xn;
-  tc_tile_run(smem, &sh, arow, brow, d, acc, &xn);
+  tc_tile_run(smem, &sh, arow, brow, nullptr, d, acc, &xn);
   float* slabs = reinterpret_cast<float*>(smem);
 
   const int gr = row0 + tid;
@@ -200,7 +211,7 @@ template <int METRIC>
 __global__ void __launch_bounds__(TC_NT)
     ivf_listmajor_tc_kernel(const float* __restrict__ xq, int64_t ldq, int d, const LmTile* __restrict__ tiles,
                             const int32_t* __restrict__ pair_q, const int64_t* __restrict__ pair_off,
-                            ListDirectory dir, float* __restrict__ scores) {
+                            ListDirectory dir, const float* __restrict__ shifts, float* __restrict__ scores) {
   extern __shared__ __align__(1024) unsigned char smem[];
   __shared__ TcShared sh;
   const int tid = threadIdx.x;
@@ -214,7 +225,7 @@ __global__ void __launch_bounds__(TC_NT)
   const float* brow = tid < t.nrows ? dir.vecs[t.list] + (int64_t)(t.row0 + tid) * d : nullptr;
   float acc[2][64];
   float xn;
-  tc_tile_run(smem, &sh, arow, brow, d, acc, &xn);
+  tc_tile_run(smem, &sh, arow, brow, shifts ? shifts + (int64_t)t.list * ldq : nullptr, d, acc, &xn);
   float* slabs = reinterpret_cast<float*>(smem);
   // Epilogue.  Thread t owns accumulator row t, but its row lands in a score segment far away from
   // its neighbours' rows, so writing straight from registers would touch 32 different cache lines
@@ -398,8 +409,8 @@ template <int METRIC>
 __global__ void __launch_bounds__(LW_NT, 1)
     ivf_listmajor_pipe_kernel(const float* __restrict__ xq, int64_t ldq, int d, const LmTile* __restrict__ items,
                               const int64_t* __restrict__ totals, const int64_t* __restrict__ pair_j, int nprobe,
-                              ListDirectory dir, int k, int nseg_max, FilterArgs f, unsigned long long* tau_g,
-                              unsigned long long* __restrict__ out) {
+                              ListDirectory dir, const float* __restrict__ shifts, int k, int nseg_max, FilterArgs f,
+                              unsigned long long* tau_g, unsigned long long* __restrict__ out) {
   extern __shared__ __align__(1024) unsigned char smem[];  // [ring][slabs][key sets: k * 1 KiB]
   __shared__ LwShared sh;
   if ((int64_t)blockIdx.x >= totals[1]) return;
@@ -455,6 +466,7 @@ __global__ void __launch_bounds__(LW_NT, 1)
     const float* arow = nullptr;
     if (p < t.npairs) arow = xq + (pair_j[t.pair0 + p] / nprobe) * ldq;
     const float* lvecs = dir.vecs[t.list];
+    const float* shift = shifts ? shifts + (int64_t)t.list * ldq : nullptr;
     const int64_t* __restrict__ lids = dir.ids[t.list];
     const uint32_t row_off = (uint32_t)(p >> 3) * SBO + (uint32_t)(p & 7) * 16;
     constexpr int NV = TC_BK / 4;
@@ -473,6 +485,11 @@ __global__ void __launch_bounds__(LW_NT, 1)
         pb[kb] = pa[kb];
         if (arow && gk < d) pa[kb] = __ldg(reinterpret_cast<const float4*>(arow + gk));
         if (brow && gk < d) pb[kb] = __ldg(reinterpret_cast<const float4*>(brow + gk));
+        if (shift && gk < d) {
+          const float4 s4 = __ldg(reinterpret_cast<const float4*>(shift + gk));
+          if (arow) pa[kb] = f4_sub(pa[kb], s4);
+          if (brow) pb[kb] = f4_sub(pb[kb], s4);
+        }
       }
     };
     auto chunk = [&](int n, float4 (&pa)[NV], float4 (&pb)[NV]) {
@@ -650,8 +667,10 @@ __global__ void __launch_bounds__(LT_NT, 1)
 
 
 // one operand row -> its 16-byte units of every K chunk, TF32 head and fp32 remainder, canonical
-// K-major layout; returns |row|^2 accumulated in index order (the order the staging loops use)
-__device__ __forceinline__ float tc_split_row(const float* __restrict__ src, int d, int k16, int r, float* tile) {
+// K-major layout; returns |row|^2 accumulated in index order (the order the staging loops use).
+// shift: nullptr, or a row subtracted first (the K3 list shift: src - s_l; a missing row stays zero)
+__device__ __forceinline__ float tc_split_row(const float* __restrict__ src, const float* __restrict__ shift, int d, int k16,
+                                              int r, float* tile) {
   float nrm = 0.f;
   for (int kc = 0; kc < k16 / TC_BK; kc++) {
     float* hi = tile + (int64_t)kc * (TC_STAGE_BYTES / 8);  // 16 KiB per chunk = 4096 floats: hi then lo
@@ -661,6 +680,7 @@ __device__ __forceinline__ float tc_split_row(const float* __restrict__ src, int
       const int gk = kc * TC_BK + k4 * 4;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (src && gk < d) v = __ldg(reinterpret_cast<const float4*>(src + gk));
+      if (src && shift && gk < d) v = f4_sub(v, __ldg(reinterpret_cast<const float4*>(shift + gk)));
       nrm = fmaf(v.x, v.x, nrm), nrm = fmaf(v.y, v.y, nrm), nrm = fmaf(v.z, v.z, nrm), nrm = fmaf(v.w, v.w, nrm);
       float4 h, l;
       h.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u), l.x = v.x - h.x;
@@ -676,8 +696,8 @@ __device__ __forceinline__ float tc_split_row(const float* __restrict__ src, int
 }
 
 __global__ void __launch_bounds__(TC_N)
-    tc_mirror_build_kernel(ListDirectory dir, int d, int k16, const int64_t* __restrict__ tile0, float* __restrict__ mirror,
-                           float* __restrict__ norms) {
+    tc_mirror_build_kernel(ListDirectory dir, int d, int k16, const int64_t* __restrict__ tile0,
+                           const float* __restrict__ shifts, float* __restrict__ mirror, float* __restrict__ norms) {
   const int64_t gt = blockIdx.x;
   int lo = 0, hi = dir.nlist;  // last list whose first tile is <= gt
   while (hi - lo > 1) {
@@ -687,20 +707,62 @@ __global__ void __launch_bounds__(TC_N)
   const int l = lo, r = threadIdx.x;
   const int row = (int)(gt - tile0[l]) * TC_N + r;
   const float* src = row < dir.len[l] ? dir.vecs[l] + (int64_t)row * d : nullptr;
-  norms[gt * TC_N + r] = tc_split_row(src, d, k16, r, mirror + gt * ((int64_t)TC_N * k16 * 2));
+  norms[gt * TC_N + r] = tc_split_row(src, shifts ? shifts + (int64_t)l * d : nullptr, d, k16, r,
+                                      mirror + gt * ((int64_t)TC_N * k16 * 2));
+}
+
+// The K3 list shifts (one block per list l): rho = half the distance from c_l to its nearest other centroid (fp64,
+// direct form), g = the largest power of two <= rho / sqrt(d), s_l = round(c_l / g) * g; s_l = c_l when rho = 0.
+// The grid keeps integer data integer: an integer centroid, or any g >= 1, gives an integer shift.
+__global__ void __launch_bounds__(256)
+    list_shift_kernel(const float* __restrict__ cent, int64_t ldc, int nlist, int d, float* __restrict__ shifts) {
+  __shared__ double red[8];
+  const int l = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const float* cl = cent + (int64_t)l * ldc;
+  double best = INFINITY;
+  for (int j = warp; j < nlist; j += 8) {
+    if (j == l) continue;
+    const float* cj = cent + (int64_t)j * ldc;
+    double acc = 0.0;
+    for (int c = lane; c < d; c += 32) {
+      const double t = (double)cl[c] - (double)cj[c];
+      acc = fma(t, t, acc);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    best = fmin(best, acc);
+  }
+  if (lane == 0) red[warp] = best;
+  __syncthreads();
+  double r2 = red[0];  // squared distance to the nearest other centroid (inf if nlist == 1)
+  for (int w = 1; w < 8; w++) r2 = fmin(r2, red[w]);
+  const double t = r2 / 4.0 / (double)d;  // (rho / sqrt(d))^2
+  const bool exact = !(t > 0.0) || isinf(t);
+  double g = 0.0;
+  if (!exact) {
+    int e;
+    frexp(t, &e);  // t in [2^(e-1), 2^e): g^2 <= t for g = 2^p iff 2p <= e - 1
+    const int E = e - 1;
+    g = ldexp(1.0, E >= 0 ? E / 2 : -((1 - E) / 2));
+  }
+  for (int c = tid; c < ldc; c += blockDim.x) {
+    const float v = cl[c];
+    shifts[(int64_t)l * ldc + c] = exact ? v : (float)(rint((double)v / g) * g);
+  }
 }
 
 __global__ void tc_mirror_append_kernel(const float* __restrict__ x, int64_t ldx, int64_t n, int d, int k16,
                                         const int32_t* __restrict__ list, const int32_t* __restrict__ pos,
-                                        const int64_t* __restrict__ tile0, float* __restrict__ mirror,
-                                        float* __restrict__ norms) {
+                                        const int64_t* __restrict__ tile0, const float* __restrict__ shifts,
+                                        float* __restrict__ mirror, float* __restrict__ norms) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int l = list[i];
   if (l < 0) return;
   const int p = pos[i];
   const int64_t gt = tile0[l] + p / TC_N;
-  norms[gt * TC_N + p % TC_N] = tc_split_row(x + i * ldx, d, k16, p % TC_N, mirror + gt * ((int64_t)TC_N * k16 * 2));
+  norms[gt * TC_N + p % TC_N] = tc_split_row(x + i * ldx, shifts ? shifts + (int64_t)l * d : nullptr, d, k16, p % TC_N,
+                                             mirror + gt * ((int64_t)TC_N * k16 * 2));
 }
 
 // Stages 128-row operand tiles (canonical layout, hi + lo per K chunk) and their row norms.  With items: tile = pair
@@ -709,20 +771,22 @@ __global__ void tc_mirror_append_kernel(const float* __restrict__ x, int64_t ldx
 __global__ void __launch_bounds__(TC_M)
     lm_stage_queries_kernel(const float* __restrict__ xq, int64_t ldq, int d, int k16, const LmTile* __restrict__ items,
                             const int64_t* __restrict__ totals, const int64_t* __restrict__ pair_j, int nprobe, int64_t nrows,
-                            float* __restrict__ a_scratch, float* __restrict__ a_norms) {
+                            const float* __restrict__ shifts, float* __restrict__ a_scratch, float* __restrict__ a_norms) {
   const int r = threadIdx.x;
   int64_t grp = blockIdx.x;
   const float* src = nullptr;
+  const float* shift = nullptr;
   if (items) {
     if ((int64_t)blockIdx.x >= totals[1]) return;
     const LmTile t = items[blockIdx.x];
     if (t.seg != 0) return;  // one staging per pair group: the first item of the group owns the slot
     grp = t.grp;
     if (r < t.npairs) src = xq + (pair_j[t.pair0 + r] / nprobe) * ldq;
+    if (shifts) shift = shifts + (int64_t)t.list * ldq;
   } else if (grp * TC_M + r < nrows) {
     src = xq + (grp * TC_M + r) * ldq;
   }
-  a_norms[grp * TC_M + r] = tc_split_row(src, d, k16, r, a_scratch + grp * ((int64_t)TC_M * k16 * 2));
+  a_norms[grp * TC_M + r] = tc_split_row(src, shift, d, k16, r, a_scratch + grp * ((int64_t)TC_M * k16 * 2));
 }
 
 // ---- K2 fused: the coarse quantiser's top-nprobe on the tensor cores ----------------------------
@@ -1109,19 +1173,21 @@ cudaError_t launch_dist_argmin_tc(const float* X, int64_t ldx, int n, const floa
 }
 
 cudaError_t launch_ivf_listmajor_tc(const float* xq, int64_t ldq, int d, const LmTile* tiles, int ntiles,
-                                    const int32_t* pair_q, const int64_t* pair_off, ListDirectory dir, int metric,
-                                    float* scores, cudaStream_t st) {
+                                    const int32_t* pair_q, const int64_t* pair_off, ListDirectory dir,
+                                    const float* shifts, int metric, float* scores, cudaStream_t st) {
   if ((d & 3) || (ldq & 3)) return cudaErrorInvalidValue;
   if (ntiles <= 0) return cudaSuccess;
   cudaError_t e;
   if (metric == kMetricL2) {
     e = cudaFuncSetAttribute(ivf_listmajor_tc_kernel<kMetricL2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM);
     if (e != cudaSuccess) return e;
-    ivf_listmajor_tc_kernel<kMetricL2><<<ntiles, TC_NT, TC_SMEM, st>>>(xq, ldq, d, tiles, pair_q, pair_off, dir, scores);
+    ivf_listmajor_tc_kernel<kMetricL2><<<ntiles, TC_NT, TC_SMEM, st>>>(xq, ldq, d, tiles, pair_q, pair_off, dir, shifts,
+                                                                      scores);
   } else {
     e = cudaFuncSetAttribute(ivf_listmajor_tc_kernel<kMetricIP>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM);
     if (e != cudaSuccess) return e;
-    ivf_listmajor_tc_kernel<kMetricIP><<<ntiles, TC_NT, TC_SMEM, st>>>(xq, ldq, d, tiles, pair_q, pair_off, dir, scores);
+    ivf_listmajor_tc_kernel<kMetricIP><<<ntiles, TC_NT, TC_SMEM, st>>>(xq, ldq, d, tiles, pair_q, pair_off, dir, shifts,
+                                                                      scores);
   }
   note_launch();
   return cudaGetLastError();
@@ -1175,28 +1241,39 @@ cudaError_t launch_lmk_group(const int32_t* probe_ids, int64_t npairs, ListDirec
   return cudaGetLastError();
 }
 
+cudaError_t launch_list_shifts(const float* cent, int64_t ldc, int nlist, int d, float* shifts, cudaStream_t st) {
+  if (nlist <= 0) return cudaSuccess;
+  if (d <= 0 || ldc < d) return cudaErrorInvalidValue;
+  list_shift_kernel<<<nlist, 256, 0, st>>>(cent, ldc, nlist, d, shifts);
+  note_launch();
+  return cudaGetLastError();
+}
+
 cudaError_t launch_tc_mirror_build(ListDirectory dir, int d, int k16, const int64_t* tile0, int64_t total_tiles,
-                                   float* mirror, float* norms, cudaStream_t st) {
+                                   const float* shifts, float* mirror, float* norms, cudaStream_t st) {
   if (total_tiles <= 0) return cudaSuccess;
   if (total_tiles > INT32_MAX || (d & 3) || (k16 % TC_BK)) return cudaErrorInvalidValue;
-  tc_mirror_build_kernel<<<(unsigned)total_tiles, TC_N, 0, st>>>(dir, d, k16, tile0, mirror, norms);
+  tc_mirror_build_kernel<<<(unsigned)total_tiles, TC_N, 0, st>>>(dir, d, k16, tile0, shifts, mirror, norms);
   note_launch();
   return cudaGetLastError();
 }
 
 cudaError_t launch_tc_mirror_append(const float* x, int64_t ldx, int64_t n, int d, int k16, const int32_t* list,
-                                    const int32_t* pos, const int64_t* tile0, float* mirror, float* norms, cudaStream_t st) {
+                                    const int32_t* pos, const int64_t* tile0, const float* shifts, float* mirror,
+                                    float* norms, cudaStream_t st) {
   if (n <= 0) return cudaSuccess;
-  tc_mirror_append_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(x, ldx, n, d, k16, list, pos, tile0, mirror, norms);
+  tc_mirror_append_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(x, ldx, n, d, k16, list, pos, tile0, shifts, mirror,
+                                                                       norms);
   note_launch();
   return cudaGetLastError();
 }
 
 cudaError_t launch_lm_stage_queries(const float* xq, int64_t ldq, int d, int k16, const LmTile* items, int max_items,
-                                    const int64_t* totals, const int64_t* pair_j, int nprobe, float* a_scratch,
-                                    float* a_norms, cudaStream_t st) {
+                                    const int64_t* totals, const int64_t* pair_j, int nprobe, const float* shifts,
+                                    float* a_scratch, float* a_norms, cudaStream_t st) {
   if (max_items <= 0) return cudaSuccess;
-  lm_stage_queries_kernel<<<max_items, TC_M, 0, st>>>(xq, ldq, d, k16, items, totals, pair_j, nprobe, 0, a_scratch, a_norms);
+  lm_stage_queries_kernel<<<max_items, TC_M, 0, st>>>(xq, ldq, d, k16, items, totals, pair_j, nprobe, 0, shifts, a_scratch,
+                                                      a_norms);
   note_launch();
   return cudaGetLastError();
 }
@@ -1206,7 +1283,7 @@ cudaError_t launch_tc_stage_rows(const float* x, int64_t ldx, int64_t n, int d, 
   if (n <= 0) return cudaSuccess;
   if ((d & 3) || (ldx & 3) || (k16 % TC_BK) || k16 < d) return cudaErrorInvalidValue;
   lm_stage_queries_kernel<<<(unsigned)((n + TC_M - 1) / TC_M), TC_M, 0, st>>>(x, ldx, d, k16, nullptr, nullptr, nullptr, 1, n,
-                                                                              tiles, norms);
+                                                                              nullptr, tiles, norms);
   note_launch();
   return cudaGetLastError();
 }
@@ -1267,9 +1344,9 @@ cudaError_t launch_ivf_listmajor_tma(const float* a_scratch, const float* a_norm
 }
 
 cudaError_t launch_ivf_listmajor_pipe(const float* xq, int64_t ldq, int d, const LmTile* items, int max_items,
-                                      const int64_t* totals, const int64_t* pair_j, int nprobe, ListDirectory dir, int k,
-                                      int nseg_max, int metric, FilterArgs f, unsigned long long* tau_g,
-                                      unsigned long long* out, cudaStream_t st) {
+                                      const int64_t* totals, const int64_t* pair_j, int nprobe, ListDirectory dir,
+                                      const float* shifts, int k, int nseg_max, int metric, FilterArgs f,
+                                      unsigned long long* tau_g, unsigned long long* out, cudaStream_t st) {
   if ((d & 3) || (ldq & 3) || k <= 0 || k > kLmkMaxK) return cudaErrorInvalidValue;
   if (max_items <= 0) return cudaSuccess;
   const size_t smem = (size_t)LW_RING + kSlabBytes + (size_t)k * TC_NT * 8;
@@ -1277,13 +1354,13 @@ cudaError_t launch_ivf_listmajor_pipe(const float* xq, int64_t ldq, int d, const
   if (metric == kMetricL2) {
     e = cudaFuncSetAttribute(ivf_listmajor_pipe_kernel<kMetricL2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    ivf_listmajor_pipe_kernel<kMetricL2><<<max_items, LW_NT, smem, st>>>(xq, ldq, d, items, totals, pair_j, nprobe, dir, k,
-                                                                        nseg_max, f, tau_g, out);
+    ivf_listmajor_pipe_kernel<kMetricL2><<<max_items, LW_NT, smem, st>>>(xq, ldq, d, items, totals, pair_j, nprobe, dir,
+                                                                        shifts, k, nseg_max, f, tau_g, out);
   } else {
     e = cudaFuncSetAttribute(ivf_listmajor_pipe_kernel<kMetricIP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    ivf_listmajor_pipe_kernel<kMetricIP><<<max_items, LW_NT, smem, st>>>(xq, ldq, d, items, totals, pair_j, nprobe, dir, k,
-                                                                        nseg_max, f, tau_g, out);
+    ivf_listmajor_pipe_kernel<kMetricIP><<<max_items, LW_NT, smem, st>>>(xq, ldq, d, items, totals, pair_j, nprobe, dir,
+                                                                        shifts, k, nseg_max, f, tau_g, out);
   }
   note_launch();
   return cudaGetLastError();

@@ -296,6 +296,16 @@ class GammaIndex:
     def mirror_builds(self):
         return int(_lib.lib().gb_index_mirror_builds(self._h))
 
+    @property
+    def last_coarse_kernel(self):
+        return _lib.lib().gb_index_last_coarse_kernel(self._h).decode()
+
+    def get_list_shifts(self):
+        """IVFFLAT under L2: the per-list shifts s_l (nlist x d) the list-major scan subtracts from both operands."""
+        out = np.empty((self.nlist, self.d), np.float32)
+        _check(_lib.lib().gb_index_get_list_shifts(self._h, _ptr(out)), "get_list_shifts")
+        return out
+
     def compact(self):
         _check(_lib.lib().gb_index_compact(self._h), "compact")
 
