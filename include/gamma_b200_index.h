@@ -135,10 +135,10 @@ int gb_index_get_list_shifts(gb_index *index, float *out);
  * "dist_tc_kernel+select_rows_kernel" (>= 32 queries) or "dist_tile_kernel+select_rows_kernel" (exact) */
 const char *gb_index_last_coarse_kernel(gb_index *index);
 int gb_index_load(gb_index *index, const char *dir, const char *abs_name, int64_t *load_num);
-/* quantizer->search (gamma_index_ivfflat.cc:568) */
+/* quantizer->search (gamma_index_ivfflat.cc:568); refuses an untrained index and nprobe outside [1, min(nlist, 4096)] */
 int gb_index_coarse_search(gb_index *index, int nq, const float *x, int nprobe, float *out_dis, int64_t *out_ids);
 /* search_preassigned (gamma_index_ivfflat.cc:579, gamma_index_ivfpq.cc:730) with caller-given
- * probe lists and coarse distances */
+ * probe lists and coarse distances; refuses an untrained index, topK or nprobe outside [1, 4096] */
 int gb_index_search_preassigned(gb_index *index, int nq, const float *x, int k, const int64_t *keys,
                                 const float *coarse_dis, int nprobe, const char *retrieval_params_json,
                                 const uint8_t *del_bitmap, const uint8_t *filter_bitmap, int64_t bitmap_bits,

@@ -213,6 +213,68 @@ def test_parameters_and_refusals():
     assert np.array_equal(a[0], b[0])
 
 
+def searched_index(n=20000, cs=16, nlist=64, seed=41):
+    db = synth.binary_clustered(n, cs * 8, seed=seed, n_clusters=32, flip=0.2)
+    idx, _ = built(db, cs, nlist)
+    return idx
+
+
+def test_retrieval_metric_type_is_ignored():
+    # Hamming distances rank smaller first whatever metric_type the retrieval parameters carry
+    idx = searched_index()
+    xq = synth.binary_clustered(40, 128, seed=42, n_clusters=32, flip=0.2)
+    for kw in ({"params": {"nprobe": 8}}, {"brute_force": True}):
+        want = idx.search(xq, 20, **kw)
+        params = dict(kw.get("params", {}), metric_type="InnerProduct")
+        got = idx.search(xq, 20, **dict(kw, params=params))
+        assert np.array_equal(got[0], want[0]) and np.array_equal(got[1], want[1])
+        assert np.all(np.diff(got[0], axis=1) >= 0)
+
+
+def test_concurrent_small_searches_equal_one_batch():
+    # small searches without bitmaps from several threads are merged into shared device batches (request coalescing);
+    # each caller gets exactly its slice of the one-batch result
+    import threading
+    idx = searched_index()
+    xq = synth.binary_clustered(32, 128, seed=43, n_clusters=32, flip=0.2)
+    for kw in ({"params": {"nprobe": 8}}, {"brute_force": True}):
+        want = idx.search(xq, 10, **kw)
+        got = [None] * 8
+        start = threading.Barrier(8)
+
+        def run(t):
+            start.wait()
+            for _ in range(5):
+                got[t] = idx.search(xq[4 * t:4 * t + 4], 10, **kw)
+
+        threads = [threading.Thread(target=run, args=(t,)) for t in range(8)]
+        for th in threads:
+            th.start()
+        for th in threads:
+            th.join()
+        assert np.array_equal(np.concatenate([g[0] for g in got]), want[0])
+        assert np.array_equal(np.concatenate([g[1] for g in got]), want[1])
+
+
+def test_large_batch_equals_its_slices():
+    # an IVF search runs its queries in batches of 16384; every query's result is its own
+    idx = searched_index()
+    xq = synth.binary_clustered(20000, 128, seed=44, n_clusters=32, flip=0.2)
+    dis, ids = idx.search(xq, 10, params={"nprobe": 8})
+    for q0, q1 in ((0, 16384), (16384, 20000)):
+        d, i = idx.search(xq[q0:q1], 10, params={"nprobe": 8})
+        assert np.array_equal(dis[q0:q1], d) and np.array_equal(ids[q0:q1], i)
+
+
+def test_scan_kernel_names():
+    idx = searched_index()
+    xq = synth.binary_clustered(20, 128, seed=45, n_clusters=32, flip=0.2)
+    idx.search(xq, 10, brute_force=True)
+    assert idx.last_scan_kernel == "hamming_tile_kernel+select_rows_kernel"
+    idx.search(xq, 10, params={"nprobe": 8})
+    assert idx.last_scan_kernel == "binary_ivf_scan_kernel"
+
+
 # ---- the engine (gamma C-ABI): a BINARYIVF table end to end -----------------------------------------------------------
 def eng_mod():
     from vearch_b200 import engine

@@ -861,14 +861,7 @@ Status Engine::Search(const SearchRequestPB& req, std::string* pb_out) {
       ctx.bitmap_bits = max_docid_;
     }
   }
-  int rc;
-  if (BinaryIvfIndex* bq = dynamic_cast<BinaryIvfIndex*>(qindex)) {
-    rc = bq->search_codes(ctx, n, reinterpret_cast<const uint8_t*>(vq.value.data()), topN, dis.data(), ids.data());
-  } else {
-    std::vector<float> x((size_t)n * qdim);
-    memcpy(x.data(), vq.value.data(), x.size() * 4);
-    rc = qindex->search(ctx, n, x.data(), topN, dis.data(), ids.data());
-  }
+  const int rc = qindex->search(ctx, n, vq.value.data(), topN, dis.data(), ids.data());
   if (rc == -2 || IsKilled(req.request_id, req.partition_id)) return Status::Make(kMemoryExceeded, "");
   if (rc != 0) return Status::Make(kInvalidArgument, "faild search of query " + vq.name + ": " + last_error());
 

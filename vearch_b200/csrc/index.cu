@@ -764,46 +764,42 @@ int Index::upload_bitmaps(const SearchContext& ctx, FilterArgs* f, Scratch& s) {
   return 0;
 }
 
-int Index::search_device(const SearchContext& ctx, int nq, const float* x_dev, int64_t ldx, int k, float* out_dis_dev,
-                         int64_t* out_ids_dev, cudaStream_t st, unsigned long long* out_keys_dev) {
-  if (nq <= 0) return 0;
+const void* Index::upload_queries(int nq, const void* x, Scratch& s) {
+  const size_t rb = store_->row_bytes(), ld = store_->stride();
+  void* dq = s.alloc((size_t)nq * ld);
+  if (!dq) return nullptr;
+  cudaError_t e = rb == ld ? cudaSuccess : cudaMemsetAsync(dq, 0, (size_t)nq * ld, s.stream());
+  if (e == cudaSuccess) e = cudaMemcpy2DAsync(dq, ld, x, rb, rb, nq, cudaMemcpyHostToDevice, s.stream());
+  if (e != cudaSuccess) {
+    set_last_error(std::string("query upload: ") + cudaGetErrorString(e));
+    return nullptr;
+  }
+  return dq;
+}
+
+int Index::download_results(const unsigned long long* keys, int nq, int k, int metric, float* out_dis, int64_t* out_ids,
+                            Scratch& s) {
+  cudaStream_t st = s.stream();
+  GB_ALLOC(dd, float, (size_t)nq * k, s);
+  GB_ALLOC(di, int64_t, (size_t)nq * k, s);
+  GB_CUDA(launch_decode_keys(keys, k, nq, k, metric, dd, di, 0, st));
+  GB_CUDA(cudaMemcpyAsync(out_dis, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int Index::search_keys(const SearchContext& ctx, int nq, const void* xq, int k, unsigned long long** out_keys, Scratch& s) {
   if (k <= 0 || k > 4096) {
     set_last_error("topK must be in [1, 4096]");
     return -1;
   }
-  if (store_->row_bytes() != 4 * d_) {  // BINARYIVF: packed queries only (BinaryIvfIndex::search_codes)
-    set_last_error(type_ + ": queries are packed binary rows, not floats");
-    return -1;
-  }
-  cudaSetDevice(device_);
-  std::shared_lock<std::shared_mutex> lk(mu_);
-  Scratch s(st);
-  const float* xq = x_dev;
-  int64_t ldq = ldx;
-  if ((ldx & 3) || (reinterpret_cast<uintptr_t>(x_dev) & 15)) {  // re-pack into 16-byte aligned rows
-    float* buf = s.alloc_n<float>((size_t)nq * dpad_);
-    if (!buf) return -1;
-    GB_CUDA(cudaMemsetAsync(buf, 0, (size_t)nq * dpad_ * 4, st));
-    GB_CUDA(cudaMemcpy2DAsync(buf, (size_t)dpad_ * 4, x_dev, (size_t)ldx * 4, (size_t)d_ * 4, nq,
-                              cudaMemcpyDeviceToDevice, st));
-    xq = buf;
-    ldq = dpad_;
-  } else if (ldx < dpad_) {
-    set_last_error("query row stride smaller than padded dimension");
-    return -1;
-  }
+  cudaStream_t st = s.stream();
   FilterArgs f;
   if (upload_bitmaps(ctx, &f, s)) return -1;
-  int metric = ctx.params.metric >= 0 ? ctx.params.metric : mp_.metric;
+  const int metric = search_metric(ctx);
   GB_ALLOC(keys, unsigned long long, (size_t)nq * k, s);
-  // the device kernels take a dense nq x dpad block
-  if (ldq != dpad_) {
-    float* buf = s.alloc_n<float>((size_t)nq * dpad_);
-    if (!buf) return -1;
-    GB_CUDA(cudaMemcpy2DAsync(buf, (size_t)dpad_ * 4, xq, (size_t)ldq * 4, (size_t)dpad_ * 4, nq,
-                              cudaMemcpyDeviceToDevice, st));
-    xq = buf;
-  }
+  *out_keys = keys;
   int rc;
   if (ctx.params.brute_force || !trained_) {
     // brute-force fallback of the IVF models (gamma_index_ivfflat.cc:541-550, ivfpq.cc:561-570)
@@ -826,13 +822,43 @@ int Index::search_device(const SearchContext& ctx, int nq, const float* x_dev, i
       }
     }
   }
-  if (rc) {
-    note_search_enqueued(st);
-    return rc;
-  }
-  if (out_keys_dev) GB_CUDA(cudaMemcpyAsync(out_keys_dev, keys, (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, st));
-  if (out_dis_dev && out_ids_dev) GB_CUDA(launch_decode_keys(keys, k, nq, k, metric, out_dis_dev, out_ids_dev, 0, st));
   note_search_enqueued(st);
+  return rc;
+}
+
+int Index::search_device(const SearchContext& ctx, int nq, const float* x_dev, int64_t ldx, int k, float* out_dis_dev,
+                         int64_t* out_ids_dev, cudaStream_t st, unsigned long long* out_keys_dev) {
+  if (nq <= 0) return 0;
+  cudaSetDevice(device_);
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  Scratch s(st);
+  const float* xq = x_dev;
+  int64_t ldq = ldx;
+  if ((ldx & 3) || (reinterpret_cast<uintptr_t>(x_dev) & 15)) {  // re-pack into 16-byte aligned rows
+    float* buf = s.alloc_n<float>((size_t)nq * dpad_);
+    if (!buf) return -1;
+    GB_CUDA(cudaMemsetAsync(buf, 0, (size_t)nq * dpad_ * 4, st));
+    GB_CUDA(cudaMemcpy2DAsync(buf, (size_t)dpad_ * 4, x_dev, (size_t)ldx * 4, (size_t)d_ * 4, nq,
+                              cudaMemcpyDeviceToDevice, st));
+    xq = buf;
+    ldq = dpad_;
+  } else if (ldx < dpad_) {
+    set_last_error("query row stride smaller than padded dimension");
+    return -1;
+  }
+  // the device kernels take a dense nq x dpad block
+  if (ldq != dpad_) {
+    float* buf = s.alloc_n<float>((size_t)nq * dpad_);
+    if (!buf) return -1;
+    GB_CUDA(cudaMemcpy2DAsync(buf, (size_t)dpad_ * 4, xq, (size_t)ldq * 4, (size_t)dpad_ * 4, nq,
+                              cudaMemcpyDeviceToDevice, st));
+    xq = buf;
+  }
+  unsigned long long* keys;
+  if (int rc = search_keys(ctx, nq, xq, k, &keys, s)) return rc;
+  if (out_keys_dev) GB_CUDA(cudaMemcpyAsync(out_keys_dev, keys, (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, st));
+  if (out_dis_dev && out_ids_dev)
+    GB_CUDA(launch_decode_keys(keys, k, nq, k, search_metric(ctx), out_dis_dev, out_ids_dev, 0, st));
   return 0;
 }
 
@@ -859,7 +885,8 @@ static bool same_signature(const SearchContext& a, int ka, const SearchContext& 
 void Index::coalesce_loop() {
   cudaSetDevice(device_);
   std::vector<CoReq*> batch;
-  std::vector<float> xs, dd;
+  std::vector<unsigned char> xs;
+  std::vector<float> dd;
   std::vector<int64_t> ii;
   for (;;) {
     batch.clear();
@@ -887,12 +914,13 @@ void Index::coalesce_loop() {
     if (batch.size() == 1) {
       rc = search_direct(*batch[0]->ctx, batch[0]->nq, batch[0]->x, k, batch[0]->out_dis, batch[0]->out_ids);
     } else {
-      xs.resize((size_t)total * d_);
+      const size_t rb = store_->row_bytes();
+      xs.resize((size_t)total * rb);
       dd.resize((size_t)total * k);
       ii.resize((size_t)total * k);
       size_t o = 0;
       for (CoReq* r : batch) {
-        memcpy(xs.data() + o * d_, r->x, (size_t)r->nq * d_ * 4);
+        memcpy(xs.data() + o * rb, r->x, (size_t)r->nq * rb);
         o += r->nq;
       }
       rc = search_direct(*batch[0]->ctx, total, xs.data(), k, dd.data(), ii.data());
@@ -918,7 +946,7 @@ void Index::coalesce_loop() {
   }
 }
 
-int Index::search(const SearchContext& ctx, int nq, const float* x, int k, float* out_dis, int64_t* out_ids) {
+int Index::search(const SearchContext& ctx, int nq, const void* x, int k, float* out_dis, int64_t* out_ids) {
   if (nq <= 0) return 0;
   if (!coalescable(ctx, nq)) return search_direct(ctx, nq, x, k, out_dis, out_ids);
   CoReq req;
@@ -937,56 +965,46 @@ int Index::search(const SearchContext& ctx, int nq, const float* x, int k, float
   return req.rc;
 }
 
-int Index::search_direct(const SearchContext& ctx, int nq, const float* x, int k, float* out_dis, int64_t* out_ids) {
+int Index::search_direct(const SearchContext& ctx, int nq, const void* x, int k, float* out_dis, int64_t* out_ids) {
   if (nq <= 0) return 0;
   cudaSetDevice(device_);
-  cudaStream_t st = thread_stream(device_);
-  float* dq = nullptr;
-  float* dd = nullptr;
-  int64_t* di = nullptr;
-  int rc = -1;
-  do {
-    if (cudaMallocAsync(&dq, (size_t)nq * dpad_ * 4, st) != cudaSuccess) break;
-    if (cudaMallocAsync(&dd, (size_t)nq * k * 4, st) != cudaSuccess) break;
-    if (cudaMallocAsync(&di, (size_t)nq * k * 8, st) != cudaSuccess) break;
-    if (upload_rows_padded(dq, x, nq, d_, dpad_, st) != cudaSuccess) break;
-    rc = search_device(ctx, nq, dq, dpad_, k, dd, di, st);
-    if (rc) break;
-    rc = -1;
-    if (cudaMemcpyAsync(out_dis, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) break;
-    if (cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) break;
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-      set_last_error(std::string("search: ") + cudaGetErrorString(e));
-      break;
-    }
-    rc = 0;
-  } while (0);
-  if (rc == -1 && !*last_error()) set_last_error(std::string("search: ") + cudaGetErrorString(cudaGetLastError()));
-  if (dq) cudaFreeAsync(dq, st);
-  if (dd) cudaFreeAsync(dd, st);
-  if (di) cudaFreeAsync(di, st);
-  return rc;
+  Scratch s(thread_stream(device_));
+  const void* xq = upload_queries(nq, x, s);
+  if (!xq) return -1;
+  unsigned long long* keys;
+  {
+    std::shared_lock<std::shared_mutex> lk(mu_);
+    if (int rc = search_keys(ctx, nq, xq, k, &keys, s)) return rc;
+  }
+  return download_results(keys, nq, k, search_metric(ctx), out_dis, out_ids, s);
+}
+
+cudaError_t Index::flat_tile(const void* xq, int nq, const void* rows, int m, int metric, float* scores, int64_t ldo,
+                             cudaStream_t st) {
+  last_scan_kernel_ = "dist_tile_kernel+select_rows_kernel";
+  return launch_dist_matrix(static_cast<const float*>(xq), dpad_, nq, static_cast<const float*>(rows), dpad_, m, dpad_, metric,
+                            scores, ldo, st);
 }
 
 // GammaFLATIndex::Search (gamma_index_flat.cc:130-370): every stored row, filters before top-k.
-int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
+int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xqv, int k,
                            int64_t nrows, unsigned long long* out_keys, Scratch& s, int64_t row_begin) {
   (void)ctx;
   cudaStream_t st = s.stream();
-  const int64_t flat_row_begin_ = row_begin;
   if (nrows <= row_begin) return launch_fill_u64(out_keys, (int64_t)nq * k, kKeySentinel, st) == cudaSuccess ? 0 : -1;
+  const unsigned char* xq = static_cast<const unsigned char*>(xqv);
+  const int64_t ld = store_->stride();
   const int64_t CC = std::min<int64_t>(131072, store_->seg_rows());  // DB rows per distance block
   struct Chunk {
-    const float* base;
+    const unsigned char* base;
     int64_t id0;
     int cnt;
   };
   std::vector<Chunk> chunks;
-  for (int64_t r = flat_row_begin_; r < nrows;) {
+  for (int64_t r = row_begin; r < nrows;) {
     int64_t si = r >> store_->seg_shift(), off = r & (store_->seg_rows() - 1);
     int64_t cnt = std::min<int64_t>(std::min(nrows - r, store_->seg_rows() - off), CC);
-    chunks.push_back({store_->seg((int)si) + off * dpad_, r, (int)cnt});
+    chunks.push_back({store_->seg_bytes((int)si) + off * ld, r, (int)cnt});
     r += cnt;
   }
   const int nch = (int)chunks.size();
@@ -998,7 +1016,6 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
     partial = s.alloc_n<unsigned long long>((size_t)nq * nch * k);
     if (!partial) return -1;
   }
-  last_scan_kernel_ = "dist_tile_kernel+select_rows_kernel";
   if (store_->on_host()) {
     // Host placement: each chunk is copied once, on a copy stream, into one of two HBM staging buffers, so the copy of
     // chunk c + 1 overlaps the distance and select kernels of chunk c.  The chunks, kernels and partial merge are those
@@ -1012,9 +1029,9 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
     } lane{this, lane_acquire()};
     if (!lane.l) return -1;
     CopyLane& cl = *lane.l;
-    float* stage[2];
+    void* stage[2];
     for (int b = 0; b < 2; b++) {
-      stage[b] = s.alloc_n<float>((size_t)CC * dpad_);
+      stage[b] = s.alloc((size_t)CC * ld);
       if (!stage[b]) return -1;
       GB_CUDA(cudaEventRecord(cl.reusable[b], st));  // the buffers are allocated in stream order on st
     }
@@ -1022,13 +1039,12 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
     for (int c = 0; c < nch; c++) {
       const int b = c & 1;
       GB_CUDA(cudaStreamWaitEvent(cl.cs, cl.reusable[b], 0));
-      GB_CUDA(cudaMemcpyAsync(stage[b], chunks[c].base, (size_t)chunks[c].cnt * dpad_ * 4, cudaMemcpyHostToDevice, cl.cs));
+      GB_CUDA(cudaMemcpyAsync(stage[b], chunks[c].base, (size_t)chunks[c].cnt * ld, cudaMemcpyHostToDevice, cl.cs));
       GB_CUDA(cudaEventRecord(cl.copied[b], cl.cs));
       GB_CUDA(cudaStreamWaitEvent(st, cl.copied[b], 0));
       for (int q0 = 0; q0 < nq; q0 += QB) {
         int qb = std::min(QB, nq - q0);
-        GB_CUDA(launch_dist_matrix(xq + (int64_t)q0 * dpad_, dpad_, qb, stage[b], dpad_, chunks[c].cnt, dpad_, metric,
-                                   scores, ldo, st));
+        GB_CUDA(flat_tile(xq + q0 * ld, qb, stage[b], chunks[c].cnt, metric, scores, ldo, st));
         GB_CUDA(launch_select_scores(scores, ldo, qb, chunks[c].cnt, chunks[c].id0, k, metric, f,
                                      partial + ((int64_t)q0 * nch + c) * k, (int64_t)nch * k, st));
       }
@@ -1042,8 +1058,7 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
   for (int q0 = 0; q0 < nq; q0 += QB) {
     int qb = std::min(QB, nq - q0);
     for (int c = 0; c < nch; c++) {
-      GB_CUDA(launch_dist_matrix(xq + (int64_t)q0 * dpad_, dpad_, qb, chunks[c].base, dpad_, chunks[c].cnt, dpad_,
-                                 metric, scores, ldo, st));
+      GB_CUDA(flat_tile(xq + q0 * ld, qb, chunks[c].base, chunks[c].cnt, metric, scores, ldo, st));
       GB_CUDA(launch_select_scores(scores, ldo, qb, chunks[c].cnt, chunks[c].id0, k, metric, f,
                                    partial + ((int64_t)q0 * nch + c) * k, (int64_t)nch * k, st));
     }
@@ -1053,7 +1068,7 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
   return 0;
 }
 
-int FlatIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
+int FlatIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, int k,
                                unsigned long long* out_keys, Scratch& s) {
   return flat_search_dev(ctx, f, metric, nq, xq, k, store_->size(), out_keys, s);
 }
@@ -1525,9 +1540,10 @@ static int coarse_seg_tiles(int nqt, int ntc, int nsm) {
 }
 
 // quantizer->search (gamma_index_ivfflat.cc:568 / gamma_index_ivfpq.cc:595)
-int IvfIndex::coarse_dev(int nq, const float* xq, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis,
+int IvfIndex::coarse_dev(int nq, const void* xqv, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis,
                          Scratch& s) {
   cudaStream_t st = s.stream();
+  const float* xq = static_cast<const float*>(xqv);
   GB_ALLOC(keys, unsigned long long, (size_t)nq * nprobe, s);
   const bool tc = nlist_ >= 64 && nq >= 32;
   const int k16 = (int)round_up(dpad_, 16);
@@ -1749,13 +1765,14 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
   return 0;
 }
 
-int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq,
-                           const float* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
+int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xqv,
+                           const void* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
                            unsigned long long* out_keys, Scratch& s) {
   (void)ctx;
   (void)xq_raw;  // no transform: xq is the raw queries
   (void)coarse_dis;
   cudaStream_t st = s.stream();
+  const float* xq = static_cast<const float*>(xqv);
   // The list-major scan selects on 3xTF32 tensor-core scores.  Under L2 it evaluates |x - s|^2 + |y - s|^2 -
   // 2 (x - s).(y - s) with s = s_l, the shift of the probed list (d_shifts_, near its centroid), so the cancellation
   // error scales with the residual norms: on raw vectors with a common offset (|x|^2 ~ 1e8 at offset 1000, d = 128) the
@@ -1795,35 +1812,42 @@ int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int me
 }
 
 // GammaIVFFlatIndex::Search (gamma_index_ivfflat.cc:524-577)
-int IvfIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq_in, int k,
+int IvfIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq_in, int k,
                               unsigned long long* out_keys, Scratch& s) {
-  const float* xq = transform_dev(xq_in, nq, s);
+  const void* xq = transform_dev(static_cast<const float*>(xq_in), nq, s);  // the identity unless an OPQ rotation is set
   if (!xq) return -1;
   const int nprobe = resolve_nprobe(ctx);
+  const int64_t ld = store_->stride();
   const int QB = 16384;
   for (int q0 = 0; q0 < nq; q0 += QB) {
     int qb = std::min(QB, nq - q0);
     Scratch sb(s.stream());
     GB_ALLOC(probe_ids, int32_t, (size_t)qb * nprobe, sb);
     GB_ALLOC(coarse_dis, float, (size_t)qb * nprobe, sb);
-    if (coarse_dev(qb, xq + (int64_t)q0 * dpad_, nprobe, coarse_metric(metric), probe_ids, coarse_dis, sb)) return -1;
-    if (scan_dev(ctx, f, metric, qb, xq + (int64_t)q0 * dpad_, xq_in + (int64_t)q0 * dpad_, k, probe_ids, coarse_dis, nprobe,
+    const void* xb = static_cast<const unsigned char*>(xq) + q0 * ld;
+    if (coarse_dev(qb, xb, nprobe, coarse_metric(metric), probe_ids, coarse_dis, sb)) return -1;
+    if (scan_dev(ctx, f, metric, qb, xb, static_cast<const unsigned char*>(xq_in) + q0 * ld, k, probe_ids, coarse_dis, nprobe,
                  out_keys + (int64_t)q0 * k, sb))
       return -1;
   }
   return 0;
 }
 
-int IvfIndex::coarse_search_host(int nq, const float* x, int nprobe, float* out_dis, int64_t* out_ids) {
+int IvfIndex::coarse_search_host(int nq, const void* x, int nprobe, float* out_dis, int64_t* out_ids) {
+  if (nq <= 0) return 0;
+  if (!trained_ || nprobe <= 0 || nprobe > std::min(nlist_, 4096)) {
+    set_last_error("coarse_search: untrained index or nprobe out of range");
+    return -1;
+  }
   cudaSetDevice(device_);
   cudaStream_t st = thread_stream(device_);
   std::shared_lock<std::shared_mutex> lk(mu_);
   Scratch s(st);
-  GB_ALLOC(dq, float, (size_t)nq * dpad_, s);
-  GB_CUDA(upload_rows_padded(dq, x, nq, d_, dpad_, st));
+  const void* dq = upload_queries(nq, x, s);
+  if (!dq) return -1;
   GB_ALLOC(ids, int32_t, (size_t)nq * nprobe, s);
   GB_ALLOC(dis, float, (size_t)nq * nprobe, s);
-  const float* dqt = transform_dev(dq, nq, s);
+  const float* dqt = transform_dev(static_cast<const float*>(dq), nq, s);
   if (!dqt || coarse_dev(nq, dqt, nprobe, coarse_metric(mp_.metric), ids, dis, s)) return -1;
   std::vector<int32_t> h((size_t)nq * nprobe);
   GB_CUDA(cudaMemcpyAsync(h.data(), ids, h.size() * 4, cudaMemcpyDeviceToHost, st));
@@ -1833,38 +1857,37 @@ int IvfIndex::coarse_search_host(int nq, const float* x, int nprobe, float* out_
   return 0;
 }
 
-int IvfIndex::search_preassigned_host(const SearchContext& ctx, int nq, const float* x, int k, const int64_t* keys,
+int IvfIndex::search_preassigned_host(const SearchContext& ctx, int nq, const void* x, int k, const int64_t* keys,
                                       const float* coarse_dis, int nprobe, float* out_dis, int64_t* out_ids) {
-  if (!trained_ || !lists_) {
-    set_last_error("index not trained");
+  if (nq <= 0) return 0;
+  if (!trained_ || !lists_ || k <= 0 || k > 4096 || nprobe <= 0 || nprobe > 4096) {
+    set_last_error("search_preassigned: untrained index, topK or nprobe out of range");
     return -1;
   }
   cudaSetDevice(device_);
   cudaStream_t st = thread_stream(device_);
   std::shared_lock<std::shared_mutex> lk(mu_);
   Scratch s(st);
-  GB_ALLOC(dq, float, (size_t)nq * dpad_, s);
-  GB_CUDA(upload_rows_padded(dq, x, nq, d_, dpad_, st));
+  const void* dq = upload_queries(nq, x, s);
+  if (!dq) return -1;
   std::vector<int32_t> h((size_t)nq * nprobe);
   for (size_t i = 0; i < h.size(); i++) h[i] = (int32_t)keys[i];
   GB_ALLOC(ids, int32_t, h.size(), s);
   GB_ALLOC(dis, float, h.size(), s);
   GB_CUDA(cudaMemcpyAsync(ids, h.data(), h.size() * 4, cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemcpyAsync(dis, coarse_dis, h.size() * 4, cudaMemcpyHostToDevice, st));
+  if (coarse_dis) {
+    GB_CUDA(cudaMemcpyAsync(dis, coarse_dis, h.size() * 4, cudaMemcpyHostToDevice, st));
+  } else {
+    GB_CUDA(cudaMemsetAsync(dis, 0, h.size() * 4, st));
+  }
   FilterArgs f;
   if (upload_bitmaps(ctx, &f, s)) return -1;
-  int metric = ctx.params.metric >= 0 ? ctx.params.metric : mp_.metric;
+  const int metric = search_metric(ctx);
   GB_ALLOC(okeys, unsigned long long, (size_t)nq * k, s);
-  const float* dqt = transform_dev(dq, nq, s);
+  const float* dqt = transform_dev(static_cast<const float*>(dq), nq, s);
   if (!dqt) return -1;
   if (scan_dev(ctx, f, metric, nq, dqt, dq, k, ids, dis, nprobe, okeys, s)) return -1;
-  GB_ALLOC(dd, float, (size_t)nq * k, s);
-  GB_ALLOC(di, int64_t, (size_t)nq * k, s);
-  GB_CUDA(launch_decode_keys(okeys, k, nq, k, metric, dd, di, 0, st));
-  GB_CUDA(cudaMemcpyAsync(out_dis, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return download_results(okeys, nq, k, metric, out_dis, out_ids, s);  // synchronises before h goes
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2395,10 +2418,11 @@ int IvfPqBase::scan_pq_dev(const char* kernel, const SearchContext& ctx, const F
 }
 
 // GammaIVFPQIndex::search_preassigned (gamma_index_ivfpq.cc:730-947)
-int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq,
-                         const float* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
+int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xqv,
+                         const void* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
                          unsigned long long* out_keys, Scratch& s) {
   cudaStream_t st = s.stream();
+  const float* xq = static_cast<const float*>(xqv);
   float* ip = nullptr;
   auto prepare = [&](int kk, unsigned long long* keys, bool need_sorted) {
     ip = s.alloc_n<float>((size_t)nq * M_ * ksub_);
@@ -2419,7 +2443,8 @@ int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metr
                              partial, st);
   };
   // "for opq, rerank need raw vector" (gamma_index_ivfpq.cc:735): original queries against the raw store
-  return scan_pq_dev(nbits_ < 8 ? "ivfpq_packed_scan_kernel" : "ivfpq_scan_kernel", ctx, f, metric, nq, xq_raw, k, nprobe,
+  return scan_pq_dev(nbits_ < 8 ? "ivfpq_packed_scan_kernel" : "ivfpq_scan_kernel", ctx, f, metric, nq,
+                     static_cast<const float*>(xq_raw), k, nprobe,
                      ivfpq_scan_max_k(M_, nbits_), out_keys, s, prepare, launch);
 }
 
@@ -2463,11 +2488,12 @@ int IVFPQFastScanIndex::lut_host(int nq, const float* x, int metric, uint8_t* lu
 
 // IndexIVFFastScan::search_preassigned restated over this engine's lists, filters applied before selection;
 // recall_num > 0 re-ranks the recall_num best exactly from the raw vectors, as IVFPQ does
-int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq,
-                                 const float* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
+int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xqv,
+                                 const void* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
                                  unsigned long long* out_keys, Scratch& s) {
   (void)coarse_dis;  // no residual: the list's coarse distance takes no part in the score
   cudaStream_t st = s.stream();
+  const float* xq = static_cast<const float*>(xqv);
   uint8_t* lut = nullptr;
   float* ab = nullptr;
   auto prepare = [&](int, unsigned long long*, bool) {
@@ -2481,7 +2507,8 @@ int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, 
   auto launch = [&](int kk, int pg, unsigned long long* partial) {
     return launch_ivfpqfs_scan(lut, ab, nq, probe_ids, nprobe, pg, lists_->directory(), M_, kk, metric, f, partial, st);
   };
-  return scan_pq_dev("ivfpqfs_scan_kernel", ctx, f, metric, nq, xq_raw, k, nprobe, 4096, out_keys, s, prepare, launch);
+  return scan_pq_dev("ivfpqfs_scan_kernel", ctx, f, metric, nq, static_cast<const float*>(xq_raw), k, nprobe, 4096, out_keys, s,
+                     prepare, launch);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2496,32 +2523,27 @@ BinaryIvfIndex::BinaryIvfIndex(int d_bits, const ModelParams& mp, int device, in
 BinaryIvfIndex::~BinaryIvfIndex() { cudaFree(d_bcent_); }
 int64_t BinaryIvfIndex::index_mem_bytes() const { return IvfIndex::index_mem_bytes() + (int64_t)nlist_ * ldw_ * 4; }
 
-// GammaIndexBinaryIVF::Indexing (gamma_index_binary_ivf.cc:212-270) -> faiss IndexBinaryIVF::train: the first num rows
-// expanded to +-1 floats, faiss Clustering (niter 10, Init) with an IndexFlatL2, centroids packed by sign
-int BinaryIvfIndex::train() {
-  std::lock_guard<std::mutex> bg(build_mu_);
-  if (trained_) return 0;
-  cudaSetDevice(device_);
-  const int64_t num = training_threshold();
-  if (num > store_->size()) {
-    set_last_error("vector total count less than training_threshold");
-    return -1;
-  }
-  std::unique_lock<std::shared_mutex> lk(mu_);
-  drain_searches();
-  cudaStream_t st = build_stream_;
-  Scratch s(st);
-  GB_ALLOC(raw, uint8_t, (size_t)num * ldw_ * 4, s);
-  GB_CUDA(store_->copy_rows_to_device(0, num, raw, st));
-  GB_ALLOC(xf, float, (size_t)num * dpad_, s);
-  GB_CUDA(launch_binary_to_real(raw, ldw_ * 4, num, d_, xf, dpad_, st));
+// GammaIndexBinaryIVF::Indexing (gamma_index_binary_ivf.cc:212-270) -> faiss IndexBinaryIVF::train, through
+// IvfIndex::train: the first num rows expanded to +-1 floats, faiss Clustering (niter 10, Init) with an IndexFlatL2,
+// centroids packed by sign
+KMeansParams BinaryIvfIndex::coarse_kmeans_params() const {
   KMeansParams kp;
   kp.niter = 10;  // gamma_index_binary_ivf.cc:97
-  if (kmeans_device(xf, dpad_, num, d_, nlist_, kp, d_centroids_, dpad_, st, nullptr)) return -1;
+  return kp;
+}
+// xt: the packed training rows as RawStore::contiguous leaves them; the result is one fp32 slab of n x dpad floats
+const float* BinaryIvfIndex::train_transform(const float* xt, int64_t n, Scratch& s) {
+  float* xf = s.alloc_n<float>((size_t)n * dpad_);
+  if (!xf) return nullptr;
+  const cudaError_t e = launch_binary_to_real(reinterpret_cast<const uint8_t*>(xt), ldw_ * 4, n, d_, xf, dpad_, s.stream());
+  if (e != cudaSuccess) {
+    set_last_error(std::string("BINARYIVF: binary_to_real: ") + cudaGetErrorString(e));
+    return nullptr;
+  }
+  return xf;
+}
+int BinaryIvfIndex::centroids_changed(cudaStream_t st) {
   GB_CUDA(launch_real_to_binary(d_centroids_, dpad_, nlist_, d_, d_bcent_, ldw_ * 4, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  if (!lists_) lists_.reset(new IvfLists(nlist_, code_bytes()));
-  trained_ = true;
   return 0;
 }
 
@@ -2545,18 +2567,17 @@ int BinaryIvfIndex::get_binary_centroids(uint8_t* host) const {
   return 0;
 }
 
-int BinaryIvfIndex::hamming_topk(const uint32_t* xq, int64_t ldq, int nq, const uint32_t* rows, int64_t ldr, int m,
-                                 int64_t id_base, int k, const FilterArgs& f, unsigned long long* out_keys,
-                                 int64_t out_stride, Scratch& s) {
+int BinaryIvfIndex::hamming_topk(const uint32_t* xq, int nq, int k, unsigned long long* keys, Scratch& s) {
   cudaStream_t st = s.stream();
-  const int64_t ldo = round_up(m, 4);
+  const int64_t ldo = round_up(nlist_, 4);
   const int QB = (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)nq, ((int64_t)1 << 28) / ldo, 65536}));
   GB_ALLOC(scores, float, (size_t)QB * ldo, s);
+  const FilterArgs none{nullptr, nullptr, -FLT_MAX, FLT_MAX};
   for (int q0 = 0; q0 < nq; q0 += QB) {
     const int qb = std::min(QB, nq - q0);
-    GB_CUDA(launch_hamming_tile(xq + (int64_t)q0 * ldq, ldq, qb, rows, ldr, m, (cb_ + 3) / 4, scores, ldo, st));
-    GB_CUDA(launch_select_scores(scores, ldo, qb, m, id_base, k, kMetricL2, f, out_keys + (int64_t)q0 * out_stride,
-                                 out_stride, st));
+    GB_CUDA(launch_hamming_tile(xq + (int64_t)q0 * ldw_, ldw_, qb, reinterpret_cast<const uint32_t*>(d_bcent_), ldw_, nlist_,
+                                (cb_ + 3) / 4, scores, ldo, st));
+    GB_CUDA(launch_select_scores(scores, ldo, qb, nlist_, 0, k, kMetricL2, none, keys + (int64_t)q0 * k, k, st));
   }
   return 0;
 }
@@ -2565,13 +2586,7 @@ int BinaryIvfIndex::hamming_topk(const uint32_t* xq, int64_t ldq, int nq, const 
 int BinaryIvfIndex::assign_batch(const void* x, int64_t n, const void** xc, int32_t* out, Scratch& s) {
   *xc = x;
   GB_ALLOC(best, unsigned long long, n, s);
-  const FilterArgs none{nullptr, nullptr, -FLT_MAX, FLT_MAX};
-  for (int64_t i0 = 0; i0 < n; i0 += 65536) {
-    const int nb = (int)std::min<int64_t>(65536, n - i0);
-    if (hamming_topk(static_cast<const uint32_t*>(x) + i0 * ldw_, ldw_, nb, reinterpret_cast<const uint32_t*>(d_bcent_),
-                     ldw_, nlist_, 0, 1, none, best + i0, 1, s))
-      return -1;
-  }
+  if (hamming_topk(static_cast<const uint32_t*>(x), (int)n, 1, best, s)) return -1;
   GB_CUDA(launch_split_keys(best, n, kMetricL2, nullptr, out, s.stream()));
   return 0;
 }
@@ -2588,59 +2603,39 @@ int BinaryIvfIndex::append_batch(const void* x, int64_t n, int64_t vid0, const i
   return 0;
 }
 
-int BinaryIvfIndex::scan_dev(const SearchContext&, const FilterArgs&, int, int, const float*, const float*, int,
-                             const int32_t*, const float*, int, unsigned long long*, Scratch&) {
-  set_last_error(type_ + ": queries are packed binary rows, not floats");
-  return -1;
-}
-
-int BinaryIvfIndex::flat_codes(const FilterArgs& f, int nq, const uint32_t* xq, int k, int64_t row_begin, int64_t row_end,
-                               unsigned long long* out_keys, Scratch& s) {
-  cudaStream_t st = s.stream();
-  if (row_end <= row_begin) return launch_fill_u64(out_keys, (int64_t)nq * k, kKeySentinel, st) == cudaSuccess ? 0 : -1;
-  const int64_t CC = std::min<int64_t>(131072, store_->seg_rows());
-  std::vector<std::pair<int64_t, int>> chunks;  // (first row, rows), inside one segment
-  for (int64_t r = row_begin; r < row_end;) {
-    const int64_t off = r & (store_->seg_rows() - 1);
-    const int cnt = (int)std::min<int64_t>(std::min(row_end - r, store_->seg_rows() - off), CC);
-    chunks.emplace_back(r, cnt);
-    r += cnt;
-  }
-  const int nch = (int)chunks.size();
-  unsigned long long* partial = out_keys;
-  if (nch > 1) {
-    partial = s.alloc_n<unsigned long long>((size_t)nq * nch * k);
-    if (!partial) return -1;
-  }
+// launch_hamming_tile, in launches of at most kHammingTileMaxQueries queries
+cudaError_t BinaryIvfIndex::flat_tile(const void* xq, int nq, const void* rows, int m, int metric, float* scores, int64_t ldo,
+                                      cudaStream_t st) {
+  (void)metric;
   last_scan_kernel_ = "hamming_tile_kernel+select_rows_kernel";
-  scan_timer_begin(st);
-  for (int c = 0; c < nch; c++) {
-    // host placement: the chunk is copied to HBM first, in stream order (the same chunks, so the same keys)
-    const uint32_t* rows = static_cast<const uint32_t*>(store_rows_dev(chunks[c].first, chunks[c].second, s));
-    if (!rows) return -1;
-    if (hamming_topk(xq, ldw_, nq, rows, ldw_, chunks[c].second, chunks[c].first, k, f, partial + (int64_t)c * k,
-                     (int64_t)nch * k, s))
-      return -1;
+  for (int q0 = 0; q0 < nq; q0 += kHammingTileMaxQueries) {
+    const cudaError_t e = launch_hamming_tile(static_cast<const uint32_t*>(xq) + q0 * ldw_, ldw_,
+                                              std::min(kHammingTileMaxQueries, nq - q0), static_cast<const uint32_t*>(rows),
+                                              ldw_, m, (cb_ + 3) / 4, scores + q0 * ldo, ldo, st);
+    if (e != cudaSuccess) return e;
   }
-  if (nch > 1) GB_CUDA(launch_select_keys(partial, (int64_t)nch * k, nq, nch * k, k, out_keys, k, st));
-  scan_timer_end(st);
-  return 0;
+  return cudaSuccess;
 }
 
 // quantizer->search: the nprobe Hamming-nearest centroids, the smaller list id among equals
-int BinaryIvfIndex::coarse_codes(int nq, const uint32_t* xq, int nprobe, int32_t* probe_ids, float* coarse_dis, Scratch& s) {
+int BinaryIvfIndex::coarse_dev(int nq, const void* xq, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis,
+                               Scratch& s) {
+  (void)metric;
   GB_ALLOC(keys, unsigned long long, (size_t)nq * nprobe, s);
-  const FilterArgs none{nullptr, nullptr, -FLT_MAX, FLT_MAX};
-  if (hamming_topk(xq, ldw_, nq, reinterpret_cast<const uint32_t*>(d_bcent_), ldw_, nlist_, 0, nprobe, none, keys, nprobe, s))
-    return -1;
+  if (hamming_topk(static_cast<const uint32_t*>(xq), nq, nprobe, keys, s)) return -1;
   GB_CUDA(launch_split_keys(keys, (int64_t)nq * nprobe, kMetricL2, coarse_dis, probe_ids, s.stream()));
   return 0;
 }
 
 // search_knn_hamming_heap over the probed lists: the shared query-major list scan with the Hamming codec, then the merge
 // of its CTA groups
-int BinaryIvfIndex::scan_codes(const FilterArgs& f, int nq, const uint32_t* xq, int k, const int32_t* probe_ids, int nprobe,
-                               unsigned long long* out_keys, Scratch& s) {
+int BinaryIvfIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq,
+                             const void* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
+                             unsigned long long* out_keys, Scratch& s) {
+  (void)ctx;
+  (void)metric;
+  (void)xq_raw;  // no transform
+  (void)coarse_dis;  // the list's coarse distance takes no part in the score
   cudaStream_t st = s.stream();
   const int max_k = binary_scan_max_k(cb_);
   if (k > max_k) {
@@ -2655,7 +2650,8 @@ int BinaryIvfIndex::scan_codes(const FilterArgs& f, int nq, const uint32_t* xq, 
   last_scan_kernel_ = "binary_ivf_scan_kernel";
   snprintf(last_scan_info_, sizeof(last_scan_info_), "{\"probes_per_cta\": %d}", pg);
   scan_timer_begin(st);
-  GB_CUDA(launch_binary_ivf_scan(xq, ldw_, nq, probe_ids, nprobe, pg, lists_->directory(), cb_, k, f, partial, st));
+  GB_CUDA(launch_binary_ivf_scan(static_cast<const uint32_t*>(xq), ldw_, nq, probe_ids, nprobe, pg, lists_->directory(), cb_, k,
+                                 f, partial, st));
   scan_timer_end(st);
   if (ngroups > 1) {
     GB_CUDA(launch_select_keys(partial, (int64_t)ngroups * k, nq, ngroups * k, k, out_keys, k, st));
@@ -2663,113 +2659,6 @@ int BinaryIvfIndex::scan_codes(const FilterArgs& f, int nq, const uint32_t* xq, 
     GB_CUDA(cudaMemcpyAsync(out_keys, partial, (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, st));
   }
   return 0;
-}
-
-const uint32_t* BinaryIvfIndex::upload_queries(int nq, const uint8_t* x, Scratch& s) {
-  uint32_t* dq = s.alloc_n<uint32_t>((size_t)nq * ldw_);
-  if (!dq) return nullptr;
-  if (cudaMemsetAsync(dq, 0, (size_t)nq * ldw_ * 4, s.stream()) != cudaSuccess ||
-      cudaMemcpy2DAsync(dq, (size_t)ldw_ * 4, x, cb_, cb_, nq, cudaMemcpyHostToDevice, s.stream()) != cudaSuccess) {
-    set_last_error("BINARYIVF: query upload failed");
-    return nullptr;
-  }
-  return dq;
-}
-
-int BinaryIvfIndex::finish_host(const unsigned long long* keys, int nq, int k, float* out_dis, int64_t* out_ids,
-                                cudaStream_t st) {
-  Scratch s(st);
-  GB_ALLOC(dd, float, (size_t)nq * k, s);
-  GB_ALLOC(di, int64_t, (size_t)nq * k, s);
-  GB_CUDA(launch_decode_keys(keys, k, nq, k, kMetricL2, dd, di, 0, st));
-  GB_CUDA(cudaMemcpyAsync(out_dis, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  return 0;
-}
-
-// GammaIndexBinaryIVF::Search (gamma_index_binary_ivf.cc:290-325) with this engine's brute-force and realtime-tail rules
-// (Index::search_device): brute_force or an untrained index scan every stored row exactly; search_unindexed_tail adds
-// the stored but not yet indexed rows, merged by distance
-int BinaryIvfIndex::search_codes(const SearchContext& ctx, int nq, const uint8_t* x, int k, float* out_dis, int64_t* out_ids) {
-  if (nq <= 0) return 0;
-  if (k <= 0 || k > 4096) {
-    set_last_error("topK must be in [1, 4096]");
-    return -1;
-  }
-  cudaSetDevice(device_);
-  cudaStream_t st = thread_stream(device_);
-  std::shared_lock<std::shared_mutex> lk(mu_);
-  Scratch s(st);
-  const uint32_t* xq = upload_queries(nq, x, s);
-  if (!xq) return -1;
-  FilterArgs f;
-  if (upload_bitmaps(ctx, &f, s)) return -1;
-  GB_ALLOC(keys, unsigned long long, (size_t)nq * k, s);
-  if (ctx.params.brute_force || !trained_) {
-    if (flat_codes(f, nq, xq, k, 0, store_->size(), keys, s)) return -1;
-  } else {
-    const int nprobe = resolve_nprobe(ctx);
-    GB_ALLOC(probe_ids, int32_t, (size_t)nq * nprobe, s);
-    GB_ALLOC(coarse_dis, float, (size_t)nq * nprobe, s);
-    if (coarse_codes(nq, xq, nprobe, probe_ids, coarse_dis, s)) return -1;
-    if (scan_codes(f, nq, xq, k, probe_ids, nprobe, keys, s)) return -1;
-    const int64_t tail0 = indexed_count_, tail1 = store_->size();
-    if (ctx.search_unindexed_tail && tail1 > tail0) {
-      GB_ALLOC(both, unsigned long long, (size_t)nq * 2 * k, s);
-      GB_CUDA(cudaMemcpy2DAsync(both, (size_t)2 * k * 8, keys, (size_t)k * 8, (size_t)k * 8, nq, cudaMemcpyDeviceToDevice, st));
-      GB_ALLOC(tailk, unsigned long long, (size_t)nq * k, s);
-      if (flat_codes(f, nq, xq, k, tail0, tail1, tailk, s)) return -1;
-      GB_CUDA(cudaMemcpy2DAsync(both + k, (size_t)2 * k * 8, tailk, (size_t)k * 8, (size_t)k * 8, nq, cudaMemcpyDeviceToDevice,
-                                st));
-      GB_CUDA(launch_select_keys(both, (int64_t)2 * k, nq, 2 * k, k, keys, k, st));
-    }
-  }
-  return finish_host(keys, nq, k, out_dis, out_ids, st);
-}
-
-int BinaryIvfIndex::coarse_search_codes(int nq, const uint8_t* x, int nprobe, float* out_dis, int64_t* out_ids) {
-  if (nq <= 0) return 0;
-  if (!trained_ || nprobe <= 0 || nprobe > std::min(nlist_, 4096)) {
-    set_last_error("coarse_search: untrained index or nprobe out of range");
-    return -1;
-  }
-  cudaSetDevice(device_);
-  cudaStream_t st = thread_stream(device_);
-  std::shared_lock<std::shared_mutex> lk(mu_);
-  Scratch s(st);
-  const uint32_t* xq = upload_queries(nq, x, s);
-  if (!xq) return -1;
-  GB_ALLOC(keys, unsigned long long, (size_t)nq * nprobe, s);
-  const FilterArgs none{nullptr, nullptr, -FLT_MAX, FLT_MAX};
-  if (hamming_topk(xq, ldw_, nq, reinterpret_cast<const uint32_t*>(d_bcent_), ldw_, nlist_, 0, nprobe, none, keys, nprobe, s))
-    return -1;
-  return finish_host(keys, nq, nprobe, out_dis, out_ids, st);
-}
-
-int BinaryIvfIndex::search_preassigned_codes(const SearchContext& ctx, int nq, const uint8_t* x, int k, const int64_t* keys,
-                                             int nprobe, float* out_dis, int64_t* out_ids) {
-  if (nq <= 0) return 0;
-  if (!lists_ || k <= 0 || k > 4096 || nprobe <= 0 || nprobe > 4096) {
-    set_last_error("search_preassigned: untrained index, topK or nprobe out of range");
-    return -1;
-  }
-  cudaSetDevice(device_);
-  cudaStream_t st = thread_stream(device_);
-  std::shared_lock<std::shared_mutex> lk(mu_);
-  Scratch s(st);
-  const uint32_t* xq = upload_queries(nq, x, s);
-  if (!xq) return -1;
-  FilterArgs f;
-  if (upload_bitmaps(ctx, &f, s)) return -1;
-  std::vector<int32_t> h_ids((size_t)nq * nprobe);
-  for (size_t i = 0; i < h_ids.size(); i++) h_ids[i] = (int32_t)keys[i];
-  GB_ALLOC(probe_ids, int32_t, h_ids.size(), s);
-  GB_CUDA(cudaMemcpyAsync(probe_ids, h_ids.data(), h_ids.size() * 4, cudaMemcpyHostToDevice, st));
-  GB_ALLOC(okeys, unsigned long long, (size_t)nq * k, s);
-  if (scan_codes(f, nq, xq, k, probe_ids, nprobe, okeys, s)) return -1;
-  const int rc = finish_host(okeys, nq, k, out_dis, out_ids, st);  // synchronises before h_ids goes
-  return rc;
 }
 
 // ------------------------------------------------------------------------------------------

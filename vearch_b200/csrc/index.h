@@ -82,7 +82,8 @@ class RawStore {
   int update_host(int64_t vid, const void* x, cudaStream_t st);
   int get_host(int64_t vid, void* out) const;
   int get_rows_host(int64_t start, int64_t n, void* out) const;  // n x row_bytes, packed
-  // contiguous copy of the fp32 rows [0, n) (training slab, GetVectorHeader): returns device ptr, owned by `s`
+  // the rows [0, n) contiguous in device memory, stride() bytes apart (training slab, GetVectorHeader): the segment
+  // itself or a copy owned by `s`
   const float* contiguous(int64_t n, Scratch& s);
   // rows [start, start + n) (stride() bytes apart) into device memory at dst, ordered on st
   cudaError_t copy_rows_to_device(int64_t start, int64_t n, void* dst, cudaStream_t st) const;
@@ -220,11 +221,12 @@ class Index {
   // Engine::Update -> RawVector update + IndexModel::Update (search/engine.cc:774-850;
   // realtime_mem_data.cc:298-320: old entry tombstoned, vector re-appended to its new list)
   virtual int update_vector(int64_t vid, const void* x);  // x: one row of store().row_bytes() bytes
-  // IndexModel::Search (index_model.h:296): x = nq x d floats; out = nq x k, unfilled id -1.
-  // Returns 0, -1 on error (last_error), -2 if killed.  x/out pointers are host unless *_dev.
-  int search(const SearchContext& ctx, int nq, const float* x, int k, float* out_dis, int64_t* out_ids);
+  // IndexModel::Search (index_model.h:296): x = nq host rows of store().row_bytes() bytes (d floats; BINARYIVF: d / 8
+  // packed bytes); out = nq x k, unfilled id -1.  Returns 0, -1 on error (last_error), -2 if killed.
+  int search(const SearchContext& ctx, int nq, const void* x, int k, float* out_dis, int64_t* out_ids);
   // one H2D -> kernels -> D2H round trip on the calling thread's stream
-  int search_direct(const SearchContext& ctx, int nq, const float* x, int k, float* out_dis, int64_t* out_ids);
+  int search_direct(const SearchContext& ctx, int nq, const void* x, int k, float* out_dis, int64_t* out_ids);
+  // float queries already in device memory (nq rows of d floats, ldx floats apart), results left there, ordered on st.
   // out_keys_dev (optional): the nq x k result keys, (order-preserving score bits << 32) | vid, best first,
   // sentinel padded -- what the multi-GPU merge exchanges (one all-gather instead of scores + ids)
   int search_device(const SearchContext& ctx, int nq, const float* x_dev, int64_t ldx, int k, float* out_dis_dev,
@@ -245,10 +247,25 @@ class Index {
   const char* last_scan_info() const { return last_scan_info_; }  // JSON details of the last scan path (bench)
 
  protected:
-  // GammaFLATIndex::Search (gamma_index_flat.cc:130-370) over rows [0, nrows)
-  int flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
+  // Device queries, here and below: nq rows store().stride() bytes apart, zero padded (dpad floats; BINARYIVF: words).
+  // nq host rows of store().row_bytes() bytes as device queries in `s`; nullptr on failure (last_error set)
+  const void* upload_queries(int nq, const void* x, Scratch& s);
+  // the search behind every query entry point, with mu_ held shared: bitmaps, brute force or the index, the realtime
+  // tail; the nq x k result keys into *keys (allocated in s)
+  int search_keys(const SearchContext& ctx, int nq, const void* xq, int k, unsigned long long** keys, Scratch& s);
+  // the nq x k result keys decoded under `metric` into the host arrays; returns once they are there
+  int download_results(const unsigned long long* keys, int nq, int k, int metric, float* out_dis, int64_t* out_ids,
+                       Scratch& s);
+  // the metric a search ranks by: the retrieval parameters' metric_type, else the index's
+  virtual int search_metric(const SearchContext& ctx) const { return ctx.params.metric >= 0 ? ctx.params.metric : mp_.metric; }
+  // GammaFLATIndex::Search (gamma_index_flat.cc:130-370) over rows [row_begin, nrows)
+  int flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, int k,
                       int64_t nrows, unsigned long long* out_keys, Scratch& s, int64_t row_begin = 0);
-  virtual int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
+  // flat_search_dev's distance tile: scores [nq][ldo] of queries xq against m device rows (both store().stride() bytes
+  // apart), exact; names the scan's kernels in last_scan_kernel_
+  virtual cudaError_t flat_tile(const void* xq, int nq, const void* rows, int m, int metric, float* scores, int64_t ldo,
+                                cudaStream_t st);
+  virtual int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, int k,
                               unsigned long long* out_keys, Scratch& s) = 0;
   int upload_bitmaps(const SearchContext& ctx, FilterArgs* f, Scratch& s);
   // rows [vid0, vid0 + n) as device rows (store().stride() bytes apart): in HBM the segment itself (the rows must lie in
@@ -291,7 +308,7 @@ class Index {
   struct CoReq {
     const SearchContext* ctx;
     int nq, k;
-    const float* x;
+    const void* x;
     float* out_dis;
     int64_t* out_ids;
     int rc = 0;
@@ -358,7 +375,7 @@ class FlatIndex : public Index {
   }
 
  protected:
-  int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
+  int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, int k,
                       unsigned long long* out_keys, Scratch& s) override;
 };
 
@@ -402,10 +419,10 @@ class IvfIndex : public Index {
   int get_centroids(float* host) const;
   const char* last_coarse_kernel() const { return last_coarse_kernel_; }  // test hook: which coarse path ran last
   IvfLists* lists() { return lists_.get(); }
-  // quantizer->search (ivfflat.cc:568): top-nprobe lists per query
-  int coarse_search_host(int nq, const float* x, int nprobe, float* out_dis, int64_t* out_ids);
-  // search_preassigned with caller-provided (keys, coarse_dis): host in/out
-  int search_preassigned_host(const SearchContext& ctx, int nq, const float* x, int k, const int64_t* keys,
+  // quantizer->search (ivfflat.cc:568): top-nprobe lists per query; x: host rows as Index::search takes them
+  int coarse_search_host(int nq, const void* x, int nprobe, float* out_dis, int64_t* out_ids);
+  // search_preassigned with caller-provided (keys, coarse_dis): host in/out; coarse_dis may be null (zeros)
+  int search_preassigned_host(const SearchContext& ctx, int nq, const void* x, int k, const int64_t* keys,
                               const float* coarse_dis, int nprobe, float* out_dis, int64_t* out_ids);
   // re-pack the inverted lists into one tight slab (IvfLists::compact); also done automatically after
   // a bulk add_pending when more than half of the slab space is dead
@@ -424,12 +441,13 @@ class IvfIndex : public Index {
   virtual int64_t default_training_threshold() const = 0;
   // k-means of the coarse centroids (default: faiss ClusteringParameters)
   virtual KMeansParams coarse_kmeans_params() const { return KMeansParams(); }
-  int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, int k,
+  int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, int k,
                       unsigned long long* out_keys, Scratch& s) override;
-  int coarse_dev(int nq, const float* xq, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis, Scratch& s);
+  // the nprobe nearest lists of each query (after transform_dev)
+  virtual int coarse_dev(int nq, const void* xq, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis, Scratch& s);
   // xq: the queries after transform_dev; xq_raw: the same queries untransformed (the exact re-rank reads the raw store)
-  virtual int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq,
-                       const float* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
+  virtual int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq,
+                       const void* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
                        unsigned long long* out_keys, Scratch& s) = 0;
   // List-major pair grouping (launch_lmk_group): the (query, probe) pairs grouped by list, `group` pairs per group, each
   // group cut into nseg row segments.  Items, pair order and totals are left in `s` for the list-major kernels.
@@ -493,7 +511,7 @@ class IVFFlatIndex : public IvfIndex {
  protected:
   GammaFileFormat gamma_format() const override;
   int64_t default_training_threshold() const override { return (int64_t)nlist_ * 200; }  // gamma_index_ivfflat.cc:239
-  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, const float* xq_raw, int k,
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, const void* xq_raw, int k,
                const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
                Scratch& s) override;
   // list-major IVF-Flat scan on the tensor cores (kernels_tc.cu); returns 1 if not applicable
@@ -589,7 +607,7 @@ class IVFPQIndex : public IvfPqBase {
   GammaFileFormat gamma_format() const override;
   int64_t default_training_threshold() const override;
   KMeansParams coarse_kmeans_params() const override;
-  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, const float* xq_raw, int k,
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, const void* xq_raw, int k,
                const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
                Scratch& s) override;
   void reset_codec() override { opq_trained_ = false; }
@@ -657,7 +675,7 @@ class IVFPQFastScanIndex : public IvfPqBase {
   int coarse_metric(int metric) const override { (void)metric; return kMetricL2; }
   cudaError_t encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st) override;
   int train_extra(const float* xtrain, int64_t n, Scratch& s) override;
-  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, const float* xq_raw, int k,
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, const void* xq_raw, int k,
                const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
                Scratch& s) override;
 };
@@ -665,8 +683,9 @@ class IVFPQFastScanIndex : public IvfPqBase {
 // GammaIndexBinaryIVF (index/impl/gamma_index_binary_ivf.{h,cc}): faiss::IndexBinaryIVF over packed binary rows of
 // d / 8 bytes (d in bits), compared by Hamming distance, smaller first.  The coarse centroids are trained by faiss
 // Clustering on the rows expanded to +-1 floats (binary_to_real), kept as floats in d_centroids_ and packed again
-// (real_to_binary) for the coarse quantiser; list entries are the raw d / 8 bytes.  Rows and queries cross this class
-// as packed bytes only: its float entry points (Index::search, coarse_search_host, ...) are refused.
+// (real_to_binary) for the coarse quantiser; list entries are the raw d / 8 bytes.  Rows and queries are packed bytes
+// (store().row_bytes()), searched through the shared entry points: Index::search, coarse_search_host,
+// search_preassigned_host.
 class BinaryIvfIndex : public IvfIndex {
  public:
   static constexpr int kDefaultNlist = 256;   // BinaryModelParams() (gamma_index_binary_ivf.cc:23)
@@ -675,40 +694,32 @@ class BinaryIvfIndex : public IvfIndex {
   ~BinaryIvfIndex() override;
   int code_bytes() const override { return cb_; }
   bool persists_trained_state() const override { return false; }
-  int train() override;
   int64_t index_mem_bytes() const override;
-  // x: nq x d / 8 bytes on host; out: nq x k, integer distances as floats, unfilled id -1
-  int search_codes(const SearchContext& ctx, int nq, const uint8_t* x, int k, float* out_dis, int64_t* out_ids);
   // packed centroids [nlist][d / 8] (set_binary_centroids marks the index trained)
   int set_binary_centroids(const uint8_t* host, int nlist);
   int get_binary_centroids(uint8_t* host) const;
-  int coarse_search_codes(int nq, const uint8_t* x, int nprobe, float* out_dis, int64_t* out_ids);
-  int search_preassigned_codes(const SearchContext& ctx, int nq, const uint8_t* x, int k, const int64_t* keys, int nprobe,
-                               float* out_dis, int64_t* out_ids);
 
  protected:
   GammaFileFormat gamma_format() const override { return GammaFileFormat(); }  // Dump writes nothing
   int64_t default_training_threshold() const override { return (int64_t)nlist_ * 39; }  // nlist * min_points_per_centroid
+  KMeansParams coarse_kmeans_params() const override;
+  const float* train_transform(const float* xt, int64_t n, Scratch& s) override;
+  int centroids_changed(cudaStream_t st) override;
+  // Hamming distances rank like L2, whatever metric_type the retrieval parameters carry
+  int search_metric(const SearchContext& ctx) const override { (void)ctx; return kMetricL2; }
+  cudaError_t flat_tile(const void* xq, int nq, const void* rows, int m, int metric, float* scores, int64_t ldo,
+                        cudaStream_t st) override;
+  int coarse_dev(int nq, const void* xq, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis, Scratch& s) override;
   int assign_batch(const void* x, int64_t n, const void** xc, int32_t* out, Scratch& s) override;
   int append_batch(const void* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
                    const std::vector<int>& add, Scratch& s) override;
-  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* xq, const float* xq_raw, int k,
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, const void* xq_raw, int k,
                const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
                Scratch& s) override;
 
  private:
-  // the k nearest of rows [0, m) (ldr words apart, ids id_base + row) for nq queries (ldq words apart), filtered:
-  // out_keys[q * out_stride ..], sorted
-  int hamming_topk(const uint32_t* xq, int64_t ldq, int nq, const uint32_t* rows, int64_t ldr, int m, int64_t id_base, int k,
-                   const FilterArgs& f, unsigned long long* out_keys, int64_t out_stride, Scratch& s);
-  // brute force over the stored rows [row_begin, row_end)
-  int flat_codes(const FilterArgs& f, int nq, const uint32_t* xq, int k, int64_t row_begin, int64_t row_end,
-                 unsigned long long* out_keys, Scratch& s);
-  int coarse_codes(int nq, const uint32_t* xq, int nprobe, int32_t* probe_ids, float* coarse_dis, Scratch& s);
-  int scan_codes(const FilterArgs& f, int nq, const uint32_t* xq, int k, const int32_t* probe_ids, int nprobe,
-                 unsigned long long* out_keys, Scratch& s);
-  const uint32_t* upload_queries(int nq, const uint8_t* x, Scratch& s);
-  int finish_host(const unsigned long long* keys, int nq, int k, float* out_dis, int64_t* out_ids, cudaStream_t st);
+  // the k Hamming-nearest lists of nq device rows (ldw_ words apart), the smaller list id among equals: keys [nq][k], sorted
+  int hamming_topk(const uint32_t* xq, int nq, int k, unsigned long long* keys, Scratch& s);
   int cb_;             // bytes per row, d / 8
   int64_t ldw_;        // words between device rows (the raw store's stride)
   uint8_t* d_bcent_ = nullptr;  // [nlist][4 ldw_] packed centroids

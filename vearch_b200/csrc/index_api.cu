@@ -151,6 +151,14 @@ static T* as(gb_index* index) {
   return index && index->impl ? dynamic_cast<T*>(index->impl) : nullptr;
 }
 
+// A BINARYIVF index stores and searches packed binary rows: every entry point taking or returning float rows, queries or
+// centroids refuses it (the _binary ones serve it)
+static bool packed_binary(gb_index* index) {
+  if (!as<BinaryIvfIndex>(index)) return false;
+  set_last_error("BINARYIVF: rows, queries and centroids are packed binary; use the _binary entry points");
+  return true;
+}
+
 extern "C" {
 
 const char* gb_last_error(void) { return last_error(); }
@@ -188,29 +196,29 @@ void gb_index_destroy(gb_index* index) {
 
 int gb_index_add_vectors(gb_index* index, int64_t n, const float* x) {
   IDX_OR_FAIL(index);
-  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
+  if (packed_binary(index)) return -1;
   return index->impl->add_vectors(x, n);
 }
 int gb_index_add_vectors_device(gb_index* index, int64_t n, const float* x_dev, int64_t ld) {
   IDX_OR_FAIL(index);
-  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
+  if (packed_binary(index)) return -1;
   return index->impl->add_vectors_device(x_dev, ld, n);
 }
 int gb_index_update_vector(gb_index* index, int64_t vid, const float* x) {
   IDX_OR_FAIL(index);
-  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
+  if (packed_binary(index)) return -1;
   cudaSetDevice(index->impl->device());
   return index->impl->update_vector(vid, x);  // RawVector update + IndexModel::Update
 }
 int gb_index_get_vector(gb_index* index, int64_t vid, float* out) {
   IDX_OR_FAIL(index);
-  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
+  if (packed_binary(index)) return -1;
   cudaSetDevice(index->impl->device());
   return index->impl->store().get_host(vid, out);
 }
 int gb_index_get_vectors(gb_index* index, int64_t start, int64_t n, float* out) {
   IDX_OR_FAIL(index);
-  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
+  if (packed_binary(index)) return -1;
   cudaSetDevice(index->impl->device());
   return index->impl->store().get_rows_host(start, n, out);
 }
@@ -238,6 +246,7 @@ int gb_index_search(gb_index* index, int nq, const float* x, int k, const char* 
                     const uint8_t* del_bitmap, const uint8_t* filter_bitmap, int64_t bitmap_bits, float min_score,
                     float max_score, float* out_scores, int64_t* out_ids) {
   IDX_OR_FAIL(index);
+  if (packed_binary(index)) return -1;
   SearchContext ctx;
   if (fill_ctx(&ctx, retrieval_params_json, brute_force, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score))
     return -1;
@@ -248,6 +257,7 @@ int gb_index_search_device(gb_index* index, int nq, const float* x_dev, int64_t 
                            const char* retrieval_params_json, int brute_force, float* out_scores_dev,
                            int64_t* out_ids_dev, void* stream) {
   IDX_OR_FAIL(index);
+  if (packed_binary(index)) return -1;
   SearchContext ctx;
   if (fill_ctx(&ctx, retrieval_params_json, brute_force, nullptr, nullptr, 0, -3.4028235e38f, 3.4028235e38f)) return -1;
   return index->impl->search_device(ctx, nq, x_dev, ld, k, out_scores_dev, out_ids_dev,
@@ -258,6 +268,7 @@ int gb_index_search_device_keys(gb_index* index, int nq, const float* x_dev, int
                                 const char* retrieval_params_json, int brute_force, unsigned long long* out_keys_dev,
                                 float* out_scores_dev, int64_t* out_ids_dev, void* stream) {
   IDX_OR_FAIL(index);
+  if (packed_binary(index)) return -1;
   SearchContext ctx;
   if (fill_ctx(&ctx, retrieval_params_json, brute_force, nullptr, nullptr, 0, -3.4028235e38f, 3.4028235e38f)) return -1;
   return index->impl->search_device(ctx, nq, x_dev, ld, k, out_scores_dev, out_ids_dev, static_cast<cudaStream_t>(stream),
@@ -308,12 +319,12 @@ int gb_index_nlist(gb_index* index) {
 }
 int gb_index_set_centroids(gb_index* index, const float* centroids, int nlist) {
   IVF_OR_FAIL(ivf, index);
-  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
+  if (packed_binary(index)) return -1;
   return ivf->set_centroids(centroids, nlist);
 }
 int gb_index_get_centroids(gb_index* index, float* centroids) {
   IVF_OR_FAIL(ivf, index);
-  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
+  if (packed_binary(index)) return -1;
   return ivf->get_centroids(centroids);
 }
 int gb_index_pq_m(gb_index* index) {
@@ -418,7 +429,7 @@ int gb_index_tombstone(gb_index* index, int list, int pos) {
 }
 int gb_index_coarse_search(gb_index* index, int nq, const float* x, int nprobe, float* out_dis, int64_t* out_ids) {
   IVF_OR_FAIL(ivf, index);
-  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
+  if (packed_binary(index)) return -1;
   return ivf->coarse_search_host(nq, x, nprobe, out_dis, out_ids);
 }
 int gb_index_search_preassigned(gb_index* index, int nq, const float* x, int k, const int64_t* keys,
@@ -426,7 +437,7 @@ int gb_index_search_preassigned(gb_index* index, int nq, const float* x, int k, 
                                 const uint8_t* del_bitmap, const uint8_t* filter_bitmap, int64_t bitmap_bits,
                                 float min_score, float max_score, float* out_scores, int64_t* out_ids) {
   IVF_OR_FAIL(ivf, index);
-  if (as<BinaryIvfIndex>(index)) return set_last_error("BINARYIVF: use the _binary entry points"), -1;
+  if (packed_binary(index)) return -1;
   SearchContext ctx;
   if (fill_ctx(&ctx, retrieval_params_json, 0, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score)) return -1;
   return ivf->search_preassigned_host(ctx, nq, x, k, keys, coarse_dis, nprobe, out_scores, out_ids);
@@ -459,7 +470,7 @@ int gb_index_search_binary(gb_index* index, int nq, const uint8_t* x, int k, con
   if (fill_ctx(&ctx, retrieval_params_json, brute_force, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score))
     return -1;
   ctx.search_unindexed_tail = search_unindexed_tail != 0;
-  return b->search_codes(ctx, nq, x, k, out_scores, out_ids);
+  return b->search(ctx, nq, x, k, out_scores, out_ids);
 }
 int gb_index_set_binary_centroids(gb_index* index, const uint8_t* centroids, int nlist) {
   BIN_OR_FAIL(b, index);
@@ -475,7 +486,7 @@ int gb_index_get_real_centroids(gb_index* index, float* centroids) {
 }
 int gb_index_coarse_search_binary(gb_index* index, int nq, const uint8_t* x, int nprobe, float* out_dis, int64_t* out_ids) {
   BIN_OR_FAIL(b, index);
-  return b->coarse_search_codes(nq, x, nprobe, out_dis, out_ids);
+  return b->coarse_search_host(nq, x, nprobe, out_dis, out_ids);
 }
 int gb_index_search_preassigned_binary(gb_index* index, int nq, const uint8_t* x, int k, const int64_t* keys, int nprobe,
                                        const uint8_t* del_bitmap, const uint8_t* filter_bitmap, int64_t bitmap_bits,
@@ -483,7 +494,7 @@ int gb_index_search_preassigned_binary(gb_index* index, int nq, const uint8_t* x
   BIN_OR_FAIL(b, index);
   SearchContext ctx;
   if (fill_ctx(&ctx, "", 0, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score)) return -1;
-  return b->search_preassigned_codes(ctx, nq, x, k, keys, nprobe, out_scores, out_ids);
+  return b->search_preassigned_host(ctx, nq, x, k, keys, nullptr, nprobe, out_scores, out_ids);
 }
 
 int gb_kmeans(int device, const float* x, int64_t n, int d, int k, int niter, int64_t seed, int spherical,

@@ -242,6 +242,7 @@ cudaError_t launch_ivfpqfs_scan(const uint8_t* lut8, const float* ab, int nq, co
 // ---- K12: BINARYIVF (kernels_binary.cu): packed binary rows, Hamming distance on the CUDA cores ---------------------
 // out[q][r] = popcount(Q_q ^ R_r) over `words` 32-bit words (rows zero padded to whole words; strides in words), exact
 // integers as fp32.  Used for every query x rows job: coarse search (rows = centroids), add-time assignment, brute force.
+constexpr int kHammingTileMaxQueries = 65535 * 16;  // queries of one launch: grid.y of 16-query tiles
 cudaError_t launch_hamming_tile(const uint32_t* Q, int64_t ldq, int nq, const uint32_t* R, int64_t ldr, int m, int words,
                                 float* out, int64_t ldo, cudaStream_t st);
 // faiss binary_to_real / real_to_binary: bit j of a packed row (byte j >> 3, bit j & 7) <-> +1 / -1 (a float > 0 is 1)

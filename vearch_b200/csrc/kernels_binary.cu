@@ -135,7 +135,8 @@ int64_t blocks_of(int64_t n, int nt) { return (n + nt - 1) / nt; }
 cudaError_t launch_hamming_tile(const uint32_t* Q, int64_t ldq, int nq, const uint32_t* R, int64_t ldr, int m, int words,
                                 float* out, int64_t ldo, cudaStream_t st) {
   if (nq <= 0 || m <= 0) return cudaSuccess;
-  if (words <= 0 || nq > 65535 * HT_QB) return cudaErrorInvalidValue;
+  static_assert(kHammingTileMaxQueries == 65535 * HT_QB, "one launch: at most 65535 query tiles");
+  if (words <= 0 || nq > kHammingTileMaxQueries) return cudaErrorInvalidValue;
   dim3 grid((unsigned)blocks_of(m, HT_ROWS), (unsigned)blocks_of(nq, HT_QB));
   hamming_tile_kernel<<<grid, HT_ROWS, 0, st>>>(Q, ldq, nq, R, ldr, m, words, out, ldo);
   note_launch();
