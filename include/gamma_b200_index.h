@@ -169,6 +169,14 @@ int gb_index_pq_encode(gb_index *index, int64_t n, const float *x, const int64_t
    the low nibble of byte j.  The uint8 look-up tables of a query batch: lut8 = nq x M x 16, ab = nq x (a, b), the
    score of an entry being accu * (1/a) + b; metric -1 = the index metric. */
 int gb_index_pqfs_lut(gb_index *index, int nq, const float *x, int metric, uint8_t *lut8, float *ab);
+/* IVFRABITQ (DESIGN.md section 3, K13): the model's nb_bits and qb; list entries of n rows assigned to lists `assign`
+   (n x code_size bytes: nb_bits bit-planes of ceil(d / 32) words, sign plane first, then the fp32 factors |r|^2, f, S);
+   the scan's estimate of every entry of list lists[j] for query j, the lists' entries one after another in out, under
+   qb in [0, 8] and metric (-1 = the index metric) */
+int gb_index_rabitq_nb_bits(gb_index *index);
+int gb_index_rabitq_qb(gb_index *index);
+int gb_index_rabitq_encode(gb_index *index, int64_t n, const float *x, const int64_t *assign, uint8_t *codes);
+int gb_index_rabitq_estimate(gb_index *index, int nq, const float *x, const int64_t *lists, int qb, int metric, float *out);
 
 /* ---- standalone kernels exposed for tests / bench ---- */
 /* faiss Clustering restated (k-means), host in/out; obj (niter floats) may be NULL */

@@ -323,7 +323,8 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     return Status::Make(kNotSupported, vec_name_ + ": BINARYIVF is not supported in a multi-vector table");
   Index* idx = create_index(index_type_, dim_, mp, device_, 20);
   if (!idx) return Status::Make(index_type_ == "FLAT" || index_type_ == "IVFFLAT" || index_type_ == "IVFPQ" ||
-                                        index_type_ == "IVFPQFastScan" || index_type_ == "BINARYIVF"
+                                        index_type_ == "IVFPQFastScan" || index_type_ == "BINARYIVF" ||
+                                        index_type_ == "IVFRABITQ"
                                     ? kInvalidArgument
                                     : kNotSupported,
                                 last_error());

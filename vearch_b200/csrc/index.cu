@@ -879,7 +879,8 @@ bool Index::coalescable(const SearchContext& ctx, int nq) const {
 static bool same_signature(const SearchContext& a, int ka, const SearchContext& b, int kb) {
   return ka == kb && a.min_score == b.min_score && a.max_score == b.max_score && a.params.nprobe == b.params.nprobe &&
          a.params.metric == b.params.metric && a.params.recall_num == b.params.recall_num &&
-         a.params.brute_force == b.params.brute_force && a.search_unindexed_tail == b.search_unindexed_tail;
+         a.params.brute_force == b.params.brute_force && a.search_unindexed_tail == b.search_unindexed_tail &&
+         a.params.qb == b.params.qb;
 }
 
 void Index::coalesce_loop() {
@@ -2365,10 +2366,11 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
 }
 
 // Metric check, ADC depth, query-major list scan + merge of its CTA groups, exact re-rank
-int IvfPqBase::scan_pq_dev(const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric, int nq,
-                           const float* rerank_xq, int k, int nprobe, int max_kk, unsigned long long* out_keys, Scratch& s,
-                           const std::function<int(int, unsigned long long*, bool)>& prepare,
-                           const std::function<cudaError_t(int, int, unsigned long long*)>& launch) {
+int IvfIndex::scan_query_major_dev(const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric, int nq,
+                                   const float* rerank_xq, int k, int nprobe, int max_kk, const std::string& limit_at,
+                                   unsigned long long* out_keys, Scratch& s,
+                                   const std::function<int(int, unsigned long long*, bool)>& prepare,
+                                   const std::function<cudaError_t(int, int, unsigned long long*)>& launch) {
   cudaStream_t st = s.stream();
   if (metric != mp_.metric) {
     set_last_error(type_ + ": per-request metric must equal the trained metric");
@@ -2379,7 +2381,7 @@ int IvfPqBase::scan_pq_dev(const char* kernel, const SearchContext& ctx, const F
   const int kk = std::max(k, ctx.params.recall_num);
   if (kk > max_kk) {
     set_last_error(type_ + ": recall_num / topn [" + std::to_string(kk) + "] above " + std::to_string(max_kk) +
-                   " is not supported by this engine at nsubvector " + std::to_string(M_));
+                   " is not supported by this engine at " + limit_at);
     return -1;
   }
   unsigned long long* keys = out_keys;
@@ -2443,9 +2445,9 @@ int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metr
                              partial, st);
   };
   // "for opq, rerank need raw vector" (gamma_index_ivfpq.cc:735): original queries against the raw store
-  return scan_pq_dev(nbits_ < 8 ? "ivfpq_packed_scan_kernel" : "ivfpq_scan_kernel", ctx, f, metric, nq,
-                     static_cast<const float*>(xq_raw), k, nprobe,
-                     ivfpq_scan_max_k(M_, nbits_), out_keys, s, prepare, launch);
+  return scan_query_major_dev(nbits_ < 8 ? "ivfpq_packed_scan_kernel" : "ivfpq_scan_kernel", ctx, f, metric, nq,
+                              static_cast<const float*>(xq_raw), k, nprobe, ivfpq_scan_max_k(M_, nbits_),
+                              "nsubvector " + std::to_string(M_), out_keys, s, prepare, launch);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2507,8 +2509,8 @@ int IVFPQFastScanIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, 
   auto launch = [&](int kk, int pg, unsigned long long* partial) {
     return launch_ivfpqfs_scan(lut, ab, nq, probe_ids, nprobe, pg, lists_->directory(), M_, kk, metric, f, partial, st);
   };
-  return scan_pq_dev("ivfpqfs_scan_kernel", ctx, f, metric, nq, static_cast<const float*>(xq_raw), k, nprobe, 4096, out_keys, s,
-                     prepare, launch);
+  return scan_query_major_dev("ivfpqfs_scan_kernel", ctx, f, metric, nq, static_cast<const float*>(xq_raw), k, nprobe, 4096,
+                              "nsubvector " + std::to_string(M_), out_keys, s, prepare, launch);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2662,6 +2664,122 @@ int BinaryIvfIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int 
 }
 
 // ------------------------------------------------------------------------------------------
+// GammaIVFRABITQIndex (gamma_index_ivfrabitq.cc)
+int64_t RaBitQIndex::default_training_threshold() const {  // gamma_index_ivfrabitq.cc:69-76, as IVFPQ
+  return std::max<int64_t>((int64_t)nlist_ * 200, 256);
+}
+// gamma_index_ivfrabitq.cc:80-120: IndexFlat quantiser under the index metric, niter 10, spherical for IP.  faiss's
+// RaBitQuantizer::train [faiss-restated, not verifiable here] learns nothing, so the coarse centroids are the whole model.
+KMeansParams RaBitQIndex::coarse_kmeans_params() const {
+  KMeansParams kp;
+  kp.niter = 10;
+  kp.spherical = mp_.metric == kMetricIP;
+  return kp;
+}
+
+// by_residual: each row's code is of its residual to the list it was assigned to
+int RaBitQIndex::append_batch(const void* xv, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                              const std::vector<int>& add, Scratch& s) {
+  (void)add;
+  cudaStream_t st = s.stream();
+  const int cb = code_bytes();
+  GB_ALLOC(codes, uint8_t, (size_t)n * cb, s);
+  GB_CUDA(launch_rabitq_encode(static_cast<const float*>(xv), dpad_, n, d_list, d_centroids_, dpad_, d_, nb_bits_, codes, st));
+  GB_CUDA(launch_ivf_append_codes(codes, n, cb, d_list, d_pos, reinterpret_cast<uint8_t* const*>(lists_->d_data()),
+                                  lists_->d_ids(), vid0, st));
+  return 0;
+}
+
+int RaBitQIndex::encode_host(const float* x, int64_t n, const int64_t* assign, uint8_t* codes_out) {
+  std::shared_lock<std::shared_mutex> lk(mu_);  // the centroids stay put while the rows are encoded against them
+  if (!trained_) {
+    set_last_error("IVFRABITQ: encode needs trained centroids");
+    return -1;
+  }
+  cudaSetDevice(device_);
+  cudaStream_t st = thread_stream(device_);
+  Scratch s(st);
+  const int cb = code_bytes();
+  GB_ALLOC(dx, float, (size_t)n * dpad_, s);
+  GB_CUDA(upload_rows_padded(dx, x, n, d_, dpad_, st));
+  std::vector<int32_t> h(assign, assign + n);
+  for (int32_t l : h)
+    if (l < 0 || l >= nlist_) {
+      set_last_error("IVFRABITQ: list id out of range");
+      return -1;
+    }
+  GB_ALLOC(da, int32_t, n, s);
+  GB_CUDA(cudaMemcpyAsync(da, h.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  GB_ALLOC(codes, uint8_t, (size_t)n * cb, s);
+  GB_CUDA(launch_rabitq_encode(dx, dpad_, n, da, d_centroids_, dpad_, d_, nb_bits_, codes, st));
+  GB_CUDA(cudaMemcpyAsync(codes_out, codes, (size_t)n * cb, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int RaBitQIndex::estimate_host(int nq, const float* x, const int64_t* lists, int qb, int metric, float* out) {
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  if (!trained_ || !lists_) {
+    set_last_error("IVFRABITQ: estimate needs a trained index");
+    return -1;
+  }
+  if (qb < 0 || qb > 8) {
+    set_last_error("IVFRABITQ: qb must be in [0, 8]");
+    return -1;
+  }
+  cudaSetDevice(device_);
+  cudaStream_t st = thread_stream(device_);
+  Scratch s(st);
+  std::vector<int32_t> qo(nq), lo(nq);
+  std::vector<int64_t> off(nq);
+  int64_t total = 0;
+  for (int j = 0; j < nq; j++) {
+    if (lists[j] < 0 || lists[j] >= nlist_) {
+      set_last_error("IVFRABITQ: list id out of range");
+      return -1;
+    }
+    qo[j] = j;
+    lo[j] = (int32_t)lists[j];
+    off[j] = total;
+    total += lists_->lens()[lists[j]];
+  }
+  GB_ALLOC(dx, float, (size_t)nq * dpad_, s);
+  GB_CUDA(upload_rows_padded(dx, x, nq, d_, dpad_, st));
+  GB_ALLOC(dq, int32_t, nq, s);
+  GB_ALLOC(dl, int32_t, nq, s);
+  GB_ALLOC(doff, int64_t, nq, s);
+  GB_ALLOC(dout, float, total + 1, s);
+  GB_CUDA(cudaMemcpyAsync(dq, qo.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaMemcpyAsync(dl, lo.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaMemcpyAsync(doff, off.data(), (size_t)nq * 8, cudaMemcpyHostToDevice, st));
+  GB_CUDA(launch_rabitq_estimate(dx, dpad_, d_centroids_, dpad_, d_, nb_bits_, qb, metric, lists_->directory(), dq, dl, doff, nq,
+                                 dout, st));
+  GB_CUDA(cudaMemcpyAsync(out, dout, (size_t)total * 4, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// IVFRaBitQ search_preassigned over this engine's lists (gamma_index_ivfrabitq.cc:553-633): the estimator scan selects the
+// k' = max(k, recall_num) best estimates, filters applied before selection; recall_num > 0 re-ranks them exactly from the
+// raw vectors, otherwise the estimates are the scores
+int RaBitQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xqv, const void* xq_raw,
+                          int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
+                          Scratch& s) {
+  (void)xq_raw;      // no transform
+  (void)coarse_dis;  // dis0 is recomputed by the scan in its own fixed order
+  const float* xq = static_cast<const float*>(xqv);
+  const int qb = (ctx.params.qb >= 0 && ctx.params.qb <= 8) ? ctx.params.qb : qb_;  // gamma_index_ivfrabitq.cc:215-223
+  auto prepare = [&](int, unsigned long long*, bool) { return 1; };  // the scan forms its tables per (query, list)
+  auto launch = [&](int kk, int pg, unsigned long long* partial) {
+    snprintf(last_scan_info_, sizeof(last_scan_info_), "{\"probes_per_cta\": %d, \"qb\": %d}", pg, qb);
+    return launch_rabitq_scan(xq, dpad_, nq, d_centroids_, dpad_, d_, nb_bits_, qb, probe_ids, nprobe, pg, lists_->directory(),
+                              kk, metric, f, partial, s.stream());
+  };
+  return scan_query_major_dev("rabitq_scan_kernel", ctx, f, metric, nq, xq, k, nprobe, rabitq_scan_max_k(d_, nb_bits_, qb),
+                              "dimension " + std::to_string(d_), out_keys, s, prepare, launch);
+}
+
+// ------------------------------------------------------------------------------------------
 Index* create_index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
@@ -2762,6 +2880,33 @@ Index* create_index(const std::string& type, int d, const ModelParams& mp, int d
       return nullptr;
     }
     return new BinaryIvfIndex(d, bmp, device, seg_shift);
+  }
+  if (type == "IVFRABITQ") {  // IVFRABITQModelParams::Parse / Validate (gamma_index_ivfrabitq.h:370-510)
+    if (mp.nb_bits < 1 || mp.nb_bits > 9) {
+      set_last_error("invalid nb_bits =" + std::to_string(mp.nb_bits) + " should be integer in [1, 9]");
+      return nullptr;
+    }
+    if (mp.qb < 0 || mp.qb > 8) {
+      set_last_error("invalid qb =" + std::to_string(mp.qb) + " should be integer in [0, 8]");
+      return nullptr;
+    }
+    if (mp.ncentroids <= 0 || mp.nprobe > mp.ncentroids) {
+      set_last_error("nprobe should be less than ncentroids");
+      return nullptr;
+    }
+    if (d > kRabitqMaxDim) {
+      set_last_error("IVFRABITQ: dimension [" + std::to_string(d) + "] above " + std::to_string(kRabitqMaxDim) +
+                     " is not supported by this engine");
+      return nullptr;
+    }
+    // the scan's shared memory (stages, the k' queue, the qb = 8 table) must admit k' = 4096 (the lane rule of
+    // kernels_rabitq.cu makes it so for every accepted (d, nb_bits)); refused here rather than at every search
+    if (rabitq_scan_max_k(d, mp.nb_bits, 8) < 4096) {
+      set_last_error("IVFRABITQ: dimension [" + std::to_string(d) + "] at nb_bits " + std::to_string(mp.nb_bits) +
+                     " is too large for the list scan of this engine");
+      return nullptr;
+    }
+    return new RaBitQIndex(d, mp, device, seg_shift);
   }
   set_last_error("unsupported index type " + type);
   return nullptr;

@@ -175,6 +175,8 @@ struct ModelParams {  // index/impl/gamma_index_ivfpq.h:1031-1257, gamma_index_i
   int bbs = 32;                 // IVFPQFastScan block size as given (gamma_index_ivfpqfs.h:126-133; <= 0 => 32)
   bool host_store = false;      // raw vectors in pinned host memory (store_type "RocksDB"); otherwise in HBM
   int ncentroids_arg = 0;       // "ncentroids" as given, 0 if absent (BINARYIVF has its own default and range check)
+  int nb_bits = 4;              // IVFRABITQ bits per dimension as given (validated by create_index: [1, 9])
+  int qb = 4;                   // IVFRABITQ query bits as given (validated by create_index: [0, 8])
 };
 
 struct RetrievalParams {  // gamma_index_ivfpq.cc:233-294, gamma_index_ivfflat.cc:293-340
@@ -183,6 +185,8 @@ struct RetrievalParams {  // gamma_index_ivfpq.cc:233-294, gamma_index_ivfflat.c
   int recall_num = -1;
   int parallel_on_queries = 1;
   bool brute_force = false;
+  int qb = -1;            // IVFRABITQ query bits, -1 => the index's (a value outside [0, 8] falls back to it)
+  bool centered = false;  // IVFRABITQ: parsed, no effect (the estimate already centres the query on the list)
 };
 
 struct SearchContext {  // RetrievalContext / SearchCondition (common/gamma_common_data.h:33-121)
@@ -449,6 +453,17 @@ class IvfIndex : public Index {
   virtual int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq,
                        const void* xq_raw, int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe,
                        unsigned long long* out_keys, Scratch& s) = 0;
+  // scan_dev of the estimating codecs (IVFPQ, IVFPQFastScan, IVFRABITQ) through the query-major list scan, with the
+  // recall_num / re-rank semantics of gamma_index_ivfpq.cc:764-770: the k' = max(k, recall_num) best estimates, re-ranked
+  // exactly from the raw vectors (rerank_xq) when recall_num > 0.  `prepare(kk, keys, need_sorted)` builds the per-query
+  // tables and may serve the scan another way (0 = served, 1 = not, < 0 = error); `launch(kk, pg, partial)` launches the
+  // scan kernel, named `kernel`, over pg probes per CTA; max_kk: the largest k' it selects, `limit_at` names what bounds
+  // it in the error ("nsubvector 16")
+  int scan_query_major_dev(const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric, int nq,
+                           const float* rerank_xq, int k, int nprobe, int max_kk, const std::string& limit_at,
+                           unsigned long long* out_keys, Scratch& s,
+                           const std::function<int(int, unsigned long long*, bool)>& prepare,
+                           const std::function<cudaError_t(int, int, unsigned long long*)>& launch);
   // List-major pair grouping (launch_lmk_group): the (query, probe) pairs grouped by list, `group` pairs per group, each
   // group cut into nseg row segments.  Items, pair order and totals are left in `s` for the list-major kernels.
   struct LmGrouping {
@@ -577,14 +592,6 @@ class IvfPqBase : public IvfIndex {
                    const std::vector<int>& add, Scratch& s) override;
   // faiss ProductQuantizer::train on n rows (stride dpad): M independent ksub-means on the dsub-wide slices
   int train_codebook(const float* x, int64_t n, Scratch& s);
-  // scan_dev of the PQ-coded indexes through the query-major list scan: `prepare(kk, keys, need_sorted)` builds the
-  // per-query tables and may serve the scan another way (0 = served, 1 = not, < 0 = error); `launch(kk, pg, partial)`
-  // launches the scan kernel, named `kernel`, over pg probes per CTA; max_kk: the largest ADC depth it selects
-  int scan_pq_dev(const char* kernel, const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const float* rerank_xq,
-                  int k, int nprobe, int max_kk, unsigned long long* out_keys, Scratch& s,
-                  const std::function<int(int, unsigned long long*, bool)>& prepare,
-                  const std::function<cudaError_t(int, int, unsigned long long*)>& launch);
-
   int M_, dsub_, ksub_;
   float* d_pq_ = nullptr;  // [M][ksub][dsub]
 };
@@ -723,6 +730,37 @@ class BinaryIvfIndex : public IvfIndex {
   int cb_;             // bytes per row, d / 8
   int64_t ldw_;        // words between device rows (the raw store's stride)
   uint8_t* d_bcent_ = nullptr;  // [nlist][4 ldw_] packed centroids
+};
+
+// GammaIVFRABITQIndex (index/impl/gamma_index_ivfrabitq.{h,cc}): IVF with by_residual = true and a multi-bit RaBitQ code
+// of each residual (kernels_rabitq.cu, DESIGN.md §3 K13).  The coarse quantiser is exact under the index metric (an
+// "hnsw" object is accepted and ignored).  recall_num > 0 re-ranks the estimated candidates exactly from the raw vectors.
+class RaBitQIndex : public IvfIndex {
+ public:
+  RaBitQIndex(int d, const ModelParams& mp, int device, int seg_shift)
+      : IvfIndex("IVFRABITQ", d, mp, device, seg_shift), nb_bits_(mp.nb_bits), qb_(mp.qb) {}
+  int code_bytes() const override { return rabitq_code_bytes(d_, nb_bits_); }
+  bool persists_trained_state() const override { return false; }
+  int nb_bits() const { return nb_bits_; }
+  int qb() const { return qb_; }
+  // test hooks: list entries of n host rows assigned to lists `assign`; the scan's estimates of every entry of list
+  // lists[j] for query j (out: the lists' entries one after another), under `metric` and `qb`
+  int encode_host(const float* x, int64_t n, const int64_t* assign, uint8_t* codes_out);
+  int estimate_host(int nq, const float* x, const int64_t* lists, int qb, int metric, float* out);
+
+ protected:
+  // the reference dumps no usable file here: a loaded table trains and fills this index again from its raw vectors
+  GammaFileFormat gamma_format() const override { return GammaFileFormat(); }
+  int64_t default_training_threshold() const override;
+  KMeansParams coarse_kmeans_params() const override;
+  int append_batch(const void* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                   const std::vector<int>& add, Scratch& s) override;
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, const void* xq_raw, int k,
+               const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
+               Scratch& s) override;
+
+ private:
+  int nb_bits_, qb_;
 };
 
 // host rows n x d (stride d) -> device rows n x dpad, the padding columns zeroed

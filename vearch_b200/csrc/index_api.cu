@@ -88,6 +88,9 @@ bool parse_model_params(const std::string& text, ModelParams* mp, std::string* e
   // IVFPQFastScan only (validated by create_index): the reference's bbs-blocked list layout never leaves its process, so
   // the block size has no effect here beyond being checked
   if (jv.get_int("bbs", &v)) mp->bbs = v;
+  // IVFRABITQ only (validated by create_index, gamma_index_ivfrabitq.h:392-410)
+  if (jv.get_int("nb_bits", &v)) mp->nb_bits = v;
+  if (jv.get_int("qb", &v)) mp->qb = v;
   if (jv.get_int("training_threshold", &v) && v > 0) mp->training_threshold = v;
   // placement of the raw vectors (VectorManager::DetermineVectorStorageType, vector_manager.cc:50-89): "RocksDB" keeps
   // them out of HBM, in pinned host memory; every other value, and none, keeps them in HBM
@@ -119,6 +122,10 @@ bool parse_retrieval_params(const std::string& text, RetrievalParams* rp, std::s
   if (jv.get_int("recall_num", &v) && v > 0) rp->recall_num = v;
   if (jv.get_int("nprobe", &v) && v > 0) rp->nprobe = v;
   if (jv.get_int("parallel_on_queries", &v)) rp->parallel_on_queries = v != 0;
+  // IVFRABITQ (gamma_index_ivfrabitq.cc:215-229): a qb outside [0, 8] falls back to the index's
+  if (jv.get_int("qb", &v) && v >= 0 && v <= 8) rp->qb = v;
+  bool b;
+  if (jv.get_bool("centered", &b)) rp->centered = b;
   return true;
 }
 
@@ -495,6 +502,24 @@ int gb_index_search_preassigned_binary(gb_index* index, int nq, const uint8_t* x
   SearchContext ctx;
   if (fill_ctx(&ctx, "", 0, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score)) return -1;
   return b->search_preassigned_host(ctx, nq, x, k, keys, nullptr, nprobe, out_scores, out_ids);
+}
+
+#define RQ_OR_FAIL(v, index) AS_OR_FAIL(RaBitQIndex, v, index, "IVFRABITQ")
+int gb_index_rabitq_nb_bits(gb_index* index) {
+  RQ_OR_FAIL(rq, index);
+  return rq->nb_bits();
+}
+int gb_index_rabitq_qb(gb_index* index) {
+  RQ_OR_FAIL(rq, index);
+  return rq->qb();
+}
+int gb_index_rabitq_encode(gb_index* index, int64_t n, const float* x, const int64_t* assign, uint8_t* codes) {
+  RQ_OR_FAIL(rq, index);
+  return rq->encode_host(x, n, assign, codes);
+}
+int gb_index_rabitq_estimate(gb_index* index, int nq, const float* x, const int64_t* lists, int qb, int metric, float* out) {
+  RQ_OR_FAIL(rq, index);
+  return rq->estimate_host(nq, x, lists, qb, metric >= 0 ? metric : rq->metric(), out);
 }
 
 int gb_kmeans(int device, const float* x, int64_t n, int d, int k, int niter, int64_t seed, int spherical,

@@ -255,6 +255,24 @@ cudaError_t launch_binary_ivf_scan(const uint32_t* queries, int64_t ldq, int nq,
                                    cudaStream_t st);
 int binary_scan_max_k(int code_size);  // the largest k (<= 4096) the scan can select at this code size, 0 if none
 
+// ---- K13: IVFRABITQ (kernels_rabitq.cu): multi-bit RaBitQ codes of residuals, estimator scan ------------------------
+// dimensions above this are refused: the encoder keeps 16 bytes per dimension of a vector in shared memory, and the
+// scan's integer sums stay below 2^31
+constexpr int kRabitqMaxDim = 4096;
+int rabitq_code_bytes(int d, int nb_bits);  // 4 (nb_bits ceil(d / 32) + 3): bit-planes, then |r|^2, f, S
+// codes[i] of the residual x_i - cents[lists[i]] (rows of x and cents zero padded, strides in floats)
+cudaError_t launch_rabitq_encode(const float* x, int64_t ldx, int64_t n, const int32_t* lists, const float* cents, int64_t ldc,
+                                 int d, int nb_bits, uint8_t* codes, cudaStream_t st);
+// query-major estimator scan of the probed lists: partial[q][group][k] sorted, as launch_ivfpq_scan; qb in [0, 8]
+cudaError_t launch_rabitq_scan(const float* xq, int64_t ldq, int nq, const float* cents, int64_t ldc, int d, int nb_bits, int qb,
+                               const int32_t* probe_ids, int nprobe, int pg, ListDirectory dir, int k, int metric, FilterArgs f,
+                               unsigned long long* partial, cudaStream_t st);
+int rabitq_scan_max_k(int d, int nb_bits, int qb);  // the largest k (<= 4096) the scan can select, 0 if none
+// test hook: out[out_off[j] + e] = the scan's estimate of entry e of list l_of[j] for query q_of[j], every entry
+cudaError_t launch_rabitq_estimate(const float* xq, int64_t ldq, const float* cents, int64_t ldc, int d, int nb_bits, int qb,
+                                   int metric, ListDirectory dir, const int32_t* q_of, const int32_t* l_of,
+                                   const int64_t* out_off, int npairs, float* out, cudaStream_t st);
+
 // ---- K6/K8: build-side kernels ------------------------------------------------------------
 // centroids[c] = (sum of x[perm[off[c]..off[c+1])] in that order) * (1/count); empty => zeros
 cudaError_t launch_segment_mean(const float* x, int64_t ldx, int d, const int32_t* perm, const int32_t* off, int k,

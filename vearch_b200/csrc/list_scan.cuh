@@ -25,6 +25,12 @@
 //                                     the stage, not 4-byte aligned in general; it may read the aligned 32-bit word
 //                                     holding the entry's last byte (the launcher pads the window by 16 bytes)
 // and is launched with MW = 0 only.  The other codecs keep the [code_bytes()][256] table and table_sum.
+//
+// A kCodeSum codec whose entries are too wide for one thread each (IVFRABITQ) also declares kLanes = true and supplies
+//   lanes()                           L, a power of two <= 32: L consecutive threads score one entry together
+//   score_lanes(code, tab, lane)      the entry's score, returned in each of its L lanes (lane = tid % L); every thread
+//                                     of the CTA calls it the same number of times, so it may shuffle within its group
+// Its tile_entries() is then a multiple of LS_NT / L; start / finish / code_sum are not called.
 #pragma once
 #include "common.cuh"
 
@@ -85,6 +91,26 @@ template <class Codec>
 struct LsCodeSum<Codec, decltype(void(Codec::kCodeSum))> {
   static constexpr bool value = Codec::kCodeSum;
 };
+
+// LsLanes<Codec>::value: the codec scores an entry with lanes() threads (and supplies score_lanes)
+template <class Codec, class = void>
+struct LsLanes {
+  static constexpr bool value = false;
+};
+template <class Codec>
+struct LsLanes<Codec, decltype(void(Codec::kLanes))> {
+  static constexpr bool value = Codec::kLanes;
+};
+
+// threads that score one entry
+template <class Codec>
+__host__ __device__ __forceinline__ int ls_lanes(const Codec& c) {
+  if constexpr (LsLanes<Codec>::value) {
+    return c.lanes();
+  } else {
+    return 1;
+  }
+}
 
 // Entry elements of the codec's table
 template <class Codec>
@@ -203,7 +229,7 @@ __global__ void __launch_bounds__(LS_NT, Codec::kMinCtasPerSm)
   // entries per thread per tile: compile-time for the vector-load code layouts (gives the compiler PT independent
   // chains to interleave), runtime for the generic layout
   constexpr int PT = MW > 0 ? Codec::pt(MW) : 1;
-  const int per_thread = MW > 0 ? PT : tile_e / LS_NT;
+  const int per_thread = MW > 0 ? PT : tile_e / (LS_NT / ls_lanes(c));
   int est = 0;  // upper bound of the queue fill, identical in every thread
 
   for (int gt = 0; gt < total_tiles; gt++) {
@@ -252,9 +278,20 @@ __global__ void __launch_bounds__(LS_NT, Codec::kMinCtasPerSm)
 #pragma unroll
       for (int u = 0; u < PT; u++) consider(u * LS_NT + tid, c.finish(acc[u]));
     } else {
-      for (int u = 0; u < per_thread; u++) {
-        const int e = u * LS_NT + tid;
-        consider(e, e < n_e ? c.finish(ls_entry_sum<MW>(c, st + (size_t)e * cb, tab, c.start(dis0), cb)) : 0.f);
+      if constexpr (LsLanes<Codec>::value) {
+        // L threads per entry; only the group's first lane offers it to the queue (e = tile_e masks the others)
+        const int L = c.lanes();
+        const int lane = tid & (L - 1);
+        for (int u = 0; u < per_thread; u++) {
+          const int e = u * (LS_NT / L) + tid / L;
+          const float dis = c.score_lanes(st + (size_t)e * cb, tab, lane);
+          consider(lane == 0 ? e : tile_e, dis);
+        }
+      } else {
+        for (int u = 0; u < per_thread; u++) {
+          const int e = u * LS_NT + tid;
+          consider(e, e < n_e ? c.finish(ls_entry_sum<MW>(c, st + (size_t)e * cb, tab, c.start(dis0), cb)) : 0.f);
+        }
       }
     }
     // stage consumed + pushes done; the count is identical in every thread (no 2nd barrier needed)

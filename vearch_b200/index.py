@@ -456,6 +456,46 @@ class BinaryIVFIndex(GammaIndex):
         return dis, ids
 
 
+class RaBitQIndex(GammaIndex):
+    """IVFRABITQ (gamma_index_ivfrabitq.cc): IVF over multi-bit RaBitQ codes of the residuals, nb_bits in [1, 9] per
+    dimension, queries quantised to qb in [0, 8] bits per (query, list).  Rows and queries are float32 [n, d] as for
+    the other float types; the estimator contract is DESIGN.md section 3, K13 (numpy twin: oracle_rabitq)."""
+
+    def __init__(self, d, params=None, device=0, store_type=None):
+        super().__init__("IVFRABITQ", d, params, device, store_type)
+
+    @property
+    def nb_bits(self):
+        return int(_lib.lib().gb_index_rabitq_nb_bits(self._h))
+
+    @property
+    def qb(self):
+        return int(_lib.lib().gb_index_rabitq_qb(self._h))
+
+    def encode(self, x, assign):
+        """List entries (uint8 [n, code_size]) of rows x whose residuals are taken to the lists `assign`."""
+        x = _f32(x)
+        assign = np.ascontiguousarray(assign, np.int64)
+        assert x.ndim == 2 and x.shape[1] == self.d and assign.shape == (x.shape[0],)
+        codes = np.empty((x.shape[0], self.code_size), np.uint8)
+        _check(_lib.lib().gb_index_rabitq_encode(self._h, x.shape[0], _ptr(x), _ptr(assign), _ptr(codes)), "rabitq_encode")
+        return codes
+
+    def estimate(self, x, lists, qb=None, metric=-1):
+        """The scan's scores of every entry of list lists[j] for query x[j]: a list of float32 arrays, one per query,
+        in list order."""
+        x = _f32(x)
+        lists = np.ascontiguousarray(lists, np.int64)
+        assert x.ndim == 2 and x.shape[1] == self.d and lists.shape == (x.shape[0],)
+        lens = [self.list_len(int(l)) for l in lists]
+        out = np.empty(max(1, sum(lens)), np.float32)
+        q = self.qb if qb is None else int(qb)
+        _check(_lib.lib().gb_index_rabitq_estimate(self._h, x.shape[0], _ptr(x), _ptr(lists), q, metric, _ptr(out)),
+               "rabitq_estimate")
+        off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+        return [out[off[j]:off[j + 1]].copy() for j in range(len(lens))]
+
+
 def index_factory(d, description, metric=METRIC_L2, device=0, **extra):
     """index/index.h index_factory: "IVF1024,Flat" | "IVF4096,PQ16x8" | "IVF256,PQ32x4" (PQ<M>x<nbits>) | "Flat"."""
     parts = [p.strip() for p in description.split(",")]
