@@ -32,12 +32,15 @@ long long gb_launch_count(void);
 
 /* reflector().GetNewIndex(type) + IndexModel::Init(model_parameters, training_threshold)
  * (index/reflector.h:68-80, vector/vector_manager.cc:171; gamma_index_ivfflat.cc:215-291,
- * gamma_index_ivfpq.cc:112-231).  index_type: "FLAT" | "IVFFLAT" | "IVFPQ".
+ * gamma_index_ivfpq.cc:112-231).  index_type: "FLAT" | "IVFFLAT" | "IVFPQ" | "GPU_IVFFLAT" | "GPU_IVFPQ" | ...
+ * (GPU_IVFFLAT / GPU_IVFPQ: IVFFLAT / IVFPQ under gamma's GPU parameter and request contracts, DESIGN.md section 8).
  * model_params_json keys: ncentroids, nprobe, metric_type ("L2"|"InnerProduct"), nsubvector,
  * nbits_per_idx (IVFPQ: 1..8), training_threshold, bucket_init_size, bucket_max_size, store_type ("RocksDB", any
  * case: raw vectors in pinned host memory; anything else: in HBM) (may be NULL/""). */
 gb_index *gb_index_create(const char *index_type, int dimension, const char *model_params_json, int device);
 void gb_index_destroy(gb_index *index);
+/* the registered type name the index was created under (Index::type) */
+const char *gb_index_type(gb_index *index);
 
 /* VectorManager::AddToStore (vector_manager.cc:455): append n raw vectors (n x d fp32). */
 int gb_index_add_vectors(gb_index *index, int64_t n, const float *x);

@@ -59,6 +59,8 @@ def _declare(l):
     l.gb_index_last_scan_ms.restype = f32
     l.gb_index_last_scan_ms.argtypes = [vp]
     l.gb_index_last_scan_kernel.restype = cstr
+    l.gb_index_type.restype = cstr
+    l.gb_index_type.argtypes = [vp]
     l.gb_index_last_scan_kernel.argtypes = [vp]
     l.gb_index_last_scan_info.restype = cstr
     l.gb_index_last_scan_info.argtypes = [vp]

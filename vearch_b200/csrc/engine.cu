@@ -312,7 +312,7 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
   if (index_type_.empty()) return Status::Make(kInvalidArgument, vec_name_ + " index type is empty");
   ModelParams mp;
   std::string err;
-  if (!parse_model_params(index_params_, &mp, &err)) return Status::Make(kInvalidArgument, err);
+  if (!parse_model_params(index_params_, index_type_, &mp, &err)) return Status::Make(kInvalidArgument, err);
   if (table_index_params.empty() && mp.training_threshold > training_threshold_)
     training_threshold_ = mp.training_threshold;  // table.cc:143-150
   if (training_threshold_ > 0) mp.training_threshold = training_threshold_;
@@ -324,7 +324,7 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
   Index* idx = create_index(index_type_, dim_, mp, device_, 20);
   if (!idx) return Status::Make(index_type_ == "FLAT" || index_type_ == "IVFFLAT" || index_type_ == "IVFPQ" ||
                                         index_type_ == "IVFPQFastScan" || index_type_ == "BINARYIVF" ||
-                                        index_type_ == "IVFRABITQ"
+                                        index_type_ == "IVFRABITQ" || is_gpu_index_type(index_type_)
                                     ? kInvalidArgument
                                     : kNotSupported,
                                 last_error());
@@ -347,7 +347,7 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     }
     if (vf.index_type.empty()) return Status::Make(kInvalidArgument, vf.name + " index type is empty");
     ModelParams emp;
-    if (!parse_model_params(vf.index_params, &emp, &err)) return Status::Make(kInvalidArgument, err);
+    if (!parse_model_params(vf.index_params, vf.index_type, &emp, &err)) return Status::Make(kInvalidArgument, err);
     if (training_threshold_ > 0) emp.training_threshold = training_threshold_;
     emp.host_store = !strcasecmp(ev.str(4).c_str(), "RocksDB");
     if (vf.index_type == "BINARYIVF")

@@ -518,7 +518,7 @@ void quiesce_all_indexes() {
 }  // namespace
 
 Index::Index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int row_bytes)
-    : type_(type), d_(d), dpad_((int)round_up(d, 4)), device_(device), mp_(mp) {
+    : type_(type), gpu_contract_(is_gpu_index_type(type)), d_(d), dpad_((int)round_up(d, 4)), device_(device), mp_(mp) {
   cudaSetDevice(device_);
   cudaMemPool_t pool;
   if (cudaDeviceGetDefaultMemPool(&pool, device_) == cudaSuccess) {
@@ -829,6 +829,7 @@ int Index::search_keys(const SearchContext& ctx, int nq, const void* xq, int k, 
 int Index::search_device(const SearchContext& ctx, int nq, const float* x_dev, int64_t ldx, int k, float* out_dis_dev,
                          int64_t* out_ids_dev, cudaStream_t st, unsigned long long* out_keys_dev) {
   if (nq <= 0) return 0;
+  if (check_gpu_request(ctx, nq, k)) return -1;
   cudaSetDevice(device_);
   std::shared_lock<std::shared_mutex> lk(mu_);
   Scratch s(st);
@@ -947,8 +948,24 @@ void Index::coalesce_loop() {
   }
 }
 
+int Index::check_gpu_request(const SearchContext& ctx, int nq, int k) const {
+  if (!gpu_contract_) return 0;
+  if (nq > kGpuMaxReq) {  // CommonSearch (gamma_gpu_search_base.h:48-52)
+    set_last_error("req num [" + std::to_string(nq) + "] should not larger than [" + std::to_string(kGpuMaxReq) + "]");
+    return -1;
+  }
+  // GetRecallNum: max(k, recall_num) for GPU_IVFPQ; GPU_IVFFLAT's is always k (gamma_gpu_search_base.h:74-81)
+  const int recall = type_ == "GPU_IVFPQ" ? std::max(k, ctx.params.recall_num) : k;
+  if (recall > kGpuMaxK) {
+    set_last_error("topK num [" + std::to_string(recall) + "] should not larger than [" + std::to_string(kGpuMaxK) + "]");
+    return -1;
+  }
+  return 0;
+}
+
 int Index::search(const SearchContext& ctx, int nq, const void* x, int k, float* out_dis, int64_t* out_ids) {
   if (nq <= 0) return 0;
+  if (check_gpu_request(ctx, nq, k)) return -1;  // per call, before coalescing merges calls into one device batch
   if (!coalescable(ctx, nq)) return search_direct(ctx, nq, x, k, out_dis, out_ids);
   CoReq req;
   req.ctx = &ctx, req.nq = nq, req.k = k, req.x = x, req.out_dis = out_dis, req.out_ids = out_ids;
@@ -1231,8 +1248,8 @@ IvfIndex::~IvfIndex() {
   cudaFree(d_cent_tiles_);
   cudaFree(d_cent_norms_);
 }
-IVFFlatIndex::IVFFlatIndex(int d, const ModelParams& mp, int device, int seg_shift)
-    : IvfIndex("IVFFLAT", d, mp, device, seg_shift) {
+IVFFlatIndex::IVFFlatIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift)
+    : IvfIndex(type, d, mp, device, seg_shift) {
   if (metric() == kMetricL2) {  // inner products are scanned unshifted: no table
     cudaMalloc(&d_shifts_, (size_t)nlist_ * dpad_ * 4);
     cudaMemset(d_shifts_, 0, (size_t)nlist_ * dpad_ * 4);  // = the zero centroids of an untrained index
@@ -1513,7 +1530,9 @@ int IvfIndex::update_vector(int64_t vid, const void* x) {
 
 int IvfIndex::resolve_nprobe(const SearchContext& ctx) const {
   int nprobe = mp_.nprobe;
-  if (ctx.params.nprobe > 0 && ctx.params.nprobe <= nlist_) nprobe = ctx.params.nprobe;  // ivfflat.cc:551-559
+  // ivfflat.cc:551-559; the GPU types' GetNprobe (gamma_index_ivfpq_gpu.cc:584-594) also refuses a request above kGpuMaxK
+  const int max_req = gpu_contract_ ? std::min(nlist_, kGpuMaxK) : nlist_;
+  if (ctx.params.nprobe > 0 && ctx.params.nprobe <= max_req) nprobe = ctx.params.nprobe;
   if (nprobe > nlist_) nprobe = nlist_;
   if (nprobe > 4096) nprobe = 4096;
   return nprobe;
@@ -1861,6 +1880,7 @@ int IvfIndex::coarse_search_host(int nq, const void* x, int nprobe, float* out_d
 int IvfIndex::search_preassigned_host(const SearchContext& ctx, int nq, const void* x, int k, const int64_t* keys,
                                       const float* coarse_dis, int nprobe, float* out_dis, int64_t* out_ids) {
   if (nq <= 0) return 0;
+  if (check_gpu_request(ctx, nq, k)) return -1;
   if (!trained_ || !lists_ || k <= 0 || k > 4096 || nprobe <= 0 || nprobe > 4096) {
     set_last_error("search_preassigned: untrained index, topK or nprobe out of range");
     return -1;
@@ -1966,8 +1986,8 @@ int IvfPqBase::encode_host(const float* x, int64_t n, const int64_t* assign, uin
 
 // ------------------------------------------------------------------------------------------
 // gamma_index_ivfpq.cc:122-124: nsubvector defaults to d / 2
-IVFPQIndex::IVFPQIndex(int d, const ModelParams& mp, int device, int seg_shift)
-    : IvfPqBase("IVFPQ", d, mp, device, seg_shift, std::max(1, mp.nsubvector > 0 ? mp.nsubvector : d / 2), 1 << mp.nbits),
+IVFPQIndex::IVFPQIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift)
+    : IvfPqBase(type, d, mp, device, seg_shift, std::max(1, mp.nsubvector > 0 ? mp.nsubvector : d / 2), 1 << mp.nbits),
       nbits_(mp.nbits) {
   if (mp.opq_nsubvector > 0) {  // faiss::OPQMatrix(d, opq_nsubvector, d) (gamma_index_ivfpq.cc:168-178)
     cudaMalloc(&d_opq_, (size_t)d * dpad_ * 4);
@@ -2171,8 +2191,11 @@ IVFPQIndex::~IVFPQIndex() {
   if (pqn_.base) cudaFree(pqn_.base);
   if (pqn_.d_off) cudaFree(pqn_.d_off);
 }
-// gamma_index_ivfpq.cc:139-144
-int64_t IVFPQIndex::default_training_threshold() const { return std::max<int64_t>((int64_t)nlist_ * 200, 256); }
+// gamma_index_ivfpq.cc:139-144; GPU_IVFPQ: ncentroids * max_points_per_centroid (gamma_index_ivfpq_gpu.cc:208-212)
+int64_t IVFPQIndex::default_training_threshold() const {
+  if (gpu_contract_) return (int64_t)nlist_ * 256;
+  return std::max<int64_t>((int64_t)nlist_ * 200, 256);
+}
 KMeansParams IVFPQIndex::coarse_kmeans_params() const {
   KMeansParams kp;
   kp.niter = 10;                            // gamma_index_ivfpq.cc:188
@@ -2376,9 +2399,10 @@ int IvfIndex::scan_query_major_dev(const char* kernel, const SearchContext& ctx,
     set_last_error(type_ + ": per-request metric must equal the trained metric");
     return -1;
   }
-  // recall_num / re-rank semantics: gamma_index_ivfpq.cc:764-770
-  const bool rerank = ctx.params.recall_num > 0;
-  const int kk = std::max(k, ctx.params.recall_num);
+  // recall_num / re-rank semantics: gamma_index_ivfpq.cc:764-770.  The GPU types never re-rank ("IVFPQ doesn't support
+  // rerank", gamma_index_ivfpq_gpu.cc:565): recall_num is checked at the search entry and changes nothing else.
+  const bool rerank = ctx.params.recall_num > 0 && !gpu_contract_;
+  const int kk = rerank ? std::max(k, ctx.params.recall_num) : k;
   if (kk > max_kk) {
     set_last_error(type_ + ": recall_num / topn [" + std::to_string(kk) + "] above " + std::to_string(max_kk) +
                    " is not supported by this engine at " + limit_at);
@@ -2796,7 +2820,7 @@ Index* create_index(const std::string& type, int d, const ModelParams& mp, int d
       set_last_error("nprobe should be less than ncentroids");
       return nullptr;
     }
-    return new IVFFlatIndex(d, mp, device, seg_shift);
+    return new IVFFlatIndex(type, d, mp, device, seg_shift);
   }
   if (type == "IVFPQ") {
     int M = mp.nsubvector > 0 ? mp.nsubvector : d / 2;
@@ -2832,7 +2856,57 @@ Index* create_index(const std::string& type, int d, const ModelParams& mp, int d
       set_last_error("nprobe should be less than ncentroids");
       return nullptr;
     }
-    return new IVFPQIndex(d, mp, device, seg_shift);
+    return new IVFPQIndex(type, d, mp, device, seg_shift);
+  }
+  if (type == "GPU_IVFPQ") {  // IVFPQGPUModelParams::Parse / Validate, GammaIVFPQGPUIndex::Init (gamma_index_ivfpq_gpu.cc:62-200)
+    std::string err;
+    const int M = mp.has_nsubvector ? mp.nsubvector_arg : IVFPQIndex::kGpuDefaultM;
+    if (mp.has_ncentroids && mp.ncentroids_arg <= 0)
+      err = "invalid ncentroids =" + std::to_string(mp.ncentroids_arg);
+    else if (mp.has_nsubvector && mp.nsubvector_arg <= 0)
+      err = "invalid nsubvector =" + std::to_string(mp.nsubvector_arg);
+    else if (mp.has_nbits && mp.nbits_arg <= 0)
+      err = "invalid nbits_per_idx =" + std::to_string(mp.nbits_arg);
+    else if (mp.has_nprobe && mp.nprobe_arg <= 0)
+      err = "invalid nprobe =" + std::to_string(mp.nprobe_arg);
+    else if (mp.has_nprobe && mp.nprobe > mp.ncentroids)
+      err = "nprobe should less than ncentroids";
+    else if (!mp.metric_unknown.empty())
+      err = "invalid metric_type = " + mp.metric_unknown;
+    else if (M % 4 != 0)  // Validate() logs these and returns ParamError() without text
+      err = "only support multiple of 4 now, nsubvector=" + std::to_string(M);
+    else if (mp.nbits != 8)
+      err = "only support 8 now, nbits_per_idx=" + std::to_string(mp.nbits);
+    else if (d % M != 0)
+      err = "Dimension [" + std::to_string(d) + "] cannot divide by nsubvector [" + std::to_string(M) + "].";
+    else if (ivfpq_scan_max_k(M, 8) < Index::kGpuMaxK) {
+      // the query-major scan must select the type's own ceiling k' = 2048 beside the [M][256] fp32 table
+      int max_m = M;
+      while (max_m > 4 && ivfpq_scan_max_k(max_m, 8) < Index::kGpuMaxK) max_m -= 4;
+      err = "GPU_IVFPQ: nsubvector [" + std::to_string(M) + "] above " + std::to_string(max_m) +
+            " is not supported by this engine";
+    }
+    if (!err.empty()) {
+      set_last_error(err);
+      return nullptr;
+    }
+    ModelParams g = mp;
+    g.nsubvector = M;
+    g.opq_nsubvector = 0;  // the GPU type reads no "opq" object
+    g.has_opq = false;
+    return new IVFPQIndex(type, d, g, device, seg_shift);
+  }
+  if (type == "GPU_IVFFLAT") {  // IVFFlatGPUModelParams::Parse / Validate (gamma_index_ivfflat_gpu.h:64-110)
+    // ncentroids and nprobe as given (even <= 0); an unknown metric_type was ignored; nprobe > ncentroids is accepted
+    ModelParams g = mp;
+    if (mp.has_ncentroids) g.ncentroids = mp.ncentroids_arg;
+    if (mp.has_nprobe) g.nprobe = mp.nprobe_arg;
+    if (g.ncentroids <= 0 || g.nprobe <= 0 || mp.bucket_init_arg <= 0 || mp.bucket_max_arg <= 0 ||
+        mp.bucket_init_arg > mp.bucket_max_arg) {
+      set_last_error("Invalid parameters");
+      return nullptr;
+    }
+    return new IVFFlatIndex(type, d, g, device, seg_shift);
   }
   if (type == "IVFPQFastScan") {  // IVFPQFastScanModelParams::Validate (gamma_index_ivfpqfs.h:231-245)
     if (mp.nsubvector <= 0 || d % mp.nsubvector != 0) {

@@ -177,7 +177,17 @@ struct ModelParams {  // index/impl/gamma_index_ivfpq.h:1031-1257, gamma_index_i
   int ncentroids_arg = 0;       // "ncentroids" as given, 0 if absent (BINARYIVF has its own default and range check)
   int nb_bits = 4;              // IVFRABITQ bits per dimension as given (validated by create_index: [1, 9])
   int qb = 4;                   // IVFRABITQ query bits as given (validated by create_index: [0, 8])
+  // The GPU_* types check the values as given, in their own order and with their own messages (create_index): whether
+  // each key was present, its value even when <= 0, and a metric_type that is neither L2 nor InnerProduct
+  bool has_ncentroids = false, has_nprobe = false, has_nsubvector = false, has_nbits = false;
+  int nprobe_arg = 0, nsubvector_arg = 0, nbits_arg = 0;
+  int bucket_init_arg = 1000, bucket_max_arg = 1000000;  // GPU_IVFFLAT's defaults (IVFFlatGPUModelParams)
+  std::string metric_unknown;
 };
+
+// gamma's two GPU index types (index/impl/gpu/): GPU_IVFPQ is an IVFPQIndex and GPU_IVFFLAT an IVFFlatIndex, created
+// under the reference's GPU parameter contract and searched under its GPU request contract (Index::gpu_contract)
+inline bool is_gpu_index_type(const std::string& type) { return type == "GPU_IVFPQ" || type == "GPU_IVFFLAT"; }
 
 struct RetrievalParams {  // gamma_index_ivfpq.cc:233-294, gamma_index_ivfflat.cc:293-340
   int nprobe = -1;
@@ -204,6 +214,11 @@ class Index {
   Index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int row_bytes = 0);
   virtual ~Index();
   const std::string& type() const { return type_; }
+  // The GPU_* types' request contract (CommonSearch, gamma_gpu_search_base.h:40-112): at most kGpuMaxReq queries per
+  // call and k' = max(k, recall_num) at most kGpuMaxK, refused before request coalescing; no exact re-rank; a request
+  // nprobe outside (0, min(nlist, kGpuMaxK)] falls back to the model's (resolve_nprobe)
+  static constexpr int kGpuMaxReq = 512, kGpuMaxK = 2048;
+  bool gpu_contract() const { return gpu_contract_; }
   int d() const { return d_; }
   int device() const { return device_; }
   int metric() const { return mp_.metric; }
@@ -288,7 +303,11 @@ class Index {
   std::vector<std::unique_ptr<CopyLane>> lanes_;
   std::vector<CopyLane*> free_lanes_;
 
+  // the GPU_* request limits above, for a search of nq queries at top k; 0 or -1 (last_error set)
+  int check_gpu_request(const SearchContext& ctx, int nq, int k) const;
+
   std::string type_;
+  bool gpu_contract_;
   int d_, dpad_, device_;
   ModelParams mp_;
   std::unique_ptr<RawStore> store_;
@@ -513,10 +532,11 @@ class IvfIndex : public Index {
   std::vector<uint64_t> vid2pos_;  // vid -> (list << 32 | pos), ~0 = not in a list (vid_bucket_no_pos_)
 };
 
-// GammaIVFFlatIndex (index/impl/gamma_index_ivfflat.{h,cc}): the lists hold the raw fp32 rows
+// GammaIVFFlatIndex (index/impl/gamma_index_ivfflat.{h,cc}): the lists hold the raw fp32 rows.  type: "IVFFLAT", or
+// "GPU_IVFFLAT" (GammaIVFFlatGPUIndex, the same index under the GPU contract)
 class IVFFlatIndex : public IvfIndex {
  public:
-  IVFFlatIndex(int d, const ModelParams& mp, int device, int seg_shift);
+  IVFFlatIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift);
   ~IVFFlatIndex() override;
   int64_t index_mem_bytes() const override;
   int code_bytes() const override { return dpad_ * 4; }
@@ -525,7 +545,8 @@ class IVFFlatIndex : public IvfIndex {
 
  protected:
   GammaFileFormat gamma_format() const override;
-  int64_t default_training_threshold() const override { return (int64_t)nlist_ * 200; }  // gamma_index_ivfflat.cc:239
+  // gamma_index_ivfflat.cc:239; GPU_IVFFLAT: ncentroids * max_points_per_centroid (gamma_index_ivfflat_gpu.cc)
+  int64_t default_training_threshold() const override { return (int64_t)nlist_ * (gpu_contract_ ? 256 : 200); }
   int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, const void* xq_raw, int k,
                const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
                Scratch& s) override;
@@ -598,12 +619,14 @@ class IvfPqBase : public IvfIndex {
 
 // GammaIVFPQIndex (index/impl/gamma_index_ivfpq.{h,cc}) at nbits_per_idx 1..8: ksub = 2^nbits centroids per
 // sub-quantiser; list entries hold the residual codes bit-packed in ceil(M nbits / 8) bytes (faiss PQEncoderGeneric:
-// code m at bits [m nbits, (m + 1) nbits), LSB-first), one byte per code at nbits = 8.
+// code m at bits [m nbits, (m + 1) nbits), LSB-first), one byte per code at nbits = 8.  type: "IVFPQ", or "GPU_IVFPQ"
+// (GammaIVFPQGPUIndex, the same index at nbits 8 under the GPU contract)
 class IVFPQIndex : public IvfPqBase {
  public:
   // nbits_per_idx above this: faiss's 16-bit codes (PQDecoder16), whose [M][65536] fp32 table no scan keeps in shared memory
   static constexpr int kMaxNbits = 8;
-  IVFPQIndex(int d, const ModelParams& mp, int device, int seg_shift);
+  static constexpr int kGpuDefaultM = 64;  // GPU_IVFPQ's nsubvector default (IVFPQGPUModelParams)
+  IVFPQIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift);
   ~IVFPQIndex() override;
   int64_t index_mem_bytes() const override;
   int nbits() const { return nbits_; }

@@ -20,11 +20,15 @@ namespace gb {
 
 // IVFFlatModelParams::Parse / IVFPQModelParams::Parse (gamma_index_ivfflat.cc:64-196,
 // gamma_index_ivfpq.h:1031-1257)
-bool parse_model_params(const std::string& text, ModelParams* mp, std::string* err) {
+bool parse_model_params(const std::string& text, const std::string& type, ModelParams* mp, std::string* err) {
   if (text.empty()) return true;
+  const bool gpu = is_gpu_index_type(type);
   JsonValue jv;
   if (!JsonParser::parse(text, &jv) || jv.type != JsonValue::Object) {
-    *err = "parse model parameters error: " + text;
+    // IVFPQGPUModelParams::Parse / IVFFlatGPUModelParams::Parse (gamma_index_ivfpq_gpu.cc:63-69, ivfflat_gpu.h:67-73)
+    *err = type == "GPU_IVFPQ"     ? "failed to parse IVFPQ retrieval parameters"
+           : type == "GPU_IVFFLAT" ? "Parse model parameters error"
+                                   : "parse model parameters error: " + text;
     return false;
   }
   int v;
@@ -35,20 +39,25 @@ bool parse_model_params(const std::string& text, ModelParams* mp, std::string* e
     }
     if (v > 0) mp->ncentroids = v;
     mp->ncentroids_arg = v;
+    mp->has_ncentroids = true;
   }
   if (jv.get_int("nprobe", &v)) {
-    if (v < -1) {
+    mp->has_nprobe = true;
+    mp->nprobe_arg = v;
+    if (v < -1 && !gpu) {
       *err = "invalid nprobe =" + std::to_string(v);
       return false;
     }
     if (v > 0) mp->nprobe = v;
-    if (mp->nprobe > mp->ncentroids) {
+    if (mp->nprobe > mp->ncentroids && !gpu) {
       *err = "nprobe should less than ncentroids";
       return false;
     }
   }
   if (jv.get_int("nsubvector", &v)) {
-    if (v < -1) {
+    mp->has_nsubvector = true;
+    mp->nsubvector_arg = v;
+    if (v < -1 && !gpu) {
       *err = "invalid nsubvector =" + std::to_string(v);
       return false;
     }
@@ -65,21 +74,25 @@ bool parse_model_params(const std::string& text, ModelParams* mp, std::string* e
     }
   }
   if (jv.get_int("nbits_per_idx", &v)) {
-    if (v < -1) {
+    mp->has_nbits = true;
+    mp->nbits_arg = v;
+    if (v < -1 && !gpu) {
       *err = "invalid nbits_per_idx =" + std::to_string(v);
       return false;
     }
     if (v > 0) mp->nbits = v;
   }
   if (jv.get_int("bucket_init_size", &v)) {
-    if (v < -1) {
+    mp->bucket_init_arg = v;
+    if (v < -1 && !gpu) {
       *err = "invalid bucket_init_size =" + std::to_string(v);
       return false;
     }
     if (v > 0) mp->bucket_init_size = v;
   }
   if (jv.get_int("bucket_max_size", &v)) {
-    if (v < -1) {
+    mp->bucket_max_arg = v;
+    if (v < -1 && !gpu) {
       *err = "invalid bucket_max_size =" + std::to_string(v);
       return false;
     }
@@ -99,6 +112,10 @@ bool parse_model_params(const std::string& text, ModelParams* mp, std::string* e
   std::string mt;
   if (jv.get_string("metric_type", &mt)) {
     if (strcasecmp("L2", mt.c_str()) && strcasecmp("InnerProduct", mt.c_str())) {
+      if (gpu) {  // GPU_IVFPQ refuses it in create_index; GPU_IVFFLAT ignores it and keeps InnerProduct
+        mp->metric_unknown = mt;
+        return true;
+      }
       *err = "invalid metric_type = " + mt;
       return false;
     }
@@ -181,7 +198,7 @@ int gb_device_count(void) {
 gb_index* gb_index_create(const char* index_type, int dimension, const char* model_params_json, int device) {
   ModelParams mp;
   std::string err;
-  if (!parse_model_params(model_params_json ? model_params_json : "", &mp, &err)) {
+  if (!parse_model_params(model_params_json ? model_params_json : "", index_type ? index_type : "", &mp, &err)) {
     set_last_error(err);
     return nullptr;
   }
@@ -191,6 +208,8 @@ gb_index* gb_index_create(const char* index_type, int dimension, const char* mod
   h->impl = impl;
   return h;
 }
+
+const char* gb_index_type(gb_index* index) { return index && index->impl ? index->impl->type().c_str() : ""; }
 
 void gb_index_destroy(gb_index* index) {
   if (!index) return;

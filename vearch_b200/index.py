@@ -86,6 +86,11 @@ class GammaIndex:
         return int(_lib.lib().gb_index_training_threshold(self._h))
 
     @property
+    def type(self):
+        """The registered type name the index was created under ("GPU_IVFPQ" is an IVFPQ index under that name)."""
+        return _lib.lib().gb_index_type(self._h).decode()
+
+    @property
     def nlist(self):
         return int(_lib.lib().gb_index_nlist(self._h))
 
