@@ -180,6 +180,17 @@ int gb_index_rabitq_nb_bits(gb_index *index);
 int gb_index_rabitq_qb(gb_index *index);
 int gb_index_rabitq_encode(gb_index *index, int64_t n, const float *x, const int64_t *assign, uint8_t *codes);
 int gb_index_rabitq_estimate(gb_index *index, int nq, const float *x, const int64_t *lists, int qb, int metric, float *out);
+/* VEARCH (DESIGN.md section 3, K14): nsubvector and the block count (one more than nsubvector when d % nsubvector != 0);
+   the codebook, 16 d floats (block b's 16 centres of its width each, from float 16 b (d / nsubvector)); the list codes
+   of n rows ((blocks + 1) / 2 bytes, block 2j in the low nibble of byte j) of the residuals to the lists `assign` under
+   InnerProduct (assign ignored, may be NULL, under L2); the biased uint8 tables of a query batch, lut = nq x blocks x 16,
+   and their multipliers mult = nq floats */
+int gb_index_vearch_nsub(gb_index *index);
+int gb_index_vearch_blocks(gb_index *index);
+int gb_index_vearch_set_codebook(gb_index *index, const float *codebook);
+int gb_index_vearch_get_codebook(gb_index *index, float *codebook);
+int gb_index_vearch_encode(gb_index *index, int64_t n, const float *x, const int64_t *assign, uint8_t *codes);
+int gb_index_vearch_lut(gb_index *index, int nq, const float *x, uint8_t *lut, float *mult);
 
 /* ---- standalone kernels exposed for tests / bench ---- */
 /* faiss Clustering restated (k-means), host in/out; obj (niter floats) may be NULL */

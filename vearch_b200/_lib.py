@@ -104,6 +104,12 @@ def _declare(l):
     l.gb_index_rabitq_qb.argtypes = [vp]
     l.gb_index_rabitq_encode.argtypes = [vp, i64, vp, vp, vp]
     l.gb_index_rabitq_estimate.argtypes = [vp, i32, vp, vp, i32, i32, vp]
+    l.gb_index_vearch_nsub.argtypes = [vp]
+    l.gb_index_vearch_blocks.argtypes = [vp]
+    l.gb_index_vearch_set_codebook.argtypes = [vp, vp]
+    l.gb_index_vearch_get_codebook.argtypes = [vp, vp]
+    l.gb_index_vearch_encode.argtypes = [vp, i64, vp, vp, vp]
+    l.gb_index_vearch_lut.argtypes = [vp, i32, vp, vp, vp]
     l.gb_kmeans.argtypes = [i32, vp, i64, i32, i32, i32, i64, i32, i32, vp, vp]
     l.gb_kmeans_update.argtypes = [i32, vp, i64, i32, i32, vp, vp]
     l.gb_merge_partitions_device.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, vp]

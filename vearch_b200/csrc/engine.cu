@@ -324,7 +324,7 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
   Index* idx = create_index(index_type_, dim_, mp, device_, 20);
   if (!idx) return Status::Make(index_type_ == "FLAT" || index_type_ == "IVFFLAT" || index_type_ == "IVFPQ" ||
                                         index_type_ == "IVFPQFastScan" || index_type_ == "BINARYIVF" ||
-                                        index_type_ == "IVFRABITQ" || is_gpu_index_type(index_type_)
+                                        index_type_ == "IVFRABITQ" || index_type_ == "VEARCH" || is_gpu_index_type(index_type_)
                                     ? kInvalidArgument
                                     : kNotSupported,
                                 last_error());

@@ -881,7 +881,7 @@ static bool same_signature(const SearchContext& a, int ka, const SearchContext& 
   return ka == kb && a.min_score == b.min_score && a.max_score == b.max_score && a.params.nprobe == b.params.nprobe &&
          a.params.metric == b.params.metric && a.params.recall_num == b.params.recall_num &&
          a.params.brute_force == b.params.brute_force && a.search_unindexed_tail == b.search_unindexed_tail &&
-         a.params.qb == b.params.qb;
+         a.params.qb == b.params.qb && a.params.given == b.params.given;
 }
 
 void Index::coalesce_loop() {
@@ -2804,6 +2804,196 @@ int RaBitQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int met
 }
 
 // ------------------------------------------------------------------------------------------
+// GammaVearchIndex (gamma_index_vearch.cc) over ScaNN's asymmetric hashing (GetConfig, :128-259)
+VearchIndex::VearchIndex(int d, const ModelParams& mp, int device, int seg_shift)
+    : IvfIndex("VEARCH", d, mp, device, seg_shift), nb_(scann_blocks(d, mp.nsubvector)) {
+  // GetConfig: a negative threshold is written as nan, and L2 forces nan (no noise shaping)
+  if (mp_.ns_threshold < 0 || mp_.metric == kMetricL2) mp_.ns_threshold = std::nan("");
+  cudaMalloc(&d_cb_, (size_t)16 * d * 4);
+  cudaMemset(d_cb_, 0, (size_t)16 * d * 4);
+}
+VearchIndex::~VearchIndex() { cudaFree(d_cb_); }
+int64_t VearchIndex::index_mem_bytes() const { return IvfIndex::index_mem_bytes() + (int64_t)16 * d_ * 4; }
+
+// partitioning: 12 iterations, SPHERICAL under IP, the database assigned by SquaredL2Distance
+KMeansParams VearchIndex::coarse_kmeans_params() const {
+  KMeansParams kp;
+  kp.niter = 12;
+  kp.spherical = mp_.metric == kMetricIP;
+  kp.l2_assign = true;
+  return kp;
+}
+
+// GammaVearchIndex::Search (:483-487): the request's nprobe when it is in (0, ncentroids), else the index's 512 leaves.
+// The request's nprobe defaults to 50 for an empty parameter string (VearchRetrievalParameters(type), the constructor
+// Parse takes then) and to 80 otherwise (VearchRetrievalParameters()).  The leaves are clamped to nlist here.
+int VearchIndex::resolve_nprobe(const SearchContext& ctx) const {
+  const int req = ctx.params.nprobe > 0 ? ctx.params.nprobe : (ctx.params.given ? 80 : 50);
+  const int leaves = req < nlist_ ? req : std::min(kDefaultLeaves, nlist_);
+  return std::min(leaves, 4096);
+}
+
+cudaError_t VearchIndex::encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st) {
+  // residuals under IP (use_residual_quantization), raw rows under L2
+  return launch_scann_encode(x, dpad_, n, mp_.metric == kMetricIP ? lists : nullptr, d_centroids_, dpad_, d_, mp_.nsubvector,
+                             d_cb_, mp_.ns_threshold, codes, st);
+}
+
+// AhImpl::TrainAsymmetricHashing (asymmetric_hashing_impl.cc:150-248): per block a 16-centre k-means (10 iterations) of
+// the training sample's residuals (IP) or rows (L2), its centres then ordered by cluster size, largest first (a stable
+// order among equal sizes; ScaNN's std::sort leaves it open), rotated by ((b / 2) % max(1, 16 / 16)) * 16 = 0 places,
+// and reversed in every odd block b
+int VearchIndex::train_extra(const float* xtrain, int64_t n, Scratch& s) {
+  cudaStream_t st = s.stream();
+  const float* xs = xtrain;
+  if (mp_.metric == kMetricIP) {
+    GB_ALLOC(assign, int32_t, n, s);
+    if (assign_dev(xtrain, dpad_, n, assign, s)) return -1;
+    GB_ALLOC(res, float, (size_t)n * dpad_, s);
+    GB_CUDA(launch_residual(xtrain, dpad_, n, d_, d_centroids_, dpad_, assign, res, dpad_, st));
+    xs = res;
+  }
+  const int w = d_ / mp_.nsubvector;
+  const int wmax = std::max(w, d_ - mp_.nsubvector * w);
+  const int dsp = (int)round_up(wmax, 4);
+  GB_ALLOC(slice, float, (size_t)n * dsp, s);
+  GB_ALLOC(cent, float, (size_t)16 * dsp, s);
+  GB_ALLOC(best, unsigned long long, n, s);
+  KMeansParams kp;
+  kp.niter = 10;
+  kp.max_points_per_centroid = 0;  // the whole sample (expected_sample_size = the training threshold)
+  std::vector<float> cb((size_t)16 * d_), hc((size_t)16 * dsp);
+  std::vector<unsigned long long> hb(n);
+  for (int b = 0; b < nb_; b++) {
+    const int s0 = b * w, wb = b < mp_.nsubvector ? w : d_ - mp_.nsubvector * w;
+    GB_CUDA(launch_slice_cols(xs, dpad_, n, s0, wb, slice, dsp, st));
+    GB_CUDA(cudaMemsetAsync(cent, 0, (size_t)16 * dsp * 4, st));
+    if (kmeans_device(slice, dsp, n, wb, 16, kp, cent, dsp, st, nullptr)) return -1;
+    // cluster sizes: the sample assigned to the final centres (L2, the first minimum)
+    GB_CUDA(launch_fill_u64(best, n, kKeySentinel, st));
+    GB_CUDA(launch_dist_argmin(slice, dsp, (int)n, cent, dsp, 16, dsp, kMetricL2, best, 0, st));
+    GB_CUDA(cudaMemcpyAsync(hb.data(), best, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+    GB_CUDA(cudaMemcpyAsync(hc.data(), cent, hc.size() * 4, cudaMemcpyDeviceToHost, st));
+    GB_CUDA(cudaStreamSynchronize(st));
+    std::vector<int64_t> size(16, 0);
+    for (int64_t i = 0; i < n; i++) size[(uint32_t)hb[i] & 15]++;
+    std::vector<int> perm(16);
+    for (int c = 0; c < 16; c++) perm[c] = c;
+    std::stable_sort(perm.begin(), perm.end(), [&](int a, int c) { return size[a] > size[c]; });
+    if (b & 1) std::reverse(perm.begin(), perm.end());
+    for (int c = 0; c < 16; c++)
+      memcpy(&cb[(size_t)16 * s0 + (size_t)c * wb], &hc[(size_t)perm[c] * dsp], (size_t)wb * 4);
+  }
+  GB_CUDA(cudaMemcpyAsync(d_cb_, cb.data(), cb.size() * 4, cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaStreamSynchronize(st));  // cb leaves scope
+  return 0;
+}
+
+int VearchIndex::append_batch(const void* xv, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                              const std::vector<int>& add, Scratch& s) {
+  (void)add;
+  cudaStream_t st = s.stream();
+  const int cb = code_bytes();
+  GB_ALLOC(codes, uint8_t, (size_t)n * cb, s);
+  GB_CUDA(encode_dev(static_cast<const float*>(xv), n, d_list, codes, st));
+  GB_CUDA(launch_ivf_append_codes(codes, n, cb, d_list, d_pos, reinterpret_cast<uint8_t* const*>(lists_->d_data()),
+                                  lists_->d_ids(), vid0, st));
+  return 0;
+}
+
+int VearchIndex::set_codebook(const float* host) {
+  cudaSetDevice(device_);
+  std::unique_lock<std::shared_mutex> lk(mu_);
+  drain_searches();
+  GB_CUDA(cudaMemcpy(d_cb_, host, (size_t)16 * d_ * 4, cudaMemcpyHostToDevice));
+  return 0;
+}
+int VearchIndex::get_codebook(float* host) const {
+  std::shared_lock<std::shared_mutex> lk(mu_);  // set_codebook and training write it under the exclusive lock
+  cudaSetDevice(device_);
+  GB_CUDA(cudaMemcpy(host, d_cb_, (size_t)16 * d_ * 4, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int VearchIndex::encode_host(const float* x, int64_t n, const int64_t* assign, uint8_t* codes_out) {
+  std::shared_lock<std::shared_mutex> lk(mu_);  // the centroids stay put while the rows are encoded against them
+  cudaSetDevice(device_);
+  cudaStream_t st = thread_stream(device_);
+  Scratch s(st);
+  GB_ALLOC(dx, float, (size_t)n * dpad_, s);
+  GB_CUDA(upload_rows_padded(dx, x, n, d_, dpad_, st));
+  GB_ALLOC(da, int32_t, std::max<int64_t>(n, 1), s);
+  if (mp_.metric == kMetricIP) {
+    std::vector<int32_t> h(n);
+    for (int64_t i = 0; i < n; i++) {
+      if (!assign || assign[i] < 0 || assign[i] >= nlist_) {
+        set_last_error("VEARCH: encode needs each row's list id in [0, nlist) under InnerProduct");
+        return -1;
+      }
+      h[i] = (int32_t)assign[i];
+    }
+    GB_CUDA(cudaMemcpyAsync(da, h.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    GB_CUDA(cudaStreamSynchronize(st));  // h leaves scope
+  }
+  GB_ALLOC(codes, uint8_t, (size_t)n * code_bytes(), s);
+  GB_CUDA(encode_dev(dx, n, da, codes, st));
+  GB_CUDA(cudaMemcpyAsync(codes_out, codes, (size_t)n * code_bytes(), cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int VearchIndex::lut_host(int nq, const float* x, uint8_t* lut_out, float* mult_out) {
+  std::shared_lock<std::shared_mutex> lk(mu_);  // the codebook stays put while the tables are built from it
+  cudaSetDevice(device_);
+  cudaStream_t st = thread_stream(device_);
+  Scratch s(st);
+  GB_ALLOC(dx, float, (size_t)nq * dpad_, s);
+  GB_CUDA(upload_rows_padded(dx, x, nq, d_, dpad_, st));
+  GB_ALLOC(lut, uint8_t, (size_t)nq * nb_ * 16, s);
+  GB_ALLOC(mult, float, nq, s);
+  GB_CUDA(launch_scann_lut(dx, dpad_, nq, d_, mp_.nsubvector, d_cb_, mp_.metric, lut, mult, st));
+  GB_CUDA(cudaMemcpyAsync(lut_out, lut, (size_t)nq * nb_ * 16, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaMemcpyAsync(mult_out, mult, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// ScannSearch over this engine's lists: the table sum (plus <q, c_l> under IP) ranks the entries, filters, tombstones
+// and the score window apply before selection, and with reordering the k' = max(k, recall_num) best are re-ranked
+// exactly from the raw vectors.  recall_num defaults to 100 (both VearchRetrievalParameters constructors).
+int VearchIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xqv, const void* xq_raw,
+                          int k, const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
+                          Scratch& s) {
+  (void)xq_raw;  // no transform
+  cudaStream_t st = s.stream();
+  const float* xq = static_cast<const float*>(xqv);
+  SearchContext c = ctx;
+  c.params.recall_num = mp_.reordering ? (ctx.params.recall_num > 0 ? ctx.params.recall_num : 100) : 0;
+  uint8_t* lut = nullptr;
+  float* mult = nullptr;
+  const float* leaf = coarse_dis;  // read only under IP, where it is replaced by the fixed-order <q, c_l>
+  auto prepare = [&](int, unsigned long long*, bool) {
+    lut = s.alloc_n<uint8_t>((size_t)nq * nb_ * 16);
+    mult = s.alloc_n<float>(nq);
+    if (!lut || !mult) return -1;
+    StageScope stage(this, "scann_lut_kernel", st);
+    GB_CUDA(launch_scann_lut(xq, dpad_, nq, d_, mp_.nsubvector, d_cb_, metric, lut, mult, st));
+    if (metric == kMetricIP) {
+      float* lf = s.alloc_n<float>((size_t)nq * nprobe);
+      if (!lf) return -1;
+      GB_CUDA(launch_scann_leaf(xq, dpad_, nq, probe_ids, nprobe, d_centroids_, dpad_, nlist_, d_, lf, st));
+      leaf = lf;
+    }
+    return 1;
+  };
+  auto launch = [&](int kk, int pg, unsigned long long* partial) {
+    return launch_vearch_scan(lut, mult, leaf, nq, probe_ids, nprobe, pg, lists_->directory(), nb_, kk, metric, f, partial, st);
+  };
+  return scan_query_major_dev("vearch_scan_kernel", c, f, metric, nq, xq, k, nprobe, vearch_scan_max_k(nb_),
+                              "nsubvector " + std::to_string(mp_.nsubvector), out_keys, s, prepare, launch);
+}
+
+// ------------------------------------------------------------------------------------------
 Index* create_index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
@@ -2981,6 +3171,25 @@ Index* create_index(const std::string& type, int d, const ModelParams& mp, int d
       return nullptr;
     }
     return new RaBitQIndex(d, mp, device, seg_shift);
+  }
+  if (type == "VEARCH") {  // VearchModelParams::Parse / Validate (gamma_index_vearch.cc:40-115); the limits are this engine's
+    if (mp.nsubvector > d) {
+      set_last_error("VEARCH: nsubvector [" + std::to_string(mp.nsubvector) + "] above the dimension [" + std::to_string(d) +
+                     "] is not supported by this engine");
+      return nullptr;
+    }
+    const int nb = scann_blocks(d, mp.nsubvector);
+    if (nb > VearchIndex::kMaxBlocks) {
+      set_last_error("VEARCH: " + std::to_string(nb) + " blocks (nsubvector " + std::to_string(mp.nsubvector) + ") above " +
+                     std::to_string(VearchIndex::kMaxBlocks) + " is not supported by this engine");
+      return nullptr;
+    }
+    // every accepted block count must let the scan select k' = 4096 beside its byte-pair table
+    if (vearch_scan_max_k(nb) < 4096) {
+      set_last_error("VEARCH: " + std::to_string(nb) + " blocks are too many for the list scan of this engine");
+      return nullptr;
+    }
+    return new VearchIndex(d, mp, device, seg_shift);
   }
   set_last_error("unsupported index type " + type);
   return nullptr;

@@ -183,6 +183,8 @@ struct ModelParams {  // index/impl/gamma_index_ivfpq.h:1031-1257, gamma_index_i
   int nprobe_arg = 0, nsubvector_arg = 0, nbits_arg = 0;
   int bucket_init_arg = 1000, bucket_max_arg = 1000000;  // GPU_IVFFLAT's defaults (IVFFlatGPUModelParams)
   std::string metric_unknown;
+  double ns_threshold = 0.2;  // VEARCH noise-shaping threshold (VearchModelParams); NaN: no noise shaping
+  bool reordering = false;    // VEARCH exact re-rank of the k' best codes
 };
 
 // gamma's two GPU index types (index/impl/gpu/): GPU_IVFPQ is an IVFPQIndex and GPU_IVFFLAT an IVFFlatIndex, created
@@ -197,6 +199,7 @@ struct RetrievalParams {  // gamma_index_ivfpq.cc:233-294, gamma_index_ivfflat.c
   bool brute_force = false;
   int qb = -1;            // IVFRABITQ query bits, -1 => the index's (a value outside [0, 8] falls back to it)
   bool centered = false;  // IVFRABITQ: parsed, no effect (the estimate already centres the query on the list)
+  bool given = false;     // the parameter string was not empty (VEARCH's defaults depend on it)
 };
 
 struct SearchContext {  // RetrievalContext / SearchCondition (common/gamma_common_data.h:33-121)
@@ -496,7 +499,7 @@ class IvfIndex : public Index {
   // the rows of a batch as the codec takes them (*xc) and each row's nearest list (out): fp32 rows (stride dpad) through
   // transform_dev and assign_dev; BINARYIVF: the packed rows as they are, by Hamming distance
   virtual int assign_batch(const void* x, int64_t n, const void** xc, int32_t* out, Scratch& s);
-  int resolve_nprobe(const SearchContext& ctx) const;
+  virtual int resolve_nprobe(const SearchContext& ctx) const;
   // metric of the coarse quantiser (list assignment and probe choice) for a search under `metric`
   virtual int coarse_metric(int metric) const { return metric; }
   // write rows x [vid0, vid0+n) (as assign_batch left them) into the lists at (d_list, d_pos), after reserve and before
@@ -784,6 +787,54 @@ class RaBitQIndex : public IvfIndex {
 
  private:
   int nb_bits_, qb_;
+};
+
+// GammaVearchIndex (index/impl/scann/gamma_index_vearch.{h,cc}) over ScaNN's asymmetric hashing, restated: IVF lists of
+// 4-bit codes, one per block of the VARIABLE_CHUNK split (kernels_scann.cu, DESIGN.md §3 K14).  Under IP the lists hold
+// anisotropic (noise-shaped) codes of the residuals to spherical centroids and a search adds <q, c_l> to the table sum;
+// under L2 they hold the nearest-centre codes of the raw rows.  reordering re-ranks k' = max(k, recall_num) candidates
+// exactly from the raw vectors.
+class VearchIndex : public IvfIndex {
+ public:
+  static constexpr int kDefaultNlist = 2048, kDefaultNsub = 64;  // VearchModelParams()
+  // blocks above this: the byte-pair table, two code stages and a k' = 4096 queue no longer fit the scan's shared memory
+  // with room to spare
+  static constexpr int kMaxBlocks = 256;
+  static constexpr int kDefaultLeaves = 512;  // GammaVearchIndex::leaves_
+  VearchIndex(int d, const ModelParams& mp, int device, int seg_shift);
+  ~VearchIndex() override;
+  int code_bytes() const override { return (nb_ + 1) / 2; }
+  bool persists_trained_state() const override { return false; }
+  int64_t index_mem_bytes() const override;
+  int nsub() const { return mp_.nsubvector; }
+  int nblocks() const { return nb_; }
+  double ns_threshold() const { return mp_.ns_threshold; }
+  bool reordering() const { return mp_.reordering; }
+  // test hooks: the codebook [16 d] floats (set marks nothing trained by itself), the list codes of n host rows assigned
+  // to `assign` (IP; ignored under L2), the biased uint8 tables [nq][nblocks][16] and multipliers [nq] of a query batch
+  int set_codebook(const float* host);
+  int get_codebook(float* host) const;
+  int encode_host(const float* x, int64_t n, const int64_t* assign, uint8_t* codes_out);
+  int lut_host(int nq, const float* x, uint8_t* lut_out, float* mult_out);
+
+ protected:
+  GammaFileFormat gamma_format() const override { return GammaFileFormat(); }  // Dump and Load touch no file
+  int64_t default_training_threshold() const override { return (int64_t)nlist_ * 256; }
+  KMeansParams coarse_kmeans_params() const override;
+  // the codes are built for the index metric: a request's metric_type does not change the ranking
+  int search_metric(const SearchContext& ctx) const override { (void)ctx; return mp_.metric; }
+  int resolve_nprobe(const SearchContext& ctx) const override;
+  int train_extra(const float* xtrain, int64_t n, Scratch& s) override;
+  int append_batch(const void* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
+                   const std::vector<int>& add, Scratch& s) override;
+  int scan_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, const void* xq_raw, int k,
+               const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* out_keys,
+               Scratch& s) override;
+
+ private:
+  cudaError_t encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st);
+  int nb_;
+  float* d_cb_ = nullptr;  // [16 d]
 };
 
 // host rows n x d (stride d) -> device rows n x dpad, the padding columns zeroed

@@ -20,7 +20,54 @@ namespace gb {
 
 // IVFFlatModelParams::Parse / IVFPQModelParams::Parse (gamma_index_ivfflat.cc:64-196,
 // gamma_index_ivfpq.h:1031-1257)
+// VearchModelParams::Parse (gamma_index_vearch.cc:40-126): ncentroids and nsubvector are required, ns_threshold < 0 means
+// no noise shaping, metric_type defaults to InnerProduct; thread_num has no effect here
+static bool parse_vearch_params(const std::string& text, ModelParams* mp, std::string* err) {
+  JsonValue jv;
+  if (!JsonParser::parse(text, &jv) || jv.type != JsonValue::Object) {
+    *err = "parse vearch retrieval parameters error: " + text;
+    return false;
+  }
+  int v;
+  mp->ncentroids = VearchIndex::kDefaultNlist;
+  mp->nsubvector = VearchIndex::kDefaultNsub;
+  mp->metric = kMetricIP;
+  const char* required[2] = {"ncentroids", "nsubvector"};
+  int* target[2] = {&mp->ncentroids, &mp->nsubvector};
+  for (int i = 0; i < 2; i++) {
+    if (!jv.get_int(required[i], &v)) {
+      *err = std::string("cannot get ") + required[i] + " for vearch, set it when create space";
+      return false;
+    }
+    if (v < -1) {
+      *err = std::string("invalid ") + required[i] + " =" + std::to_string(v);
+      return false;
+    }
+    if (v > 0) *target[i] = v;
+  }
+  mp->has_ncentroids = true;
+  mp->ncentroids_arg = mp->ncentroids;
+  double t;
+  if (jv.get_double("ns_threshold", &t)) mp->ns_threshold = t;
+  std::string mt;
+  if (jv.get_string("metric_type", &mt)) {
+    if (strcasecmp("L2", mt.c_str()) && strcasecmp("InnerProduct", mt.c_str())) {
+      *err = "invalid metric_type = " + mt;
+      return false;
+    }
+    mp->metric = !strcasecmp("L2", mt.c_str()) ? kMetricL2 : kMetricIP;
+  }
+  bool b;
+  if (jv.get_bool("reordering", &b)) mp->reordering = b;
+  // this engine's own keys, as for every type
+  if (jv.get_int("training_threshold", &v) && v > 0) mp->training_threshold = v;
+  std::string stt;
+  if (jv.get_string("store_type", &stt)) mp->host_store = !strcasecmp("RocksDB", stt.c_str());
+  return true;
+}
+
 bool parse_model_params(const std::string& text, const std::string& type, ModelParams* mp, std::string* err) {
+  if (type == "VEARCH") return parse_vearch_params(text, mp, err);
   if (text.empty()) return true;
   const bool gpu = is_gpu_index_type(type);
   JsonValue jv;
@@ -133,6 +180,7 @@ bool parse_retrieval_params(const std::string& text, RetrievalParams* rp, std::s
     *err = "parse retrieval parameters error: " + text;
     return false;
   }
+  rp->given = true;
   std::string mt;
   if (jv.get_string("metric_type", &mt)) rp->metric = !strcasecmp("L2", mt.c_str()) ? kMetricL2 : kMetricIP;
   int v;
@@ -539,6 +587,32 @@ int gb_index_rabitq_encode(gb_index* index, int64_t n, const float* x, const int
 int gb_index_rabitq_estimate(gb_index* index, int nq, const float* x, const int64_t* lists, int qb, int metric, float* out) {
   RQ_OR_FAIL(rq, index);
   return rq->estimate_host(nq, x, lists, qb, metric >= 0 ? metric : rq->metric(), out);
+}
+
+#define VR_OR_FAIL(v, index) AS_OR_FAIL(VearchIndex, v, index, "VEARCH")
+int gb_index_vearch_nsub(gb_index* index) {
+  VR_OR_FAIL(vr, index);
+  return vr->nsub();
+}
+int gb_index_vearch_blocks(gb_index* index) {
+  VR_OR_FAIL(vr, index);
+  return vr->nblocks();
+}
+int gb_index_vearch_set_codebook(gb_index* index, const float* codebook) {
+  VR_OR_FAIL(vr, index);
+  return vr->set_codebook(codebook);
+}
+int gb_index_vearch_get_codebook(gb_index* index, float* codebook) {
+  VR_OR_FAIL(vr, index);
+  return vr->get_codebook(codebook);
+}
+int gb_index_vearch_encode(gb_index* index, int64_t n, const float* x, const int64_t* assign, uint8_t* codes) {
+  VR_OR_FAIL(vr, index);
+  return vr->encode_host(x, n, assign, codes);
+}
+int gb_index_vearch_lut(gb_index* index, int nq, const float* x, uint8_t* lut, float* mult) {
+  VR_OR_FAIL(vr, index);
+  return vr->lut_host(nq, x, lut, mult);
 }
 
 int gb_kmeans(int device, const float* x, int64_t n, int d, int k, int niter, int64_t seed, int spherical,

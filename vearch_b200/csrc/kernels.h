@@ -273,6 +273,27 @@ cudaError_t launch_rabitq_estimate(const float* xq, int64_t ldq, const float* ce
                                    int metric, ListDirectory dir, const int32_t* q_of, const int32_t* l_of,
                                    const int64_t* out_off, int npairs, float* out, cudaStream_t st);
 
+// ---- K14: VEARCH (kernels_scann.cu): anisotropic 4-bit codes, fixed-point tables, scan ------------------------------
+// blocks of a d-dimensional vector split into nsub: nsub of d / nsub dims, plus one of d % nsub dims when that is > 0.
+// The codebook is [16 d] floats: block b's 16 centres of width_b floats each, from float 16 * b * (d / nsub).
+int scann_blocks(int d, int nsub);
+// codes[i] ((nb + 1) / 2 bytes, block 2j in the low nibble of byte j): lists non-null (IP) codes the residual
+// x_i - cents[lists[i]], by CoordinateDescentAHQuantize when ns_threshold is not NaN, else the nearest centre per block;
+// lists null (L2): the nearest centre per block of the raw row
+cudaError_t launch_scann_encode(const float* x, int64_t ldx, int64_t n, const int32_t* lists, const float* cents, int64_t ldc,
+                                int d, int nsub, const float* codebook, double ns_threshold, uint8_t* codes, cudaStream_t st);
+// per query: the [nb][16] float table (IP -<q_b, c>, L2 |q_b - c|^2) as biased uint8 lut, and its multiplier mult[q]
+cudaError_t launch_scann_lut(const float* xq, int64_t ldq, int nq, int d, int nsub, const float* codebook, int metric,
+                             uint8_t* lut, float* mult, cudaStream_t st);
+// leaf[q][p] = <q, cents[probe_ids[q][p]]> (fp32, dims in order; 0 for a probe < 0)
+cudaError_t launch_scann_leaf(const float* xq, int64_t ldq, int nq, const int32_t* probe_ids, int nprobe, const float* cents,
+                              int64_t ldc, int nlist, int d, float* leaf, cudaStream_t st);
+// query-major scan of the probed lists: partial[q][group][k] sorted, as launch_ivfpq_scan; leaf [nq][nprobe] read under IP
+cudaError_t launch_vearch_scan(const uint8_t* lut, const float* mult, const float* leaf, int nq, const int32_t* probe_ids,
+                               int nprobe, int pg, ListDirectory dir, int nb, int k, int metric, FilterArgs f,
+                               unsigned long long* partial, cudaStream_t st);
+int vearch_scan_max_k(int nb);  // the largest k (<= 4096) the scan can select at nb blocks, 0 if none
+
 // ---- K6/K8: build-side kernels ------------------------------------------------------------
 // centroids[c] = (sum of x[perm[off[c]..off[c+1])] in that order) * (1/count); empty => zeros
 cudaError_t launch_segment_mean(const float* x, int64_t ldx, int d, const int32_t* perm, const int32_t* off, int k,

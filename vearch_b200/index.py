@@ -501,6 +501,54 @@ class RaBitQIndex(GammaIndex):
         return [out[off[j]:off[j + 1]].copy() for j in range(len(lens))]
 
 
+class VearchIndex(GammaIndex):
+    """VEARCH (gamma_index_vearch.cc over ScaNN's asymmetric hashing): IVF over 4-bit codes, one per block of
+    d / nsubvector dims (plus one block of the d % nsubvector remaining dims).  Under InnerProduct the codes are the
+    anisotropic (noise-shaped) codes of the residuals to spherical centroids, under L2 the nearest-centre codes of the raw
+    rows.  ncentroids and nsubvector are required parameters.  The contract is DESIGN.md section 3, K14 (numpy twin:
+    oracle_scann)."""
+
+    def __init__(self, d, params=None, device=0, store_type=None):
+        super().__init__("VEARCH", d, params, device, store_type)
+
+    @property
+    def nsub(self):
+        return int(_lib.lib().gb_index_vearch_nsub(self._h))
+
+    @property
+    def blocks(self):
+        return int(_lib.lib().gb_index_vearch_blocks(self._h))
+
+    def set_codebook(self, cb):
+        """The 16 d floats of the per-block codebooks (block b's 16 centres, from float 16 b (d // nsub))."""
+        cb = _f32(cb).reshape(-1)
+        assert cb.size == 16 * self.d
+        _check(_lib.lib().gb_index_vearch_set_codebook(self._h, _ptr(cb)), "vearch_set_codebook")
+
+    def get_codebook(self):
+        out = np.empty(16 * self.d, np.float32)
+        _check(_lib.lib().gb_index_vearch_get_codebook(self._h, _ptr(out)), "vearch_get_codebook")
+        return out
+
+    def encode(self, x, assign=None):
+        """List codes (uint8 [n, code_size]) of rows x: of their residuals to the lists `assign` under InnerProduct, of
+        the rows themselves under L2 (assign ignored)."""
+        x = _f32(x)
+        assign = None if assign is None else np.ascontiguousarray(assign, np.int64)
+        codes = np.empty((x.shape[0], self.code_size), np.uint8)
+        _check(_lib.lib().gb_index_vearch_encode(self._h, x.shape[0], _ptr(x), _ptr(assign), _ptr(codes)), "vearch_encode")
+        return codes
+
+    def lut(self, x):
+        """The biased uint8 tables [nq, blocks, 16] of a query batch and their fixed-point multipliers [nq]."""
+        x = _f32(x)
+        nq = x.shape[0]
+        lut = np.empty((nq, self.blocks, 16), np.uint8)
+        mult = np.empty(nq, np.float32)
+        _check(_lib.lib().gb_index_vearch_lut(self._h, nq, _ptr(x), _ptr(lut), _ptr(mult)), "vearch_lut")
+        return lut, mult
+
+
 def index_factory(d, description, metric=METRIC_L2, device=0, **extra):
     """index/index.h index_factory: "IVF1024,Flat" | "IVF4096,PQ16x8" | "IVF256,PQ32x4" (PQ<M>x<nbits>) | "Flat"."""
     parts = [p.strip() for p in description.split(",")]
