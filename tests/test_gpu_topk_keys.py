@@ -271,7 +271,7 @@ def test_ivfpq_query_major(metric, d, M, regime):
 
 
 def test_ivfpq_large_m_limits():
-    """M = 128: the [128][256] fp32 table leaves room for a queue of k' <= 2048 only; M >= 149 cannot search at all and
+    """M = 128: the [128][256] fp32 table leaves room for a queue of k' <= 2048 only; M >= 147 cannot search at all and
     is refused at create, naming nsubvector (the default nsubvector = d / 2 included)"""
     d, n, nq = 256, 6000, 4
     db, xq = make_data("pool", n, d, nq, L2, seed=5)

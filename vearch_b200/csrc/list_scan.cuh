@@ -349,7 +349,12 @@ size_t list_scan_smem(const Codec& c, int k, int* KP_out = nullptr, int* SORTN_o
   return (size_t)ls_table_entries(c) * sizeof(typename Codec::Entry) + (size_t)SORTN * 8 +
          (size_t)LS_NST * tile_e * c.code_bytes() + (LsCodeSum<Codec>::value ? 16 : 0);
 }
-constexpr size_t kListScanMaxSmem = 227 * 1024;
+// A CTA's shared memory, static and dynamic together, is at most 227 KiB on sm_90.  The kernel's own static arrays
+// (CandQueue's histogram, the probe group's tables, the barriers) take 2688 to 2816 bytes depending on the codec, so
+// the dynamic window gets what is left after a 3 KiB reserve; without it a scan within ~3 KiB of the cap was accepted
+// here and refused by cudaFuncSetAttribute.  GPU_IVFPQ at M = 128, k' = 2048 needs exactly this window.
+constexpr size_t kListScanStaticSmem = 3 * 1024;
+constexpr size_t kListScanMaxSmem = 227 * 1024 - kListScanStaticSmem;
 
 // the largest k (<= 4096) a codec's scan can select, 0 if none: the shared memory grows with k only through KP
 template <class Codec>
