@@ -2186,7 +2186,7 @@ const float* IVFPQIndex::train_transform(const float* xt, int64_t n_in, Scratch&
 IVFPQIndex::~IVFPQIndex() {
   if (d_opq_) cudaFree(d_opq_);
   cudaFree(d_table_);
-  cudaFree(d_cb16_);
+  cudaFree(d_cb8_);
   cudaFree(d_cbnrm_);
   if (pqn_.base) cudaFree(pqn_.base);
   if (pqn_.d_off) cudaFree(pqn_.d_off);
@@ -2207,12 +2207,12 @@ int64_t IVFPQIndex::index_mem_bytes() const {
 }
 int IVFPQIndex::codebook_changed(cudaStream_t st) {
   pq_gen_++;  // the per-entry norm cache belongs to the previous codebook
-  // tables of the tensor-core filter (kernels_pqtc.cu): fp16 codebook pre-scaled by -2 sb (L2) / -sb (IP), sb a power of two,
-  // centroid norms, and the bound on |r| its error margin uses
+  // tables of the tensor-core filter (kernels_pqtc.cu): int8 codebook (one scale sb), centroid norms, and the bounds on
+  // |r| and on its quantisation error that its error margin uses
   if (ksub_ == 256 && pqtc_supported(M_, dsub_)) {
-    if (!d_cb16_) GB_CUDA(cudaMalloc(&d_cb16_, (size_t)M_ * 256 * dsub_ * 2));
+    if (!d_cb8_) GB_CUDA(cudaMalloc(&d_cb8_, (size_t)M_ * 256 * dsub_));
     if (!d_cbnrm_) GB_CUDA(cudaMalloc(&d_cbnrm_, ((size_t)M_ * 256 + 4) * 4));
-    GB_CUDA(launch_pqtc_tables(d_pq_, M_, dsub_, mp_.metric, d_cb16_, d_cbnrm_, d_cbnrm_ + (size_t)M_ * 256, st));
+    GB_CUDA(launch_pqtc_tables(d_pq_, M_, dsub_, d_cb8_, d_cbnrm_, d_cbnrm_ + (size_t)M_ * 256, st));
   }
   if (mp_.metric != kMetricL2) return 0;  // IP: tab = ip table, dis0 = <x, centroid>
   if (!d_table_) GB_CUDA(cudaMalloc(&d_table_, (size_t)nlist_ * M_ * ksub_ * 4));
@@ -2301,7 +2301,7 @@ int IVFPQIndex::ensure_pq_norms(cudaStream_t st) {
 int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const float* xq, int kk, const float* ip,
                                   const int32_t* probe_ids, const float* coarse_dis, int nprobe,
                                   unsigned long long* adc_out, bool need_sorted, Scratch& s) {
-  if (ksub_ != 256 || !d_cb16_ || !pqtc_supported(M_, dsub_) || dpad_ != d_) return 1;  // the filter reads 8-bit codes
+  if (ksub_ != 256 || !d_cb8_ || !pqtc_supported(M_, dsub_) || dpad_ != d_) return 1;  // the filter reads 8-bit codes
   if (kk > 2048 || nprobe < 2 || nprobe > 65535 || nq > 65535) return 1;  // (query, probe) travel as 16-bit fields of a candidate record
   const int64_t npairs = (int64_t)nq * nprobe;
   if (npairs < (int64_t)nlist_ * 32) return 1;  // < 32 queries per list on average
@@ -2350,7 +2350,7 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   const int64_t max_items = max_groups * nseg;
   if (max_items > INT32_MAX) return 1;
   GB_ALLOC(d_cand_cnt, int, nq, s);
-  const size_t tile_bytes = (size_t)(d_ / 8) * 2048;
+  const size_t tile_bytes = (size_t)(d_ / 16) * 2048;
   const size_t a_bytes = (size_t)max_groups * 2 * tile_bytes;
   const size_t meta_bytes = (size_t)max_groups * pq_group * pqtc_pair_meta_bytes();
   const size_t cand_bytes = (size_t)nq * cap * 8;
@@ -2369,7 +2369,7 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   stage_end(st);
   scan_timer_begin(st);  // the dominant kernel: the roofline in bench.py is this launch alone
   stage_begin("pqtc_scan_kernel", st);
-  GB_CUDA(launch_pqtc_scan(a_scratch, meta, d_cb16_, pqn_.base, pqn_.d_off, g.items, (int)max_items, g.totals, dir, M_, dsub_, f,
+  GB_CUDA(launch_pqtc_scan(a_scratch, meta, d_cb8_, pqn_.base, pqn_.d_off, g.items, (int)max_items, g.totals, dir, M_, dsub_, f,
                            metric, d_cand_cnt, cand, cap, nsm, st));
   stage_end(st);
   scan_timer_end(st);

@@ -660,8 +660,8 @@ class IVFPQIndex : public IvfPqBase {
   int nbits_;
   float* d_table_ = nullptr;  // [nlist][M][ksub] (L2 only)
   // the tensor-core filter and its tables exist at nbits = 8 only; packed codes are scanned query-major
-  uint16_t* d_cb16_ = nullptr;  // [M][256][dsub] fp16, pre-scaled (tensor-core filter)
-  float* d_cbnrm_ = nullptr;    // [M][256] |pq|^2, then rmax2, sb
+  int8_t* d_cb8_ = nullptr;     // [M][256][dsub] int8 codebook (tensor-core filter)
+  float* d_cbnrm_ = nullptr;    // [M][256] |pq|^2, then R^2, sb, D
   // |r_e|^2 of every list entry (L2), flat with 32-entry aligned list segments: built by the first list-major search
   // after the lists or the codebook changed (lists are append-only: same list set + same lengths = same content)
   struct PqNormCache {

@@ -186,15 +186,15 @@ cudaError_t launch_ivfpq_packed_scan(const float* ip_table, int nq, const int32_
 // ---- K5 list-major: tensor-core filter + exact re-score (kernels_pqtc.cu) ---------------------------
 bool pqtc_supported(int M, int dsub);
 size_t pqtc_pair_meta_bytes();
-// cb[m][c][.] = fp16(-2 sb pq) (L2) / fp16(-sb pq) (IP), sb = rmax2[1] a power of two; nrm[m][c] = |pq[m][c]|^2; rmax2[0] = sum_m max_c nrm
-cudaError_t launch_pqtc_tables(const float* pq, int M, int dsub, int metric, uint16_t* cb, float* nrm, float* rmax2,
-                               cudaStream_t st);
+// cb[m][c][.] = int8 rn(pq / sb), sb = rmax2[1] = max |pq| / 127; nrm[m][c] = |pq[m][c]|^2; rmax2[0] = sum_m max_c nrm;
+// rmax2[2] = sqrt(sum_m max_c |pq[m][c] - sb cb[m][c]|^2)
+cudaError_t launch_pqtc_tables(const float* pq, int M, int dsub, int8_t* cb, float* nrm, float* rmax2, cudaStream_t st);
 // phase A's plan: per query its first P_q probes in full (fewest with >= target entries together, at most pa_max);
 // probes_a / probes_b = probe_ids with the other phase's probes set to -1, row_limit[q][p] = rows phase A scores exactly
 cudaError_t launch_pqtc_plan_phase_a(const int32_t* probe_ids, int64_t npairs, int nprobe, int pa_max, long long target,
                                      const int* list_len, int32_t* probes_a, int32_t* probes_b, int* row_limit,
                                      cudaStream_t st);
-// per pair group: fp16 operand tile (rows scaled by their own power of two) of (x - centroid) (L2) / x (IP) rows + the pairs' filter thresholds from
+// per pair group: int8 operand tile (each row rn(a / sa), sa = max |a| / 127) of a = x - centroid (L2) / x (IP) + the pairs' filter thresholds from
 // bound_keys[q][kprime - 1] (phase A's k'-th key); queries without a bound get cand_cnt = cap + 1
 cudaError_t launch_pq_stage_pairs(const float* xq, int64_t ldq, int d, const float* coarse, int64_t ldc, const LmTile* items,
                                   int max_items, const int64_t* totals, const int64_t* pair_j, int nprobe,
@@ -202,7 +202,7 @@ cudaError_t launch_pq_stage_pairs(const float* xq, int64_t ldq, int d, const flo
                                   int kprime, const float* rmax2, FilterArgs f, int metric, unsigned char* a_scratch,
                                   void* meta, int* cand_cnt, int cap, const int* row_limit, cudaStream_t st);
 // persistent kernel, one CTA per SM: candidates (probe << 32 | position) appended to cand[q][cap]
-cudaError_t launch_pqtc_scan(const unsigned char* a_scratch, const void* meta, const uint16_t* cb, const float* pqnorm, const int64_t* pqnorm_off,
+cudaError_t launch_pqtc_scan(const unsigned char* a_scratch, const void* meta, const int8_t* cb, const float* pqnorm, const int64_t* pqnorm_off,
                              const LmTile* items, int max_items, const int64_t* totals, ListDirectory dir, int M, int dsub,
                              FilterArgs f, int metric, int* cand_cnt, unsigned long long* cand, int cap, int num_sms,
                              cudaStream_t st);

@@ -9,22 +9,22 @@
 // LDS wavefronts, not by HBM.  When every list is probed by dozens of queries of the same batch the
 // same numbers are a dense contraction:
 //     sum_m tab[m][code[m]] = |r_e|^2 - 2 <x - c_list, r_e>,   r_e = the entry's PQ reconstruction,
-// i.e. (query, list) pairs x decoded entries.  This file computes THAT with wgmma in fp16 (power-of-two scaled) and uses it
+// i.e. (query, list) pairs x decoded entries.  This file computes THAT with wgmma on int8 operands (exact s32 sums) and uses it
 // only as a FILTER; every number that leaves the pipeline is recomputed with the reference's own
 // arithmetic, so results stay bit-identical to the LUT kernel and to the oracle:
 //
 //   phase A  the exact LUT kernel scans each query's leading probes in full (the fewest whose lists hold
 //            >= 4 k' entries, pqtc_plan_phase_a_kernel) and yields k' exact keys, unordered, the largest --
 //            B_q, an upper bound of the query's final k'-th score -- in slot k' - 1;
-//   phase B  (this file) for the remaining probes: pairs grouped by list (lmk_group), per group a
-//            fp16 operand tile of sa * (x - c_list) rows staged once (pq_stage_pairs_kernel), then a
+//   phase B  (this file) for the remaining probes: pairs grouped by list (lmk_group), per group an
+//            int8 operand tile of rn((x - c_list) / sa) rows staged once (pq_stage_pairs_kernel), then a
 //            persistent warp-specialised kernel (pqtc_scan_kernel) decodes 128 entries at a time
-//            from their codes into the second operand (codebook in shared memory, pre-scaled by -2),
+//            from their codes into the second operand (int8 codebook rn(pq / sb) in shared memory),
 //            multiplies up to 256 pairs x 128 entries x d on the tensor core (two consumer warpgroups of 128
 //            pairs share each decoded tile) and compares
-//            acc + |r_e|^2 against  B_q - dis0 + eps(pair).  eps bounds |approximate - reference fp32|
-//            rigorously (fp16 rounding of both operands: 2^-10 |a||r| ; fp32 noise of both evaluations),
-//            so every entry whose reference score is <= B_q passes.  |r_e|^2 comes from a per-entry cache
+//            |r_e|^2 - 2 sa sb acc against  B_q - dis0 + eps(pair).  eps bounds |approximate - reference fp32|
+//            rigorously (int8 quantisation of both operands, Cauchy-Schwarz over the quantisation errors; fp32
+//            noise of both evaluations), so every entry whose reference score is <= B_q passes.  |r_e|^2 comes from a per-entry cache
 //            in HBM (pq_entry_norms_kernel), streamed with the codes.  Passing entries (a few per query)
 //            go through a shared-memory queue to a drain warp that appends (probe, position) to the
 //            query's candidate list, so no global atomic sits in the epilogue;
@@ -33,10 +33,10 @@
 //   A query whose candidate list overflows (no usable bound, adversarial data) is redone by the
 //   exact kernel over all its probes (flag-gated launch), so the result never depends on the filter.
 //
-// Operand layout: canonical no-swizzle K-major tiles of fp16 (8-row x 16-byte core matrices,
-// LBO 2048 = next core matrix along K, SBO 128 = next 8 rows).  With dsub = 8 a sub-quantiser's
-// centroid IS one 16-byte core-matrix row: decoding an entry is M x (LDS.128 from the codebook,
-// STS.128 into the tile), conflict-free on the store side (consecutive entries -> consecutive rows).
+// Operand layout: canonical no-swizzle K-major tiles of int8 (8-row x 16-byte core matrices,
+// LBO 2048 = next core matrix along K, SBO 128 = next 8 rows).  A centroid is dsub bytes: with dsub = 8
+// two sub-quantisers fill one 16-byte core-matrix row (2 x LDS.64 from the codebook, one STS.128 into
+// the tile), conflict-free on the store side (consecutive entries -> consecutive rows).
 //
 // Algorithmic bytes: (M + 8) per scanned entry per 256-pair group instead of per pair.
 #include <float.h>
@@ -64,7 +64,7 @@ constexpr int PT_KSUB = 256;
 
 struct PtShared {
   uint64_t code_full[PT_CS], code_empty[PT_CS];
-  uint64_t b_full[2], b_empty[2], a_full, a_empty, acc_empty[2];
+  uint64_t b_full[2], b_empty[2], a_full[2], a_empty[2], acc_empty[2];
   alignas(16) float ne[2][PT_N];  // |r_e|^2 of the tile's entries, +inf = can never be returned
   // candidate queue: the epilogue warps append (query, probe, position) records with shared-memory atomics and move on;
   // the drain warp turns them into the global per-query lists.  A global atomicAdd-with-return costs ~1 us of latency:
@@ -74,23 +74,15 @@ struct PtShared {
   unsigned long long q_rec[PT_RQ];  // (q << 48 | p << 32 | pos), kRecEmpty = free slot
 };
 
-__device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
-  uint32_t r;
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));  // first source -> upper half
-  return r;
-}
-// power of two that brings a magnitude `mx` into [2^13, 2^14): fp16 keeps 11 significant bits there and a further
-// factor 2 (the -2 of the L2 form) still fits below 65504
-__device__ __forceinline__ float pow2_scale_for(float mx) { return mx > 0.f && mx < INFINITY ? ldexpf(1.0f, 13 - ilogbf(mx)) : 1.0f; }
-
 // ---- tables derived from the PQ codebook ---------------------------------------------------------
-// sb = power of two scaling the largest codebook component into [2^13, 2^14) (exact in fp32 and fp16);
-// cb[m][c][0..dsub) = fp16(scale * sb * pq[m][c][.]),  nrm[m][c] = |pq[m][c]|^2 (fp32, L2 only),
-// rmax2[0] = sum_m max_c |pq[m][c]|^2,  rmax2[1] = sb   (single CTA of 256 threads)
+// sb = max |pq| / 127 (one scale for the whole codebook); cb[m][c][0..dsub) = int8 rn(pq[m][c][.] / sb);
+// nrm[m][c] = |pq[m][c]|^2 (fp32, L2 only); rmax2[0] = R^2 = sum_m max_c |pq[m][c]|^2, rmax2[1] = sb (0 when the codebook
+// is all zero or not finite: no filter), rmax2[2] = D = sqrt(sum_m max_c |pq[m][c] - sb cb[m][c]|^2), the largest
+// quantisation error of a reconstruction   (single CTA of 256 threads)
 __global__ void __launch_bounds__(256)
-    pqtc_tables_kernel(const float* __restrict__ pq, int M, int dsub, float scale, uint16_t* __restrict__ cb,
-                       float* __restrict__ nrm, float* __restrict__ rmax2) {
-  __shared__ float s_max[256];
+    pqtc_tables_kernel(const float* __restrict__ pq, int M, int dsub, int8_t* __restrict__ cb, float* __restrict__ nrm,
+                       float* __restrict__ rmax2) {
+  __shared__ float s_max[256], s_err[256];
   const int c = threadIdx.x;
   float mx = 0.f;
   for (int i = c; i < M * PT_KSUB * dsub; i += 256) mx = fmaxf(mx, fabsf(pq[i]));
@@ -100,29 +92,33 @@ __global__ void __launch_bounds__(256)
     if (c < off) s_max[c] = fmaxf(s_max[c], s_max[c + off]);
     __syncthreads();
   }
-  const float sb = pow2_scale_for(s_max[0]);
+  const float cbmax = s_max[0];
+  const bool ok = cbmax > 0.f && cbmax < INFINITY;
+  const float sb = ok ? cbmax / 127.f : 0.f, inv = ok ? 127.f / cbmax : 0.f;
   __syncthreads();
-  float total = 0.f;
+  float total = 0.f, err = 0.f;
   for (int m = 0; m < M; m++) {
     const float* p = pq + ((int64_t)m * PT_KSUB + c) * dsub;
-    float n2 = 0.f;
+    float n2 = 0.f, e2 = 0.f;
     for (int j = 0; j < dsub; j++) {
       const float v = p[j];
       n2 = fmaf(v, v, n2);
-      const uint32_t b = pack_f16x2(scale * sb * v, 0.f);
-      cb[((int64_t)m * PT_KSUB + c) * dsub + j] = (uint16_t)(b & 0xFFFFu);
+      const int qv = max(-127, min(127, __float2int_rn(v * inv)));
+      const float dv = v - sb * (float)qv;
+      e2 = fmaf(dv, dv, e2);
+      cb[((int64_t)m * PT_KSUB + c) * dsub + j] = (int8_t)qv;
     }
     nrm[m * PT_KSUB + c] = n2;
-    s_max[c] = n2;
+    s_max[c] = n2, s_err[c] = e2;
     __syncthreads();
     for (int off = 128; off > 0; off >>= 1) {
-      if (c < off) s_max[c] = fmaxf(s_max[c], s_max[c + off]);
+      if (c < off) s_max[c] = fmaxf(s_max[c], s_max[c + off]), s_err[c] = fmaxf(s_err[c], s_err[c + off]);
       __syncthreads();
     }
-    total += s_max[0];
+    total += s_max[0], err += s_err[0];
     __syncthreads();
   }
-  if (threadIdx.x == 0) rmax2[0] = total, rmax2[1] = sb;
+  if (threadIdx.x == 0) rmax2[0] = total, rmax2[1] = sb, rmax2[2] = sqrtf(err);
 }
 
 // ---- phase A's plan ---------------------------------------------------------------------------------------------------
@@ -157,10 +153,16 @@ __global__ void pqtc_plan_phase_a_kernel(const int32_t* __restrict__ probe_ids, 
 }
 
 // ---- per pair group: the A operand tile and the pairs' thresholds ---------------------------------
+// The accumulator of pair (query, list) and entry e is the exact integer acc = <qa, qr_e>, biased by kAccBias: its bits
+// read as a float are 12582912 + acc exactly (|acc| <= 127^2 d < 2^22).  The filter evaluates v = ne * c - (bias + acc)
+// = (ne - f s acc) / (f s) - bias with one fma, f = 2 (L2) / 1 (IP), s = sa sb; v <= thr passes.
+constexpr uint32_t kAccBias = 0x4B400000u;  // 1.5 * 2^23: floats in [2^23, 2^24) step by 1 per unit of their bits
+constexpr double kAccBiasF = 12582912.0;
+
 struct PairMeta {
-  float thr;  // candidate  <=>  acc + c * ne <= thr   (thr, lo already multiplied by c)
-  float lo;   // ... and acc + c * ne >= lo  (the other side of the score window, checked on the rare path)
-  float c;    // sa * sb: the operands' power-of-two scales (accumulator = c * (-2 <a, r>))
+  float thr;  // candidate  <=>  v = fma(ne, c, -(bias + acc)) <= thr
+  float lo;   // ... and v >= lo  (the other side of the score window, checked on the rare path)
+  float c;    // 1 / (f sa sb): accumulator units per score unit
   int q, p;
   int lim;    // rows [0, lim) of this pair's list were scored exactly by phase A: never candidates
 };
@@ -182,7 +184,7 @@ __global__ void __launch_bounds__(PT_G)
   if (t.seg != 0) return;  // one staging per pair group: the first item of the group owns the slot
   const int h = threadIdx.x / PT_M, r = threadIdx.x % PT_M;
   const int n0 = (t.npairs + 1) / 2;  // pairs of tile 0
-  const int kc_n = d / 8;
+  const int kc_n = d / 16;
   unsigned char* tile = a_scratch + ((int64_t)t.grp * 2 + h) * ((int64_t)kc_n * 2048);
   PairMeta pm{-INFINITY, INFINITY, 1.0f, -1, 0, 0};
   const float* x = nullptr;
@@ -194,77 +196,104 @@ __global__ void __launch_bounds__(PT_G)
     x = xq + (int64_t)pm.q * ldq;
     c = coarse + (int64_t)t.list * ldc;
   }
-  // pass 1: norms and the largest component of the row a = x - c (L2) / x (IP)
+  // the row a = x - c (L2) / x (IP), 16 components (one core-matrix row of int8) at a time
+  auto load16 = [&](int kc, float (&a)[16]) {
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const float4 v = __ldg(reinterpret_cast<const float4*>(x + kc * 16 + 4 * u));
+      a[4 * u] = v.x, a[4 * u + 1] = v.y, a[4 * u + 2] = v.z, a[4 * u + 3] = v.w;
+    }
+  };
+  // pass 1: norms and the largest component of a
   float na2 = 0.f, nx2 = 0.f, nc2 = 0.f, amax = 0.f;
   if (x) {
     for (int kc = 0; kc < kc_n; kc++) {
-      const float4 x0 = __ldg(reinterpret_cast<const float4*>(x + kc * 8)), x1 = __ldg(reinterpret_cast<const float4*>(x + kc * 8 + 4));
-      float a[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+      float a[16];
+      load16(kc, a);
       if (METRIC == kMetricL2) {
-        const float4 c0 = __ldg(reinterpret_cast<const float4*>(c + kc * 8)), c1 = __ldg(reinterpret_cast<const float4*>(c + kc * 8 + 4));
-        const float cc[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
 #pragma unroll
-        for (int u = 0; u < 8; u++) {
-          nx2 = fmaf(a[u], a[u], nx2);
-          nc2 = fmaf(cc[u], cc[u], nc2);
-          a[u] -= cc[u];
+        for (int u = 0; u < 4; u++) {
+          const float4 cv = __ldg(reinterpret_cast<const float4*>(c + kc * 16 + 4 * u));
+          const float cc[4] = {cv.x, cv.y, cv.z, cv.w};
+#pragma unroll
+          for (int v = 0; v < 4; v++) {
+            nx2 = fmaf(a[4 * u + v], a[4 * u + v], nx2);
+            nc2 = fmaf(cc[v], cc[v], nc2);
+            a[4 * u + v] -= cc[v];
+          }
         }
       }
 #pragma unroll
-      for (int u = 0; u < 8; u++) na2 = fmaf(a[u], a[u], na2), amax = fmaxf(amax, fabsf(a[u]));
+      for (int u = 0; u < 16; u++) na2 = fmaf(a[u], a[u], na2), amax = fmaxf(amax, fabsf(a[u]));
     }
   }
-  // pass 2: the row as fp16(sa * a), sa a power of two (exact), in the canonical K-major operand layout
-  const float sa = pow2_scale_for(amax);
+  // pass 2: qa = rn(a / sa), sa = amax / 127, as int8 in the canonical K-major operand layout; da2 = |a - sa qa|^2
+  const bool a_ok = amax > 0.f && amax < INFINITY;
+  const float sa = a_ok ? amax / 127.f : 0.f, inv = a_ok ? 127.f / amax : 0.f;
+  float da2 = 0.f;
   for (int kc = 0; kc < kc_n; kc++) {
-    uint4 out = make_uint4(0u, 0u, 0u, 0u);
+    uint32_t wv[4] = {0u, 0u, 0u, 0u};
     if (x) {
-      const float4 x0 = __ldg(reinterpret_cast<const float4*>(x + kc * 8)), x1 = __ldg(reinterpret_cast<const float4*>(x + kc * 8 + 4));
-      float a[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+      float a[16];
+      load16(kc, a);
       if (METRIC == kMetricL2) {
-        const float4 c0 = __ldg(reinterpret_cast<const float4*>(c + kc * 8)), c1 = __ldg(reinterpret_cast<const float4*>(c + kc * 8 + 4));
-        a[0] -= c0.x, a[1] -= c0.y, a[2] -= c0.z, a[3] -= c0.w, a[4] -= c1.x, a[5] -= c1.y, a[6] -= c1.z, a[7] -= c1.w;
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+          const float4 cv = __ldg(reinterpret_cast<const float4*>(c + kc * 16 + 4 * u));
+          a[4 * u] -= cv.x, a[4 * u + 1] -= cv.y, a[4 * u + 2] -= cv.z, a[4 * u + 3] -= cv.w;
+        }
       }
-      out.x = pack_f16x2(sa * a[0], sa * a[1]), out.y = pack_f16x2(sa * a[2], sa * a[3]);
-      out.z = pack_f16x2(sa * a[4], sa * a[5]), out.w = pack_f16x2(sa * a[6], sa * a[7]);
+#pragma unroll
+      for (int u = 0; u < 16; u++) {
+        const int qv = max(-127, min(127, __float2int_rn(a[u] * inv)));
+        const float dv = a[u] - sa * (float)qv;
+        da2 = fmaf(dv, dv, da2);
+        wv[u >> 2] |= ((uint32_t)qv & 0xFFu) << (8 * (u & 3));
+      }
     }
-    *reinterpret_cast<uint4*>(tile + (int64_t)kc * 2048 + r * 16) = out;
+    *reinterpret_cast<uint4*>(tile + (int64_t)kc * 2048 + r * 16) = make_uint4(wv[0], wv[1], wv[2], wv[3]);
   }
   if (x) {
     const float dis0 = coarse_dis[(int64_t)pm.q * nprobe + pm.p];
     pm.lim = row_limit ? row_limit[(int64_t)pm.q * nprobe + pm.p] : 0;
     const unsigned long long bk = bound_keys[(int64_t)pm.q * bound_stride + kprime - 1];
-    const float R2 = rmax2[0], R = sqrtf(R2);
-    pm.c = sa * rmax2[1];
+    const float R2 = rmax2[0], R = sqrtf(R2), sb = rmax2[1], Dq = rmax2[2];
     // eps below has relative terms only.  Near fp32's subnormal range (|a|^2 or the codebook's largest |r|^2 below
-    // 2^-96) the roundings of the exact table evaluation are absolute (2^-149 each) and can exceed it: no filter there
+    // 2^-96) the roundings of the exact table evaluation are absolute (2^-149 each) and can exceed it: no filter there.
+    // A zero or non-finite row or codebook has no int8 scale: no filter either
     const bool tiny = (amax > 0.f && na2 < 0x1p-96f) || (R2 > 0.f && R2 < 0x1p-96f);
-    if (bk == kKeySentinel || tiny) {
+    if (bk == kKeySentinel || tiny || !a_ok || !(sb > 0.f && sb < INFINITY)) {
       // phase A found fewer than k' entries (no bound), or the bound would not hold -> the exact kernel redoes this query
       atomicMax(cand_cnt + pm.q, cap + 1);
     } else {
+      // |<a, r> - s <qa, qr>| = |<da, r> + <sa qa, dr>| <= |da| R + (|a| + |da|) D   (Cauchy-Schwarz; da = a - sa qa,
+      //   dr = r - sb qr, |r| <= R and |dr| <= D for every entry, s = sa sb, the products s <qa, qr> are exact integers
+      //   times s); the 5 % slack covers the fp32 roundings of |a|, |da|, R and D.  Scores scale it by f = 2 (L2) / 1 (IP).
+      // + fp32 noise of the reference evaluation, bounded by 2^-17 of the magnitudes that enter it
+      // + the filter's own fp32: v = fma(ne, c, -(bias + acc)) rounds once at magnitude < 2^24 + ne c (<= 1 unit of
+      //   1 / (f s), i.e. f s in score units, plus 2^-24 ne) and c = fl(1 / (f s)) is off by 2^-24 relative (2^-24 ne)
+      const double na = sqrt((double)na2), da = sqrt((double)da2), s = (double)sa * (double)sb;
+      const double f = METRIC == kMetricL2 ? 2.0 : 1.0;
+      const double quant = f * 1.05 * (da * R + (na + da) * Dq);
       const float B = ord2score((uint32_t)(bk >> 32), METRIC);
-      float thr, lo;
+      double thr, lo;
       if (METRIC == kMetricL2) {
-        // |approx - reference| <= 2^-10 (1 + 2^-12) |a| |r|: fp16 rounding (unit roundoff 2^-12) of both operands of
-        //   -2 <a, r>; the power-of-two scales are exact, components below fp16's normal range are >= 2^27 times
-        //   smaller than the row's largest and fall inside the 5 % slack, as does the fp32 accumulation of the MMA
-        //   (<= 2^-15 |a| |r| for d <= 4096 even if every add truncated)
-        //   + fp32 noise of the reference evaluation, bounded by 2^-17 of the magnitudes that enter it
-        const float Z = fabsf(dis0) + R2 + 2.f * (sqrtf(nx2) + sqrtf(nc2)) * R;
-        const float eps = 1.05f * 0.0009765625f * sqrtf(na2) * R + 7.62939453125e-6f * Z;
-        thr = fminf(B, max_score) - dis0 + eps;
-        lo = min_score - dis0 - eps;
+        const double Z = fabs((double)dis0) + R2 + 2.0 * (sqrt((double)nx2) + sqrt((double)nc2)) * R;
+        const double eps = quant + 0x1p-17 * Z + f * s + 0x1p-22 * R2;
+        thr = (double)fminf(B, max_score) - dis0 + eps;
+        lo = (double)min_score - dis0 - eps;
       } else {
-        // score = dis0 - acc / c (the codebook is staged negated); better = larger
-        const float Z = fabsf(dis0) + sqrtf(na2) * R;
-        const float eps = 1.05f * 0.00048828125f * sqrtf(na2) * R + 7.62939453125e-6f * Z;
-        thr = dis0 - fmaxf(B, min_score) + eps;
-        lo = dis0 - max_score - eps;
+        // score = dis0 + s acc; better = larger, so the test runs on -s acc
+        const double Z = fabs((double)dis0) + na * R;
+        const double eps = quant + 0x1p-17 * Z + f * s;
+        thr = (double)dis0 - fmaxf(B, min_score) + eps;
+        lo = (double)dis0 - max_score - eps;
       }
-      // compared against acc + c * ne; FLT_MAX keeps masked entries (ne = +inf) out even when the product overflows
-      pm.thr = fminf(thr * pm.c, FLT_MAX);
-      pm.lo = lo * pm.c;
+      // in accumulator units, rounded outwards; FLT_MAX keeps masked entries (ne = +inf) out
+      const double fs = f * s;
+      pm.c = (float)(1.0 / fs);
+      pm.thr = fminf(__double2float_ru(thr / fs - kAccBiasF), FLT_MAX);
+      pm.lo = __double2float_rd(lo / fs - kAccBiasF);
     }
   }
   meta[(int64_t)t.grp * PT_G + threadIdx.x] = pm;
@@ -279,7 +308,7 @@ __device__ __forceinline__ int pt_frag_row(int f4, int t) { return (f4 >> 1) * 6
 // its own fragments again (the same fmaf as the fast path, now with the score window's lower side and the phase-A row
 // limit) and the warp appends the hits to the CTA's queue with one shared-memory atomic.  Inlined: the fragments are
 // registers, and handing them over by reference would force a local-memory copy of the accumulator in the hot loop.
-__device__ __forceinline__ void pt_push_frag_hits(const float (&acc)[2][64], const float* ne, const float (&fthr)[4],
+__device__ __forceinline__ void pt_push_frag_hits(const uint32_t (&acc)[2][64], const float* ne, const float (&fthr)[4],
                                                   const float (&fc)[4], const PairMeta* gm, uint32_t pos0,
                                                   PtShared* sh) {
   const int t = threadIdx.x & 127, lane = t & 31;
@@ -302,9 +331,9 @@ __device__ __forceinline__ void pt_push_frag_hits(const float (&acc)[2][64], con
       const int col = 8 * j + 2 * (lane & 3) + e;
 #pragma unroll
       for (int f4 = 0; f4 < 4; f4++) {
-        // ns = -(acc + c * ne) exactly (fma rounds symmetrically).  Written as the fast path's fmaf, ptxas would keep
-        // all 128 sums of the fast path alive for this rarely taken path and spill them
-        const float ns = fmaf(-(e ? n2.y : n2.x), fc[f4], -acc[f4 >> 1][4 * j + 2 * (f4 & 1) + e]);
+        // ns = -v exactly (fma rounds symmetrically).  Written as the fast path's fmaf, ptxas would keep all 128 sums of
+        // the fast path alive for this rarely taken path and spill them
+        const float ns = fmaf(-(e ? n2.y : n2.x), fc[f4], __uint_as_float(acc[f4 >> 1][4 * j + 2 * (f4 & 1) + e]));
         // rows phase A has scored exactly stay out
         if (ns >= -fthr[f4] && ns <= -lo[f4] && (int)(pos0 + col) >= lim[f4]) mask[f4] |= 1u << (2 * j + e);
       }
@@ -355,28 +384,30 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 template <int M, int DSUB, bool HAS_NORM, bool EAGER>
 __global__ void __launch_bounds__(PT_NT, 1)
     pqtc_scan_kernel(const unsigned char* __restrict__ a_scratch, const PairMeta* __restrict__ meta,
-                     const uint16_t* __restrict__ cb_g, const float* __restrict__ pqnorm,
+                     const int8_t* __restrict__ cb_g, const float* __restrict__ pqnorm,
                      const int64_t* __restrict__ pqnorm_off, const LmTile* __restrict__ items,
                      const int64_t* __restrict__ totals, ListDirectory dir, FilterArgs f, int* __restrict__ cand_cnt,
                      unsigned long long* __restrict__ cand, int cap) {
   constexpr int D = M * DSUB;
-  constexpr int KC = D / 8;                // core matrices along K
+  constexpr int KC = D / 16;               // core matrices (16 int8 wide) along K
   constexpr int TILE = KC * 2048;          // one 128-row operand tile, bytes
-  constexpr int CB_BYTES = M * PT_KSUB * DSUB * 2;
+  constexpr int CB_BYTES = M * PT_KSUB * DSUB;
   // |r_e|^2 of every list entry is cached in HBM beside the lists (IVFPQIndex::ensure_pq_norms) and arrives with the
   // codes: 512 bytes per tile by TMA instead of 16 table gathers per entry in the decode warps
   constexpr int NRM_BYTES = HAS_NORM ? PT_CS * PT_N * 4 : 0;
   constexpr int CODE_STAGE = PT_N * M;
-  constexpr int UNIT = DSUB * 2;           // bytes of one centroid in the fp16 codebook
-  static_assert(D % 16 == 0 && M % 4 == 0, "shape");
+  constexpr int UNIT = DSUB;               // bytes of one centroid in the int8 codebook
+  // K = 32 per MMA; |acc| <= 127^2 D < 2^22 keeps the biased accumulator exact
+  static_assert(D % 32 == 0 && D <= 256 && M % 4 == 0 && (UNIT % 16 == 0 || 16 % UNIT == 0), "shape");
   extern __shared__ __align__(1024) unsigned char smem[];
   __shared__ PtShared sh;
   unsigned char* cb = smem;
   float* nstage = reinterpret_cast<float*>(smem + CB_BYTES);  // [PT_CS][PT_N] norms of the staged tiles
-  // [codebook][norms][A tiles x 2][B tiles x 2][code stages]; the operand tiles start on 4 KiB boundaries
+  // [codebook][norms][A tiles: 2 items x 2 warpgroups][B tiles x 2][code stages]; the operand tiles start on 4 KiB
+  // boundaries.  The A tiles are double-buffered: the producer loads item i + 1's pairs while item i's tiles run
   unsigned char* a_buf = smem + CB_BYTES + NRM_BYTES;
   a_buf += (4096u - (smem_u32(a_buf) & 4095u)) & 4095u;
-  unsigned char* b_buf = a_buf + 2 * TILE;
+  unsigned char* b_buf = a_buf + 4 * TILE;
   unsigned char* code_buf = b_buf + 2 * TILE;
 
   const int tid = threadIdx.x, warp = tid >> 5;
@@ -392,13 +423,15 @@ __global__ void __launch_bounds__(PT_NT, 1)
       mbar_init(&sh.b_empty[b], PT_G);      // every MMA thread of both warpgroups, once its MMAs are complete
       mbar_init(&sh.acc_empty[b], PT_G);    // every epilogue thread of both warpgroups
     }
-    mbar_init(&sh.a_full, 1);               // bulk copies
-    mbar_init(&sh.a_empty, PT_G);           // every MMA thread, after the item's last tile
+    for (int b = 0; b < 2; b++) {
+      mbar_init(&sh.a_full[b], 1);          // bulk copies
+      mbar_init(&sh.a_empty[b], PT_G);      // every MMA thread, after the item's last tile
+    }
     mbar_fence_init();
     sh.q_head = 0, sh.q_tail = 0, sh.q_done = 0;
   }
   for (int i = tid; i < PT_RQ; i += PT_NT) sh.q_rec[i] = kRecEmpty;
-  // codebook (fp16, pre-scaled) and centroid norms: resident for the CTA's lifetime
+  // codebook (int8): resident for the CTA's lifetime
   for (int i = tid; i < CB_BYTES / 16; i += PT_NT)
     reinterpret_cast<uint4*>(cb)[i] = __ldg(reinterpret_cast<const uint4*>(cb_g) + i);
   __syncthreads();
@@ -412,7 +445,7 @@ __global__ void __launch_bounds__(PT_NT, 1)
     const uint32_t a_base = smem_u32(a_buf) + (uint32_t)(h * TILE), b_base = smem_u32(b_buf);
     uint32_t an = 0, bn = 0;
     bool turns = false;  // warpgroup 0 has issued a tile: from then on it waits for warpgroup 1's turn
-    float acc[2][64];
+    uint32_t acc[2][64];
     for (int64_t it = blockIdx.x; it < n_items; it += gridDim.x) {
       const LmTile tl = items[it];
       if (tl.nrows <= 0) continue;  // every role skips empty segments the same way
@@ -424,7 +457,8 @@ __global__ void __launch_bounds__(PT_NT, 1)
         const PairMeta* m = gm + pt_frag_row(f4, t);
         fthr[f4] = __ldg(&m->thr), fc[f4] = __ldg(&m->c);
       }
-      mbar_wait(&sh.a_full, an & 1);
+      const int ab = an & 1;
+      mbar_wait(&sh.a_full[ab], (an >> 1) & 1);
       const int ntiles = (tl.nrows + PT_N - 1) / PT_N;
       for (int i = 0; i < ntiles; i++, bn++) {
         const int b = bn & 1;
@@ -433,13 +467,13 @@ __global__ void __launch_bounds__(PT_NT, 1)
         else if (turns) bar_sync_256(2);
         // every warpgroup runs both m64 halves of every tile, empty rows included (their thresholds are -inf): a
         // branch around the MMAs or the wait makes ptxas serialise every wgmma of the kernel
-        const uint64_t da = lt_desc(a_base), db = lt_desc(b_base + (uint32_t)(b * TILE));
+        const uint64_t da = lt_desc(a_base + (uint32_t)(ab * 2 * TILE)), db = lt_desc(b_base + (uint32_t)(b * TILE));
         wg_fence();
 #pragma unroll
-        for (int kk = 0; kk < KC / 2; kk++) {  // K = 16 per instruction: two core matrices = 4096 bytes further
+        for (int kk = 0; kk < KC / 2; kk++) {  // K = 32 per instruction: two core matrices = 4096 bytes further
           const uint64_t adv = (uint64_t)((kk * 4096) >> 4);
-          wg_mma_f16(acc[0], da + adv, db + adv, kk != 0);
-          wg_mma_f16(acc[1], da + adv + kDescHalfM, db + adv, kk != 0);
+          wg_mma_s8(acc[0], da + adv, db + adv, kk != 0);
+          wg_mma_s8(acc[1], da + adv + kDescHalfM, db + adv, kk != 0);
         }
         wg_commit();
         bar_arrive_256(h ? 2 : 3);
@@ -447,17 +481,23 @@ __global__ void __launch_bounds__(PT_NT, 1)
         wg_wait<0>();
         wg_fence_acc(acc);
         mbar_arrive(&sh.b_empty[b]);
-        if (i == ntiles - 1) mbar_arrive(&sh.a_empty);
-        // Fast path: min over the tile of acc + c * ne per pair, on the fragments themselves.  A warp where some pair
-        // has a candidate redoes the test per entry and pushes the hits (pt_push_frag_hits).
+        // biased, the accumulators' bits are floats without a conversion (PairMeta).  (Starting the MMAs from the bias
+        // instead makes ptxas serialise every wgmma of the kernel, C7520.)
+#pragma unroll
+        for (int u = 0; u < 2; u++)
+#pragma unroll
+          for (int k = 0; k < 64; k++) acc[u][k] += kAccBias;
+        if (i == ntiles - 1) mbar_arrive(&sh.a_empty[ab]);
+        // Fast path: min over the tile of v = c * ne - (bias + acc) per pair, on the fragments themselves.  A warp where
+        // some pair has a candidate redoes the test per entry and pushes the hits (pt_push_frag_hits).
         float mn[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
 #pragma unroll
         for (int j = 0; j < PT_N / 8; j++) {
           const float2 n2 = *reinterpret_cast<const float2*>(&sh.ne[b][8 * j + 2 * (t & 3)]);
 #pragma unroll
           for (int f4 = 0; f4 < 4; f4++) {
-            const float* a2 = &acc[f4 >> 1][4 * j + 2 * (f4 & 1)];
-            mn[f4] = fminf(mn[f4], fminf(fmaf(n2.x, fc[f4], a2[0]), fmaf(n2.y, fc[f4], a2[1])));
+            const uint32_t* a2 = &acc[f4 >> 1][4 * j + 2 * (f4 & 1)];
+            mn[f4] = fminf(mn[f4], fminf(fmaf(n2.x, fc[f4], -__uint_as_float(a2[0])), fmaf(n2.y, fc[f4], -__uint_as_float(a2[1]))));
           }
         }
         bool hit = false;
@@ -522,20 +562,22 @@ __global__ void __launch_bounds__(PT_NT, 1)
         mbar_wait(&sh.b_empty[b], ((bn >> 1) & 1) ^ 1);
         unsigned char* brow = b_buf + b * TILE + e * 16;
         const float nsum = nstaged;
+        auto centroid = [&](int m) { return cb + (m * PT_KSUB + ((w[m >> 2] >> (8 * (m & 3))) & 0xFFu)) * UNIT; };
+        // one 16-byte core-matrix row per step: 16 / UNIT centroids (UNIT = 4, 8) or a 16-byte piece of one (16, 32)
 #pragma unroll
-        for (int m = 0; m < M; m++) {
-          const uint32_t c = (w[m >> 2] >> (8 * (m & 3))) & 0xFFu;
-          const unsigned char* src = cb + (m * PT_KSUB + c) * UNIT;
-          if (DSUB == 4) {  // two sub-quantisers share a core-matrix row
-            const uint2 val = *reinterpret_cast<const uint2*>(src);
-            *reinterpret_cast<uint2*>(brow + (m >> 1) * 2048 + (m & 1) * 8) = val;
+        for (int kc = 0; kc < KC; kc++) {
+          uint4 val;
+          if constexpr (UNIT >= 16) {
+            val = reinterpret_cast<const uint4*>(centroid(kc / (UNIT / 16)))[kc % (UNIT / 16)];
+          } else if constexpr (UNIT == 8) {
+            const uint2 v0 = *reinterpret_cast<const uint2*>(centroid(2 * kc));
+            const uint2 v1 = *reinterpret_cast<const uint2*>(centroid(2 * kc + 1));
+            val = make_uint4(v0.x, v0.y, v1.x, v1.y);
           } else {
-#pragma unroll
-            for (int u = 0; u < UNIT / 16; u++) {
-              const uint4 val = reinterpret_cast<const uint4*>(src)[u];
-              *reinterpret_cast<uint4*>(brow + (m * (UNIT / 16) + u) * 2048) = val;
-            }
+            val = make_uint4(*reinterpret_cast<const uint32_t*>(centroid(4 * kc)), *reinterpret_cast<const uint32_t*>(centroid(4 * kc + 1)),
+                             *reinterpret_cast<const uint32_t*>(centroid(4 * kc + 2)), *reinterpret_cast<const uint32_t*>(centroid(4 * kc + 3)));
           }
+          *reinterpret_cast<uint4*>(brow + kc * 2048) = val;
         }
         // ne[b] is read by the epilogue of tile bn - 2: wait until it has released the buffer
         mbar_wait(&sh.acc_empty[b], ((bn >> 1) & 1) ^ 1);
@@ -552,11 +594,12 @@ __global__ void __launch_bounds__(PT_NT, 1)
       for (int64_t it = blockIdx.x; it < n_items; it += gridDim.x) {
         const LmTile t = items[it];
         if (t.nrows <= 0) continue;  // every role skips empty segments the same way
-        mbar_wait(&sh.a_empty, (an & 1) ^ 1);
+        const int ab = an & 1;
+        mbar_wait(&sh.a_empty[ab], ((an >> 1) & 1) ^ 1);
         if (elect_one()) {
-          mbar_arrive_expect_tx(&sh.a_full, 2 * TILE);
+          mbar_arrive_expect_tx(&sh.a_full[ab], 2 * TILE);
           for (int h = 0; h < 2; h++)
-            bulk_g2s(a_buf + h * TILE, a_scratch + ((int64_t)t.grp * 2 + h) * TILE, TILE, &sh.a_full);
+            bulk_g2s(a_buf + (ab * 2 + h) * TILE, a_scratch + ((int64_t)t.grp * 2 + h) * TILE, TILE, &sh.a_full[ab]);
         }
         __syncwarp();
         const unsigned char* lcodes = dir.codes[t.list];
@@ -715,12 +758,12 @@ __global__ void __launch_bounds__(RS_NT)
 }
 
 template <int M, int DSUB>
-cudaError_t launch_scan_shape(const unsigned char* a_scratch, const PairMeta* meta, const uint16_t* cb, const float* pqnorm,
+cudaError_t launch_scan_shape(const unsigned char* a_scratch, const PairMeta* meta, const int8_t* cb, const float* pqnorm,
                               const int64_t* pqnorm_off,
                               const LmTile* items, const int64_t* totals, ListDirectory dir, FilterArgs f, int metric,
                               int* cand_cnt, unsigned long long* cand, int cap, int grid, cudaStream_t st) {
-  constexpr int TILE = (M * DSUB / 8) * 2048;
-  const size_t base = (size_t)M * PT_KSUB * DSUB * 2 + 4 * (size_t)TILE + (size_t)PT_CS * PT_N * M + 4096;
+  constexpr int TILE = (M * DSUB / 16) * 2048;
+  const size_t base = (size_t)M * PT_KSUB * DSUB + 6 * (size_t)TILE + (size_t)PT_CS * PT_N * M + 4096;
   const bool l2 = metric == kMetricL2;
   const bool eager = f.del_bits != nullptr || f.filter_bits != nullptr;
   if (l2 && (!pqnorm || !pqnorm_off)) return cudaErrorInvalidValue;
@@ -785,9 +828,8 @@ bool pqtc_supported(int M, int dsub) {
 
 size_t pqtc_pair_meta_bytes() { return sizeof(PairMeta); }
 
-cudaError_t launch_pqtc_tables(const float* pq, int M, int dsub, int metric, uint16_t* cb, float* nrm, float* rmax2,
-                               cudaStream_t st) {
-  pqtc_tables_kernel<<<1, 256, 0, st>>>(pq, M, dsub, metric == kMetricL2 ? -2.0f : -1.0f, cb, nrm, rmax2);
+cudaError_t launch_pqtc_tables(const float* pq, int M, int dsub, int8_t* cb, float* nrm, float* rmax2, cudaStream_t st) {
+  pqtc_tables_kernel<<<1, 256, 0, st>>>(pq, M, dsub, cb, nrm, rmax2);
   note_launch();
   return cudaGetLastError();
 }
@@ -808,7 +850,7 @@ cudaError_t launch_pq_stage_pairs(const float* xq, int64_t ldq, int d, const flo
                                   int kprime, const float* rmax2, FilterArgs f, int metric, unsigned char* a_scratch,
                                   void* meta, int* cand_cnt, int cap, const int* row_limit, cudaStream_t st) {
   if (max_items <= 0) return cudaSuccess;
-  if (d % 16) return cudaErrorInvalidValue;
+  if (d % 32) return cudaErrorInvalidValue;
   if (metric == kMetricL2)
     pq_stage_pairs_kernel<kMetricL2><<<max_items, PT_G, 0, st>>>(xq, ldq, d, coarse, ldc, items, totals, pair_j, nprobe,
                                                                 coarse_dis, bound_keys, bound_stride, kprime, rmax2,
@@ -823,7 +865,7 @@ cudaError_t launch_pq_stage_pairs(const float* xq, int64_t ldq, int d, const flo
   return cudaGetLastError();
 }
 
-cudaError_t launch_pqtc_scan(const unsigned char* a_scratch, const void* meta, const uint16_t* cb, const float* pqnorm,
+cudaError_t launch_pqtc_scan(const unsigned char* a_scratch, const void* meta, const int8_t* cb, const float* pqnorm,
                              const int64_t* pqnorm_off,
                              const LmTile* items, int max_items, const int64_t* totals, ListDirectory dir, int M, int dsub,
                              FilterArgs f, int metric, int* cand_cnt, unsigned long long* cand, int cap, int num_sms,
