@@ -115,7 +115,20 @@ int gb_index_list_len(gb_index *index, int list);
 int gb_index_code_size(gb_index *index);
 /* copy one inverted list to the host: codes = len x code_size bytes, ids = len int64 */
 int gb_index_get_list(gb_index *index, int list, uint8_t *codes, int64_t *ids);
+/* test hook: tombstone one entry where it is (and count it dead); never purges by itself */
 int gb_index_tombstone(gb_index *index, int list, int pos);
+/* The other half of gamma's realtime list container (RTInvertIndex::Delete, RealTimeMemData::CompactIfNeed,
+ * index/realtime/realtime_mem_data.cc:186-196, 347-373).  delete: the documents vids[0..n) were deleted; their entries
+ * stay in the lists, hidden by the deletion bitmap of each search, and are counted dead (a vid that is in no list, or
+ * already counted, is ignored).  purge: every list whose counted dead share (deleted + tombstoned by updates) is
+ * >= threshold (the reference: 0.3; 0: every list with a dead entry) is rewritten on the GPU without its tombstoned
+ * entries and without the entries whose bit is set in del_bitmap (bitmap_bytes bytes, bit vid & 7 of byte vid >> 3;
+ * may be NULL), the survivors in their old order; *dropped (may be NULL) = entries removed.  No search result changes:
+ * a dead entry was never returned.  dead_counts: out[nlist], the dead entries counted per list since its last purge.
+ * delete and purge are no-ops on a FLAT index. */
+int gb_index_delete(gb_index *index, const int64_t *vids, int64_t n);
+int gb_index_purge(gb_index *index, float threshold, const uint8_t *del_bitmap, int64_t bitmap_bytes, int64_t *dropped);
+int gb_index_dead_counts(gb_index *index, int *out);
 /* IndexModel::Dump / Load (index/index_model.h) in gamma's own file formats -- "IvFl" / "IwPQ" header,
  * IndexFlat quantizer, "ilar" inverted lists (index/impl/gamma_index_ivfflat.cc:807-892,
  * gamma_index_ivfpq.cc:1019-1116, index/index_io.cc:108-194): <dir>/<abs_name>/{ivfflat,ivfpq}.index.

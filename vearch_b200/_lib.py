@@ -81,6 +81,9 @@ def _declare(l):
     l.gb_index_code_size.argtypes = [vp]
     l.gb_index_get_list.argtypes = [vp, i32, vp, vp]
     l.gb_index_tombstone.argtypes = [vp, i32, i32]
+    l.gb_index_delete.argtypes = [vp, vp, i64]
+    l.gb_index_purge.argtypes = [vp, f32, vp, i64, vp]
+    l.gb_index_dead_counts.argtypes = [vp, vp]
     l.gb_index_dump.argtypes = [vp, cstr, cstr]
     l.gb_index_compact.argtypes = [vp]
     l.gb_index_mirror_builds.argtypes = [vp]

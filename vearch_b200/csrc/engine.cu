@@ -466,6 +466,7 @@ int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
       if (flush_pending_locked()) return -1;
       if (extra_[ei].index->update_vector(docid, x.data())) return -1;
     }
+    purge_indexes(delete_num_ > 0 ? del_bitmap_.data() : nullptr, (size_t)(max_docid_ >> 3) + 1);
     return 0;
   } else if (docid >= max_docid_) {
     return -2;
@@ -513,7 +514,20 @@ int Engine::Delete(const std::string& key) {
   del_bitmap_[docid >> 3] |= (uint8_t)(1u << (docid & 7));
   ++delete_num_;
   key2docid_.erase(it);  // table_->Delete(key)
+  // vec_manager_->Delete(docid) (engine.cc:868): the lists count the entry dead; the bitmap keeps hiding it
+  const int64_t vid = docid;
+  if (index_) index_->delete_vectors(&vid, 1);
+  for (auto& e : extra_) e.index->delete_vectors(&vid, 1);
   return 0;
+}
+
+void Engine::purge_indexes(const uint8_t* bitmap, size_t bytes) {
+  auto purge = [&](Index* ix, const std::string& field) {
+    if (ix && ix->purge_lists(0.3f, bitmap, (int64_t)bytes, nullptr))
+      fprintf(stderr, "gamma: purge of the dead list entries of field %s failed: %s\n", field.c_str(), last_error());
+  };
+  purge(index_.get(), vec_name_);
+  for (auto& e : extra_) purge(e.index.get(), e.name);
 }
 
 void Engine::serialize_doc(int docid, bool with_docid, std::string* out) {
@@ -1225,6 +1239,7 @@ void Engine::indexing_loop() {
     if (!has_error && index_->add_pending(bm.empty() ? nullptr : bm.data()) != 0) has_error = true;
     for (auto& e : extra_)
       if (!has_error && e.index->add_pending(bm.empty() ? nullptr : bm.data()) != 0) has_error = true;
+    if (!has_error) purge_indexes(bm.empty() ? nullptr : bm.data(), bm.size());
     if (!has_error) index_status_.store(2);
     // sleep refresh_interval ms, waking early on Close
     std::unique_lock<std::mutex> lk(idx_mu_);

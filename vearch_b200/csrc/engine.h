@@ -208,6 +208,9 @@ class Engine {
   Index* index_of(const std::string& vec_name, int* dim);  // nullptr: no such vector field
 
   std::vector<uint8_t> del_bitmap_;
+  // RealTimeMemData::CompactIfNeed for every vector field's index: lists that are 30 % dead are rewritten without the
+  // entries that updates tombstoned and `bitmap` marks deleted.  A failure is logged and leaves the index as it was.
+  void purge_indexes(const uint8_t* bitmap, size_t bytes);
   int max_docid_ = 0, delete_num_ = 0;
   int training_threshold_ = 0;
   int refresh_interval_ = 1000;

@@ -343,6 +343,7 @@ IvfLists::IvfLists(int nlist, int code_bytes) : nlist_(nlist), code_bytes_(code_
   h_ids_.assign(nlist, nullptr);
   h_len_.assign(nlist, 0);
   h_cap_.assign(nlist, 0);
+  h_dead_.assign(nlist, 0);
   cudaMalloc(&d_data_, sizeof(void*) * nlist);
   cudaMalloc(&d_ids_, sizeof(int64_t*) * nlist);
   cudaMalloc(&d_len_, sizeof(int) * nlist);
@@ -373,6 +374,17 @@ void* IvfLists::slab_alloc(size_t bytes) {
   slab_left_ -= bytes;
   return p;
 }
+int IvfLists::slab_reserve(size_t need_bytes) {
+  if (need_bytes <= slab_left_) return 0;
+  size_t slab = std::max<size_t>(need_bytes, (size_t)64 << 20);
+  void* p = nullptr;
+  GB_CUDA(cudaMalloc(&p, slab));
+  slabs_.push_back(p);
+  slab_cur_ = static_cast<char*>(p);
+  slab_left_ = slab;
+  bytes_ += (int64_t)slab;
+  return 0;
+}
 int IvfLists::reserve(const std::vector<int>& add, cudaStream_t st) {
   // pass 1: how many bytes do the growing lists need
   std::vector<int> newcap(nlist_, 0);
@@ -392,15 +404,7 @@ int IvfLists::reserve(const std::vector<int>& add, cudaStream_t st) {
     need_bytes += (size_t)round_up(nc * code_bytes_ + 16, 256) + (size_t)round_up(nc * 8, 256);
   }
   if (need_bytes == 0) return 0;
-  if (need_bytes > slab_left_) {
-    size_t slab = std::max<size_t>(need_bytes, (size_t)64 << 20);
-    void* p = nullptr;
-    GB_CUDA(cudaMalloc(&p, slab));
-    slabs_.push_back(p);
-    slab_cur_ = static_cast<char*>(p);
-    slab_left_ = slab;
-    bytes_ += (int64_t)slab;
-  }
+  if (slab_reserve(need_bytes)) return -1;
   for (int l = 0; l < nlist_; l++) {
     if (!newcap[l]) continue;
     void* nd = slab_alloc((size_t)newcap[l] * code_bytes_ + 16);
@@ -478,9 +482,95 @@ int IvfLists::tombstone(int list, int pos, cudaStream_t st) {
   int64_t v;
   GB_CUDA(cudaMemcpyAsync(&v, h_ids_[list] + pos, 8, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
+  if (v & kDelIdxMask) return 0;  // already tombstoned, already counted
   v |= kDelIdxMask;
   GB_CUDA(cudaMemcpyAsync(h_ids_[list] + pos, &v, 8, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaStreamSynchronize(st));
+  h_dead_[list]++;  // realtime_mem_data.cc:315
+  return 0;
+}
+
+int IvfLists::purge(const std::vector<int>& lists, const uint32_t* d_del_bits, cudaStream_t st, Purged* out) {
+  *out = Purged();
+  std::vector<int> sel, chunk0(1, 0);
+  std::vector<PurgeChunk> chunks;
+  for (int l : lists) {
+    if (l < 0 || l >= nlist_ || h_len_[l] == 0) continue;
+    for (int first = 0; first < h_len_[l]; first += kPurgeChunk) chunks.push_back(PurgeChunk{(int)sel.size(), first});
+    sel.push_back(l);
+    chunk0.push_back((int)chunks.size());
+  }
+  const int nsel = (int)sel.size(), nchunks = (int)chunks.size();
+  if (nsel == 0) return 0;
+  Scratch s(st);
+  GB_ALLOC(d_sel, int, nsel, s);
+  GB_ALLOC(d_chunk0, int, nsel + 1, s);
+  GB_ALLOC(d_chunks, PurgeChunk, nchunks, s);
+  GB_ALLOC(d_chunk_off, int, nchunks, s);
+  GB_ALLOC(d_counts, unsigned long long, nsel + 2, s);  // vid range, then the lists' live counts (as ints)
+  int* d_live = reinterpret_cast<int*>(d_counts + 2);
+  GB_CUDA(cudaMemcpyAsync(d_sel, sel.data(), sizeof(int) * nsel, cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaMemcpyAsync(d_chunk0, chunk0.data(), sizeof(int) * (nsel + 1), cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaMemcpyAsync(d_chunks, chunks.data(), sizeof(PurgeChunk) * nchunks, cudaMemcpyHostToDevice, st));
+  const ListDirectory dir = directory();
+  GB_CUDA(launch_purge_count(dir, d_sel, d_chunk0, nsel, d_chunks, nchunks, d_del_bits, d_chunk_off, d_live, d_counts, st));
+  // the one download that sizes the destinations and the new-position table
+  std::vector<unsigned long long> h_counts((size_t)2 + (nsel + 1) / 2);
+  GB_CUDA(cudaMemcpyAsync(h_counts.data(), d_counts, 16 + sizeof(int) * nsel, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  const int* live = reinterpret_cast<const int*>(h_counts.data() + 2);
+  const int64_t vid_min = (int64_t)h_counts[0], vid_span = (int64_t)h_counts[1] - vid_min + 1;
+  // fresh regions, as reserve() takes them: the old ones stay valid for whatever still reads them
+  std::vector<int> newcap(nsel, 0);
+  size_t need_bytes = 0;
+  for (int i = 0; i < nsel; i++) {
+    out->dropped += h_len_[sel[i]] - live[i];
+    if (live[i] == 0) continue;
+    newcap[i] = (int)round_up(live[i], 32);
+    need_bytes += (size_t)round_up((int64_t)newcap[i] * code_bytes_ + 16, 256) + (size_t)round_up((int64_t)newcap[i] * 8, 256);
+  }
+  if (out->dropped == 0) return 0;  // nothing to drop: the lists stay where they are
+  if (slab_reserve(need_bytes)) return -1;
+  std::vector<void*> nd(nsel, nullptr);
+  std::vector<int64_t*> ni(nsel, nullptr);
+  uintptr_t bits = (uintptr_t)code_bytes_ | 16;
+  for (int i = 0; i < nsel; i++) {
+    if (!newcap[i]) continue;
+    nd[i] = slab_alloc((size_t)newcap[i] * code_bytes_ + 16);
+    ni[i] = static_cast<int64_t*>(slab_alloc((size_t)newcap[i] * 8));
+    if (!nd[i] || !ni[i]) {
+      set_last_error("slab exhausted");
+      return -1;
+    }
+    bits |= (uintptr_t)nd[i] | (uintptr_t)h_data_[sel[i]];
+  }
+  const int align = (int)(bits & (~bits + 1));  // lowest set bit: at most 16
+  GB_ALLOC(d_nd, void*, nsel, s);
+  GB_ALLOC(d_ni, int64_t*, nsel, s);
+  GB_ALLOC(d_newpos, unsigned long long, vid_span, s);
+  GB_CUDA(cudaMemcpyAsync(d_nd, nd.data(), sizeof(void*) * nsel, cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaMemcpyAsync(d_ni, ni.data(), sizeof(int64_t*) * nsel, cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaMemsetAsync(d_newpos, 0xFF, (size_t)vid_span * 8, st));
+  GB_CUDA(launch_purge_scatter(dir, d_sel, d_chunks, nchunks, d_del_bits, d_chunk_off, code_bytes_, align, d_nd, d_ni, d_newpos,
+                               vid_min, st));
+  out->vid_min = vid_min;
+  out->newpos.resize((size_t)vid_span);
+  GB_CUDA(cudaMemcpyAsync(out->newpos.data(), d_newpos, (size_t)vid_span * 8, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));  // the scatter is done (and has not failed) before anything is published
+  for (int i = 0; i < nsel; i++) {
+    const int l = sel[i];
+    h_data_[l] = nd[i], h_ids_[l] = ni[i], h_cap_[l] = newcap[i];
+  }
+  GB_CUDA(cudaMemcpyAsync(d_data_, h_data_.data(), sizeof(void*) * nlist_, cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaMemcpyAsync(d_ids_, h_ids_.data(), sizeof(int64_t*) * nlist_, cudaMemcpyHostToDevice, st));
+  for (int i = 0; i < nsel; i++) {
+    h_len_[sel[i]] = live[i];
+    h_dead_[sel[i]] = 0;
+  }
+  total_ -= out->dropped;
+  max_len_ = *std::max_element(h_len_.begin(), h_len_.end());
+  GB_CUDA(cudaMemcpyAsync(d_len_, h_len_.data(), sizeof(int) * nlist_, cudaMemcpyHostToDevice, st));
+  content_gen_++;
   return 0;
 }
 int IvfLists::download_list(int l, std::vector<uint8_t>* codes, std::vector<int64_t>* ids) const {
@@ -1445,7 +1535,7 @@ int IvfIndex::add_pending(const uint8_t* del_bitmap) {
   }
   // a bulk build leaves most of the slab space in regions the lists have outgrown: re-pack once the
   // waste is worth a copy (more than half of the live bytes and more than 1 GiB)
-  if (lists_ && lists_->mem_bytes() - lists_->packed_bytes() > std::max<int64_t>((int64_t)1 << 30, lists_->packed_bytes() / 2)) {
+  if (lists_ && lists_->compact_due()) {
     std::unique_lock<std::shared_mutex> lk(mu_);
     if (compact_locked()) return -1;
   }
@@ -1459,6 +1549,7 @@ int IvfIndex::reset_index() {
   cudaDeviceSynchronize();  // kernels of earlier device-resident searches may still read the lists
   lists_.reset();
   vid2pos_.clear();
+  del_counted_.clear();
   reset_codec();
   indexed_count_ = 0;
   trained_ = false;
@@ -1520,12 +1611,86 @@ int IvfIndex::update_vector(int64_t vid, const void* x) {
   if (!trained_ || vid >= indexed_count_) return 0;  // not indexed yet: the add path will pick it up
   if (vid < (int64_t)vid2pos_.size() && vid2pos_[vid] != ~(uint64_t)0) {
     std::unique_lock<std::shared_mutex> lk(mu_);
-    if (lists_->tombstone((int)(vid2pos_[vid] >> 32), (int)(uint32_t)vid2pos_[vid], build_stream_)) return -1;
+    const int l = (int)(vid2pos_[vid] >> 32);
+    if (vid < (int64_t)del_counted_.size() && del_counted_[vid]) {  // counted as deleted: the tombstone counts it instead
+      del_counted_[vid] = false;
+      lists_->add_dead(l, -1);
+    }
+    if (lists_->tombstone(l, (int)(uint32_t)vid2pos_[vid], build_stream_)) return -1;
   }
   Scratch s(build_stream_);
   const void* x_dev = store_rows_dev(vid, 1, s);
   if (!x_dev) return -1;
   return index_batch(x_dev, 1, vid, nullptr);
+}
+
+int IvfIndex::delete_vectors(const int64_t* vids, int64_t n) {
+  std::lock_guard<std::mutex> bg(build_mu_);
+  if (!lists_) return 0;
+  for (int64_t i = 0; i < n; i++) {
+    const int64_t vid = vids[i];
+    if (vid < 0 || vid >= (int64_t)vid2pos_.size() || vid2pos_[vid] == ~(uint64_t)0) continue;
+    if (del_counted_.size() < vid2pos_.size()) del_counted_.resize(vid2pos_.size(), false);
+    if (del_counted_[vid]) continue;
+    del_counted_[vid] = true;
+    lists_->add_dead((int)(vid2pos_[vid] >> 32), 1);  // realtime_mem_data.cc:194
+  }
+  return 0;
+}
+
+int IvfIndex::dead_counts(int* out) {
+  std::lock_guard<std::mutex> bg(build_mu_);
+  for (int l = 0; l < nlist_; l++) out[l] = lists_ ? lists_->dead_counts()[l] : 0;
+  return 0;
+}
+
+int IvfIndex::purge_lists(float threshold, const uint8_t* del_bitmap, int64_t bitmap_bytes, int64_t* dropped) {
+  if (dropped) *dropped = 0;
+  std::lock_guard<std::mutex> bg(build_mu_);
+  if (!lists_) return 0;
+  std::vector<int> sel;
+  std::vector<char> purged(nlist_, 0);
+  for (int l = 0; l < nlist_; l++) {
+    const int dead = lists_->dead_counts()[l], len = lists_->lens()[l];
+    if (dead > 0 && len > 0 && (float)dead / (float)len >= threshold) {  // Compactable (realtime_mem_data.cc:366-370)
+      sel.push_back(l);
+      purged[l] = 1;
+    }
+  }
+  if (sel.empty()) return 0;
+  cudaSetDevice(device_);
+  cudaStream_t st = build_stream_;
+  Scratch s(st);
+  std::unique_lock<std::shared_mutex> lk(mu_);
+  SearchContext ctx;
+  ctx.del_bitmap = del_bitmap;
+  ctx.bitmap_bits = del_bitmap ? bitmap_bytes * 8 : 0;
+  FilterArgs f;
+  if (upload_bitmaps(ctx, &f, s)) return -1;
+  drain_searches();  // kernels of earlier searches read lengths and base pointers at run time
+  IvfLists::Purged pg;
+  if (lists_->purge(sel, f.del_bits, st, &pg)) return -1;
+  if (pg.dropped == 0) return 0;
+  // vid_bucket_no_pos_ of every vid that was in a purged list, from the table the scatter wrote
+  const int64_t hi = std::min<int64_t>((int64_t)vid2pos_.size(), pg.vid_min + (int64_t)pg.newpos.size());
+  for (int64_t vid = pg.vid_min; vid < hi; vid++) {
+    const uint64_t old = vid2pos_[vid];
+    if (old == ~(uint64_t)0 || !purged[old >> 32]) continue;
+    const uint64_t now = pg.newpos[vid - pg.vid_min];
+    vid2pos_[vid] = now;
+    if (vid < (int64_t)del_counted_.size() && del_counted_[vid]) {
+      if (now == ~(uint64_t)0)
+        del_counted_[vid] = false;
+      else
+        lists_->add_dead((int)(now >> 32), 1);  // deleted, but not in this bitmap: still there, still counted
+    }
+  }
+  if (lists_changed(st)) return -1;
+  GB_CUDA(cudaStreamSynchronize(st));
+  if (dropped) *dropped = pg.dropped;
+  // the regions the purged lists left behind are reclaimed by the re-pack, under its own policy
+  if (lists_->compact_due() && compact_locked()) return -1;
+  return 0;
 }
 
 int IvfIndex::resolve_nprobe(const SearchContext& ctx) const {
@@ -1630,8 +1795,9 @@ int IVFFlatIndex::mirror_append(const float* x, int64_t n, const int32_t* d_list
   if (!mirror_.base || mirror_.disabled || mirror_.lens.size() != (size_t)nlist_) return 0;
   std::vector<int> lens = lists_->lens();  // lengths BEFORE this batch is committed
   for (int l = 0; l < nlist_; l++) {
-    if (mirror_.lens[l] != lens[l] || (int64_t)lens[l] + add[l] > (int64_t)mirror_.list_tiles[l] * 128) {
-      mirror_.lens.clear();  // stale: outgrown (or out of step); rebuilt by the next list-major search
+    if (mirror_.lens[l] != lens[l] || mirror_.content_gen != lists_->content_gen() ||
+        (int64_t)lens[l] + add[l] > (int64_t)mirror_.list_tiles[l] * 128) {
+      mirror_.lens.clear();  // stale: outgrown, purged or out of step; rebuilt by the next list-major search
       return 0;
     }
     lens[l] += add[l];
@@ -1646,11 +1812,11 @@ int IVFFlatIndex::ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStr
   if (!lists_) return 1;
   lk.lock();
   if (mirror_.disabled) return 1;
-  if (mirror_.base && mirror_.lens == lists_->lens()) return 0;
+  if (mirror_current()) return 0;
   lk.unlock();
   {
     std::unique_lock<std::shared_mutex> x(mirror_rw_);
-    if (!mirror_.disabled && !(mirror_.base && mirror_.lens == lists_->lens())) {
+    if (!mirror_.disabled && !mirror_current()) {
       const std::vector<int>& lens = lists_->lens();
       const int k16 = (int)round_up(dpad_, 16);
       const size_t tile_bytes = (size_t)tc_mirror_tile_floats(k16) * 4;
@@ -1694,13 +1860,14 @@ int IVFFlatIndex::ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStr
         GB_CUDA(cudaStreamSynchronize(st));  // tile0 is a stack vector; other streams may use the mirror next
         mirror_.tiles = tiles;
         mirror_.lens = lens;
+        mirror_.content_gen = lists_->content_gen();
         mirror_.builds++;
       }
     }
   }
   lk.lock();
   if (mirror_.disabled) return 1;
-  return (mirror_.base && mirror_.lens == lists_->lens()) ? 0 : 1;
+  return mirror_current() ? 0 : 1;
 }
 
 int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, const float* xq, int k,
@@ -2261,13 +2428,16 @@ cudaError_t IVFPQIndex::encode_dev(const float* x, int64_t n, const int32_t* lis
 }
 
 // Cache of |r_e|^2 per list entry for the tensor-core filter.  Searches hold mu_ shared, appends hold it exclusively and
-// drain in-flight searches before the lists change, so whenever the key (list set, lengths, codebook generation) differs
+// drain in-flight searches before the lists change, so whenever the key (list set, content generation, lengths, codebook
+// generation) differs
 // from the cached one no kernel is reading the cache; the rebuild (one pass over the codes) is serialised by pqn_mu_ and
 // synchronised before other streams may use it.
 int IVFPQIndex::ensure_pq_norms(cudaStream_t st) {
   std::lock_guard<std::mutex> g(pqn_mu_);
   const std::vector<int>& lens = lists_->lens();
-  if (pqn_.base && pqn_.lists_uid == lists_->uid() && pqn_.pq_gen == pq_gen_ && pqn_.lens == lens) return 0;
+  if (pqn_.base && pqn_.lists_uid == lists_->uid() && pqn_.content_gen == lists_->content_gen() && pqn_.pq_gen == pq_gen_ &&
+      pqn_.lens == lens)
+    return 0;
   std::vector<int64_t> off((size_t)nlist_ + 1, 0);
   for (int l = 0; l < nlist_; l++) off[l + 1] = off[l] + round_up(lens[l], 32);
   const size_t total = (size_t)off[nlist_] + 128;  // a tile's 16-byte rounded tail may run past the last entry
@@ -2291,6 +2461,7 @@ int IVFPQIndex::ensure_pq_norms(cudaStream_t st) {
   GB_CUDA(cudaStreamSynchronize(st));
   pqn_.lens = lens;
   pqn_.lists_uid = lists_->uid();
+  pqn_.content_gen = lists_->content_gen();
   pqn_.pq_gen = pq_gen_;
   return 0;
 }

@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <condition_variable>
 #include <functional>
 #include <memory>
@@ -143,11 +144,34 @@ class IvfLists {
   // exclude concurrent searches; in-flight kernels are drained before the old slabs go.
   int64_t packed_bytes() const;
   int compact(cudaStream_t st);
+  // whether the slab space the lists have left behind is worth a re-pack: more than half of the live bytes and more
+  // than 1 GiB
+  bool compact_due() const { return bytes_ - packed_bytes() > std::max<int64_t>((int64_t)1 << 30, packed_bytes() / 2); }
+  // Dead entries reported per list (deleted_nums_ of the reference): tombstone() counts the entry it marks,
+  // add_dead() the deletions and loaded tombstones the owner knows of.  They choose the lists to purge; what a purge
+  // drops is decided entry by entry on the device.
+  const std::vector<int>& dead_counts() const { return h_dead_; }
+  void add_dead(int list, int n) { h_dead_[list] += n; }
+  // Bumped by purge(): entries moved inside their lists, so "same list set + same lengths" no longer means "same
+  // content".  Whatever caches per-entry data beside the lists keys on it.
+  uint64_t content_gen() const { return content_gen_; }
+  // Drop the dead entries (tombstoned, or set in the device bitmap d_del_bits, nullable) of `lists`, in one pass over
+  // the device (RealTimeMemData::CompactBucket, realtime_mem_data.cc:94-146).  Survivors keep their order and move to
+  // fresh regions, as copy-on-grow does, so a kernel still reading an old region reads valid memory; pointers are
+  // published before lengths.  The caller holds the index lock exclusively with earlier searches drained.
+  // newpos[vid - vid_min] = (list << 32 | pos) of every surviving vid, ~0 for vids no longer in these lists.
+  struct Purged {
+    int64_t dropped = 0, vid_min = 0;
+    std::vector<uint64_t> newpos;
+  };
+  int purge(const std::vector<int>& lists, const uint32_t* d_del_bits, cudaStream_t st, Purged* out);
 
  private:
   void* slab_alloc(size_t bytes);
+  int slab_reserve(size_t need_bytes);  // a new slab unless the current one has need_bytes left
   int nlist_, code_bytes_;
-  uint64_t uid_;
+  uint64_t uid_, content_gen_ = 0;
+  std::vector<int> h_dead_;
   std::vector<void*> h_data_;
   std::vector<int64_t*> h_ids_;
   std::vector<int> h_len_, h_cap_;
@@ -243,6 +267,17 @@ class Index {
   // Engine::Update -> RawVector update + IndexModel::Update (search/engine.cc:774-850;
   // realtime_mem_data.cc:298-320: old entry tombstoned, vector re-appended to its new list)
   virtual int update_vector(int64_t vid, const void* x);  // x: one row of store().row_bytes() bytes
+  // IndexModel::Delete (RTInvertIndex::Delete, realtime_mem_data.cc:186-196): the documents were deleted.  Their
+  // entries stay where they are, hidden by the deletion bitmap at search time; the lists only count them.
+  virtual int delete_vectors(const int64_t* vids, int64_t n) { (void)vids; (void)n; return 0; }
+  // RealTimeMemData::CompactIfNeed (realtime_mem_data.cc:347-370): rewrite every list whose counted dead share is at
+  // least `threshold` (the reference: 0.3f; 0 = every list with a dead entry) without its tombstoned entries and the
+  // entries set in del_bitmap (host, bitmap_bytes bytes, nullable).  *dropped (optional) = entries removed.
+  virtual int purge_lists(float threshold, const uint8_t* del_bitmap, int64_t bitmap_bytes, int64_t* dropped) {
+    (void)threshold; (void)del_bitmap; (void)bitmap_bytes;
+    if (dropped) *dropped = 0;
+    return 0;
+  }
   // IndexModel::Search (index_model.h:296): x = nq host rows of store().row_bytes() bytes (d floats; BINARYIVF: d / 8
   // packed bytes); out = nq x k, unfilled id -1.  Returns 0, -1 on error (last_error), -2 if killed.
   int search(const SearchContext& ctx, int nq, const void* x, int k, float* out_dis, int64_t* out_ids);
@@ -436,6 +471,9 @@ class IvfIndex : public Index {
   int train() override;
   int add_pending(const uint8_t* del_bitmap) override;
   int update_vector(int64_t vid, const void* x) override;
+  int delete_vectors(const int64_t* vids, int64_t n) override;  // a vid not in a list, or already counted, is ignored
+  int purge_lists(float threshold, const uint8_t* del_bitmap, int64_t bitmap_bytes, int64_t* dropped) override;
+  int dead_counts(int* out);  // [nlist] dead entries counted per list since its last purge
   int reset_index() override;
   int64_t index_mem_bytes() const override;
   int nlist() const { return nlist_; }
@@ -533,6 +571,7 @@ class IvfIndex : public Index {
   virtual int centroids_changed(cudaStream_t st) { (void)st; return 0; }
   std::unique_ptr<IvfLists> lists_;
   std::vector<uint64_t> vid2pos_;  // vid -> (list << 32 | pos), ~0 = not in a list (vid_bucket_no_pos_)
+  std::vector<bool> del_counted_;  // vid's entry is counted dead by delete_vectors (so it is counted once)
 };
 
 // GammaIVFFlatIndex (index/impl/gamma_index_ivfflat.{h,cc}): the lists hold the raw fp32 rows.  type: "IVFFLAT", or
@@ -580,6 +619,7 @@ class IVFFlatIndex : public IvfIndex {
     int64_t* d_tile0 = nullptr;
     int64_t tiles = 0, cap_tiles = 0;
     std::vector<int> lens;        // rows mirrored per list
+    uint64_t content_gen = 0;     // IvfLists::content_gen() they were mirrored at: a purge moves rows inside lists
     std::vector<int> list_tiles;  // tiles reserved per list (a little slack, so appends go in place)
     bool disabled = false;
     int builds = 0;  // full (re)builds so far
@@ -590,6 +630,9 @@ class IVFFlatIndex : public IvfIndex {
                     cudaStream_t st);
   std::shared_mutex mirror_rw_;  // taken after mu_
   int ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStream_t st);  // 0 = usable and current
+  bool mirror_current() const {
+    return mirror_.base && mirror_.lens == lists_->lens() && mirror_.content_gen == lists_->content_gen();
+  }
 };
 
 // Product-quantiser base of IVFPQ and IVFPQFastScan: M sub-quantisers of ksub centroids each over dsub-wide slices, the
@@ -663,13 +706,14 @@ class IVFPQIndex : public IvfPqBase {
   int8_t* d_cb8_ = nullptr;     // [M][256][dsub] int8 codebook (tensor-core filter)
   float* d_cbnrm_ = nullptr;    // [M][256] |pq|^2, then R^2, sb, D
   // |r_e|^2 of every list entry (L2), flat with 32-entry aligned list segments: built by the first list-major search
-  // after the lists or the codebook changed (lists are append-only: same list set + same lengths = same content)
+  // after the lists or the codebook changed (between purges lists are append-only: same list set + same content
+  // generation + same lengths = same content)
   struct PqNormCache {
     float* base = nullptr;
     int64_t* d_off = nullptr;
     size_t cap = 0;
     std::vector<int> lens;
-    uint64_t lists_uid = 0, pq_gen = 0;
+    uint64_t lists_uid = 0, content_gen = 0, pq_gen = 0;
   } pqn_;
   std::mutex pqn_mu_;
   uint64_t pq_gen_ = 1;

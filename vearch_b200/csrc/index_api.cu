@@ -501,6 +501,24 @@ int gb_index_tombstone(gb_index* index, int list, int pos) {
   cudaSetDevice(ivf->device());
   return ivf->lists()->tombstone(list, pos, nullptr);
 }
+int gb_index_delete(gb_index* index, const int64_t* vids, int64_t n) {
+  IDX_OR_FAIL(index);
+  if (n < 0 || (n > 0 && !vids)) return -1;
+  return index->impl->delete_vectors(vids, n);
+}
+int gb_index_purge(gb_index* index, float threshold, const uint8_t* del_bitmap, int64_t bitmap_bytes, int64_t* dropped) {
+  IDX_OR_FAIL(index);
+  if (!(threshold >= 0.f) || bitmap_bytes < 0) {
+    set_last_error("purge: threshold must be >= 0 and bitmap_bytes >= 0");
+    return -1;
+  }
+  return index->impl->purge_lists(threshold, del_bitmap, bitmap_bytes, dropped);
+}
+int gb_index_dead_counts(gb_index* index, int* out) {
+  IVF_OR_FAIL(ivf, index);
+  if (!out) return -1;
+  return ivf->dead_counts(out);
+}
 int gb_index_coarse_search(gb_index* index, int nq, const float* x, int nprobe, float* out_dis, int64_t* out_ids) {
   IVF_OR_FAIL(ivf, index);
   if (packed_binary(index)) return -1;

@@ -233,6 +233,7 @@ int IvfIndex::load_gamma(const std::string& dir, const std::string& abs_name, in
   std::vector<int64_t> ids;
   int64_t live = 0, max_vid = -1;
   std::vector<uint64_t> v2p;  // vid_bucket_no_pos_, installed only if the whole file loads
+  std::vector<int> dead(nlist_, 0);
   const size_t my_cb = (size_t)code_bytes();
   for (int l = 0; l < nlist_; l++) {
     const size_t len = sizes[l];
@@ -251,7 +252,10 @@ int IvfIndex::load_gamma(const std::string& dir, const std::string& abs_name, in
     GB_CUDA(cudaStreamSynchronize(st));  // the staging vectors are reused by the next list
     for (size_t pos = 0; pos < len; pos++) {
       const int64_t id = ids[pos];
-      if (id < 0) continue;             // deleted_nums_[bno]++ (index_io.cc:178-181)
+      if (id < 0) {  // deleted_nums_[bno]++ (index_io.cc:178-181)
+        dead[l]++;
+        continue;
+      }
       live++;
       max_vid = std::max(max_vid, id);
       if ((size_t)id >= v2p.size()) v2p.resize(std::max<size_t>((size_t)id + 1, v2p.size() * 2), ~(uint64_t)0);
@@ -271,6 +275,7 @@ int IvfIndex::load_gamma(const std::string& dir, const std::string& abs_name, in
     std::unique_lock<std::shared_mutex> lk(mu_);
     if (lists_->commit(add, st)) return -1;
     vid2pos_.swap(v2p);
+    for (int l = 0; l < nlist_; l++) lists_->add_dead(l, dead[l]);
     if (lists_changed(st)) return -1;  // IVF-Flat on a host store: the row pointers into the loaded lists
     GB_CUDA(cudaStreamSynchronize(st));
   }

@@ -322,6 +322,26 @@ cudaError_t launch_ivf_append_vecs(const float* x, int64_t ldx, int64_t n, int d
 cudaError_t launch_ivf_append_codes(const uint8_t* codes, int64_t n, int M, const int32_t* list, const int32_t* pos,
                                     uint8_t* const* list_codes, int64_t* const* list_ids, int64_t vid0,
                                     cudaStream_t st);
+// IVF purge (RealTimeMemData::CompactBucket): stable compaction of the nsel lists sel_list[] into fresh regions, keeping
+// the entries that are neither tombstoned nor set in del_bits (nullable), in their old order.  The lists are cut into
+// chunks of kPurgeChunk entries (chunks[], list by list; sel_chunk0[s] = the first chunk of sel_list[s], [nsel] = nchunks).
+constexpr int kPurgeChunk = 1024;
+constexpr int kPurgeMaxCodeBytes = 1 << 20;  // keeps a chunk's copy units inside an int
+struct PurgeChunk {
+  int sel, first;  // ordinal in sel_list, first entry
+};
+// chunk_off[c] = live entries of the list before chunk c, sel_live[s] = live entries of sel_list[s], vid_range = the
+// smallest and largest vid among all entries of the selected lists, dead ones included ({~0, 0}: no entries)
+cudaError_t launch_purge_count(ListDirectory dir, const int* sel_list, const int* sel_chunk0, int nsel,
+                               const PurgeChunk* chunks, int nchunks, const uint32_t* del_bits, int* chunk_off,
+                               int* sel_live, unsigned long long* vid_range, cudaStream_t st);
+// live entry with rank r of sel_list[s]: code -> dst_data[s] + r code_bytes, id -> dst_ids[s][r], and
+// newpos[vid - vid_min] = list << 32 | r (the caller pre-fills newpos with ~0, so a dropped vid reads ~0).  align: the
+// widest power of two <= 16 that divides code_bytes and every source and destination base.
+cudaError_t launch_purge_scatter(ListDirectory dir, const int* sel_list, const PurgeChunk* chunks, int nchunks,
+                                 const uint32_t* del_bits, const int* chunk_off, int code_bytes, int align,
+                                 void* const* dst_data, int64_t* const* dst_ids, unsigned long long* newpos,
+                                 int64_t vid_min, cudaStream_t st);
 cudaError_t launch_fill_u64(unsigned long long* p, int64_t n, unsigned long long v, cudaStream_t st);
 cudaError_t launch_pad_rows(const float* src, int64_t n, int d, float* dst, int64_t ldd, cudaStream_t st);
 

@@ -273,6 +273,164 @@ cudaError_t launch_ivf_rowptrs(ListDirectory dir, int ld, const float** rowptr, 
   return cudaGetLastError();
 }
 
+// ---- purge: stable compaction of a set of lists (RealTimeMemData::CompactBucket, realtime_mem_data.cc:94-146) ----
+// The selected lists are cut into chunks of kPurgeChunk entries, one CTA per chunk, so one long list spreads over the
+// device and a thousand short ones cost one launch.
+namespace {
+
+// live = not tombstoned and not set in the deletion bitmap: what every list scan tests before it scores an entry
+__device__ __forceinline__ bool purge_live(int64_t id, const uint32_t* __restrict__ del_bits) {
+  return id >= 0 && !(del_bits && bit_test(del_bits, (uint32_t)id));
+}
+
+__global__ void __launch_bounds__(256)
+    purge_count_kernel(ListDirectory dir, const int* __restrict__ sel_list, const PurgeChunk* __restrict__ chunks,
+                       const uint32_t* __restrict__ del_bits, int* __restrict__ chunk_cnt, unsigned long long* vid_range) {
+  __shared__ int s_cnt;
+  __shared__ unsigned long long s_min, s_max;
+  if (threadIdx.x == 0) s_cnt = 0, s_min = ~0ull, s_max = 0;
+  __syncthreads();
+  const PurgeChunk c = chunks[blockIdx.x];
+  const int list = sel_list[c.sel];
+  const int64_t* __restrict__ ids = dir.ids[list];
+  const int end = min(c.first + kPurgeChunk, dir.len[list]);
+  int cnt = 0;
+  unsigned long long lo = ~0ull, hi = 0;
+  for (int p = c.first + threadIdx.x; p < end; p += blockDim.x) {
+    const int64_t id = ids[p];
+    cnt += purge_live(id, del_bits);
+    const unsigned long long vid = (unsigned long long)(id & ~kDelIdxMask);
+    lo = min(lo, vid);
+    hi = max(hi, vid);
+  }
+  cnt = __reduce_add_sync(0xffffffffu, cnt);
+  for (int o = 16; o; o >>= 1) {
+    lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+  }
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(&s_cnt, cnt);
+    atomicMin(&s_min, lo);
+    atomicMax(&s_max, hi);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    chunk_cnt[blockIdx.x] = s_cnt;
+    atomicMin(vid_range, s_min);
+    atomicMax(vid_range + 1, s_max);
+  }
+}
+
+// one warp per selected list: its chunks' live counts -> exclusive offsets in place, the total to sel_live
+__global__ void __launch_bounds__(32)
+    purge_scan_kernel(const int* __restrict__ sel_chunk0, int* __restrict__ chunk_cnt, int* __restrict__ sel_live) {
+  const int c0 = sel_chunk0[blockIdx.x], c1 = sel_chunk0[blockIdx.x + 1];
+  const int lane = threadIdx.x;
+  int carry = 0;
+  for (int b = c0; b < c1; b += 32) {
+    const int v = b + lane < c1 ? chunk_cnt[b + lane] : 0;
+    int incl = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += t;
+    }
+    if (b + lane < c1) chunk_cnt[b + lane] = carry + incl - v;
+    carry += __shfl_sync(0xffffffffu, incl, 31);
+  }
+  if (lane == 0) sel_live[blockIdx.x] = carry;
+}
+
+// V: the widest unit (<= 16 bytes) that divides code_bytes and both bases.  Ranks come from ballots over the chunk in
+// position order, so survivors keep their order; the codes then move as one flat run of units, consecutive threads on
+// consecutive units of the destination: a warp or more shares a long row, and a warp covers many short ones.
+template <typename V>
+__global__ void __launch_bounds__(256)
+    purge_scatter_kernel(ListDirectory dir, const int* __restrict__ sel_list, const PurgeChunk* __restrict__ chunks,
+                         const uint32_t* __restrict__ del_bits, const int* __restrict__ chunk_off, int code_bytes,
+                         void* const* __restrict__ dst_data, int64_t* const* __restrict__ dst_ids,
+                         unsigned long long* __restrict__ newpos, int64_t vid_min) {
+  __shared__ int s_src[kPurgeChunk];
+  __shared__ int s_warp[8];
+  const PurgeChunk c = chunks[blockIdx.x];
+  const int list = sel_list[c.sel];
+  const int64_t* __restrict__ ids = dir.ids[list];
+  int64_t* __restrict__ out_ids = dst_ids[c.sel];
+  const int end = min(c.first + kPurgeChunk, dir.len[list]);
+  const int off = chunk_off[blockIdx.x];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int nlive = 0;
+  for (int p0 = c.first; p0 < end; p0 += 256) {
+    const int p = p0 + threadIdx.x;
+    const int64_t id = p < end ? ids[p] : -1;
+    const bool live = p < end && purge_live(id, del_bits);
+    const unsigned m = __ballot_sync(0xffffffffu, live);
+    if (lane == 0) s_warp[warp] = __popc(m);
+    __syncthreads();
+    int before = 0, tot = 0;
+#pragma unroll
+    for (int w = 0; w < 8; w++) {
+      const int v = s_warp[w];
+      before += w < warp ? v : 0;
+      tot += v;
+    }
+    if (live) {
+      const int r = nlive + before + __popc(m & ((1u << lane) - 1u));
+      s_src[r] = p;
+      out_ids[off + r] = id;
+      newpos[id - vid_min] = ((unsigned long long)list << 32) | (unsigned)(off + r);
+    }
+    nlive += tot;
+    __syncthreads();
+  }
+  const int vpr = code_bytes / (int)sizeof(V);  // units per row
+  const V* __restrict__ src = reinterpret_cast<const V*>(dir.codes[list]);
+  V* __restrict__ dst = reinterpret_cast<V*>(dst_data[c.sel]) + (int64_t)off * vpr;
+  const int units = nlive * vpr;  // <= kPurgeChunk x 16 KiB / sizeof(V)
+#pragma unroll 4
+  for (int u = threadIdx.x; u < units; u += 256) {
+    const int e = u / vpr;
+    dst[u] = src[(int64_t)s_src[e] * vpr + (u - e * vpr)];
+  }
+}
+
+}  // namespace
+
+cudaError_t launch_purge_count(ListDirectory dir, const int* sel_list, const int* sel_chunk0, int nsel,
+                               const PurgeChunk* chunks, int nchunks, const uint32_t* del_bits, int* chunk_off,
+                               int* sel_live, unsigned long long* vid_range, cudaStream_t st) {
+  if (nsel <= 0 || nchunks <= 0) return cudaSuccess;
+  cudaError_t e = cudaMemsetAsync(vid_range, 0xFF, 8, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(vid_range + 1, 0, 8, st);
+  if (e != cudaSuccess) return e;
+  purge_count_kernel<<<nchunks, 256, 0, st>>>(dir, sel_list, chunks, del_bits, chunk_off, vid_range);
+  purge_scan_kernel<<<nsel, 32, 0, st>>>(sel_chunk0, chunk_off, sel_live);
+  note_launch(2);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_purge_scatter(ListDirectory dir, const int* sel_list, const PurgeChunk* chunks, int nchunks,
+                                 const uint32_t* del_bits, const int* chunk_off, int code_bytes, int align,
+                                 void* const* dst_data, int64_t* const* dst_ids, unsigned long long* newpos,
+                                 int64_t vid_min, cudaStream_t st) {
+  if (nchunks <= 0) return cudaSuccess;
+  if (code_bytes <= 0 || code_bytes > kPurgeMaxCodeBytes || align <= 0 || code_bytes % align) return cudaErrorInvalidValue;
+#define GB_PURGE_SCATTER(V)                                                                                          \
+  purge_scatter_kernel<V><<<nchunks, 256, 0, st>>>(dir, sel_list, chunks, del_bits, chunk_off, code_bytes, dst_data, \
+                                                   dst_ids, newpos, vid_min)
+  switch (align) {
+    case 16: GB_PURGE_SCATTER(uint4); break;
+    case 8: GB_PURGE_SCATTER(uint2); break;
+    case 4: GB_PURGE_SCATTER(uint32_t); break;
+    case 2: GB_PURGE_SCATTER(uint16_t); break;
+    case 1: GB_PURGE_SCATTER(uint8_t); break;
+    default: return cudaErrorInvalidValue;
+  }
+#undef GB_PURGE_SCATTER
+  note_launch();
+  return cudaGetLastError();
+}
+
 cudaError_t launch_ivf_append_codes(const uint8_t* codes, int64_t n, int M, const int32_t* list, const int32_t* pos,
                                     uint8_t* const* list_codes, int64_t* const* list_ids, int64_t vid0,
                                     cudaStream_t st) {

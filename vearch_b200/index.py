@@ -327,6 +327,28 @@ class GammaIndex:
     def tombstone(self, l, pos):
         _check(_lib.lib().gb_index_tombstone(self._h, l, pos), "tombstone")
 
+    def delete_vectors(self, vids):
+        """The documents `vids` were deleted: their list entries are counted dead (a search still needs the deletion
+        bitmap to hide them).  A vid that is in no list, or already counted, is ignored."""
+        v = np.ascontiguousarray(np.atleast_1d(vids), np.int64)
+        _check(_lib.lib().gb_index_delete(self._h, _ptr(v), v.size), "delete_vectors")
+
+    def purge(self, threshold=0.3, del_bitmap=None):
+        """RealTimeMemData::CompactIfNeed: rewrite every list whose counted dead share is >= threshold without its
+        tombstoned entries and the entries set in del_bitmap; threshold 0 purges every list with a dead entry.
+        Returns the number of entries dropped."""
+        b = _bitmap(del_bitmap)
+        n = np.zeros(1, np.int64)
+        _check(_lib.lib().gb_index_purge(self._h, C.c_float(threshold), _ptr(b), 0 if b is None else b.size, _ptr(n)),
+               "purge")
+        return int(n[0])
+
+    def dead_counts(self):
+        """Dead entries counted per list (updates' tombstones + delete_vectors) since the list's last purge."""
+        out = np.zeros(self.nlist, np.int32)
+        _check(_lib.lib().gb_index_dead_counts(self._h, _ptr(out)), "dead_counts")
+        return out
+
     def coarse_search(self, x, nprobe):
         x = _f32(x)
         nq = x.shape[0]
