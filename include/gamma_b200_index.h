@@ -87,6 +87,11 @@ int gb_index_search_device_keys(gb_index *index, int nq, const float *x_dev, int
 /* {"stage": ms, ...}: device time per stage of the searches run since the last call with timing enabled
  * (CUDA events on the launching stream); *json_out is malloc'd, the caller frees it */
 int gb_index_stage_times(gb_index *index, char **json_out, int *out_len);
+/* while on, searches that re-rank through the two-pass kernel record per query the candidates whose fp32 rows they
+ * read (and wait for the count); gb_index_rerank_survivors hands them over (*out malloc'd, the caller frees it) and
+ * clears them */
+void gb_index_set_rerank_stats(gb_index *index, int on);
+int gb_index_rerank_survivors(gb_index *index, int **out, int64_t *n);
 /* device time of the dominant scan kernel(s) of the last search, ms (0 unless timing enabled) */
 void gb_index_set_scan_timing(gb_index *index, int on);
 float gb_index_last_scan_ms(gb_index *index);

@@ -54,6 +54,9 @@ def _declare(l):
     l.gb_index_search_device_keys.argtypes = [vp, i32, vp, i64, i32, cstr, i32, vp, vp, vp, vp]
     l.gb_index_stage_times.argtypes = [vp, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]
     l.gb_merge_partition_keys_device.argtypes = [i32, vp, i32, i32, i32, i32, vp, vp, vp]
+    l.gb_index_set_rerank_stats.restype = None
+    l.gb_index_set_rerank_stats.argtypes = [vp, i32]
+    l.gb_index_rerank_survivors.argtypes = [vp, C.POINTER(C.c_void_p), C.POINTER(i64)]
     l.gb_index_set_scan_timing.restype = None
     l.gb_index_set_scan_timing.argtypes = [vp, i32]
     l.gb_index_last_scan_ms.restype = f32

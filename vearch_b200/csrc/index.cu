@@ -248,11 +248,13 @@ int RawStore::append_host(const void* xv, int64_t n, cudaStream_t st) {
     } else {
       GB_CUDA(cudaMemcpy2DAsync(segs_[si].base + off * stride_, stride_, x + done * row_bytes_, row_bytes_, row_bytes_,
                                 (size_t)cnt, cudaMemcpyHostToDevice, st));
+      if (encode_shadow(si, off, cnt, st)) return -1;
     }
     done += cnt;
   }
   GB_CUDA(cudaStreamSynchronize(st));
   n_ += n;
+  if (shadow_) shadow_->n_ = n_;
   return 0;
 }
 int RawStore::append_device(const void* xv, int64_t ld_bytes, int64_t n, cudaStream_t st) {
@@ -265,10 +267,12 @@ int RawStore::append_device(const void* xv, int64_t ld_bytes, int64_t n, cudaStr
     int64_t cnt = std::min(n - done, seg_rows() - off);
     GB_CUDA(cudaMemcpy2DAsync(segs_[si].base + off * stride_, stride_, x + done * ld_bytes, (size_t)ld_bytes, row_bytes_,
                               (size_t)cnt, host_ ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, st));
+    if (encode_shadow(si, off, cnt, st)) return -1;
     done += cnt;
   }
   GB_CUDA(cudaStreamSynchronize(st));
   n_ += n;
+  if (shadow_) shadow_->n_ = n_;
   return 0;
 }
 int RawStore::update_host(int64_t vid, const void* x, cudaStream_t st) {
@@ -279,7 +283,21 @@ int RawStore::update_host(int64_t vid, const void* x, cudaStream_t st) {
     return 0;
   }
   GB_CUDA(cudaMemcpyAsync(segs_[si].base + off * stride_, x, row_bytes_, cudaMemcpyHostToDevice, st));
+  if (encode_shadow(si, off, 1, st)) return -1;
   GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+void RawStore::enable_shadow() {
+  if (host_ || shadow_ || n_ > 0 || row_bytes_ % 4) return;
+  const int cols16 = (int)round_up(stride_ / 4, 16);
+  shadow_.reset(new RawStore(cols16 + 16, seg_shift_, false));
+}
+// the shadow rows of fp32 rows [off, off + cnt) of segment si, ordered on st after their copy
+int RawStore::encode_shadow(int64_t si, int64_t off, int64_t cnt, cudaStream_t st) {
+  if (!shadow_) return 0;
+  if (shadow_->ensure((si << seg_shift_) + off + cnt)) return -1;
+  GB_CUDA(launch_shadow_encode(seg((int)si) + off * stride_ / 4, stride_ / 4, cnt, (int)(stride_ / 4),
+                               shadow_->segs_[si].base + off * shadow_->stride_, shadow_->stride_, st));
   return 0;
 }
 int RawStore::get_host(int64_t vid, void* out) const {
@@ -2156,6 +2174,7 @@ int IvfPqBase::encode_host(const float* x, int64_t n, const int64_t* assign, uin
 IVFPQIndex::IVFPQIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift)
     : IvfPqBase(type, d, mp, device, seg_shift, std::max(1, mp.nsubvector > 0 ? mp.nsubvector : d / 2), 1 << mp.nbits),
       nbits_(mp.nbits) {
+  if (!gpu_contract_) store_->enable_shadow();  // GPU_IVFPQ never re-ranks
   if (mp.opq_nsubvector > 0) {  // faiss::OPQMatrix(d, opq_nsubvector, d) (gamma_index_ivfpq.cc:168-178)
     cudaMalloc(&d_opq_, (size_t)d * dpad_ * 4);
     cudaMemset(d_opq_, 0, (size_t)d * dpad_ * 4);
@@ -2605,7 +2624,21 @@ int IvfIndex::scan_query_major_dev(const char* kernel, const SearchContext& ctx,
       GB_CUDA(cudaMemcpyAsync(keys, partial, (size_t)nq * kk * 8, cudaMemcpyDeviceToDevice, st));
     }
   }
-  if (rerank) {
+  if (rerank && store_->has_shadow()) {
+    int* surv = rr_stats_ ? s.alloc_n<int>((size_t)nq) : nullptr;
+    {
+      StageScope stage(this, "rerank_kernel", st);
+      GB_CUDA(launch_rerank_prefilter(keys, kk, nq, rerank_xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_,
+                                      store_->shadow_segs(), store_->shadow_stride(), k, metric, f, out_keys, surv, st));
+    }
+    if (surv) {
+      std::vector<int> h(nq);
+      GB_CUDA(cudaMemcpyAsync(h.data(), surv, (size_t)nq * sizeof(int), cudaMemcpyDeviceToHost, st));
+      GB_CUDA(cudaStreamSynchronize(st));
+      std::lock_guard<std::mutex> g(ev_mu_);
+      rr_survivors_.insert(rr_survivors_.end(), h.begin(), h.end());
+    }
+  } else if (rerank) {
     StageScope stage(this, "rerank_kernel", st);
     // host placement: the candidate rows come over PCIe straight from the mapped segments
     GB_CUDA(launch_rerank(keys, kk, nq, rerank_xq, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_,
@@ -2982,6 +3015,7 @@ VearchIndex::VearchIndex(int d, const ModelParams& mp, int device, int seg_shift
   if (mp_.ns_threshold < 0 || mp_.metric == kMetricL2) mp_.ns_threshold = std::nan("");
   cudaMalloc(&d_cb_, (size_t)16 * d * 4);
   cudaMemset(d_cb_, 0, (size_t)16 * d * 4);
+  if (mp_.reordering) store_->enable_shadow();  // only reordering re-ranks
 }
 VearchIndex::~VearchIndex() { cudaFree(d_cb_); }
 int64_t VearchIndex::index_mem_bytes() const { return IvfIndex::index_mem_bytes() + (int64_t)16 * d_ * 4; }

@@ -88,10 +88,21 @@ class RawStore {
   const float* contiguous(int64_t n, Scratch& s);
   // rows [start, start + n) (stride() bytes apart) into device memory at dst, ordered on st
   cudaError_t copy_rows_to_device(int64_t start, int64_t n, void* dst, cudaStream_t st) const;
-  int64_t mem_bytes() const { return phys_bytes_; }  // physical HBM behind the store (0 for host placement)
+  // physical HBM behind the store, its int8 shadow included (0 for host placement)
+  int64_t mem_bytes() const { return phys_bytes_ + (shadow_ ? shadow_->phys_bytes_ : 0); }
   int64_t host_bytes() const { return host_bytes_; }  // pinned host memory behind the store
+  // The int8 shadow of fp32 rows that the two-pass exact re-rank screens candidates with (launch_rerank_prefilter):
+  // row vid at shadow_segs()[vid >> seg_shift()] + (vid & (seg_rows() - 1)) * shadow_stride().  Written with the fp32
+  // rows in the same stream-ordered step, so whatever sees a row sees its shadow.  Only an HBM store of fp32 rows gets
+  // one, and only while it is empty (enable_shadow is a no-op otherwise).
+  void enable_shadow();
+  bool has_shadow() const { return shadow_ != nullptr; }
+  const unsigned char* const* shadow_segs() const { return shadow_->d_segs_; }
+  int64_t shadow_stride() const { return shadow_->stride_; }
 
  private:
+  int encode_shadow(int64_t si, int64_t off, int64_t cnt, cudaStream_t st);
+  std::unique_ptr<RawStore> shadow_;
   int ensure(int64_t n_total);
   int new_segment();
   int map_rows(int si, int64_t rows);
@@ -302,6 +313,13 @@ class Index {
   void set_time_scan(bool on) { time_scan_ = on; }
   const char* last_scan_kernel() const { return last_scan_kernel_; }
   const char* last_scan_info() const { return last_scan_info_; }  // JSON details of the last scan path (bench)
+  // While on, every search that re-ranks through the two-pass kernel records, per query, how many candidates' fp32
+  // rows it read (and waits for the count); take_rerank_survivors() returns and clears them.  Off by default.
+  void set_rerank_stats(bool on) { rr_stats_ = on; }
+  std::vector<int> take_rerank_survivors() {
+    std::lock_guard<std::mutex> g(ev_mu_);
+    return std::move(rr_survivors_);
+  }
 
  protected:
   // Device queries, here and below: nq rows store().stride() bytes apart, zero padded (dpad floats; BINARYIVF: words).
@@ -425,6 +443,8 @@ class Index {
   std::mutex ev_mu_;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> scan_events_;
   bool time_scan_ = false;
+  bool rr_stats_ = false;
+  std::vector<int> rr_survivors_;  // under ev_mu_
   const char* last_scan_kernel_ = "";  // which scan path served the last search (bench roofline label)
   char last_scan_info_[160] = "{}";
 };
@@ -735,7 +755,9 @@ class IVFPQFastScanIndex : public IvfPqBase {
  public:
   static constexpr int kKsub = 16;
   IVFPQFastScanIndex(int d, const ModelParams& mp, int device, int seg_shift)
-      : IvfPqBase("IVFPQFastScan", d, mp, device, seg_shift, mp.nsubvector, kKsub) {}
+      : IvfPqBase("IVFPQFastScan", d, mp, device, seg_shift, mp.nsubvector, kKsub) {
+    store_->enable_shadow();
+  }
   int code_bytes() const override { return (M_ + 1) / 2; }
   // M above this: faiss's 16-bit table sums could wrap (255 * 257 < 2^16), and the byte-pair table grows past what
   // the scan's shared memory holds beside its stages and queue
@@ -808,7 +830,9 @@ class BinaryIvfIndex : public IvfIndex {
 class RaBitQIndex : public IvfIndex {
  public:
   RaBitQIndex(int d, const ModelParams& mp, int device, int seg_shift)
-      : IvfIndex("IVFRABITQ", d, mp, device, seg_shift), nb_bits_(mp.nb_bits), qb_(mp.qb) {}
+      : IvfIndex("IVFRABITQ", d, mp, device, seg_shift), nb_bits_(mp.nb_bits), qb_(mp.qb) {
+    store_->enable_shadow();
+  }
   int code_bytes() const override { return rabitq_code_bytes(d_, nb_bits_); }
   bool persists_trained_state() const override { return false; }
   int nb_bits() const { return nb_bits_; }

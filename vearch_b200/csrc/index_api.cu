@@ -369,6 +369,20 @@ int gb_index_stage_times(gb_index* index, char** json_out, int* out_len) {
   return 0;
 }
 
+void gb_index_set_rerank_stats(gb_index* index, int on) {
+  if (index && index->impl) index->impl->set_rerank_stats(on != 0);
+}
+int gb_index_rerank_survivors(gb_index* index, int** out, int64_t* n) {
+  IDX_OR_FAIL(index);
+  const std::vector<int> v = index->impl->take_rerank_survivors();
+  int* p = static_cast<int*>(malloc(std::max<size_t>(1, v.size()) * sizeof(int)));
+  if (!p) return -1;
+  if (!v.empty()) memcpy(p, v.data(), v.size() * sizeof(int));
+  *out = p;
+  *n = (int64_t)v.size();
+  return 0;
+}
+
 void gb_index_set_scan_timing(gb_index* index, int on) {
   if (index && index->impl) index->impl->set_time_scan(on != 0);
 }

@@ -218,6 +218,48 @@ struct IvfpqPackedCodec {
 // ---------------- exact re-rank -------------------------------------------------------------
 constexpr int RR_NT = 256;
 
+// The exact score of RR_U rows (nullptr: no row, score unused) against the query q4 (shared memory, d a multiple of 4):
+// lane l takes the float4 columns l, l + 32, ... of each row into four FMA accumulators, then (a0 + a1) + (a2 + a3) and
+// an xor-shuffle tree, so every lane ends with the same dis[u].  Both re-rank kernels score through this routine only:
+// the two-pass kernel's keys are bit-identical to the one-pass kernel's by construction.
+template <int RR_U>
+__device__ __forceinline__ void rr_exact_scores(const float4* q4, const float4* const (&row)[RR_U], int d, int metric,
+                                                float (&dis)[RR_U]) {
+  const int lane = threadIdx.x & 31;
+  float acc[RR_U][4];
+#pragma unroll
+  for (int u = 0; u < RR_U; u++) acc[u][0] = acc[u][1] = acc[u][2] = acc[u][3] = 0.f;
+  for (int c = lane; c < (d >> 2); c += 32) {
+    const float4 w = q4[c];
+    float4 v[RR_U];
+#pragma unroll
+    for (int u = 0; u < RR_U; u++) v[u] = row[u] ? __ldg(row[u] + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int u = 0; u < RR_U; u++) {
+      if (metric == kMetricL2) {
+        const float t0 = v[u].x - w.x, t1 = v[u].y - w.y, t2 = v[u].z - w.z, t3 = v[u].w - w.w;
+        acc[u][0] = fmaf(t0, t0, acc[u][0]), acc[u][1] = fmaf(t1, t1, acc[u][1]);
+        acc[u][2] = fmaf(t2, t2, acc[u][2]), acc[u][3] = fmaf(t3, t3, acc[u][3]);
+      } else {
+        acc[u][0] = fmaf(v[u].x, w.x, acc[u][0]), acc[u][1] = fmaf(v[u].y, w.y, acc[u][1]);
+        acc[u][2] = fmaf(v[u].z, w.z, acc[u][2]), acc[u][3] = fmaf(v[u].w, w.w, acc[u][3]);
+      }
+    }
+  }
+#pragma unroll
+  for (int u = 0; u < RR_U; u++) {
+    dis[u] = (acc[u][0] + acc[u][1]) + (acc[u][2] + acc[u][3]);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) dis[u] += __shfl_xor_sync(0xffffffffu, dis[u], off);
+  }
+}
+
+__device__ __forceinline__ const float4* rr_row(const float* const* raw_segments, int seg_shift, int64_t ld_raw,
+                                                 uint32_t vid) {
+  return reinterpret_cast<const float4*>(raw_segments[vid >> seg_shift] +
+                                         (int64_t)(vid & ((1u << seg_shift) - 1u)) * ld_raw);
+}
+
 // RR_U: candidates a warp gathers per iteration.  Four keep 2 KiB of independent row loads in flight per warp, which
 // covers HBM latency (eight cost occupancy; the gather is pure latency: recall_num random 4d-byte rows per query).
 // Rows in mapped host memory come over PCIe, whose round trip is several times longer: eight per warp there.
@@ -235,51 +277,340 @@ __global__ void __launch_bounds__(RR_NT)
   for (int i = threadIdx.x; i < NP; i += RR_NT) buf[i] = kKeySentinel;
   __syncthreads();
   const float4* q4 = reinterpret_cast<const float4*>(qs);
-  const uint32_t seg_mask = (1u << seg_shift) - 1u;
   for (int j0 = warp * RR_U; j0 < ncand; j0 += (RR_NT / 32) * RR_U) {
     uint32_t vid[RR_U];
     const float4* row[RR_U];
-    bool live[RR_U];
 #pragma unroll
     for (int u = 0; u < RR_U; u++) {
       const int j = j0 + u;
       const unsigned long long ck = j < ncand ? cand_keys[(int64_t)q * ncand + j] : kKeySentinel;
-      live[u] = ck != kKeySentinel;  // recall_idxi[j] < 0 (ivfpq.cc:691)
-      vid[u] = live[u] ? (uint32_t)ck : 0u;
-      row[u] = live[u] ? reinterpret_cast<const float4*>(raw_segments[vid[u] >> seg_shift] + (int64_t)(vid[u] & seg_mask) * ld_raw)
-                       : nullptr;
+      vid[u] = (uint32_t)ck;
+      row[u] = ck != kKeySentinel ? rr_row(raw_segments, seg_shift, ld_raw, vid[u]) : nullptr;  // recall_idxi[j] < 0 (ivfpq.cc:691)
     }
-    float acc[RR_U][4];
+    float dis[RR_U];
+    rr_exact_scores<RR_U>(q4, row, d, metric, dis);
 #pragma unroll
-    for (int u = 0; u < RR_U; u++) acc[u][0] = acc[u][1] = acc[u][2] = acc[u][3] = 0.f;
-    for (int c = lane; c < (d >> 2); c += 32) {
-      const float4 w = q4[c];
-      float4 v[RR_U];
-#pragma unroll
-      for (int u = 0; u < RR_U; u++) v[u] = live[u] ? __ldg(row[u] + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int u = 0; u < RR_U; u++) {
-        if (metric == kMetricL2) {
-          const float t0 = v[u].x - w.x, t1 = v[u].y - w.y, t2 = v[u].z - w.z, t3 = v[u].w - w.w;
-          acc[u][0] = fmaf(t0, t0, acc[u][0]), acc[u][1] = fmaf(t1, t1, acc[u][1]);
-          acc[u][2] = fmaf(t2, t2, acc[u][2]), acc[u][3] = fmaf(t3, t3, acc[u][3]);
-        } else {
-          acc[u][0] = fmaf(v[u].x, w.x, acc[u][0]), acc[u][1] = fmaf(v[u].y, w.y, acc[u][1]);
-          acc[u][2] = fmaf(v[u].z, w.z, acc[u][2]), acc[u][3] = fmaf(v[u].w, w.w, acc[u][3]);
-        }
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < RR_U; u++) {
-      float dis = (acc[u][0] + acc[u][1]) + (acc[u][2] + acc[u][3]);
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) dis += __shfl_xor_sync(0xffffffffu, dis, off);
-      if (lane == 0 && live[u] && dis <= f.max_score && dis >= f.min_score) buf[j0 + u] = make_key(score2ord(dis, metric), vid[u]);
-    }
+    for (int u = 0; u < RR_U; u++)
+      if (lane == 0 && row[u] && dis[u] <= f.max_score && dis[u] >= f.min_score)
+        buf[j0 + u] = make_key(score2ord(dis[u], metric), vid[u]);
   }
   __syncthreads();
   block_bitonic_sort(buf, NP);
   for (int i = threadIdx.x; i < k; i += RR_NT) out_keys[(int64_t)q * k + i] = i < NP ? buf[i] : kKeySentinel;
+}
+
+// ---------------- two-pass exact re-rank over the int8 shadow of the raw rows ---------------------------------------
+// Shadow row of y (RawStore, kernels_ivfpq.cu shadow_encode_kernel): cols16 = round_up(dpad, 16) int8 values
+// qy = rn(y / s), s = max|y| / 127, zero padded, then float4 {s, e, nrm, 0} with e >= |y - s qy| and nrm >= |s qy|
+// (both rounded up).  A row whose scale is zero or not finite has e = nrm = inf: it is unbounded.
+//
+// Pass 1 bounds every candidate's fp32 score from its shadow row (DESIGN §3, "Exact re-rank"): [lo, hi] surely holds
+// the value rr_exact_scores returns.  B = the k-th best hi among the live bounded candidates whose whole interval lies
+// inside the score window; a candidate whose lo is worse than B has k candidates surely better than it, so it cannot
+// be among the k results.  Pass 2 reads the fp32 rows of the others (lo <= B, so ties at the k-th score survive; and
+// every unbounded one) and scores them through rr_exact_scores.
+constexpr int RS_U = 4;  // candidates per 8-lane group in pass 1: 16 shadow rows (2.3 KiB at d = 128) in flight per warp
+constexpr uint32_t kOrdDead = 0xFFFFFFFFu;   // lo of a dead candidate, hi of one that does not bound B
+constexpr uint32_t kOrdNoBound = 0xFFFFFFFEu;  // B with fewer than k bounding candidates: every live one survives
+
+// the k-th smallest of v[0, n) (1 <= k <= n), by an MSB-first radix select over the bytes: four histogram passes
+__device__ __forceinline__ uint32_t block_kth_smallest(const uint32_t* v, int n, int k) {
+  __shared__ int s_hist[256];
+  __shared__ uint32_t s_prefix;
+  __shared__ int s_need;
+  const int tid = threadIdx.x, lane = tid & 31;
+  uint32_t prefix = 0;
+  int need = k;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = tid; i < 256; i += blockDim.x) s_hist[i] = 0;
+    __syncthreads();
+    for (int i = tid; i < n; i += blockDim.x) {
+      const uint32_t x = v[i];
+      if (shift == 24 || (x >> (shift + 8)) == (prefix >> (shift + 8))) atomicAdd(&s_hist[(x >> shift) & 255], 1);
+    }
+    __syncthreads();
+    if (tid < 32) {
+      int h[8], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; j++) sum += (h[j] = s_hist[lane * 8 + j]);
+      int incl = sum;
+#pragma unroll
+      for (int off = 1; off < 32; off <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, off);
+        if (lane >= off) incl += t;
+      }
+      int before = incl - sum;
+      if (before < need && need <= incl) {
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+          if (before < need && need <= before + h[j]) {
+            s_prefix = prefix | ((uint32_t)(lane * 8 + j) << shift);
+            s_need = need - before;
+          }
+          before += h[j];
+        }
+      }
+    }
+    __syncthreads();
+    prefix = s_prefix;
+    need = s_need;
+  }
+  return prefix;
+}
+
+// ascending sort of one key per lane
+__device__ __forceinline__ unsigned long long warp_sort32(unsigned long long x) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int k = 2; k <= 32; k <<= 1) {
+#pragma unroll
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      const unsigned long long y = __shfl_xor_sync(0xffffffffu, x, j);
+      const bool keep_min = ((lane & j) == 0) == ((lane & k) == 0);
+      x = keep_min ? (x < y ? x : y) : (x < y ? y : x);
+    }
+  }
+  return x;
+}
+
+// int8 byte b of w (two's complement) as an exact float: the byte, offset by 128, is the low mantissa byte of 2^23
+__device__ __forceinline__ float rs_qy(uint32_t w_biased, int b) {
+  return __uint_as_float(__byte_perm(w_biased, 0x4B000000u, 0x7540u + b)) - 8388736.0f;
+}
+
+template <int METRIC>
+__global__ void __launch_bounds__(RR_NT)
+    rerank_prefilter_kernel(const unsigned long long* __restrict__ cand_keys, int ncand, int NP,
+                            const float* __restrict__ xq, int64_t ldq, int d, const float* const* __restrict__ raw_segments,
+                            int seg_shift, int64_t ld_raw, const unsigned char* const* __restrict__ shadow_segs,
+                            int64_t shadow_stride, int cols16, int k, FilterArgs f,
+                            unsigned long long* __restrict__ out_keys, int* __restrict__ survivors) {
+  extern __shared__ __align__(16) unsigned char rr_smem[];
+  unsigned long long* buf = reinterpret_cast<unsigned long long*>(rr_smem);  // [NP] survivors' keys
+  float* qs = reinterpret_cast<float*>(buf + NP);                              // [cols16], zero padded
+  uint32_t* lo = reinterpret_cast<uint32_t*>(qs + cols16);                     // [NP] best ordinal a candidate can have
+  uint32_t* hi = lo + NP;                                                      // [NP] worst ordinal; then survivors' vids
+  __shared__ double s_qn;
+  __shared__ int s_nsurv;
+  const int q = blockIdx.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int i = threadIdx.x; i < cols16; i += RR_NT) qs[i] = i < d ? xq[(int64_t)q * ldq + i] : 0.f;
+  for (int i = threadIdx.x; i < NP; i += RR_NT) buf[i] = kKeySentinel;
+  if (threadIdx.x == 0) s_nsurv = 0;
+  __syncthreads();
+  if (warp == 0) {  // |q|, rounded up
+    double a = 0.0;
+    for (int i = lane; i < d; i += 32) a = __fma_ru((double)qs[i], (double)qs[i], a);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) a = __dadd_ru(a, __shfl_xor_sync(0xffffffffu, a, off));
+    if (lane == 0) s_qn = __dsqrt_ru(a);
+  }
+  __syncthreads();
+  // Rounding of fp32 sums of d (cols16) terms in any order, relative (u = 2^-24) ...
+  const double u = 0x1p-24;
+  const double g1 = 1.01 * (cols16 + 3) * u, gr = 1.01 * (d + 3) * u;
+  // ... plus at most 2^-150 per fp32 operation whose result is subnormal (the relative terms alone fail there)
+  const double ab = (4.0 * cols16 + 64.0) * 0x1p-149;
+  const double qn = s_qn;
+
+  // ---- pass 1: an interval per candidate from its shadow row; 8 lanes x 16 bytes per row ----
+  const int g = lane >> 3, sub = lane & 7;
+  const int nch = cols16 >> 4;
+  const float4* q4 = reinterpret_cast<const float4*>(qs);
+  for (int j0 = warp * 4 * RS_U; j0 < ncand; j0 += (RR_NT / 32) * 4 * RS_U) {
+    const unsigned char* srow[RS_U];
+    float4 meta[RS_U];
+#pragma unroll
+    for (int u2 = 0; u2 < RS_U; u2++) {
+      const int j = j0 + u2 * 4 + g;
+      const unsigned long long ck = j < ncand ? cand_keys[(int64_t)q * ncand + j] : kKeySentinel;
+      const uint32_t vid = (uint32_t)ck;
+      srow[u2] = ck != kKeySentinel
+                     ? shadow_segs[vid >> seg_shift] + (int64_t)(vid & ((1u << seg_shift) - 1u)) * shadow_stride
+                     : nullptr;
+      meta[u2] = srow[u2] ? __ldg(reinterpret_cast<const float4*>(srow[u2] + cols16)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    float acc[RS_U];
+#pragma unroll
+    for (int u2 = 0; u2 < RS_U; u2++) acc[u2] = 0.f;
+    for (int c = sub; c < nch; c += 8) {
+      uint4 w[RS_U];
+#pragma unroll
+      for (int u2 = 0; u2 < RS_U; u2++)
+        w[u2] = srow[u2] ? __ldg(reinterpret_cast<const uint4*>(srow[u2]) + c) : make_uint4(0u, 0u, 0u, 0u);
+      float qv[16];
+#pragma unroll
+      for (int t = 0; t < 4; t++) {
+        const float4 x = q4[c * 4 + t];
+        qv[4 * t] = x.x, qv[4 * t + 1] = x.y, qv[4 * t + 2] = x.z, qv[4 * t + 3] = x.w;
+      }
+#pragma unroll
+      for (int u2 = 0; u2 < RS_U; u2++) {
+        const uint32_t ww[4] = {w[u2].x ^ 0x80808080u, w[u2].y ^ 0x80808080u, w[u2].z ^ 0x80808080u,
+                                w[u2].w ^ 0x80808080u};
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+          const float y = rs_qy(ww[i >> 2], i & 3);
+          if (METRIC == kMetricL2) {
+            const float t = fmaf(-meta[u2].x, y, qv[i]);  // q - s qy, one rounding
+            acc[u2] = fmaf(t, t, acc[u2]);
+          } else {
+            acc[u2] = fmaf(qv[i], y, acc[u2]);
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int u2 = 0; u2 < RS_U; u2++) {
+      acc[u2] += __shfl_xor_sync(0xffffffffu, acc[u2], 1);
+      acc[u2] += __shfl_xor_sync(0xffffffffu, acc[u2], 2);
+      acc[u2] += __shfl_xor_sync(0xffffffffu, acc[u2], 4);
+    }
+    // lane sub < RS_U of group g finishes candidate j0 + sub * 4 + g
+    float a = 0.f;
+    float4 m = make_float4(0.f, 0.f, 0.f, 0.f);
+    bool live = false;
+#pragma unroll
+    for (int u2 = 0; u2 < RS_U; u2++)
+      if (u2 == sub) a = acc[u2], m = meta[u2], live = srow[u2] != nullptr;
+    const int j = j0 + sub * 4 + g;
+    if (sub < RS_U && j < ncand) {
+      uint32_t jlo = kOrdDead, jhi = kOrdDead;
+      if (live) {
+        const double st = a, s = m.x, e = m.y, nrm = m.z;
+        double slo, shi, mag;
+        if (METRIC == kMetricL2) {
+          // real |q - s qy|^2 from the fp32 sum; then |q - y| within e of its root; then the reference's own rounding
+          const double r2lo = fmax(0.0, __dmul_rd(__dsub_rd(st, ab), __dsub_rd(1.0, g1)));
+          const double r2hi = __dmul_ru(__dadd_ru(st, ab), __dadd_ru(1.0, 2.0 * g1));
+          const double rlo = fmax(0.0, __dsub_rd(__dsqrt_rd(r2lo), e));
+          const double rhi = __dadd_ru(__dsqrt_ru(r2hi), e);
+          slo = fmax(0.0, __dsub_rd(__dmul_rd(__dmul_rd(rlo, rlo), __dsub_rd(1.0, gr)), ab));
+          shi = __dadd_ru(__dmul_ru(__dmul_ru(rhi, rhi), __dadd_ru(1.0, gr)), ab);
+          mag = shi;
+        } else {
+          // <q, s qy> = s st within g1 |q| nrm + s ab; <q, y - s qy> within |q| e; the reference's rounding within
+          // gr sum |q_i y_i| + ab <= gr |q| (nrm + e) + ab
+          const double c = s * st;  // exact: two fp32 factors
+          double r = __dmul_ru(__dmul_ru(g1, qn), nrm);
+          r = __dadd_ru(r, __dmul_ru(s, ab));
+          r = __dadd_ru(r, __dmul_ru(qn, e));
+          const double yb = __dmul_ru(qn, __dadd_ru(nrm, e));
+          r = __dadd_ru(__dadd_ru(r, __dmul_ru(gr, yb)), ab);
+          slo = __dsub_rd(c, r);
+          shi = __dadd_ru(c, r);
+          mag = __dadd_ru(__dmul_ru(yb, __dadd_ru(1.0, gr)), ab);
+        }
+        // every partial sum of either evaluation stays below 2^126: no overflow; NaN or inf anywhere: unbounded
+        if (mag <= 0x1p126) {
+          const float flo = __double2float_rd(slo), fhi = __double2float_ru(shi);
+          jlo = score2ord<METRIC>(METRIC == kMetricL2 ? flo : fhi);
+          if (flo >= f.min_score && fhi <= f.max_score) jhi = score2ord<METRIC>(METRIC == kMetricL2 ? fhi : flo);
+        } else {
+          jlo = 0;
+        }
+      }
+      lo[j] = jlo;
+      hi[j] = jhi;
+    }
+  }
+  __syncthreads();
+
+  // ---- the bound, then the survivors' vids (compacted into hi) ----
+  uint32_t B = block_kth_smallest(hi, ncand, k < ncand ? k : ncand);
+  if (B == kOrdDead) B = kOrdNoBound;
+  for (int j0 = 0; j0 < ncand; j0 += RR_NT) {
+    const int j = j0 + threadIdx.x;
+    const bool keep = j < ncand && lo[j] <= B;
+    const unsigned mask = __ballot_sync(0xffffffffu, keep);
+    if (mask) {
+      int base = 0;
+      if (lane == 0) base = atomicAdd(&s_nsurv, __popc(mask));
+      base = __shfl_sync(0xffffffffu, base, 0);
+      if (keep) hi[base + __popc(mask & ((1u << lane) - 1u))] = (uint32_t)cand_keys[(int64_t)q * ncand + j];
+    }
+  }
+  __syncthreads();
+  const int nsurv = s_nsurv;
+
+  // ---- pass 2: exact scores of the survivors ----
+  for (int i0 = warp * 4; i0 < nsurv; i0 += (RR_NT / 32) * 4) {
+    const float4* row[4];
+    uint32_t vid[4];
+#pragma unroll
+    for (int u2 = 0; u2 < 4; u2++) {
+      vid[u2] = i0 + u2 < nsurv ? hi[i0 + u2] : 0u;
+      row[u2] = i0 + u2 < nsurv ? rr_row(raw_segments, seg_shift, ld_raw, vid[u2]) : nullptr;
+    }
+    float dis[4];
+    rr_exact_scores<4>(q4, row, d, METRIC, dis);
+#pragma unroll
+    for (int u2 = 0; u2 < 4; u2++)
+      if (lane == 0 && row[u2] && dis[u2] <= f.max_score && dis[u2] >= f.min_score)
+        buf[i0 + u2] = make_key(score2ord<METRIC>(dis[u2]), vid[u2]);
+  }
+  __syncthreads();
+  if (nsurv <= 32) {
+    if (warp == 0) {
+      const unsigned long long x = warp_sort32(lane < NP ? buf[lane] : kKeySentinel);
+      if (lane < NP) buf[lane] = x;
+    }
+    __syncthreads();
+  } else {
+    block_bitonic_sort(buf, next_pow2(nsurv));
+  }
+  for (int i = threadIdx.x; i < k; i += RR_NT) out_keys[(int64_t)q * k + i] = i < NP ? buf[i] : kKeySentinel;
+  if (survivors && threadIdx.x == 0) survivors[q] = nsurv;
+}
+
+// ---------------- the int8 shadow rows (one warp per row) -------------------------------------------------------------
+constexpr int SE_NT = 256;
+__global__ void __launch_bounds__(SE_NT)
+    shadow_encode_kernel(const float* __restrict__ rows, int64_t ld, int64_t n, int cols, int cols16,
+                         unsigned char* __restrict__ out, int64_t out_stride) {
+  const int64_t r = (int64_t)blockIdx.x * (SE_NT / 32) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= n) return;
+  const float* y = rows + r * ld;
+  unsigned char* o = out + r * out_stride;
+  float amax = 0.f;
+  bool bad = false;
+  for (int i = lane; i < cols; i += 32) {
+    const float v = y[i];
+    bad |= !isfinite(v);
+    amax = fmaxf(amax, fabsf(v));
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, off));
+  bad = __any_sync(0xffffffffu, bad);
+  const float s = __fdiv_rn(amax, 127.0f);
+  const bool ok = !bad && s > 0.f && isfinite(s);
+  double e2 = 0.0, n2 = 0.0;
+  for (int i = lane; i < cols16; i += 32) {
+    float qv = 0.f;
+    if (ok && i < cols) {
+      qv = fminf(127.f, fmaxf(-127.f, rintf(__fdiv_rn(y[i], s))));
+      const double t = (double)y[i] - (double)s * (double)qv;  // s qv is exact in fp64
+      e2 += t * t;
+      n2 += (double)qv * (double)qv;  // exact
+    }
+    o[i] = (unsigned char)(signed char)(int)qv;
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    e2 += __shfl_xor_sync(0xffffffffu, e2, off);
+    n2 += __shfl_xor_sync(0xffffffffu, n2, off);
+  }
+  if (lane == 0) {
+    float4 m = make_float4(0.f, __int_as_float(0x7F800000), __int_as_float(0x7F800000), 0.f);
+    if (ok) {
+      // e2 is within (cols + 5) 2^-53 of the exact sum: the factor 1 + 2^-30 covers that for any row width here
+      m.x = s;
+      m.y = __double2float_ru(__dmul_ru(__dsqrt_ru(e2), 1.0 + 0x1p-30));
+      m.z = __double2float_ru(__dmul_ru((double)s, __dsqrt_ru(n2)));
+    }
+    *reinterpret_cast<float4*>(o + cols16) = m;
+  }
 }
 
 // ---------------- PQ encode -------------------------------------------------------------------
@@ -410,6 +741,39 @@ cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq
   }
   kern<<<nq, RR_NT, smem, st>>>(cand_keys, ncand, NP, xq, ldq, d, raw_segments, seg_shift, ld_raw, k, metric, f,
                                 out_keys);
+  note_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_rerank_prefilter(const unsigned long long* cand_keys, int ncand, int nq, const float* xq, int64_t ldq,
+                                    int d, const float* const* raw_segments, int seg_shift, int64_t ld_raw,
+                                    const unsigned char* const* shadow_segs, int64_t shadow_stride, int k, int metric,
+                                    FilterArgs f, unsigned long long* out_keys, int* survivors, cudaStream_t st) {
+  if (nq <= 0) return cudaSuccess;
+  const int cols16 = (d + 15) & ~15;
+  if (ncand <= 0 || ncand > 8192 || k <= 0 || k > ncand || (d & 3) || shadow_stride != cols16 + 16)
+    return cudaErrorInvalidValue;
+  const int NP = next_pow2(ncand < 2 ? 2 : ncand);
+  const size_t smem = (size_t)NP * 8 + (size_t)cols16 * 4 + (size_t)NP * 8;
+  auto kern = metric == kMetricL2 ? rerank_prefilter_kernel<kMetricL2> : rerank_prefilter_kernel<kMetricIP>;
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
+  kern<<<nq, RR_NT, smem, st>>>(cand_keys, ncand, NP, xq, ldq, d, raw_segments, seg_shift, ld_raw, shadow_segs,
+                                shadow_stride, cols16, k, f, out_keys, survivors);
+  note_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_shadow_encode(const float* rows, int64_t ld, int64_t n, int cols, unsigned char* out,
+                                 int64_t out_stride, cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
+  const int cols16 = (cols + 15) & ~15;
+  if (out_stride != cols16 + 16) return cudaErrorInvalidValue;
+  const int64_t rows_per_cta = SE_NT / 32;
+  shadow_encode_kernel<<<(unsigned)((n + rows_per_cta - 1) / rows_per_cta), SE_NT, 0, st>>>(rows, ld, n, cols, cols16, out,
+                                                                                           out_stride);
   note_launch();
   return cudaGetLastError();
 }

@@ -201,6 +201,19 @@ class GammaIndex:
         C.CDLL(None).free(C.c_void_p(p.value))
         return json.loads(js)
 
+    def set_rerank_stats(self, on):
+        """while on, every search that re-ranks through the two-pass kernel records, per query, the candidates whose
+        fp32 rows it read (the search then waits for the count)"""
+        _lib.lib().gb_index_set_rerank_stats(self._h, int(on))
+
+    def rerank_survivors(self):
+        """int32 array of the per-query survivor counts recorded since the last call (set_rerank_stats(True) first)"""
+        p, n = C.c_void_p(), C.c_int64()
+        _check(_lib.lib().gb_index_rerank_survivors(self._h, C.byref(p), C.byref(n)), "rerank_survivors")
+        out = np.frombuffer(C.string_at(p.value, 4 * n.value), np.int32).copy()
+        C.CDLL(None).free(C.c_void_p(p.value))
+        return out
+
     def set_scan_timing(self, on):
         _lib.lib().gb_index_set_scan_timing(self._h, int(on))
 
