@@ -228,6 +228,10 @@ int gb_merge_partition_keys_device(int device, const unsigned long long *keys_de
 int gb_debug_dist_matrix(int device, const float *x, int n, const float *c, int m, int d, int metric, int use_tc,
                          float *out);
 
+/* the device's default memory pool, which every search's scratch comes from: bytes in use and the high-water mark
+ * since the last reset (after the device's pending work); reset_peak != 0 then restarts the mark at the current use */
+int gb_device_pool_usage(int device, int reset_peak, int64_t *used, int64_t *peak);
+
 /* ---- host-logic test hooks: run the C++ wire codecs of the gamma boundary without a GPU ---- */
 /* RequestConcurrentController (search/engine.cc:47-119): op 0 threshold, 1 in-flight, 2 set threshold (<= 0: system value),
  * 3 Acquire(value) -> 1/0, 4 Release(value) */

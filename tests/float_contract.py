@@ -6,11 +6,17 @@ inputs within a rigorous bound on the error of its arithmetic form.  Let u = 2^-
 
   direct L2   t = fl(x_j - y_j), t^2 accumulated       1.01 (d + 3) u sum (x_j - y_j)^2
   direct IP   x_j y_j accumulated                      1.01 (d + 1) u sum |x_j y_j|
-  3xTF32 dot  wgmma, hi*hi + hi*lo + lo*hi             C_TC (d + 4) u sum |a_j b_j|
+  3xTF32 dot  wgmma, hi*hi + hi*lo + lo*hi             (48 + C_TC (d + 4)) u sum |a_j b_j|
   expanded L2 |a|^2 + |b|^2 - 2 a.b over a, b          2 dot margin + (d + 2) u (|a|^2 + |b|^2) + u score
 
+The 3xTF32 dot has two parts.  Representation: a = hi + lo exactly (hi keeps 10 explicit mantissa bits, so
+|lo| <= 2^-10 |a|), but wgmma reads lo as TF32 too, dropping its low bits (|lo - lo'| <= 2^-10 |lo| <= 2^-20 |a|), and
+lo*lo is never formed (|lo_a lo_b| <= 2^-20 |a b|): the three products miss a_j b_j by at most 3 * 2^-20 = 48 u of
+|a_j b_j|, whatever d.  Accumulation: the products and their fp32 sums, C_TC (d + 4) u.  Below d ~ 8 the first part
+dominates; without it dist_tc_kernel exceeded the margin at d = 1 by 1.5 %.
 Hopper does not document its wgmma fp32 accumulation as round-to-nearest, so C_TC is a model constant, checked on the
-GPU element-wise against the exact kernel's inputs (tests/test_gpu_float_accuracy.py).
+GPU element-wise against the exact kernel's inputs (tests/test_gpu_float_accuracy.py,
+tests/test_gpu_float_shape_limits.py from d = 1 to 4096).
 
 The fp64 reference uses the direct form: fp32 differences and products are exact or within 2^-53 relative in fp64,
 so its error is ~2^-29 of the fp32 margins; scores64 asserts it is below 1/1000 of them.
@@ -107,8 +113,11 @@ def direct_margin(f, absdot, d, metric):
     return l2_direct_margin(f, d) if metric == METRIC_L2 else ip_direct_margin(absdot, d)
 
 
+TF32_SPLIT = 3 * 2.0 ** -20  # the split's representation error per product, relative to |a_j b_j| (see above)
+
+
 def tc_dot_margin(absdot, d, c_tc=C_TC):
-    return c_tc * (d + 4) * U * np.asarray(absdot)
+    return (TF32_SPLIT + c_tc * (d + 4) * U) * np.asarray(absdot)
 
 
 def expanded_l2_margin(absdot, na, nb, score, d, c_tc=C_TC):

@@ -1137,9 +1137,13 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
   int64_t ldo = round_up(std::min<int64_t>(CC, nrows - row_begin), 4);
   int QB = (int)std::max<int64_t>(1, std::min<int64_t>(nq, ((int64_t)1 << 28) / ldo));  // <= 1 GiB of scores
   GB_ALLOC(scores, float, (size_t)QB * ldo, s);
+  // the chunks' partial keys of a block of PB queries stay within kScanPartialBudget (one query at least); each block is
+  // merged into out_keys before the next one reuses them
+  const int PB = nch > 1 ? (int)std::max<int64_t>(1, std::min<int64_t>(nq, kScanPartialBudget / ((int64_t)nch * k * 8)))
+                         : nq;
   unsigned long long* partial = out_keys;
   if (nch > 1) {
-    partial = s.alloc_n<unsigned long long>((size_t)nq * nch * k);
+    partial = s.alloc_n<unsigned long long>((size_t)PB * nch * k);
     if (!partial) return -1;
   }
   if (store_->on_host()) {
@@ -1162,34 +1166,45 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
       GB_CUDA(cudaEventRecord(cl.reusable[b], st));  // the buffers are allocated in stream order on st
     }
     scan_timer_begin(st);
-    for (int c = 0; c < nch; c++) {
-      const int b = c & 1;
-      GB_CUDA(cudaStreamWaitEvent(cl.cs, cl.reusable[b], 0));
-      GB_CUDA(cudaMemcpyAsync(stage[b], chunks[c].base, (size_t)chunks[c].cnt * ld, cudaMemcpyHostToDevice, cl.cs));
-      GB_CUDA(cudaEventRecord(cl.copied[b], cl.cs));
-      GB_CUDA(cudaStreamWaitEvent(st, cl.copied[b], 0));
-      for (int q0 = 0; q0 < nq; q0 += QB) {
-        int qb = std::min(QB, nq - q0);
-        GB_CUDA(flat_tile(xq + q0 * ld, qb, stage[b], chunks[c].cnt, metric, scores, ldo, st));
-        GB_CUDA(launch_select_scores(scores, ldo, qb, chunks[c].cnt, chunks[c].id0, k, metric, f,
-                                     partial + ((int64_t)q0 * nch + c) * k, (int64_t)nch * k, st));
+    int copies = 0;
+    for (int p0 = 0; p0 < nq; p0 += PB) {  // one block unless the partials need more: the rows stream once per block
+      const int pb = std::min(PB, nq - p0);
+      for (int c = 0; c < nch; c++, copies++) {
+        const int b = copies & 1;
+        GB_CUDA(cudaStreamWaitEvent(cl.cs, cl.reusable[b], 0));
+        GB_CUDA(cudaMemcpyAsync(stage[b], chunks[c].base, (size_t)chunks[c].cnt * ld, cudaMemcpyHostToDevice, cl.cs));
+        GB_CUDA(cudaEventRecord(cl.copied[b], cl.cs));
+        GB_CUDA(cudaStreamWaitEvent(st, cl.copied[b], 0));
+        for (int q0 = 0; q0 < pb; q0 += QB) {
+          int qb = std::min(QB, pb - q0);
+          GB_CUDA(flat_tile(xq + (p0 + q0) * ld, qb, stage[b], chunks[c].cnt, metric, scores, ldo, st));
+          GB_CUDA(launch_select_scores(scores, ldo, qb, chunks[c].cnt, chunks[c].id0, k, metric, f,
+                                       (nch > 1 ? partial + (int64_t)q0 * nch * k : out_keys + (int64_t)(p0 + q0) * k) +
+                                           (int64_t)c * k,
+                                       (int64_t)nch * k, st));
+        }
+        GB_CUDA(cudaEventRecord(cl.reusable[b], st));
       }
-      GB_CUDA(cudaEventRecord(cl.reusable[b], st));
+      if (nch > 1) GB_CUDA(launch_select_keys(partial, (int64_t)nch * k, pb, nch * k, k, out_keys + (int64_t)p0 * k, k, st));
     }
-    if (nch > 1) GB_CUDA(launch_select_keys(partial, (int64_t)nch * k, nq, nch * k, k, out_keys, k, st));
     scan_timer_end(st);
     return 0;
   }
   scan_timer_begin(st);
-  for (int q0 = 0; q0 < nq; q0 += QB) {
-    int qb = std::min(QB, nq - q0);
-    for (int c = 0; c < nch; c++) {
-      GB_CUDA(flat_tile(xq + q0 * ld, qb, chunks[c].base, chunks[c].cnt, metric, scores, ldo, st));
-      GB_CUDA(launch_select_scores(scores, ldo, qb, chunks[c].cnt, chunks[c].id0, k, metric, f,
-                                   partial + ((int64_t)q0 * nch + c) * k, (int64_t)nch * k, st));
+  for (int p0 = 0; p0 < nq; p0 += PB) {
+    const int pb = std::min(PB, nq - p0);
+    for (int q0 = 0; q0 < pb; q0 += QB) {
+      int qb = std::min(QB, pb - q0);
+      for (int c = 0; c < nch; c++) {
+        GB_CUDA(flat_tile(xq + (p0 + q0) * ld, qb, chunks[c].base, chunks[c].cnt, metric, scores, ldo, st));
+        GB_CUDA(launch_select_scores(scores, ldo, qb, chunks[c].cnt, chunks[c].id0, k, metric, f,
+                                     (nch > 1 ? partial + (int64_t)q0 * nch * k : out_keys + (int64_t)(p0 + q0) * k) +
+                                         (int64_t)c * k,
+                                     (int64_t)nch * k, st));
+      }
     }
+    if (nch > 1) GB_CUDA(launch_select_keys(partial, (int64_t)nch * k, pb, nch * k, k, out_keys + (int64_t)p0 * k, k, st));
   }
-  if (nch > 1) GB_CUDA(launch_select_keys(partial, (int64_t)nch * k, nq, nch * k, k, out_keys, k, st));
   scan_timer_end(st);
   return 0;
 }
@@ -2005,14 +2020,26 @@ int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int me
     }
     return 0;
   }
+  // Every query keeps k keys per (probe, split) until the merge, and the split count follows the longest list of the
+  // index: one list of 2^20 rows gives every query 128 splits per probe.  The batch is scanned in query blocks whose
+  // partials stay within kScanPartialBudget, as flat_search_dev blocks its score tiles.  A block holds one query at
+  // least, so a single query's nprobe x nsplit x k keys are the residual (nprobe 2048 over a 2^20-row list at
+  // k = 4096: 8.6 GB); cutting the probes as well would bound that too.
   int nparts = ivfflat_scan_nparts(nprobe, lists_->max_len());
-  GB_ALLOC(partial, unsigned long long, (size_t)nq * nparts * k, s);
-  scan_timer_begin(st);
+  const int64_t per_query = (int64_t)nparts * k * 8;
+  const int QB = (int)std::max<int64_t>(1, std::min<int64_t>(nq, kScanPartialBudget / per_query));
+  GB_ALLOC(partial, unsigned long long, (size_t)QB * nparts * k, s);
   int avg_len = (int)(lists_->total() / std::max(1, nlist_));
-  GB_CUDA(launch_ivfflat_scan(xq, dpad_, nq, dpad_, probe_ids, nprobe, lists_->directory(), lists_->max_len(), avg_len, k,
-                              metric, f, partial, &nparts, &last_scan_kernel_, st));
-  scan_timer_end(st);
-  GB_CUDA(launch_select_keys(partial, (int64_t)nparts * k, nq, nparts * k, k, out_keys, k, st));
+  for (int q0 = 0; q0 < nq; q0 += QB) {  // the scan timer covers the scans, never the merges (last_scan_ms sums them)
+    const int qb = std::min(QB, nq - q0);
+    nparts = ivfflat_scan_nparts(nprobe, lists_->max_len());
+    scan_timer_begin(st);
+    GB_CUDA(launch_ivfflat_scan(xq + (int64_t)q0 * dpad_, dpad_, qb, dpad_, probe_ids + (int64_t)q0 * nprobe, nprobe,
+                                lists_->directory(), lists_->max_len(), avg_len, k, metric, f, partial, &nparts,
+                                &last_scan_kernel_, st));
+    scan_timer_end(st);
+    GB_CUDA(launch_select_keys(partial, (int64_t)nparts * k, qb, nparts * k, k, out_keys + (int64_t)q0 * k, k, st));
+  }
   return 0;
 }
 
@@ -3210,6 +3237,22 @@ Index* create_index(const std::string& type, int d, const ModelParams& mp, int d
     return nullptr;
   }
   if (type == "FLAT") return new FlatIndex(d, mp, device, seg_shift);
+  if (type == "IVFFLAT" || type == "GPU_IVFFLAT") {
+    // small batches scan query-major (ivfflat_scan_kernel), whose ring, query and k = 4096 queue must fit one CTA's
+    // shared memory; refused here rather than as a CUDA error at every such search
+    int max_d = 0;
+    cudaError_t e = cudaSetDevice(device);
+    if (e == cudaSuccess) e = ivfflat_scan_max_dim(&max_d);
+    if (e != cudaSuccess) {
+      set_last_error(type + ": cannot query the list scan kernel: " + cudaGetErrorString(e));
+      return nullptr;
+    }
+    if (round_up(d, 4) > max_d) {
+      set_last_error(type + ": dimension [" + std::to_string(d) + "] above " + std::to_string(max_d) +
+                     " is not supported by this engine");
+      return nullptr;
+    }
+  }
   if (type == "IVFFLAT") {
     if (mp.ncentroids <= 0 || mp.nprobe > mp.ncentroids) {  // gamma_index_ivfflat.cc:277-286
       set_last_error("nprobe should be less than ncentroids");

@@ -256,6 +256,9 @@ class Index {
   // call and k' = max(k, recall_num) at most kGpuMaxK, refused before request coalescing; no exact re-rank; a request
   // nprobe outside (0, min(nlist, kGpuMaxK)] falls back to the model's (resolve_nprobe)
   static constexpr int kGpuMaxReq = 512, kGpuMaxK = 2048;
+  // bytes of per-(query, part) partial keys one scan step may hold (FLAT chunks, IVF-Flat query-major splits); larger
+  // batches are cut into query blocks
+  static constexpr int64_t kScanPartialBudget = (int64_t)1 << 30;
   bool gpu_contract() const { return gpu_contract_; }
   int d() const { return d_; }
   int device() const { return device_; }

@@ -741,6 +741,26 @@ int gb_debug_dist_matrix(int device, const float* x, int n, const float* c, int 
   return 0;
 }
 
+int gb_device_pool_usage(int device, int reset_peak, int64_t* used, int64_t* peak) {
+  if (cudaSetDevice(device) != cudaSuccess) {
+    set_last_error("no CUDA device");
+    return -1;
+  }
+  cudaMemPool_t pool;
+  uint64_t u = 0, h = 0;
+  GB_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
+  GB_CUDA(cudaDeviceSynchronize());  // stream-ordered frees of finished searches are returned to the pool
+  GB_CUDA(cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &u));
+  GB_CUDA(cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &h));
+  if (used) *used = (int64_t)u;
+  if (peak) *peak = (int64_t)h;
+  if (reset_peak) {
+    uint64_t zero = 0;  // the only value accepted: the high-water mark restarts at the current use
+    GB_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &zero));
+  }
+  return 0;
+}
+
 int gb_merge_partitions_device(int device, const float* dis_dev, const int64_t* ids_dev, int nparts, int nq, int k,
                                int metric, float* out_dis_dev, int64_t* out_ids_dev, void* stream) {
   if (cudaSetDevice(device) != cudaSuccess) {

@@ -79,6 +79,12 @@ cudaError_t launch_ivfflat_scan(const float* xq, int64_t ldq, int nq, int d, con
                                 ListDirectory dir, int max_list_len, int avg_list_len, int k, int metric, FilterArgs f,
                                 unsigned long long* partial, int* nparts_out, const char** kernel_out, cudaStream_t st);
 int ivfflat_scan_nparts(int nprobe, int max_list_len);
+// *nst = ring depth (4, 3 or 2) of the generic query-major scan at row width d (a multiple of 4) and k, 0 if none fits
+// (on the current device; an error if its image of the kernel cannot be queried)
+cudaError_t ivfflat_scan_stages(int d, int k, int* nst);
+// *max_d = the largest row width (a multiple of 4) the generic scan serves at k = 4096: IVFFLAT and GPU_IVFFLAT refuse
+// any d whose padded width is above it (4604 on sm_90; pinned, and restated from the shared-memory formula, in the tests)
+cudaError_t ivfflat_scan_max_dim(int* max_d);
 
 // K3 list-major (tensor cores): (query, probe) pairs grouped by list; tile = 128 pairs x 128 rows.
 struct LmTile {

@@ -8,15 +8,19 @@
 //
 // Two kernels.  ivfflat_scan_warp_kernel serves every d with a compile-time geometry (dispatch_warp);
 // ivfflat_scan_kernel, the generic one, any other d: one CTA per (query, probed list, list split).
-// The list's rows stream HBM -> shared memory through a 4-stage ring of TMA 1-D bulk copies
-// (cp.async.bulk + mbarrier complete_tx), so the copy engine keeps 4 x 16 KB in flight per CTA with
-// no register staging.  LPR lanes share one row (float4 chunks, rotated start so both the row and
+// The list's rows stream HBM -> shared memory through a ring of TMA 1-D bulk copies (cp.async.bulk +
+// mbarrier complete_tx), so the copy engine keeps up to 4 x 16 KB in flight per CTA with no register
+// staging.  The ring is 4 stages deep wherever the CTA's shared memory allows it; above d = 2436 at
+// k = 4096 it shrinks to 3 and then 2 stages (ivfflat_scan_stages), which serves every d up to
+// ivfflat_scan_max_dim().  LPR lanes share one row (float4 chunks, rotated start so both the row and
 // the query reads are bank-conflict-free), partial sums meet through warp shuffles, and candidates
 // that beat the running k-th best go to the CandQueue (common.cuh).  List ids are only read for
 // candidates that beat the threshold.
 //
 // Algorithmic bytes: (4*d + 8) per scanned entry (SURVEY.md 8d); roofline: HBM.
 #include <float.h>
+
+#include <algorithm>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -26,7 +30,9 @@ namespace gb {
 namespace {
 
 constexpr int IVF_NT = 128;
-constexpr int IVF_NST = 4;                 // pipeline stages
+constexpr int IVF_NST = 4;                 // pipeline stages: the deepest ring (ivfflat_scan_stages picks 4, 3 or 2)
+constexpr int IVF_MIN_NST = 2;
+constexpr size_t IVF_CTA_SMEM = 227 * 1024; // sm_90: shared memory of one CTA, static and dynamic
 constexpr int IVF_STAGE_BYTES = 16 * 1024; // target bytes per stage
 constexpr int IVF_CHUNK_ROWS = 8192;       // rows per CTA (long lists are split)
 
@@ -54,11 +60,11 @@ __host__ __device__ inline IvfGeom ivf_geom(int d) {
 template <int METRIC>
 __global__ void __launch_bounds__(IVF_NT)
     ivfflat_scan_kernel(const float* __restrict__ xq, int64_t ldq, int d, const int32_t* __restrict__ probe_ids,
-                        int nprobe, int nsplit, ListDirectory dir, IvfGeom g, int k, int KP, int SORTN, FilterArgs f,
-                        unsigned long long* __restrict__ partial) {
+                        int nprobe, int nsplit, ListDirectory dir, IvfGeom g, int nst, int k, int KP, int SORTN,
+                        FilterArgs f, unsigned long long* __restrict__ partial) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* stages = reinterpret_cast<float*>(smem_raw);
-  float* qs = reinterpret_cast<float*>(smem_raw + (size_t)IVF_NST * g.stage_bytes);
+  float* qs = reinterpret_cast<float*>(smem_raw + (size_t)nst * g.stage_bytes);
   unsigned long long* buf = reinterpret_cast<unsigned long long*>(qs + d);
   __shared__ __align__(8) uint64_t full_bar[IVF_NST];
   __shared__ int s_cnt;
@@ -85,7 +91,7 @@ __global__ void __launch_bounds__(IVF_NT)
   CandQueue cq{buf, &s_cnt, &s_tau, k, KP, SORTN};
   for (int i = tid; i < d; i += IVF_NT) qs[i] = xq[(int64_t)q * ldq + i];
   if (tid == 0) {
-    for (int s = 0; s < IVF_NST; s++) mbar_init(&full_bar[s], 1);
+    for (int s = 0; s < nst; s++) mbar_init(&full_bar[s], 1);
     mbar_fence_init();
   }
   cq.init();  // includes __syncthreads()
@@ -93,7 +99,7 @@ __global__ void __launch_bounds__(IVF_NT)
   const int ntiles = (r1 - r0 + g.T - 1) / g.T;
   const int row_bytes = d * 4;
   auto issue = [&](int t) {
-    int s = t % IVF_NST;
+    int s = t % nst;
     int rows = min(g.T, r1 - (r0 + t * g.T));
     uint32_t bytes = (uint32_t)rows * row_bytes;
     mbar_arrive_expect_tx(&full_bar[s], bytes);
@@ -101,15 +107,15 @@ __global__ void __launch_bounds__(IVF_NT)
              lvecs + (int64_t)(r0 + t * g.T) * d, bytes, &full_bar[s]);
   };
   if (tid == 0)
-    for (int t = 0; t < IVF_NST && t < ntiles; t++) issue(t);
+    for (int t = 0; t < nst && t < ntiles; t++) issue(t);
 
   const int grp = tid / g.LPR;      // row slot inside a round
   const int p = tid - grp * g.LPR;  // lane inside the row group
   const float4* qs4 = reinterpret_cast<const float4*>(qs);
 
   for (int t = 0; t < ntiles; t++) {
-    const int s = t % IVF_NST;
-    mbar_wait(&full_bar[s], (t / IVF_NST) & 1);
+    const int s = t % nst;
+    mbar_wait(&full_bar[s], (t / nst) & 1);
     const int tile_rows = min(g.T, r1 - (r0 + t * g.T));
     const unsigned long long tau = s_tau;
     const uint32_t tau_hi = (uint32_t)(tau >> 32);
@@ -159,7 +165,7 @@ __global__ void __launch_bounds__(IVF_NT)
     }
     __syncthreads();  // stage s fully consumed, all pushes of this tile done
     const int c_now = s_cnt;
-    if (tid == 0 && t + IVF_NST < ntiles) issue(t + IVF_NST);
+    if (tid == 0 && t + nst < ntiles) issue(t + nst);
     __syncthreads();  // everyone holds the same c_now before any warp pushes again
     if (t + 1 < ntiles && c_now + g.T > cq.cap()) cq.flush();
   }
@@ -170,6 +176,13 @@ __global__ void __launch_bounds__(IVF_NT)
 void ivf_cq_geometry(int k, int T, int* KP, int* SORTN) {
   *KP = next_pow2(k < 16 ? 16 : k);
   *SORTN = next_pow2(*KP + 2 * T);
+}
+
+// dynamic shared memory of ivfflat_scan_kernel with an nst-stage ring: the stages, the query, the candidate queue
+size_t ivf_scan_smem(const IvfGeom& g, int d, int k, int nst) {
+  int KP, SORTN;
+  ivf_cq_geometry(k, g.T, &KP, &SORTN);
+  return (size_t)nst * g.stage_bytes + (size_t)d * 4 + (size_t)SORTN * 8;
 }
 
 // ---- fixed-geometry kernel (dimensions with an instantiation) --------------------------------
@@ -432,7 +445,48 @@ cudaError_t dispatch_warp(int S, const float* xq, int64_t ldq, int nq, const int
   return cudaErrorNotSupported;
 }
 
+// ivfflat_scan_kernel's own __shared__ arrays (the mbarriers, the queue's radix histogram: 1152 B with CUDA 12.9), which
+// count against the same per-CTA limit as the dynamic window.  Read from the current device's image of the kernel; a
+// failure is returned (and cleared from the runtime's last error), never cached.
+cudaError_t ivf_static_smem(size_t* out) {
+  cudaFuncAttributes a, b;
+  cudaError_t e = cudaFuncGetAttributes(&a, ivfflat_scan_kernel<kMetricL2>);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&b, ivfflat_scan_kernel<kMetricIP>);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return e;
+  }
+  *out = std::max(a.sharedSizeBytes, b.sharedSizeBytes);
+  return cudaSuccess;
+}
+
+int stages_beside(size_t static_smem, int d, int k) {
+  if (d <= 0 || (d & 3) || k <= 0 || k > 4096) return 0;
+  const IvfGeom g = ivf_geom(d);
+  for (int nst = IVF_NST; nst >= IVF_MIN_NST; nst--)
+    if (ivf_scan_smem(g, d, k, nst) + static_smem <= IVF_CTA_SMEM) return nst;
+  return 0;
+}
+
 }  // namespace
+
+cudaError_t ivfflat_scan_stages(int d, int k, int* nst) {
+  size_t st = 0;
+  const cudaError_t e = ivf_static_smem(&st);
+  if (e != cudaSuccess) return e;
+  *nst = stages_beside(st, d, k);
+  return cudaSuccess;
+}
+
+cudaError_t ivfflat_scan_max_dim(int* max_d) {
+  size_t st = 0;
+  const cudaError_t e = ivf_static_smem(&st);
+  if (e != cudaSuccess) return e;
+  int d = 4;
+  while (stages_beside(st, d + 4, 4096) > 0) d += 4;
+  *max_d = d;
+  return cudaSuccess;
+}
 
 int ivfflat_scan_nparts(int nprobe, int max_list_len) {
   int nsplit = (max_list_len + IVF_CHUNK_ROWS - 1) / IVF_CHUNK_ROWS;
@@ -462,25 +516,20 @@ cudaError_t launch_ivfflat_scan(const float* xq, int64_t ldq, int nq, int d, con
     }
   }
   if (kernel_out) *kernel_out = "ivfflat_scan_kernel";
+  // the deepest ring that fits: 4 stages wherever they fit (every d <= 2436 at k = 4096), else 3 or 2
+  int nst = 0;
+  cudaError_t e = ivfflat_scan_stages(d, k, &nst);
+  if (e != cudaSuccess) return e;
+  if (nst == 0) return cudaErrorInvalidValue;  // d above ivfflat_scan_max_dim(), which create_index refuses
   int KP, SORTN;
   ivf_cq_geometry(k, g.T, &KP, &SORTN);
-  size_t smem = (size_t)IVF_NST * g.stage_bytes + (size_t)d * 4 + (size_t)SORTN * 8;
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;
+  const size_t smem = ivf_scan_smem(g, d, k, nst);
   dim3 grid(nparts, nq);
-  cudaError_t e;
-  if (metric == kMetricL2) {
-    e = cudaFuncSetAttribute(ivfflat_scan_kernel<kMetricL2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    ivfflat_scan_kernel<kMetricL2><<<grid, IVF_NT, smem, st>>>(xq, ldq, d, probe_ids, nprobe, nsplit, dir, g, k, KP,
-                                                               SORTN, f, partial);
-                                                               note_launch();
-  } else {
-    e = cudaFuncSetAttribute(ivfflat_scan_kernel<kMetricIP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    ivfflat_scan_kernel<kMetricIP><<<grid, IVF_NT, smem, st>>>(xq, ldq, d, probe_ids, nprobe, nsplit, dir, g, k, KP,
-                                                               SORTN, f, partial);
-                                                               note_launch();
-  }
+  auto kern = metric == kMetricL2 ? ivfflat_scan_kernel<kMetricL2> : ivfflat_scan_kernel<kMetricIP>;
+  e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  kern<<<grid, IVF_NT, smem, st>>>(xq, ldq, d, probe_ids, nprobe, nsplit, dir, g, nst, k, KP, SORTN, f, partial);
+  note_launch();
   return cudaGetLastError();
 }
 

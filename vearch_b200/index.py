@@ -651,6 +651,14 @@ def merge_partition_keys_device(keys, metric):
     return od, oi
 
 
+def pool_usage(reset_peak=False, device=0):
+    """(bytes in use, high-water mark) of the device's default memory pool, where search scratch is allocated, after
+    the device's pending work; reset_peak=True then restarts the mark at the current use."""
+    used, peak = C.c_int64(), C.c_int64()
+    _check(_lib.lib().gb_device_pool_usage(device, int(reset_peak), C.byref(used), C.byref(peak)), "pool_usage")
+    return used.value, peak.value
+
+
 def debug_dist_matrix(x, c, metric, use_tc, device=0):
     """score matrix through the exact CUDA-core kernel (use_tc=0) or the wgmma 3xTF32 kernel (use_tc=1)."""
     x, c = _f32(x), _f32(c)
