@@ -35,7 +35,10 @@ struct CStatus {
 };
 
 /* gamma_api.cc:35-70.  config JSON: {"path": ..., "space_name": ..., "log_dir": ...,
- * optional "device": GPU ordinal (default 0; partitions map to GPUs, SURVEY.md 8e)}.
+ * optional "device": GPU ordinal (default 0; partitions map to GPUs, SURVEY.md 8e),
+ * optional "devices": GPU ordinals [0, 1, ...] or "all": GPU_IVFPQ / GPU_IVFFLAT fields are sharded over them and
+ * devices[0] replaces "device"; an ordinal outside the visible devices makes Init return NULL}.
+ * The environment variables GAMMA_B200_DEVICE and GAMMA_B200_DEVICES ("0,1,2,3" or "all") override the two keys.
  * Returns NULL on failure (gammacb/gamma.go:84-88). */
 void *Init(const char *config_str, int len);
 /* gamma_api.cc:137-141 */

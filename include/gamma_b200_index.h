@@ -38,6 +38,15 @@ long long gb_launch_count(void);
  * nbits_per_idx (IVFPQ: 1..8), training_threshold, bucket_init_size, bucket_max_size, store_type ("RocksDB", any
  * case: raw vectors in pinned host memory; anything else: in HBM) (may be NULL/""). */
 gb_index *gb_index_create(const char *index_type, int dimension, const char *model_params_json, int device);
+/* A GPU_IVFPQ or GPU_IVFFLAT index sharded over devices[0..ndevices) (an ordinal may repeat): global vid v is held by
+ * shard v % ndevices, on devices[v % ndevices]; the raw vectors, training, brute force and the cross-shard merge stay on
+ * devices[0].  One device, or any other type: gb_index_create on devices[0]. */
+gb_index *gb_index_create_sharded(const char *index_type, int dimension, const char *model_params_json,
+                                  const int *devices, int ndevices);
+/* shards of the index (1 unless sharded), and a handle on shard i's index structures (its lists, centroids, codebook
+ * and tables; its own raw store is empty), valid while the index lives: gb_index_destroy frees only the handle */
+int gb_index_shard_count(gb_index *index);
+gb_index *gb_index_shard(gb_index *index, int shard);
 void gb_index_destroy(gb_index *index);
 /* the registered type name the index was created under (Index::type) */
 const char *gb_index_type(gb_index *index);

@@ -33,6 +33,11 @@ def _declare(l):
     l.gb_launch_count.restype = C.c_longlong
     l.gb_index_create.restype = vp
     l.gb_index_create.argtypes = [cstr, i32, cstr, i32]
+    l.gb_index_create_sharded.restype = vp
+    l.gb_index_create_sharded.argtypes = [cstr, i32, cstr, C.POINTER(i32), i32]
+    l.gb_index_shard_count.argtypes = [vp]
+    l.gb_index_shard.restype = vp
+    l.gb_index_shard.argtypes = [vp, i32]
     l.gb_index_destroy.restype = None
     l.gb_index_destroy.argtypes = [vp]
     l.gb_index_add_vectors.argtypes = [vp, i64, vp]

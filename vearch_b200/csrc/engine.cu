@@ -214,8 +214,23 @@ struct AdmissionGuard {  // every return path of Engine::Search releases what it
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------
-Engine::Engine(const std::string& path, const std::string& space_name, int device)
-    : path_(path), space_name_(space_name), device_(device) {}
+Engine::Engine(const std::string& path, const std::string& space_name, int device, const std::vector<int>& devices)
+    : path_(path), space_name_(space_name), device_(devices.empty() ? device : devices[0]), devices_(devices) {}
+
+// the GPU types shard over a device list of two entries or more (IndexShards); everything else lives on device_
+Index* Engine::make_index(const std::string& type, int dim, const ModelParams& mp) const {
+  if (devices_.size() > 1 && is_gpu_index_type(type)) return create_sharded_index(type, dim, mp, devices_, 20);
+  return create_index(type, dim, mp, device_, 20);
+}
+
+namespace {
+// the trained state a Dump writes beside the rows and a Load restores: the IVF index, or a sharded index's first shard
+// (every shard holds the same; ShardedIndex::train copies shard 0's to the others)
+IvfIndex* trained_state_of(Index* ix) {
+  if (ShardedIndex* sh = dynamic_cast<ShardedIndex*>(ix)) return sh->shard(0);
+  return dynamic_cast<IvfIndex*>(ix);
+}
+}  // namespace
 
 namespace {
 struct LiveEngines {
@@ -321,7 +336,7 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
   // than one vector field cannot join Hamming and float scores here
   if (index_type_ == "BINARYIVF" && nvec > 1)
     return Status::Make(kNotSupported, vec_name_ + ": BINARYIVF is not supported in a multi-vector table");
-  Index* idx = create_index(index_type_, dim_, mp, device_, 20);
+  Index* idx = make_index(index_type_, dim_, mp);
   if (!idx) return Status::Make(index_type_ == "FLAT" || index_type_ == "IVFFLAT" || index_type_ == "IVFPQ" ||
                                         index_type_ == "IVFPQFastScan" || index_type_ == "BINARYIVF" ||
                                         index_type_ == "IVFRABITQ" || index_type_ == "VEARCH" || is_gpu_index_type(index_type_)
@@ -352,7 +367,7 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     emp.host_store = !strcasecmp(ev.str(4).c_str(), "RocksDB");
     if (vf.index_type == "BINARYIVF")
       return Status::Make(kNotSupported, vf.name + ": BINARYIVF is not supported in a multi-vector table");
-    Index* eidx = create_index(vf.index_type, vf.dim, emp, device_, 20);
+    Index* eidx = make_index(vf.index_type, vf.dim, emp);
     if (!eidx) return Status::Make(kInvalidArgument, last_error());
     vf.index.reset(eidx);
     extra_.push_back(std::move(vf));
@@ -1346,8 +1361,8 @@ int Engine::Dump() {
   int trained = index_->trained() ? 1 : 0;
   wr<int32_t>(f, trained);
   // an index whose trained state does not persist (IVFPQFastScan) is trained again by Load
-  IvfIndex* ivf = index_->persists_trained_state() ? dynamic_cast<IvfIndex*>(index_.get()) : nullptr;
-  IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(index_.get());
+  IvfIndex* ivf = index_->persists_trained_state() ? trained_state_of(index_.get()) : nullptr;
+  IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(ivf);
   if (trained && ivf) {
     std::vector<float> c((size_t)ivf->nlist() * dim_);
     if (ivf->get_centroids(c.data())) return -1;
@@ -1361,7 +1376,7 @@ int Engine::Dump() {
   f.close();
   // the index itself in gamma's own format (IndexModel::Dump via VectorManager::Dump,
   // vector_manager.cc:1155-1170): <dir>/<vector name>.000/{ivfflat,ivfpq}.index
-  if (trained && ivf && ivf->dump_gamma(dir, vec_name_ + ".000")) return -1;
+  if (trained && ivf && index_->dump_gamma(dir, vec_name_ + ".000")) return -1;
   for (auto& e : extra_) {  // the other vector fields: raw rows next to the table, index in gamma's format
     std::ofstream ef(dir + "/" + table_name_ + "." + e.name + ".gbvec", std::ios::binary | std::ios::trunc);
     std::vector<float> erows((size_t)max_docid_ * e.dim);
@@ -1370,8 +1385,7 @@ int Engine::Dump() {
     wr<int32_t>(ef, e.dim);
     ef.write(reinterpret_cast<const char*>(erows.data()), (std::streamsize)(erows.size() * 4));
     if (ef.fail()) return -1;
-    IvfIndex* eivf = dynamic_cast<IvfIndex*>(e.index.get());
-    if (eivf && eivf->trained() && eivf->dump_gamma(dir, e.name + ".000")) return -1;
+    if (e.index->trained() && e.index->dump_gamma(dir, e.name + ".000")) return -1;
   }
   std::ofstream done(dir + "/dump.done");
   done << "ok";
@@ -1428,12 +1442,11 @@ int Engine::Load() {
     std::vector<float> erows((size_t)maxd * e.dim);
     if (maxd && !ef.read(reinterpret_cast<char*>(erows.data()), (std::streamsize)(erows.size() * 4))) return -1;
     if (maxd && e.index->add_vectors(erows.data(), maxd)) return -1;
-    IvfIndex* eivf = dynamic_cast<IvfIndex*>(e.index.get());
     int64_t eload = 0;
-    if (eivf) eivf->load_gamma(dir, e.name + ".000", &eload);  // trained state + lists; absent: trained again later
+    e.index->load_gamma(dir, e.name + ".000", &eload);  // trained state + lists; absent: trained again later
   }
-  IvfIndex* ivf = index_->persists_trained_state() ? dynamic_cast<IvfIndex*>(index_.get()) : nullptr;
-  IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(index_.get());
+  IvfIndex* ivf = index_->persists_trained_state() ? trained_state_of(index_.get()) : nullptr;
+  IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(ivf);
   if (trained && ivf) {
     std::vector<float> c((size_t)ivf->nlist() * dim_);
     if (!f.read(reinterpret_cast<char*>(c.data()), (std::streamsize)(c.size() * 4))) return -1;
@@ -1448,7 +1461,7 @@ int Engine::Load() {
     // IndexModel::Load: take the inverted lists from the index file when it matches this table; a
     // missing or refused file only means the indexing thread re-adds the vectors itself
     int64_t load_num = 0;
-    if (ivf->load_gamma(dir, vec_name_ + ".000", &load_num) == 0 && load_num > 0) index_status_.store(2);
+    if (index_->load_gamma(dir, vec_name_ + ".000", &load_num) == 0 && load_num > 0) index_status_.store(2);
   }
   lk.unlock();
   if (trained) BuildIndex();  // train() is a no-op on a trained index; the loop adds what the file did not cover

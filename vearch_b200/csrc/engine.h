@@ -108,7 +108,9 @@ struct QueryRequestPB {  // vearchpb.QueryRequest (router_grpc.proto:147-166), c
 
 class Engine {
  public:
-  Engine(const std::string& path, const std::string& space_name, int device);
+  // devices: Init's "devices" (empty: one device); a GPU_IVFPQ / GPU_IVFFLAT field is sharded over two or more, every
+  // other index lives on device, which is devices[0] when they are given
+  Engine(const std::string& path, const std::string& space_name, int device, const std::vector<int>& devices = {});
   ~Engine();
 
   Status CreateTable(const uint8_t* fb, size_t len);
@@ -145,6 +147,8 @@ class Engine {
 
   std::string path_, space_name_;
   int device_;
+  std::vector<int> devices_;
+  Index* make_index(const std::string& type, int dim, const ModelParams& mp) const;
   bool created_table_ = false;
 
   // table (table/table.{h,cc} reduced to an in-memory column store)

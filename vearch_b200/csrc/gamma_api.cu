@@ -6,6 +6,7 @@
 
 #include <atomic>
 #include <string>
+#include <vector>
 
 #include "../../include/gamma_api.h"
 #include "engine.h"
@@ -33,6 +34,46 @@ static void out_buffer(const std::string& s, char** out, int* len) {
 
 static std::atomic<int> g_log_dir_flag{0};
 
+// Init's device list: a JSON array of ordinals or "all", or the environment's "0,1,2,3" / "all" in its place.  false:
+// malformed, empty, or an ordinal outside [0, ndev)
+static bool parse_devices(const gb::JsonValue* jv, const char* env, int ndev, std::vector<int>* out) {
+  out->clear();
+  std::string all;
+  if (env) {
+    all = env;
+    if (all != "all") {
+      size_t at = 0;
+      for (;;) {  // every comma-separated token an integer: "0,", ",1" and "0,,1" are malformed
+        const size_t comma = all.find(',', at);
+        const std::string tok = all.substr(at, comma == std::string::npos ? std::string::npos : comma - at);
+        char* end = nullptr;
+        const long v = strtol(tok.c_str(), &end, 10);
+        if (tok.empty() || *end) return false;
+        out->push_back((int)v);
+        if (comma == std::string::npos) break;
+        at = comma + 1;
+      }
+    }
+  } else if (jv) {
+    if (jv->type == gb::JsonValue::String) {
+      if (jv->str != "all") return false;
+      all = "all";
+    } else if (jv->type == gb::JsonValue::Array && !jv->arr.empty()) {
+      for (const gb::JsonValue& v : jv->arr) {
+        if (v.type != gb::JsonValue::Number || v.num != (double)(int)v.num) return false;
+        out->push_back((int)v.num);
+      }
+    } else {
+      return false;
+    }
+  }
+  if (all == "all")
+    for (int d = 0; d < ndev; d++) out->push_back(d);
+  for (int d : *out)
+    if (d < 0 || d >= ndev) return false;
+  return true;
+}
+
 extern "C" {
 
 void* Init(const char* config_str, int len) {
@@ -51,7 +92,13 @@ void* Init(const char* config_str, int len) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return nullptr;  // no CPU path
   if (device < 0 || device >= ndev) device = ((device % ndev) + ndev) % ndev;
-  return static_cast<void*>(new Engine(path, space, device));
+  // "devices": the GPU_IVFPQ / GPU_IVFFLAT fields shard over them (IndexShards), devices[0] is the partition's device;
+  // GAMMA_B200_DEVICES ("0,1,2,3" or "all") overrides it as GAMMA_B200_DEVICE overrides "device"
+  std::vector<int> devices;
+  const char* env_devices = getenv("GAMMA_B200_DEVICES");
+  if (env_devices && !*env_devices) env_devices = nullptr;  // set but empty: as if unset
+  if (!parse_devices(j.get("devices"), env_devices, ndev, &devices)) return nullptr;
+  return static_cast<void*>(new Engine(path, space, device, devices));
 }
 
 int Close(void* engine) {

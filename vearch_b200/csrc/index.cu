@@ -1449,12 +1449,13 @@ int IvfIndex::get_centroids(float* host) const {
 }
 
 // GammaIVFFlatIndex::Indexing (gamma_index_ivfflat.cc:342-411): train on the FIRST num vectors.
-int IvfIndex::train() {
+int IvfIndex::train() { return train_on(*store_); }
+int IvfIndex::train_on(RawStore& src) {
   std::lock_guard<std::mutex> bg(build_mu_);
   if (trained_) return 0;
   cudaSetDevice(device_);
   int64_t num = training_threshold();
-  if (num > store_->size()) {
+  if (num > src.size()) {
     set_last_error("vector total count less than training_threshold");
     return -1;
   }
@@ -1462,7 +1463,7 @@ int IvfIndex::train() {
   drain_searches();
   cudaStream_t st = build_stream_;
   Scratch s(st);
-  const float* xt = store_->contiguous(num, s);
+  const float* xt = src.contiguous(num, s);
   if (!xt) return -1;
   xt = train_transform(xt, num, s);  // OPQ: learn the rotation, continue on the rotated slab
   if (!xt) return -1;
@@ -1516,14 +1517,14 @@ int IvfIndex::index_batch(const void* x, int64_t n, int64_t vid0, const uint8_t*
   const std::vector<int>& lens = lists_->lens();
   if ((int64_t)vid2pos_.size() < vid0 + n) vid2pos_.resize(vid0 + n, ~(uint64_t)0);
   for (int64_t i = 0; i < n; i++) {
-    int64_t vid = vid0 + i;
+    int64_t vid = vid0 + i, gvid = global_vid(vid);
     int l = h_list[i];
-    if (del_bitmap && ((del_bitmap[vid >> 3] >> (vid & 7)) & 1)) {  // ivfflat.cc:436: deleted before indexing
+    if (del_bitmap && ((del_bitmap[gvid >> 3] >> (gvid & 7)) & 1)) {  // ivfflat.cc:436: deleted before indexing
       h_list[i] = -1;
       h_pos[i] = 0;
       continue;
     }
-    if (l < 0 || l >= nlist_) l = (int)(vid % nlist_);  // ivfflat.cc:443-446
+    if (l < 0 || l >= nlist_) l = (int)(gvid % nlist_);  // ivfflat.cc:443-446
     h_list[i] = l;
     h_pos[i] = lens[l] + add[l]++;  // insertion (vid) order inside the list
     vid2pos_[vid] = ((uint64_t)l << 32) | (uint32_t)h_pos[i];
@@ -1589,6 +1590,19 @@ int IvfIndex::reset_index() {
   return 0;
 }
 
+void IvfIndex::clear_lists() {
+  std::lock_guard<std::mutex> bg(build_mu_);
+  cudaSetDevice(device_);
+  std::unique_lock<std::shared_mutex> lk(mu_);
+  drain_searches();
+  if (lists_) lists_.reset(new IvfLists(nlist_, code_bytes()));
+  vid2pos_.clear();
+  del_counted_.clear();
+  indexed_count_ = 0;
+  if (lists_) lists_changed(build_stream_);
+  cudaStreamSynchronize(build_stream_);
+}
+
 void IVFFlatIndex::reset_codec() {
   std::unique_lock<std::shared_mutex> ml(mirror_rw_);
   mirror_.lens.clear();
@@ -1611,7 +1625,7 @@ int IvfIndex::compact_locked() {
 // a per-vid row-pointer table, so an IVF-Flat search never reads host memory.  Rebuilt whole after every change of the
 // lists (growth and compaction move them), with mu_ held exclusively and earlier searches drained.
 int IVFFlatIndex::lists_changed(cudaStream_t st) {
-  if (!store_->on_host() || !lists_) return 0;
+  if (!rescore_from_lists() || !lists_) return 0;
   drain_searches();  // no kernel of an earlier search reads the table while it is rewritten or freed
   const int64_t need = (int64_t)vid2pos_.size();
   if (need > rowptr_cap_) {
@@ -1642,6 +1656,12 @@ int IvfIndex::update_vector(int64_t vid, const void* x) {
   std::lock_guard<std::mutex> bg(build_mu_);
   if (Index::update_vector(vid, x)) return -1;
   if (!trained_ || vid >= indexed_count_) return 0;  // not indexed yet: the add path will pick it up
+  Scratch s(build_stream_);
+  const void* x_dev = store_rows_dev(vid, 1, s);
+  if (!x_dev) return -1;
+  return reindex_vector(vid, x_dev);
+}
+int IvfIndex::reindex_vector(int64_t vid, const void* x_dev) {
   if (vid < (int64_t)vid2pos_.size() && vid2pos_[vid] != ~(uint64_t)0) {
     std::unique_lock<std::shared_mutex> lk(mu_);
     const int l = (int)(vid2pos_[vid] >> 32);
@@ -1651,9 +1671,6 @@ int IvfIndex::update_vector(int64_t vid, const void* x) {
     }
     if (lists_->tombstone(l, (int)(uint32_t)vid2pos_[vid], build_stream_)) return -1;
   }
-  Scratch s(build_stream_);
-  const void* x_dev = store_rows_dev(vid, 1, s);
-  if (!x_dev) return -1;
   return index_batch(x_dev, 1, vid, nullptr);
 }
 
@@ -1677,32 +1694,39 @@ int IvfIndex::dead_counts(int* out) {
   return 0;
 }
 
+std::vector<int> IvfIndex::purge_candidates(float threshold) const {
+  std::vector<int> sel;
+  if (!lists_) return sel;
+  for (int l = 0; l < nlist_; l++) {
+    const int dead = lists_->dead_counts()[l], len = lists_->lens()[l];
+    if (dead > 0 && len > 0 && (float)dead / (float)len >= threshold) sel.push_back(l);  // Compactable (realtime_mem_data.cc:366-370)
+  }
+  return sel;
+}
+
 int IvfIndex::purge_lists(float threshold, const uint8_t* del_bitmap, int64_t bitmap_bytes, int64_t* dropped) {
   if (dropped) *dropped = 0;
   std::lock_guard<std::mutex> bg(build_mu_);
-  if (!lists_) return 0;
-  std::vector<int> sel;
-  std::vector<char> purged(nlist_, 0);
-  for (int l = 0; l < nlist_; l++) {
-    const int dead = lists_->dead_counts()[l], len = lists_->lens()[l];
-    if (dead > 0 && len > 0 && (float)dead / (float)len >= threshold) {  // Compactable (realtime_mem_data.cc:366-370)
-      sel.push_back(l);
-      purged[l] = 1;
-    }
-  }
+  const std::vector<int> sel = purge_candidates(threshold);
   if (sel.empty()) return 0;
   cudaSetDevice(device_);
-  cudaStream_t st = build_stream_;
-  Scratch s(st);
+  Scratch s(build_stream_);
   std::unique_lock<std::shared_mutex> lk(mu_);
   SearchContext ctx;
   ctx.del_bitmap = del_bitmap;
   ctx.bitmap_bits = del_bitmap ? bitmap_bytes * 8 : 0;
   FilterArgs f;
   if (upload_bitmaps(ctx, &f, s)) return -1;
+  return purge_locked(sel, f.del_bits, dropped);
+}
+
+int IvfIndex::purge_locked(const std::vector<int>& sel, const uint32_t* d_del_bits, int64_t* dropped) {
+  cudaStream_t st = build_stream_;
+  std::vector<char> purged(nlist_, 0);
+  for (int l : sel) purged[l] = 1;
   drain_searches();  // kernels of earlier searches read lengths and base pointers at run time
   IvfLists::Purged pg;
-  if (lists_->purge(sel, f.del_bits, st, &pg)) return -1;
+  if (lists_->purge(sel, d_del_bits, st, &pg)) return -1;
   if (pg.dropped == 0) return 0;
   // vid_bucket_no_pos_ of every vid that was in a purged list, from the table the scatter wrote
   const int64_t hi = std::min<int64_t>((int64_t)vid2pos_.size(), pg.vid_min + (int64_t)pg.newpos.size());
@@ -2005,7 +2029,7 @@ int IVFFlatIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int me
   if (lm < 0) return lm;
   if (lm == 0) {
     if ((dpad_ & 3) == 0 && k <= 8192) {
-      if (store_->on_host()) {  // the list rows, through the row-pointer table (lists_changed)
+      if (rescore_from_lists()) {  // the list rows, through the row-pointer table (lists_changed)
         if (!d_rowptr_) {
           set_last_error("IVFFLAT: the row-pointer table of the host store was not built");
           return -1;

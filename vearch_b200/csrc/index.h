@@ -306,6 +306,13 @@ class Index {
   // VectorManager::ReCreateVectorIndexes, search/engine.cc:991-1089): the next train() starts over
   virtual int reset_index() { return 0; }
   virtual int64_t index_mem_bytes() const { return 0; }
+  // gamma's own index file of the type (IvfIndex::dump_gamma / load_gamma); the types without one write and read nothing
+  virtual int dump_gamma(const std::string& dir, const std::string& abs_name) { (void)dir; (void)abs_name; return 0; }
+  virtual int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) {
+    (void)dir; (void)abs_name;
+    *load_num = 0;
+    return 0;
+  }
   // stop the background worker (request coalescer); also run from an atexit hook for objects the host
   // never closed, so no thread of ours is inside the CUDA runtime while it is being torn down
   void quiesce();
@@ -516,10 +523,35 @@ class IvfIndex : public Index {
   int compact_lists();
   // gamma's own index files (index_io.cu): <dir>/<abs_name>/<gamma_format().file>.  load: the vector
   // store must already hold the vectors the file indexes; *load_num = IndexModel::Load's load_num
-  int dump_gamma(const std::string& dir, const std::string& abs_name);
-  int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num);
+  int dump_gamma(const std::string& dir, const std::string& abs_name) override;
+  int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) override;
 
  protected:
+  friend class ShardedIndex;
+  // One shard of a ShardedIndex holds the global vids v with v % shard_count_ == shard_id_ as local vid v / shard_count_;
+  // the deletion bitmap of add_pending and the list fallback of a row without a nearest list take the global vid
+  int64_t shard_count_ = 1, shard_id_ = 0;
+  int64_t global_vid(int64_t local) const { return local * shard_count_ + shard_id_; }
+  // train() on the first training_threshold() rows of `src` (a sharded index trains its first shard on its own store)
+  int train_on(RawStore& src);
+  // Update's list part: tombstone vid's entry, append the row x_dev (device, store().stride() bytes) to its new list;
+  // build_mu_ held
+  int reindex_vector(int64_t vid, const void* x_dev);
+  // empty lists, the trained state kept (a sharded Load that failed part way)
+  void clear_lists();
+  // the lists whose counted dead share is at least threshold, and their purge with the device bitmap d_del_bits (by
+  // vid, nullable), ordered on build_stream_; build_mu_ and mu_ held exclusively
+  std::vector<int> purge_candidates(float threshold) const;
+  int purge_locked(const std::vector<int>& sel, const uint32_t* d_del_bits, int64_t* dropped);
+  // the gamma index file with this index's header and trained state, `lens` and the list contents `fetch` gives
+  // (codes of code_bytes() bytes and ids per list); build_mu_ held
+  int write_gamma(const std::string& dir, const std::string& abs_name, int64_t indexed, const std::vector<int>& lens,
+                  const std::function<int(int, std::vector<uint8_t>*, std::vector<int64_t>*)>& fetch);
+  // load_gamma keeping only the file's entries of this shard (global vid % shard_count_ == shard_id_, as local vids);
+  // store_rows: the rows of the (global) vector store; *file_indexed = the file's indexed count (IvFl) or this shard's
+  // live entries (IwPQ)
+  int load_gamma_part(const std::string& dir, const std::string& abs_name, int64_t store_rows, int64_t* load_num,
+                      int64_t* file_indexed);
   virtual GammaFileFormat gamma_format() const = 0;
   // codec blocks after the coarse quantiser (product quantizer, OPQ)
   virtual int dump_gamma_extra(FILE* f) { (void)f; return 0; }
@@ -626,7 +658,9 @@ class IVFFlatIndex : public IvfIndex {
   // The list shifts s_l [nlist][dpad] of the list-major scan of an L2 index (nullptr under IP) (launch_list_shifts): its tensor-core operands are
   // x - s_l and y - s_l, so the rounding of the expanded form scales with the residual norms, not the raw ones.
   float* d_shifts_ = nullptr;
-  // host placement: rowptr[vid] = the list row holding vid, for the winner re-score (lists_changed)
+  // host placement, and every shard of a ShardedIndex (whose raw rows live with the sharded index): rowptr[vid] = the
+  // list row holding vid, for the winner re-score (lists_changed)
+  bool rescore_from_lists() const { return store_->on_host() || shard_count_ > 1; }
   const float** d_rowptr_ = nullptr;
   int64_t rowptr_cap_ = 0;
 
@@ -911,8 +945,65 @@ class VearchIndex : public IvfIndex {
 // host rows n x d (stride d) -> device rows n x dpad, the padding columns zeroed
 cudaError_t upload_rows_padded(float* dst, const float* src, int64_t n, int d, int dpad, cudaStream_t st);
 
+// gamma's GPU types over several devices (faiss::IndexShards, gamma_index_ivfpq_gpu.cc:269-298,
+// gamma_index_ivfflat_gpu.cc:140-173): S shards of one IVF type, shard s on devices[s], holding the global vids
+// v % S == s as local vids v / S (so a shard's (score, local vid) order is the (score, global vid) order).  The raw
+// vectors stay in this index's store on devices[0], the primary device; shards hold only index structures.  Training
+// runs once, on the primary device, and its state is copied to every shard.  A search runs the request checks, the
+// coalescer, brute force and the realtime tail here, each shard's coarse search and scan on its own device and stream
+// (bitmaps cut per shard on the device), and merges the S sorted key rows of every query on the primary device
+// (index_shards.cu, DESIGN.md §7).
+class ShardedIndex : public Index {
+ public:
+  ShardedIndex(const std::string& type, int d, const ModelParams& mp, const std::vector<int>& devices, int seg_shift,
+               std::vector<std::unique_ptr<IvfIndex>> shards);
+  ~ShardedIndex() override;
+  int nshards() const { return (int)shards_.size(); }
+  IvfIndex* shard(int s) { return shards_[s].get(); }
+  int training_threshold() const override { return shards_[0]->training_threshold(); }
+  int train() override;
+  int add_pending(const uint8_t* del_bitmap) override;
+  int update_vector(int64_t vid, const void* x) override;
+  int delete_vectors(const int64_t* vids, int64_t n) override;
+  int purge_lists(float threshold, const uint8_t* del_bitmap, int64_t bitmap_bytes, int64_t* dropped) override;
+  int reset_index() override;
+  int64_t index_mem_bytes() const override;
+  // the unsharded type's file: list l is the merge of the shards' lists l by global vid, ids written as global vids
+  int dump_gamma(const std::string& dir, const std::string& abs_name) override;
+  // every shard reads the file and keeps its own entries
+  int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) override;
+
+ protected:
+  int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, int k,
+                      unsigned long long* out_keys, Scratch& s) override;
+
+ private:
+  // shard 0's trained state (centroids, OPQ, PQ codebook and with it the precomputed table) to every other shard
+  int sync_trained_state();
+  // f's bitmaps (covering `bits` vids) cut into S per-shard bitmaps of shard_words(bits) words each, in s
+  int64_t shard_words(int64_t bits) const;
+  int split_bitmap(const uint32_t* src, int64_t bits, uint32_t** out, Scratch& s);
+  // a stream per shard and their events, for one search at a time; pooled
+  struct ShardLane {
+    cudaEvent_t start = nullptr;        // primary device: queries and bitmaps are ready
+    std::vector<cudaStream_t> st;       // shard s's device
+    std::vector<cudaEvent_t> done;      // shard s's keys are on the primary device
+  };
+  ShardLane* shard_lane_acquire();
+  void shard_lane_release(ShardLane* l);
+  void shard_lane_free(ShardLane* l);
+  std::vector<int> devices_;
+  std::vector<std::unique_ptr<IvfIndex>> shards_;
+  cudaEvent_t build_ev_ = nullptr;  // primary device: rows staged for a shard on build_stream_
+  std::mutex shard_lane_mu_;
+  std::vector<ShardLane*> shard_lanes_, free_shard_lanes_;
+};
+
 // reflector (index/reflector.h:68-80): type name -> index object
 Index* create_index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift);
+// a GPU_IVFPQ / GPU_IVFFLAT index sharded over `devices` (at least two entries; an entry may repeat)
+Index* create_sharded_index(const std::string& type, int d, const ModelParams& mp, const std::vector<int>& devices,
+                            int seg_shift);
 
 // cross-partition merge (router semantics, internal/client/client.go:1530-1609) on device:
 // in: nparts x nq x k (dis, ids) sorted per partition; out: nq x k, ids = (part << 32) | local id

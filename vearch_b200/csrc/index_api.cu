@@ -14,6 +14,7 @@ using namespace gb;
 
 struct gb_index {
   Index* impl;
+  bool view = false;  // a shard of a sharded index (gb_index_shard): destroying the handle leaves the index alone
 };
 
 namespace gb {
@@ -231,6 +232,26 @@ static bool packed_binary(gb_index* index) {
   return true;
 }
 
+// A shard handle (gb_index_shard) reads a shard's structures; changing them goes through the sharded index, which keeps
+// the shards consistent with each other and with its raw store
+static bool shard_view(gb_index* index) {
+  if (!index || !index->view) return false;
+  set_last_error("a shard handle is read-only: change the sharded index instead");
+  return true;
+}
+
+// the IVF index whose trained state (centroids, codebook, tables, coarse quantiser) a handle answers for: the index, or
+// a sharded index's first shard (every shard holds the same state)
+template <class T>
+static T* state_of(gb_index* index) {
+  if (ShardedIndex* sh = index && index->impl ? dynamic_cast<ShardedIndex*>(index->impl) : nullptr)
+    return dynamic_cast<T*>(sh->shard(0));
+  return as<T>(index);
+}
+static ShardedIndex* sharded(gb_index* index) {
+  return index && index->impl ? dynamic_cast<ShardedIndex*>(index->impl) : nullptr;
+}
+
 extern "C" {
 
 const char* gb_last_error(void) { return last_error(); }
@@ -257,11 +278,51 @@ gb_index* gb_index_create(const char* index_type, int dimension, const char* mod
   return h;
 }
 
+gb_index* gb_index_create_sharded(const char* index_type, int dimension, const char* model_params_json, const int* devices,
+                                  int ndevices) {
+  if (!devices || ndevices < 1) {
+    set_last_error("gb_index_create_sharded: at least one device");
+    return nullptr;
+  }
+  const std::string type = index_type ? index_type : "";
+  // one device, or a type that is not sharded: the index lives on the first device, as gb_index_create places it
+  if (ndevices == 1 || !is_gpu_index_type(type)) return gb_index_create(index_type, dimension, model_params_json, devices[0]);
+  ModelParams mp;
+  std::string err;
+  if (!parse_model_params(model_params_json ? model_params_json : "", type, &mp, &err)) {
+    set_last_error(err);
+    return nullptr;
+  }
+  Index* impl = create_sharded_index(type, dimension, mp, std::vector<int>(devices, devices + ndevices), 20);
+  if (!impl) return nullptr;
+  gb_index* h = new gb_index;
+  h->impl = impl;
+  return h;
+}
+
+int gb_index_shard_count(gb_index* index) {
+  if (!index || !index->impl) return 0;
+  ShardedIndex* sh = dynamic_cast<ShardedIndex*>(index->impl);
+  return sh ? sh->nshards() : 1;
+}
+
+gb_index* gb_index_shard(gb_index* index, int shard) {
+  ShardedIndex* sh = index && index->impl ? dynamic_cast<ShardedIndex*>(index->impl) : nullptr;
+  if (!sh || shard < 0 || shard >= sh->nshards()) {
+    set_last_error("gb_index_shard: not a sharded index, or no such shard");
+    return nullptr;
+  }
+  gb_index* h = new gb_index;
+  h->impl = sh->shard(shard);
+  h->view = true;
+  return h;
+}
+
 const char* gb_index_type(gb_index* index) { return index && index->impl ? index->impl->type().c_str() : ""; }
 
 void gb_index_destroy(gb_index* index) {
   if (!index) return;
-  if (index->impl) {
+  if (index->impl && !index->view) {
     cudaSetDevice(index->impl->device());
     delete index->impl;
   }
@@ -269,16 +330,19 @@ void gb_index_destroy(gb_index* index) {
 }
 
 int gb_index_add_vectors(gb_index* index, int64_t n, const float* x) {
+  if (shard_view(index)) return -1;
   IDX_OR_FAIL(index);
   if (packed_binary(index)) return -1;
   return index->impl->add_vectors(x, n);
 }
 int gb_index_add_vectors_device(gb_index* index, int64_t n, const float* x_dev, int64_t ld) {
+  if (shard_view(index)) return -1;
   IDX_OR_FAIL(index);
   if (packed_binary(index)) return -1;
   return index->impl->add_vectors_device(x_dev, ld, n);
 }
 int gb_index_update_vector(gb_index* index, int64_t vid, const float* x) {
+  if (shard_view(index)) return -1;
   IDX_OR_FAIL(index);
   if (packed_binary(index)) return -1;
   cudaSetDevice(index->impl->device());
@@ -297,10 +361,12 @@ int gb_index_get_vectors(gb_index* index, int64_t start, int64_t n, float* out) 
   return index->impl->store().get_rows_host(start, n, out);
 }
 int gb_index_train(gb_index* index) {
+  if (shard_view(index)) return -1;
   IDX_OR_FAIL(index);
   return index->impl->train();
 }
 int gb_index_add_pending(gb_index* index, const uint8_t* del_bitmap) {
+  if (shard_view(index)) return -1;
   IDX_OR_FAIL(index);
   return index->impl->add_pending(del_bitmap);
 }
@@ -399,36 +465,44 @@ float gb_index_last_scan_ms(gb_index* index) { return index && index->impl ? ind
     return -1;                                 \
   }
 #define IVF_OR_FAIL(v, index) AS_OR_FAIL(IvfIndex, v, index, "IVF")
+#define STATE_OR_FAIL(T, v, index, what)      \
+  T* v = state_of<T>(index);                   \
+  if (!v) {                                    \
+    set_last_error("not an " what " index");   \
+    return -1;                                 \
+  }
 #define PQ_OR_FAIL(v, index) AS_OR_FAIL(IvfPqBase, v, index, "IVFPQ")
 
 int gb_index_nlist(gb_index* index) {
-  IVF_OR_FAIL(ivf, index);
+  STATE_OR_FAIL(IvfIndex, ivf, index, "IVF");
   return ivf->nlist();
 }
 int gb_index_set_centroids(gb_index* index, const float* centroids, int nlist) {
+  if (shard_view(index)) return -1;
   IVF_OR_FAIL(ivf, index);
   if (packed_binary(index)) return -1;
   return ivf->set_centroids(centroids, nlist);
 }
 int gb_index_get_centroids(gb_index* index, float* centroids) {
-  IVF_OR_FAIL(ivf, index);
+  STATE_OR_FAIL(IvfIndex, ivf, index, "IVF");
   if (packed_binary(index)) return -1;
   return ivf->get_centroids(centroids);
 }
 int gb_index_pq_m(gb_index* index) {
-  PQ_OR_FAIL(pq, index);
+  STATE_OR_FAIL(IvfPqBase, pq, index, "IVFPQ");
   return pq->M();
 }
 int gb_index_pq_ksub(gb_index* index) {
-  PQ_OR_FAIL(pq, index);
+  STATE_OR_FAIL(IvfPqBase, pq, index, "IVFPQ");
   return pq->ksub();
 }
 int gb_index_set_pq_centroids(gb_index* index, const float* pqc) {
+  if (shard_view(index)) return -1;
   PQ_OR_FAIL(pq, index);
   return pq->set_pq_centroids(pqc);
 }
 int gb_index_get_pq_centroids(gb_index* index, float* pqc) {
-  PQ_OR_FAIL(pq, index);
+  STATE_OR_FAIL(IvfPqBase, pq, index, "IVFPQ");
   return pq->get_pq_centroids(pqc);
 }
 int gb_index_pqfs_lut(gb_index* index, int nq, const float* x, int metric, uint8_t* lut8, float* ab) {
@@ -436,21 +510,22 @@ int gb_index_pqfs_lut(gb_index* index, int nq, const float* x, int metric, uint8
   return fs->lut_host(nq, x, metric, lut8, ab);
 }
 int gb_index_get_precomputed_table(gb_index* index, float* table) {
-  AS_OR_FAIL(IVFPQIndex, pq, index, "IVFPQ");
+  STATE_OR_FAIL(IVFPQIndex, pq, index, "IVFPQ");
   return pq->get_precomputed_table(table);
 }
 int gb_index_has_opq(gb_index* index) {
-  IVFPQIndex* pq = as<IVFPQIndex>(index);
+  IVFPQIndex* pq = state_of<IVFPQIndex>(index);
   return pq && pq->has_opq() ? 1 : 0;
 }
 int gb_index_set_opq(gb_index* index, const float* A) {
+  if (shard_view(index)) return -1;
   IDX_OR_FAIL(index);
   IVFPQIndex* pq = as<IVFPQIndex>(index);
   return pq ? pq->set_opq(A) : -1;
 }
 int gb_index_get_opq(gb_index* index, float* A) {
   IDX_OR_FAIL(index);
-  IVFPQIndex* pq = as<IVFPQIndex>(index);
+  IVFPQIndex* pq = state_of<IVFPQIndex>(index);
   return pq ? pq->get_opq(A) : -1;
 }
 int gb_index_apply_opq(gb_index* index, int64_t n, const float* x, float* out) {
@@ -464,38 +539,54 @@ int gb_index_mirror_builds(gb_index* index) {
   return ivf ? ivf->mirror_builds() : 0;
 }
 int gb_index_get_list_shifts(gb_index* index, float* out) {
-  AS_OR_FAIL(IVFFlatIndex, ivf, index, "IVFFLAT");
+  STATE_OR_FAIL(IVFFlatIndex, ivf, index, "IVFFLAT");
   return ivf->get_list_shifts(out);
 }
 const char* gb_index_last_coarse_kernel(gb_index* index) {
-  IvfIndex* ivf = as<IvfIndex>(index);
+  IvfIndex* ivf = state_of<IvfIndex>(index);
   return ivf ? ivf->last_coarse_kernel() : "";
 }
 int gb_index_compact(gb_index* index) {
   IDX_OR_FAIL(index);
+  if (shard_view(index)) return -1;
+  if (ShardedIndex* sh = sharded(index)) {  // every shard's lists
+    for (int s = 0; s < sh->nshards(); s++)
+      if (sh->shard(s)->compact_lists()) return -1;
+    cudaSetDevice(sh->device());
+    return 0;
+  }
   IvfIndex* ivf = as<IvfIndex>(index);
   return ivf ? ivf->compact_lists() : 0;
 }
 int gb_index_dump(gb_index* index, const char* dir, const char* abs_name) {
   IDX_OR_FAIL(index);
   if (!dir || !abs_name) return -1;
-  IvfIndex* ivf = as<IvfIndex>(index);
-  return ivf ? ivf->dump_gamma(dir, abs_name) : 0;
+  cudaSetDevice(index->impl->device());
+  return index->impl->dump_gamma(dir, abs_name);
 }
 int gb_index_load(gb_index* index, const char* dir, const char* abs_name, int64_t* load_num) {
+  if (shard_view(index)) return -1;
   IDX_OR_FAIL(index);
   if (!dir || !abs_name || !load_num) return -1;
-  *load_num = 0;
-  IvfIndex* ivf = as<IvfIndex>(index);
-  return ivf ? ivf->load_gamma(dir, abs_name, load_num) : 0;
+  cudaSetDevice(index->impl->device());
+  return index->impl->load_gamma(dir, abs_name, load_num);
+}
+static int gb_index_list_len_of(IvfIndex* ivf, int list) {
+  if (!ivf->lists() || list < 0 || list >= ivf->nlist()) return 0;
+  return ivf->lists()->lens()[list];
 }
 int gb_index_list_len(gb_index* index, int list) {
+  if (ShardedIndex* sh = sharded(index)) {  // the list's entries over every shard
+    int n = 0;
+    for (int s = 0; s < sh->nshards(); s++) n += gb_index_list_len_of(sh->shard(s), list);
+    return n;
+  }
   IVF_OR_FAIL(ivf, index);
   if (!ivf->lists() || list < 0 || list >= ivf->nlist()) return 0;
   return ivf->lists()->lens()[list];
 }
 int gb_index_code_size(gb_index* index) {
-  IVF_OR_FAIL(ivf, index);
+  STATE_OR_FAIL(IvfIndex, ivf, index, "IVF");
   return ivf->code_bytes();
 }
 int gb_index_get_list(gb_index* index, int list, uint8_t* codes, int64_t* ids) {
@@ -510,17 +601,20 @@ int gb_index_get_list(gb_index* index, int list, uint8_t* codes, int64_t* ids) {
   return 0;
 }
 int gb_index_tombstone(gb_index* index, int list, int pos) {
+  if (shard_view(index)) return -1;
   IVF_OR_FAIL(ivf, index);
   if (!ivf->lists()) return -1;
   cudaSetDevice(ivf->device());
   return ivf->lists()->tombstone(list, pos, nullptr);
 }
 int gb_index_delete(gb_index* index, const int64_t* vids, int64_t n) {
+  if (shard_view(index)) return -1;
   IDX_OR_FAIL(index);
   if (n < 0 || (n > 0 && !vids)) return -1;
   return index->impl->delete_vectors(vids, n);
 }
 int gb_index_purge(gb_index* index, float threshold, const uint8_t* del_bitmap, int64_t bitmap_bytes, int64_t* dropped) {
+  if (shard_view(index)) return -1;
   IDX_OR_FAIL(index);
   if (!(threshold >= 0.f) || bitmap_bytes < 0) {
     set_last_error("purge: threshold must be >= 0 and bitmap_bytes >= 0");
@@ -529,12 +623,21 @@ int gb_index_purge(gb_index* index, float threshold, const uint8_t* del_bitmap, 
   return index->impl->purge_lists(threshold, del_bitmap, bitmap_bytes, dropped);
 }
 int gb_index_dead_counts(gb_index* index, int* out) {
-  IVF_OR_FAIL(ivf, index);
   if (!out) return -1;
+  if (ShardedIndex* sh = sharded(index)) {  // per list, summed over the shards
+    std::vector<int> part(sh->shard(0)->nlist());
+    for (int l = 0; l < (int)part.size(); l++) out[l] = 0;
+    for (int s = 0; s < sh->nshards(); s++) {
+      if (sh->shard(s)->dead_counts(part.data())) return -1;
+      for (int l = 0; l < (int)part.size(); l++) out[l] += part[l];
+    }
+    return 0;
+  }
+  IVF_OR_FAIL(ivf, index);
   return ivf->dead_counts(out);
 }
 int gb_index_coarse_search(gb_index* index, int nq, const float* x, int nprobe, float* out_dis, int64_t* out_ids) {
-  IVF_OR_FAIL(ivf, index);
+  STATE_OR_FAIL(IvfIndex, ivf, index, "IVF");
   if (packed_binary(index)) return -1;
   return ivf->coarse_search_host(nq, x, nprobe, out_dis, out_ids);
 }

@@ -26,8 +26,10 @@
 #include <sys/stat.h>
 
 #include <algorithm>
+#include <functional>
 #include <memory>
 
+#include "common.cuh"
 #include "index.h"
 
 namespace gb {
@@ -93,9 +95,17 @@ GammaFileFormat IVFPQIndex::gamma_format() const { return {"ivfpq.index", fourcc
 
 // ---- Dump -----------------------------------------------------------------------------------
 int IvfIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
-  const GammaFileFormat gf = gamma_format();
-  if (!trained_ || !gf.file) return 0;  // "gamma index is not trained, skip dumping" (ivfflat.cc:808-811)
+  if (!trained_ || !gamma_format().file) return 0;  // "gamma index is not trained, skip dumping" (ivfflat.cc:808-811)
   std::lock_guard<std::mutex> bg(build_mu_);  // no list mutation while the lists are copied out
+  return write_gamma(dir, abs_name, indexed_count_, lists_->lens(),
+                     [this](int l, std::vector<uint8_t>* codes, std::vector<int64_t>* ids) {
+                       return lists_->download_list(l, codes, ids);
+                     });
+}
+
+int IvfIndex::write_gamma(const std::string& dir, const std::string& abs_name, int64_t indexed, const std::vector<int>& lens,
+                          const std::function<int(int, std::vector<uint8_t>*, std::vector<int64_t>*)>& fetch) {
+  const GammaFileFormat gf = gamma_format();
   cudaSetDevice(device_);
   const std::string index_dir = dir + "/" + abs_name;
   mkdir(dir.c_str(), 0755);
@@ -106,7 +116,7 @@ int IvfIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
   if (!f) return fail("cannot open " + path);
   bool ok = wr<uint32_t>(f, gf.magic);
   // write_ivf_header (index_io.cc:41-47)
-  ok = ok && wr_index_header(f, d_, indexed_count_, mp_.metric);
+  ok = ok && wr_index_header(f, d_, indexed, mp_.metric);
   ok = ok && wr<uint64_t>(f, (uint64_t)nlist_) && wr<uint64_t>(f, (uint64_t)mp_.nprobe);
   std::vector<float> cent((size_t)nlist_ * d_);
   if (get_centroids(cent.data())) return -1;
@@ -120,13 +130,12 @@ int IvfIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
   const uint64_t cb = gf.code_size;
   ok = wr<uint32_t>(f, fourcc("ilar")) && wr<uint64_t>(f, (uint64_t)nlist_) && wr<uint64_t>(f, cb) &&
        wr<uint32_t>(f, fourcc("full")) && wr<uint64_t>(f, (uint64_t)nlist_);
-  const std::vector<int> lens = lists_->lens();
   for (int l = 0; ok && l < nlist_; l++) ok = wr<uint64_t>(f, (uint64_t)lens[l]);
   std::vector<uint8_t> codes, packed;
   std::vector<int64_t> ids;
   for (int l = 0; ok && l < nlist_; l++) {
     if (lens[l] == 0) continue;
-    if (lists_->download_list(l, &codes, &ids)) return -1;
+    if (fetch(l, &codes, &ids)) return -1;
     const size_t n = (size_t)lens[l];
     if (ids.size() < n) return fail("list shrank during dump");
     const uint8_t* src = codes.data();
@@ -137,7 +146,7 @@ int IvfIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
     }
     ok = wr_bytes(f, src, n * cb) && wr_bytes(f, ids.data(), n * 8);
   }
-  if (ok && gf.indexed_count) ok = wr<int32_t>(f, (int32_t)indexed_count_);  // ivfflat.cc:835
+  if (ok && gf.indexed_count) ok = wr<int32_t>(f, (int32_t)indexed);  // ivfflat.cc:835
   if (!ok || fflush(f)) return fail("write error in " + path);
   return 0;
 }
@@ -161,7 +170,14 @@ int IVFPQIndex::dump_gamma_extra(FILE* f) {
 
 // ---- Load -----------------------------------------------------------------------------------
 int IvfIndex::load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) {
+  int64_t file_indexed = 0;
+  return load_gamma_part(dir, abs_name, store_->size(), load_num, &file_indexed);
+}
+
+int IvfIndex::load_gamma_part(const std::string& dir, const std::string& abs_name, int64_t store_rows, int64_t* load_num,
+                              int64_t* file_indexed) {
   *load_num = 0;
+  *file_indexed = 0;
   const GammaFileFormat gf = gamma_format();
   if (!gf.file) return 0;
   const std::string path = dir + "/" + abs_name + "/" + gf.file;
@@ -224,23 +240,47 @@ int IvfIndex::load_gamma(const std::string& dir, const std::string& abs_name, in
     if (sizes[l] > (uint64_t)INT32_MAX) return fail("inverted list too long");
     add[l] = (int)sizes[l];
   }
+  // a shard keeps the entries whose global vid it owns: count them first, so its lists reserve no more than they take
+  const int64_t S = shard_count_;
+  auto mine = [&](int64_t id) { return (id & ~kDelIdxMask) % S == shard_id_; };
+  std::vector<int64_t> ids;
+  if (S > 1) {
+    const long lists_at = ftell(f);
+    for (int l = 0; l < nlist_; l++) {
+      if (!sizes[l]) continue;
+      ids.resize(sizes[l]);
+      if (fseek(f, (long)(sizes[l] * cb), SEEK_CUR) || !rd_bytes(f, ids.data(), sizes[l] * 8))
+        return fail("truncated list in " + path);
+      add[l] = (int)std::count_if(ids.begin(), ids.end(), mine);
+    }
+    if (lists_at < 0 || fseek(f, lists_at, SEEK_SET)) return fail("cannot seek in " + path);
+  }
   cudaStream_t st = build_stream_;
   {
     std::unique_lock<std::shared_mutex> lk(mu_);
     if (lists_->reserve(add, st)) return -1;
   }
   std::vector<uint8_t> codes, padded;
-  std::vector<int64_t> ids;
   int64_t live = 0, max_vid = -1;
   std::vector<uint64_t> v2p;  // vid_bucket_no_pos_, installed only if the whole file loads
   std::vector<int> dead(nlist_, 0);
   const size_t my_cb = (size_t)code_bytes();
   for (int l = 0; l < nlist_; l++) {
-    const size_t len = sizes[l];
+    size_t len = sizes[l];
     if (!len) continue;
     codes.resize(len * cb);
     ids.resize(len);
     if (!rd_bytes(f, codes.data(), codes.size()) || !rd_bytes(f, ids.data(), len * 8)) return fail("truncated list in " + path);
+    if (S > 1) {  // this shard's entries in file order, as local vids, tombstone bits kept
+      size_t w = 0;
+      for (size_t r = 0; r < len; r++) {
+        if (!mine(ids[r])) continue;
+        if (w != r) memmove(codes.data() + w * cb, codes.data() + r * cb, cb);
+        ids[w++] = ((ids[r] & ~kDelIdxMask) / S) | (ids[r] & kDelIdxMask);
+      }
+      len = w;
+      if (!len) continue;
+    }
     const uint8_t* src = codes.data();
     if (my_cb != cb) {  // padded rows in memory
       padded.assign(len * my_cb, 0);
@@ -263,14 +303,17 @@ int IvfIndex::load_gamma(const std::string& dir, const std::string& abs_name, in
     }
   }
   int64_t indexed = live;  // IwPQ: ReadInvertedLists' running count (total - tombstones)
+  *file_indexed = live;
   if (gf.indexed_count) {
     int32_t cnt = 0;
     if (!rd(f, &cnt) || cnt < 0) return fail("invalid indexed count in " + path);  // ivfflat.cc:871-878
-    indexed = cnt;
+    *file_indexed = cnt;
+    indexed = cnt > shard_id_ ? (cnt - shard_id_ + S - 1) / S : 0;  // the vids below cnt this shard owns
   }
-  if (indexed > store_->size() || max_vid >= store_->size())
-    return fail("index file covers " + std::to_string(std::max(indexed, max_vid + 1)) + " vectors, the vector store holds " +
-                std::to_string(store_->size()));
+  const int64_t rows = store_rows > shard_id_ ? (store_rows - shard_id_ + S - 1) / S : 0;
+  if (indexed > rows || max_vid >= rows || *file_indexed > store_rows)
+    return fail("index file covers " + std::to_string(std::max(*file_indexed, global_vid(max_vid) + 1)) +
+                " vectors, the vector store holds " + std::to_string(store_rows));
   {  // publish: nothing above this point changed what a search can see
     std::unique_lock<std::shared_mutex> lk(mu_);
     if (lists_->commit(add, st)) return -1;

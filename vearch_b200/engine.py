@@ -93,8 +93,13 @@ def _status(st):
 
 
 class GammaEngine:
-    def __init__(self, path, space_name="default", log_dir="/tmp/gamma_b200_logs", device=0):
-        cfg = json.dumps({"path": path, "space_name": space_name, "log_dir": log_dir, "device": device}).encode()
+    def __init__(self, path, space_name="default", log_dir="/tmp/gamma_b200_logs", device=0, devices=None):
+        """devices: CUDA ordinals or "all" (Init's "devices"): GPU_IVFPQ / GPU_IVFFLAT fields are sharded over them and
+        devices[0] replaces `device`."""
+        conf = {"path": path, "space_name": space_name, "log_dir": log_dir, "device": device}
+        if devices is not None:
+            conf["devices"] = devices if isinstance(devices, str) else [int(v) for v in devices]
+        cfg = json.dumps(conf).encode()
         self._h = _api().Init(cfg, len(cfg))
         if not self._h:
             raise RuntimeError("gamma Init failed (no CUDA device or bad config)")

@@ -42,20 +42,43 @@ def _bitmap(a):
 class GammaIndex:
     """One vector field's raw store + index model on one GPU."""
 
-    def __init__(self, index_type, d, params=None, device=0, store_type=None):
+    def __init__(self, index_type, d, params=None, device=0, store_type=None, devices=None):
         """store_type: where the raw vectors live, as a table's VectorInfo.store_type: "RocksDB" (any case) keeps them
-        in pinned host memory, read over PCIe, so HBM holds only the index; anything else keeps them in HBM."""
+        in pinned host memory, read over PCIe, so HBM holds only the index; anything else keeps them in HBM.
+        devices: CUDA ordinals (one may repeat) a GPU_IVFPQ / GPU_IVFFLAT index is sharded over, vid v in shard
+        v % len(devices); devices[0] holds the raw vectors and replaces `device`.  One entry, or another type: the index
+        lives on devices[0]."""
         t = index_type.upper()
         self.index_type = "IVFPQFastScan" if t == "IVFPQFASTSCAN" else t  # gamma's spelling of the registered name
         self.d = int(d)
-        self.device = device
+        self.device = device if not devices else int(devices[0])
+        self._view = False
         params = dict(params or {})
         if store_type is not None:
             params["store_type"] = store_type
         pj = json.dumps(params).encode()
-        self._h = _lib.lib().gb_index_create(self.index_type.encode(), self.d, pj, device)
+        if devices is None:
+            self._h = _lib.lib().gb_index_create(self.index_type.encode(), self.d, pj, device)
+        else:
+            devs = (C.c_int * len(devices))(*[int(v) for v in devices])
+            self._h = _lib.lib().gb_index_create_sharded(self.index_type.encode(), self.d, pj, devs, len(devices))
         if not self._h:
             raise GammaError(f"create {index_type}: {_lib.last_error()}")
+
+    @property
+    def shard_count(self):
+        """Shards of the index: 1 unless it was created sharded over two devices or more."""
+        return int(_lib.lib().gb_index_shard_count(self._h))
+
+    def shard(self, i):
+        """Shard i's index structures (lists, centroids, codebook, tables) as a GammaIndex, valid while this index
+        lives; its raw store is empty (the rows stay with the sharded index).  close() frees only the handle."""
+        h = _lib.lib().gb_index_shard(self._h, int(i))
+        if not h:
+            raise GammaError(f"shard {i}: {_lib.last_error()}")
+        v = object.__new__(type(self))
+        v.index_type, v.d, v.device, v._view, v._h, v._owner = self.index_type, self.d, None, True, h, self
+        return v
 
     def close(self):
         if getattr(self, "_h", None):
