@@ -1375,8 +1375,9 @@ int Engine::Dump() {
   }
   f.close();
   // the index itself in gamma's own format (IndexModel::Dump via VectorManager::Dump,
-  // vector_manager.cc:1155-1170): <dir>/<vector name>.000/{ivfflat,ivfpq}.index
-  if (trained && ivf && index_->dump_gamma(dir, vec_name_ + ".000")) return -1;
+  // vector_manager.cc:1155-1170): <dir>/<vector name>.000/{ivfflat,ivfpq}.index, or this engine's own file of a
+  // quantised type (gb_ivfpqfs, gb_ivfrabitq, gb_vearch, gb_binaryivf.index); FLAT writes none
+  if (trained && index_->dump_gamma(dir, vec_name_ + ".000")) return -1;
   for (auto& e : extra_) {  // the other vector fields: raw rows next to the table, index in gamma's format
     std::ofstream ef(dir + "/" + table_name_ + "." + e.name + ".gbvec", std::ios::binary | std::ios::trunc);
     std::vector<float> erows((size_t)max_docid_ * e.dim);
@@ -1443,7 +1444,9 @@ int Engine::Load() {
     if (maxd && !ef.read(reinterpret_cast<char*>(erows.data()), (std::streamsize)(erows.size() * 4))) return -1;
     if (maxd && e.index->add_vectors(erows.data(), maxd)) return -1;
     int64_t eload = 0;
-    e.index->load_gamma(dir, e.name + ".000", &eload);  // trained state + lists; absent: trained again later
+    if (e.index->load_gamma(dir, e.name + ".000", &eload))  // trained state + lists; absent or refused: trained again later
+      fprintf(stderr, "gamma: index file of vector field %s not loaded, the index is built again: %s\n", e.name.c_str(),
+              last_error());
   }
   IvfIndex* ivf = index_->persists_trained_state() ? trained_state_of(index_.get()) : nullptr;
   IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(ivf);
@@ -1462,6 +1465,17 @@ int Engine::Load() {
     // missing or refused file only means the indexing thread re-adds the vectors itself
     int64_t load_num = 0;
     if (index_->load_gamma(dir, vec_name_ + ".000", &load_num) == 0 && load_num > 0) index_status_.store(2);
+  } else if (trained && !index_->persists_trained_state()) {
+    // the quantised types keep their trained state in their own index file only: a file that loads leaves the index
+    // trained and searchable at once; without one, the indexing thread trains it again from the raw rows
+    int64_t load_num = 0;
+    if (index_->load_gamma(dir, vec_name_ + ".000", &load_num))
+      fprintf(stderr, "gamma: index file of vector field %s refused, the index is trained again: %s\n", vec_name_.c_str(),
+              last_error());
+    else if (!index_->trained())
+      fprintf(stderr, "gamma: no index file for vector field %s, the index is trained again\n", vec_name_.c_str());
+    else if (load_num > 0)
+      index_status_.store(2);
   }
   lk.unlock();
   if (trained) BuildIndex();  // train() is a no-op on a trained index; the loop adds what the file did not cover

@@ -268,7 +268,9 @@ class Index {
   int64_t indexed_count() const { return indexed_count_; }
   bool trained() const { return trained_; }
   virtual int training_threshold() const { return 0; }
-  // whether Engine::Dump saves the trained state (centroids, codebook) for Load to restore; false: Load trains again
+  // whether Engine::Dump saves the trained state (centroids, codebook) beside the rows for Load to restore; false: the
+  // trained state lives only in the type's index file (dump_gamma), and Load trains again when that file is missing or
+  // refused
   virtual bool persists_trained_state() const { return true; }
 
   // AddToStore (vector_manager.cc:455): append raw vectors, host rows n x store().row_bytes() bytes
@@ -484,8 +486,8 @@ int kmeans_device(const float* x, int64_t ldx, int64_t n, int d, int k, const KM
 
 // What an IVF index's codec puts into gamma's index file (index_io.cu)
 struct GammaFileFormat {
-  const char* file = nullptr;  // <dir>/<abs_name>/<file>; nullptr: the reference writes no index file for this type
-  uint32_t magic = 0;          // faiss fourcc of the index
+  const char* file = nullptr;  // <dir>/<abs_name>/<file>; nullptr: no index file for this type
+  uint32_t magic = 0;          // fourcc of the index: faiss's, or this engine's own for the types gamma writes no file of
   uint64_t code_size = 0;      // bytes per list entry on disk (in memory: code_bytes(), rows padded when they differ)
   bool indexed_count = false;  // an i32 indexed_count follows the lists
 };
@@ -804,8 +806,10 @@ class IVFPQFastScanIndex : public IvfPqBase {
   int lut_host(int nq, const float* x, int metric, uint8_t* lut8_out, float* ab_out);
 
  protected:
-  // the reference dumps no index file: a loaded table trains and fills this index again from its raw vectors
-  GammaFileFormat gamma_format() const override { return GammaFileFormat(); }
+  // the reference dumps no index file for this type; this engine writes its own (index_io.cu), which only it reads
+  GammaFileFormat gamma_format() const override;
+  int dump_gamma_extra(FILE* f) override;
+  int load_gamma_extra(FILE* f) override;
   int64_t default_training_threshold() const override { return (int64_t)nlist_ * 39; }  // gamma_index_ivfpqfs.cc
   KMeansParams coarse_kmeans_params() const override;
   int coarse_metric(int metric) const override { (void)metric; return kMetricL2; }
@@ -836,7 +840,10 @@ class BinaryIvfIndex : public IvfIndex {
   int get_binary_centroids(uint8_t* host) const;
 
  protected:
-  GammaFileFormat gamma_format() const override { return GammaFileFormat(); }  // Dump writes nothing
+  // this engine's own index file (index_io.cu): the float centroids as the coarse quantiser, the packed ones after it
+  GammaFileFormat gamma_format() const override;
+  int dump_gamma_extra(FILE* f) override;
+  int load_gamma_extra(FILE* f) override;
   int64_t default_training_threshold() const override { return (int64_t)nlist_ * 39; }  // nlist * min_points_per_centroid
   KMeansParams coarse_kmeans_params() const override;
   const float* train_transform(const float* xt, int64_t n, Scratch& s) override;
@@ -880,8 +887,11 @@ class RaBitQIndex : public IvfIndex {
   int estimate_host(int nq, const float* x, const int64_t* lists, int qb, int metric, float* out);
 
  protected:
-  // the reference dumps no usable file here: a loaded table trains and fills this index again from its raw vectors
-  GammaFileFormat gamma_format() const override { return GammaFileFormat(); }
+  // the reference's ivfrabitq.index is faiss's IndexIVFRaBitQ, which this engine neither reads nor writes; it writes its
+  // own file under another name (index_io.cu)
+  GammaFileFormat gamma_format() const override;
+  int dump_gamma_extra(FILE* f) override;
+  int load_gamma_extra(FILE* f) override;
   int64_t default_training_threshold() const override;
   KMeansParams coarse_kmeans_params() const override;
   int append_batch(const void* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
@@ -923,7 +933,9 @@ class VearchIndex : public IvfIndex {
   int lut_host(int nq, const float* x, uint8_t* lut_out, float* mult_out);
 
  protected:
-  GammaFileFormat gamma_format() const override { return GammaFileFormat(); }  // Dump and Load touch no file
+  GammaFileFormat gamma_format() const override;  // this engine's own index file (index_io.cu)
+  int dump_gamma_extra(FILE* f) override;
+  int load_gamma_extra(FILE* f) override;
   int64_t default_training_threshold() const override { return (int64_t)nlist_ * 256; }
   KMeansParams coarse_kmeans_params() const override;
   // the codes are built for the index metric: a request's metric_type does not change the ranking

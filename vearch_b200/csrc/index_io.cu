@@ -20,7 +20,20 @@
 //   IvFl only  : i32 indexed_count
 // An IndexHNSWFlat coarse quantiser ("IHNf") is read for its centroids (the graph is skipped: the coarse
 // search here is exact); Dump always writes the IndexFlat form.  An OPQ block ("LTra") follows the product quantizer when the table has opq.
+//
+// The quantised types the reference writes no file of that this engine could read (IVFPQFastScan, VEARCH, BINARYIVF:
+// none; IVFRABITQ: faiss's IndexIVFRaBitQ) get files of this engine's own, under names the reference never opens, so a
+// CPU partition never meets them and a CPU-written ivfrabitq.index is never read here.  They share the skeleton above,
+// the IvFl trailing i32 indexed_count included, with their own fourcc and codec block after the direct map:
+//   "GbFS" gb_ivfpqfs.index   : u64 code_size, u64 d, u64 M, u64 nbits (4), u64 M*16*dsub, fp32 codebook [M][16][dsub]
+//   "GbRQ" gb_ivfrabitq.index : u64 code_size, i32 nb_bits, i32 qb
+//   "GbVR" gb_vearch.index    : u64 code_size, i32 nsubvector, i32 nblocks, f64 ns_threshold (NaN: none), u8 reordering,
+//                               u64 16*d, fp32 block codebooks [16 d] (each block's centres in their trained order)
+//   "GbBI" gb_binaryivf.index : u64 code_size (d / 8), u64 nlist*code_size, packed centroids [nlist][d / 8]
+// d is in bits for BINARYIVF, whose coarse-quantiser block holds the float k-means centroids (metric L2).  A file is
+// refused unless d, nlist, metric and every codec parameter match the table; the index is then left untrained.
 #include <errno.h>
+#include <math.h>
 #include <stdio.h>
 #include <string.h>
 #include <sys/stat.h>
@@ -92,6 +105,16 @@ int fail(const std::string& msg) {
 // IVF-Flat rows are padded to a multiple of 4 floats here; gamma's are not
 GammaFileFormat IVFFlatIndex::gamma_format() const { return {"ivfflat.index", fourcc("IvFl"), (uint64_t)d_ * 4, true}; }
 GammaFileFormat IVFPQIndex::gamma_format() const { return {"ivfpq.index", fourcc("IwPQ"), (uint64_t)code_bytes(), false}; }
+GammaFileFormat IVFPQFastScanIndex::gamma_format() const {
+  return {"gb_ivfpqfs.index", fourcc("GbFS"), (uint64_t)code_bytes(), true};
+}
+GammaFileFormat RaBitQIndex::gamma_format() const {
+  return {"gb_ivfrabitq.index", fourcc("GbRQ"), (uint64_t)code_bytes(), true};
+}
+GammaFileFormat VearchIndex::gamma_format() const { return {"gb_vearch.index", fourcc("GbVR"), (uint64_t)code_bytes(), true}; }
+GammaFileFormat BinaryIvfIndex::gamma_format() const {
+  return {"gb_binaryivf.index", fourcc("GbBI"), (uint64_t)code_bytes(), true};
+}
 
 // ---- Dump -----------------------------------------------------------------------------------
 int IvfIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
@@ -168,10 +191,46 @@ int IVFPQIndex::dump_gamma_extra(FILE* f) {
   return ok ? 0 : -1;
 }
 
+int IVFPQFastScanIndex::dump_gamma_extra(FILE* f) {
+  std::vector<float> pq((size_t)M_ * ksub_ * dsub_);
+  if (get_pq_centroids(pq.data())) return -1;
+  const bool ok = wr<uint64_t>(f, (uint64_t)code_bytes()) && wr<uint64_t>(f, (uint64_t)d_) && wr<uint64_t>(f, (uint64_t)M_) &&
+                  wr<uint64_t>(f, 4) && wr<uint64_t>(f, (uint64_t)pq.size()) && wr_bytes(f, pq.data(), pq.size() * 4);
+  return ok ? 0 : -1;
+}
+
+int RaBitQIndex::dump_gamma_extra(FILE* f) {
+  return wr<uint64_t>(f, (uint64_t)code_bytes()) && wr<int32_t>(f, nb_bits_) && wr<int32_t>(f, qb_) ? 0 : -1;
+}
+
+int VearchIndex::dump_gamma_extra(FILE* f) {
+  std::vector<float> cb((size_t)16 * d_);
+  if (get_codebook(cb.data())) return -1;
+  const bool ok = wr<uint64_t>(f, (uint64_t)code_bytes()) && wr<int32_t>(f, mp_.nsubvector) && wr<int32_t>(f, nb_) &&
+                  wr<double>(f, mp_.ns_threshold) && wr<uint8_t>(f, mp_.reordering ? 1 : 0) &&
+                  wr<uint64_t>(f, (uint64_t)cb.size()) && wr_bytes(f, cb.data(), cb.size() * 4);
+  return ok ? 0 : -1;
+}
+
+int BinaryIvfIndex::dump_gamma_extra(FILE* f) {
+  std::vector<uint8_t> bc((size_t)nlist_ * cb_);
+  if (get_binary_centroids(bc.data())) return -1;
+  return wr<uint64_t>(f, (uint64_t)cb_) && wr<uint64_t>(f, (uint64_t)bc.size()) && wr_bytes(f, bc.data(), bc.size()) ? 0 : -1;
+}
+
 // ---- Load -----------------------------------------------------------------------------------
 int IvfIndex::load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) {
+  const bool was_trained = trained_;
   int64_t file_indexed = 0;
-  return load_gamma_part(dir, abs_name, store_->size(), load_num, &file_indexed);
+  const int rc = load_gamma_part(dir, abs_name, store_->size(), load_num, &file_indexed);
+  // A refused file of a type whose trained state lives only in that file leaves no part of it behind: the index is
+  // untrained again (its centroids may have been taken before the refusal), so it trains from the raw rows.
+  if (rc && !was_trained && trained_ && !persists_trained_state()) {
+    const std::string why = last_error();
+    reset_index();
+    set_last_error(why);
+  }
+  return rc;
 }
 
 int IvfIndex::load_gamma_part(const std::string& dir, const std::string& abs_name, int64_t store_rows, int64_t* load_num,
@@ -355,6 +414,61 @@ int IVFPQIndex::load_gamma_extra(FILE* f) {
     if (set_opq(A.data())) return -1;
   }
   return set_pq_centroids(pq.data());  // also recomputes the precomputed table (ivfpq.cc:1093-1095)
+}
+
+int IVFPQFastScanIndex::load_gamma_extra(FILE* f) {
+  uint64_t code_size = 0, d = 0, M = 0, nbits = 0, n = 0;
+  if (!rd(f, &code_size) || !rd(f, &d) || !rd(f, &M) || !rd(f, &nbits) || !rd(f, &n)) return fail("truncated IVFPQFastScan codebook");
+  if (d != (uint64_t)d_ || M != (uint64_t)M_ || nbits != 4 || code_size != (uint64_t)code_bytes() ||
+      n != (uint64_t)M_ * ksub_ * dsub_)
+    return fail("IVFPQFastScan codebook does not match the table: d=" + std::to_string(d) + " M=" + std::to_string(M) +
+                " nbits=" + std::to_string(nbits) + " code_size=" + std::to_string(code_size) + " (table: d=" +
+                std::to_string(d_) + " M=" + std::to_string(M_) + " nbits=4)");
+  std::vector<float> pq((size_t)n);
+  if (!rd_bytes(f, pq.data(), pq.size() * 4)) return fail("truncated IVFPQFastScan codebook");
+  return set_pq_centroids(pq.data());
+}
+
+int RaBitQIndex::load_gamma_extra(FILE* f) {
+  uint64_t code_size = 0;
+  int32_t nb_bits = 0, qb = 0;
+  if (!rd(f, &code_size) || !rd(f, &nb_bits) || !rd(f, &qb)) return fail("truncated IVFRABITQ parameters");
+  if (nb_bits != nb_bits_ || qb != qb_ || code_size != (uint64_t)code_bytes())
+    return fail("IVFRABITQ parameters do not match the table: nb_bits=" + std::to_string(nb_bits) + " qb=" +
+                std::to_string(qb) + " code_size=" + std::to_string(code_size) + " (table: nb_bits=" +
+                std::to_string(nb_bits_) + " qb=" + std::to_string(qb_) + ")");
+  return 0;  // the codes depend on the centroids and nb_bits alone: no rotation, no seed
+}
+
+int VearchIndex::load_gamma_extra(FILE* f) {
+  uint64_t code_size = 0, n = 0;
+  int32_t nsub = 0, nb = 0;
+  double t = 0;
+  uint8_t reordering = 0;
+  if (!rd(f, &code_size) || !rd(f, &nsub) || !rd(f, &nb) || !rd(f, &t) || !rd(f, &reordering) || !rd(f, &n))
+    return fail("truncated VEARCH codebook");
+  const bool same_t = (isnan(t) && isnan(mp_.ns_threshold)) || t == mp_.ns_threshold;
+  if (nsub != mp_.nsubvector || nb != nb_ || !same_t || (reordering != 0) != mp_.reordering ||
+      code_size != (uint64_t)code_bytes() || n != (uint64_t)16 * d_)
+    return fail("VEARCH codebook does not match the table: nsubvector=" + std::to_string(nsub) + " blocks=" +
+                std::to_string(nb) + " ns_threshold=" + std::to_string(t) + " reordering=" + std::to_string(reordering) +
+                " (table: nsubvector=" + std::to_string(mp_.nsubvector) + " blocks=" + std::to_string(nb_) +
+                " ns_threshold=" + std::to_string(mp_.ns_threshold) + " reordering=" + std::to_string(mp_.reordering) + ")");
+  std::vector<float> cb((size_t)n);
+  if (!rd_bytes(f, cb.data(), cb.size() * 4)) return fail("truncated VEARCH codebook");
+  return set_codebook(cb.data());
+}
+
+int BinaryIvfIndex::load_gamma_extra(FILE* f) {
+  uint64_t code_size = 0, n = 0;
+  if (!rd(f, &code_size) || !rd(f, &n)) return fail("truncated BINARYIVF centroids");
+  if (code_size != (uint64_t)cb_ || n != (uint64_t)nlist_ * cb_)
+    return fail("BINARYIVF centroids do not match the table: code_size=" + std::to_string(code_size) +
+                " (table: " + std::to_string(cb_) + ")");
+  std::vector<uint8_t> bc((size_t)n);
+  if (!rd_bytes(f, bc.data(), bc.size())) return fail("truncated BINARYIVF centroids");
+  // the packed centroids as they were, not re-derived from the float ones (set_binary_centroids may have set them alone)
+  return set_binary_centroids(bc.data(), nlist_);
 }
 
 }  // namespace gb

@@ -351,11 +351,13 @@ class GammaIndex:
         _check(_lib.lib().gb_index_compact(self._h), "compact")
 
     def dump(self, directory, abs_name):
-        """IndexModel::Dump in gamma's own format: <directory>/<abs_name>/{ivfflat,ivfpq}.index."""
+        """IndexModel::Dump: <directory>/<abs_name>/{ivfflat,ivfpq}.index in gamma's own format; IVFPQFastScan, IVFRABITQ,
+        VEARCH and BINARYIVF write this engine's own gb_{ivfpqfs,ivfrabitq,vearch,binaryivf}.index."""
         _check(_lib.lib().gb_index_dump(self._h, str(directory).encode(), abs_name.encode()), "dump")
 
     def load(self, directory, abs_name):
-        """IndexModel::Load; returns load_num (0: no file).  The vectors must already be in the store."""
+        """IndexModel::Load; returns load_num (0: no file).  The vectors must already be in the store.  A refused file raises;
+        an index of the four quantised types is then left untrained."""
         n = np.zeros(1, np.int64)
         _check(_lib.lib().gb_index_load(self._h, str(directory).encode(), abs_name.encode(), _ptr(n)), "load")
         return int(n[0])
