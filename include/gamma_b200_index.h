@@ -93,6 +93,13 @@ int gb_index_search_device(gb_index *index, int nq, const float *x_dev, int64_t 
 int gb_index_search_device_keys(gb_index *index, int nq, const float *x_dev, int64_t ld, int k,
                                 const char *retrieval_params_json, int brute_force, unsigned long long *out_keys_dev,
                                 float *out_scores_dev, int64_t *out_ids_dev, void *stream);
+/* gb_index_search_device with a deletion and a filter bitmap in device memory on the index's device (either NULL),
+ * in gb_index_search's layout: ceil(bitmap_bits / 8) LSB-first bytes, bit set => deleted / allowed, ids at or above
+ * bitmap_bits neither; any alignment.  They are read on `stream`; the score window is [min_score, max_score]. */
+int gb_index_search_device_filtered(gb_index *index, int nq, const float *x_dev, int64_t ld, int k,
+                                    const char *retrieval_params_json, int brute_force, const uint8_t *del_bits_dev,
+                                    const uint8_t *filter_bits_dev, int64_t bitmap_bits, float min_score,
+                                    float max_score, float *out_scores_dev, int64_t *out_ids_dev, void *stream);
 /* {"stage": ms, ...}: device time per stage of the searches run since the last call with timing enabled
  * (CUDA events on the launching stream); *json_out is malloc'd, the caller frees it */
 int gb_index_stage_times(gb_index *index, char **json_out, int *out_len);

@@ -57,6 +57,7 @@ def _declare(l):
     l.gb_index_search.argtypes = [vp, i32, vp, i32, cstr, i32, vp, vp, i64, f32, f32, vp, vp]
     l.gb_index_search_device.argtypes = [vp, i32, vp, i64, i32, cstr, i32, vp, vp, vp]
     l.gb_index_search_device_keys.argtypes = [vp, i32, vp, i64, i32, cstr, i32, vp, vp, vp, vp]
+    l.gb_index_search_device_filtered.argtypes = [vp, i32, vp, i64, i32, cstr, i32, vp, vp, i64, f32, f32, vp, vp, vp]
     l.gb_index_stage_times.argtypes = [vp, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]
     l.gb_merge_partition_keys_device.argtypes = [i32, vp, i32, i32, i32, i32, vp, vp, vp]
     l.gb_index_set_rerank_stats.restype = None

@@ -293,8 +293,8 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     fields_.push_back({"_id", DT_STRING, false});
   }
   values_.assign(fields_.size(), {});
-  sidx_.assign(fields_.size(), ScalarIndex());
-  for (size_t fi = 0; fi < fields_.size(); fi++) sidx_[fi].built = fields_[fi].indexed;
+  sidx_.clear();
+  sidx_.resize(fields_.size());
   size_t nvec = t.vec_len(2);
   if (nvec == 0) return Status::Make(kInvalidArgument, space_name_ + " table has no vector field");
   FbTable v = t.vec_table(2, 0);
@@ -379,6 +379,8 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     live_engines().all.push_back(this);
   }
   if (training_threshold_ <= 0) training_threshold_ = index_->training_threshold();
+  for (size_t fi = 0; fi < fields_.size(); fi++)
+    if (fields_[fi].indexed && scalar_index_rebuild((int)fi)) return Status::Make(kIndexError, last_error());
   created_table_ = true;
   // <path>/<table>.schema, as the reference writes it (engine.cc:676-684)
   if (!path_.empty()) {
@@ -403,6 +405,7 @@ Index* Engine::index_of(const std::string& vec_name, int* dim) {
 }
 
 int Engine::flush_pending_locked() {
+  if (scalar_flush_locked()) return -1;
   if (pending_n_ == 0) return 0;
   // Row i of every vector field must stay document i: a field is appended only while its store is as long as the
   // primary one was when this flush began, so a retry after a partial failure appends exactly the missing fields,
@@ -464,9 +467,10 @@ int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
   if (docid != -1 && docid < max_docid_) {  // Update (engine.cc:703-710, 774-850)
     for (auto& f : table_fields) {
       const int fi = field_idx_[f.name];
+      scalar_index_put(fi, docid, f.value, &values_[fi][docid]);
       values_[fi][docid] = f.value;
-      scalar_index_put(fi, docid, f.value);
     }
+    if (scalar_staged() >= kScalarFlushRows && scalar_flush_locked()) return -1;
     if (has_vec) {
       if (vec_len != vbytes_) return -1;
       std::vector<unsigned char> x(vec, vec + vec_len);
@@ -495,7 +499,7 @@ int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
   for (auto& f : table_fields) values_[field_idx_[f.name]][max_docid_] = f.value;
   values_[field_idx_["_id"]][max_docid_] = key;
   for (size_t fi = 0; fi < fields_.size(); fi++)
-    if (fields_[fi].indexed) scalar_index_put((int)fi, max_docid_, values_[fi][max_docid_]);
+    if (fields_[fi].indexed) scalar_index_put((int)fi, max_docid_, values_[fi][max_docid_], nullptr);
   keys_.push_back(key);
   key2docid_[key] = max_docid_;
   pending_.resize((size_t)(pending_n_ + 1) * vbytes_);
@@ -508,7 +512,7 @@ int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
   pending_n_++;
   ++max_docid_;
   if ((size_t)(max_docid_ >> 3) + 1 > del_bitmap_.size()) del_bitmap_.resize((size_t)(max_docid_ >> 3) + 4096, 0);
-  if (pending_n_ >= 8192 && flush_pending_locked()) return -5;
+  if ((pending_n_ >= 8192 || scalar_staged() >= kScalarFlushRows) && flush_pending_locked()) return -5;
   // auto-start indexing (engine.cc:753-761)
   if (refresh_interval_ >= 0 && indexing_state_.load() == 0 && index_status_.load() == 0 &&
       max_docid_ - delete_num_ >= training_threshold_ &&
@@ -638,25 +642,6 @@ int Engine::GetDocByDocid(int docid, bool next, std::string* fb_out) {
 // Search(): the per-filter sets are intersected (operator And) or united (Or).  A filter on a field
 // without a scalar index, or an empty result, means "no result" (scalar_index_manager.cc:598-610).
 namespace {
-template <typename T>
-int cmp_num(const std::string& a, const std::string& b) {
-  T x, y;
-  memcpy(&x, a.data(), sizeof(T));
-  memcpy(&y, b.data(), sizeof(T));
-  return x < y ? -1 : (x > y ? 1 : 0);
-}
-// -2: not comparable (wrong width)
-int cmp_typed(int dt, const std::string& a, const std::string& b) {
-  size_t w = (dt == DT_INT || dt == DT_FLOAT) ? 4 : (dt == DT_BOOL ? 1 : 8);
-  if (a.size() != w || b.size() != w) return -2;
-  switch (dt) {
-    case DT_INT: return cmp_num<int32_t>(a, b);
-    case DT_FLOAT: return cmp_num<float>(a, b);
-    case DT_DOUBLE: return cmp_num<double>(a, b);
-    case DT_BOOL: return cmp_num<uint8_t>(a, b);
-    default: return cmp_num<int64_t>(a, b);  // DT_LONG, DT_DATE
-  }
-}
 std::vector<std::string> split001(const std::string& s) {
   std::vector<std::string> out;
   size_t a = 0;
@@ -695,124 +680,100 @@ static bool decode_num(int dt, const std::string& v, int64_t* iv, double* fv) {
   }
 }
 
-void Engine::scalar_index_put(int fi, int docid, const std::string& value) {
-  if (fi >= (int)sidx_.size() || !sidx_[fi].built) return;
-  ScalarIndex& si = sidx_[fi];
-  const int dt = fields_[fi].data_type;
-  if (is_string_type(dt)) {
-    if (dt == DT_STRINGARRAY) {
-      for (const auto& e : split001(value)) {
-        auto& pl = si.postings[e];
-        if (pl.empty() || pl.back() != docid) pl.push_back(docid);
-      }
-    } else {
-      auto& pl = si.postings[value];
-      if (pl.empty() || pl.back() != docid) pl.push_back(docid);
-    }
-    return;
-  }
-  if ((int)si.ok.size() <= docid) {
-    si.ok.resize((size_t)docid + 1, 0);
-    if (is_float_type(dt)) si.f64.resize((size_t)docid + 1, 0.0);
-    else si.i64.resize((size_t)docid + 1, 0);
-  }
-  int64_t iv = 0;
-  double fv = 0;
-  si.ok[docid] = decode_num(dt, value, &iv, &fv) ? 1 : 0;
-  if (is_float_type(dt)) si.f64[docid] = fv;
-  else si.i64[docid] = iv;
+void Engine::scalar_index_put(int fi, int docid, const std::string& value, const std::string* old) {
+  if (fi < (int)sidx_.size() && sidx_[fi].built()) sidx_[fi].stage(docid, value, old);
 }
 
-void Engine::scalar_index_rebuild(int fi) {
+int Engine::scalar_index_rebuild(int fi) {
   if (fi >= (int)sidx_.size()) sidx_.resize(fields_.size());
-  ScalarIndex& si = sidx_[fi];
-  si = ScalarIndex();
-  si.built = true;
-  for (int d = 0; d < (int)values_[fi].size(); d++) scalar_index_put(fi, d, values_[fi][d]);
+  cudaSetDevice(device_);
+  if (sidx_[fi].build(fields_[fi].data_type, values_[fi]) == 0) return 0;
+  sidx_[fi].release();
+  return -1;
 }
 
-int64_t Engine::eval_filters(const std::vector<SearchRequestPB::Filter>& filters, int op, std::vector<uint8_t>* bitmap) const {
-  const int n = max_docid_;
-  const size_t nbytes = (size_t)(n >> 3) + 1;
-  bitmap->assign(nbytes, 0);
-  std::vector<uint8_t> cur(nbytes);
-  bool first = true;
-  auto set_bit = [&](int d) { cur[d >> 3] |= (uint8_t)(1u << (d & 7)); };
+int64_t Engine::scalar_staged() const {
+  int64_t n = 0;
+  for (const auto& c : sidx_) n = std::max(n, c.staged());
+  return n;
+}
+
+int Engine::scalar_flush_locked() {
+  if (scalar_staged() == 0) return 0;
+  cudaSetDevice(device_);
+  for (size_t fi = 0; fi < sidx_.size(); fi++) {
+    ScalarColumn& c = sidx_[fi];
+    if (c.flush(cudaStreamPerThread)) return -1;
+    if (c.wants_repack() && c.build(fields_[fi].data_type, values_[fi])) return -1;  // the live runs, packed
+  }
+  return 0;
+}
+
+// A request's filter bitmap on device_: ceil(n / 32) + 1 words, zero at and above n, so every scan reads it in place.
+// Allocated on the calling thread's stream of device_ and freed there when the request ends.
+struct Engine::FilterBits {
+  int device;
+  Scratch s;
+  uint32_t* bits = nullptr;
+  int64_t words = 0;
+  explicit FilterBits(int dev) : device(dev), s(cudaStreamPerThread) {}
+  ~FilterBits() { cudaSetDevice(device); }  // before s frees on the stream of that device
+};
+
+int64_t Engine::eval_filters(const std::vector<SearchRequestPB::Filter>& filters, int op, FilterBits* out) const {
+  const int64_t n = max_docid_;
+  std::vector<FilterDesc> fd;
+  std::vector<int32_t> terms, codes;
+  std::vector<size_t> term_at;  // fd[i]'s first term in `terms`
   for (const auto& fl : filters) {
     auto it = field_idx_.find(fl.field);
     if (it == field_idx_.end() || !fields_[it->second].indexed) return 0;
     const int fi = it->second, dt = fields_[fi].data_type;
     const bool is_str = is_string_type(dt);
     if (fl.lower.empty() && (is_str || fl.upper.empty())) continue;  // Filter() returns an untouched result
-    if (fi >= (int)sidx_.size() || !sidx_[fi].built) return 0;
-    const ScalarIndex& si = sidx_[fi];
-    std::fill(cur.begin(), cur.end(), 0);
-    const bool neg = fl.is_union == 2;
+    if (fi >= (int)sidx_.size() || !sidx_[fi].built()) return 0;
+    FilterDesc d;
+    memset(&d, 0, sizeof d);
+    sidx_[fi].describe(&d);
+    d.neg = fl.is_union == 2;
     if (is_str) {
-      // In / NotIn over the inverted map; postings may hold documents whose value has changed since: re-check
-      const std::vector<std::string> items = split001(fl.lower);
-      for (const auto& item : items) {
-        auto pit = si.postings.find(item);
-        if (pit == si.postings.end()) continue;
-        for (int d : pit->second) {
-          if (d >= n) continue;
-          const std::string& v = values_[fi][d];
-          bool in;
-          if (dt == DT_STRINGARRAY) {
-            in = false;
-            for (const auto& e : split001(v))
-              if (e == item) in = true;
-          } else {
-            in = v == item;
-          }
-          if (in) set_bit(d);
-        }
-      }
-      if (neg) {
-        for (size_t i = 0; i < nbytes; i++) cur[i] = (uint8_t)~cur[i];
-      }
+      sidx_[fi].codes_of(split001(fl.lower), &codes);  // terms the dictionary does not know match no document
+      d.nterms = (int)codes.size();
+      term_at.push_back(terms.size());
+      terms.insert(terms.end(), codes.begin(), codes.end());
     } else {
-      int64_t lo_i = 0, hi_i = 0;
-      double lo_f = 0, hi_f = 0;
-      const bool has_lo = !fl.lower.empty(), has_hi = !fl.upper.empty();
-      const bool lo_ok = has_lo && decode_num(dt, fl.lower, &lo_i, &lo_f);
-      const bool hi_ok = has_hi && decode_num(dt, fl.upper, &hi_i, &hi_f);
-      const bool equal = fl.lower == fl.upper;
-      const int m = std::min<int>(n, (int)si.ok.size());
-      auto scan = [&](auto* col, auto lo, auto hi) {
-        for (int d = 0; d < m; d++) {
-          if (!si.ok[d]) continue;
-          const auto v = col[d];
-          bool hit;
-          if (equal) {
-            hit = lo_ok && (neg ? v != lo : v == lo);
-          } else {
-            hit = true;
-            if (has_lo) hit = lo_ok && (v > lo || (v == lo && fl.include_lower));
-            if (hit && has_hi) hit = hi_ok && (v < hi || (v == hi && fl.include_upper));
-          }
-          if (hit) set_bit(d);
-        }
-      };
-      if (is_float_type(dt)) scan(si.f64.data(), lo_f, hi_f);
-      else scan(si.i64.data(), lo_i, hi_i);
+      term_at.push_back(terms.size());
+      d.has_lo = !fl.lower.empty(), d.has_hi = !fl.upper.empty();
+      d.lo_ok = d.has_lo && decode_num(dt, fl.lower, &d.lo_i, &d.lo_f);
+      d.hi_ok = d.has_hi && decode_num(dt, fl.upper, &d.hi_i, &d.hi_f);
+      d.inc_lo = fl.include_lower, d.inc_hi = fl.include_upper;
+      d.equal = fl.lower == fl.upper;
+      d.neg = d.equal && d.neg;  // is_union means nothing else to a numeric field
+      d.is_float = is_float_type(dt);
     }
-    if (n & 7) cur[nbytes - 1] &= (uint8_t)((1u << (n & 7)) - 1u);  // no bits at or above max_docid
-    else cur[nbytes - 1] = 0;
-    if (first) {
-      bitmap->swap(cur);
-      cur.resize(bitmap->size());
-      first = false;
-    } else if (op == 0) {
-      for (size_t i = 0; i < cur.size(); i++) (*bitmap)[i] &= cur[i];
-    } else if (op == 1) {
-      for (size_t i = 0; i < cur.size(); i++) (*bitmap)[i] |= cur[i];
-    }
+    fd.push_back(d);
   }
-  if (first) return 0;
-  int64_t card = 0;
-  for (uint8_t b : *bitmap) card += __builtin_popcount(b);
-  return card;
+  if (fd.empty()) return 0;
+  cudaSetDevice(device_);
+  cudaStream_t st = out->s.stream();
+  // one upload: the cardinality counter (zero), the descriptors, the term codes
+  const size_t desc_at = 16, codes_at = desc_at + fd.size() * sizeof(FilterDesc);
+  std::vector<uint8_t> blob(codes_at + terms.size() * 4, 0);
+  out->words = (n + 31) / 32 + 1;
+  out->bits = out->s.alloc_n<uint32_t>((size_t)out->words);
+  uint8_t* dblob = out->s.alloc_n<uint8_t>(blob.size());
+  if (!out->bits || !dblob) return -1;
+  for (size_t i = 0; i < fd.size(); i++) fd[i].terms = reinterpret_cast<const int32_t*>(dblob + codes_at) + term_at[i];
+  memcpy(blob.data() + desc_at, fd.data(), fd.size() * sizeof(FilterDesc));
+  if (!terms.empty()) memcpy(blob.data() + codes_at, terms.data(), terms.size() * 4);
+  unsigned long long card = 0;
+  auto* dcard = reinterpret_cast<unsigned long long*>(dblob);
+  GB_CUDA(cudaMemcpyAsync(dblob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
+  GB_CUDA(launch_filter_eval(reinterpret_cast<const FilterDesc*>(dblob + desc_at), (int)fd.size(), op, n, out->words,
+                             out->bits, dcard, st));
+  GB_CUDA(cudaMemcpyAsync(&card, dcard, 8, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));  // the columns may change once the shared lock is released
+  return (int64_t)card;
 }
 
 // Engine::Search (search/engine.cc:242-402) + VectorManager::Search (vector_manager.cc:739-1079)
@@ -854,12 +815,13 @@ Status Engine::Search(const SearchRequestPB& req, std::string* pb_out) {
   const int topN = req.topn + req.offset;
   std::vector<float> dis((size_t)n * topN);
   std::vector<int64_t> ids((size_t)n * topN);
-  std::vector<uint8_t> bm, fbm;
+  std::vector<uint8_t> bm;
+  FilterBits fbits(device_);
   int total_docs;
   {
     std::unique_lock<std::shared_mutex> wl(mu_, std::defer_lock);
     std::shared_lock<std::shared_mutex> rl(mu_);
-    bool need_flush = pending_n_ > 0;
+    bool need_flush = pending_n_ > 0 || scalar_staged() > 0;
     rl.unlock();
     if (need_flush) {
       wl.lock();
@@ -874,7 +836,9 @@ Status Engine::Search(const SearchRequestPB& req, std::string* pb_out) {
     }
     total_docs = doc_num();
     if (!req.filters.empty()) {  // ScalarIndexQuery (search/engine.cc:349-366, 525-580)
-      if (eval_filters(req.filters, req.filter_operator, &fbm) == 0) {
+      const int64_t card = eval_filters(req.filters, req.filter_operator, &fbits);
+      if (card < 0) return Status::Make(kIndexError, last_error());
+      if (card == 0) {
         PbWriter resp;
         for (int i = 0; i < req.req_num; i++) {
           PbWriter sr, st;
@@ -887,7 +851,8 @@ Status Engine::Search(const SearchRequestPB& req, std::string* pb_out) {
         *pb_out = resp.out;
         return Status::OK();
       }
-      ctx.filter_bitmap = fbm.data();
+      ctx.filter_bits_dev = fbits.bits;
+      ctx.bits_dev_words = fbits.words;
       ctx.bitmap_bits = max_docid_;
     }
   }
@@ -996,11 +961,20 @@ Status Engine::SearchMulti(const SearchRequestPB& req, std::string* pb_out) {
   base.params.brute_force = brute != 0;
   base.search_unindexed_tail = enable_realtime_;
   const int topN = req.topn + req.offset;
-  std::vector<uint8_t> bm, fbm;
+  std::vector<uint8_t> bm;
+  FilterBits fbits(device_);
   int total_docs;
   {
-    std::unique_lock<std::shared_mutex> wl(mu_);
-    if (pending_n_ > 0 && flush_pending_locked()) return Status::Make(kIndexError, last_error());
+    std::unique_lock<std::shared_mutex> wl(mu_, std::defer_lock);
+    std::shared_lock<std::shared_mutex> rl(mu_);
+    bool need_flush = pending_n_ > 0 || scalar_staged() > 0;
+    rl.unlock();
+    if (need_flush) {
+      wl.lock();
+      if (flush_pending_locked()) return Status::Make(kIndexError, last_error());
+      wl.unlock();
+    }
+    rl.lock();
     if (delete_num_ > 0) {
       bm.assign(del_bitmap_.begin(), del_bitmap_.begin() + (max_docid_ >> 3) + 1);
       base.del_bitmap = bm.data();
@@ -1008,7 +982,9 @@ Status Engine::SearchMulti(const SearchRequestPB& req, std::string* pb_out) {
     }
     total_docs = doc_num();
     if (!req.filters.empty()) {
-      if (eval_filters(req.filters, req.filter_operator, &fbm) == 0) {
+      const int64_t card = eval_filters(req.filters, req.filter_operator, &fbits);
+      if (card < 0) return Status::Make(kIndexError, last_error());
+      if (card == 0) {
         PbWriter resp;
         for (int i = 0; i < req.req_num; i++) {
           PbWriter sr, st;
@@ -1021,7 +997,8 @@ Status Engine::SearchMulti(const SearchRequestPB& req, std::string* pb_out) {
         *pb_out = resp.out;
         return Status::OK();
       }
-      base.filter_bitmap = fbm.data();
+      base.filter_bits_dev = fbits.bits;
+      base.bits_dev_words = fbits.words;
       base.bitmap_bits = max_docid_;
     }
   }
@@ -1101,7 +1078,7 @@ Status Engine::Query(const QueryRequestPB& req, std::string* pb_out) {
     // lock, then serve the query under the shared one (filters, field reads and the per-document device reads
     // of put_doc_fields do not block ingest or other searches)
     std::unique_lock<std::shared_mutex> wl(mu_);
-    if (pending_n_ > 0 && flush_pending_locked()) return Status::Make(kIndexError, last_error());
+    if ((pending_n_ > 0 || scalar_staged() > 0) && flush_pending_locked()) return Status::Make(kIndexError, last_error());
   }
   std::shared_lock<std::shared_mutex> rl(mu_);
   std::vector<int> docids;
@@ -1123,9 +1100,11 @@ Status Engine::Query(const QueryRequestPB& req, std::string* pb_out) {
     }
   } else {
     const int topn = req.limit;
-    std::vector<uint8_t> fbm;
     if (!req.filters.empty()) {
-      if (eval_filters(req.filters, req.filter_operator, &fbm) == 0) {
+      FilterBits fbits(device_);
+      const int64_t card = eval_filters(req.filters, req.filter_operator, &fbits);
+      if (card < 0) return Status::Make(kIndexError, last_error());
+      if (card == 0) {
         PbWriter resp, sr, st;
         st.put_int32(1, 0);
         st.put_int32(3, 0);
@@ -1135,6 +1114,10 @@ Status Engine::Query(const QueryRequestPB& req, std::string* pb_out) {
         *pb_out = resp.out;
         return Status::OK();
       }
+      std::vector<uint8_t> fbm((size_t)fbits.words * 4);  // the words, LSB-first, are the bytes of the host layout
+      if (cudaMemcpyAsync(fbm.data(), fbits.bits, fbm.size(), cudaMemcpyDeviceToHost, fbits.s.stream()) != cudaSuccess ||
+          cudaStreamSynchronize(fbits.s.stream()) != cudaSuccess)
+        return Status::Make(kIndexError, "filter bitmap download failed");
       int skipped = 0;
       for (int d = 0; d < max_docid_ && (int)docids.size() < topn; d++) {
         if (!((fbm[d >> 3] >> (d & 7)) & 1)) continue;
@@ -1169,11 +1152,16 @@ Status Engine::SetFieldIndexed(const std::string& field, bool indexed) {
     return Status::Make(kNotSupported, "the index of vector field " + field + " is fixed when the table is created");
   auto it = field_idx_.find(field);
   if (it == field_idx_.end()) return Status::Make(kInvalidArgument, "field " + field + " not found");
-  fields_[it->second].indexed = indexed;
-  if (indexed) {
-    scalar_index_rebuild(it->second);  // AddFieldIndex builds the index over the documents already stored
-  } else if (it->second < (int)sidx_.size()) {
-    sidx_[it->second] = ScalarIndex();
+  cudaSetDevice(device_);
+  if (indexed) {  // AddFieldIndex builds the index over the documents already stored
+    fields_[it->second].indexed = true;
+    if (scalar_index_rebuild(it->second)) {
+      fields_[it->second].indexed = false;
+      return Status::Make(kIndexError, last_error());
+    }
+  } else {
+    fields_[it->second].indexed = false;
+    if (it->second < (int)sidx_.size()) sidx_[it->second].release();
   }
   return Status::OK();
 }
@@ -1286,10 +1274,12 @@ std::string Engine::MemoryInfo() {  // search/engine.cc:1178-1200
   long long vec_mem = index_ ? index_->store().mem_bytes() + index_->store().host_bytes() : 0;
   for (auto& e : extra_)
     index_mem += e.index->index_mem_bytes(), vec_mem += e.index->store().mem_bytes() + e.index->store().host_bytes();
+  long long field_range_mem = 0;  // the scalar indexes: device columns, string-array pools, dictionaries
+  for (auto& c : sidx_) field_range_mem += c.mem_bytes();
   char buf[256];
   snprintf(buf, sizeof buf,
-           "{\"bitmap_mem\":%lld,\"field_range_mem\":0,\"index_mem\":%lld,\"table_mem\":%lld,\"vector_mem\":%lld}",
-           (long long)del_bitmap_.size(), index_mem, table_mem, vec_mem);
+           "{\"bitmap_mem\":%lld,\"field_range_mem\":%lld,\"index_mem\":%lld,\"table_mem\":%lld,\"vector_mem\":%lld}",
+           (long long)del_bitmap_.size(), field_range_mem, index_mem, table_mem, vec_mem);
   return buf;
 }
 
@@ -1426,7 +1416,7 @@ int Engine::Load() {
   int32_t trained;
   if (!rdv(f, &trained)) return -1;
   for (size_t fi = 0; fi < fields_.size(); fi++)
-    if (fields_[fi].indexed) scalar_index_rebuild((int)fi);
+    if (fields_[fi].indexed && scalar_index_rebuild((int)fi)) return -1;
   keys_.resize(maxd);
   int idf = field_idx_["_id"];
   for (int d = 0; d < maxd; d++) {

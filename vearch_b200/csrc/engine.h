@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "index.h"
+#include "scalar_index.h"
 
 namespace gb {
 struct PbWriter;
@@ -130,8 +131,8 @@ class Engine {
   int Load();
   const std::string& space_name() const { return space_name_; }
   void quiesce();  // stop the indexing thread (also from an atexit hook for engines never Closed)
-  // Engine::AddFieldIndex / RemoveFieldIndex (search/engine.cc:1471-1600): here a scalar field's "index" is
-  // the permission to filter on it (filters scan the in-memory column), so both are a flag flip
+  // Engine::AddFieldIndex / RemoveFieldIndex (search/engine.cc:1471-1600): build the field's device columns over the
+  // documents already stored, or free them
   Status SetFieldIndexed(const std::string& field, bool indexed);
 
   // cooperative cancellation (c_api/api_data/request_context.h:51-88)
@@ -158,9 +159,11 @@ class Engine {
     int data_type;
     bool indexed = false;  // FieldInfo.is_index: only indexed fields can be filtered on
   };
-  // ScalarIndexManager::Search (table/scalar_index_manager.cc:294-345, 588-651) as a scan of the
-  // in-memory columns: dense LSB-first bitmap of the docids that pass; returns the cardinality
-  int64_t eval_filters(const std::vector<SearchRequestPB::Filter>& filters, int op, std::vector<uint8_t>* bitmap) const;
+  // ScalarIndexManager::Search (table/scalar_index_manager.cc:294-345, 588-651) on the device columns, with the table
+  // held shared: the LSB-first bitmap of the docids that pass, as uint32 words on device_ in `bits` (the request owns
+  // it); returns the cardinality (0: "no result"), -1 on a CUDA error (last_error)
+  struct FilterBits;
+  int64_t eval_filters(const std::vector<SearchRequestPB::Filter>& filters, int op, FilterBits* bits) const;
   struct FieldSel {
     std::vector<int> attr;           // table fields, in name order (std::map order of the reference)
     std::vector<std::string> vecs;   // vector fields asked for by name
@@ -175,20 +178,16 @@ class Engine {
   std::vector<FieldDef> fields_;
   std::unordered_map<std::string, int> field_idx_;
   std::vector<std::vector<std::string>> values_;  // [field][docid]
-  // Scalar indexes of the fields created with is_index (table/scalar_index_manager.cc: one index per field): numeric
-  // fields keep a typed column (a filter is one pass over int64 / double values, no string handling), string fields
-  // an inverted map term -> docids (postings are append-only: an updated document is re-verified against its current
-  // value at query time).  Built at AddOrUpdate / Load / AddFieldIndex, evaluated under the SHARED table lock.
-  struct ScalarIndex {
-    bool built = false;
-    std::vector<int64_t> i64;   // DT_INT / DT_LONG / DT_DATE / DT_BOOL
-    std::vector<double> f64;    // DT_FLOAT / DT_DOUBLE
-    std::vector<uint8_t> ok;    // value present with the field type's width
-    std::unordered_map<std::string, std::vector<int>> postings;  // DT_STRING / DT_STRINGARRAY
-  };
-  std::vector<ScalarIndex> sidx_;  // [field]
-  void scalar_index_put(int fi, int docid, const std::string& value);
-  void scalar_index_rebuild(int fi);
+  // Scalar indexes of the fields created with is_index (table/scalar_index_manager.cc: one index per field): device
+  // columns on device_ (scalar_index.h).  AddOrUpdate stages values; flush_pending_locked applies them; Load and
+  // AddFieldIndex build a field in bulk.  Changed only under the EXCLUSIVE table lock, evaluated under the SHARED one.
+  std::vector<ScalarColumn> sidx_;  // [field]
+  // docid's value of field fi is now `value` (old: the value it replaces, nullptr for a new document)
+  void scalar_index_put(int fi, int docid, const std::string& value, const std::string* old);
+  int scalar_index_rebuild(int fi);
+  int scalar_flush_locked();  // apply what AddOrUpdate staged; re-pack string-array pools that are half dead
+  int64_t scalar_staged() const;  // the most values any field has staged
+  static constexpr int kScalarFlushRows = 8192;  // staged values of one field that trigger a flush from AddOrUpdate
   std::unordered_map<std::string, int> key2docid_;
   std::vector<std::string> keys_;  // docid -> _id
 

@@ -857,13 +857,24 @@ int Index::upload_bitmaps(const SearchContext& ctx, FilterArgs* f, Scratch& s) {
   size_t words = (size_t)((bits + 31) / 32) + 1;
   size_t have = (size_t)((ctx.bitmap_bits + 7) / 8);
   for (int which = 0; which < 2; which++) {
+    const uint32_t* src_dev = which == 0 ? ctx.del_bits_dev : ctx.filter_bits_dev;
     const uint8_t* src = which == 0 ? ctx.del_bitmap : ctx.filter_bitmap;
-    if (!src) continue;
+    if (!src && !src_dev) continue;
+    if (src_dev && ctx.bits_dev_words >= (int64_t)words) {  // already padded: the scan reads it in place
+      if (which == 0)
+        f->del_bits = src_dev;
+      else
+        f->filter_bits = src_dev;
+      continue;
+    }
     uint32_t* dev = s.alloc_n<uint32_t>(words);
     if (!dev) return -1;
     // ids beyond the caller's bitmap: not deleted / not allowed
     GB_CUDA(cudaMemsetAsync(dev, 0, words * 4, s.stream()));
-    GB_CUDA(cudaMemcpyAsync(dev, src, have, cudaMemcpyHostToDevice, s.stream()));
+    if (src_dev)
+      GB_CUDA(cudaMemcpyAsync(dev, src_dev, have, cudaMemcpyDeviceToDevice, s.stream()));
+    else
+      GB_CUDA(cudaMemcpyAsync(dev, src, have, cudaMemcpyHostToDevice, s.stream()));
     if (which == 0)
       f->del_bits = dev;
     else
@@ -982,7 +993,8 @@ static constexpr int kCoalesceMaxNq = 16;     // requests at most this large are
 static constexpr int kCoalesceMaxBatch = 512;  // queries per merged device batch (reference kMaxBatch)
 
 bool Index::coalescable(const SearchContext& ctx, int nq) const {
-  return coalesce_enabled() && nq <= kCoalesceMaxNq && !ctx.del_bitmap && !ctx.filter_bitmap;
+  return coalesce_enabled() && nq <= kCoalesceMaxNq && !ctx.del_bitmap && !ctx.filter_bitmap && !ctx.del_bits_dev &&
+         !ctx.filter_bits_dev;
 }
 
 static bool same_signature(const SearchContext& a, int ka, const SearchContext& b, int kb) {

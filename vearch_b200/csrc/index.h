@@ -240,6 +240,13 @@ struct RetrievalParams {  // gamma_index_ivfpq.cc:233-294, gamma_index_ivfflat.c
 struct SearchContext {  // RetrievalContext / SearchCondition (common/gamma_common_data.h:33-121)
   const uint8_t* del_bitmap = nullptr;     // host, bit set => deleted
   const uint8_t* filter_bitmap = nullptr;  // host, bit set => allowed (nullptr => no filter)
+  // the same bitmaps as uint32 words on the index's device, used in place of the host ones; they must be readable
+  // when the search starts (written on its stream, or waited for)
+  const uint32_t* del_bits_dev = nullptr;
+  const uint32_t* filter_bits_dev = nullptr;
+  // words readable at each device bitmap, zero past bitmap_bits; 0: only its ceil(bitmap_bits / 8) bytes.  A bitmap
+  // that covers what the scan reads (upload_bitmaps) is used as it is, any other is copied into padded scratch.
+  int64_t bits_dev_words = 0;
   int64_t bitmap_bits = 0;
   float min_score = -3.4028235e38f, max_score = 3.4028235e38f;
   bool search_unindexed_tail = false;  // table.enable_realtime: brute-force the not-yet-indexed vectors too

@@ -404,6 +404,26 @@ int gb_index_search_device(gb_index* index, int nq, const float* x_dev, int64_t 
                                     static_cast<cudaStream_t>(stream));
 }
 
+int gb_index_search_device_filtered(gb_index* index, int nq, const float* x_dev, int64_t ld, int k,
+                                    const char* retrieval_params_json, int brute_force, const uint8_t* del_bits_dev,
+                                    const uint8_t* filter_bits_dev, int64_t bitmap_bits, float min_score,
+                                    float max_score, float* out_scores_dev, int64_t* out_ids_dev, void* stream) {
+  IDX_OR_FAIL(index);
+  if (packed_binary(index)) return -1;
+  if (bitmap_bits < 0) {
+    set_last_error("bitmap_bits must not be negative");
+    return -1;
+  }
+  SearchContext ctx;
+  if (fill_ctx(&ctx, retrieval_params_json, brute_force, nullptr, nullptr, bitmap_bits, min_score, max_score)) return -1;
+  // byte bitmaps of any alignment: search_device copies them into word-aligned, padded scratch on `stream`
+  ctx.del_bits_dev = reinterpret_cast<const uint32_t*>(del_bits_dev);
+  ctx.filter_bits_dev = reinterpret_cast<const uint32_t*>(filter_bits_dev);
+  ctx.bits_dev_words = 0;
+  return index->impl->search_device(ctx, nq, x_dev, ld, k, out_scores_dev, out_ids_dev,
+                                    static_cast<cudaStream_t>(stream));
+}
+
 int gb_index_search_device_keys(gb_index* index, int nq, const float* x_dev, int64_t ld, int k,
                                 const char* retrieval_params_json, int brute_force, unsigned long long* out_keys_dev,
                                 float* out_scores_dev, int64_t* out_ids_dev, void* stream) {

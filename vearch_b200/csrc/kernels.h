@@ -364,4 +364,34 @@ cudaError_t launch_purge_scatter(ListDirectory dir, const int* sel_list, const P
 cudaError_t launch_fill_u64(unsigned long long* p, int64_t n, unsigned long long v, cudaStream_t st);
 cudaError_t launch_pad_rows(const float* src, int64_t n, int d, float* dst, int64_t ldd, cudaStream_t st);
 
+// ---- scalar filters (kernels_filter.cu) ------------------------------------------------------
+// One evaluated filter of a request, on the device columns of its field.  A document d < ncol has a value; d >= ncol
+// has none.  Numeric columns are `width` bytes per document (1: uint8, 4: int32 / float, 8: int64 / double) with a
+// validity bit each, compared in int64 (is_float 0) or double (is_float 1).  String columns hold an int32 dictionary
+// code per document; string-array columns an (offset, count) run of codes in `pool`.
+enum FilterKind { kFilterNumeric = 0, kFilterString = 1, kFilterStringArray = 2 };
+struct FilterDesc {
+  int kind, width, is_float;
+  int equal, neg;  // numeric: Equal (NotEqual when neg); string: NotIn when neg
+  int has_lo, has_hi, lo_ok, hi_ok, inc_lo, inc_hi;
+  int nterms;                    // string: sorted codes in terms[]
+  int64_t lo_i, hi_i;
+  double lo_f, hi_f;
+  int64_t ncol;
+  const void* col;               // numeric values
+  const uint32_t* valid;         // numeric validity bits
+  const int32_t* codes;          // string codes
+  const int64_t* arr_off;        // string-array runs
+  const int32_t* arr_cnt;
+  const int32_t* pool;
+  const int32_t* terms;
+};
+// out[w], w < words: bit b = the request's filters, combined in order (op 0 And, 1 Or, else the first one's set), on
+// document 32 w + b; zero at and above n.  *card (zeroed by the caller) += the set bits.
+cudaError_t launch_filter_eval(const FilterDesc* fd, int nf, int op, int64_t n, int64_t words, uint32_t* out,
+                               unsigned long long* card, cudaStream_t st);
+// col[docs[i]] = the low `width` bytes of vals[i], i < m (docids distinct); valid (nullable): bit docs[i] = ok[i]
+cudaError_t launch_scatter_column(const int32_t* docs, const uint64_t* vals, const uint8_t* ok, int64_t m, int width,
+                                  void* col, uint32_t* valid, cudaStream_t st);
+
 }  // namespace gb

@@ -185,8 +185,11 @@ class GammaIndex:
         _check(rc, "search")
         return dis, ids
 
-    def search_device(self, x, k, params=None, brute_force=False, out=None):
-        """Queries and results stay in HBM (torch CUDA tensors); asynchronous on torch's current stream."""
+    def search_device(self, x, k, params=None, brute_force=False, out=None, del_bitmap=None, filter_bitmap=None,
+                      min_score=-FLT_MAX, max_score=FLT_MAX):
+        """Queries and results stay in HBM (torch CUDA tensors); asynchronous on torch's current stream.
+        del_bitmap / filter_bitmap: CUDA uint8 tensors of one length on the index's device in search()'s layout
+        (LSB-first, bit set => deleted / allowed, ids past the bitmap neither), read on that stream."""
         import torch
         assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1
         nq = x.shape[0]
@@ -195,9 +198,28 @@ class GammaIndex:
                    torch.empty((nq, k), dtype=torch.int64, device=x.device))
         pj = json.dumps(params).encode() if params else b""
         st = torch.cuda.current_stream(x.device).cuda_stream
-        rc = _lib.lib().gb_index_search_device(self._h, nq, C.c_void_p(x.data_ptr()), x.stride(0), k, pj,
-                                               int(brute_force), C.c_void_p(out[0].data_ptr()),
-                                               C.c_void_p(out[1].data_ptr()), C.c_void_p(st))
+        if del_bitmap is None and filter_bitmap is None and min_score == -FLT_MAX and max_score == FLT_MAX:
+            rc = _lib.lib().gb_index_search_device(self._h, nq, C.c_void_p(x.data_ptr()), x.stride(0), k, pj,
+                                                   int(brute_force), C.c_void_p(out[0].data_ptr()),
+                                                   C.c_void_p(out[1].data_ptr()), C.c_void_p(st))
+            _check(rc, "search_device")
+            return out
+        # one bitmap_bits covers both bitmaps, as in search()
+        assert del_bitmap is None or filter_bitmap is None or del_bitmap.numel() == filter_bitmap.numel()
+        bits, ptrs = 0, []
+        for b in (del_bitmap, filter_bitmap):
+            if b is None:
+                ptrs.append(None)
+                continue
+            assert b.is_cuda and b.dtype == torch.uint8 and b.dim() == 1 and b.is_contiguous()
+            bits = max(bits, b.numel() * 8)
+            if b.numel() == 0:  # an empty bitmap is still a bitmap: it allows (or deletes) nothing
+                b = torch.zeros(1, dtype=torch.uint8, device=b.device)
+            ptrs.append(C.c_void_p(b.data_ptr()))
+        rc = _lib.lib().gb_index_search_device_filtered(self._h, nq, C.c_void_p(x.data_ptr()), x.stride(0), k, pj,
+                                                        int(brute_force), ptrs[0], ptrs[1], bits, C.c_float(min_score),
+                                                        C.c_float(max_score), C.c_void_p(out[0].data_ptr()),
+                                                        C.c_void_p(out[1].data_ptr()), C.c_void_p(st))
         _check(rc, "search_device")
         return out
 
