@@ -1779,20 +1779,6 @@ static bool coarse_fused_enabled() {
   return e ? atoi(e) != 0 : true;
 }
 
-// centroid tiles per segment of the fused coarse quantiser: fewest (waves of one CTA per SM) x (tiles per item + 1),
-// the + 1 standing for an item's fixed cost (pipeline fill, a fresh key set); ties go to fewer segments
-static int coarse_seg_tiles(int nqt, int ntc, int nsm) {
-  int best = ntc;
-  int64_t best_cost = INT64_MAX;
-  for (int t = ntc; t >= 1; t--) {
-    const int nseg = (ntc + t - 1) / t;
-    if (nseg > 16) break;  // bounds the per-query keys the merge reads
-    const int64_t cost = ((int64_t)nqt * nseg + nsm - 1) / nsm * (t + 1);
-    if (cost < best_cost) best_cost = cost, best = t;
-  }
-  return best;
-}
-
 // quantizer->search (gamma_index_ivfflat.cc:568 / gamma_index_ivfpq.cc:595)
 int IvfIndex::coarse_dev(int nq, const void* xqv, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis,
                          Scratch& s) {
@@ -1802,21 +1788,16 @@ int IvfIndex::coarse_dev(int nq, const void* xqv, int nprobe, int metric, int32_
   const bool tc = nlist_ >= 64 && nq >= 32;
   const int k16 = (int)round_up(dpad_, 16);
   if (tc && coarse_fused_enabled() && nprobe <= kCoarseMaxK && k16 > 16) {
-    // fused: per (query tile, centroid segment) the best nprobe keys, merged per query; no score matrix
-    const int nqt = (nq + 127) / 128, ntc = (nlist_ + 127) / 128;
-    const int seg_tiles = coarse_seg_tiles(nqt, ntc, sm_count(device_));
-    const int nseg = (ntc + seg_tiles - 1) / seg_tiles;
+    // fused: each query's best nprobe keys straight from the tensor-core tiles; no score matrix
+    const int nqt = (nq + 127) / 128, nsm = sm_count(device_);
     GB_ALLOC(a_tiles, float, (size_t)nqt * tc_mirror_tile_floats(k16), s);
     GB_ALLOC(a_norms, float, (size_t)nqt * 128, s);
-    GB_ALLOC(tau, unsigned long long, nq, s);
-    GB_ALLOC(part, unsigned long long, (size_t)nq * nseg * nprobe, s);
+    GB_ALLOC(ws, unsigned char, coarse_topk_workspace_bytes(nq, nlist_, nprobe, nsm), s);
     StageScope stage(this, "coarse_quantizer", st);
     last_coarse_kernel_ = "coarse_topk_kernel";
-    GB_CUDA(cudaMemsetAsync(tau, 0xFF, sizeof(unsigned long long) * nq, st));
     GB_CUDA(launch_tc_stage_rows(xq, dpad_, nq, dpad_, k16, a_tiles, a_norms, st));
-    GB_CUDA(launch_coarse_topk(a_tiles, a_norms, nq, d_cent_tiles_, d_cent_norms_, nlist_, k16, seg_tiles, metric, nprobe, tau,
-                               part, st));
-    GB_CUDA(launch_select_keys(part, (int64_t)nseg * nprobe, nq, nseg * nprobe, nprobe, keys, nprobe, st));
+    GB_CUDA(launch_coarse_topk(a_tiles, a_norms, nq, d_cent_tiles_, d_cent_norms_, nlist_, k16, metric, nprobe, nsm, ws, keys,
+                               st));
     GB_CUDA(launch_split_keys(keys, (int64_t)nq * nprobe, metric, coarse_dis, probe_ids, st));
     return 0;
   }

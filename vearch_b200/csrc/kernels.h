@@ -41,14 +41,14 @@ cudaError_t launch_dist_argmin_tc(const float* X, int64_t ldx, int n, const floa
 // past n are zero
 cudaError_t launch_tc_stage_rows(const float* x, int64_t ldx, int64_t n, int d, int k16, float* tiles, float* norms,
                                  cudaStream_t st);
-// fused coarse quantiser (3xTF32 scores, bit-equal to launch_dist_matrix_tc): for every query q and centroid segment
-// s (seg_tiles 128-centroid tiles, nseg = ceil(ceil(nlist / 128) / seg_tiles)) the k best keys of the segment, in
-// any order, sentinel padded: out[(q * nseg + s) * k + i].  a_* / c_*: launch_tc_stage_rows of the queries and the
-// centroids; tau_g[nq] pre-set to the sentinel.
+// fused coarse quantiser (3xTF32 scores, bit-equal to launch_dist_matrix_tc): every query's k best keys, sorted
+// ascending, sentinel padded: out[q * k + i].  a_* / c_*: launch_tc_stage_rows of the queries and the centroids;
+// nsm: the device's SM count (one CTA each); ws: coarse_topk_workspace_bytes of device memory.
 constexpr int kCoarseMaxK = 64;
+size_t coarse_topk_workspace_bytes(int nq, int nlist, int k, int nsm);
 cudaError_t launch_coarse_topk(const float* a_tiles, const float* a_norms, int nq, const float* c_tiles, const float* c_norms,
-                               int nlist, int k16, int seg_tiles, int metric, int k, unsigned long long* tau_g,
-                               unsigned long long* out, cudaStream_t st);
+                               int nlist, int k16, int metric, int k, int nsm, void* ws, unsigned long long* out,
+                               cudaStream_t st);
 
 // ---- K7: top-k selection / merge ----------------------------------------------------------
 // Per row r: select the k best of m candidates.  Input is either scores (fp32, vid = id_base+col)

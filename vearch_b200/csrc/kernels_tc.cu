@@ -5,7 +5,7 @@
 //    gamma_index_ivfflat.cc:407 / gamma_index_ivfpq.cc:372).  faiss itself evaluates this
 //    contraction as sgemm + norms (IndexFlat, >= 20 queries).
 //  * K2 fused  coarse_topk_kernel: the coarse quantiser's top-nprobe without a score matrix (TMA-fed, the
-//    same MMAs as dist_tc_kernel, per-query key sets in the epilogue).
+//    same MMAs as dist_tc_kernel, per-query key sets kept by selection warpgroups beside the MMA warpgroup).
 //  * K3 list-major: when many queries of a batch probe the same list the IVF-Flat scan
 //    (gamma_index_ivfflat.cc:579-787) IS a dense contraction.  The (query, probe) pairs are grouped by
 //    list on the device (lm_count / lmk_scan / lmk_assign / lmk_items); a work item multiplies a group
@@ -33,6 +33,8 @@
 // and |y_t|^2.  TMA kernel: the same tiles already exist in global memory (tc_mirror_build_kernel,
 // lm_stage_queries_kernel) and arrive as 16 KiB bulk copies.
 #include <float.h>
+
+#include <algorithm>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -790,94 +792,201 @@ __global__ void __launch_bounds__(TC_M)
 }
 
 // ---- K2 fused: the coarse quantiser's top-nprobe on the tensor cores ----------------------------
-// The coarse quantiser's key set: the same admission rule and the same kept set as lmk_consider, but once full the
-// k keys form a max-heap, so a replacement costs one sift-down (log2 k levels of two independent shared loads)
-// instead of a scan of all k slots.  Nearly every key a query admits past the first k replaces one, and these
-// dependent shared-memory chains are what the epilogue waits on.
-__device__ __forceinline__ void ck_sift_down(unsigned long long* hk, int k, int i, unsigned long long key) {
+// Warp roles (ck_nt<TPQ>() threads, one CTA per SM):
+//   warps 0-3           one warpgroup: the wgmma sequence of dist_tc_kernel (the same chunks, MMAs and order, so every
+//                       score is bit-equal to the matrix that kernel writes) for tile i + 1 while the selection warps
+//                       scan tile i; then the accumulator goes to the score buffer (four slabs, acc_to_slab layout).
+//                       Thread 0 refills each ring stage by TMA once every warp's MMAs of it are complete: a
+//                       producer warp of its own would lower every thread's register budget below the 128 registers
+//                       the accumulator alone takes.
+//   next 128 * TPQ      selection: TPQ threads per query, thread (r, h) scans columns [h, h + 1) * 128 / TPQ of query
+//                       r's row of every tile and keeps its own key set of k keys
+// The score buffer is single (full / empty mbarriers); the accumulator registers are the second buffer.
+//
+// Work split: the nqt x ntc (query tile, centroid tile) pairs, query-tile-major, are cut into gridDim.x equal
+// contiguous ranges, one per CTA.  A query tile shared by several CTAs gets one partial key set per CTA and thread;
+// the CTA that completes it last (a per-tile counter) merges them, sorts and writes the tile's keys.  Every key set
+// of a query holds only keys below a bound that is the k-th best of k of its valid keys (tau_g shares the bounds of
+// one query across threads and CTAs), so their union holds the query's true top k; the merge runs without that bound.
+constexpr int CK_NST = LT_STAGES;
+constexpr int CK_SCORE_BYTES = 4 * kSlabFloats * 4;  // the 128 x 128 dot products of one tile: 64 KiB
+constexpr int CK_MIN_TILES = 4;                      // fewest tile pairs per CTA (bounds the partial sets a merge reads)
+
+// threads per query: as many as fit their key sets (k keys of 8 bytes each) in 64 KiB, at most two
+__host__ __device__ constexpr int ck_tpq(int k) { return k <= 32 ? 2 : 1; }
+template <int TPQ>
+__host__ __device__ constexpr int ck_nt() {
+  return TC_M * (1 + TPQ);
+}
+// the CTA whose range holds tile pair w, for W pairs cut into G ranges [b W / G, (b + 1) W / G)
+__host__ __device__ __forceinline__ int ck_owner(int64_t w, int64_t W, int G) { return (int)(((w + 1) * G - 1) / W); }
+
+struct CkShared {
+  alignas(16) float cn[TC_N];  // |y|^2 of the buffered tile's centroids
+  uint64_t full[CK_NST], sfull, sempty;
+  int last;
+};
+
+// named barrier of the selection threads (barrier 1 is wg0_sync's)
+template <int NSEL>
+__device__ __forceinline__ void ck_sel_sync() {
+  asm volatile("bar.sync 2, %0;" ::"n"(NSEL) : "memory");
+}
+
+// A key set: slot i of selection thread s at hk[i * S].  Once it holds k keys they form a max-heap, so a replacement
+// costs one sift-down (log2 k levels of two independent shared loads) instead of a scan of all k slots.
+template <int S>
+__device__ __forceinline__ void ck_sift_down(unsigned long long* hk, int n, int i, unsigned long long key) {
   for (;;) {
     const int l = 2 * i + 1;
-    if (l >= k) break;
-    const unsigned long long vl = hk[l * TC_NT], vr = l + 1 < k ? hk[(l + 1) * TC_NT] : 0ull;
+    if (l >= n) break;
+    const unsigned long long vl = hk[l * S], vr = l + 1 < n ? hk[(l + 1) * S] : 0ull;
     const int c = vr > vl ? l + 1 : l;
     const unsigned long long vc = vr > vl ? vr : vl;
     if (vc <= key) break;
-    hk[i * TC_NT] = vc;
+    hk[i * S] = vc;
     i = c;
   }
-  hk[i * TC_NT] = key;
+  hk[i * S] = key;
 }
 
-template <int METRIC>
-__device__ __noinline__ LmkState ck_consider(unsigned long long* hk, int k, uint32_t vid, float sc, LmkState st) {
-  // the score window of select_rows_kernel: non-finite scores never enter
-  if (vid == kLmkNoVid || !(sc <= FLT_MAX && sc >= -FLT_MAX)) return st;
-  const unsigned long long key = make_key(score2ord<METRIC>(sc), vid);
+// the admission rule of lmk_consider: key < st.tau enters; k keys kept
+template <int S>
+__device__ __noinline__ LmkState ck_insert(unsigned long long* hk, int k, unsigned long long key, LmkState st) {
   if (key >= st.tau) return st;
   if (st.n < k) {
-    hk[st.n * TC_NT] = key;
+    hk[st.n * S] = key;
     if (++st.n < k) return st;
-    for (int i = k / 2 - 1; i >= 0; i--) ck_sift_down(hk, k, i, hk[i * TC_NT]);  // the set is full: heapify
+    for (int i = k / 2 - 1; i >= 0; i--) ck_sift_down<S>(hk, k, i, hk[i * S]);  // the set is full: heapify
   } else {
-    ck_sift_down(hk, k, 0, key);  // key < st.tau <= the largest key: it replaces the top
+    ck_sift_down<S>(hk, k, 0, key);  // key < st.tau <= the largest key: it replaces the top
   }
   const unsigned long long mx = hk[0];
   if (mx < st.tau) st.tau = mx;
   return st;
 }
 
-// Work item = (128-query tile, segment of consecutive 128-centroid tiles).  Both operands sit in global memory in
-// the canonical operand layout (queries staged per call, centroids whenever they change), so the CTA is fed as
-// ivf_listmajor_tma_kernel is: warp 4 issues cp.async.bulk copies into a ring, warpgroup 0 runs the wgmma sequence of
-// dist_tc_kernel (the same chunks, MMAs and order, so every score is bit-equal to the matrix that kernel writes) and
-// thread t keeps query t's k best keys of the segment.  Segments of one query share their bound through tau_g.
-// A column leaves the hot loop only if it beats the thread's bound; each lane then walks its OWN hits, re-reading
-// the dot product from the slab, so a warp iterates as often as its busiest lane and not once per column that any
-// lane hit (early in a segment nearly every column is a hit somewhere in the warp).
-template <int METRIC>
-__global__ void __launch_bounds__(LT_NT, 1)
-    coarse_topk_kernel(const float* __restrict__ a_tiles, const float* __restrict__ a_norms, int nq,
-                       const float* __restrict__ c_tiles, const float* __restrict__ c_norms, int nlist, int k16,
-                       int seg_tiles, int nseg, int k, unsigned long long* tau_g, unsigned long long* __restrict__ out) {
-  extern __shared__ __align__(1024) unsigned char smem[];  // [ring: NST * STAGE] [slabs] [key sets: k * 1 KiB]
-  __shared__ LtShared sh;
-  constexpr int NST = LT_STAGES;
-  constexpr int STAGE = TC_STAGE_BYTES;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int qt = blockIdx.x / nseg, sg = blockIdx.x - qt * nseg;
-  const int ct0 = sg * seg_tiles;
-  const int ntiles = min(seg_tiles, (nlist + TC_N - 1) / TC_N - ct0);
-  const int nk = k16 / TC_BK;
-  unsigned char* ring = smem;
+template <int METRIC, int S>
+__device__ __forceinline__ LmkState ck_consider(unsigned long long* hk, int k, uint32_t vid, float sc, LmkState st) {
+  // the score window of select_rows_kernel: non-finite scores never enter
+  if (vid == kLmkNoVid || !(sc <= FLT_MAX && sc >= -FLT_MAX)) return st;
+  return ck_insert<S>(hk, k, make_key(score2ord<METRIC>(sc), vid), st);
+}
 
-  if (tid == 0) ring_init(sh.full, sh.empty, NST, 1);  // the producer's arrive.expect_tx; the copies complete the phase
+// keys of a partial set -> this thread's set, eight loads in flight
+template <int S>
+__device__ __forceinline__ LmkState ck_absorb(unsigned long long* hk, int k, const unsigned long long* src, int64_t stride,
+                                              LmkState st) {
+  for (int i0 = 0; i0 < k; i0 += 8) {
+    unsigned long long v[8];
+#pragma unroll
+    for (int u = 0; u < 8; u++) v[u] = i0 + u < k ? __ldcg(src + (int64_t)(i0 + u) * stride) : kKeySentinel;
+#pragma unroll
+    for (int u = 0; u < 8; u++)
+      if (v[u] < st.tau) st = ck_insert<S>(hk, k, v[u], st);
+  }
+  return st;
+}
+
+template <int METRIC, int TPQ>
+__global__ void __launch_bounds__(ck_nt<TPQ>(), 1)
+    coarse_topk_kernel(const float* __restrict__ a_tiles, const float* __restrict__ a_norms, int nq,
+                       const float* __restrict__ c_tiles, const float* __restrict__ c_norms, int nlist, int k16, int k,
+                       int nparts, unsigned long long* tau_g, unsigned int* cnt, unsigned long long* part,
+                       unsigned long long* __restrict__ out) {
+  extern __shared__ __align__(1024) unsigned char smem[];  // [ring: NST * STAGE] [score buffer] [key sets: k * NSEL * 8]
+  __shared__ CkShared sh;
+  constexpr int NST = CK_NST, STAGE = TC_STAGE_BYTES, NSEL = TC_M * TPQ, SLICE = TC_N / TPQ;
+  const int tid = threadIdx.x, warp = tid >> 5;
+  const int nk = k16 / TC_BK, ntc = (nlist + TC_N - 1) / TC_N;
+  const int64_t W = (int64_t)((nq + TC_M - 1) / TC_M) * ntc;
+  const int G = gridDim.x, b = blockIdx.x;
+  const int64_t w0 = b * W / G, w1 = (b + 1) * W / G;
+  unsigned char* ring = smem;
+  float* scores = reinterpret_cast<float*>(smem + (size_t)NST * STAGE);
+
+  if (tid == 0) {
+    for (int s = 0; s < NST; s++) mbar_init(&sh.full[s], 1);  // thread 0's arrive.expect_tx; the copies complete the phase
+    mbar_init(&sh.sfull, TC_M);
+    mbar_init(&sh.sempty, NSEL);
+    mbar_fence_init();
+  }
   __syncthreads();
 
   if (warp < 4) {
-    // ======================= MMA + epilogue =======================
-    unsigned long long* hk = reinterpret_cast<unsigned long long*>(ring + (size_t)NST * STAGE + kSlabBytes) + tid;
-    float* slabs = reinterpret_cast<float*>(ring + (size_t)NST * STAGE);
-    const int q = qt * TC_M + tid;
-    const bool valid = q < nq;
-    LmkState st{valid ? __ldcg(tau_g + q) : 0ull, 0};  // bound 0: padding rows admit nothing
-    float bound = key_bound<METRIC>(st.tau);
-    const float xn = a_norms[q];
+    // ======================= MMA =======================
+    // chunk n of this CTA's sequence: K chunk n % nk of tile pair w0 + n / nk, in ring stage n % NST
+    const int64_t nchunks = (w1 - w0) * nk;
+    auto issue = [&](int64_t n) {
+      const int64_t w = w0 + n / nk;
+      const int kc = (int)(n % nk), qt = (int)(w / ntc), ct = (int)(w % ntc);
+      unsigned char* stage = ring + (size_t)(n % NST) * STAGE;
+      uint64_t* full = &sh.full[n % NST];
+      mbar_arrive_expect_tx(full, STAGE);
+      bulk_g2s(stage, reinterpret_cast<const char*>(a_tiles) + ((int64_t)qt * nk + kc) * LT_HALF, LT_HALF, full);
+      bulk_g2s(stage + LT_HALF, reinterpret_cast<const char*>(c_tiles) + ((int64_t)ct * nk + kc) * LT_HALF, LT_HALF, full);
+    };
+    // the stage of chunk m has been read by every warp's MMAs (their wgmma groups are complete): chunk m + NST
+    auto refill = [&](int64_t m) {
+      wg0_sync();
+      if (tid == 0 && m + NST < nchunks) issue(m + NST);
+    };
+    if (tid == 0)
+      for (int64_t n = 0; n < NST && n < nchunks; n++) issue(n);
     float acc[2][64];
-    for (int i = 0; i < ntiles; i++) {
-      const int b = i & 1, ct = ct0 + i;
+    int64_t n = 0;
+    int i = 0;
+    for (int64_t w = w0; w < w1; w++, i++) {
+      const int ct = (int)(w % ntc);
       const float cn = c_norms[ct * TC_N + tid];  // issued before the MMAs, stored after them
-      ring_tile_mma<NST, STAGE>(acc, smem_u32(ring), sh.full, sh.empty, i * nk, nk, TC_TILE_BYTES, LT_HALF,
-                                LT_HALF + TC_TILE_BYTES);
-      sh.cn[b][tid] = cn;  // buffer b was last read in tile i - 2, before tile i - 1's exchange barriers
-      sh.vid[b][tid] = ct * TC_N + tid < nlist ? (uint32_t)(ct * TC_N + tid) : kLmkNoVid;
+      for (int kc = 0; kc < nk; kc++, n++) {
+        mbar_wait(&sh.full[n % NST], (uint32_t)((n / NST) & 1));
+        const uint32_t a = smem_u32(ring) + (uint32_t)(n % NST) * STAGE;
+        wg_fence();
+        tc_chunk_mma(acc, a, a + TC_TILE_BYTES, a + LT_HALF, a + LT_HALF + TC_TILE_BYTES, kc == 0);
+        wg_commit();
+        if (kc > 0) {
+          wg_wait<1>();
+          refill(n - 1);
+        }
+      }
+      wg_wait<0>();
+      wg_fence_acc(acc);
+      refill(n - 1);
+      mbar_wait(&sh.sempty, (uint32_t)((i & 1) ^ 1));  // the selection threads are done with tile i - 1
 #pragma unroll
-      for (int c0 = 0; c0 < TC_N; c0 += 32) {
+      for (int c0 = 0; c0 < TC_N; c0 += 32) acc_to_slab(acc, c0, scores + (c0 >> 5) * kSlabFloats);
+      sh.cn[tid] = cn;
+      mbar_arrive(&sh.sfull);
+    }
+  } else {
+    // ======================= selection =======================
+    const int sid = tid - TC_M, r = sid & (TC_M - 1), h = sid / TC_M;
+    unsigned long long* hk = reinterpret_cast<unsigned long long*>(scores + 4 * kSlabFloats) + sid;
+    LmkState st{0ull, 0};
+    float bound = 0.f, xn = 0.f;
+    int q = 0;
+    bool valid = false;
+    int i = 0;
+    for (int64_t w = w0; w < w1; w++, i++) {
+      const int qt = (int)(w / ntc), ct = (int)(w - (int64_t)qt * ntc);
+      if (ct == 0 || w == w0) {  // this CTA's first tile of query tile qt: a fresh key set
+        q = qt * TC_M + r;
+        valid = q < nq;
+        st = LmkState{valid ? __ldcg(tau_g + q) : 0ull, 0};  // bound 0: padding rows admit nothing
+        bound = key_bound<METRIC>(st.tau);
+        xn = a_norms[q];
+      }
+      mbar_wait(&sh.sfull, (uint32_t)(i & 1));
+#pragma unroll
+      for (int c0 = h * SLICE; c0 < (h + 1) * SLICE; c0 += 32) {
+        const float* slab = scores + (c0 >> 5) * kSlabFloats;
         uint32_t v[32];
-        acc_cols(acc, c0, slabs, v);
+        slab_row(slab, v);
         uint32_t hit = 0;
 #pragma unroll
         for (int j4 = 0; j4 < 32; j4 += 4) {
-          const float4 c4 = *reinterpret_cast<const float4*>(&sh.cn[b][c0 + j4]);
+          const float4 c4 = *reinterpret_cast<const float4*>(&sh.cn[c0 + j4]);
           const float cc[4] = {c4.x, c4.y, c4.z, c4.w};
 #pragma unroll
           for (int u = 0; u < 4; u++) {
@@ -885,23 +994,74 @@ __global__ void __launch_bounds__(LT_NT, 1)
             hit |= (METRIC == kMetricL2 ? sc <= bound : sc >= bound) ? (1u << (j4 + u)) : 0u;
           }
         }
-        const float* srow = slabs + ((c0 >> 5) & 1) * kSlabFloats + tid * 32;  // this thread's row (acc_cols layout)
+        // Each lane walks its OWN hits, re-reading the dot product from the slab, so a warp iterates as often as
+        // its busiest lane and not once per column that any lane hit.
+        const float* srow = slab + r * 32;  // this thread's row (acc_to_slab layout)
         while (hit) {
           const int jj = __ffs(hit) - 1;
           hit &= hit - 1;
-          const float sc = tc_score<METRIC>(srow[(((jj >> 2) ^ (tid & 7)) << 2) | (jj & 3)], xn, sh.cn[b][c0 + jj]);
-          st = ck_consider<METRIC>(hk, k, sh.vid[b][c0 + jj], sc, st);
+          const float sc = tc_score<METRIC>(srow[(((jj >> 2) ^ (r & 7)) << 2) | (jj & 3)], xn, sh.cn[c0 + jj]);
+          const int col = ct * TC_N + c0 + jj;
+          st = ck_consider<METRIC, NSEL>(hk, k, col < nlist ? (uint32_t)col : kLmkNoVid, sc, st);
         }
         bound = key_bound<METRIC>(st.tau);
       }
-      if (valid) lmk_exchange_bound<METRIC>(tau_g + q, st, bound);  // with the other segments of this query
+      mbar_arrive(&sh.sempty);
+      if (valid) lmk_exchange_bound<METRIC>(tau_g + q, st, bound);  // with the query's other threads and CTAs
+      if (ct != ntc - 1 && w != w1 - 1) continue;
+
+      // ---- this CTA is done with query tile qt ----
+      for (int j = st.n; j < k; j++) hk[j * NSEL] = kKeySentinel;  // a set of fewer than k keys reads as k
+      const int first = ck_owner((int64_t)qt * ntc, W, G);
+      const int nown = ck_owner((int64_t)qt * ntc + ntc - 1, W, G) - first + 1;
+      const int slot = b - first;
+      // partial set (query tile, slot, h): k keys, key i of row r at [i][r]
+      auto part_at = [&](int s, int hh) { return part + (((int64_t)qt * nparts + s) * TPQ + hh) * k * TC_M + r; };
+      bool merge = true;
+      if (nown > 1) {
+        if (valid) {
+          unsigned long long* o = part_at(slot, h);
+          for (int j = 0; j < k; j++) o[(int64_t)j * TC_M] = hk[j * NSEL];
+        }
+        __threadfence();
+        ck_sel_sync<NSEL>();
+        if (sid == 0) sh.last = atomicAdd(cnt + qt, 1u) == (unsigned)(nown - 1);
+        ck_sel_sync<NSEL>();
+        merge = sh.last;  // the other CTAs of this tile have published theirs
+        if (merge) __threadfence();
+      }
+      if (!merge) continue;
+      // exact union of the sets: no borrowed bound from here on
+      st.tau = st.n == k ? hk[0] : kKeySentinel;
+      if (valid)
+        for (int s = 0; s < nown; s++)
+          if (s != slot) st = ck_absorb<NSEL>(hk, k, part_at(s, h), TC_M, st);
+      for (int j = st.n; j < k; j++) hk[j * NSEL] = kKeySentinel;
+      if (TPQ > 1) ck_sel_sync<NSEL>();  // the partner's set is complete
+      if (h == 0 && valid) {
+        for (int hh = 1; hh < TPQ; hh++)
+          for (int j = 0; j < k; j++) st = ck_insert<NSEL>(hk, k, hk[(j * NSEL) + hh * TC_M], st);
+        // ascending order: a set of k keys is a max-heap; a smaller one is heapified first
+        const int n = st.n;
+        if (n < k)
+          for (int j = n / 2 - 1; j >= 0; j--) ck_sift_down<NSEL>(hk, n, j, hk[j * NSEL]);
+        for (int m = n - 1; m > 0; m--) {
+          const unsigned long long top = hk[0];
+          ck_sift_down<NSEL>(hk, m, 0, hk[m * NSEL]);
+          hk[m * NSEL] = top;
+        }
+        unsigned long long* o = out + (int64_t)q * k;
+        for (int j = 0; j < k; j++) o[j] = j < n ? hk[j * NSEL] : kKeySentinel;
+      }
+      if (TPQ > 1) ck_sel_sync<NSEL>();  // the partner's set is read before its next tile refills it
     }
-    if (valid) lmk_write_keys(out + ((int64_t)q * nseg + sg) * k, hk, k, st.n);
-  } else {
-    // ======================= TMA producer =======================
-    ring_tma_produce(ring, sh.full, sh.empty, reinterpret_cast<const char*>(a_tiles) + (int64_t)qt * nk * LT_HALF,
-                     reinterpret_cast<const char*>(c_tiles) + (int64_t)ct0 * nk * LT_HALF, ntiles, nk);
   }
+}
+
+__global__ void coarse_init_kernel(unsigned long long* __restrict__ tau_g, int nq, unsigned int* __restrict__ cnt, int nqt) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nq) tau_g[i] = kKeySentinel;
+  if (i < nqt) cnt[i] = 0;
 }
 
 // ---- grouping for the fused kernel: histogram (lm_count_kernel) -> scan -> slots -> items ----
@@ -1288,31 +1448,67 @@ cudaError_t launch_tc_stage_rows(const float* x, int64_t ldx, int64_t n, int d, 
   return cudaGetLastError();
 }
 
-template <int METRIC>
+// the fused coarse quantiser's split: G CTAs (one per SM, at least CK_MIN_TILES tile pairs each) and the most CTAs
+// that share one query tile (its partial sets)
+struct CkGeometry {
+  int nqt, ntc, G, nparts;
+  int64_t W;
+};
+static CkGeometry ck_geometry(int nq, int nlist, int nsm) {
+  CkGeometry g;
+  g.nqt = (nq + TC_M - 1) / TC_M;
+  g.ntc = (nlist + TC_N - 1) / TC_N;
+  g.W = (int64_t)g.nqt * g.ntc;
+  g.G = (int)std::max<int64_t>(1, std::min<int64_t>(nsm, g.W / CK_MIN_TILES));
+  g.nparts = 1;
+  for (int qt = 0; qt < g.nqt; qt++) {
+    const int64_t w = (int64_t)qt * g.ntc;
+    g.nparts = std::max(g.nparts, ck_owner(w + g.ntc - 1, g.W, g.G) - ck_owner(w, g.W, g.G) + 1);
+  }
+  return g;
+}
+
+// workspace: tau_g[nq], the partial sets, cnt[nqt]
+static size_t ck_part_keys(const CkGeometry& g, int k) { return (size_t)g.nqt * g.nparts * ck_tpq(k) * k * TC_M; }
+
+size_t coarse_topk_workspace_bytes(int nq, int nlist, int k, int nsm) {
+  if (nq <= 0 || nlist <= 0 || k <= 0) return 0;
+  const CkGeometry g = ck_geometry(nq, nlist, nsm);
+  return ((size_t)nq + ck_part_keys(g, k)) * 8 + (size_t)g.nqt * 4;
+}
+
+template <int METRIC, int TPQ>
 static cudaError_t launch_coarse_topk_t(const float* a_tiles, const float* a_norms, int nq, const float* c_tiles,
-                                        const float* c_norms, int nlist, int k16, int seg_tiles, int nseg, int k,
-                                        unsigned long long* tau_g, unsigned long long* out, cudaStream_t st) {
-  const size_t smem = (size_t)LT_RING + kSlabBytes + (size_t)k * TC_NT * 8;
-  cudaError_t e = cudaFuncSetAttribute(coarse_topk_kernel<METRIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+                                        const float* c_norms, int nlist, int k16, int k, const CkGeometry& g, void* ws,
+                                        unsigned long long* out, cudaStream_t st) {
+  unsigned long long* tau_g = static_cast<unsigned long long*>(ws);
+  unsigned long long* part = tau_g + nq;
+  unsigned int* cnt = reinterpret_cast<unsigned int*>(part + ck_part_keys(g, k));
+  const int n = std::max(nq, g.nqt);
+  coarse_init_kernel<<<(n + 255) / 256, 256, 0, st>>>(tau_g, nq, cnt, g.nqt);
+  note_launch();
+  const size_t smem = (size_t)CK_NST * TC_STAGE_BYTES + CK_SCORE_BYTES + (size_t)k * TC_M * TPQ * 8;
+  cudaError_t e = cudaFuncSetAttribute(coarse_topk_kernel<METRIC, TPQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  const int64_t grid = (int64_t)((nq + TC_M - 1) / TC_M) * nseg;
-  coarse_topk_kernel<METRIC><<<(unsigned)grid, LT_NT, smem, st>>>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16,
-                                                                  seg_tiles, nseg, k, tau_g, out);
+  coarse_topk_kernel<METRIC, TPQ><<<g.G, ck_nt<TPQ>(), smem, st>>>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16, k,
+                                                                   g.nparts, tau_g, cnt, part, out);
   note_launch();
   return cudaGetLastError();
 }
 
 cudaError_t launch_coarse_topk(const float* a_tiles, const float* a_norms, int nq, const float* c_tiles, const float* c_norms,
-                               int nlist, int k16, int seg_tiles, int metric, int k, unsigned long long* tau_g,
-                               unsigned long long* out, cudaStream_t st) {
-  const int ntc = (nlist + TC_N - 1) / TC_N;
-  if (k <= 0 || k > kCoarseMaxK || k16 <= TC_BK || (k16 % TC_BK) || seg_tiles <= 0) return cudaErrorInvalidValue;
+                               int nlist, int k16, int metric, int k, int nsm, void* ws, unsigned long long* out,
+                               cudaStream_t st) {
+  if (k <= 0 || k > kCoarseMaxK || k16 <= TC_BK || (k16 % TC_BK) || nsm <= 0) return cudaErrorInvalidValue;
   if (nq <= 0 || nlist <= 0) return cudaSuccess;
-  const int nseg = (ntc + seg_tiles - 1) / seg_tiles;
-  if ((int64_t)((nq + TC_M - 1) / TC_M) * nseg > INT32_MAX) return cudaErrorInvalidValue;
+  const CkGeometry g = ck_geometry(nq, nlist, nsm);
+  if (ck_tpq(k) == 2)
+    return metric == kMetricL2
+               ? launch_coarse_topk_t<kMetricL2, 2>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16, k, g, ws, out, st)
+               : launch_coarse_topk_t<kMetricIP, 2>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16, k, g, ws, out, st);
   return metric == kMetricL2
-             ? launch_coarse_topk_t<kMetricL2>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16, seg_tiles, nseg, k, tau_g, out, st)
-             : launch_coarse_topk_t<kMetricIP>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16, seg_tiles, nseg, k, tau_g, out, st);
+             ? launch_coarse_topk_t<kMetricL2, 1>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16, k, g, ws, out, st)
+             : launch_coarse_topk_t<kMetricIP, 1>(a_tiles, a_norms, nq, c_tiles, c_norms, nlist, k16, k, g, ws, out, st);
 }
 
 template <int METRIC>
