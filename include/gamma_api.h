@@ -18,9 +18,10 @@
  * Scope of this build (DESIGN.md, INTEGRATION.md): full semantics for Init / Close / CreateTable /
  * AddOrUpdateDoc / DeleteDoc / GetDocByID / GetDocByDocID / BuildIndex / Search / Query /
  * GetEngineStatus / GetMemoryInfo / SetConfig / GetConfig / Dump / Load / SetKillStatus /
- * DeleteKillStatus / AddFieldIndexWithParams / RemoveFieldIndex / RebuildIndex for tables whose vector
- * fields are indexed as FLAT, IVFFLAT or IVFPQ (optionally with OPQ); Backup returns kNotSupported,
- * SetMemoryLimitConfig is a no-op (vectors live in HBM).
+ * DeleteKillStatus / AddFieldIndexWithParams / RemoveFieldIndex / RebuildIndex / SetMemoryLimitConfig for
+ * tables whose vector fields are indexed as FLAT, IVFFLAT or IVFPQ (optionally with OPQ); Backup returns
+ * kNotSupported.  SetMemoryLimitConfig(p) limits what this library holds to p % of each device's HBM and of host
+ * memory (0: no limit): past it AddOrUpdateDoc refuses new documents with -5 and Search / Query return code 8.
  */
 #ifndef GAMMA_API_H_
 #define GAMMA_API_H_
@@ -76,7 +77,8 @@ struct CStatus AddFieldIndexWithParams(void *engine, const char *field_name, int
                                        const char *index_type, int index_type_len, const char *index_params,
                                        int index_params_len);
 struct CStatus RemoveFieldIndex(void *engine, const char *field_name, int field_name_len);
-/* gamma_api.cc:352-374 */
+/* gamma_api.cc:352-374.  memory_limit: percent of each device's total HBM and of host memory this process's library
+ * allocations may hold (DESIGN.md section 8); 0 removes the limit */
 void SetMemoryLimitConfig(int memory_limit);
 void SetKillStatus(const char *request_id, int partition_id, int reason);
 void DeleteKillStatus(const char *request_id, int partition_id);

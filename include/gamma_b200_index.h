@@ -248,6 +248,14 @@ int gb_debug_dist_matrix(int device, const float *x, int n, const float *c, int 
  * since the last reset (after the device's pending work); reset_peak != 0 then restarts the mark at the current use */
 int gb_device_pool_usage(int device, int reset_peak, int64_t *used, int64_t *peak);
 
+/* the memory ledger behind SetMemoryLimitConfig (DESIGN.md section 8), device >= 0 or -1 for the host: *usage = the bytes
+ * this library holds there (on a device: tracked allocations + the reserved bytes of its default pool),
+ * *pool_reserved = that pool's part, *limit = the limit in bytes (0: none); any pointer may be NULL */
+int gb_memory_ledger(int device, int64_t *usage, int64_t *pool_reserved, int64_t *limit);
+/* test hook: the total memory SetMemoryLimitConfig's percentage applies to on a device (-1: the host) becomes `bytes`;
+ * 0 restores the real one (cudaDeviceProp::totalGlobalMem; the host's MemTotal or cgroup v1 limit) */
+void gb_memory_set_total(int device, int64_t bytes);
+
 /* ---- host-logic test hooks: run the C++ wire codecs of the gamma boundary without a GPU ---- */
 /* RequestConcurrentController (search/engine.cc:47-119): op 0 threshold, 1 in-flight, 2 set threshold (<= 0: system value),
  * 3 Acquire(value) -> 1/0, 4 Release(value) */

@@ -125,6 +125,9 @@ def _declare(l):
     l.gb_kmeans.argtypes = [i32, vp, i64, i32, i32, i32, i64, i32, i32, vp, vp]
     l.gb_kmeans_update.argtypes = [i32, vp, i64, i32, i32, vp, vp]
     l.gb_device_pool_usage.argtypes = [i32, i32, C.POINTER(i64), C.POINTER(i64)]
+    l.gb_memory_ledger.argtypes = [i32, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64)]
+    l.gb_memory_set_total.restype = None
+    l.gb_memory_set_total.argtypes = [i32, i64]
     l.gb_merge_partitions_device.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, vp]
 
 

@@ -427,6 +427,29 @@ int Engine::flush_pending_locked() {
   return 0;
 }
 
+void Engine::memory_places(std::vector<mem::Charge>* out, int64_t bytes) const {
+  out->push_back({device_, bytes});
+  for (int d : devices_)
+    if (d != device_) out->push_back({d, bytes});
+  bool host = index_ && index_->store().on_host();
+  for (auto& e : extra_) host = host || e.index->store().on_host();
+  if (host) out->push_back({mem::kHost, bytes});
+}
+bool Engine::rows_admitted(int64_t n_total) {
+  if (!mem::limited()) return true;
+  std::vector<mem::Charge> c;
+  memory_places(&c, 0);  // nothing to grow still needs usage within the limit
+  index_->memory_charges(n_total, &c);
+  for (auto& e : extra_) e.index->memory_charges(n_total, &c);
+  return mem::admit(c);
+}
+bool Engine::request_admitted(int64_t bytes) const {
+  if (!mem::limited()) return true;
+  std::vector<mem::Charge> c;
+  memory_places(&c, bytes);
+  return mem::admit(c);
+}
+
 // Engine::AddOrUpdate (search/engine.cc:691-772) + Doc::Deserialize (doc.cc:43-76)
 int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
   if (!created_table_) return -1;
@@ -495,6 +518,9 @@ int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
   for (size_t ei = 0; ei < extra_.size(); ei++)
     if (!evec[ei].first || evec[ei].second != (size_t)extra_[ei].dim * 4) return -3;
   if (key.empty()) return -3;
+  // VectorManager::AddToStore fails when the raw vectors' next segment would pass the memory limit
+  // (memory_raw_vector.cc:165-185): the document is refused before anything of it is stored
+  if (!rows_admitted((int64_t)max_docid_ + 1)) return -5;
   for (size_t fi = 0; fi < fields_.size(); fi++) values_[fi].emplace_back();
   for (auto& f : table_fields) values_[field_idx_[f.name]][max_docid_] = f.value;
   values_[field_idx_["_id"]][max_docid_] = key;

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "index.h"
+#include "mem_ledger.h"
 #include "scalar_index.h"
 
 namespace gb {
@@ -134,6 +135,8 @@ class Engine {
   // Engine::AddFieldIndex / RemoveFieldIndex (search/engine.cc:1471-1600): build the field's device columns over the
   // documents already stored, or free them
   Status SetFieldIndexed(const std::string& field, bool indexed);
+  // whether a Search / Query request of `bytes` fits the memory limit (mem_ledger.h) on every place the table uses
+  bool request_admitted(int64_t bytes) const;
 
   // cooperative cancellation (c_api/api_data/request_context.h:51-88)
   static void SetKill(const std::string& request_id, int partition_id, int reason);
@@ -145,6 +148,11 @@ class Engine {
   void indexing_loop();
   void serialize_doc(int docid, bool with_docid, std::string* out);
   int doc_num() const { return max_docid_ - delete_num_; }
+  // whether the vector fields may grow to n_total rows under the memory limit: the stores' growth and the index bytes
+  // of the rows it makes room for
+  bool rows_admitted(int64_t n_total);
+  // a charge of `bytes` on every place the table keeps memory: its devices, and the host when a field is stored there
+  void memory_places(std::vector<mem::Charge>* out, int64_t bytes) const;
 
   std::string path_, space_name_;
   int device_;

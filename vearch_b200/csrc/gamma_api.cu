@@ -165,6 +165,11 @@ struct CStatus Search(void* engine, const char* request_str, int req_len, char**
     to_cstatus(gb::Status::Make(gb::kInvalidArgument, "null engine"), &c);
     return c;
   }
+  // gamma_api.cc:179-185: refused while usage + the request passes the memory limit, before admission control
+  if (!static_cast<Engine*>(engine)->request_admitted(req_len)) {
+    to_cstatus(gb::Status::Make(gb::kMemoryExceeded, ""), &c);
+    return c;
+  }
   gb::SearchRequestPB req;
   if (!req.parse(reinterpret_cast<const uint8_t*>(request_str), (size_t)req_len)) {
     to_cstatus(gb::Status::Make(gb::kInvalidArgument, "parse search request failed"), &c);
@@ -181,6 +186,10 @@ struct CStatus Query(void* engine, const char* request_str, int req_len, char** 
   struct CStatus c;
   if (!engine) {
     to_cstatus(gb::Status::Make(gb::kInvalidArgument, "null engine"), &c);
+    return c;
+  }
+  if (!static_cast<Engine*>(engine)->request_admitted(req_len)) {  // gamma_api.cc:205-211
+    to_cstatus(gb::Status::Make(gb::kMemoryExceeded, ""), &c);
     return c;
   }
   gb::QueryRequestPB req;
@@ -232,7 +241,9 @@ struct CStatus RemoveFieldIndex(void* engine, const char* field_name, int field_
   return c;
 }
 
-void SetMemoryLimitConfig(int) {}  // host-RSS watchdog (memory/memoryManager.cc): not applicable, vectors live in HBM
+// MemoryManager's limit (memory/memoryManager.cc:17-26): memory_limit % of each device's HBM and of host memory, over
+// what this library holds (mem_ledger.h); 0 removes it
+void SetMemoryLimitConfig(int memory_limit) { gb::mem::set_limit_percent(memory_limit); }
 
 void SetKillStatus(const char* request_id, int partition_id, int reason) {
   if (request_id) Engine::SetKill(request_id, partition_id, reason);
@@ -271,6 +282,15 @@ int gb_debug_concurrency(int op, int value) {
   }
   return -1;
 }
+
+int gb_memory_ledger(int device, int64_t* usage, int64_t* pool_reserved, int64_t* limit) {
+  if (usage) *usage = gb::mem::usage(device);
+  if (pool_reserved) *pool_reserved = device >= 0 ? gb::mem::pool_reserved(device) : 0;
+  if (limit) *limit = gb::mem::limit(device);
+  return 0;
+}
+
+void gb_memory_set_total(int device, int64_t bytes) { gb::mem::set_total(device, bytes); }
 
 int gb_debug_parse_search_request(const char* buf, int len, char** json_out, int* out_len) {
   gb::SearchRequestPB r;

@@ -11,6 +11,7 @@
 #include <random>
 
 #include "common.cuh"
+#include "mem_ledger.h"
 
 namespace gb {
 
@@ -109,33 +110,56 @@ const VmmApi& vmm_api() {
   }();
   return api;
 }
+// the VMM allocation granularity on a device; 0 without VMM
+size_t vmm_granularity(int device) {
+  static std::atomic<size_t> cache[64];
+  if (device >= 0 && device < 64 && cache[device].load()) return cache[device].load();
+  const VmmApi& api = vmm_api();
+  if (!api.ok) return 0;
+  CUmemAllocationProp prop = {};
+  prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  prop.location.id = device;
+  size_t gran = 0;
+  if (api.granularity(&gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM) != CUDA_SUCCESS) return 0;
+  if (device >= 0 && device < 64) cache[device] = gran;
+  return gran;
+}
+// the next chunk mapped into a segment with `mapped` of va_bytes mapped and `need` wanted: geometric steps (a quarter of
+// what is mapped, at least one granule, at most 256 MiB), never past the segment
+size_t map_step(size_t mapped, size_t need, size_t gran, size_t va_bytes) {
+  size_t step = std::max(gran, std::min<size_t>(mapped / 4, (size_t)256 << 20));
+  step = (size_t)round_up((int64_t)std::max(step, std::min(need - mapped, (size_t)256 << 20)), (int64_t)gran);
+  return std::min(step, va_bytes - mapped);
+}
 }  // namespace
 
 RawStore::RawStore(int row_bytes, int seg_shift, bool host)
     : row_bytes_(row_bytes), stride_((int)round_up(row_bytes, 16)), seg_shift_(host ? std::min(seg_shift, kHostSegShift) : seg_shift), host_(host) {
-  cudaMalloc(&d_segs_, sizeof(float*) * kMaxSegs);
+  mem::dev_malloc(&d_segs_, sizeof(float*) * kMaxSegs);
   cudaGetDevice(&device_);
 }
 RawStore::~RawStore() {
   const VmmApi& api = vmm_api();
   for (Seg& sg : segs_) {
     if (host_) {
-      cudaFreeHost(sg.base);
+      mem::host_free(sg.base);
       continue;
     }
     if (!sg.vmm) {
-      cudaFree(sg.base);
+      mem::dev_free(sg.base);
       continue;
     }
     size_t off = 0;
     for (auto& c : sg.chunks) {
       api.unmap((CUdeviceptr)sg.base + off, c.second);
       api.release(c.first);
+      mem::charge(device_, -(int64_t)c.second);
       off += c.second;
     }
     api.addr_free((CUdeviceptr)sg.base, sg.va_bytes);
   }
-  cudaFree(d_segs_);
+  mem::dev_free(d_segs_);
 }
 int RawStore::new_segment() {
   if ((int)segs_.size() >= kMaxSegs) {
@@ -145,12 +169,12 @@ int RawStore::new_segment() {
   Seg sg;
   const size_t bytes = (size_t)seg_rows() * stride_;
   if (host_) {  // pinned, mapped into every device's address space; kernels read it through the device pointer
-    GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&sg.base), bytes, cudaHostAllocMapped | cudaHostAllocPortable));
+    GB_CUDA(mem::host_alloc(reinterpret_cast<void**>(&sg.base), bytes, cudaHostAllocMapped | cudaHostAllocPortable));
     memset(sg.base, 0, bytes);  // pad columns must read as zero
     unsigned char* dev = nullptr;
     const cudaError_t e = cudaHostGetDevicePointer(reinterpret_cast<void**>(&dev), sg.base, 0);
     if (e != cudaSuccess) {
-      cudaFreeHost(sg.base);
+      mem::host_free(sg.base);
       set_last_error(std::string("raw store: cudaHostGetDevicePointer: ") + cudaGetErrorString(e));
       return -1;
     }
@@ -162,12 +186,8 @@ int RawStore::new_segment() {
   }
   const VmmApi& api = vmm_api();
   if (api.ok) {
-    CUmemAllocationProp prop = {};
-    prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
-    prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-    prop.location.id = device_;
-    size_t gran = 0;
-    if (api.granularity(&gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM) == CUDA_SUCCESS && gran > 0) {
+    const size_t gran = vmm_granularity(device_);
+    if (gran > 0) {
       sg.gran = gran;
       sg.va_bytes = (size_t)round_up((int64_t)bytes, (int64_t)gran);
       CUdeviceptr p = 0;
@@ -178,7 +198,7 @@ int RawStore::new_segment() {
     }
   }
   if (!sg.vmm) {  // no VMM: the whole segment at once
-    GB_CUDA(cudaMalloc(&sg.base, bytes));
+    GB_CUDA(mem::dev_malloc(&sg.base, bytes));
     GB_CUDA(cudaMemset(sg.base, 0, bytes));
     sg.mapped = bytes;
     phys_bytes_ += (int64_t)bytes;
@@ -194,10 +214,7 @@ int RawStore::map_rows(int si, int64_t rows) {
   if (need <= sg.mapped) return 0;
   const VmmApi& api = vmm_api();
   while (sg.mapped < need) {
-    // geometric steps (a quarter of what is mapped, at least one granule, at most 256 MiB), never past the segment
-    size_t step = std::max(sg.gran, std::min<size_t>(sg.mapped / 4, (size_t)256 << 20));
-    step = (size_t)round_up((int64_t)std::max(step, std::min(need - sg.mapped, (size_t)256 << 20)), (int64_t)sg.gran);
-    step = std::min(step, sg.va_bytes - sg.mapped);
+    const size_t step = map_step(sg.mapped, need, sg.gran, sg.va_bytes);
     CUmemAllocationProp prop = {};
     prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
     prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
@@ -218,6 +235,7 @@ int RawStore::map_rows(int si, int64_t rows) {
     }
     GB_CUDA(cudaMemset(reinterpret_cast<void*>(at), 0, step));  // pad columns must read as zero
     sg.chunks.emplace_back(hnd, step);
+    mem::charge(device_, (int64_t)step);
     sg.mapped += step;
     phys_bytes_ += (int64_t)step;
   }
@@ -231,6 +249,30 @@ int RawStore::ensure(int64_t n_total) {
     if (rows > 0 && map_rows(si, rows)) return -1;
   }
   return 0;
+}
+int64_t RawStore::growth_bytes(int64_t n_total, int64_t* rows) const {
+  const size_t seg_bytes = (size_t)seg_rows() * stride_;
+  const size_t gran = host_ ? 0 : vmm_granularity(device_);
+  int64_t b = 0;
+  for (int64_t si = n_ >> seg_shift_; si * seg_rows() < n_total; si++) {
+    const size_t need = (size_t)std::min<int64_t>(seg_rows(), n_total - si * seg_rows()) * stride_;
+    const bool exists = si < (int64_t)segs_.size();
+    if (exists ? !segs_[si].vmm : (host_ || !gran)) {  // a whole segment at once, or already there
+      if (!exists) b += (int64_t)seg_bytes;
+      continue;
+    }
+    size_t mapped = exists ? segs_[si].mapped : 0;
+    const size_t sg_gran = exists ? segs_[si].gran : gran;
+    const size_t va = exists ? segs_[si].va_bytes : (size_t)round_up((int64_t)seg_bytes, (int64_t)gran);
+    while (mapped < need) {
+      const size_t step = map_step(mapped, need, sg_gran, va);
+      mapped += step;
+      b += (int64_t)step;
+    }
+  }
+  if (rows) *rows = b / stride_;
+  if (shadow_) b += shadow_->growth_bytes(n_total, nullptr);
+  return b;
 }
 // Host placement: the segments are ordinary (pinned) host memory, so host rows move with memcpy and device rows with
 // device-to-host copies.  A search may still be reading a row when update_host overwrites it: the caller holds the
@@ -362,18 +404,18 @@ IvfLists::IvfLists(int nlist, int code_bytes) : nlist_(nlist), code_bytes_(code_
   h_len_.assign(nlist, 0);
   h_cap_.assign(nlist, 0);
   h_dead_.assign(nlist, 0);
-  cudaMalloc(&d_data_, sizeof(void*) * nlist);
-  cudaMalloc(&d_ids_, sizeof(int64_t*) * nlist);
-  cudaMalloc(&d_len_, sizeof(int) * nlist);
+  mem::dev_malloc(&d_data_, sizeof(void*) * nlist);
+  mem::dev_malloc(&d_ids_, sizeof(int64_t*) * nlist);
+  mem::dev_malloc(&d_len_, sizeof(int) * nlist);
   cudaMemset(d_data_, 0, sizeof(void*) * nlist);
   cudaMemset(d_ids_, 0, sizeof(int64_t*) * nlist);
   cudaMemset(d_len_, 0, sizeof(int) * nlist);
 }
 IvfLists::~IvfLists() {
-  for (void* p : slabs_) cudaFree(p);
-  cudaFree(d_data_);
-  cudaFree(d_ids_);
-  cudaFree(d_len_);
+  for (void* p : slabs_) mem::dev_free(p);
+  mem::dev_free(d_data_);
+  mem::dev_free(d_ids_);
+  mem::dev_free(d_len_);
 }
 ListDirectory IvfLists::directory() const {
   ListDirectory dir;
@@ -396,7 +438,7 @@ int IvfLists::slab_reserve(size_t need_bytes) {
   if (need_bytes <= slab_left_) return 0;
   size_t slab = std::max<size_t>(need_bytes, (size_t)64 << 20);
   void* p = nullptr;
-  GB_CUDA(cudaMalloc(&p, slab));
+  GB_CUDA(mem::dev_malloc(&p, slab));
   slabs_.push_back(p);
   slab_cur_ = static_cast<char*>(p);
   slab_left_ = slab;
@@ -466,7 +508,7 @@ int IvfLists::compact(cudaStream_t st) {
   const int64_t need = packed_bytes();
   if (need == 0 || slabs_.empty()) return 0;
   void* slab = nullptr;
-  if (cudaMalloc(&slab, (size_t)need) != cudaSuccess) {
+  if (mem::dev_malloc(&slab, (size_t)need) != cudaSuccess) {
     cudaGetLastError();
     return 0;  // not enough room to re-pack: keep the current layout
   }
@@ -488,7 +530,7 @@ int IvfLists::compact(cudaStream_t st) {
   GB_CUDA(cudaMemcpyAsync(d_data_, h_data_.data(), sizeof(void*) * nlist_, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemcpyAsync(d_ids_, h_ids_.data(), sizeof(int64_t*) * nlist_, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaDeviceSynchronize());  // copies done, and no kernel of an earlier search still reads the old slabs
-  for (void* p : slabs_) cudaFree(p);
+  for (void* p : slabs_) mem::dev_free(p);
   slabs_.assign(1, slab);
   slab_cur_ = nullptr;
   slab_left_ = 0;
@@ -615,6 +657,12 @@ LiveIndexes& live_indexes() {
   static LiveIndexes* s = new LiveIndexes;  // leaked on purpose: must outlive every static destructor
   return *s;
 }
+// the memory limit's trim: the idle scan scratch of every index on the device
+void release_idle_scratch_on(int device) {
+  std::lock_guard<std::mutex> g(live_indexes().mu);
+  for (Index* i : live_indexes().all)
+    if (i->device() == device) i->release_idle_scratch();
+}
 void quiesce_all_indexes() {
   std::vector<Index*> v;
   {
@@ -628,14 +676,10 @@ void quiesce_all_indexes() {
 Index::Index(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int row_bytes)
     : type_(type), gpu_contract_(is_gpu_index_type(type)), d_(d), dpad_((int)round_up(d, 4)), device_(device), mp_(mp) {
   cudaSetDevice(device_);
-  cudaMemPool_t pool;
-  if (cudaDeviceGetDefaultMemPool(&pool, device_) == cudaSuccess) {
-    uint64_t thr = UINT64_MAX;  // keep scratch memory cached between searches
-    cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
-  }
+  mem::configure_pool(device_);
   {  // the CUDA runtime is initialised by now, so this hook runs before its teardown
     std::lock_guard<std::mutex> g(live_indexes().mu);
-    static bool hooked = (atexit(quiesce_all_indexes), true);
+    static bool hooked = (atexit(quiesce_all_indexes), mem::set_scratch_release(release_idle_scratch_on), true);
     (void)hooked;
     live_indexes().all.push_back(this);
   }
@@ -660,7 +704,7 @@ Index::~Index() {
   }
   quiesce();
   for (auto& b : big_) {
-    cudaFree(b.p);
+    mem::dev_free(b.p);
     cudaEventDestroy(b.done);
   }
   if (build_stream_) cudaStreamDestroy(build_stream_);
@@ -671,22 +715,13 @@ void* Index::big_acquire(size_t bytes, cudaStream_t st) {
   for (size_t i = 0; i < big_.size(); i++)
     if (!big_[i].busy && big_[i].cap >= bytes && (best < 0 || big_[i].cap < big_[best].cap)) best = (int)i;
   if (best < 0) {
-    for (size_t i = 0; i < big_.size();) {  // drop idle buffers that are too small before growing
-      if (!big_[i].busy) {
-        cudaEventSynchronize(big_[i].done);
-        cudaFree(big_[i].p);
-        cudaEventDestroy(big_[i].done);
-        big_.erase(big_.begin() + i);
-      } else {
-        i++;
-      }
-    }
+    free_idle_big_locked();  // drop idle buffers that are too small before growing
     BigBuf b;
     b.cap = bytes + bytes / 4;
     b.busy = false;
-    if (cudaMalloc(&b.p, b.cap) != cudaSuccess) {
+    if (mem::dev_malloc(&b.p, b.cap) != cudaSuccess) {
       b.cap = bytes;
-      if (cudaMalloc(&b.p, b.cap) != cudaSuccess) {
+      if (mem::dev_malloc(&b.p, b.cap) != cudaSuccess) {
         set_last_error("cudaMalloc(" + std::to_string(bytes) + ") failed for scan scratch");
         return nullptr;
       }
@@ -699,6 +734,38 @@ void* Index::big_acquire(size_t bytes, cudaStream_t st) {
   big_[best].busy = true;
   cudaStreamWaitEvent(st, big_[best].done, 0);  // previous user's kernels (possibly on another stream)
   return big_[best].p;
+}
+void Index::free_idle_big_locked() {
+  for (size_t i = 0; i < big_.size();) {
+    if (!big_[i].busy) {
+      cudaEventSynchronize(big_[i].done);
+      mem::dev_free(big_[i].p);
+      cudaEventDestroy(big_[i].done);
+      big_.erase(big_.begin() + i);
+    } else {
+      i++;
+    }
+  }
+}
+void Index::release_idle_scratch() {
+  std::lock_guard<std::mutex> g(big_mu_);
+  free_idle_big_locked();
+}
+void Index::memory_charges(int64_t n_total, std::vector<mem::Charge>* out) {
+  int64_t rows = 0;
+  const int64_t grow = store_->growth_bytes(n_total, &rows);
+  if (grow == 0) return;
+  out->push_back({store_->on_host() ? mem::kHost : device_, grow});
+  charge_index_rows(rows, out);
+}
+void IvfIndex::charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) {
+  out->push_back({device_, rows * (code_bytes() + 8)});
+}
+void IVFFlatIndex::charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) {
+  IvfIndex::charge_index_rows(rows, out);
+  std::shared_lock<std::shared_mutex> lk(mirror_rw_);
+  if (mirror_.base)  // a tile of 128 rows and their norms
+    out->push_back({device_, rows * (int64_t)((size_t)tc_mirror_tile_floats((int)round_up(dpad_, 16)) * 4 + 512) / 128});
 }
 void Index::big_release(void* p, cudaStream_t st) {
   std::lock_guard<std::mutex> g(big_mu_);
@@ -1370,32 +1437,32 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
 // ------------------------------------------------------------------------------------------
 IvfIndex::IvfIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int row_bytes)
     : Index(type, d, mp, device, seg_shift, row_bytes), nlist_(mp.ncentroids) {
-  cudaMalloc(&d_centroids_, (size_t)nlist_ * dpad_ * 4);
+  mem::dev_malloc(&d_centroids_, (size_t)nlist_ * dpad_ * 4);
   cudaMemset(d_centroids_, 0, (size_t)nlist_ * dpad_ * 4);
   const int64_t ctiles = (nlist_ + 127) / 128;
-  cudaMalloc(&d_cent_tiles_, (size_t)ctiles * tc_mirror_tile_floats((int)round_up(dpad_, 16)) * 4);
-  cudaMalloc(&d_cent_norms_, (size_t)ctiles * 128 * 4);
+  mem::dev_malloc(&d_cent_tiles_, (size_t)ctiles * tc_mirror_tile_floats((int)round_up(dpad_, 16)) * 4);
+  mem::dev_malloc(&d_cent_norms_, (size_t)ctiles * 128 * 4);
   rebuild_centroid_tiles(0);
   cudaStreamSynchronize(0);
 }
 IvfIndex::~IvfIndex() {
-  cudaFree(d_centroids_);
-  cudaFree(d_cent_tiles_);
-  cudaFree(d_cent_norms_);
+  mem::dev_free(d_centroids_);
+  mem::dev_free(d_cent_tiles_);
+  mem::dev_free(d_cent_norms_);
 }
 IVFFlatIndex::IVFFlatIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift)
     : IvfIndex(type, d, mp, device, seg_shift) {
   if (metric() == kMetricL2) {  // inner products are scanned unshifted: no table
-    cudaMalloc(&d_shifts_, (size_t)nlist_ * dpad_ * 4);
+    mem::dev_malloc(&d_shifts_, (size_t)nlist_ * dpad_ * 4);
     cudaMemset(d_shifts_, 0, (size_t)nlist_ * dpad_ * 4);  // = the zero centroids of an untrained index
   }
 }
 IVFFlatIndex::~IVFFlatIndex() {
-  if (d_shifts_) cudaFree(d_shifts_);
-  if (mirror_.base) cudaFree(mirror_.base);
-  if (mirror_.norms) cudaFree(mirror_.norms);
-  if (mirror_.d_tile0) cudaFree(mirror_.d_tile0);
-  if (d_rowptr_) cudaFree(d_rowptr_);
+  if (d_shifts_) mem::dev_free(d_shifts_);
+  if (mirror_.base) mem::dev_free(mirror_.base);
+  if (mirror_.norms) mem::dev_free(mirror_.norms);
+  if (mirror_.d_tile0) mem::dev_free(mirror_.d_tile0);
+  if (d_rowptr_) mem::dev_free(d_rowptr_);
 }
 int IvfIndex::rebuild_centroid_tiles(cudaStream_t st) {
   GB_CUDA(launch_tc_stage_rows(d_centroids_, dpad_, nlist_, dpad_, (int)round_up(dpad_, 16), d_cent_tiles_, d_cent_norms_, st));
@@ -1643,9 +1710,9 @@ int IVFFlatIndex::lists_changed(cudaStream_t st) {
   if (need > rowptr_cap_) {
     const int64_t cap = std::max<int64_t>(need, rowptr_cap_ + rowptr_cap_ / 2);
     const float** p = nullptr;
-    GB_CUDA(cudaMalloc(&p, (size_t)cap * sizeof(float*)));
+    GB_CUDA(mem::dev_malloc(&p, (size_t)cap * sizeof(float*)));
     GB_CUDA(cudaMemsetAsync(p, 0, (size_t)cap * sizeof(float*), st));
-    if (d_rowptr_) GB_CUDA(cudaFree(d_rowptr_));
+    mem::dev_free(d_rowptr_);
     d_rowptr_ = p;
     rowptr_cap_ = cap;
   }
@@ -1871,8 +1938,8 @@ int IVFFlatIndex::ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStr
       const int k16 = (int)round_up(dpad_, 16);
       const size_t tile_bytes = (size_t)tc_mirror_tile_floats(k16) * 4;
       cudaDeviceSynchronize();  // kernels of other searches may still be reading the mirror
-      if (mirror_.base) cudaFree(mirror_.base);
-      if (mirror_.norms) cudaFree(mirror_.norms);
+      if (mirror_.base) mem::dev_free(mirror_.base);
+      if (mirror_.norms) mem::dev_free(mirror_.norms);
       mirror_.base = mirror_.norms = nullptr;
       mirror_.cap_tiles = 0;
       size_t free_b = 0, total_b = 0;
@@ -1889,9 +1956,9 @@ int IVFFlatIndex::ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStr
         tiles = tile0[nlist_];
         const size_t need = (size_t)std::max<int64_t>(tiles, 1) * (tile_bytes + 512);
         if (need + ((size_t)4 << 30) > free_b) continue;
-        if (cudaMalloc(&mirror_.base, (size_t)std::max<int64_t>(tiles, 1) * tile_bytes) != cudaSuccess ||
-            cudaMalloc(&mirror_.norms, (size_t)std::max<int64_t>(tiles, 1) * 512) != cudaSuccess) {
-          if (mirror_.base) cudaFree(mirror_.base);
+        if (mem::dev_malloc(&mirror_.base, (size_t)std::max<int64_t>(tiles, 1) * tile_bytes) != cudaSuccess ||
+            mem::dev_malloc(&mirror_.norms, (size_t)std::max<int64_t>(tiles, 1) * 512) != cudaSuccess) {
+          if (mirror_.base) mem::dev_free(mirror_.base);
           mirror_.base = nullptr;
           cudaGetLastError();
         }
@@ -1903,7 +1970,7 @@ int IVFFlatIndex::ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStr
         mirror_.list_tiles = list_tiles;
       }
       if (!mirror_.disabled) {
-        if (!mirror_.d_tile0 && cudaMalloc(&mirror_.d_tile0, sizeof(int64_t) * (nlist_ + 1)) != cudaSuccess) return -1;
+        if (!mirror_.d_tile0 && mem::dev_malloc(&mirror_.d_tile0, sizeof(int64_t) * (nlist_ + 1)) != cudaSuccess) return -1;
         GB_CUDA(cudaMemcpyAsync(mirror_.d_tile0, tile0.data(), sizeof(int64_t) * (nlist_ + 1), cudaMemcpyHostToDevice, st));
         GB_CUDA(launch_tc_mirror_build(lists_->directory(), dpad_, k16, mirror_.d_tile0, tiles,
                                        d_shifts_, mirror_.base, mirror_.norms, st));
@@ -2143,10 +2210,10 @@ int IvfIndex::search_preassigned_host(const SearchContext& ctx, int nq, const vo
 // ------------------------------------------------------------------------------------------
 IvfPqBase::IvfPqBase(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int M, int ksub)
     : IvfIndex(type, d, mp, device, seg_shift), M_(M), dsub_(d / M), ksub_(ksub) {
-  cudaMalloc(&d_pq_, (size_t)M_ * ksub_ * dsub_ * 4);
+  mem::dev_malloc(&d_pq_, (size_t)M_ * ksub_ * dsub_ * 4);
   cudaMemset(d_pq_, 0, (size_t)M_ * ksub_ * dsub_ * 4);
 }
-IvfPqBase::~IvfPqBase() { cudaFree(d_pq_); }
+IvfPqBase::~IvfPqBase() { mem::dev_free(d_pq_); }
 int64_t IvfPqBase::index_mem_bytes() const { return IvfIndex::index_mem_bytes() + (int64_t)M_ * ksub_ * dsub_ * 4; }
 int IvfPqBase::set_pq_centroids(const float* host) {
   cudaSetDevice(device_);
@@ -2220,7 +2287,7 @@ IVFPQIndex::IVFPQIndex(const std::string& type, int d, const ModelParams& mp, in
       nbits_(mp.nbits) {
   if (!gpu_contract_) store_->enable_shadow();  // GPU_IVFPQ never re-ranks
   if (mp.opq_nsubvector > 0) {  // faiss::OPQMatrix(d, opq_nsubvector, d) (gamma_index_ivfpq.cc:168-178)
-    cudaMalloc(&d_opq_, (size_t)d * dpad_ * 4);
+    mem::dev_malloc(&d_opq_, (size_t)d * dpad_ * 4);
     cudaMemset(d_opq_, 0, (size_t)d * dpad_ * 4);
   }
 }
@@ -2414,12 +2481,12 @@ const float* IVFPQIndex::train_transform(const float* xt, int64_t n_in, Scratch&
 }
 
 IVFPQIndex::~IVFPQIndex() {
-  if (d_opq_) cudaFree(d_opq_);
-  cudaFree(d_table_);
-  cudaFree(d_cb8_);
-  cudaFree(d_cbnrm_);
-  if (pqn_.base) cudaFree(pqn_.base);
-  if (pqn_.d_off) cudaFree(pqn_.d_off);
+  if (d_opq_) mem::dev_free(d_opq_);
+  mem::dev_free(d_table_);
+  mem::dev_free(d_cb8_);
+  mem::dev_free(d_cbnrm_);
+  if (pqn_.base) mem::dev_free(pqn_.base);
+  if (pqn_.d_off) mem::dev_free(pqn_.d_off);
 }
 // gamma_index_ivfpq.cc:139-144; GPU_IVFPQ: ncentroids * max_points_per_centroid (gamma_index_ivfpq_gpu.cc:208-212)
 int64_t IVFPQIndex::default_training_threshold() const {
@@ -2440,12 +2507,12 @@ int IVFPQIndex::codebook_changed(cudaStream_t st) {
   // tables of the tensor-core filter (kernels_pqtc.cu): int8 codebook (one scale sb), centroid norms, and the bounds on
   // |r| and on its quantisation error that its error margin uses
   if (ksub_ == 256 && pqtc_supported(M_, dsub_)) {
-    if (!d_cb8_) GB_CUDA(cudaMalloc(&d_cb8_, (size_t)M_ * 256 * dsub_));
-    if (!d_cbnrm_) GB_CUDA(cudaMalloc(&d_cbnrm_, ((size_t)M_ * 256 + 4) * 4));
+    if (!d_cb8_) GB_CUDA(mem::dev_malloc(&d_cb8_, (size_t)M_ * 256 * dsub_));
+    if (!d_cbnrm_) GB_CUDA(mem::dev_malloc(&d_cbnrm_, ((size_t)M_ * 256 + 4) * 4));
     GB_CUDA(launch_pqtc_tables(d_pq_, M_, dsub_, d_cb8_, d_cbnrm_, d_cbnrm_ + (size_t)M_ * 256, st));
   }
   if (mp_.metric != kMetricL2) return 0;  // IP: tab = ip table, dis0 = <x, centroid>
-  if (!d_table_) GB_CUDA(cudaMalloc(&d_table_, (size_t)nlist_ * M_ * ksub_ * 4));
+  if (!d_table_) GB_CUDA(mem::dev_malloc(&d_table_, (size_t)nlist_ * M_ * ksub_ * 4));
   GB_CUDA(launch_pq_precompute_table(d_centroids_, dpad_, nlist_, d_pq_, M_, dsub_, d_table_, st, ksub_));
   return 0;
 }
@@ -2507,18 +2574,18 @@ int IVFPQIndex::ensure_pq_norms(cudaStream_t st) {
   if (total > pqn_.cap) {
     if (pqn_.base) {
       cudaDeviceSynchronize();
-      cudaFree(pqn_.base);
+      mem::dev_free(pqn_.base);
       pqn_.base = nullptr;
     }
     const size_t cap = total + total / 4;
-    if (cudaMalloc(&pqn_.base, cap * 4) != cudaSuccess) {
+    if (mem::dev_malloc(&pqn_.base, cap * 4) != cudaSuccess) {
       cudaGetLastError();
       pqn_.cap = 0;
       return 1;  // no room: the caller scans with the exact kernel
     }
     pqn_.cap = cap;
   }
-  if (!pqn_.d_off) GB_CUDA(cudaMalloc(&pqn_.d_off, sizeof(int64_t) * ((size_t)nlist_ + 1)));
+  if (!pqn_.d_off) GB_CUDA(mem::dev_malloc(&pqn_.d_off, sizeof(int64_t) * ((size_t)nlist_ + 1)));
   GB_CUDA(cudaMemcpyAsync(pqn_.d_off, off.data(), sizeof(int64_t) * ((size_t)nlist_ + 1), cudaMemcpyHostToDevice, st));
   GB_CUDA(launch_pq_entry_norms(lists_->directory(), nlist_, lists_->max_len(), M_, d_cbnrm_, pqn_.d_off, pqn_.base, st));
   GB_CUDA(cudaStreamSynchronize(st));
@@ -2791,10 +2858,10 @@ BinaryIvfIndex::BinaryIvfIndex(int d_bits, const ModelParams& mp, int device, in
     : IvfIndex("BINARYIVF", d_bits, mp, device, seg_shift, d_bits / 8), cb_(d_bits / 8) {
   ldw_ = store_->stride() / 4;
   mp_.metric = kMetricL2;  // Hamming distances rank like L2: smaller first
-  cudaMalloc(&d_bcent_, (size_t)nlist_ * ldw_ * 4);
+  mem::dev_malloc(&d_bcent_, (size_t)nlist_ * ldw_ * 4);
   cudaMemset(d_bcent_, 0, (size_t)nlist_ * ldw_ * 4);
 }
-BinaryIvfIndex::~BinaryIvfIndex() { cudaFree(d_bcent_); }
+BinaryIvfIndex::~BinaryIvfIndex() { mem::dev_free(d_bcent_); }
 int64_t BinaryIvfIndex::index_mem_bytes() const { return IvfIndex::index_mem_bytes() + (int64_t)nlist_ * ldw_ * 4; }
 
 // GammaIndexBinaryIVF::Indexing (gamma_index_binary_ivf.cc:212-270) -> faiss IndexBinaryIVF::train, through
@@ -3057,11 +3124,11 @@ VearchIndex::VearchIndex(int d, const ModelParams& mp, int device, int seg_shift
     : IvfIndex("VEARCH", d, mp, device, seg_shift), nb_(scann_blocks(d, mp.nsubvector)) {
   // GetConfig: a negative threshold is written as nan, and L2 forces nan (no noise shaping)
   if (mp_.ns_threshold < 0 || mp_.metric == kMetricL2) mp_.ns_threshold = std::nan("");
-  cudaMalloc(&d_cb_, (size_t)16 * d * 4);
+  mem::dev_malloc(&d_cb_, (size_t)16 * d * 4);
   cudaMemset(d_cb_, 0, (size_t)16 * d * 4);
   if (mp_.reordering) store_->enable_shadow();  // only reordering re-ranks
 }
-VearchIndex::~VearchIndex() { cudaFree(d_cb_); }
+VearchIndex::~VearchIndex() { mem::dev_free(d_cb_); }
 int64_t VearchIndex::index_mem_bytes() const { return IvfIndex::index_mem_bytes() + (int64_t)16 * d_ * 4; }
 
 // partitioning: 12 iterations, SPHERICAL under IP, the database assigned by SquaredL2Distance

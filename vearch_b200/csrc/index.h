@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "kernels.h"
+#include "mem_ledger.h"
 
 namespace gb {
 
@@ -88,6 +89,9 @@ class RawStore {
   const float* contiguous(int64_t n, Scratch& s);
   // rows [start, start + n) (stride() bytes apart) into device memory at dst, ordered on st
   cudaError_t copy_rows_to_device(int64_t start, int64_t n, void* dst, cudaStream_t st) const;
+  // bytes ensure(n_total) would newly obtain (its granules and segments, the shadow's included), and in *rows the rows
+  // of this store they make room for: what the memory limit admits before documents are accepted
+  int64_t growth_bytes(int64_t n_total, int64_t* rows) const;
   // physical HBM behind the store, its int8 shadow included (0 for host placement)
   int64_t mem_bytes() const { return phys_bytes_ + (shadow_ ? shadow_->phys_bytes_ : 0); }
   int64_t host_bytes() const { return host_bytes_; }  // pinned host memory behind the store
@@ -315,6 +319,13 @@ class Index {
   // VectorManager::ReCreateVectorIndexes, search/engine.cc:991-1089): the next train() starts over
   virtual int reset_index() { return 0; }
   virtual int64_t index_mem_bytes() const { return 0; }
+  // Admission under the memory limit (mem_ledger.h): what storing rows up to n_total costs -- the store's growth where
+  // the store lives, and for every row that growth makes room for, the index bytes it will take once indexed
+  void memory_charges(int64_t n_total, std::vector<mem::Charge>* out);
+  // the index bytes `rows` new rows will take once indexed, on the devices that will hold them (none for FLAT)
+  virtual void charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) { (void)rows; (void)out; }
+  // free the scan scratch buffers no search is using (the memory limit's trim)
+  void release_idle_scratch();
   // gamma's own index file of the type (IvfIndex::dump_gamma / load_gamma); the types without one write and read nothing
   virtual int dump_gamma(const std::string& dir, const std::string& abs_name) { (void)dir; (void)abs_name; return 0; }
   virtual int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) {
@@ -425,6 +436,7 @@ class Index {
   // such blocks on every search when the caller's stream is the legacy default stream
   void* big_acquire(size_t bytes, cudaStream_t st);
   void big_release(void* p, cudaStream_t st);
+  void free_idle_big_locked();  // big_mu_ held
   struct BigBuf {
     void* p;
     size_t cap;
@@ -517,6 +529,7 @@ class IvfIndex : public Index {
   int64_t index_mem_bytes() const override;
   int nlist() const { return nlist_; }
   virtual int code_bytes() const = 0;  // bytes per list entry
+  void charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) override;  // a list entry and its id
   // parity hooks: exchange index state with the oracle
   int set_centroids(const float* host, int nlist);  // marks trained
   int get_centroids(float* host) const;
@@ -646,6 +659,7 @@ class IVFFlatIndex : public IvfIndex {
   ~IVFFlatIndex() override;
   int64_t index_mem_bytes() const override;
   int code_bytes() const override { return dpad_ * 4; }
+  void charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) override;  // and its mirror row, while kept
   int mirror_builds() const { return mirror_.builds; }  // test hook
   int get_list_shifts(float* host) const;               // test hook: d_shifts_ as [nlist][d] (L2 indexes only)
 
@@ -987,6 +1001,7 @@ class ShardedIndex : public Index {
   int purge_lists(float threshold, const uint8_t* del_bitmap, int64_t bitmap_bytes, int64_t* dropped) override;
   int reset_index() override;
   int64_t index_mem_bytes() const override;
+  void charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) override;  // each shard its share
   // the unsharded type's file: list l is the merge of the shards' lists l by global vid, ids written as global vids
   int dump_gamma(const std::string& dir, const std::string& abs_name) override;
   // every shard reads the file and keeps its own entries

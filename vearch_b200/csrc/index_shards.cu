@@ -394,6 +394,10 @@ int64_t ShardedIndex::index_mem_bytes() const {
   for (auto& sh : shards_) b += sh->index_mem_bytes();
   return b;
 }
+void ShardedIndex::charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) {
+  const int S = nshards();  // vid v goes to shard v % S
+  for (int s = 0; s < S; s++) shards_[s]->charge_index_rows(rows / S + (s < rows % S ? 1 : 0), out);
+}
 
 // ---- gamma's index file ----------------------------------------------------------------------
 int ShardedIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {

@@ -7,6 +7,7 @@
 #include <numeric>
 
 #include "engine.h"
+#include "mem_ledger.h"
 
 namespace gb {
 
@@ -49,7 +50,7 @@ bool raw_value(int width, const std::string& v, uint64_t* raw) {
 template <typename T>
 cudaError_t dev_alloc(T** p, int64_t n) {
   *p = nullptr;
-  return n > 0 ? cudaMalloc(reinterpret_cast<void**>(p), (size_t)n * sizeof(T)) : cudaSuccess;
+  return n > 0 ? mem::dev_malloc(p, (size_t)n * sizeof(T)) : cudaSuccess;
 }
 // a zeroed buffer of n elements holding the first `keep` elements of old (old is freed)
 template <typename T>
@@ -60,10 +61,10 @@ cudaError_t dev_regrow(T** p, int64_t keep, int64_t n, cudaStream_t st) {
   if (e == cudaSuccess && keep > 0) e = cudaMemcpyAsync(q, *p, (size_t)keep * sizeof(T), cudaMemcpyDeviceToDevice, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) {
-    cudaFree(q);
+    mem::dev_free(q);
     return e;
   }
-  cudaFree(*p);
+  mem::dev_free(*p);
   *p = q;
   return cudaSuccess;
 }
@@ -88,7 +89,7 @@ bool ScalarColumn::dt_is_array() const { return dt_ == DT_STRINGARRAY; }
 
 void ScalarColumn::release() {
   for (void* p : {col_, (void*)valid_, (void*)codes_, (void*)arr_off_, (void*)arr_cnt_, (void*)pool_})
-    if (p) cudaFree(p);
+    mem::dev_free(p);
   col_ = nullptr, valid_ = nullptr, codes_ = nullptr, arr_off_ = nullptr, arr_cnt_ = nullptr, pool_ = nullptr;
   built_ = false;
   cap_ = ndoc_ = pool_size_ = pool_cap_ = pool_dead_ = dict_bytes_ = 0;

@@ -92,6 +92,23 @@ def _status(st):
         raise GammaStatusError(st.code, msg)
 
 
+def set_memory_limit(percent):
+    """SetMemoryLimitConfig: limit this process to `percent` % of each device's HBM and of host memory (0: no limit)."""
+    _api().SetMemoryLimitConfig(int(percent))
+
+
+def memory_ledger(device):
+    """(usage, pool_reserved, limit) in bytes on a device, or the host for device -1 (limit 0: none)."""
+    u, p, lim = C.c_int64(), C.c_int64(), C.c_int64()
+    _api().gb_memory_ledger(device, C.byref(u), C.byref(p), C.byref(lim))
+    return u.value, p.value, lim.value
+
+
+def set_memory_total(device, nbytes):
+    """test hook: the total memory the limit's percentage applies to on a device (-1: host); 0 restores the real one."""
+    _api().gb_memory_set_total(device, int(nbytes))
+
+
 class GammaEngine:
     def __init__(self, path, space_name="default", log_dir="/tmp/gamma_b200_logs", device=0, devices=None):
         """devices: CUDA ordinals or "all" (Init's "devices"): GPU_IVFPQ / GPU_IVFFLAT fields are sharded over them and
