@@ -46,6 +46,62 @@ static cudaStream_t thread_stream(int device) {
   return st[device];
 }
 
+// A second stream beside thread_stream(device), for work a search forks off its own stream and joins back (ForkJoin),
+// with the two events that order it.  Same (default) priority as the search stream: the side chain's blocks then take
+// what the search stream's grid leaves free instead of displacing its CTAs (at high priority the IVF-PQ phase A slowed
+// by as much as the side chain saved, BASELINE.md section 4).  Per thread, like the search stream, so concurrent
+// searches never share one.
+struct SideStream {
+  cudaStream_t st = nullptr;
+  cudaEvent_t fork = nullptr, join = nullptr;
+};
+static const SideStream* thread_side_stream(int device) {
+  static thread_local SideStream ss[64];
+  if (device < 0 || device >= 64) return nullptr;
+  SideStream& s = ss[device];
+  if (!s.st) {
+    cudaSetDevice(device);
+    if (cudaEventCreateWithFlags(&s.fork, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&s.join, cudaEventDisableTiming) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&s.st, cudaStreamNonBlocking) != cudaSuccess) {
+      s.st = nullptr;
+      return nullptr;
+    }
+  }
+  return &s;
+}
+
+// Work on a side stream between a fork from the parent stream and the join back into it.  Scratch is allocated and
+// freed stream-ordered on the parent, so what the side stream uses must be allocated before fork(), and every exit path
+// joins (the destructor) before that scratch is freed.
+class ForkJoin {
+ public:
+  ForkJoin(cudaStream_t parent, const SideStream& side) : parent_(parent), side_(side) {}
+  ForkJoin(const ForkJoin&) = delete;
+  ForkJoin& operator=(const ForkJoin&) = delete;
+  ~ForkJoin() { join(); }
+  cudaError_t fork() {
+    cudaError_t e = cudaEventRecord(side_.fork, parent_);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(side_.st, side_.fork, 0);
+    if (e == cudaSuccess) forked_ = true;
+    return e;
+  }
+  cudaError_t join() {
+    if (!forked_) return cudaSuccess;
+    forked_ = false;
+    cudaError_t e = cudaEventRecord(side_.join, side_.st);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(parent_, side_.join, 0);
+    if (e != cudaSuccess) cudaStreamSynchronize(side_.st);  // the parent cannot wait for it: nothing may still run there
+    return e;
+  }
+  cudaStream_t side() const { return side_.st; }
+
+ private:
+  cudaStream_t parent_;
+  const SideStream& side_;
+  bool forked_ = false;
+};
+
 // ------------------------------------------------------------------------------------------
 Scratch::~Scratch() {
   for (void* p : ptrs_) cudaFreeAsync(p, st_);
@@ -1888,8 +1944,7 @@ int IvfIndex::coarse_dev(int nq, const void* xqv, int nprobe, int metric, int32_
 // score segment of len(list) floats, cut (list, 128 pairs, 128 rows) tiles; device side: grouped
 // GEMM on wgmma + segment select.
 
-int IvfIndex::group_pairs_by_list(const int32_t* probe_ids, int64_t npairs, int nseg, int group, int64_t max_items,
-                                  LmGrouping* g, Scratch& s) {
+int IvfIndex::alloc_pair_grouping(int64_t npairs, int64_t max_items, LmGrouping* g, Scratch& s) {
   GB_ALLOC(d_cnt, int32_t, nlist_, s);
   GB_ALLOC(d_start, int32_t, nlist_, s);
   GB_ALLOC(d_cursor, int32_t, nlist_, s);
@@ -1898,10 +1953,13 @@ int IvfIndex::group_pairs_by_list(const int32_t* probe_ids, int64_t npairs, int 
   GB_ALLOC(totals, int64_t, 3, s);
   GB_ALLOC(pair_j, int64_t, npairs, s);
   GB_ALLOC(items, LmTile, max_items, s);
-  GB_CUDA(launch_lmk_group(probe_ids, npairs, lists_->directory(), nseg, group, d_cnt, d_start, d_cursor, d_item_start,
-                           d_grp_start, totals, pair_j, items, s.stream()));
-  *g = {totals, pair_j, items};
+  *g = {d_cnt, d_start, d_cursor, d_item_start, d_grp_start, totals, pair_j, items};
   return 0;
+}
+cudaError_t IvfIndex::group_pairs_by_list(const int32_t* probe_ids, int64_t npairs, int nseg, int group,
+                                          const LmGrouping& g, cudaStream_t st) {
+  return launch_lmk_group(probe_ids, npairs, lists_->directory(), nseg, group, g.cnt, g.start, g.cursor, g.item_start,
+                          g.grp_start, g.totals, g.pair_j, g.items, st);
 }
 
 // called from index_batch with mu_ held exclusively: no search is inside ensure_mirror.  Kernels of an
@@ -2008,7 +2066,8 @@ int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, co
     GB_CUDA(cudaMemsetAsync(d_tau, 0xFF, sizeof(unsigned long long) * nq, st));
     GB_CUDA(cudaMemsetAsync(d_out, 0xFF, sizeof(unsigned long long) * nout, st));
     LmGrouping g;
-    if (group_pairs_by_list(probe_ids, npairs, nseg, 128, max_items, &g, s)) return -1;
+    if (alloc_pair_grouping(npairs, max_items, &g, s)) return -1;
+    GB_CUDA(group_pairs_by_list(probe_ids, npairs, nseg, 128, g, st));
     const int k16 = (int)round_up(dpad_, 16);
     const int64_t max_groups = npairs / 128 + nlist_;
     const size_t slot_bytes = (size_t)128 * k16 * 8, a_bytes = (size_t)max_groups * (slot_bytes + 128 * 4);
@@ -2598,19 +2657,34 @@ int IVFPQIndex::ensure_pq_norms(cudaStream_t st) {
 
 // List-major IVF-PQ scan (kernels_pqtc.cu): exact scan of the first pa probes -> per-query bound ->
 // tensor-core filter over the remaining probes -> exact re-score of the candidates.  Returns 1 when
-// the batch / shape does not qualify (caller runs the exact kernel over all probes).
-int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const float* xq, int kk, const float* ip,
+// the batch / shape does not qualify (caller builds ip and runs the exact kernel over all probes), before any work.
+// Otherwise it builds the query's inner-product table ip itself.
+//
+// Only the filter's thresholds need phase A's bounds: the pair grouping and the operand staging read the plan alone, so
+// they run on a side stream while this stream builds ip and runs phase A, and pq_bind_bounds sets the thresholds after
+// the join.
+int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const float* xq, int kk, float* ip,
                                   const int32_t* probe_ids, const float* coarse_dis, int nprobe,
                                   unsigned long long* adc_out, bool need_sorted, Scratch& s) {
   if (ksub_ != 256 || !d_cb8_ || !pqtc_supported(M_, dsub_) || dpad_ != d_) return 1;  // the filter reads 8-bit codes
   if (kk > 2048 || nprobe < 2 || nprobe > 65535 || nq > 65535) return 1;  // (query, probe) travel as 16-bit fields of a candidate record
   const int64_t npairs = (int64_t)nq * nprobe;
   if (npairs < (int64_t)nlist_ * 32) return 1;  // < 32 queries per list on average
+  const int nseg = (int)std::min<int64_t>(64, std::max<int64_t>(1, (lists_->max_len() + kLmkSegRows - 1) / kLmkSegRows));
+  const int pq_group = 256;  // pairs per group: two 128-row operand tiles that share every decoded entry tile
+  const int64_t max_groups = npairs / pq_group + nlist_;
+  const int64_t max_items = max_groups * nseg;
+  if (max_items > INT32_MAX) return 1;
   if (metric == kMetricL2) {
     const int nr = ensure_pq_norms(s.stream());
     if (nr) return nr;
   }
   cudaStream_t st = s.stream();
+  const SideStream* side = thread_side_stream(device_);
+  if (!side) {
+    set_last_error("cannot create the list-major scan's side stream");
+    return -1;
+  }
   ListDirectory dir = lists_->directory();
   // phase A, per query: its first probes in full -- the fewest whose lists hold >= 4 k' entries together (so that its
   // k'-th exact score is a tight bound B_q), at most pa_max; phase B filters the other probes.
@@ -2627,29 +2701,15 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   GB_CUDA(launch_pqtc_plan_phase_a(probe_ids, npairs, nprobe, pa_max, pa_target, dir.len, d_probes_a, d_probes_b, d_row_limit,
                                    st));
 
-  // ---- phase A: exact keys of each query's leading probes ----
   const int pgA = nq >= nsm * 4 ? std::min(pa_max, 32) : 1;  // one CTA per query when there are queries enough
   const int ngA = (pa_max + pgA - 1) / pgA;
   GB_ALLOC(partA, unsigned long long, (size_t)nq * ngA * kk, s);
-  stage_begin("pq_phaseA_exact_scan", st);
-  // one group per query: its k' best come back unordered with the largest (the bound) in slot k' - 1 -- nobody needs
-  // them sorted (launch_select_keys below, used when the probes were split over groups, sorts anyway)
-  GB_CUDA(launch_ivfpq_scan(ip, nq, d_probes_a, coarse_dis, pa_max, pgA, dir, M_, d_table_, kk, metric, f, partA, st, nprobe,
-                            nullptr, 0, d_row_limit, /*sorted_out=*/ngA > 1));
   unsigned long long* keysA = partA;
   if (ngA > 1) {
     keysA = s.alloc_n<unsigned long long>((size_t)nq * kk);
     if (!keysA) return -1;
-    GB_CUDA(launch_select_keys(partA, (int64_t)ngA * kk, nq, ngA * kk, kk, keysA, kk, st));
   }
-  stage_end(st);
-
-  // ---- phase B: group the remaining pairs by list, stage the operand tiles, filter ----
-  const int nseg = (int)std::min<int64_t>(64, std::max<int64_t>(1, (lists_->max_len() + kLmkSegRows - 1) / kLmkSegRows));
-  const int pq_group = 256;  // pairs per group: two 128-row operand tiles that share every decoded entry tile
-  const int64_t max_groups = npairs / pq_group + nlist_;
-  const int64_t max_items = max_groups * nseg;
-  if (max_items > INT32_MAX) return 1;
+  // phase B's scratch: everything the side stream touches is allocated before the fork
   GB_ALLOC(d_cand_cnt, int, nq, s);
   const size_t tile_bytes = (size_t)(d_ / 16) * 2048;
   const size_t a_bytes = (size_t)max_groups * 2 * tile_bytes;
@@ -2660,14 +2720,40 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   unsigned char* a_scratch = static_cast<unsigned char*>(big.p);
   void* meta = a_scratch + a_bytes;
   unsigned long long* cand = reinterpret_cast<unsigned long long*>(a_scratch + a_bytes + meta_bytes);
-  stage_begin("pq_group_and_stage_pairs", st);
-  GB_CUDA(cudaMemsetAsync(d_cand_cnt, 0, sizeof(int) * nq, st));
   LmGrouping g;
-  if (group_pairs_by_list(d_probes_b, npairs, nseg, pq_group, max_items, &g, s)) return -1;
+  if (alloc_pair_grouping(npairs, max_items, &g, s)) return -1;
+
+  // ---- phase B's set-up on the side stream: group the remaining pairs by list, stage the operand tiles ----
+  ForkJoin fj(st, *side);  // declared after the scratch: joined on every exit before any of it is freed
+  GB_CUDA(fj.fork());
+  stage_begin("pq_group_and_stage_pairs", fj.side());
+  GB_CUDA(cudaMemsetAsync(d_cand_cnt, 0, sizeof(int) * nq, fj.side()));
+  GB_CUDA(group_pairs_by_list(d_probes_b, npairs, nseg, pq_group, g, fj.side()));
   GB_CUDA(launch_pq_stage_pairs(xq, dpad_, d_, d_centroids_, dpad_, g.items, (int)max_items, g.totals, g.pair_j, nprobe,
-                                coarse_dis, keysA, kk, kk, d_cbnrm_ + (size_t)M_ * 256, f, metric, a_scratch,
-                                meta, d_cand_cnt, cap, d_row_limit, st));
+                                coarse_dis, d_cbnrm_ + (size_t)M_ * 256, f, metric, a_scratch, meta, max_groups,
+                                d_cand_cnt, cap, d_row_limit, fj.side()));
+  stage_end(fj.side());
+
+  // ---- meanwhile, phase A: exact keys of each query's leading probes ----
+  {
+    StageScope stage(this, "pq_ip_table", st);
+    GB_CUDA(launch_pq_ip_table(xq, dpad_, nq, d_pq_, M_, dsub_, ip, st, ksub_));
+  }
+  stage_begin("pq_phaseA_exact_scan", st);
+  // one group per query: its k' best come back unordered with the largest (the bound) in slot k' - 1 -- nobody needs
+  // them sorted (launch_select_keys below, used when the probes were split over groups, sorts anyway)
+  GB_CUDA(launch_ivfpq_scan(ip, nq, d_probes_a, coarse_dis, pa_max, pgA, dir, M_, d_table_, kk, metric, f, partA, st, nprobe,
+                            nullptr, 0, d_row_limit, /*sorted_out=*/ngA > 1));
+  if (ngA > 1) GB_CUDA(launch_select_keys(partA, (int64_t)ngA * kk, nq, ngA * kk, kk, keysA, kk, st));
   stage_end(st);
+
+  // ---- phase B: the pairs' thresholds from the bounds, filter ----
+  GB_CUDA(fj.join());
+  {
+    StageScope stage(this, "pq_bind_bounds", st);
+    GB_CUDA(launch_pq_bind_bounds(g.totals, max_groups, nprobe, coarse_dis, keysA, kk, kk, f, metric, meta, d_cand_cnt,
+                                  cap, st));
+  }
   scan_timer_begin(st);  // the dominant kernel: the roofline in bench.py is this launch alone
   stage_begin("pqtc_scan_kernel", st);
   GB_CUDA(launch_pqtc_scan(a_scratch, meta, d_cb8_, pqn_.base, pqn_.d_off, g.items, (int)max_items, g.totals, dir, M_, dsub_, f,
@@ -2768,12 +2854,13 @@ int IVFPQIndex::scan_dev(const SearchContext& ctx, const FilterArgs& f, int metr
   auto prepare = [&](int kk, unsigned long long* keys, bool need_sorted) {
     ip = s.alloc_n<float>((size_t)nq * M_ * ksub_);
     if (!ip) return -1;
-    {
+    // the list-major scan builds ip itself, beside its pair grouping; it declines (1) before that
+    const int lm = scan_listmajor_pq(f, metric, nq, xq, kk, ip, probe_ids, coarse_dis, nprobe, keys, need_sorted, s);
+    if (lm == 0) last_scan_kernel_ = "pqtc_scan_kernel";
+    if (lm == 1) {
       StageScope stage(this, "pq_ip_table", st);
       GB_CUDA(launch_pq_ip_table(xq, dpad_, nq, d_pq_, M_, dsub_, ip, st, ksub_));
     }
-    const int lm = scan_listmajor_pq(f, metric, nq, xq, kk, ip, probe_ids, coarse_dis, nprobe, keys, need_sorted, s);
-    if (lm == 0) last_scan_kernel_ = "pqtc_scan_kernel";
     return lm;
   };
   auto launch = [&](int kk, int pg, unsigned long long* partial) {

@@ -602,14 +602,18 @@ class IvfIndex : public Index {
                            const std::function<int(int, unsigned long long*, bool)>& prepare,
                            const std::function<cudaError_t(int, int, unsigned long long*)>& launch);
   // List-major pair grouping (launch_lmk_group): the (query, probe) pairs grouped by list, `group` pairs per group, each
-  // group cut into nseg row segments.  Items, pair order and totals are left in `s` for the list-major kernels.
+  // group cut into nseg row segments.  Items, pair order and totals are left in `s` for the list-major kernels.  The
+  // scratch is allocated first (alloc_pair_grouping, stream-ordered on s), so the grouping may run on a stream forked
+  // from s's after it.
   struct LmGrouping {
+    int32_t *cnt, *start, *cursor, *item_start, *grp_start;
     int64_t* totals;
     int64_t* pair_j;
     LmTile* items;
   };
-  int group_pairs_by_list(const int32_t* probe_ids, int64_t npairs, int nseg, int group, int64_t max_items, LmGrouping* g,
-                          Scratch& s);
+  int alloc_pair_grouping(int64_t npairs, int64_t max_items, LmGrouping* g, Scratch& s);
+  cudaError_t group_pairs_by_list(const int32_t* probe_ids, int64_t npairs, int nseg, int group, const LmGrouping& g,
+                                  cudaStream_t st);
   int assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* assign_dev_out, Scratch& s);
   // the rows of a batch as the codec takes them (*xc) and each row's nearest list (out): fp32 rows (stride dpad) through
   // transform_dev and assign_dev; BINARYIVF: the packed rows as they are, by Hamming distance
@@ -773,7 +777,7 @@ class IVFPQIndex : public IvfPqBase {
   int train_extra(const float* xtrain, int64_t n, Scratch& s) override;
   int codebook_changed(cudaStream_t st) override;
   // list-major scan through the tensor-core filter (kernels_pqtc.cu); 1 = not applicable
-  int scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const float* xq, int kk, const float* ip,
+  int scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const float* xq, int kk, float* ip,
                         const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* adc_out,
                         bool need_sorted, Scratch& s);
 

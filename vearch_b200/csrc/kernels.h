@@ -191,6 +191,8 @@ cudaError_t launch_ivfpq_packed_scan(const float* ip_table, int nq, const int32_
 
 // ---- K5 list-major: tensor-core filter + exact re-score (kernels_pqtc.cu) ---------------------------
 bool pqtc_supported(int M, int dsub);
+// bytes per pair slot of `meta` below: the filter's per-pair record, then (after all max_groups x 256 of those) the
+// doubles that its threshold needs besides the bound
 size_t pqtc_pair_meta_bytes();
 // cb[m][c][.] = int8 rn(pq / sb), sb = rmax2[1] = max |pq| / 127; nrm[m][c] = |pq[m][c]|^2; rmax2[0] = sum_m max_c nrm;
 // rmax2[2] = sqrt(sum_m max_c |pq[m][c] - sb cb[m][c]|^2)
@@ -200,13 +202,19 @@ cudaError_t launch_pqtc_tables(const float* pq, int M, int dsub, int8_t* cb, flo
 cudaError_t launch_pqtc_plan_phase_a(const int32_t* probe_ids, int64_t npairs, int nprobe, int pa_max, long long target,
                                      const int* list_len, int32_t* probes_a, int32_t* probes_b, int* row_limit,
                                      cudaStream_t st);
-// per pair group: int8 operand tile (each row rn(a / sa), sa = max |a| / 127) of a = x - centroid (L2) / x (IP) + the pairs' filter thresholds from
-// bound_keys[q][kprime - 1] (phase A's k'-th key); queries without a bound get cand_cnt = cap + 1
+// per pair group: int8 operand tile (each row rn(a / sa), sa = max |a| / 127) of a = x - centroid (L2) / x (IP) + the
+// pairs' filter records except the bound-dependent threshold; independent of phase A.  Queries whose rows cannot be
+// bounded get cand_cnt = cap + 1
 cudaError_t launch_pq_stage_pairs(const float* xq, int64_t ldq, int d, const float* coarse, int64_t ldc, const LmTile* items,
                                   int max_items, const int64_t* totals, const int64_t* pair_j, int nprobe,
-                                  const float* coarse_dis, const unsigned long long* bound_keys, int64_t bound_stride,
-                                  int kprime, const float* rmax2, FilterArgs f, int metric, unsigned char* a_scratch,
-                                  void* meta, int* cand_cnt, int cap, const int* row_limit, cudaStream_t st);
+                                  const float* coarse_dis, const float* rmax2, FilterArgs f, int metric,
+                                  unsigned char* a_scratch, void* meta, int64_t max_groups, int* cand_cnt, int cap,
+                                  const int* row_limit, cudaStream_t st);
+// after phase A and the staging: every staged pair's threshold from bound_keys[q][kprime - 1] (phase A's k'-th key);
+// queries without a bound get cand_cnt = cap + 1
+cudaError_t launch_pq_bind_bounds(const int64_t* totals, int64_t max_groups, int nprobe, const float* coarse_dis,
+                                  const unsigned long long* bound_keys, int64_t bound_stride, int kprime, FilterArgs f,
+                                  int metric, void* meta, int* cand_cnt, int cap, cudaStream_t st);
 // persistent kernel, one CTA per SM: candidates (probe << 32 | position) appended to cand[q][cap]
 cudaError_t launch_pqtc_scan(const unsigned char* a_scratch, const void* meta, const int8_t* cb, const float* pqnorm, const int64_t* pqnorm_off,
                              const LmTile* items, int max_items, const int64_t* totals, ListDirectory dir, int M, int dsub,

@@ -167,18 +167,26 @@ struct PairMeta {
   int lim;    // rows [0, lim) of this pair's list were scored exactly by phase A: never candidates
 };
 
+// What the threshold of a pair needs besides the bound B_q, in double: eps (the error margin in score units) and fs = f s
+// (score units per accumulator unit).  fs = 0: the pair has no filter test (an empty row, or one already sent to the
+// exact kernel while staging).  A filtered pair has fs > 0: a_ok and sb > 0, and a subnormal sa would make the row tiny.
+struct PairBound {
+  double eps, fs;
+};
+
 // A group of up to PT_G pairs is staged as two stacked 128-row tiles, one per consumer warpgroup; its pairs are split
 // evenly over the two (the first ceil(n / 2) in tile 0), so neither runs a mostly empty remainder.  Thread r = row r % 128
-// of tile r / 128; meta[grp * PT_G + r] is that row's pair.
+// of tile r / 128; meta[grp * PT_G + r] is that row's pair.  Nothing here reads phase A's keys, so the staging runs
+// beside phase A; pq_bind_bounds_kernel sets thr from B_q afterwards (thr = -inf until then).
 template <int METRIC>
 __global__ void __launch_bounds__(PT_G)
     pq_stage_pairs_kernel(const float* __restrict__ xq, int64_t ldq, int d, const float* __restrict__ coarse, int64_t ldc,
                           const LmTile* __restrict__ items, const int64_t* __restrict__ totals,
                           const int64_t* __restrict__ pair_j, int nprobe, const float* __restrict__ coarse_dis,
-                          const unsigned long long* __restrict__ bound_keys, int64_t bound_stride, int kprime,
                           const float* __restrict__ rmax2, float min_score, float max_score,
-                          unsigned char* __restrict__ a_scratch, PairMeta* __restrict__ meta, int* __restrict__ cand_cnt,
-                          int cap, const int* __restrict__ row_limit) {
+                          unsigned char* __restrict__ a_scratch, PairMeta* __restrict__ meta,
+                          PairBound* __restrict__ bounds, int* __restrict__ cand_cnt, int cap,
+                          const int* __restrict__ row_limit) {
   if ((int64_t)blockIdx.x >= totals[1]) return;
   const LmTile t = items[blockIdx.x];
   if (t.seg != 0) return;  // one staging per pair group: the first item of the group owns the slot
@@ -253,17 +261,17 @@ __global__ void __launch_bounds__(PT_G)
     }
     *reinterpret_cast<uint4*>(tile + (int64_t)kc * 2048 + r * 16) = make_uint4(wv[0], wv[1], wv[2], wv[3]);
   }
+  PairBound pb{0.0, 0.0};
   if (x) {
     const float dis0 = coarse_dis[(int64_t)pm.q * nprobe + pm.p];
     pm.lim = row_limit ? row_limit[(int64_t)pm.q * nprobe + pm.p] : 0;
-    const unsigned long long bk = bound_keys[(int64_t)pm.q * bound_stride + kprime - 1];
     const float R2 = rmax2[0], R = sqrtf(R2), sb = rmax2[1], Dq = rmax2[2];
     // eps below has relative terms only.  Near fp32's subnormal range (|a|^2 or the codebook's largest |r|^2 below
     // 2^-96) the roundings of the exact table evaluation are absolute (2^-149 each) and can exceed it: no filter there.
     // A zero or non-finite row or codebook has no int8 scale: no filter either
     const bool tiny = (amax > 0.f && na2 < 0x1p-96f) || (R2 > 0.f && R2 < 0x1p-96f);
-    if (bk == kKeySentinel || tiny || !a_ok || !(sb > 0.f && sb < INFINITY)) {
-      // phase A found fewer than k' entries (no bound), or the bound would not hold -> the exact kernel redoes this query
+    if (tiny || !a_ok || !(sb > 0.f && sb < INFINITY)) {
+      // the bound would not hold -> the exact kernel redoes this query
       atomicMax(cand_cnt + pm.q, cap + 1);
     } else {
       // |<a, r> - s <qa, qr>| = |<da, r> + <sa qa, dr>| <= |da| R + (|a| + |da|) D   (Cauchy-Schwarz; da = a - sa qa,
@@ -275,28 +283,62 @@ __global__ void __launch_bounds__(PT_G)
       const double na = sqrt((double)na2), da = sqrt((double)da2), s = (double)sa * (double)sb;
       const double f = METRIC == kMetricL2 ? 2.0 : 1.0;
       const double quant = f * 1.05 * (da * R + (na + da) * Dq);
-      const float B = ord2score((uint32_t)(bk >> 32), METRIC);
-      double thr, lo;
+      double eps, lo;
       if (METRIC == kMetricL2) {
         const double Z = fabs((double)dis0) + R2 + 2.0 * (sqrt((double)nx2) + sqrt((double)nc2)) * R;
-        const double eps = quant + 0x1p-17 * Z + f * s + 0x1p-22 * R2;
-        thr = (double)fminf(B, max_score) - dis0 + eps;
+        eps = quant + 0x1p-17 * Z + f * s + 0x1p-22 * R2;
         lo = (double)min_score - dis0 - eps;
       } else {
         // score = dis0 + s acc; better = larger, so the test runs on -s acc
         const double Z = fabs((double)dis0) + na * R;
-        const double eps = quant + 0x1p-17 * Z + f * s;
-        thr = (double)dis0 - fmaxf(B, min_score) + eps;
+        eps = quant + 0x1p-17 * Z + f * s;
         lo = (double)dis0 - max_score - eps;
       }
-      // in accumulator units, rounded outwards; FLT_MAX keeps masked entries (ne = +inf) out
+      // in accumulator units, rounded outwards (thr: pq_bind_bounds_kernel)
       const double fs = f * s;
       pm.c = (float)(1.0 / fs);
-      pm.thr = fminf(__double2float_ru(thr / fs - kAccBiasF), FLT_MAX);
       pm.lo = __double2float_rd(lo / fs - kAccBiasF);
+      pb = {eps, fs};
     }
   }
-  meta[(int64_t)t.grp * PT_G + threadIdx.x] = pm;
+  const int64_t slot = (int64_t)t.grp * PT_G + threadIdx.x;
+  meta[slot] = pm;
+  bounds[slot] = pb;
+}
+
+// One thread per pair slot, after phase A: thr from the query's bound B_q = the k'-th key of phase A (slot k' - 1).
+// A query whose phase A found fewer than k' entries has no bound: its pairs get no filter test and the exact kernel
+// redoes it.  Same double expressions and roundings as the staging kernel's lo, so the thresholds are exact functions
+// of (B_q, dis0, eps, fs).
+template <int METRIC>
+__global__ void __launch_bounds__(256)
+    pq_bind_bounds_kernel(const int64_t* __restrict__ totals, int64_t max_slots, int nprobe,
+                          const float* __restrict__ coarse_dis, const unsigned long long* __restrict__ bound_keys,
+                          int64_t bound_stride, int kprime, float min_score, float max_score,
+                          const PairBound* __restrict__ bounds, PairMeta* __restrict__ meta, int* __restrict__ cand_cnt,
+                          int cap) {
+  const int64_t slot = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (slot >= max_slots || slot / PT_G >= totals[0]) return;  // totals[0] = pair groups staged
+  const PairBound pb = bounds[slot];
+  if (!(pb.fs > 0.0)) return;
+  PairMeta* pm = meta + slot;
+  const int q = pm->q, p = pm->p;
+  const unsigned long long bk = bound_keys[(int64_t)q * bound_stride + kprime - 1];
+  if (bk == kKeySentinel) {
+    atomicMax(cand_cnt + q, cap + 1);
+    pm->lo = INFINITY;
+    pm->c = 1.0f;
+    return;
+  }
+  const float dis0 = coarse_dis[(int64_t)q * nprobe + p];
+  const float B = ord2score((uint32_t)(bk >> 32), METRIC);
+  double thr;
+  if (METRIC == kMetricL2)
+    thr = (double)fminf(B, max_score) - dis0 + pb.eps;
+  else
+    thr = (double)dis0 - fmaxf(B, min_score) + pb.eps;
+  // FLT_MAX keeps masked entries (ne = +inf) out
+  pm->thr = fminf(__double2float_ru(thr / pb.fs - kAccBiasF), FLT_MAX);
 }
 
 // ---- the scan ---------------------------------------------------------------------------------------
@@ -826,7 +868,7 @@ bool pqtc_supported(int M, int dsub) {
          (M == 4 && dsub == 16) || (M == 4 && dsub == 32) || (M == 4 && dsub == 8) || (M == 8 && dsub == 4);
 }
 
-size_t pqtc_pair_meta_bytes() { return sizeof(PairMeta); }
+size_t pqtc_pair_meta_bytes() { return sizeof(PairMeta) + sizeof(PairBound); }
 
 cudaError_t launch_pqtc_tables(const float* pq, int M, int dsub, int8_t* cb, float* nrm, float* rmax2, cudaStream_t st) {
   pqtc_tables_kernel<<<1, 256, 0, st>>>(pq, M, dsub, cb, nrm, rmax2);
@@ -846,21 +888,39 @@ cudaError_t launch_pqtc_plan_phase_a(const int32_t* probe_ids, int64_t npairs, i
 
 cudaError_t launch_pq_stage_pairs(const float* xq, int64_t ldq, int d, const float* coarse, int64_t ldc, const LmTile* items,
                                   int max_items, const int64_t* totals, const int64_t* pair_j, int nprobe,
-                                  const float* coarse_dis, const unsigned long long* bound_keys, int64_t bound_stride,
-                                  int kprime, const float* rmax2, FilterArgs f, int metric, unsigned char* a_scratch,
-                                  void* meta, int* cand_cnt, int cap, const int* row_limit, cudaStream_t st) {
+                                  const float* coarse_dis, const float* rmax2, FilterArgs f, int metric,
+                                  unsigned char* a_scratch, void* meta, int64_t max_groups, int* cand_cnt, int cap,
+                                  const int* row_limit, cudaStream_t st) {
   if (max_items <= 0) return cudaSuccess;
   if (d % 32) return cudaErrorInvalidValue;
+  PairMeta* pm = static_cast<PairMeta*>(meta);
+  PairBound* pb = reinterpret_cast<PairBound*>(pm + max_groups * PT_G);
   if (metric == kMetricL2)
     pq_stage_pairs_kernel<kMetricL2><<<max_items, PT_G, 0, st>>>(xq, ldq, d, coarse, ldc, items, totals, pair_j, nprobe,
-                                                                coarse_dis, bound_keys, bound_stride, kprime, rmax2,
-                                                                f.min_score, f.max_score, a_scratch,
-                                                                static_cast<PairMeta*>(meta), cand_cnt, cap, row_limit);
+                                                                coarse_dis, rmax2, f.min_score, f.max_score, a_scratch, pm,
+                                                                pb, cand_cnt, cap, row_limit);
   else
     pq_stage_pairs_kernel<kMetricIP><<<max_items, PT_G, 0, st>>>(xq, ldq, d, coarse, ldc, items, totals, pair_j, nprobe,
-                                                                coarse_dis, bound_keys, bound_stride, kprime, rmax2,
-                                                                f.min_score, f.max_score, a_scratch,
-                                                                static_cast<PairMeta*>(meta), cand_cnt, cap, row_limit);
+                                                                coarse_dis, rmax2, f.min_score, f.max_score, a_scratch, pm,
+                                                                pb, cand_cnt, cap, row_limit);
+  note_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pq_bind_bounds(const int64_t* totals, int64_t max_groups, int nprobe, const float* coarse_dis,
+                                  const unsigned long long* bound_keys, int64_t bound_stride, int kprime, FilterArgs f,
+                                  int metric, void* meta, int* cand_cnt, int cap, cudaStream_t st) {
+  if (max_groups <= 0) return cudaSuccess;
+  PairMeta* pm = static_cast<PairMeta*>(meta);
+  const PairBound* pb = reinterpret_cast<const PairBound*>(pm + max_groups * PT_G);
+  const int64_t slots = max_groups * PT_G;
+  const unsigned nb = (unsigned)((slots + 255) / 256);
+  if (metric == kMetricL2)
+    pq_bind_bounds_kernel<kMetricL2><<<nb, 256, 0, st>>>(totals, slots, nprobe, coarse_dis, bound_keys, bound_stride, kprime,
+                                                        f.min_score, f.max_score, pb, pm, cand_cnt, cap);
+  else
+    pq_bind_bounds_kernel<kMetricIP><<<nb, 256, 0, st>>>(totals, slots, nprobe, coarse_dis, bound_keys, bound_stride, kprime,
+                                                        f.min_score, f.max_score, pb, pm, cand_cnt, cap);
   note_launch();
   return cudaGetLastError();
 }
