@@ -71,7 +71,7 @@ int gb_index_add_pending(gb_index *index, const uint8_t *del_bitmap);
 int64_t gb_index_ntotal(gb_index *index);        /* stored vectors */
 int64_t gb_index_indexed_count(gb_index *index); /* vectors present in the index */
 int gb_index_is_trained(gb_index *index);
-int gb_index_training_threshold(gb_index *index);
+int64_t gb_index_training_threshold(gb_index *index);
 int64_t gb_index_mem_bytes(gb_index *index, int which /* 0 = index, 1 = raw vectors in HBM, 2 = raw vectors in host memory */);
 
 /* IndexModel::Search (index_model.h:296-298) with the RetrievalContext flattened:
@@ -230,6 +230,15 @@ int gb_index_vearch_lut(gb_index *index, int nq, const float *x, uint8_t *lut, f
 /* faiss Clustering restated (k-means), host in/out; obj (niter floats) may be NULL */
 int gb_kmeans(int device, const float *x, int64_t n, int d, int k, int niter, int64_t seed, int spherical,
               int max_points_per_centroid, float *centroids, float *obj);
+/* The same k-means run, traced step by step (a debug surface for the tests; DESIGN.md §5, training bar).  x: n x d;
+ * l2_assign: spherical, assigned by L2; init: NULL, or k x d centroids to start from (hot start).  n_s = the rows
+ * trained on: min(n, k * max_points_per_centroid), or n when max_points_per_centroid is 0.  Outputs (all required):
+ * sample [n_s] (the rows of x trained on), init_out [k][d], labels [niter][n_s], scores [niter][n_s] (the score each
+ * row's key carried), and the centroids [niter][k][d] after the segmented mean (mean), the empty-cluster split (split)
+ * and the spherical renormalisation (norm; = split when not spherical). */
+int gb_debug_kmeans_trace(int device, const float *x, int64_t n, int d, int k, int niter, int64_t seed, int spherical,
+                          int l2_assign, int max_points_per_centroid, const float *init, int64_t *sample,
+                          float *init_out, int32_t *labels, float *scores, float *mean, float *split, float *norm);
 /* centroid update only: centroids[c] = mean of x[assign == c] in point order */
 int gb_kmeans_update(int device, const float *x, int64_t n, int d, int k, const int64_t *assign, float *centroids);
 /* router merge (internal/client/client.go:1530-1609) on device memory: dis/ids are

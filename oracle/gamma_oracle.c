@@ -570,6 +570,8 @@ void orc_rand_perm(int64_t *perm, int64_t n, int64_t seed) {
  *   - each iteration: exact assign; centroid = sum(members in point order) * (1/count);
  *     empty clusters re-seeded by splitting (split_clusters, EPS = 1/1024, rng(1234));
  *     spherical => renormalise
+ * l2_assign: spherical, but assigned by L2 (faiss's default IndexFlatL2 clustering index, which IVFPQFastScan and VEARCH
+ * keep under IP).
  * centroids_out: k*d.  If assign_out != NULL it receives the last assignment (n entries, only
  * meaningful when no subsampling happened).  obj_out (may be NULL): niter objective values.
  * ---------------------------------------------------------------------------------------- */
@@ -643,7 +645,8 @@ int orc_kmeans_split(int d, int k, int64_t n, float *hassign, float *centroids) 
   return nsplit;
 }
 
-static void km_normalize(float *cent, int k, int d) {
+/* spherical k-means' renormalisation of the k x d centroids (a zero row stays zero) */
+void orc_kmeans_normalize(float *cent, int k, int d) {
   for (int c = 0; c < k; c++) {
     float *cc = cent + (size_t)c * d;
     float nr = 0;
@@ -655,7 +658,7 @@ static void km_normalize(float *cent, int k, int d) {
   }
 }
 
-int orc_kmeans(const float *x_in, int64_t n_in, int d, int k, int niter, int64_t seed, int spherical,
+int orc_kmeans(const float *x_in, int64_t n_in, int d, int k, int niter, int64_t seed, int spherical, int l2_assign,
                int max_points_per_centroid, float *centroids_out, int64_t *assign_out, float *obj_out) {
   if (n_in < k) return -1;
   const float *x = x_in;
@@ -674,7 +677,7 @@ int orc_kmeans(const float *x_in, int64_t n_in, int d, int k, int niter, int64_t
   orc_rand_perm(perm, n, seed + 1);
   for (int c = 0; c < k; c++) memcpy(centroids_out + (size_t)c * d, x + (size_t)perm[c] * d, sizeof(float) * d);
   free(perm);
-  if (spherical) km_normalize(centroids_out, k, d);
+  if (spherical) orc_kmeans_normalize(centroids_out, k, d);
 
   int64_t *assign = (int64_t *)malloc(sizeof(int64_t) * n);
   float *dis = (float *)malloc(sizeof(float) * n);
@@ -682,8 +685,8 @@ int orc_kmeans(const float *x_in, int64_t n_in, int d, int k, int niter, int64_t
   for (int it = 0; it < niter; it++) {
     /* faiss's clustering index is an IndexFlatL2 even for spherical k-means unless the caller
        passes an IP index; gamma passes its quantizer, which is IndexFlat(d, metric)
-       (gamma_index_ivfpq.cc:156) => IP assign when spherical. */
-    km_assign(x, n, d, centroids_out, k, assign, dis, spherical);
+       (gamma_index_ivfpq.cc:156) => IP assign when spherical, unless l2_assign. */
+    km_assign(x, n, d, centroids_out, k, assign, dis, spherical && !l2_assign);
     if (obj_out) {
       double obj = 0;
       for (int64_t i = 0; i < n; i++) obj += dis[i];
@@ -691,7 +694,7 @@ int orc_kmeans(const float *x_in, int64_t n_in, int d, int k, int niter, int64_t
     }
     orc_kmeans_update(x, n, d, k, assign, centroids_out, hassign);
     orc_kmeans_split(d, k, n, hassign, centroids_out);
-    if (spherical) km_normalize(centroids_out, k, d);
+    if (spherical) orc_kmeans_normalize(centroids_out, k, d);
   }
   if (assign_out && !xsub) memcpy(assign_out, assign, sizeof(int64_t) * n);
   free(assign);
@@ -712,7 +715,7 @@ int orc_pq_train(const float *x, int64_t n, int d, int M, int niter, int64_t see
   int rc = 0;
   for (int m = 0; m < M && rc == 0; m++) {
     for (int64_t i = 0; i < n; i++) memcpy(slice + (size_t)i * dsub, x + (size_t)i * d + (size_t)m * dsub, sizeof(float) * dsub);
-    rc = orc_kmeans(slice, n, dsub, ORC_KSUB, niter, seed, 0, 256, pq_centroids_out + (size_t)m * ORC_KSUB * dsub, NULL,
+    rc = orc_kmeans(slice, n, dsub, ORC_KSUB, niter, seed, 0, 0, 256, pq_centroids_out + (size_t)m * ORC_KSUB * dsub, NULL,
                     NULL);
   }
   free(slice);

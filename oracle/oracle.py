@@ -194,15 +194,34 @@ def kmeans_update(x, k, assign_ids):
     return cent, hassign
 
 
-def kmeans(x, k, niter=25, seed=1234, spherical=False, max_points_per_centroid=256):
+def kmeans_split(hassign, centroids, n):
+    """faiss's split_clusters (EPS = 1/1024, rng(1234)) on copies: every empty cluster re-seeded from a big one.  n: the
+    rows trained on.  Returns (centroids, hassign, number of splits)."""
+    cent = _f32(centroids).copy()
+    h = _f32(hassign).copy()
+    k, d = cent.shape
+    ns = lib().orc_kmeans_split(C.c_int(d), C.c_int(k), C.c_int64(n), _p(h), _p(cent))
+    return cent, h, int(ns)
+
+
+def kmeans_normalize(centroids):
+    """spherical k-means' renormalisation of the centroids, on a copy (a zero row stays zero)"""
+    cent = _f32(centroids).copy()
+    k, d = cent.shape
+    lib().orc_kmeans_normalize(_p(cent), C.c_int(k), C.c_int(d))
+    return cent
+
+
+def kmeans(x, k, niter=25, seed=1234, spherical=False, max_points_per_centroid=256, l2_assign=False):
+    """l2_assign: spherical, but assigned by L2 (the clustering index IVFPQFastScan and VEARCH keep under IP)"""
     x = _f32(x)
     n, d = x.shape
     cent = np.empty((k, d), np.float32)
     assign_ids = np.full(n, -1, np.int64)
     obj = np.zeros(niter, np.float32)
     rc = lib().orc_kmeans(_p(x), C.c_int64(n), C.c_int(d), C.c_int(k), C.c_int(niter), C.c_int64(seed),
-                          C.c_int(1 if spherical else 0), C.c_int(max_points_per_centroid), _p(cent), _p(assign_ids),
-                          _p(obj))
+                          C.c_int(1 if spherical else 0), C.c_int(1 if l2_assign else 0), C.c_int(max_points_per_centroid),
+                          _p(cent), _p(assign_ids), _p(obj))
     assert rc == 0
     return cent, assign_ids, obj
 

@@ -51,6 +51,7 @@ def _declare(l):
         getattr(l, n).restype = i64
         getattr(l, n).argtypes = [vp]
     l.gb_index_is_trained.argtypes = [vp]
+    l.gb_index_training_threshold.restype = i64
     l.gb_index_training_threshold.argtypes = [vp]
     l.gb_index_mem_bytes.restype = i64
     l.gb_index_mem_bytes.argtypes = [vp, i32]
@@ -123,6 +124,7 @@ def _declare(l):
     l.gb_index_vearch_encode.argtypes = [vp, i64, vp, vp, vp]
     l.gb_index_vearch_lut.argtypes = [vp, i32, vp, vp, vp]
     l.gb_kmeans.argtypes = [i32, vp, i64, i32, i32, i32, i64, i32, i32, vp, vp]
+    l.gb_debug_kmeans_trace.argtypes = [i32, vp, i64, i32, i32, i32, i64, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
     l.gb_kmeans_update.argtypes = [i32, vp, i64, i32, i32, vp, vp]
     l.gb_device_pool_usage.argtypes = [i32, i32, C.POINTER(i64), C.POINTER(i64)]
     l.gb_memory_ledger.argtypes = [i32, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64)]

@@ -47,6 +47,12 @@ __host__ __device__ __forceinline__ uint32_t score2ord(float s) {
 __host__ __device__ __forceinline__ uint32_t score2ord(float s, int metric) {
   return metric == kMetricL2 ? f2ord(s) : ~f2ord(s);
 }
+// ord of an arg-min key (k-means and list assignment): a NaN score ranks after every number, whatever its sign bit
+// and the metric, as faiss's `dis < best` never takes one
+template <int METRIC>
+__host__ __device__ __forceinline__ uint32_t argmin_ord(float s) {
+  return s != s ? 0xFFFFFFFFu : score2ord<METRIC>(s);
+}
 __host__ __device__ __forceinline__ float ord2score(uint32_t o, int metric) {
   return metric == kMetricL2 ? ord2f(o) : ord2f(~o);
 }

@@ -223,7 +223,7 @@ class Engine {
   // entries that updates tombstoned and `bitmap` marks deleted.  A failure is logged and leaves the index as it was.
   void purge_indexes(const uint8_t* bitmap, size_t bytes);
   int max_docid_ = 0, delete_num_ = 0;
-  int training_threshold_ = 0;
+  int64_t training_threshold_ = 0;  // the index's clamp can pass 2^31 rows (256 * nlist)
   int refresh_interval_ = 1000;
   bool enable_id_cache_ = false, enable_realtime_ = false;
   int slow_search_time_ = 0;

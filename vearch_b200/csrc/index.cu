@@ -1380,8 +1380,44 @@ static int subsample_rows(const float* x, int64_t n, int64_t n_out, int dpad, co
   return 0;
 }
 
+// the k x d centroids appended to a trace's snapshot (stream-ordered, synchronous)
+static cudaError_t trace_centroids(const float* centroids, int64_t ldc, int k, int d, std::vector<float>& out,
+                                   cudaStream_t st) {
+  const size_t at = out.size();
+  out.resize(at + (size_t)k * d);
+  cudaError_t e = cudaMemcpy2DAsync(out.data() + at, (size_t)d * 4, centroids, (size_t)ldc * 4, (size_t)d * 4, k,
+                                    cudaMemcpyDeviceToHost, st);
+  return e != cudaSuccess ? e : cudaStreamSynchronize(st);
+}
+
+// The rows whose every tensor-core score is NaN (ord 0xFFFFFFFF as argmin_ord ranks it): a row holding a NaN, or an
+// infinity, whose TF32 split hi + (inf - hi) carries a NaN into every dot.  Scored again on the exact kernel, an
+// infinite row keeps its +-inf scores, so under IP it goes to the first centroid whose dot is +inf, as faiss's and the
+// CUDA-core assignment do.  h_best: the rows' keys on the host, updated in place.
+static int rescore_unscored(const float* x, int64_t ldx, int64_t n, int d, int dpad, const float* centroids, int64_t ldc,
+                            int k, int metric, std::vector<unsigned long long>& h_best, cudaStream_t st) {
+  std::vector<int32_t> rows;
+  for (int64_t i = 0; i < n; i++)
+    if ((uint32_t)(h_best[i] >> 32) == 0xFFFFFFFFu) rows.push_back((int32_t)i);
+  if (rows.empty()) return 0;
+  const int64_t m = (int64_t)rows.size();
+  Scratch s(st);
+  GB_ALLOC(d_rows, int32_t, m, s);
+  GB_ALLOC(xr, float, (size_t)m * dpad, s);
+  GB_ALLOC(kr, unsigned long long, m, s);
+  GB_CUDA(cudaMemcpyAsync(d_rows, rows.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
+  GB_CUDA(launch_gather_rows(x, ldx, d_rows, m, d, xr, dpad, st));
+  GB_CUDA(launch_fill_u64(kr, m, kKeySentinel, st));
+  GB_CUDA(launch_dist_argmin(xr, dpad, (int)m, centroids, ldc, k, dpad, metric, kr, 0, st));
+  std::vector<unsigned long long> hk(m);
+  GB_CUDA(cudaMemcpyAsync(hk.data(), kr, (size_t)m * 8, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  for (int64_t j = 0; j < m; j++) h_best[rows[j]] = hk[j];
+  return 0;
+}
+
 int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k, const KMeansParams& kp,
-                  float* centroids, int64_t ldc, cudaStream_t st, std::vector<float>* obj) {
+                  float* centroids, int64_t ldc, cudaStream_t st, std::vector<float>* obj, KMeansTrace* trace) {
   if (n_in < k) {
     set_last_error("kmeans: fewer training points than centroids");
     return -1;
@@ -1398,6 +1434,7 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
   if (kp.max_points_per_centroid > 0 && n_in > (int64_t)k * kp.max_points_per_centroid) {
     n = (int64_t)k * kp.max_points_per_centroid;
     rand_perm_mt(perm, n_in, kp.seed);
+    if (trace) trace->sample.assign(perm.begin(), perm.begin() + n);
     GB_ALLOC(d_idx, int32_t, n, s);
     GB_CUDA(cudaMemcpyAsync(d_idx, perm.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
     GB_ALLOC(xs, float, (size_t)n * dpad, s);
@@ -1416,6 +1453,7 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
     if (kp.spherical) GB_CUDA(launch_normalize_rows(centroids, ldc, k, d, st));
   }
   GB_CUDA(cudaStreamSynchronize(st));
+  if (trace) GB_CUDA(trace_centroids(centroids, ldc, k, d, trace->init, st));
 
   GB_ALLOC(best, unsigned long long, n, s);
   std::vector<unsigned long long> h_best(n);
@@ -1432,13 +1470,22 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
     }
     GB_CUDA(cudaMemcpyAsync(h_best.data(), best, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
     GB_CUDA(cudaStreamSynchronize(st));
+    if (use_tc && rescore_unscored(x, ldx, n, d, dpad, centroids, ldc, k, metric, h_best, st)) return -1;
     // stable counting sort of the points by label (point order inside a cluster = faiss's sum order)
     std::fill(h_off.begin(), h_off.end(), 0);
     double o = 0;
     for (int64_t i = 0; i < n; i++) {
-      if ((uint32_t)h_best[i] >= (uint32_t)k) h_best[i] &= 0xFFFFFFFF00000000ull;  // NaN rows -> cluster 0
+      // faiss's assignment takes a centroid only when its score beats the start value FLT_MAX (-FLT_MAX under IP):
+      // a row without one (NaN, infinite) goes to cluster 0
+      const float sc = ord2score((uint32_t)(h_best[i] >> 32), metric);
+      if ((uint32_t)h_best[i] >= (uint32_t)k || !(metric == kMetricL2 ? sc < FLT_MAX : sc > -FLT_MAX))
+        h_best[i] &= 0xFFFFFFFF00000000ull;
       h_off[(uint32_t)h_best[i] + 1]++;
-      if (obj) o += ord2score((uint32_t)(h_best[i] >> 32), metric);
+      if (obj) o += sc;
+      if (trace) {
+        trace->labels.push_back((int32_t)(uint32_t)h_best[i]);
+        trace->scores.push_back(sc);
+      }
     }
     if (obj) obj->push_back((float)o);
     for (int c = 0; c < k; c++) {
@@ -1450,6 +1497,7 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
     GB_CUDA(cudaMemcpyAsync(d_perm, h_perm.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
     GB_CUDA(cudaMemcpyAsync(d_off, h_off.data(), (size_t)(k + 1) * 4, cudaMemcpyHostToDevice, st));
     GB_CUDA(launch_segment_mean(x, ldx, d, d_perm, d_off, k, centroids, ldc, st));
+    if (trace) GB_CUDA(trace_centroids(centroids, ldc, k, d, trace->mean, st));
     // split_clusters: re-seed empty clusters from big ones (EPS = 1/1024, rng(1234))
     bool any_empty = false;
     for (int c = 0; c < k; c++) any_empty |= (hassign[c] == 0);
@@ -1484,8 +1532,10 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
       }
       GB_CUDA(cudaMemcpyAsync(centroids, h_cent.data(), (size_t)k * ldc * 4, cudaMemcpyHostToDevice, st));
     }
+    if (trace) GB_CUDA(trace_centroids(centroids, ldc, k, d, trace->split, st));
     if (kp.spherical) GB_CUDA(launch_normalize_rows(centroids, ldc, k, d, st));
     GB_CUDA(cudaStreamSynchronize(st));
+    if (trace) GB_CUDA(trace_centroids(centroids, ldc, k, d, trace->norm, st));
   }
   return 0;
 }
@@ -1541,14 +1591,15 @@ int IVFFlatIndex::get_list_shifts(float* host) const {
   return 0;
 }
 
-int IvfIndex::training_threshold() const {
-  // Indexing() clamps to [39, 256] * nlist (gamma_index_ivfflat.cc:350-375, gamma_index_ivfpq.cc:304-329)
+int64_t IvfIndex::training_threshold() const {
+  // Indexing() clamps to [39, 256] * nlist in size_t (gamma_index_ivfflat.cc:350-375, gamma_index_ivfpq.cc:304-329):
+  // from nlist = 2^23 on, 256 * nlist no longer fits an int
   int64_t t = mp_.training_threshold ? mp_.training_threshold : default_training_threshold();
   if (t < nlist_)
     t = (int64_t)nlist_ * 39;
   else if (t > (int64_t)nlist_ * 256)
     t = (int64_t)nlist_ * 256;
-  return (int)t;
+  return t;
 }
 static int64_t tc_tile_bytes(int dpad) { return tc_mirror_tile_floats((int)round_up(dpad, 16)) * 4 + 512; }
 int64_t IvfIndex::index_mem_bytes() const {

@@ -278,7 +278,7 @@ class Index {
   RawStore& store() { return *store_; }
   int64_t indexed_count() const { return indexed_count_; }
   bool trained() const { return trained_; }
-  virtual int training_threshold() const { return 0; }
+  virtual int64_t training_threshold() const { return 0; }
   // whether Engine::Dump saves the trained state (centroids, codebook) beside the rows for Load to restore; false: the
   // trained state lives only in the type's index file (dump_gamma), and Load trains again when that file is missing or
   // refused
@@ -500,8 +500,18 @@ struct KMeansParams {
   bool hot_start = false;  // keep the centroids passed in as the initial state (ProductQuantizer::Train_hot_start)
   bool l2_assign = false;  // spherical, but assign by L2 (quantiser IndexFlatL2, as IVFPQFastScan has under IP)
 };
+// What one kmeans_device run did, step by step (gb_debug_kmeans_trace; DESIGN.md §5, training bar).  n_s = the rows
+// trained on, k x d centroid snapshots.
+struct KMeansTrace {
+  std::vector<int32_t> sample;            // [n_s] the rows of x sampled (empty: all of them, in order)
+  std::vector<float> init;                // [k][d] the initial centroids
+  std::vector<int32_t> labels;            // [niter][n_s] each row's cluster
+  std::vector<float> scores;              // [niter][n_s] the score its key carried
+  std::vector<float> mean, split, norm;   // [niter][k][d] after the segmented mean, the split, the renormalisation
+};
+// trace: nullptr on every production path
 int kmeans_device(const float* x, int64_t ldx, int64_t n, int d, int k, const KMeansParams& kp, float* centroids,
-                  int64_t ldc, cudaStream_t st, std::vector<float>* obj);
+                  int64_t ldc, cudaStream_t st, std::vector<float>* obj, KMeansTrace* trace = nullptr);
 
 // What an IVF index's codec puts into gamma's index file (index_io.cu)
 struct GammaFileFormat {
@@ -518,7 +528,7 @@ class IvfIndex : public Index {
  public:
   IvfIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int row_bytes = 0);
   ~IvfIndex() override;
-  int training_threshold() const override;
+  int64_t training_threshold() const override;
   int train() override;
   int add_pending(const uint8_t* del_bitmap) override;
   int update_vector(int64_t vid, const void* x) override;
@@ -997,7 +1007,7 @@ class ShardedIndex : public Index {
   ~ShardedIndex() override;
   int nshards() const { return (int)shards_.size(); }
   IvfIndex* shard(int s) { return shards_[s].get(); }
-  int training_threshold() const override { return shards_[0]->training_threshold(); }
+  int64_t training_threshold() const override { return shards_[0]->training_threshold(); }
   int train() override;
   int add_pending(const uint8_t* del_bitmap) override;
   int update_vector(int64_t vid, const void* x) override;

@@ -373,7 +373,7 @@ int gb_index_add_pending(gb_index* index, const uint8_t* del_bitmap) {
 int64_t gb_index_ntotal(gb_index* index) { return index && index->impl ? index->impl->store().size() : -1; }
 int64_t gb_index_indexed_count(gb_index* index) { return index && index->impl ? index->impl->indexed_count() : -1; }
 int gb_index_is_trained(gb_index* index) { return index && index->impl ? (int)index->impl->trained() : 0; }
-int gb_index_training_threshold(gb_index* index) {
+int64_t gb_index_training_threshold(gb_index* index) {
   return index && index->impl ? index->impl->training_threshold() : -1;
 }
 int64_t gb_index_mem_bytes(gb_index* index, int which) {
@@ -770,8 +770,11 @@ int gb_index_vearch_lut(gb_index* index, int nq, const float* x, uint8_t* lut, f
   return vr->lut_host(nq, x, lut, mult);
 }
 
-int gb_kmeans(int device, const float* x, int64_t n, int d, int k, int niter, int64_t seed, int spherical,
-              int max_points_per_centroid, float* centroids, float* obj) {
+}  // extern "C"
+
+// kmeans_device on host rows: gb_kmeans and its trace.  init: nullptr, or k x d starting centroids (hot start)
+static int kmeans_host(int device, const float* x, int64_t n, int d, int k, KMeansParams kp, const float* init,
+                       float* centroids, std::vector<float>* obj, KMeansTrace* trace) {
   if (cudaSetDevice(device) != cudaSuccess) {
     set_last_error("no CUDA device");
     return -1;
@@ -785,27 +788,59 @@ int gb_kmeans(int device, const float* x, int64_t n, int d, int k, int niter, in
     float* dx = s.alloc_n<float>((size_t)n * dpad);
     float* dc = s.alloc_n<float>((size_t)k * dpad);
     if (dx && dc && cudaMemsetAsync(dc, 0, (size_t)k * dpad * 4, st) == cudaSuccess &&
-        upload_rows_padded(dx, x, n, d, dpad, st) == cudaSuccess) {
-      KMeansParams kp;
-      kp.niter = niter;
-      kp.seed = seed;
-      kp.spherical = spherical != 0;
-      kp.max_points_per_centroid = max_points_per_centroid;
-      std::vector<float> o;
-      rc = kmeans_device(dx, dpad, n, d, k, kp, dc, dpad, st, obj ? &o : nullptr);
-      if (rc == 0) {
-        if (cudaMemcpy2DAsync(centroids, (size_t)d * 4, dc, (size_t)dpad * 4, (size_t)d * 4, k, cudaMemcpyDeviceToHost,
-                              st) != cudaSuccess ||
-            cudaStreamSynchronize(st) != cudaSuccess)
-          rc = -1;
-        if (obj)
-          for (size_t i = 0; i < o.size(); i++) obj[i] = o[i];
-      }
+        upload_rows_padded(dx, x, n, d, dpad, st) == cudaSuccess &&
+        (!init || cudaMemcpy2DAsync(dc, (size_t)dpad * 4, init, (size_t)d * 4, (size_t)d * 4, k, cudaMemcpyHostToDevice,
+                                    st) == cudaSuccess)) {
+      kp.hot_start = init != nullptr;
+      rc = kmeans_device(dx, dpad, n, d, k, kp, dc, dpad, st, obj, trace);
+      if (rc == 0 && (cudaMemcpy2DAsync(centroids, (size_t)d * 4, dc, (size_t)dpad * 4, (size_t)d * 4, k,
+                                        cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+                      cudaStreamSynchronize(st) != cudaSuccess))
+        rc = -1;
     }
   }
   cudaStreamSynchronize(st);
   cudaStreamDestroy(st);
   return rc;
+}
+
+extern "C" {
+
+int gb_kmeans(int device, const float* x, int64_t n, int d, int k, int niter, int64_t seed, int spherical,
+              int max_points_per_centroid, float* centroids, float* obj) {
+  KMeansParams kp;
+  kp.niter = niter;
+  kp.seed = seed;
+  kp.spherical = spherical != 0;
+  kp.max_points_per_centroid = max_points_per_centroid;
+  std::vector<float> o;
+  const int rc = kmeans_host(device, x, n, d, k, kp, nullptr, centroids, obj ? &o : nullptr, nullptr);
+  if (rc == 0 && obj)
+    for (size_t i = 0; i < o.size(); i++) obj[i] = o[i];
+  return rc;
+}
+
+int gb_debug_kmeans_trace(int device, const float* x, int64_t n, int d, int k, int niter, int64_t seed, int spherical,
+                          int l2_assign, int max_points_per_centroid, const float* init, int64_t* sample,
+                          float* init_out, int32_t* labels, float* scores, float* mean, float* split, float* norm) {
+  KMeansParams kp;
+  kp.niter = niter;
+  kp.seed = seed;
+  kp.spherical = spherical != 0;
+  kp.l2_assign = l2_assign != 0;
+  kp.max_points_per_centroid = max_points_per_centroid;
+  KMeansTrace t;
+  std::vector<float> cent((size_t)k * d);
+  if (kmeans_host(device, x, n, d, k, kp, init, cent.data(), nullptr, &t)) return -1;
+  const int64_t ns = t.sample.empty() ? n : (int64_t)t.sample.size();
+  for (int64_t i = 0; i < ns; i++) sample[i] = t.sample.empty() ? i : t.sample[i];
+  std::copy(t.init.begin(), t.init.end(), init_out);
+  std::copy(t.labels.begin(), t.labels.end(), labels);
+  std::copy(t.scores.begin(), t.scores.end(), scores);
+  std::copy(t.mean.begin(), t.mean.end(), mean);
+  std::copy(t.split.begin(), t.split.end(), split);
+  std::copy(t.norm.begin(), t.norm.end(), norm);
+  return 0;
 }
 
 int gb_kmeans_update(int device, const float* x, int64_t n, int d, int k, const int64_t* assign, float* centroids) {

@@ -113,7 +113,7 @@ __global__ void __launch_bounds__(NT)
       for (int j = 0; j < TN; j++) {
         int gc = col0 + tx * TN + j;
         if (gc < m) {
-          unsigned long long key = make_key(score2ord<METRIC>(acc[i][j]), (uint32_t)(gc + col_base));
+          unsigned long long key = make_key(argmin_ord<METRIC>(acc[i][j]), (uint32_t)(gc + col_base));
           kbest = key < kbest ? key : kbest;
         }
       }

@@ -163,10 +163,15 @@ __device__ __forceinline__ void tc_tile_run(unsigned char* smem, TcShared* sh, c
   *an = an_acc;
 }
 
+// the unclamped score: the expanded L2 form, or the dot
+template <int METRIC>
+__device__ __forceinline__ float tc_raw(float dot, float xn, float cn) {
+  return METRIC == kMetricL2 ? fmaf(-2.0f, dot, xn + cn) : dot;
+}
 template <int METRIC>
 __device__ __forceinline__ float tc_score(float dot, float xn, float cn) {
   // faiss IndexFlat clamps the expanded L2 form at 0 (SURVEY Appendix A)
-  return METRIC == kMetricL2 ? fmaxf(0.f, fmaf(-2.0f, dot, xn + cn)) : dot;
+  return METRIC == kMetricL2 ? fmaxf(0.f, tc_raw<METRIC>(dot, xn, cn)) : dot;
 }
 
 // ---- K2 / K6: dense score tile or fused row arg-min ----------------------------------------
@@ -194,10 +199,12 @@ __global__ void __launch_bounds__(TC_NT)
 #pragma unroll
     for (int j = 0; j < 32; j++) {
       const int gc = col0 + c0 + j;
-      const float s = tc_score<METRIC>(__uint_as_float(v[j]), xn, sh.cn[c0 + j]);
+      const float raw = tc_raw<METRIC>(__uint_as_float(v[j]), xn, sh.cn[c0 + j]);
+      const float s = METRIC == kMetricL2 ? fmaxf(0.f, raw) : raw;
       if (gr < n && gc < m) {
         if (EPI_ARGMIN) {
-          unsigned long long key = make_key(score2ord<METRIC>(s), (uint32_t)gc);
+          // a NaN before L2's clamp at 0 (a NaN or infinite operand: the split of inf is NaN) stays NaN for the key
+          unsigned long long key = make_key(argmin_ord<METRIC>(raw != raw ? raw : s), (uint32_t)gc);
           kbest = key < kbest ? key : kbest;
         } else {
           out[(int64_t)gr * ldo + gc] = s;

@@ -661,6 +661,28 @@ def kmeans(x, k, niter=25, seed=1234, spherical=False, max_points_per_centroid=2
     return cent, obj
 
 
+def debug_kmeans_trace(x, k, niter=25, seed=1234, spherical=False, l2_assign=False, max_points_per_centroid=256,
+                       init=None, device=0):
+    """One k-means run (the engine's training k-means), traced step by step: a dict of numpy arrays.  sample [n_s]:
+    the rows of x trained on; init [k, d]: the initial centroids (`init` given: a hot start from them); labels and
+    scores [niter, n_s]: each row's cluster and the score its key carried; mean, split, norm [niter, k, d]: the
+    centroids after the segmented mean, the empty-cluster split and the spherical renormalisation."""
+    x = _f32(x)
+    n, d = x.shape
+    ns = min(n, k * max_points_per_centroid) if max_points_per_centroid > 0 else n
+    out = {"sample": np.empty(ns, np.int64), "init": np.empty((k, d), np.float32),
+           "labels": np.empty((niter, ns), np.int32), "scores": np.empty((niter, ns), np.float32)}
+    for s in ("mean", "split", "norm"):
+        out[s] = np.empty((niter, k, d), np.float32)
+    init = None if init is None else _f32(init).reshape(k, d)
+    _check(_lib.lib().gb_debug_kmeans_trace(device, _ptr(x), n, d, k, niter, seed, int(spherical), int(l2_assign),
+                                            max_points_per_centroid, _ptr(init), _ptr(out["sample"]),
+                                            _ptr(out["init"]), _ptr(out["labels"]), _ptr(out["scores"]),
+                                            _ptr(out["mean"]), _ptr(out["split"]), _ptr(out["norm"])),
+           "debug_kmeans_trace")
+    return out
+
+
 def kmeans_update(x, k, assign, device=0):
     x = _f32(x)
     assign = np.ascontiguousarray(assign, np.int64)
