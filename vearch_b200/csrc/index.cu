@@ -2244,9 +2244,8 @@ int IvfIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int
   if (!xq) return -1;
   const int nprobe = resolve_nprobe(ctx);
   const int64_t ld = store_->stride();
-  const int QB = 16384;
-  for (int q0 = 0; q0 < nq; q0 += QB) {
-    int qb = std::min(QB, nq - q0);
+  for (int q0 = 0; q0 < nq; q0 += kQueryBlock) {
+    int qb = std::min(kQueryBlock, nq - q0);
     Scratch sb(s.stream());
     GB_ALLOC(probe_ids, int32_t, (size_t)qb * nprobe, sb);
     GB_ALLOC(coarse_dis, float, (size_t)qb * nprobe, sb);
@@ -2313,7 +2312,16 @@ int IvfIndex::search_preassigned_host(const SearchContext& ctx, int nq, const vo
   GB_ALLOC(okeys, unsigned long long, (size_t)nq * k, s);
   const float* dqt = transform_dev(static_cast<const float*>(dq), nq, s);
   if (!dqt) return -1;
-  if (scan_dev(ctx, f, metric, nq, dqt, dq, k, ids, dis, nprobe, okeys, s)) return -1;
+  // in query blocks, as search_keys_dev: the scan launchers take at most 65535 queries (one grid row each)
+  const int64_t ld = store_->stride();
+  for (int q0 = 0; q0 < nq; q0 += kQueryBlock) {
+    const int qb = std::min(kQueryBlock, nq - q0);
+    Scratch sb(st);
+    if (scan_dev(ctx, f, metric, qb, reinterpret_cast<const unsigned char*>(dqt) + q0 * ld,
+                 static_cast<const unsigned char*>(dq) + q0 * ld, k, ids + (int64_t)q0 * nprobe,
+                 dis + (int64_t)q0 * nprobe, nprobe, okeys + (int64_t)q0 * k, sb))
+      return -1;
+  }
   return download_results(okeys, nq, k, metric, out_dis, out_ids, s);  // synchronises before h goes
 }
 
@@ -2743,16 +2751,17 @@ int IVFPQIndex::scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const
   const long long pa_target = 4 * (long long)kk;
   const int cap = std::max(2048, std::min(8192, next_pow2(8 * kk)));
   const int nsm = sm_count(device_);
+  const int pgA = nq >= nsm * 4 ? std::min(pa_max, 32) : 1;  // one CTA per query when there are queries enough
   snprintf(last_scan_info_, sizeof(last_scan_info_),
-           "{\"phase_a_max_probes\": %d, \"phase_a_target_entries\": %lld, \"candidate_cap\": %d, \"kprime\": %d}", pa_max,
-           pa_target, cap, kk);
+           "{\"phase_a_max_probes\": %d, \"phase_a_probes_per_cta\": %d, \"phase_a_target_entries\": %lld, "
+           "\"candidate_cap\": %d, \"kprime\": %d}",
+           pa_max, pgA, pa_target, cap, kk);
   GB_ALLOC(d_probes_a, int32_t, npairs, s);
   GB_ALLOC(d_probes_b, int32_t, npairs, s);
   GB_ALLOC(d_row_limit, int, npairs, s);
   GB_CUDA(launch_pqtc_plan_phase_a(probe_ids, npairs, nprobe, pa_max, pa_target, dir.len, d_probes_a, d_probes_b, d_row_limit,
                                    st));
 
-  const int pgA = nq >= nsm * 4 ? std::min(pa_max, 32) : 1;  // one CTA per query when there are queries enough
   const int ngA = (pa_max + pgA - 1) / pgA;
   GB_ALLOC(partA, unsigned long long, (size_t)nq * ngA * kk, s);
   unsigned long long* keysA = partA;

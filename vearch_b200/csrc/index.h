@@ -270,6 +270,8 @@ class Index {
   // bytes of per-(query, part) partial keys one scan step may hold (FLAT chunks, IVF-Flat query-major splits); larger
   // batches are cut into query blocks
   static constexpr int64_t kScanPartialBudget = (int64_t)1 << 30;
+  // queries an IVF search hands its coarse quantiser and list scan at once (the scan launchers take <= 65535)
+  static constexpr int kQueryBlock = 16384;
   bool gpu_contract() const { return gpu_contract_; }
   int d() const { return d_; }
   int device() const { return device_; }
