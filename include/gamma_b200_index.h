@@ -274,6 +274,9 @@ int gb_debug_roundtrip_doc(const char *buf, int len, char **out, int *out_len);
 int gb_debug_parse_table(const char *buf, int len, char **json_out, int *out_len);
 int gb_debug_encode_response(int nq, int k, const double *scores, const char *const *keys, int total, char **out,
                              int *out_len);
+/* the run-time index records (AddFieldIndexWithParams / RemoveFieldIndex) at the end of a snapshot's last len bytes,
+ * as JSON {"bytes": n, "records": [[field, has_index, type, params], ...]}; -1 if a record does not parse */
+int gb_debug_index_records(const char *tail, int64_t len, char **json_out, int *out_len);
 
 #ifdef __cplusplus
 }

@@ -130,6 +130,7 @@ def _declare(l):
     l.gb_memory_ledger.argtypes = [i32, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64)]
     l.gb_memory_set_total.restype = None
     l.gb_memory_set_total.argtypes = [i32, i64]
+    l.gb_debug_index_records.argtypes = [C.c_char_p, i64, C.POINTER(C.c_void_p), C.POINTER(i32)]
     l.gb_merge_partitions_device.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, vp]
 
 

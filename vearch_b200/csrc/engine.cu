@@ -4,7 +4,9 @@
 #include <float.h>
 #include <stdio.h>
 #include <string.h>
+#include <dirent.h>
 #include <sys/stat.h>
+#include <unistd.h>
 
 #include <algorithm>
 #include <chrono>
@@ -252,9 +254,15 @@ void quiesce_all_engines() {
 }  // namespace
 
 void Engine::quiesce() {
+  field_build_stop_.store(true);
+  join_field_build();
+  stop_indexing();
+}
+void Engine::stop_indexing() {
   int st = indexing_state_.load();
   if (st != 0) indexing_state_.store(3);
   idx_cv_.notify_all();
+  std::lock_guard<std::mutex> g(indexing_thread_mu_);
   if (indexing_thread_.joinable()) indexing_thread_.join();
 }
 
@@ -313,6 +321,7 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
         tt > 0)
       training_threshold_ = tt;
   }
+  table_training_threshold_ = training_threshold_;
   // index type of the vector field: first entry of `indexes` with a matching field_name
   // (vector_manager.cc:365-373)
   index_type_.clear();
@@ -325,24 +334,12 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     }
   }
   if (index_type_.empty()) return Status::Make(kInvalidArgument, vec_name_ + " index type is empty");
-  ModelParams mp;
-  std::string err;
-  if (!parse_model_params(index_params_, index_type_, &mp, &err)) return Status::Make(kInvalidArgument, err);
-  if (table_index_params.empty() && mp.training_threshold > training_threshold_)
-    training_threshold_ = mp.training_threshold;  // table.cc:143-150
-  if (training_threshold_ > 0) mp.training_threshold = training_threshold_;
-  mp.host_store = !strcasecmp(v.str(4).c_str(), "RocksDB");  // VectorInfo.store_type
-  // BINARYIVF: the field's values are packed bits, dimension / 8 bytes (vector_manager.cc:100-130); a table with more
-  // than one vector field cannot join Hamming and float scores here
-  if (index_type_ == "BINARYIVF" && nvec > 1)
-    return Status::Make(kNotSupported, vec_name_ + ": BINARYIVF is not supported in a multi-vector table");
-  Index* idx = make_index(index_type_, dim_, mp);
-  if (!idx) return Status::Make(index_type_ == "FLAT" || index_type_ == "IVFFLAT" || index_type_ == "IVFPQ" ||
-                                        index_type_ == "IVFPQFastScan" || index_type_ == "BINARYIVF" ||
-                                        index_type_ == "IVFRABITQ" || index_type_ == "VEARCH" || is_gpu_index_type(index_type_)
-                                    ? kInvalidArgument
-                                    : kNotSupported,
-                                last_error());
+  table_params_given_ = !table_index_params.empty();
+  Index* idx = nullptr;
+  Status ist = create_field_index(vec_name_, dim_, index_type_, index_params_, true,
+                                  !strcasecmp(v.str(4).c_str(), "RocksDB"),  // VectorInfo.store_type
+                                  nvec, &training_threshold_, &idx);
+  if (!ist.ok()) return ist;
   index_.reset(idx);
   vbytes_ = (size_t)idx->store().row_bytes();
   extra_.clear();
@@ -361,14 +358,11 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
       }
     }
     if (vf.index_type.empty()) return Status::Make(kInvalidArgument, vf.name + " index type is empty");
-    ModelParams emp;
-    if (!parse_model_params(vf.index_params, vf.index_type, &emp, &err)) return Status::Make(kInvalidArgument, err);
-    if (training_threshold_ > 0) emp.training_threshold = training_threshold_;
-    emp.host_store = !strcasecmp(ev.str(4).c_str(), "RocksDB");
-    if (vf.index_type == "BINARYIVF")
-      return Status::Make(kNotSupported, vf.name + ": BINARYIVF is not supported in a multi-vector table");
-    Index* eidx = make_index(vf.index_type, vf.dim, emp);
-    if (!eidx) return Status::Make(kInvalidArgument, last_error());
+    int64_t ett = training_threshold_;
+    Index* eidx = nullptr;
+    Status est = create_field_index(vf.name, vf.dim, vf.index_type, vf.index_params, false,
+                                    !strcasecmp(ev.str(4).c_str(), "RocksDB"), nvec, &ett, &eidx);
+    if (!est.ok()) return est;
     vf.index.reset(eidx);
     extra_.push_back(std::move(vf));
   }
@@ -381,6 +375,7 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
   if (training_threshold_ <= 0) training_threshold_ = index_->training_threshold();
   for (size_t fi = 0; fi < fields_.size(); fi++)
     if (fields_[fi].indexed && scalar_index_rebuild((int)fi)) return Status::Make(kIndexError, last_error());
+  fidx_.assign(nvec, FieldIndex());
   created_table_ = true;
   // <path>/<table>.schema, as the reference writes it (engine.cc:676-684)
   if (!path_.empty()) {
@@ -389,6 +384,19 @@ Status Engine::CreateTable(const uint8_t* fb, size_t len) {
     if (f) f.write(reinterpret_cast<const char*>(fb), (std::streamsize)len);
   }
   return Status::OK();
+}
+
+int Engine::vec_field(const std::string& name) const {
+  if (name == vec_name_) return 0;
+  for (size_t i = 0; i < extra_.size(); i++)
+    if (extra_[i].name == name) return (int)i + 1;
+  return -1;
+}
+std::shared_ptr<Index> Engine::index_ref(const std::string& vec_name, int* dim) {
+  const int vi = vec_field(vec_name);
+  if (vi < 0) return nullptr;
+  *dim = vdim(vi);
+  return std::atomic_load(&vslot(vi));
 }
 
 Index* Engine::index_of(const std::string& vec_name, int* dim) {
@@ -499,6 +507,7 @@ int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
       std::vector<unsigned char> x(vec, vec + vec_len);
       if (flush_pending_locked()) return -1;
       if (index_->update_vector(docid, x.data())) return -1;
+      if (fidx_[0].building) fidx_[0].updated.push_back(docid);
     }
     for (size_t ei = 0; ei < extra_.size(); ei++) {
       if (!evec[ei].first) continue;
@@ -507,6 +516,7 @@ int Engine::AddOrUpdate(const uint8_t* fb, size_t len) {
       memcpy(x.data(), evec[ei].first, evec[ei].second);
       if (flush_pending_locked()) return -1;
       if (extra_[ei].index->update_vector(docid, x.data())) return -1;
+      if (fidx_[ei + 1].building) fidx_[ei + 1].updated.push_back(docid);
     }
     purge_indexes(delete_num_ > 0 ? del_bitmap_.data() : nullptr, (size_t)(max_docid_ >> 3) + 1);
     return 0;
@@ -563,6 +573,8 @@ int Engine::Delete(const std::string& key) {
   const int64_t vid = docid;
   if (index_) index_->delete_vectors(&vid, 1);
   for (auto& e : extra_) e.index->delete_vectors(&vid, 1);
+  for (auto& fx : fidx_)
+    if (fx.building) fx.deleted.push_back(vid);
   return 0;
 }
 
@@ -815,11 +827,11 @@ Status Engine::Search(const SearchRequestPB& req, std::string* pb_out) {
   if (req.vec_fields.size() > 1) return SearchMulti(req, pb_out);
   const auto& vq = req.vec_fields[0];
   int qdim = 0;
-  Index* qindex = index_of(vq.name, &qdim);
+  std::shared_ptr<Index> qindex = index_ref(vq.name, &qdim);
   if (!qindex) return Status::Make(kInvalidArgument, "Query name " + vq.name + " not exist in created vector table");
   int brute = req.brute_force_search;
   if (brute == 2 && index_status_.load() != 2) brute = 1;
-  if (brute == 0 && index_status_.load() != 2 && max_docid_ > 100 && !enable_realtime_)
+  if (brute == 0 && index_status_.load() != 2 && max_docid_ > 100 && !enable_realtime_ && !awaiting_training_.load())
     return Status::Make(kIndexError, space_name_ + " index not trained, brute_force_search is 0, max_docid_ = " +
                                          std::to_string(max_docid_) + ", threshold = 100");
   const size_t qbytes = (size_t)qindex->store().row_bytes();  // d * 4, or BINARYIVF's d / 8
@@ -855,6 +867,9 @@ Status Engine::Search(const SearchRequestPB& req, std::string* pb_out) {
       wl.unlock();
     }
     rl.lock();
+    const int vi = vec_field(vq.name);
+    qindex = vslot(vi);  // the index a swap left, held until the results are read
+    if (!fidx_[vi].has_index) ctx.params.brute_force = true;  // a field without an index is searched exactly
     if (delete_num_ > 0) {
       bm.assign(del_bitmap_.begin(), del_bitmap_.begin() + (max_docid_ >> 3) + 1);
       ctx.del_bitmap = bm.data();
@@ -962,12 +977,13 @@ static bool parse_ranker(const std::string& raw, size_t nvec, std::vector<double
 
 Status Engine::SearchMulti(const SearchRequestPB& req, std::string* pb_out) {
   const size_t nvec = req.vec_fields.size();
-  std::vector<Index*> idx(nvec);
+  std::vector<std::shared_ptr<Index>> idx(nvec);
   std::vector<int> dims(nvec);
+  std::vector<char> exact(nvec, 0);  // fields without an index are searched exactly
   int n = -1;
   for (size_t j = 0; j < nvec; j++) {
     const auto& vq = req.vec_fields[j];
-    idx[j] = index_of(vq.name, &dims[j]);
+    idx[j] = index_ref(vq.name, &dims[j]);
     if (!idx[j]) return Status::Make(kInvalidArgument, "Query name " + vq.name + " not exist in created vector table");
     const int nj = (int)(vq.value.size() / ((size_t)dims[j] * 4));
     if (nj <= 0 || (n >= 0 && nj != n)) return Status::Make(kInvalidArgument, "Search n shouldn't less than 0!");
@@ -978,7 +994,7 @@ Status Engine::SearchMulti(const SearchRequestPB& req, std::string* pb_out) {
   if (!parse_ranker(req.ranker, nvec, &weights, &err)) return Status::Make(kInvalidArgument, err);
   int brute = req.brute_force_search;
   if (brute == 2 && index_status_.load() != 2) brute = 1;
-  if (brute == 0 && index_status_.load() != 2 && max_docid_ > 100 && !enable_realtime_)
+  if (brute == 0 && index_status_.load() != 2 && max_docid_ > 100 && !enable_realtime_ && !awaiting_training_.load())
     return Status::Make(kIndexError, space_name_ + " index not trained, brute_force_search is 0, max_docid_ = " +
                                          std::to_string(max_docid_) + ", threshold = 100");
   if (IsKilled(req.request_id, req.partition_id)) return Status::Make(kMemoryExceeded, "");
@@ -1001,6 +1017,11 @@ Status Engine::SearchMulti(const SearchRequestPB& req, std::string* pb_out) {
       wl.unlock();
     }
     rl.lock();
+    for (size_t j = 0; j < nvec; j++) {
+      const int vi = vec_field(req.vec_fields[j].name);
+      idx[j] = vslot(vi);
+      exact[j] = !fidx_[vi].has_index;
+    }
     if (delete_num_ > 0) {
       bm.assign(del_bitmap_.begin(), del_bitmap_.begin() + (max_docid_ >> 3) + 1);
       base.del_bitmap = bm.data();
@@ -1034,6 +1055,7 @@ Status Engine::SearchMulti(const SearchRequestPB& req, std::string* pb_out) {
   for (size_t j = 0; j < nvec; j++) {
     const auto& vq = req.vec_fields[j];
     SearchContext ctx = base;
+    if (exact[j]) ctx.params.brute_force = true;
     ctx.min_score = vq.has_min ? (float)std::max(vq.min_score, -(double)FLT_MAX) : (vq.has_max ? 0.f : -FLT_MAX);
     ctx.max_score = vq.has_max ? (float)std::min(vq.max_score, (double)FLT_MAX) : (vq.has_min ? 0.f : FLT_MAX);
     if (!vq.has_min && !vq.has_max) ctx.min_score = -FLT_MAX, ctx.max_score = FLT_MAX;
@@ -1047,7 +1069,7 @@ Status Engine::SearchMulti(const SearchRequestPB& req, std::string* pb_out) {
   // the weighted sum of the per-field scores; docid order unless multi_vector_rank asks for score order
   std::vector<float> out_dis((size_t)n * topN, 0.f);
   std::vector<int64_t> out_ids((size_t)n * topN, -1);
-  const bool l2 = index_->metric() == kMetricL2;
+  const bool l2 = std::atomic_load(&index_)->metric() == kMetricL2;
   for (int i = 0; i < n; i++) {
     std::map<int64_t, std::pair<int, double>> acc;  // docid -> (fields seen, score)
     for (size_t j = 0; j < nvec; j++)
@@ -1170,12 +1192,11 @@ Status Engine::Query(const QueryRequestPB& req, std::string* pb_out) {
   return Status::OK();
 }
 
-Status Engine::SetFieldIndexed(const std::string& field, bool indexed) {
+Status Engine::SetFieldIndexed(const std::string& field, bool indexed, const std::string& index_type,
+                               const std::string& index_params) {
   if (!created_table_) return Status::Make(kIOError, "table not initialized");
+  if (vec_field(field) >= 0) return indexed ? AddFieldIndex(field, index_type, index_params) : RemoveFieldIndex(field);
   std::unique_lock<std::shared_mutex> lk(mu_);
-  int dim = 0;
-  if (index_of(field, &dim))
-    return Status::Make(kNotSupported, "the index of vector field " + field + " is fixed when the table is created");
   auto it = field_idx_.find(field);
   if (it == field_idx_.end()) return Status::Make(kInvalidArgument, "field " + field + " not found");
   cudaSetDevice(device_);
@@ -1192,6 +1213,262 @@ Status Engine::SetFieldIndexed(const std::string& field, bool indexed) {
   return Status::OK();
 }
 
+// CreateTable's rules for the index of one vector field (vector_manager.cc:343-453), for CreateTable and for
+// AddFieldIndex alike
+Status Engine::create_field_index(const std::string& name, int dim, const std::string& type, const std::string& params,
+                                  bool first, bool host, size_t nvec, int64_t* tt, Index** out) const {
+  ModelParams mp;
+  std::string err;
+  if (!parse_model_params(params, type, &mp, &err)) return Status::Make(kInvalidArgument, err);
+  if (first && !table_params_given_ && mp.training_threshold > *tt) *tt = mp.training_threshold;  // table.cc:143-150
+  if (*tt > 0) mp.training_threshold = (int)*tt;
+  mp.host_store = host;
+  // BINARYIVF: the field's values are packed bits, dimension / 8 bytes (vector_manager.cc:100-130); a table with more
+  // than one vector field cannot join Hamming and float scores here
+  if (type == "BINARYIVF" && nvec > 1)
+    return Status::Make(kNotSupported, name + ": BINARYIVF is not supported in a multi-vector table");
+  Index* idx = make_index(type, dim, mp);
+  if (!idx) {
+    const bool known = type == "FLAT" || type == "IVFFLAT" || type == "IVFPQ" || type == "IVFPQFastScan" ||
+                       type == "BINARYIVF" || type == "IVFRABITQ" || type == "VEARCH" || is_gpu_index_type(type);
+    return Status::Make(!first || known ? kInvalidArgument : kNotSupported, last_error());
+  }
+  *out = idx;
+  return Status::OK();
+}
+
+// ---- a vector field's index at run time ---------------------------------------------------------
+// CreateTable's rules for the field, and the raw rows it already stores: the new index must read them as they are
+Status Engine::make_field_index(int vi, const std::string& type, const std::string& params, std::shared_ptr<Index>* out,
+                                int64_t* tt) {
+  const std::string& name = vname(vi);
+  if (type.empty()) return Status::Make(kNotSupported, name + " index type is empty");
+  RawStore& st = vslot(vi)->store();
+  const int row_bytes = type == "BINARYIVF" ? vdim(vi) / 8 : vdim(vi) * 4;
+  if (row_bytes != st.row_bytes())
+    return Status::Make(kInvalidArgument, name + ": a " + type + " index reads rows of " + std::to_string(row_bytes) +
+                                              " bytes, the field stores rows of " + std::to_string(st.row_bytes()));
+  // the first field follows the table's threshold as CreateTable gave it; the others take the engine's
+  int64_t t = vi == 0 ? table_training_threshold_ : training_threshold_;
+  Index* idx = nullptr;
+  Status s = create_field_index(name, vdim(vi), type, params, vi == 0, st.on_host(), fidx_.size(), &t, &idx);
+  if (!s.ok()) return s;
+  out->reset(idx);
+  *tt = t > 0 ? t : idx->training_threshold();
+  return Status::OK();
+}
+
+void Engine::swap_field_index(int vi, std::shared_ptr<Index> nidx, const std::string& type, const std::string& params,
+                              bool has_index, int64_t tt) {
+  std::atomic_store(&vslot(vi), std::move(nidx));  // a search still in the old index keeps it until it returns
+  FieldIndex& fx = fidx_[vi];
+  fx.has_index = has_index;
+  fx.changed = true;
+  vtype(vi) = type;
+  vparams(vi) = params;
+  if (vi == 0) training_threshold_ = tt;
+  bool ready = true;  // every field is trained or has no index
+  for (size_t v = 0; v < fidx_.size(); v++) ready = ready && (!fidx_[v].has_index || vslot((int)v)->trained());
+  // an index swapped in before the field reaches its training threshold is left as CreateTable leaves one: the
+  // indexing thread trains it once the table has enough rows (BuildIndex's rule); until then its searches are exact
+  if (ready) {
+    index_status_.store(2);
+    awaiting_training_.store(false);
+  } else if (has_index && !vslot(vi)->trained()) {
+    index_status_.store(0);
+    awaiting_training_.store(true);
+  }
+}
+
+// the build thread and RemoveFieldIndex call this; field_build_mu_ makes them one pauser at a time
+bool Engine::pause_indexing() {
+  bool was_running = false;
+  for (;;) {
+    int st = indexing_state_.load();
+    if (st == 0) {
+      if (indexing_state_.compare_exchange_strong(st, 4)) break;
+      continue;
+    }
+    was_running = was_running || st == 1 || st == 2;
+    indexing_state_.store(3);
+    idx_cv_.notify_all();
+    std::lock_guard<std::mutex> g(indexing_thread_mu_);
+    if (indexing_thread_.joinable()) indexing_thread_.join();
+  }
+  return was_running;
+}
+void Engine::resume_indexing(bool was_running) {
+  indexing_state_.store(0);
+  if (was_running || index_status_.load() == 2) BuildIndex();
+}
+
+void Engine::join_field_build() {
+  std::lock_guard<std::mutex> g(field_build_mu_);
+  join_field_build_locked();
+}
+void Engine::join_field_build_locked() {
+  if (field_build_thread_.joinable()) field_build_thread_.join();
+}
+
+Status Engine::AddFieldIndex(const std::string& field, const std::string& type, const std::string& params) {
+  const int vi = vec_field(field);
+  if (vi < 0) return Status::Make(kInvalidArgument, "field " + field + " not found");
+  std::lock_guard<std::mutex> g(field_build_mu_);  // join, validate and spawn as one step
+  join_field_build_locked();  // one build at a time
+  cudaSetDevice(device_);
+  std::shared_ptr<Index> nidx;
+  int64_t tt = 0;
+  {
+    std::unique_lock<std::shared_mutex> lk(mu_);
+    Status st = make_field_index(vi, type, params, &nidx, &tt);
+    if (!st.ok()) return st;
+    // the new index's bytes for every row stored or accepted, beside the old index's until the swap frees them
+    const int64_t rows = vslot(vi)->store().size() + pending_n_;
+    if (mem::limited()) {
+      std::vector<mem::Charge> c;
+      memory_places(&c, 0);
+      nidx->charge_index_rows(rows, &c);
+      if (!mem::admit(c))
+        return Status::Make(kMemoryExceeded, field + ": a " + type + " index of " + std::to_string(rows) + " rows");
+    }
+    nidx->adopt_store(vslot(vi)->share_store());
+    FieldIndex& fx = fidx_[vi];
+    fx.building = nidx;
+    fx.building_type = type;
+    fx.building_params = params;
+    fx.updated.clear();
+    fx.deleted.clear();
+  }
+  field_build_stop_.store(false);
+  field_build_thread_ = std::thread(&Engine::field_build, this, vi, nidx, tt);
+  return Status::OK();
+}
+
+// Train the successor on the field's first stored rows (BuildIndex's rule), index every stored row while the field's
+// current index serves searches, then, with the indexing thread stopped and the table held exclusively, index the rows
+// added since, apply the updates and deletions made meanwhile and swap.
+void Engine::field_build(int vi, std::shared_ptr<Index> nidx, int64_t tt) {
+  cudaSetDevice(device_);
+  FieldIndex& fx = fidx_[vi];
+  const std::string name = vname(vi), type = fx.building_type;
+  auto give_up = [&](bool log) {  // mu_ held exclusively
+    if (log)
+      fprintf(stderr, "gamma: building the %s index of vector field %s failed, the field keeps its index: %s\n",
+              type.c_str(), name.c_str(), last_error());
+    fx.building.reset();
+    fx.updated.clear();
+    fx.deleted.clear();
+  };
+  auto del_bitmap = [&](std::vector<uint8_t>* bm) {  // mu_ held
+    if (delete_num_ > 0) bm->assign(del_bitmap_.begin(), del_bitmap_.begin() + (max_docid_ >> 3) + 1);
+  };
+  {
+    std::unique_lock<std::shared_mutex> lk(mu_);
+    if (flush_pending_locked()) return give_up(true);
+  }
+  // fewer rows than the training threshold: the successor replaces the index untrained, as CreateTable would leave it
+  const bool train_now = nidx->store().size() >= nidx->training_threshold();
+  bool failed = train_now && nidx->train() != 0;
+  // rows stored while a pass runs are indexed by the next one; the last few are indexed under the exclusive lock
+  for (int pass = 0; train_now && !failed && !field_build_stop_.load() && pass < 8; pass++) {
+    std::vector<uint8_t> bm;
+    int64_t stored;
+    {
+      std::shared_lock<std::shared_mutex> lk(mu_);
+      del_bitmap(&bm);
+      stored = nidx->store().size();
+    }
+    // only the rows the bitmap covers: the store grows while the pass runs
+    failed = nidx->add_pending(bm.empty() ? nullptr : bm.data(), stored) != 0;
+    if (nidx->store().size() - stored < 65536) break;
+  }
+  if (failed || field_build_stop_.load()) {
+    std::unique_lock<std::shared_mutex> lk(mu_);
+    return give_up(failed);
+  }
+  const bool was_running = pause_indexing();
+  std::shared_ptr<Index> old;
+  {
+    std::unique_lock<std::shared_mutex> lk(mu_);
+    std::vector<uint8_t> bm;
+    failed = flush_pending_locked() != 0;
+    if (train_now) {
+      del_bitmap(&bm);
+      failed = failed || nidx->add_pending(bm.empty() ? nullptr : bm.data()) != 0;
+      std::vector<unsigned char> row((size_t)nidx->store().row_bytes());
+      for (int64_t vid : fx.updated)  // the store holds the new row; the successor re-lists it
+        failed = failed || nidx->store().get_host(vid, row.data()) || nidx->update_vector(vid, row.data());
+      if (!failed && !fx.deleted.empty())
+        failed = nidx->delete_vectors(fx.deleted.data(), (int64_t)fx.deleted.size()) != 0;
+    }
+    if (failed) {
+      give_up(true);
+    } else {
+      old = vslot(vi);
+      swap_field_index(vi, nidx, type, fx.building_params, true, tt);
+      give_up(false);
+    }
+  }
+  old.reset();  // freed here unless a search still holds it
+  if (!failed) remove_index_files(name);  // the old type's file; Dump writes the new one
+  resume_indexing(was_running);
+}
+
+void Engine::remove_index_files(const std::string& field) const {  // <path>/retrieval_model_index/<field>.000/
+  if (path_.empty()) return;
+  const std::string dir = path_ + "/retrieval_model_index/" + field + ".000";
+  if (DIR* d = opendir(dir.c_str())) {
+    while (dirent* e = readdir(d))
+      if (strcmp(e->d_name, ".") && strcmp(e->d_name, "..")) unlink((dir + "/" + e->d_name).c_str());
+    closedir(d);
+  }
+  rmdir(dir.c_str());
+}
+
+// The field keeps its raw store; what serves it is an index that is never trained and that every search of the field
+// scans exactly (the brute-force path): FLAT under the old index's metric, or for packed binary rows a BINARYIVF index
+// with the old parameters, whose brute-force path is the Hamming scan.
+Status Engine::RemoveFieldIndex(const std::string& field) {
+  const int vi = vec_field(field);
+  if (vi < 0) return Status::Make(kInvalidArgument, "field " + field + " not found");
+  std::lock_guard<std::mutex> g(field_build_mu_);  // no build starts while the index is removed
+  join_field_build_locked();
+  if (!fidx_[vi].has_index) return Status::OK();
+  cudaSetDevice(device_);
+  const bool was_running = pause_indexing();
+  std::shared_ptr<Index> old;
+  Status st;
+  {
+    std::unique_lock<std::shared_mutex> lk(mu_);
+    std::shared_ptr<Index> cur = vslot(vi);
+    const bool binary = cur->type() == "BINARYIVF";
+    const std::string type = binary ? cur->type() : "FLAT";
+    const std::string params =
+        binary ? vparams(vi) : std::string("{\"metric_type\": \"") + (cur->metric() == kMetricL2 ? "L2" : "InnerProduct") + "\"}";
+    ModelParams mp;
+    std::string err;
+    if (flush_pending_locked()) {
+      st = Status::Make(kIndexError, last_error());
+    } else if (!parse_model_params(params, type, &mp, &err)) {
+      st = Status::Make(kInvalidArgument, err);
+    } else {
+      mp.host_store = cur->store().on_host();
+      std::shared_ptr<Index> none(create_index(type, vdim(vi), mp, device_, 20));
+      if (!none) {
+        st = Status::Make(kInvalidArgument, last_error());
+      } else {
+        none->adopt_store(cur->share_store());
+        old = cur;
+        swap_field_index(vi, none, type, params, false, training_threshold_);
+      }
+    }
+  }
+  old.reset();
+  if (st.ok()) remove_index_files(field);
+  resume_indexing(was_running);
+  return st;
+}
+
 int64_t Engine::now_ms() {
   return std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
@@ -1201,6 +1478,7 @@ int Engine::BuildIndex() {
   if (!created_table_) return -1;
   int expected = 0;
   if (!indexing_state_.compare_exchange_strong(expected, 1)) return 0;  // already in progress
+  std::lock_guard<std::mutex> g(indexing_thread_mu_);
   if (indexing_thread_.joinable()) indexing_thread_.join();
   indexing_thread_ = std::thread(&Engine::indexing_loop, this);
   return 0;
@@ -1215,8 +1493,10 @@ int Engine::RebuildIndex(int drop_before_rebuild, int limit_cpu, int describe) {
   (void)drop_before_rebuild;
   (void)limit_cpu;
   if (!created_table_) return -1;
+  std::lock_guard<std::mutex> g(field_build_mu_);  // a run-time index build ends in its swap or its failure first
+  join_field_build_locked();
   if (indexing_state_.load() != 2 || index_status_.load() == 0) return 0;  // "index not running, no need to rebuild!"
-  quiesce();
+  stop_indexing();
   indexing_state_.store(0);
   if (describe) return 0;
   cudaSetDevice(device_);
@@ -1224,9 +1504,8 @@ int Engine::RebuildIndex(int drop_before_rebuild, int limit_cpu, int describe) {
     std::unique_lock<std::shared_mutex> lk(mu_);
     if (flush_pending_locked()) return -1;
   }
-  if (index_->reset_index()) return -1;
-  for (auto& e : extra_)
-    if (e.index->reset_index()) return -1;
+  for (size_t vi = 0; vi < fidx_.size(); vi++)
+    if (fidx_[vi].has_index && vslot((int)vi)->reset_index()) return -1;
   index_status_.store(0);
   if (refresh_interval_ >= 0 && max_docid_ - delete_num_ >= training_threshold_) return BuildIndex();
   return 0;
@@ -1243,8 +1522,9 @@ void Engine::indexing_loop() {
     std::unique_lock<std::shared_mutex> lk(mu_);
     flush_pending_locked();
   }
-  bool train_failed = index_->train() != 0;  // e.g. fewer vectors than training_threshold
-  for (auto& e : extra_) train_failed = train_failed || e.index->train() != 0;
+  bool train_failed = false;  // e.g. fewer vectors than training_threshold; a field without an index is not trained
+  for (size_t vi = 0; vi < fidx_.size(); vi++)
+    train_failed = train_failed || (fidx_[vi].has_index && vslot((int)vi)->train() != 0);
   if (train_failed) {
     // e.g. fewer vectors than training_threshold: remember when, so AddOrUpdate does not spawn and join a new
     // indexing thread for every document until the threshold is reached (BuildIndex retries after a back-off)
@@ -1265,11 +1545,14 @@ void Engine::indexing_loop() {
       if (flush_pending_locked()) has_error = true;
       if (delete_num_ > 0) bm.assign(del_bitmap_.begin(), del_bitmap_.begin() + (max_docid_ >> 3) + 1);
     }
-    if (!has_error && index_->add_pending(bm.empty() ? nullptr : bm.data()) != 0) has_error = true;
-    for (auto& e : extra_)
-      if (!has_error && e.index->add_pending(bm.empty() ? nullptr : bm.data()) != 0) has_error = true;
+    for (size_t vi = 0; vi < fidx_.size(); vi++)
+      if (!has_error && fidx_[vi].has_index && vslot((int)vi)->add_pending(bm.empty() ? nullptr : bm.data()) != 0)
+        has_error = true;
     if (!has_error) purge_indexes(bm.empty() ? nullptr : bm.data(), bm.size());
-    if (!has_error) index_status_.store(2);
+    if (!has_error) {
+      index_status_.store(2);
+      awaiting_training_.store(false);
+    }
     // sleep refresh_interval ms, waking early on Close
     std::unique_lock<std::mutex> lk(idx_mu_);
     idx_cv_.wait_for(lk, std::chrono::milliseconds(refresh_interval_ > 0 ? refresh_interval_ : 1),
@@ -1281,8 +1564,14 @@ void Engine::indexing_loop() {
 
 std::string Engine::EngineStatus() {  // search/engine.cc:1164-1176
   std::shared_lock<std::shared_mutex> lk(mu_);
-  int64_t min_indexed = created_table_ && index_ ? index_->indexed_count() : 0;
-  for (auto& e : extra_) min_indexed = std::min(min_indexed, e.index->indexed_count());  // min over the vector fields
+  // min over the vector fields that have an index; with none, the rows every field stores
+  int64_t min_indexed = -1;
+  for (size_t vi = 0; vi < fidx_.size(); vi++)
+    if (fidx_[vi].has_index) {
+      const int64_t c = vslot((int)vi)->indexed_count();
+      min_indexed = min_indexed < 0 ? c : std::min(min_indexed, c);
+    }
+  if (min_indexed < 0) min_indexed = created_table_ && index_ ? index_->store().size() : 0;
   char buf[256];
   snprintf(buf, sizeof buf,
            "{\"backup_status\":0,\"doc_num\":%d,\"index_status\":%d,\"max_docid\":%d,\"min_indexed_num\":%lld}",
@@ -1300,6 +1589,8 @@ std::string Engine::MemoryInfo() {  // search/engine.cc:1178-1200
   long long vec_mem = index_ ? index_->store().mem_bytes() + index_->store().host_bytes() : 0;
   for (auto& e : extra_)
     index_mem += e.index->index_mem_bytes(), vec_mem += e.index->store().mem_bytes() + e.index->store().host_bytes();
+  for (auto& fx : fidx_)  // a successor being built shares the store: only its index counts
+    if (fx.building) index_mem += fx.building->index_mem_bytes();
   long long field_range_mem = 0;  // the scalar indexes: device columns, string-array pools, dictionaries
   for (auto& c : sidx_) field_range_mem += c.mem_bytes();
   char buf[256];
@@ -1348,11 +1639,75 @@ bool rd_str(std::ifstream& f, std::string* s) {
   s->resize(n);
   return n == 0 || (bool)f.read(&(*s)[0], (std::streamsize)n);
 }
+// The snapshot's optional last part: the vector fields whose index AddFieldIndex / RemoveFieldIndex changed, each as
+// (name, has index, type, params), then the part's byte length and kIndexRecordMagic.  A snapshot without it ends with
+// the trained state, as snapshots written before the record existed do.
+const char kIndexRecordMagic[8] = {'G', 'B', 'F', 'I', 'D', 'X', '0', '1'};
 }  // namespace
+
+std::string encode_index_records(const std::vector<IndexRecord>& recs) {
+  std::string out;
+  auto put = [&](const void* p, size_t n) { out.append(static_cast<const char*>(p), n); };
+  auto put_str = [&](const std::string& v) {
+    const uint64_t n = v.size();
+    put(&n, 8);
+    put(v.data(), v.size());
+  };
+  const uint32_t n = (uint32_t)recs.size();
+  put(&n, 4);
+  for (const IndexRecord& r : recs) {
+    put_str(r.field);
+    const int32_t has = r.has_index ? 1 : 0;
+    put(&has, 4);
+    put_str(r.type);
+    put_str(r.params);
+  }
+  const uint64_t len = out.size();
+  put(&len, 8);
+  put(kIndexRecordMagic, 8);
+  return out;
+}
+
+int decode_index_records(const std::string& tail, std::vector<IndexRecord>* recs, size_t* bytes) {
+  recs->clear();
+  *bytes = 0;
+  if (tail.size() < 16 || memcmp(tail.data() + tail.size() - 8, kIndexRecordMagic, 8)) return 0;
+  uint64_t len;
+  memcpy(&len, tail.data() + tail.size() - 16, 8);
+  if (len > tail.size() - 16) return -1;
+  const char* p = tail.data() + tail.size() - 16 - len;
+  const char* end = p + len;
+  auto get = [&](void* v, size_t n) {
+    if ((size_t)(end - p) < n) return false;
+    memcpy(v, p, n);
+    p += n;
+    return true;
+  };
+  auto get_str = [&](std::string* v) {
+    uint64_t n;
+    if (!get(&n, 8) || n > (uint64_t)(end - p)) return false;
+    v->assign(p, (size_t)n);
+    p += n;
+    return true;
+  };
+  uint32_t n;
+  if (!get(&n, 4)) return -1;
+  for (uint32_t i = 0; i < n; i++) {
+    IndexRecord r;
+    int32_t has;
+    if (!get_str(&r.field) || !get(&has, 4) || !get_str(&r.type) || !get_str(&r.params)) return -1;
+    r.has_index = has != 0;
+    recs->push_back(std::move(r));
+  }
+  if (p != end) return -1;
+  *bytes = (size_t)len + 16;
+  return 0;
+}
 
 // Engine::Dump (search/engine.cc:1202-1247): <path>/retrieval_model_index/<name>.gbdump + dump.done
 int Engine::Dump() {
   if (!created_table_) return -1;
+  join_field_build();  // a run-time index build ends in its swap or its failure first
   cudaSetDevice(device_);
   std::unique_lock<std::shared_mutex> lk(mu_);
   if (flush_pending_locked()) return -1;
@@ -1388,6 +1743,13 @@ int Engine::Dump() {
       if (pq->get_pq_centroids(p.data())) return -1;
       f.write(reinterpret_cast<const char*>(p.data()), (std::streamsize)(p.size() * 4));
     }
+  }
+  std::vector<IndexRecord> recs;
+  for (size_t vi = 0; vi < fidx_.size(); vi++)
+    if (fidx_[vi].changed) recs.push_back({vname((int)vi), fidx_[vi].has_index, vtype((int)vi), vparams((int)vi)});
+  if (!recs.empty()) {
+    const std::string rec = encode_index_records(recs);
+    f.write(rec.data(), (std::streamsize)rec.size());
   }
   f.close();
   // the index itself in gamma's own format (IndexModel::Dump via VectorManager::Dump,
@@ -1428,6 +1790,41 @@ int Engine::Load() {
     return -1;
   std::unique_lock<std::shared_mutex> lk(mu_);
   if (max_docid_ != 0) return -1;
+  {  // the indexes AddFieldIndex / RemoveFieldIndex left, re-created before their rows and trained state are read
+    const std::streampos at = f.tellg();
+    f.seekg(0, std::ios::end);
+    const int64_t size = (int64_t)f.tellg();
+    std::string tail((size_t)std::min<int64_t>(size, 1 << 20), '\0');
+    f.seekg(size - (int64_t)tail.size());
+    std::vector<IndexRecord> recs;
+    size_t rec_bytes = 0;
+    if (!f.read(&tail[0], (std::streamsize)tail.size()) || decode_index_records(tail, &recs, &rec_bytes)) return -1;
+    for (const IndexRecord& r : recs) {
+      const int vi = vec_field(r.field);
+      if (vi < 0) return -1;
+      std::shared_ptr<Index> idx;
+      int64_t tt = training_threshold_;
+      if (r.has_index) {
+        Status st = make_field_index(vi, r.type, r.params, &idx, &tt);
+        if (!st.ok()) {
+          fprintf(stderr, "gamma: the recorded index of vector field %s is refused: %s\n", r.field.c_str(), st.msg.c_str());
+          return -1;
+        }
+      } else {
+        ModelParams mp;
+        std::string err;
+        if (!parse_model_params(r.params, r.type, &mp, &err)) return -1;
+        mp.host_store = vslot(vi)->store().on_host();
+        idx.reset(create_index(r.type, vdim(vi), mp, device_, 20));
+        if (!idx) return -1;
+      }
+      swap_field_index(vi, idx, r.type, r.params, r.has_index, tt);
+    }
+    index_status_.store(0);  // set by the indexing thread once the rows are indexed, as for a table never changed
+    awaiting_training_.store(false);
+    f.clear();
+    f.seekg(at);
+  }
   for (size_t fi = 0; fi < fields_.size(); fi++) {
     values_[fi].resize(maxd);
     for (int d = 0; d < maxd; d++)
@@ -1493,8 +1890,10 @@ int Engine::Load() {
     else if (load_num > 0)
       index_status_.store(2);
   }
+  bool changed = false;
+  for (auto& fx : fidx_) changed = changed || fx.changed;
   lk.unlock();
-  if (trained) BuildIndex();  // train() is a no-op on a trained index; the loop adds what the file did not cover
+  if (trained || changed) BuildIndex();  // train() is a no-op on a trained index; the loop adds what the file did not cover
   return 0;
 }
 

@@ -108,6 +108,17 @@ struct QueryRequestPB {  // vearchpb.QueryRequest (router_grpc.proto:147-166), c
   bool parse(const uint8_t* data, size_t len);
 };
 
+// One vector field's index as AddFieldIndex / RemoveFieldIndex left it, as Dump records it at the end of the snapshot
+struct IndexRecord {
+  std::string field;
+  bool has_index = true;
+  std::string type, params;
+};
+std::string encode_index_records(const std::vector<IndexRecord>& recs);
+// the records at the end of a snapshot's last bytes `tail` (none when it does not end with them), and in *bytes their
+// length; -1: a record that does not parse
+int decode_index_records(const std::string& tail, std::vector<IndexRecord>* recs, size_t* bytes);
+
 class Engine {
  public:
   // devices: Init's "devices" (empty: one device); a GPU_IVFPQ / GPU_IVFFLAT field is sharded over two or more, every
@@ -132,9 +143,16 @@ class Engine {
   int Load();
   const std::string& space_name() const { return space_name_; }
   void quiesce();  // stop the indexing thread (also from an atexit hook for engines never Closed)
-  // Engine::AddFieldIndex / RemoveFieldIndex (search/engine.cc:1471-1600): build the field's device columns over the
-  // documents already stored, or free them
-  Status SetFieldIndexed(const std::string& field, bool indexed);
+  // Engine::AddFieldIndex / RemoveFieldIndex (search/engine.cc:1471-1600): for a scalar field, build the field's device
+  // columns over the documents already stored, or free them; for a vector field, AddFieldIndex / RemoveFieldIndex below
+  Status SetFieldIndexed(const std::string& field, bool indexed, const std::string& index_type = "",
+                         const std::string& index_params = "");
+  // A vector field's index at run time (vector_manager.cc:217-317).  AddFieldIndex validates `type` and `params` as
+  // CreateTable does, creates the index over the field's raw store and returns; a build thread trains and fills it from
+  // the stored rows while searches keep using the field's current index, then swaps it in.  RemoveFieldIndex drops the
+  // field's index and its files; the field is then searched exactly, as brute-force searches are.
+  Status AddFieldIndex(const std::string& field, const std::string& type, const std::string& params);
+  Status RemoveFieldIndex(const std::string& field);
   // whether a Search / Query request of `bytes` fits the memory limit (mem_ledger.h) on every place the table uses
   bool request_admitted(int64_t bytes) const;
 
@@ -202,7 +220,9 @@ class Engine {
   // vector field
   std::string vec_name_, index_type_, index_params_;
   int dim_ = 0;
-  std::unique_ptr<Index> index_;
+  // Searches take the index they search by atomic load (index_ref) and hold it until their results are read, so a swap
+  // under the exclusive lock never frees an index a search is in; every other use holds mu_
+  std::shared_ptr<Index> index_;
   // rows accepted by AddOrUpdate, not yet uploaded to HBM: vbytes_ bytes each (d fp32 values, or BINARYIVF's d / 8 bytes)
   std::vector<unsigned char> pending_;
   size_t vbytes_ = 0;
@@ -212,11 +232,55 @@ class Engine {
   struct VecField {
     std::string name, index_type, index_params;
     int dim = 0;
-    std::unique_ptr<Index> index;
+    std::shared_ptr<Index> index;
     std::vector<float> pending;
   };
   std::vector<VecField> extra_;
   Index* index_of(const std::string& vec_name, int* dim);  // nullptr: no such vector field
+  std::shared_ptr<Index> index_ref(const std::string& vec_name, int* dim);  // index_of for a search, without mu_
+
+  // Run-time index changes (AddFieldIndex / RemoveFieldIndex) of vector field vi: 0 the first, 1 + i extra_[i]
+  struct FieldIndex {
+    bool has_index = true;  // false after RemoveFieldIndex: a FLAT index over the raw store serves the field
+    bool changed = false;   // type or params differ from CreateTable's: the snapshot records them
+    std::shared_ptr<Index> building;  // the successor being trained and filled, sharing the field's raw store
+    std::string building_type, building_params;
+    std::vector<int64_t> updated, deleted;  // docids updated or deleted during the build, applied to it before the swap
+  };
+  std::vector<FieldIndex> fidx_;
+  int vec_field(const std::string& name) const;  // vi, -1: not a vector field
+  std::shared_ptr<Index>& vslot(int vi) { return vi == 0 ? index_ : extra_[vi - 1].index; }
+  std::string& vtype(int vi) { return vi == 0 ? index_type_ : extra_[vi - 1].index_type; }
+  std::string& vparams(int vi) { return vi == 0 ? index_params_ : extra_[vi - 1].index_params; }
+  const std::string& vname(int vi) const { return vi == 0 ? vec_name_ : extra_[vi - 1].name; }
+  int vdim(int vi) const { return vi == 0 ? dim_ : extra_[vi - 1].dim; }
+  // CreateTable's rules for the index of one vector field: parse, training threshold, store placement, BINARYIVF only
+  // alone, creation.  first: the table's first vector field, whose threshold follows its type when the table gave none
+  // (*tt in: the threshold so far, out: the one the field keeps); every other field takes *tt as it is
+  Status create_field_index(const std::string& name, int dim, const std::string& type, const std::string& params,
+                            bool first, bool host, size_t nvec, int64_t* tt, Index** out) const;
+  // an index of `type` / `params` for vector field vi, validated as CreateTable validates the field's; *tt: the
+  // training threshold the engine keeps for it
+  Status make_field_index(int vi, const std::string& type, const std::string& params, std::shared_ptr<Index>* out,
+                          int64_t* tt);
+  // put `nidx` in vector field vi's slot (mu_ held exclusively); the old index is freed once no search holds it
+  void swap_field_index(int vi, std::shared_ptr<Index> nidx, const std::string& type, const std::string& params,
+                        bool has_index, int64_t tt);
+  void field_build(int vi, std::shared_ptr<Index> nidx, int64_t tt);  // the build thread's work
+  void join_field_build();
+  void join_field_build_locked();  // field_build_mu_ held
+  void remove_index_files(const std::string& field) const;
+  // stop the indexing thread and keep it from being started until resume_indexing
+  bool pause_indexing();
+  void resume_indexing(bool was_running);
+  void stop_indexing();
+  // guards field_build_thread_; AddFieldIndex, RemoveFieldIndex and RebuildIndex hold it throughout
+  std::mutex field_build_mu_;
+  std::thread field_build_thread_;
+  // a field's index was swapped in untrained (below its training threshold): searches are exact until it trains
+  std::atomic<bool> awaiting_training_{false};
+  std::atomic<bool> field_build_stop_{false};
+  int64_t table_training_threshold_ = 0;  // the table's own training_threshold, 0 if it has none
 
   std::vector<uint8_t> del_bitmap_;
   // RealTimeMemData::CompactIfNeed for every vector field's index: lists that are 30 % dead are rewritten without the
@@ -224,6 +288,7 @@ class Engine {
   void purge_indexes(const uint8_t* bitmap, size_t bytes);
   int max_docid_ = 0, delete_num_ = 0;
   int64_t training_threshold_ = 0;  // the index's clamp can pass 2^31 rows (256 * nlist)
+  bool table_params_given_ = false;  // the table carried index params (table.cc:143-150)
   int refresh_interval_ = 1000;
   bool enable_id_cache_ = false, enable_realtime_ = false;
   int slow_search_time_ = 0;
@@ -232,7 +297,8 @@ class Engine {
   static constexpr int64_t kTrainRetryMs = 1000;
   std::atomic<int64_t> last_train_failure_ms_{-(int64_t)1 << 40};
   std::atomic<int> index_status_{0};    // IndexStatus: 0 UNINDEXED, 1 INDEXING, 2 INDEXED
-  std::atomic<int> indexing_state_{0};  // IndexingState: 0 IDLE, 1 STARTING, 2 RUNNING, 3 STOPPING
+  std::atomic<int> indexing_state_{0};  // IndexingState: 0 IDLE, 1 STARTING, 2 RUNNING, 3 STOPPING, 4 PAUSED
+  std::mutex indexing_thread_mu_;  // guards indexing_thread_ (started by BuildIndex, joined by whoever stops it)
   std::thread indexing_thread_;
   std::mutex idx_mu_;
   std::condition_variable idx_cv_;

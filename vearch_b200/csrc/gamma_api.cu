@@ -220,14 +220,20 @@ struct CStatus Backup(void*, int) {
   return c;
 }
 
-struct CStatus AddFieldIndexWithParams(void* engine, const char* field_name, int field_name_len, const char*, int,
-                                       const char*, int) {
+// a vector field's index type and params (gammacb/gamma.go:538-572); a scalar field ignores them
+struct CStatus AddFieldIndexWithParams(void* engine, const char* field_name, int field_name_len, const char* index_type,
+                                       int index_type_len, const char* index_params, int index_params_len) {
   struct CStatus c;
   if (!engine || !field_name) {
     to_cstatus(gb::Status::Make(gb::kInvalidArgument, "null engine"), &c);
     return c;
   }
-  to_cstatus(static_cast<Engine*>(engine)->SetFieldIndexed(std::string(field_name, (size_t)field_name_len), true), &c);
+  const std::string type = index_type && index_type_len > 0 ? std::string(index_type, (size_t)index_type_len) : "";
+  const std::string params =
+      index_params && index_params_len > 0 ? std::string(index_params, (size_t)index_params_len) : "";
+  to_cstatus(static_cast<Engine*>(engine)->SetFieldIndexed(std::string(field_name, (size_t)field_name_len), true, type,
+                                                           params),
+             &c);
   return c;
 }
 
@@ -291,6 +297,20 @@ int gb_memory_ledger(int device, int64_t* usage, int64_t* pool_reserved, int64_t
 }
 
 void gb_memory_set_total(int device, int64_t bytes) { gb::mem::set_total(device, bytes); }
+
+// the run-time index records at the end of a snapshot's last `len` bytes, as Load reads them:
+// {"bytes": <record part>, "records": [[field, has_index, type, params], ...]}; -1 if a record does not parse
+int gb_debug_index_records(const char* tail, int64_t len, char** json_out, int* out_len) {
+  std::vector<gb::IndexRecord> recs;
+  size_t bytes = 0;
+  if (gb::decode_index_records(std::string(tail, (size_t)len), &recs, &bytes)) return -1;
+  std::string j = "{\"bytes\":" + std::to_string(bytes) + ",\"records\":[";
+  for (size_t i = 0; i < recs.size(); i++)
+    j += std::string(i ? "," : "") + "[\"" + hex_escape(recs[i].field) + "\"," + (recs[i].has_index ? "true" : "false") +
+         ",\"" + hex_escape(recs[i].type) + "\",\"" + hex_escape(recs[i].params) + "\"]";
+  out_buffer(j + "]}", json_out, out_len);
+  return 0;
+}
 
 int gb_debug_parse_search_request(const char* buf, int len, char** json_out, int* out_len) {
   gb::SearchRequestPB r;

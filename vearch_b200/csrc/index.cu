@@ -352,7 +352,7 @@ int RawStore::append_host(const void* xv, int64_t n, cudaStream_t st) {
   }
   GB_CUDA(cudaStreamSynchronize(st));
   n_ += n;
-  if (shadow_) shadow_->n_ = n_;
+  if (shadow_) shadow_->n_ = n_.load();
   return 0;
 }
 int RawStore::append_device(const void* xv, int64_t ld_bytes, int64_t n, cudaStream_t st) {
@@ -370,7 +370,7 @@ int RawStore::append_device(const void* xv, int64_t ld_bytes, int64_t n, cudaStr
   }
   GB_CUDA(cudaStreamSynchronize(st));
   n_ += n;
-  if (shadow_) shadow_->n_ = n_;
+  if (shadow_) shadow_->n_ = n_.load();
   return 0;
 }
 int RawStore::update_host(int64_t vid, const void* x, cudaStream_t st) {
@@ -913,6 +913,11 @@ float Index::last_scan_ms() {
   }
   scan_events_.clear();
   return total;
+}
+std::shared_ptr<RawStore> Index::share_store() {
+  std::unique_lock<std::shared_mutex> lk(mu_);  // appends take mu_ too: the table is not growing while it moves
+  store_->reserve_segments();
+  return store_;
 }
 int Index::add_vectors(const void* x, int64_t n) {
   cudaSetDevice(device_);
@@ -1730,7 +1735,7 @@ int IvfIndex::index_batch(const void* x, int64_t n, int64_t vid0, const uint8_t*
   return 0;
 }
 
-int IvfIndex::add_pending(const uint8_t* del_bitmap) {
+int IvfIndex::add_pending(const uint8_t* del_bitmap, int64_t rows) {
   std::lock_guard<std::mutex> bg(build_mu_);
   if (!trained_) return 0;
   cudaSetDevice(device_);
@@ -1741,12 +1746,13 @@ int IvfIndex::add_pending(const uint8_t* del_bitmap) {
     Scratch s(build_stream_);
     {  // add_vectors (exclusive mu_) may append segments while we look: the segment table is read under the shared lock
       std::shared_lock<std::shared_mutex> lk(mu_);
-      if (vid0 >= store_->size()) break;
+      const int64_t end = rows < 0 ? store_->size() : std::min(rows, store_->size());
+      if (vid0 >= end) break;
       // HBM rows are indexed in place, so a batch ends at its segment's end.  Host rows are copied to HBM first, across
       // segments: their batches end at the same BATCH-aligned rows, so both placements build the same list layout.
       const int64_t span = store_->on_host() ? BATCH : store_->seg_rows();
       int64_t off = vid0 & (span - 1);
-      n = std::min<int64_t>(std::min(store_->size() - vid0, span - off), BATCH);
+      n = std::min<int64_t>(std::min(end - vid0, span - off), BATCH);
       x = store_rows_dev(vid0, n, s);
       if (!x) return -1;
     }

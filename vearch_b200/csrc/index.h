@@ -95,6 +95,9 @@ class RawStore {
   // physical HBM behind the store, its int8 shadow included (0 for host placement)
   int64_t mem_bytes() const { return phys_bytes_ + (shadow_ ? shadow_->phys_bytes_ : 0); }
   int64_t host_bytes() const { return host_bytes_; }  // pinned host memory behind the store
+  // Before a second index shares the store (Index::share_store): the segment table gets its full capacity, so appends
+  // through one index never move it while the other reads it
+  void reserve_segments() { segs_.reserve(kMaxSegs); }
   // The int8 shadow of fp32 rows that the two-pass exact re-rank screens candidates with (launch_rerank_prefilter):
   // row vid at shadow_segs()[vid >> seg_shift()] + (vid & (seg_rows() - 1)) * shadow_stride().  Written with the fp32
   // rows in the same stream-ordered step, so whatever sees a row sees its shadow.  Only an HBM store of fp32 rows gets
@@ -120,7 +123,8 @@ class RawStore {
   int64_t stride_;
   int seg_shift_, device_ = 0;
   bool host_;
-  int64_t n_ = 0, phys_bytes_ = 0, host_bytes_ = 0;
+  std::atomic<int64_t> n_{0};  // read by an index that shares the store while another appends
+  int64_t phys_bytes_ = 0, host_bytes_ = 0;
   std::vector<Seg> segs_;
   unsigned char** d_segs_ = nullptr;  // device array [kMaxSegs]
   static constexpr int kMaxSegs = 65536;
@@ -278,6 +282,12 @@ class Index {
   int metric() const { return mp_.metric; }
   const ModelParams& model_params() const { return mp_; }
   RawStore& store() { return *store_; }
+  // The field's raw store for a successor index (Engine::AddFieldIndex): both indexes hold it while the successor is
+  // built.  The rows are appended through one index only; the other reads them.
+  std::shared_ptr<RawStore> share_store();
+  // take `s` in place of the empty store this index was created with, before any row reaches it; the per-index data
+  // derived from the rows (lists, mirrors, row-pointer tables) is built by train / add_pending as for rows of its own
+  void adopt_store(std::shared_ptr<RawStore> s) { store_ = std::move(s); }
   int64_t indexed_count() const { return indexed_count_; }
   bool trained() const { return trained_; }
   virtual int64_t training_threshold() const { return 0; }
@@ -291,8 +301,12 @@ class Index {
   int add_vectors_device(const float* x, int64_t ld, int64_t n);
   // IndexModel::Indexing(): train on the first `num` stored vectors
   virtual int train() { trained_ = true; return 0; }
-  // VectorManager::AddRTVecsToIndex (vector_manager.cc:572-702): index all not-yet-indexed rows
-  virtual int add_pending(const uint8_t* del_bitmap) { indexed_count_ = store_->size(); return 0; }
+  // VectorManager::AddRTVecsToIndex (vector_manager.cc:572-702): index all not-yet-indexed rows, or those below `rows`
+  // when it is >= 0 (del_bitmap then need only cover them)
+  virtual int add_pending(const uint8_t* del_bitmap, int64_t rows = -1) {
+    indexed_count_ = rows < 0 ? store_->size() : std::max(indexed_count_, std::min(rows, store_->size()));
+    return 0;
+  }
   // Engine::Update -> RawVector update + IndexModel::Update (search/engine.cc:774-850;
   // realtime_mem_data.cc:298-320: old entry tombstoned, vector re-appended to its new list)
   virtual int update_vector(int64_t vid, const void* x);  // x: one row of store().row_bytes() bytes
@@ -398,7 +412,7 @@ class Index {
   bool gpu_contract_;
   int d_, dpad_, device_;
   ModelParams mp_;
-  std::unique_ptr<RawStore> store_;
+  std::shared_ptr<RawStore> store_;
   int64_t indexed_count_ = 0;
   bool trained_ = false;
   mutable std::shared_mutex mu_;  // searches shared, index mutation exclusive
@@ -532,7 +546,7 @@ class IvfIndex : public Index {
   ~IvfIndex() override;
   int64_t training_threshold() const override;
   int train() override;
-  int add_pending(const uint8_t* del_bitmap) override;
+  int add_pending(const uint8_t* del_bitmap, int64_t rows = -1) override;
   int update_vector(int64_t vid, const void* x) override;
   int delete_vectors(const int64_t* vids, int64_t n) override;  // a vid not in a list, or already counted, is ignored
   int purge_lists(float threshold, const uint8_t* del_bitmap, int64_t bitmap_bytes, int64_t* dropped) override;
@@ -1011,7 +1025,7 @@ class ShardedIndex : public Index {
   IvfIndex* shard(int s) { return shards_[s].get(); }
   int64_t training_threshold() const override { return shards_[0]->training_threshold(); }
   int train() override;
-  int add_pending(const uint8_t* del_bitmap) override;
+  int add_pending(const uint8_t* del_bitmap, int64_t rows = -1) override;
   int update_vector(int64_t vid, const void* x) override;
   int delete_vectors(const int64_t* vids, int64_t n) override;
   int purge_lists(float threshold, const uint8_t* del_bitmap, int64_t bitmap_bytes, int64_t* dropped) override;

@@ -225,7 +225,7 @@ int ShardedIndex::train() {
   return 0;
 }
 
-int ShardedIndex::add_pending(const uint8_t* del_bitmap) {
+int ShardedIndex::add_pending(const uint8_t* del_bitmap, int64_t rows) {
   std::lock_guard<std::mutex> bg(build_mu_);
   if (!trained_) return 0;
   const int S = nshards();
@@ -237,10 +237,11 @@ int ShardedIndex::add_pending(const uint8_t* del_bitmap) {
     Scratch s(build_stream_);
     {  // the batches of IvfIndex::add_pending
       std::shared_lock<std::shared_mutex> lk(mu_);
-      if (vid0 >= store_->size()) break;
+      const int64_t end = rows < 0 ? store_->size() : std::min(rows, store_->size());
+      if (vid0 >= end) break;
       const int64_t span = store_->on_host() ? BATCH : store_->seg_rows();
       int64_t off = vid0 & (span - 1);
-      n = std::min<int64_t>(std::min(store_->size() - vid0, span - off), BATCH);
+      n = std::min<int64_t>(std::min(end - vid0, span - off), BATCH);
       x = static_cast<const unsigned char*>(store_rows_dev(vid0, n, s));
       if (!x) return -1;
     }

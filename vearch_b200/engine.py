@@ -210,11 +210,17 @@ class GammaEngine:
     def rebuild_index(self, drop_before_rebuild=1, limit_cpu=0, describe=0):
         return _api().RebuildIndex(self._h, drop_before_rebuild, limit_cpu, describe)
 
-    def add_field_index(self, field):
-        f = field.encode()
-        _status(_api().AddFieldIndexWithParams(self._h, f, len(f), b"", 0, b"", 0))
+    def add_field_index(self, field, index_type="", index_params=None):
+        """AddFieldIndexWithParams.  A scalar field becomes filterable (type and params are ignored); a vector field gets
+        an index of `index_type` with `index_params` (a dict), built in the background while its current index keeps
+        serving, which replaces it once every stored row is indexed."""
+        f, t = field.encode(), index_type.encode()
+        p = json.dumps(index_params).encode() if index_params is not None else b""
+        _status(_api().AddFieldIndexWithParams(self._h, f, len(f), t, len(t), p, len(p)))
 
     def remove_field_index(self, field):
+        """RemoveFieldIndex: a scalar field is no longer filterable; a vector field drops its index and is then searched
+        exactly (the brute-force path)."""
         f = field.encode()
         _status(_api().RemoveFieldIndex(self._h, f, len(f)))
 
