@@ -17,10 +17,11 @@
  *
  * Scope of this build (DESIGN.md, INTEGRATION.md): full semantics for Init / Close / CreateTable /
  * AddOrUpdateDoc / DeleteDoc / GetDocByID / GetDocByDocID / BuildIndex / Search / Query /
- * GetEngineStatus / GetMemoryInfo / SetConfig / GetConfig / Dump / Load / SetKillStatus /
+ * GetEngineStatus / GetMemoryInfo / SetConfig / GetConfig / Dump / Load / Backup / SetKillStatus /
  * DeleteKillStatus / AddFieldIndexWithParams / RemoveFieldIndex / RebuildIndex / SetMemoryLimitConfig for
- * tables whose vector fields are indexed as FLAT, IVFFLAT or IVFPQ (optionally with OPQ); Backup returns
- * kNotSupported.  SetMemoryLimitConfig(p) limits what this library holds to p % of each device's HBM and of host
+ * tables whose vector fields are indexed as FLAT, IVFFLAT or IVFPQ (optionally with OPQ).  Backup(engine, 0) writes
+ * what Dump writes into <path>/backup/retrieval_model_index, captured on the device under the table lock and written
+ * after it is released; Backup(engine, 1) does nothing.  SetMemoryLimitConfig(p) limits what this library holds to p % of each device's HBM and of host
  * memory (0: no limit): past it AddOrUpdateDoc refuses new documents with -5 and Search / Query return code 8.
  */
 #ifndef GAMMA_API_H_

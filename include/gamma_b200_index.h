@@ -265,7 +265,21 @@ int gb_memory_ledger(int device, int64_t *usage, int64_t *pool_reserved, int64_t
  * 0 restores the real one (cudaDeviceProp::totalGlobalMem; the host's MemTotal or cgroup v1 limit) */
 void gb_memory_set_total(int device, int64_t bytes);
 
+/* Backup (include/gamma_api.h, DESIGN.md section 8) test hooks.  hold: op 1 makes the next Backup wait after its capture
+ * and before it writes, op 0 lets it go on, op -1 only reads; returns 0 (off), 1 (set) or 2 (a Backup is waiting).  It
+ * never blocks a Backup unless set.  stage: the bytes the last finished capture (Dump or Backup) staged in HBM and in
+ * pinned host memory. */
+int gb_debug_backup_hold(int op);
+int gb_debug_backup_stage(int64_t *device_bytes, int64_t *host_bytes);
+/* A capture of an index's file as Dump and Backup take it (index lists packed on the device into a stage, in the
+ * file's order: per list its codes of code_size bytes on disk, then its ids as stored).  out (may be NULL) receives
+ * min(cap, *bytes) of the staged lists; *on_host = 1 when the device could not hold the stage.  An unsharded index
+ * only; an untrained one or FLAT stages nothing. */
+int gb_index_capture_lists(gb_index *index, uint8_t *out, int64_t cap, int64_t *bytes, int *on_host);
+
 /* ---- host-logic test hooks: run the C++ wire codecs of the gamma boundary without a GPU ---- */
+/* an engine over `path` (may be "") made without looking for a device, for the checks that need none; Close frees it */
+void *gb_debug_engine_create(const char *path);
 /* RequestConcurrentController (search/engine.cc:47-119): op 0 threshold, 1 in-flight, 2 set threshold (<= 0: system value),
  * 3 Acquire(value) -> 1/0, 4 Release(value) */
 int gb_debug_concurrency(int op, int value);

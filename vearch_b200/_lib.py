@@ -131,6 +131,11 @@ def _declare(l):
     l.gb_memory_set_total.restype = None
     l.gb_memory_set_total.argtypes = [i32, i64]
     l.gb_debug_index_records.argtypes = [C.c_char_p, i64, C.POINTER(C.c_void_p), C.POINTER(i32)]
+    l.gb_debug_backup_hold.argtypes = [i32]
+    l.gb_debug_backup_stage.argtypes = [C.POINTER(i64), C.POINTER(i64)]
+    l.gb_debug_engine_create.restype = vp
+    l.gb_debug_engine_create.argtypes = [cstr]
+    l.gb_index_capture_lists.argtypes = [vp, vp, i64, C.POINTER(i64), C.POINTER(i32)]
     l.gb_merge_partitions_device.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, vp]
 
 

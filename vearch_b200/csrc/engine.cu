@@ -5,11 +5,15 @@
 #include <stdio.h>
 #include <string.h>
 #include <dirent.h>
+#include <errno.h>
+#include <fcntl.h>
+#include <ftw.h>
 #include <sys/stat.h>
 #include <unistd.h>
 
 #include <algorithm>
 #include <chrono>
+#include <thread>
 #include <fstream>
 #include <map>
 
@@ -1574,8 +1578,8 @@ std::string Engine::EngineStatus() {  // search/engine.cc:1164-1176
   if (min_indexed < 0) min_indexed = created_table_ && index_ ? index_->store().size() : 0;
   char buf[256];
   snprintf(buf, sizeof buf,
-           "{\"backup_status\":0,\"doc_num\":%d,\"index_status\":%d,\"max_docid\":%d,\"min_indexed_num\":%lld}",
-           doc_num(), index_status_.load(), max_docid_ - 1, (long long)min_indexed);
+           "{\"backup_status\":%d,\"doc_num\":%d,\"index_status\":%d,\"max_docid\":%d,\"min_indexed_num\":%lld}",
+           backup_status_.load(), doc_num(), index_status_.load(), max_docid_ - 1, (long long)min_indexed);
   return buf;
 }
 
@@ -1620,15 +1624,6 @@ std::string Engine::GetConfig() {  // search/engine.cc:1792-1807
 
 // ---- Dump / Load (own snapshot format; byte-compatible gamma dumps are a "next" row) --------
 namespace {
-template <typename T>
-void wr(std::ofstream& f, const T& v) {
-  f.write(reinterpret_cast<const char*>(&v), sizeof(T));
-}
-void wr_str(std::ofstream& f, const std::string& s) {
-  uint64_t n = s.size();
-  wr(f, n);
-  f.write(s.data(), (std::streamsize)n);
-}
 template <typename T>
 bool rdv(std::ifstream& f, T* v) {
   return (bool)f.read(reinterpret_cast<char*>(v), sizeof(T));
@@ -1704,71 +1699,219 @@ int decode_index_records(const std::string& tail, std::vector<IndexRecord>* recs
   return 0;
 }
 
-// Engine::Dump (search/engine.cc:1202-1247): <path>/retrieval_model_index/<name>.gbdump + dump.done
-int Engine::Dump() {
-  if (!created_table_) return -1;
-  join_field_build();  // a run-time index build ends in its swap or its failure first
-  cudaSetDevice(device_);
-  std::unique_lock<std::shared_mutex> lk(mu_);
-  if (flush_pending_locked()) return -1;
-  std::string dir = path_ + "/retrieval_model_index";
-  mkdir(path_.c_str(), 0755);
-  mkdir(dir.c_str(), 0755);
-  std::ofstream f(dir + "/" + table_name_ + ".gbdump", std::ios::binary | std::ios::trunc);
-  if (!f) return -1;
-  const char magic[8] = {'G', 'B', '2', '0', '0', 'D', 'M', 'P'};
-  f.write(magic, 8);
-  wr<int32_t>(f, 1);
-  wr<int32_t>(f, max_docid_);
-  wr<int32_t>(f, delete_num_);
-  wr<int32_t>(f, dim_);
-  wr<uint64_t>(f, fields_.size());
+struct Engine::Image {
+  std::string table_name;
+  int32_t max_docid = 0;
+  std::string head, tail;  // the .gbdump before and after the first vector field's rows
+  struct Field {
+    std::string name;
+    int32_t dim = 0;
+    Stage rows;          // rows [0, max_docid), packed
+    GammaImage index;    // its index file (none when untrained or FLAT)
+  };
+  std::vector<Field> fields;  // the first vector field (its rows in the .gbdump), then extra_ (<table>.<field>.gbvec)
+};
+
+// mu_ held exclusively, pending rows flushed: every device copy has finished when it returns
+int Engine::capture_locked(Image* img) {
+  img->table_name = table_name_;
+  img->max_docid = max_docid_;
+  std::string& h = img->head;
+  auto put = [](std::string& o, const void* p, size_t n) { o.append(static_cast<const char*>(p), n); };
+  auto put_str = [&](std::string& o, const std::string& v) {
+    const uint64_t n = v.size();
+    put(o, &n, 8);
+    o += v;
+  };
+  size_t bytes = 36 + del_bitmap_.size() + 8;
   for (size_t fi = 0; fi < fields_.size(); fi++)
-    for (int d = 0; d < max_docid_; d++) wr_str(f, values_[fi][d]);
-  wr_str(f, std::string(del_bitmap_.begin(), del_bitmap_.end()));
-  std::vector<unsigned char> rows((size_t)max_docid_ * vbytes_);
-  if (max_docid_ && index_->store().get_rows_host(0, max_docid_, rows.data())) return -1;
-  f.write(reinterpret_cast<const char*>(rows.data()), (std::streamsize)rows.size());
-  int trained = index_->trained() ? 1 : 0;
-  wr<int32_t>(f, trained);
+    for (int d = 0; d < max_docid_; d++) bytes += 8 + values_[fi][d].size();
+  h.reserve(bytes);
+  const char magic[8] = {'G', 'B', '2', '0', '0', 'D', 'M', 'P'};
+  const int32_t hdr[4] = {1, max_docid_, delete_num_, dim_};
+  const uint64_t nf = fields_.size();
+  put(h, magic, 8);
+  put(h, hdr, sizeof hdr);
+  put(h, &nf, 8);
+  for (size_t fi = 0; fi < fields_.size(); fi++)
+    for (int d = 0; d < max_docid_; d++) put_str(h, values_[fi][d]);
+  put_str(h, std::string(del_bitmap_.begin(), del_bitmap_.end()));
+  const int32_t trained = index_->trained() ? 1 : 0;
+  put(img->tail, &trained, 4);
   // an index whose trained state does not persist (IVFPQFastScan) is trained again by Load
   IvfIndex* ivf = index_->persists_trained_state() ? trained_state_of(index_.get()) : nullptr;
   IVFPQIndex* pq = dynamic_cast<IVFPQIndex*>(ivf);
   if (trained && ivf) {
     std::vector<float> c((size_t)ivf->nlist() * dim_);
     if (ivf->get_centroids(c.data())) return -1;
-    f.write(reinterpret_cast<const char*>(c.data()), (std::streamsize)(c.size() * 4));
+    put(img->tail, c.data(), c.size() * 4);
     if (pq) {
       std::vector<float> p((size_t)pq->M() * pq->ksub() * pq->dsub());
       if (pq->get_pq_centroids(p.data())) return -1;
-      f.write(reinterpret_cast<const char*>(p.data()), (std::streamsize)(p.size() * 4));
+      put(img->tail, p.data(), p.size() * 4);
     }
   }
   std::vector<IndexRecord> recs;
   for (size_t vi = 0; vi < fidx_.size(); vi++)
     if (fidx_[vi].changed) recs.push_back({vname((int)vi), fidx_[vi].has_index, vtype((int)vi), vparams((int)vi)});
-  if (!recs.empty()) {
-    const std::string rec = encode_index_records(recs);
-    f.write(rec.data(), (std::streamsize)rec.size());
+  if (!recs.empty()) img->tail += encode_index_records(recs);
+  // the raw rows, device to device (or host to host), and every index's trained state and lists
+  cudaSetDevice(device_);
+  cudaStream_t st = nullptr;
+  GB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  int rc = 0;
+  img->fields.resize(1 + extra_.size());
+  for (size_t vi = 0; rc == 0 && vi < img->fields.size(); vi++) {
+    Image::Field& f = img->fields[vi];
+    Index* idx = vslot((int)vi).get();
+    f.name = vname((int)vi);
+    f.dim = vdim((int)vi);
+    rc = idx->store().capture_rows(max_docid_, &f.rows, st);
+    if (rc == 0 && idx->trained()) rc = idx->capture_gamma(&f.index);
+    cudaSetDevice(device_);
   }
-  f.close();
-  // the index itself in gamma's own format (IndexModel::Dump via VectorManager::Dump,
-  // vector_manager.cc:1155-1170): <dir>/<vector name>.000/{ivfflat,ivfpq}.index, or this engine's own file of a
-  // quantised type (gb_ivfpqfs, gb_ivfrabitq, gb_vearch, gb_binaryivf.index); FLAT writes none
-  if (trained && index_->dump_gamma(dir, vec_name_ + ".000")) return -1;
-  for (auto& e : extra_) {  // the other vector fields: raw rows next to the table, index in gamma's format
-    std::ofstream ef(dir + "/" + table_name_ + "." + e.name + ".gbvec", std::ios::binary | std::ios::trunc);
-    std::vector<float> erows((size_t)max_docid_ * e.dim);
-    if (!ef || (max_docid_ && e.index->store().get_rows_host(0, max_docid_, erows.data()))) return -1;
-    wr<int32_t>(ef, max_docid_);
-    wr<int32_t>(ef, e.dim);
-    ef.write(reinterpret_cast<const char*>(erows.data()), (std::streamsize)(erows.size() * 4));
-    if (ef.fail()) return -1;
-    if (e.index->trained() && e.index->dump_gamma(dir, e.name + ".000")) return -1;
+  const cudaError_t e = cudaStreamSynchronize(st);
+  cudaStreamDestroy(st);
+  if (rc) return -1;
+  if (e != cudaSuccess) {
+    set_last_error(std::string("capture of the raw rows: ") + cudaGetErrorString(e));
+    return -1;
   }
-  std::ofstream done(dir + "/dump.done");
-  done << "ok";
-  return f.fail() ? -1 : 0;
+  int64_t dev = 0, host = 0;
+  for (const Image::Field& f : img->fields) {
+    (f.rows.on_host() ? host : dev) += (int64_t)f.rows.size();
+    for (const GammaImage::Part& p : f.index.parts) (p.stage.on_host() ? host : dev) += (int64_t)p.stage.size();
+  }
+  note_capture_stage(dev, host);
+  return 0;
+}
+
+namespace {
+bool write_file(const std::string& path, const std::function<bool(FILE*)>& body) {
+  FILE* f = fopen(path.c_str(), "wb");
+  if (!f) {
+    set_last_error("cannot open " + path + ": " + strerror(errno));
+    return false;
+  }
+  bool ok = body(f);
+  ok = fclose(f) == 0 && ok;
+  if (!ok) set_last_error("write error in " + path);
+  return ok;
+}
+}  // namespace
+
+// Engine::Dump's files (search/engine.cc:1202-1247): <dir>/<table>.gbdump, <dir>/<table>.<field>.gbvec for every further
+// vector field, each index in gamma's format (IndexModel::Dump via VectorManager::Dump, vector_manager.cc:1155-1170):
+// <dir>/<vector name>.000/{ivfflat,ivfpq}.index, or this engine's own file of a quantised type (gb_ivfpqfs,
+// gb_ivfrabitq, gb_vearch, gb_binaryivf.index), none for FLAT; dump.done last
+int Engine::write_image(const Image& img, const std::string& dir) {
+  if (mkdir(dir.c_str(), 0755) && errno != EEXIST) {
+    set_last_error("cannot create " + dir + ": " + strerror(errno));
+    return -1;
+  }
+  const Image::Field& first = img.fields[0];
+  if (!write_file(dir + "/" + img.table_name + ".gbdump", [&](FILE* f) {
+        return fwrite(img.head.data(), 1, img.head.size(), f) == img.head.size() &&
+               first.rows.write(f, 0, first.rows.size()) && fwrite(img.tail.data(), 1, img.tail.size(), f) == img.tail.size();
+      }))
+    return -1;
+  if (write_gamma_image(first.index, dir, first.name + ".000")) return -1;
+  for (size_t vi = 1; vi < img.fields.size(); vi++) {
+    const Image::Field& e = img.fields[vi];
+    if (!write_file(dir + "/" + img.table_name + "." + e.name + ".gbvec", [&](FILE* f) {
+          const int32_t hdr[2] = {img.max_docid, e.dim};
+          return fwrite(hdr, sizeof hdr, 1, f) == 1 && e.rows.write(f, 0, e.rows.size());
+        }))
+      return -1;
+    if (write_gamma_image(e.index, dir, e.name + ".000")) return -1;
+  }
+  return write_file(dir + "/dump.done", [](FILE* f) { return fputs("ok", f) >= 0; }) ? 0 : -1;
+}
+
+// Engine::Dump (search/engine.cc:1202-1247) into <path>/retrieval_model_index: searches and writes wait for the capture
+// only, not for the files
+int Engine::Dump() {
+  if (!created_table_) return -1;
+  join_field_build();  // a run-time index build ends in its swap or its failure first
+  std::lock_guard<std::mutex> dg(dump_mu_);
+  cudaSetDevice(device_);
+  Image img;
+  {
+    std::unique_lock<std::shared_mutex> lk(mu_);
+    if (flush_pending_locked() || capture_locked(&img)) return -1;
+  }
+  mkdir(path_.c_str(), 0755);
+  return write_image(img, path_ + "/retrieval_model_index");
+}
+
+namespace {
+std::atomic<int> g_backup_hold{0};
+
+int remove_tree(const std::string& dir) {
+  return nftw(
+      dir.c_str(), [](const char* p, const struct stat*, int, struct FTW*) { return remove(p); }, 16, FTW_DEPTH | FTW_PHYS);
+}
+// the finished backup at tmp takes dst's place: swapped in one step where the file system can, else by two renames;
+// either way dst is never a partial backup
+int replace_dir(const std::string& tmp, const std::string& dst) {
+  struct stat sb;
+  if (stat(dst.c_str(), &sb) != 0) return rename(tmp.c_str(), dst.c_str());  // the first backup
+  if (renameat2(AT_FDCWD, tmp.c_str(), AT_FDCWD, dst.c_str(), RENAME_EXCHANGE) == 0) return remove_tree(tmp) ? -1 : 0;
+  const std::string old = dst + ".old";
+  remove_tree(old);
+  if (rename(dst.c_str(), old.c_str())) return -1;
+  if (rename(tmp.c_str(), dst.c_str())) {
+    const int why = errno;
+    rename(old.c_str(), dst.c_str());
+    errno = why;
+    return -1;
+  }
+  return remove_tree(old) ? -1 : 0;
+}
+}  // namespace
+
+int backup_hold(int op) {
+  if (op == 1) g_backup_hold = 1;
+  if (op == 0) g_backup_hold = 0;
+  return g_backup_hold.load();
+}
+
+Status Engine::Backup(int command) {
+  int idle = 0;
+  if (!backup_status_.compare_exchange_strong(idle, 1)) return Status::Make(kIOError, "backup is in progress, wait done");
+  struct Idle {
+    std::atomic<int>& s;
+    ~Idle() { s = 0; }
+  } idle_at_exit{backup_status_};
+  if (command != 0) return Status::OK();  // BackupThread acts on "create" only
+  if (path_.empty()) return Status::Make(kInvalidArgument, "backup needs the engine's path, and Init was given none");
+  if (!created_table_) return Status::Make(kInvalidArgument, "backup of an engine without a table");
+  join_field_build();
+  cudaSetDevice(device_);
+  Image img;
+  {
+    std::unique_lock<std::shared_mutex> lk(mu_);
+    if (flush_pending_locked() || capture_locked(&img)) return Status::Make(kIOError, std::string("backup capture: ") + last_error());
+  }
+  int armed = 1;
+  if (g_backup_hold.compare_exchange_strong(armed, 2))
+    while (g_backup_hold.load() == 2) std::this_thread::sleep_for(std::chrono::milliseconds(1));
+  const std::string root = path_ + "/backup", dst = root + "/retrieval_model_index", tmp = dst + ".tmp";
+  mkdir(path_.c_str(), 0755);
+  mkdir(root.c_str(), 0755);
+  remove_tree(tmp);  // left by a process that died during a backup
+  if (mkdir(tmp.c_str(), 0755)) return Status::Make(kIOError, "backup: cannot create " + tmp + ": " + strerror(errno));
+  if (write_image(img, tmp)) {
+    const std::string why = last_error();
+    remove_tree(tmp);
+    return Status::Make(kIOError, "backup: " + why);
+  }
+  if (replace_dir(tmp, dst)) {
+    const std::string why = strerror(errno);
+    remove_tree(tmp);
+    return Status::Make(kIOError, "backup: cannot move " + tmp + " to " + dst + ": " + why);
+  }
+  return Status::OK();
 }
 
 // Engine::Load (search/engine.cc:1278-1400): restore the newest complete dump, then let the

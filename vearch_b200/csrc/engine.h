@@ -118,6 +118,9 @@ std::string encode_index_records(const std::vector<IndexRecord>& recs);
 // the records at the end of a snapshot's last bytes `tail` (none when it does not end with them), and in *bytes their
 // length; -1: a record that does not parse
 int decode_index_records(const std::string& tail, std::vector<IndexRecord>* recs, size_t* bytes);
+// test hook (gb_debug_backup_hold): op 1 makes the next Backup wait between its capture and its write, 0 lets it go
+// on; returns the state, 0 off, 1 set, 2 a Backup is waiting (op -1 only reads it)
+int backup_hold(int op);
 
 class Engine {
  public:
@@ -141,6 +144,10 @@ class Engine {
   std::string GetConfig();
   int Dump();
   int Load();
+  // Engine::Backup (search/engine.cc:1431-1470).  0 ("create"): the state captured as Dump captures it, written into
+  // <path>/backup/retrieval_model_index, which a backup replaces only once complete.  1 ("restore"): nothing to do (the
+  // server places the files and calls Load).  A second Backup while one runs: kIOError.
+  Status Backup(int command);
   const std::string& space_name() const { return space_name_; }
   void quiesce();  // stop the indexing thread (also from an atexit hook for engines never Closed)
   // Engine::AddFieldIndex / RemoveFieldIndex (search/engine.cc:1471-1600): for a scalar field, build the field's device
@@ -163,6 +170,13 @@ class Engine {
 
  private:
   int flush_pending_locked();
+  // Dump and Backup (DESIGN.md §8, backup and snapshots): the table's state is captured under the exclusive lock into
+  // an image, device copies into a stage (stage.h) plus the host table, and written to `dir` after the lock is released
+  struct Image;
+  int capture_locked(Image* img);
+  static int write_image(const Image& img, const std::string& dir);
+  std::mutex dump_mu_;                  // one Dump writes retrieval_model_index at a time
+  std::atomic<int> backup_status_{0};  // 1 while a Backup runs (GetEngineStatus's backup_status)
   void indexing_loop();
   void serialize_doc(int docid, bool with_docid, std::string* out);
   int doc_num() const { return max_docid_ - delete_num_; }

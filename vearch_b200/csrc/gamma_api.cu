@@ -214,9 +214,14 @@ int GetConfig(void* engine, char** config_str, int* len) {
   return 0;
 }
 
-struct CStatus Backup(void*, int) {
+// gamma_api.cc:312-318; the engine's Backup (engine.h) says what each command does
+struct CStatus Backup(void* engine, int command) {
   struct CStatus c;
-  to_cstatus(gb::Status::Make(gb::kNotSupported, "Backup is handled by the storage layer, outside the vector hot path"), &c);
+  if (!engine) {
+    to_cstatus(gb::Status::Make(gb::kInvalidArgument, "null engine"), &c);
+    return c;
+  }
+  to_cstatus(static_cast<Engine*>(engine)->Backup(command), &c);
   return c;
 }
 
@@ -297,6 +302,15 @@ int gb_memory_ledger(int device, int64_t* usage, int64_t* pool_reserved, int64_t
 }
 
 void gb_memory_set_total(int device, int64_t bytes) { gb::mem::set_total(device, bytes); }
+
+int gb_debug_backup_hold(int op) { return gb::backup_hold(op); }
+
+int gb_debug_backup_stage(int64_t* device_bytes, int64_t* host_bytes) {
+  gb::last_capture_stage(device_bytes, host_bytes);
+  return 0;
+}
+
+void* gb_debug_engine_create(const char* path) { return path ? static_cast<void*>(new Engine(path, "default", 0)) : nullptr; }
 
 // the run-time index records at the end of a snapshot's last `len` bytes, as Load reads them:
 // {"bytes": <record part>, "records": [[field, has_index, type, params], ...]}; -1 if a record does not parse

@@ -426,6 +426,23 @@ int RawStore::get_rows_host(int64_t start, int64_t n, void* outv) const {
   }
   return 0;
 }
+int RawStore::capture_rows(int64_t n, Stage* out, cudaStream_t st) const {
+  if (n < 0 || n > n_) return -1;
+  if (out->alloc((size_t)n * row_bytes_, host_ ? mem::kHost : device_)) return -1;
+  for (int64_t done = 0; done < n;) {
+    const int64_t si = done >> seg_shift_, cnt = std::min(n - done, seg_rows());
+    unsigned char* dst = out->data() + done * row_bytes_;
+    if (host_ && stride_ == (int64_t)row_bytes_) {
+      memcpy(dst, segs_[si].base, (size_t)cnt * row_bytes_);
+    } else if (host_) {
+      for (int64_t i = 0; i < cnt; i++) memcpy(dst + i * row_bytes_, segs_[si].base + i * stride_, row_bytes_);
+    } else {  // into HBM, or into pinned host memory when the device could not hold the stage
+      GB_CUDA(cudaMemcpy2DAsync(dst, row_bytes_, segs_[si].base, stride_, row_bytes_, (size_t)cnt, cudaMemcpyDefault, st));
+    }
+    done += cnt;
+  }
+  return 0;
+}
 cudaError_t RawStore::copy_rows_to_device(int64_t start, int64_t n, void* dstv, cudaStream_t st) const {
   unsigned char* dst = static_cast<unsigned char*>(dstv);
   int64_t done = 0;
@@ -688,6 +705,22 @@ int IvfLists::purge(const std::vector<int>& lists, const uint32_t* d_del_bits, c
   GB_CUDA(cudaMemcpyAsync(d_len_, h_len_.data(), sizeof(int) * nlist_, cudaMemcpyHostToDevice, st));
   content_gen_++;
   return 0;
+}
+int64_t IvfLists::pack_bytes(int file_cb) const {
+  int64_t n = 0;
+  for (int len : h_len_) n += len;
+  return n * (file_cb + 8);
+}
+void IvfLists::pack_chunks(int file_cb, uint8_t* dst, std::vector<PackChunk>* out) const {
+  const int per = std::max(1, kPackChunkBytes / code_bytes_);
+  for (int l = 0; l < nlist_; l++) {
+    const int len = h_len_[l];
+    uint8_t* ids = dst + (size_t)len * file_cb;
+    for (int first = 0; first < len; first += per)
+      out->push_back(PackChunk{static_cast<const uint8_t*>(h_data_[l]) + (size_t)first * code_bytes_, h_ids_[l] + first,
+                               dst + (size_t)first * file_cb, ids + (size_t)first * 8, std::min(per, len - first)});
+    dst = ids + (size_t)len * 8;
+  }
 }
 int IvfLists::download_list(int l, std::vector<uint8_t>* codes, std::vector<int64_t>* ids) const {
   if (l < 0 || l >= nlist_) return -1;

@@ -22,10 +22,12 @@
 
 #include "kernels.h"
 #include "mem_ledger.h"
+#include "stage.h"
 
 namespace gb {
 
 void set_last_error(const std::string& msg);
+struct GammaImage;
 const char* last_error();
 #define GB_CUDA(expr)                                                                              \
   do {                                                                                             \
@@ -84,6 +86,9 @@ class RawStore {
   int update_host(int64_t vid, const void* x, cudaStream_t st);
   int get_host(int64_t vid, void* out) const;
   int get_rows_host(int64_t start, int64_t n, void* out) const;  // n x row_bytes, packed
+  // a capture (stage.h): rows [0, n) packed into *out, device to device in stream order on st (HBM placement), or host
+  // to host (host placement)
+  int capture_rows(int64_t n, Stage* out, cudaStream_t st) const;
   // the rows [0, n) contiguous in device memory, stride() bytes apart (training slab, GetVectorHeader): the segment
   // itself or a copy owned by `s`
   const float* contiguous(int64_t n, Scratch& s);
@@ -152,8 +157,12 @@ class IvfLists {
   int commit(const std::vector<int>& add, cudaStream_t st);
   // tombstone one entry (Update path, realtime_mem_data.cc:298-320)
   int tombstone(int list, int pos, cudaStream_t st);
-  // host copies for dump / parity tests
+  // host copies for parity tests
   int download_list(int l, std::vector<uint8_t>* codes, std::vector<int64_t>* ids) const;
+  // a capture (stage.h): every list in the index file's order, each its codes cut to file_cb bytes then its ids, takes
+  // pack_bytes(file_cb) bytes; pack_chunks appends the chunks that copy them to dst (launch_list_pack)
+  int64_t pack_bytes(int file_cb) const;
+  void pack_chunks(int file_cb, uint8_t* dst, std::vector<PackChunk>* out) const;
   // append position of list l (valid after reserve): where the next entry's code / id goes
   void* list_data(int l) const { return static_cast<char*>(h_data_[l]) + (size_t)h_len_[l] * code_bytes_; }
   int64_t* list_ids(int l) const { return h_ids_[l] + h_len_[l]; }
@@ -342,8 +351,11 @@ class Index {
   virtual void charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) { (void)rows; (void)out; }
   // free the scan scratch buffers no search is using (the memory limit's trim)
   void release_idle_scratch();
-  // gamma's own index file of the type (IvfIndex::dump_gamma / load_gamma); the types without one write and read nothing
-  virtual int dump_gamma(const std::string& dir, const std::string& abs_name) { (void)dir; (void)abs_name; return 0; }
+  // gamma's own index file of the type (index_io.cu); the types without one write and read nothing.  capture_gamma
+  // copies the file's content into an image (GammaImage) under the index's build lock, write_gamma_image writes it
+  // without touching the index; dump_gamma does both
+  int dump_gamma(const std::string& dir, const std::string& abs_name);
+  virtual int capture_gamma(GammaImage* img) { (void)img; return 0; }
   virtual int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) {
     (void)dir; (void)abs_name;
     *load_num = 0;
@@ -537,6 +549,25 @@ struct GammaFileFormat {
   bool indexed_count = false;  // an i32 indexed_count follows the lists
 };
 
+// An index file as a capture took it (Index::capture_gamma): the bytes before the lists, and the lists of the index, or
+// of each shard of a sharded one, staged in the file's order with the shard's local ids
+struct GammaImage {
+  std::string file;  // <dir>/<abs_name>/<file>; empty: the index writes no file
+  std::string head;  // ivf header, coarse quantiser, direct map and codec block
+  uint64_t code_size = 0;
+  int nlist = 0;
+  int64_t indexed = 0;
+  bool indexed_count = false;
+  struct Part {
+    std::vector<int> lens;
+    Stage stage;
+  };
+  std::vector<Part> parts;  // shard s holds global vid v as local v / S when v % S == s (S = parts.size())
+};
+// the file of a captured image; the lists of several parts are merged by global vid, the smallest head first and ties
+// to the lower shard, so after adds alone a list is in vid order as the unsharded list is
+int write_gamma_image(const GammaImage& img, const std::string& dir, const std::string& abs_name);
+
 // The inverted-file skeleton shared by every IVF type: coarse centroids, inverted lists, train / add / update / reset /
 // compact, coarse search, and the gamma index-file skeleton.  A codec derived from it says how vectors become list
 // entries (append_batch, code_bytes) and how a query scans the probed lists (scan_dev).
@@ -571,7 +602,7 @@ class IvfIndex : public Index {
   int compact_lists();
   // gamma's own index files (index_io.cu): <dir>/<abs_name>/<gamma_format().file>.  load: the vector
   // store must already hold the vectors the file indexes; *load_num = IndexModel::Load's load_num
-  int dump_gamma(const std::string& dir, const std::string& abs_name) override;
+  int capture_gamma(GammaImage* img) override;
   int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) override;
 
  protected:
@@ -591,10 +622,11 @@ class IvfIndex : public Index {
   // vid, nullable), ordered on build_stream_; build_mu_ and mu_ held exclusively
   std::vector<int> purge_candidates(float threshold) const;
   int purge_locked(const std::vector<int>& sel, const uint32_t* d_del_bits, int64_t* dropped);
-  // the gamma index file with this index's header and trained state, `lens` and the list contents `fetch` gives
-  // (codes of code_bytes() bytes and ids per list); build_mu_ held
-  int write_gamma(const std::string& dir, const std::string& abs_name, int64_t indexed, const std::vector<int>& lens,
-                  const std::function<int(int, std::vector<uint8_t>*, std::vector<int64_t>*)>& fetch);
+  // the image's file, head and trained state, for `indexed` vectors; build_mu_ held
+  int capture_head(int64_t indexed, GammaImage* img);
+  // the lists of `shards` (one index, or every shard of a sharded one; build locks held) into the image's parts, one
+  // pack launch per device, finished when it returns
+  static int capture_lists(const std::vector<IvfIndex*>& shards, GammaImage* img);
   // load_gamma keeping only the file's entries of this shard (global vid % shard_count_ == shard_id_, as local vids);
   // store_rows: the rows of the (global) vector store; *file_indexed = the file's indexed count (IvFl) or this shard's
   // live entries (IwPQ)
@@ -1032,8 +1064,8 @@ class ShardedIndex : public Index {
   int reset_index() override;
   int64_t index_mem_bytes() const override;
   void charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) override;  // each shard its share
-  // the unsharded type's file: list l is the merge of the shards' lists l by global vid, ids written as global vids
-  int dump_gamma(const std::string& dir, const std::string& abs_name) override;
+  // the unsharded type's file: every shard's lists, merged by global vid when written (write_gamma_image)
+  int capture_gamma(GammaImage* img) override;
   // every shard reads the file and keeps its own entries
   int load_gamma(const std::string& dir, const std::string& abs_name, int64_t* load_num) override;
 

@@ -584,6 +584,17 @@ int gb_index_dump(gb_index* index, const char* dir, const char* abs_name) {
   cudaSetDevice(index->impl->device());
   return index->impl->dump_gamma(dir, abs_name);
 }
+int gb_index_capture_lists(gb_index* index, uint8_t* out, int64_t cap, int64_t* bytes, int* on_host) {
+  IDX_OR_FAIL(index);
+  if (!bytes || !on_host || shard_view(index) || sharded(index)) return -1;
+  cudaSetDevice(index->impl->device());
+  GammaImage img;
+  if (index->impl->capture_gamma(&img)) return -1;
+  const Stage* st = img.parts.empty() ? nullptr : &img.parts[0].stage;
+  *bytes = st ? (int64_t)st->size() : 0;
+  *on_host = st && st->on_host() ? 1 : 0;
+  return out && st ? st->read(0, (size_t)std::min<int64_t>(cap, *bytes), out) : 0;
+}
 int gb_index_load(gb_index* index, const char* dir, const char* abs_name, int64_t* load_num) {
   if (shard_view(index)) return -1;
   IDX_OR_FAIL(index);

@@ -116,60 +116,146 @@ GammaFileFormat BinaryIvfIndex::gamma_format() const {
   return {"gb_binaryivf.index", fourcc("GbBI"), (uint64_t)code_bytes(), true};
 }
 
-// ---- Dump -----------------------------------------------------------------------------------
-int IvfIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
-  if (!trained_ || !gamma_format().file) return 0;  // "gamma index is not trained, skip dumping" (ivfflat.cc:808-811)
-  std::lock_guard<std::mutex> bg(build_mu_);  // no list mutation while the lists are copied out
-  return write_gamma(dir, abs_name, indexed_count_, lists_->lens(),
-                     [this](int l, std::vector<uint8_t>* codes, std::vector<int64_t>* ids) {
-                       return lists_->download_list(l, codes, ids);
-                     });
+// ---- Dump: capture, then write ----------------------------------------------------------------
+int Index::dump_gamma(const std::string& dir, const std::string& abs_name) {
+  GammaImage img;
+  return capture_gamma(&img) ? -1 : write_gamma_image(img, dir, abs_name);
 }
 
-int IvfIndex::write_gamma(const std::string& dir, const std::string& abs_name, int64_t indexed, const std::vector<int>& lens,
-                          const std::function<int(int, std::vector<uint8_t>*, std::vector<int64_t>*)>& fetch) {
+int IvfIndex::capture_gamma(GammaImage* img) {
+  if (!trained_ || !gamma_format().file) return 0;  // "gamma index is not trained, skip dumping" (ivfflat.cc:808-811)
+  std::lock_guard<std::mutex> bg(build_mu_);  // no list mutation while the lists are copied out
+  if (capture_head(indexed_count_, img)) return -1;
+  return capture_lists({this}, img);
+}
+
+int IvfIndex::capture_head(int64_t indexed, GammaImage* img) {
   const GammaFileFormat gf = gamma_format();
   cudaSetDevice(device_);
-  const std::string index_dir = dir + "/" + abs_name;
-  mkdir(dir.c_str(), 0755);
-  if (mkdir(index_dir.c_str(), 0755) && errno != EEXIST) return fail("mkdir error, index dir=" + index_dir);
-  const std::string path = index_dir + "/" + gf.file;
-  FilePtr fp(fopen(path.c_str(), "wb"));
-  FILE* f = fp.get();
-  if (!f) return fail("cannot open " + path);
+  img->file = gf.file;
+  img->code_size = gf.code_size;
+  img->nlist = nlist_;
+  img->indexed = indexed;
+  img->indexed_count = gf.indexed_count;
+  std::vector<float> cent((size_t)nlist_ * d_);
+  if (get_centroids(cent.data())) return -1;
+  char* buf = nullptr;
+  size_t len = 0;
+  FILE* f = open_memstream(&buf, &len);
+  if (!f) return fail("cannot capture the index header");
   bool ok = wr<uint32_t>(f, gf.magic);
   // write_ivf_header (index_io.cc:41-47)
   ok = ok && wr_index_header(f, d_, indexed, mp_.metric);
   ok = ok && wr<uint64_t>(f, (uint64_t)nlist_) && wr<uint64_t>(f, (uint64_t)mp_.nprobe);
-  std::vector<float> cent((size_t)nlist_ * d_);
-  if (get_centroids(cent.data())) return -1;
   ok = ok && wr<uint32_t>(f, mp_.metric == kMetricL2 ? fourcc("IxF2") : fourcc("IxFI"));
   ok = ok && wr_index_header(f, d_, nlist_, mp_.metric);
   ok = ok && wr<uint64_t>(f, (uint64_t)cent.size()) && wr_bytes(f, cent.data(), cent.size() * 4);  // WRITEXBVECTOR
   ok = ok && wr<uint8_t>(f, 0) && wr<uint64_t>(f, 0);                                              // direct map: none
-  if (!ok) return fail("write error in " + path);
-  if (dump_gamma_extra(f)) return fail("write error in " + path);
-  // WriteInvertedLists (index_io.cc:108-141)
-  const uint64_t cb = gf.code_size;
-  ok = wr<uint32_t>(f, fourcc("ilar")) && wr<uint64_t>(f, (uint64_t)nlist_) && wr<uint64_t>(f, cb) &&
-       wr<uint32_t>(f, fourcc("full")) && wr<uint64_t>(f, (uint64_t)nlist_);
-  for (int l = 0; ok && l < nlist_; l++) ok = wr<uint64_t>(f, (uint64_t)lens[l]);
-  std::vector<uint8_t> codes, packed;
-  std::vector<int64_t> ids;
-  for (int l = 0; ok && l < nlist_; l++) {
-    if (lens[l] == 0) continue;
-    if (fetch(l, &codes, &ids)) return -1;
-    const size_t n = (size_t)lens[l];
-    if (ids.size() < n) return fail("list shrank during dump");
-    const uint8_t* src = codes.data();
-    if (cb != (uint64_t)code_bytes()) {  // padded rows in memory
-      packed.resize(n * cb);
-      for (size_t r = 0; r < n; r++) memcpy(packed.data() + r * cb, codes.data() + r * (size_t)code_bytes(), cb);
-      src = packed.data();
+  ok = ok && dump_gamma_extra(f) == 0;
+  ok = fclose(f) == 0 && ok;
+  if (ok) img->head.assign(buf, len);
+  free(buf);
+  return ok ? 0 : fail("cannot capture the trained state of the index");
+}
+
+int IvfIndex::capture_lists(const std::vector<IvfIndex*>& shards, GammaImage* img) {
+  const int S = (int)shards.size(), cb = (int)img->code_size, src_cb = shards[0]->code_bytes();
+  img->parts.clear();
+  img->parts.resize(S);
+  std::vector<std::pair<int, std::vector<PackChunk>>> by_device;  // one launch per device
+  for (int s = 0; s < S; s++) {
+    const IvfLists* lists = shards[s]->lists_.get();
+    GammaImage::Part& part = img->parts[s];
+    part.lens = lists ? lists->lens() : std::vector<int>(img->nlist, 0);
+    if (!lists || part.stage.alloc((size_t)lists->pack_bytes(cb), shards[s]->device_)) {
+      if (!lists) continue;
+      return -1;
     }
-    ok = wr_bytes(f, src, n * cb) && wr_bytes(f, ids.data(), n * 8);
+    auto at = std::find_if(by_device.begin(), by_device.end(), [&](const auto& e) { return e.first == shards[s]->device_; });
+    if (at == by_device.end()) at = by_device.emplace(by_device.end(), shards[s]->device_, std::vector<PackChunk>());
+    lists->pack_chunks(cb, part.stage.data(), &at->second);
   }
-  if (ok && gf.indexed_count) ok = wr<int32_t>(f, (int32_t)indexed);  // ivfflat.cc:835
+  for (auto& [dev, chunks] : by_device) {
+    if (chunks.empty()) continue;
+    uintptr_t bits = (uintptr_t)src_cb | (uintptr_t)cb | 16;
+    for (const PackChunk& c : chunks)
+      bits |= (uintptr_t)c.src_codes | (uintptr_t)c.src_ids | (uintptr_t)c.dst_codes | (uintptr_t)c.dst_ids;
+    const int align = (int)(bits & (~bits + 1));  // lowest set bit: at most 16
+    cudaSetDevice(dev);
+    cudaStream_t st = nullptr;
+    GB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    cudaError_t e;
+    {
+      Scratch sc(st);
+      PackChunk* d_chunks = sc.alloc_n<PackChunk>(chunks.size());
+      e = d_chunks ? cudaMemcpyAsync(d_chunks, chunks.data(), sizeof(PackChunk) * chunks.size(), cudaMemcpyHostToDevice, st)
+                   : cudaErrorMemoryAllocation;
+      if (e == cudaSuccess) e = launch_list_pack(d_chunks, (int)chunks.size(), src_cb, cb, align, st);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(st);  // the stage is complete before the lock is released
+    }
+    cudaStreamDestroy(st);
+    if (e != cudaSuccess) return fail(std::string("list pack: ") + cudaGetErrorString(e));
+  }
+  return 0;
+}
+
+int write_gamma_image(const GammaImage& img, const std::string& dir, const std::string& abs_name) {
+  if (img.file.empty()) return 0;
+  const std::string index_dir = dir + "/" + abs_name;
+  mkdir(dir.c_str(), 0755);
+  if (mkdir(index_dir.c_str(), 0755) && errno != EEXIST) return fail("mkdir error, index dir=" + index_dir);
+  const std::string path = index_dir + "/" + img.file;
+  FilePtr fp(fopen(path.c_str(), "wb"));
+  FILE* f = fp.get();
+  if (!f) return fail("cannot open " + path);
+  const int S = (int)img.parts.size(), nlist = img.nlist;
+  const uint64_t cb = img.code_size;
+  std::vector<int> lens(nlist, 0);
+  for (const GammaImage::Part& p : img.parts)
+    for (int l = 0; l < nlist; l++) lens[l] += p.lens[l];
+  // WriteInvertedLists (index_io.cc:108-141)
+  bool ok = wr_bytes(f, img.head.data(), img.head.size()) && wr<uint32_t>(f, fourcc("ilar")) &&
+            wr<uint64_t>(f, (uint64_t)nlist) && wr<uint64_t>(f, cb) && wr<uint32_t>(f, fourcc("full")) &&
+            wr<uint64_t>(f, (uint64_t)nlist);
+  for (int l = 0; ok && l < nlist; l++) ok = wr<uint64_t>(f, (uint64_t)lens[l]);
+  if (ok && S == 1) {
+    ok = img.parts[0].stage.write(f, 0, img.parts[0].stage.size());
+  } else if (ok) {
+    std::vector<std::vector<uint8_t>> part(S);
+    std::vector<size_t> at(S, 0);  // list l of shard s starts at part[s][at[s]]: its codes, then its ids
+    for (int s = 0; s < S; s++) {
+      part[s].resize(img.parts[s].stage.size());
+      if (img.parts[s].stage.read(0, part[s].size(), part[s].data())) return -1;
+    }
+    std::vector<uint8_t> codes;
+    std::vector<int64_t> ids;
+    std::vector<int> head(S);
+    auto id_of = [&](int s, int l, int j) {
+      int64_t id;
+      memcpy(&id, part[s].data() + at[s] + (size_t)img.parts[s].lens[l] * cb + (size_t)j * 8, 8);
+      return ((id & ~kDelIdxMask) * S + s) | (id & kDelIdxMask);
+    };
+    for (int l = 0; ok && l < nlist; l++) {
+      codes.resize((size_t)lens[l] * cb);
+      ids.resize(lens[l]);
+      std::fill(head.begin(), head.end(), 0);
+      for (int j = 0; j < lens[l]; j++) {
+        int best = -1;
+        int64_t best_id = 0;
+        for (int s = 0; s < S; s++) {
+          if (head[s] >= img.parts[s].lens[l]) continue;
+          const int64_t id = id_of(s, l, head[s]);
+          if (best < 0 || (id & ~kDelIdxMask) < (best_id & ~kDelIdxMask)) best = s, best_id = id;
+        }
+        memcpy(codes.data() + (size_t)j * cb, part[best].data() + at[best] + (size_t)head[best] * cb, cb);
+        ids[j] = best_id;
+        head[best]++;
+      }
+      for (int s = 0; s < S; s++) at[s] += (size_t)img.parts[s].lens[l] * (cb + 8);
+      ok = wr_bytes(f, codes.data(), codes.size()) && wr_bytes(f, ids.data(), ids.size() * 8);
+    }
+  }
+  if (ok && img.indexed_count) ok = wr<int32_t>(f, (int32_t)img.indexed);  // ivfflat.cc:835
   if (!ok || fflush(f)) return fail("write error in " + path);
   return 0;
 }

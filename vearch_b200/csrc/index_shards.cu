@@ -401,51 +401,17 @@ void ShardedIndex::charge_index_rows(int64_t rows, std::vector<mem::Charge>* out
 }
 
 // ---- gamma's index file ----------------------------------------------------------------------
-int ShardedIndex::dump_gamma(const std::string& dir, const std::string& abs_name) {
+int ShardedIndex::capture_gamma(GammaImage* img) {
   if (!trained_) return 0;
   std::lock_guard<std::mutex> bg(build_mu_);
-  const int S = nshards();
   IvfIndex* s0 = shards_[0].get();
-  const int nlist = s0->nlist();
-  std::vector<std::vector<int>> lens(S);
-  std::vector<int> total(nlist, 0);
-  for (int s = 0; s < S; s++) {
-    lens[s] = shards_[s]->lists_ ? shards_[s]->lists_->lens() : std::vector<int>(nlist, 0);
-    for (int l = 0; l < nlist; l++) total[l] += lens[s][l];
-  }
-  const size_t cb = (size_t)s0->code_bytes();
-  std::vector<std::vector<uint8_t>> codes(S);
-  std::vector<std::vector<int64_t>> ids(S);
-  // list l: the S segments merged by global vid (the smallest head first, ties to the lower shard), each segment in its
-  // own order; after adds only every segment is in vid order, and so is the merge, as the unsharded list is
-  auto fetch = [&](int l, std::vector<uint8_t>* out_codes, std::vector<int64_t>* out_ids) {
-    for (int s = 0; s < S; s++) {
-      codes[s].clear();
-      ids[s].clear();
-      if (lens[s][l] == 0) continue;
-      cudaSetDevice(shards_[s]->device());
-      if (shards_[s]->lists_->download_list(l, &codes[s], &ids[s])) return -1;
-      if ((int)ids[s].size() < lens[s][l]) return -1;
-      for (int64_t& id : ids[s]) id = ((id & ~kDelIdxMask) * S + s) | (id & kDelIdxMask);
-    }
-    out_codes->resize((size_t)total[l] * cb);
-    out_ids->resize((size_t)total[l]);
-    std::vector<int> head(S, 0);
-    for (int j = 0; j < total[l]; j++) {
-      int best = -1;
-      for (int s = 0; s < S; s++)
-        if (head[s] < lens[s][l] &&
-            (best < 0 || (ids[s][head[s]] & ~kDelIdxMask) < (ids[best][head[best]] & ~kDelIdxMask)))
-          best = s;
-      memcpy(out_codes->data() + (size_t)j * cb, codes[best].data() + (size_t)head[best] * cb, cb);
-      (*out_ids)[j] = ids[best][head[best]++];
-    }
-    return 0;
-  };
+  std::vector<IvfIndex*> shards;
+  for (auto& sh : shards_) shards.push_back(sh.get());
   int rc;
   {
     std::lock_guard<std::mutex> sbg(s0->build_mu_);  // the other shards' lists change only under build_mu_, held here
-    rc = s0->write_gamma(dir, abs_name, indexed_count_, total, fetch);
+    rc = s0->capture_head(indexed_count_, img);
+    if (!rc) rc = IvfIndex::capture_lists(shards, img);
   }
   cudaSetDevice(device_);
   return rc;

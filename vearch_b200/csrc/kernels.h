@@ -369,6 +369,20 @@ cudaError_t launch_purge_scatter(ListDirectory dir, const int* sel_list, const P
                                  const uint32_t* del_bits, const int* chunk_off, int code_bytes, int align,
                                  void* const* dst_data, int64_t* const* dst_ids, unsigned long long* newpos,
                                  int64_t vid_min, cudaStream_t st);
+// List pack (the capture of a backup or dump, stage.h): n entries of one list from its slab region into a stage, in the
+// index file's order.  Each code keeps the first dst_cb of its src_cb bytes (IVF-Flat rows drop their padding); the
+// ids are copied as stored, tombstone bits included, to dst_ids, which may sit at any byte offset.  A list is cut into
+// chunks of about kPackChunkBytes of codes, one CTA each, so a long list spreads over the device.
+constexpr int kPackChunkBytes = 64 << 10;
+struct PackChunk {
+  const uint8_t* src_codes;
+  const int64_t* src_ids;
+  uint8_t* dst_codes;
+  uint8_t* dst_ids;
+  int n;
+};
+// align: the widest power of two <= 16 that divides src_cb, dst_cb and every pointer of every chunk
+cudaError_t launch_list_pack(const PackChunk* chunks, int nchunks, int src_cb, int dst_cb, int align, cudaStream_t st);
 cudaError_t launch_fill_u64(unsigned long long* p, int64_t n, unsigned long long v, cudaStream_t st);
 cudaError_t launch_pad_rows(const float* src, int64_t n, int d, float* dst, int64_t ldd, cudaStream_t st);
 

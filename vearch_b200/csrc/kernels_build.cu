@@ -5,6 +5,8 @@
 // gamma_index_ivfflat.cc:407 and gamma_index_ivfpq.cc:372), compute_residuals
 // (gamma_index_ivfpq.cc:378-391), the training-slab merge (gamma_index_ivfflat.cc:377-405) and
 // RTInvertIndex::AddKeys / RealTimeMemData::AddKeys (index/realtime/realtime_mem_data.cc:258-296).
+#include <type_traits>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -427,6 +429,46 @@ cudaError_t launch_purge_scatter(ListDirectory dir, const int* sel_list, const P
     default: return cudaErrorInvalidValue;
   }
 #undef GB_PURGE_SCATTER
+  note_launch();
+  return cudaGetLastError();
+}
+
+namespace {
+// consecutive threads on consecutive units of the destination, as the purge's scatter; ids move in units of at most
+// 8 bytes, since a chunk's ids need not fill a 16-byte unit
+template <typename V>
+__global__ void __launch_bounds__(256)
+    list_pack_kernel(const PackChunk* __restrict__ chunks, int src_cb, int dst_cb) {
+  using I = typename std::conditional<(sizeof(V) > 8), uint2, V>::type;
+  const PackChunk c = chunks[blockIdx.x];
+  const int svpr = src_cb / (int)sizeof(V), dvpr = dst_cb / (int)sizeof(V);
+  const V* __restrict__ src = reinterpret_cast<const V*>(c.src_codes);
+  V* __restrict__ dst = reinterpret_cast<V*>(c.dst_codes);
+  const int units = c.n * dvpr;  // <= max(kPackChunkBytes, one code) / sizeof(V)
+#pragma unroll 4
+  for (int u = threadIdx.x; u < units; u += 256) {
+    const int e = u / dvpr;
+    dst[u] = src[(int64_t)e * svpr + (u - e * dvpr)];
+  }
+  const I* __restrict__ sid = reinterpret_cast<const I*>(c.src_ids);
+  I* __restrict__ did = reinterpret_cast<I*>(c.dst_ids);
+  const int iunits = c.n * (8 / (int)sizeof(I));
+#pragma unroll 4
+  for (int u = threadIdx.x; u < iunits; u += 256) did[u] = sid[u];
+}
+}  // namespace
+
+cudaError_t launch_list_pack(const PackChunk* chunks, int nchunks, int src_cb, int dst_cb, int align, cudaStream_t st) {
+  if (nchunks <= 0) return cudaSuccess;
+  if (dst_cb <= 0 || dst_cb > src_cb || align <= 0 || src_cb % align || dst_cb % align) return cudaErrorInvalidValue;
+  switch (align) {
+    case 16: list_pack_kernel<uint4><<<nchunks, 256, 0, st>>>(chunks, src_cb, dst_cb); break;
+    case 8: list_pack_kernel<uint2><<<nchunks, 256, 0, st>>>(chunks, src_cb, dst_cb); break;
+    case 4: list_pack_kernel<uint32_t><<<nchunks, 256, 0, st>>>(chunks, src_cb, dst_cb); break;
+    case 2: list_pack_kernel<uint16_t><<<nchunks, 256, 0, st>>>(chunks, src_cb, dst_cb); break;
+    case 1: list_pack_kernel<uint8_t><<<nchunks, 256, 0, st>>>(chunks, src_cb, dst_cb); break;
+    default: return cudaErrorInvalidValue;
+  }
   note_launch();
   return cudaGetLastError();
 }

@@ -104,6 +104,19 @@ def memory_ledger(device):
     return u.value, p.value, lim.value
 
 
+def backup_hold(op):
+    """test hook: 1 makes the next backup wait between its capture and its write, 0 lets it go on, -1 only reads.
+    Returns 0 (off), 1 (set) or 2 (a backup is waiting)."""
+    return _api().gb_debug_backup_hold(int(op))
+
+
+def backup_stage():
+    """(bytes in HBM, bytes in pinned host memory) the last finished capture of a dump or backup staged."""
+    d, h = C.c_int64(), C.c_int64()
+    _api().gb_debug_backup_stage(C.byref(d), C.byref(h))
+    return d.value, h.value
+
+
 def set_memory_total(device, nbytes):
     """test hook: the total memory the limit's percentage applies to on a device (-1: host); 0 restores the real one."""
     _api().gb_memory_set_total(device, int(nbytes))
@@ -229,6 +242,11 @@ class GammaEngine:
 
     def load(self):
         return _api().Load(self._h)
+
+    def backup(self, command=0):
+        """Backup: 0 ("create") captures the partition as Dump does and writes it to <path>/backup/retrieval_model_index,
+        replacing the previous backup only once complete; 1 ("restore") does nothing.  Raises GammaStatusError."""
+        _status(_api().Backup(self._h, int(command)))
 
     def set_config(self, cfg):
         b = json.dumps(cfg).encode()

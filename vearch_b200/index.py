@@ -377,6 +377,15 @@ class GammaIndex:
         VEARCH and BINARYIVF write this engine's own gb_{ivfpqfs,ivfrabitq,vearch,binaryivf}.index."""
         _check(_lib.lib().gb_index_dump(self._h, str(directory).encode(), abs_name.encode()), "dump")
 
+    def capture_lists(self):
+        """The lists as Dump and Backup capture them: (bytes, on_host), the bytes in the index file's order (per list its
+        codes at the file's code size, then its ids as stored) and whether they were staged in pinned host memory."""
+        n, host = C.c_int64(), C.c_int32()
+        _check(_lib.lib().gb_index_capture_lists(self._h, None, 0, C.byref(n), C.byref(host)), "capture_lists")
+        out = np.empty(n.value, np.uint8)
+        _check(_lib.lib().gb_index_capture_lists(self._h, _ptr(out), n.value, C.byref(n), C.byref(host)), "capture_lists")
+        return out, bool(host.value)
+
     def load(self, directory, abs_name):
         """IndexModel::Load; returns load_num (0: no file).  The vectors must already be in the store.  A refused file raises;
         an index of the four quantised types is then left untrained."""
