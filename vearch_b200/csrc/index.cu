@@ -11,6 +11,7 @@
 #include <random>
 
 #include "common.cuh"
+#include "jacobi_svd.h"
 #include "mem_ledger.h"
 
 namespace gb {
@@ -2456,45 +2457,6 @@ IVFPQIndex::IVFPQIndex(const std::string& type, int d, const ModelParams& mp, in
 // min ||X R^T - Y|| by an SVD of X^T Y }.  The projection and X^T Y run on the device, the d x d SVD (one-sided
 // Jacobi, double precision) on the host.  The random start cannot reproduce faiss's generator, so parity with
 // the reference is statistical (recall), as for k-means.
-namespace {
-// A (d x d2, row-major) = U diag(s) V^T by one-sided Jacobi on the columns; returns U (d x d2) and V (d2 x d2)
-void jacobi_svd(std::vector<double>& a, int d, int d2, std::vector<double>* u, std::vector<double>* v) {
-  v->assign((size_t)d2 * d2, 0.0);
-  for (int i = 0; i < d2; i++) (*v)[(size_t)i * d2 + i] = 1.0;
-  for (int sweep = 0; sweep < 60; sweep++) {
-    double off = 0;
-    for (int p = 0; p < d2 - 1; p++)
-      for (int q = p + 1; q < d2; q++) {
-        double alpha = 0, beta = 0, gamma = 0;
-        for (int i = 0; i < d; i++) {
-          const double x = a[(size_t)i * d2 + p], y = a[(size_t)i * d2 + q];
-          alpha += x * x, beta += y * y, gamma += x * y;
-        }
-        if (fabs(gamma) <= 1e-15 * sqrt(alpha * beta) || gamma == 0) continue;
-        off = std::max(off, fabs(gamma) / sqrt(alpha * beta + 1e-300));
-        const double zeta = (beta - alpha) / (2.0 * gamma);
-        const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
-        const double c = 1.0 / sqrt(1.0 + t * t), sn = c * t;
-        for (int i = 0; i < d; i++) {
-          const double x = a[(size_t)i * d2 + p], y = a[(size_t)i * d2 + q];
-          a[(size_t)i * d2 + p] = c * x - sn * y, a[(size_t)i * d2 + q] = sn * x + c * y;
-        }
-        for (int i = 0; i < d2; i++) {
-          const double x = (*v)[(size_t)i * d2 + p], y = (*v)[(size_t)i * d2 + q];
-          (*v)[(size_t)i * d2 + p] = c * x - sn * y, (*v)[(size_t)i * d2 + q] = sn * x + c * y;
-        }
-      }
-    if (off < 1e-12) break;
-  }
-  u->assign((size_t)d * d2, 0.0);
-  for (int j = 0; j < d2; j++) {
-    double nrm = 0;
-    for (int i = 0; i < d; i++) nrm += a[(size_t)i * d2 + j] * a[(size_t)i * d2 + j];
-    nrm = sqrt(nrm);
-    for (int i = 0; i < d; i++) (*u)[(size_t)i * d2 + j] = nrm > 1e-300 ? a[(size_t)i * d2 + j] / nrm : (i == j ? 1.0 : 0.0);
-  }
-}
-}  // namespace
 
 int IVFPQIndex::set_opq(const float* host_A) {
   if (!d_opq_) {
@@ -2553,29 +2515,56 @@ int IVFPQIndex::apply_opq_host(const float* x, int64_t n, float* out) {
 
 const float* IVFPQIndex::train_transform(const float* xt, int64_t n_in, Scratch& s) {
   if (!d_opq_) return xt;
-  if (opq_trained_) return transform_dev(xt, n_in, s);
-  cudaStream_t st = s.stream();
-  const int d = d_, Mo = mp_.opq_nsubvector, dso = d / Mo, dsp = (int)round_up(dso, 4);
+  if (!opq_trained_) {
+    if (opq_train_device(xt, n_in, d_, dpad_, mp_.opq_nsubvector, 50, d_opq_, s.stream())) return nullptr;
+    opq_trained_ = true;
+  }
+  return transform_dev(xt, n_in, s);
+}
+
+// the n x d leading block of an n x ld device matrix appended to a trace (stream-ordered, synchronous)
+template <typename T>
+static cudaError_t trace_rows(const T* x, int64_t ld, int64_t n, int d, std::vector<T>& out, cudaStream_t st) {
+  const size_t at = out.size();
+  out.resize(at + (size_t)n * d);
+  cudaError_t e = cudaMemcpy2DAsync(out.data() + at, (size_t)d * sizeof(T), x, (size_t)ld * sizeof(T),
+                                    (size_t)d * sizeof(T), n, cudaMemcpyDeviceToHost, st);
+  return e != cudaSuccess ? e : cudaStreamSynchronize(st);
+}
+
+int opq_train_device(const float* xt, int64_t n_in, int d, int dpad, int Mo, int niter, float* d_opq, cudaStream_t st,
+                     OpqTrace* trace) {
+  Scratch s(st);
+  const int dso = d / Mo, dsp = (int)round_up(dso, 4);
   const int64_t n = std::min<int64_t>(n_in, 256 * 256);  // max_train_points
   const float* xs;
-  if (subsample_rows(xt, n_in, n, dpad_, &xs, s)) return nullptr;
+  if (subsample_rows(xt, n_in, n, dpad, &xs, s)) return -1;
+  if (trace && n < n_in) {
+    std::vector<int32_t> perm;
+    rand_perm_mt(perm, n_in, 1234);
+    trace->sample.assign(perm.begin(), perm.begin() + n);
+  }
   const int64_t ldn = round_up(n, 4);
-  float* xc = s.alloc_n<float>((size_t)n * dpad_);      // centred training set
-  float* xproj = s.alloc_n<float>((size_t)n * dpad_);
-  float* recon = s.alloc_n<float>((size_t)n * dpad_);
-  float* xT = s.alloc_n<float>((size_t)d * ldn);
-  float* rT = s.alloc_n<float>((size_t)d * ldn);
-  float* xxr = s.alloc_n<float>((size_t)d * dpad_);
-  float* slice = s.alloc_n<float>((size_t)n * dsp);
-  float* cent = s.alloc_n<float>((size_t)Mo * 256 * dsp);  // per-subspace centroids, kept across rounds
-  float* pqc = s.alloc_n<float>((size_t)Mo * 256 * dso);
-  uint8_t* codes = s.alloc_n<uint8_t>((size_t)n * Mo);
-  if (!xc || !xproj || !recon || !xT || !rT || !xxr || !slice || !cent || !pqc || !codes) return nullptr;
-  auto ck = [](cudaError_t e) { return e == cudaSuccess; };
-  if (!ck(launch_center_rows(xs, dpad_, n, d, xc, dpad_, st)) || !ck(cudaMemsetAsync(xT, 0, (size_t)d * ldn * 4, st)) ||
-      !ck(cudaMemsetAsync(rT, 0, (size_t)d * ldn * 4, st)) || !ck(cudaMemsetAsync(recon, 0, (size_t)n * dpad_ * 4, st)) ||
-      !ck(launch_transpose(xc, dpad_, n, d, xT, ldn, st)))
-    return nullptr;
+  GB_ALLOC(mean, float, d, s);
+  GB_ALLOC(xc, float, (size_t)n * dpad, s);  // centred training set
+  GB_ALLOC(xproj, float, (size_t)n * dpad, s);
+  GB_ALLOC(recon, float, (size_t)n * dpad, s);
+  GB_ALLOC(xT, float, (size_t)d * ldn, s);
+  GB_ALLOC(rT, float, (size_t)d * ldn, s);
+  GB_ALLOC(xxr, float, (size_t)d * dpad, s);
+  GB_ALLOC(slice, float, (size_t)n * dsp, s);
+  GB_ALLOC(cent, float, (size_t)Mo * 256 * dsp, s);  // per-subspace centroids, kept across rounds
+  GB_ALLOC(pqc, float, (size_t)Mo * 256 * dso, s);
+  GB_ALLOC(codes, uint8_t, (size_t)n * Mo, s);
+  GB_CUDA(launch_center_rows(xs, dpad, n, d, mean, xc, dpad, st));
+  GB_CUDA(cudaMemsetAsync(xT, 0, (size_t)d * ldn * 4, st));
+  GB_CUDA(cudaMemsetAsync(rT, 0, (size_t)d * ldn * 4, st));
+  GB_CUDA(cudaMemsetAsync(recon, 0, (size_t)n * dpad * 4, st));
+  GB_CUDA(launch_transpose(xc, dpad, n, d, xT, ldn, st));
+  if (trace) {
+    GB_CUDA(trace_rows<float>(mean, d, 1, d, trace->mean, st));
+    if (trace->detail) GB_CUDA(trace_rows<float>(xc, dpad, n, d, trace->centred, st));
+  }
   // random orthonormal start: Gaussian matrix (mt19937, seed 1234), Gram-Schmidt on the rows
   std::vector<double> R((size_t)d * d);
   {
@@ -2594,33 +2583,49 @@ const float* IVFPQIndex::train_transform(const float* xt, int64_t n_in, Scratch&
       for (int j = 0; j < d; j++) R[(size_t)i * d + j] /= nrm;
     }
   }
-  std::vector<float> Rf((size_t)d * d), hx((size_t)d * dpad_);
+  if (trace) trace->r0 = R;
+  std::vector<float> Rf((size_t)d * d), hx((size_t)d * dpad);
   std::vector<double> a, U, V;
-  const int niter = 50, niter_pq_0 = 40, niter_pq = 4;
+  const int niter_pq_0 = 40, niter_pq = 4;
   for (int it = 0; it < niter; it++) {
     for (size_t i = 0; i < R.size(); i++) Rf[i] = (float)R[i];
-    if (!ck(upload_rows_padded(d_opq_, Rf.data(), d, d, dpad_, st)) || !ck(cudaMemsetAsync(xproj, 0, (size_t)n * dpad_ * 4, st)) ||
-        !ck(launch_dist_matrix(xc, dpad_, (int)n, d_opq_, dpad_, d, dpad_, kMetricIP, xproj, dpad_, st)))
-      return nullptr;
+    if (trace) trace->rf.insert(trace->rf.end(), Rf.begin(), Rf.end());
+    GB_CUDA(upload_rows_padded(d_opq, Rf.data(), d, d, dpad, st));
+    GB_CUDA(cudaMemsetAsync(xproj, 0, (size_t)n * dpad * 4, st));
+    GB_CUDA(launch_dist_matrix(xc, dpad, (int)n, d_opq, dpad, d, dpad, kMetricIP, xproj, dpad, st));
+    const bool detail = trace && trace->detail;
+    if (detail) GB_CUDA(trace_rows<float>(xproj, dpad, n, d, trace->proj, st));
     KMeansParams kp;
     kp.niter = it == 0 ? niter_pq_0 : niter_pq;
     kp.max_points_per_centroid = 1000;
     kp.hot_start = it > 0;
     for (int m = 0; m < Mo; m++) {
-      if (!ck(launch_slice_cols(xproj, dpad_, n, m * dso, dso, slice, dsp, st))) return nullptr;
-      if (kmeans_device(slice, dsp, n, dso, 256, kp, cent + (size_t)m * 256 * dsp, dsp, st, nullptr)) return nullptr;
-      if (!ck(cudaMemcpy2DAsync(pqc + (size_t)m * 256 * dso, (size_t)dso * 4, cent + (size_t)m * 256 * dsp, (size_t)dsp * 4,
-                                (size_t)dso * 4, 256, cudaMemcpyDeviceToDevice, st)))
-        return nullptr;
+      KMeansTrace* kt = nullptr;
+      if (detail) {
+        trace->km.emplace_back();
+        kt = &trace->km.back();
+      }
+      GB_CUDA(launch_slice_cols(xproj, dpad, n, m * dso, dso, slice, dsp, st));
+      if (kmeans_device(slice, dsp, n, dso, 256, kp, cent + (size_t)m * 256 * dsp, dsp, st, nullptr, kt)) return -1;
+      GB_CUDA(cudaMemcpy2DAsync(pqc + (size_t)m * 256 * dso, (size_t)dso * 4, cent + (size_t)m * 256 * dsp,
+                                (size_t)dsp * 4, (size_t)dso * 4, 256, cudaMemcpyDeviceToDevice, st));
     }
-    if (!ck(launch_pq_encode(xproj, dpad_, n, nullptr, 0, nullptr, pqc, Mo, dso, codes, st)) ||
-        !ck(launch_pq_decode(codes, n, pqc, Mo, dso, recon, dpad_, st)) || !ck(launch_transpose(recon, dpad_, n, d, rT, ldn, st)) ||
-        !ck(launch_dist_matrix(xT, ldn, d, rT, ldn, d, (int)ldn, kMetricIP, xxr, dpad_, st)) ||
-        !ck(cudaMemcpyAsync(hx.data(), xxr, (size_t)d * dpad_ * 4, cudaMemcpyDeviceToHost, st)) || !ck(cudaStreamSynchronize(st)))
-      return nullptr;
+    GB_CUDA(launch_pq_encode(xproj, dpad, n, nullptr, 0, nullptr, pqc, Mo, dso, codes, st));
+    GB_CUDA(launch_pq_decode(codes, n, pqc, Mo, dso, recon, dpad, st));
+    GB_CUDA(launch_transpose(recon, dpad, n, d, rT, ldn, st));
+    GB_CUDA(launch_dist_matrix(xT, ldn, d, rT, ldn, d, (int)ldn, kMetricIP, xxr, dpad, st));
+    GB_CUDA(cudaMemcpyAsync(hx.data(), xxr, (size_t)d * dpad * 4, cudaMemcpyDeviceToHost, st));
+    GB_CUDA(cudaStreamSynchronize(st));
+    if (detail) {
+      GB_CUDA(trace_rows<uint8_t>(codes, Mo, n, Mo, trace->codes, st));
+      GB_CUDA(trace_rows<float>(recon, dpad, n, d, trace->recon, st));
+    }
     a.assign((size_t)d * d, 0.0);  // X^T Y, d x d
     for (int i = 0; i < d; i++)
-      for (int j = 0; j < d; j++) a[(size_t)i * d + j] = hx[(size_t)i * dpad_ + j];
+      for (int j = 0; j < d; j++) a[(size_t)i * d + j] = hx[(size_t)i * dpad + j];
+    if (trace)
+      for (int i = 0; i < d; i++)
+        trace->xty.insert(trace->xty.end(), hx.begin() + (size_t)i * dpad, hx.begin() + (size_t)i * dpad + d);
     jacobi_svd(a, d, d, &U, &V);
     // R^T = U V^T  =>  R[i][j] = sum_k V[i][k] U[j][k]
     for (int i = 0; i < d; i++)
@@ -2629,12 +2634,12 @@ const float* IVFPQIndex::train_transform(const float* xt, int64_t n_in, Scratch&
         for (int kk = 0; kk < d; kk++) acc += V[(size_t)i * d + kk] * U[(size_t)j * d + kk];
         R[(size_t)i * d + j] = acc;
       }
+    if (trace) trace->r.insert(trace->r.end(), R.begin(), R.end());
   }
   for (size_t i = 0; i < R.size(); i++) Rf[i] = (float)R[i];
-  if (!ck(upload_rows_padded(d_opq_, Rf.data(), d, d, dpad_, st)) || !ck(cudaStreamSynchronize(st)))
-    return nullptr;
-  opq_trained_ = true;
-  return transform_dev(xt, n_in, s);
+  GB_CUDA(upload_rows_padded(d_opq, Rf.data(), d, d, dpad, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  return 0;
 }
 
 IVFPQIndex::~IVFPQIndex() {

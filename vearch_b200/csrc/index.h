@@ -541,6 +541,28 @@ struct KMeansTrace {
 int kmeans_device(const float* x, int64_t ldx, int64_t n, int d, int k, const KMeansParams& kp, float* centroids,
                   int64_t ldc, cudaStream_t st, std::vector<float>* obj, KMeansTrace* trace = nullptr);
 
+// What one OPQ training run did (gb_debug_opq_trace; DESIGN.md §5, OPQ bar).  n_s = the rows trained on
+// (min(n, 65536)), T = the rounds.  The bulk parts (centred rows, projections, codes, reconstructions, the
+// per-subspace k-means) are recorded only when detail is set.
+struct OpqTrace {
+  bool detail = true;            // record the bulk parts
+  std::vector<int32_t> sample;   // [n_s] the rows of the training set kept (empty: all of them, in order)
+  std::vector<float> mean;       // [d] the column means
+  std::vector<float> centred;    // [n_s][d]
+  std::vector<double> r0;        // [d][d] the random orthonormal start
+  std::vector<float> rf;         // [T][d][d] the fp32 rotation uploaded for round t
+  std::vector<float> proj;       // [T][n_s][d] the centred rows through it
+  std::vector<uint8_t> codes;    // [T][n_s][M] their PQ codes
+  std::vector<float> recon;      // [T][n_s][d] the decoded codes
+  std::vector<float> xty;        // [T][d][d] X^T Y as read back
+  std::vector<double> r;         // [T][d][d] the rotation the round's Procrustes solution gives
+  std::vector<KMeansTrace> km;   // [T][M] each subspace's k-means
+};
+// OPQ rotation (faiss OPQMatrix restated) learnt from the n rows of xt (stride dpad) in niter rounds; the final d x d
+// rotation is written to d_opq (row stride dpad).  trace: nullptr on every production path
+int opq_train_device(const float* xt, int64_t n, int d, int dpad, int M, int niter, float* d_opq, cudaStream_t st,
+                     OpqTrace* trace = nullptr);
+
 // What an IVF index's codec puts into gamma's index file (index_io.cu)
 struct GammaFileFormat {
   const char* file = nullptr;  // <dir>/<abs_name>/<file>; nullptr: no index file for this type

@@ -854,6 +854,57 @@ int gb_debug_kmeans_trace(int device, const float* x, int64_t n, int d, int k, i
   return 0;
 }
 
+int gb_debug_opq_trace(int device, const float* x, int64_t n, int d, int M, int niter, int detail, int64_t* sample,
+                       float* mean, float* centred, double* r0, float* rf, float* proj, uint8_t* codes, float* recon,
+                       float* xty, double* r, float* km_init, int32_t* km_labels, float* km_scores, float* km_mean,
+                       float* km_split, float* km_norm) {
+  if (M <= 0 || d % M != 0 || niter < 1 || n <= 0) {
+    set_last_error("opq trace: bad shape");
+    return -1;
+  }
+  if (cudaSetDevice(device) != cudaSuccess) {
+    set_last_error("no CUDA device");
+    return -1;
+  }
+  cudaStream_t st;
+  GB_CUDA(cudaStreamCreate(&st));
+  OpqTrace t;
+  t.detail = detail != 0;
+  int rc = -1;
+  {
+    Scratch s(st);
+    const int dpad = (d + 3) / 4 * 4;
+    float* dx = s.alloc_n<float>((size_t)n * dpad);
+    float* dr = s.alloc_n<float>((size_t)d * dpad);
+    if (dx && dr && upload_rows_padded(dx, x, n, d, dpad, st) == cudaSuccess)
+      rc = opq_train_device(dx, n, d, dpad, M, niter, dr, st, &t);
+  }
+  cudaStreamSynchronize(st);
+  cudaStreamDestroy(st);
+  if (rc) return rc;
+  const int64_t ns = t.sample.empty() ? n : (int64_t)t.sample.size();
+  for (int64_t i = 0; i < ns; i++) sample[i] = t.sample.empty() ? i : t.sample[i];
+  std::copy(t.mean.begin(), t.mean.end(), mean);
+  std::copy(t.r0.begin(), t.r0.end(), r0);
+  std::copy(t.rf.begin(), t.rf.end(), rf);
+  std::copy(t.xty.begin(), t.xty.end(), xty);
+  std::copy(t.r.begin(), t.r.end(), r);
+  if (!t.detail) return 0;
+  std::copy(t.centred.begin(), t.centred.end(), centred);
+  std::copy(t.proj.begin(), t.proj.end(), proj);
+  std::copy(t.codes.begin(), t.codes.end(), codes);
+  std::copy(t.recon.begin(), t.recon.end(), recon);
+  for (const KMeansTrace& k : t.km) {  // [round][subspace], each block in its own iteration count
+    km_init = std::copy(k.init.begin(), k.init.end(), km_init);
+    km_labels = std::copy(k.labels.begin(), k.labels.end(), km_labels);
+    km_scores = std::copy(k.scores.begin(), k.scores.end(), km_scores);
+    km_mean = std::copy(k.mean.begin(), k.mean.end(), km_mean);
+    km_split = std::copy(k.split.begin(), k.split.end(), km_split);
+    km_norm = std::copy(k.norm.begin(), k.norm.end(), km_norm);
+  }
+  return 0;
+}
+
 int gb_kmeans_update(int device, const float* x, int64_t n, int d, int k, const int64_t* assign, float* centroids) {
   if (cudaSetDevice(device) != cudaSuccess) {
     set_last_error("no CUDA device");

@@ -156,8 +156,10 @@ cudaError_t launch_ivf_listmajor_pipe(const float* xq, int64_t ldq, int d, const
                                       unsigned long long* tau_g, unsigned long long* out, cudaStream_t st);
 
 // ---- OPQ training helpers (kernels_build.cu) ---------------------------------------------------
-// out[i][j] = x[i][j] - mean_j (columns >= d zeroed up to ldo); mean computed on device
-cudaError_t launch_center_rows(const float* x, int64_t ldx, int64_t n, int d, float* out, int64_t ldo, cudaStream_t st);
+// mean[j] = the column means of x (fp64 sums, rounded once); out[i][j] = x[i][j] - mean_j (columns >= d zeroed up to
+// ldo).  mean: d floats of device memory
+cudaError_t launch_center_rows(const float* x, int64_t ldx, int64_t n, int d, float* mean, float* out, int64_t ldo,
+                               cudaStream_t st);
 // out[j][i] = x[i][j]  (n x d -> d x n, row stride ldo >= n)
 cudaError_t launch_transpose(const float* x, int64_t ldx, int64_t n, int d, float* out, int64_t ldo, cudaStream_t st);
 // recon[i][m * dsub + j] = pq[m][codes[i][m]][j]

@@ -180,16 +180,13 @@ __global__ void pq_decode_kernel(const uint8_t* __restrict__ codes, int64_t n, c
 
 }  // namespace
 
-cudaError_t launch_center_rows(const float* x, int64_t ldx, int64_t n, int d, float* out, int64_t ldo, cudaStream_t st) {
+cudaError_t launch_center_rows(const float* x, int64_t ldx, int64_t n, int d, float* mean, float* out, int64_t ldo,
+                               cudaStream_t st) {
   if (n <= 0) return cudaSuccess;
-  float* mean = nullptr;
-  cudaError_t e = cudaMallocAsync(&mean, sizeof(float) * d, st);
-  if (e != cudaSuccess) return e;
   col_mean_kernel<<<d, 256, 0, st>>>(x, ldx, n, mean);
   note_launch();
   center_rows_kernel<<<blocks_for(n * ldo, 256), 256, 0, st>>>(x, ldx, n, d, mean, out, ldo);
   note_launch();
-  cudaFreeAsync(mean, st);
   return cudaGetLastError();
 }
 

@@ -692,6 +692,55 @@ def debug_kmeans_trace(x, k, niter=25, seed=1234, spherical=False, l2_assign=Fal
     return out
 
 
+OPQ_MAX_TRAIN = 65536  # the rows OPQ trains on at most (faiss OPQMatrix max_train_points)
+
+
+def opq_kmeans_iters(t):
+    """k-means iterations of each subspace in OPQ round t"""
+    return 40 if t == 0 else 4
+
+
+def debug_opq_trace(x, M, niter=3, detail=True, device=0):
+    """One OPQ training run (the rotation "opq": {"nsubvector": M} learns), niter rounds, traced: a dict of numpy
+    arrays.  sample [n_s]: the rows trained on; mean [d]; r0 [d, d] float64: the random orthonormal start; rf
+    [niter, d, d]: the float32 rotation of each round; xty [niter, d, d]: X^T Y as the device formed it; r [niter, d, d]
+    float64: the rotation each round solves for.  With detail: centred [n_s, d]; proj, recon [niter, n_s, d]; codes
+    [niter, n_s, M]; km [niter][M]: each subspace's k-means trace, as debug_kmeans_trace gives it."""
+    x = _f32(x)
+    n, d = x.shape
+    ns, ds, T = min(n, OPQ_MAX_TRAIN), d // M, niter
+    out = {"sample": np.empty(ns, np.int64), "mean": np.empty(d, np.float32), "r0": np.empty((d, d), np.float64),
+           "rf": np.empty((T, d, d), np.float32), "xty": np.empty((T, d, d), np.float32),
+           "r": np.empty((T, d, d), np.float64)}
+    its = [opq_kmeans_iters(t) for t in range(T)]
+    tot = sum(its) * M
+    bulk = dict(centred=np.empty((ns, d), np.float32), proj=np.empty((T, ns, d), np.float32),
+                codes=np.empty((T, ns, M), np.uint8), recon=np.empty((T, ns, d), np.float32),
+                init=np.empty((T * M, 256, ds), np.float32), labels=np.empty((tot, ns), np.int32),
+                scores=np.empty((tot, ns), np.float32), kmean=np.empty((tot, 256, ds), np.float32),
+                split=np.empty((tot, 256, ds), np.float32), norm=np.empty((tot, 256, ds), np.float32)) if detail else {}
+    b = lambda key: _ptr(bulk.get(key))  # noqa: E731
+    _check(_lib.lib().gb_debug_opq_trace(device, _ptr(x), n, d, M, niter, int(detail), _ptr(out["sample"]),
+                                         _ptr(out["mean"]), b("centred"), _ptr(out["r0"]), _ptr(out["rf"]), b("proj"),
+                                         b("codes"), b("recon"), _ptr(out["xty"]), _ptr(out["r"]), b("init"),
+                                         b("labels"), b("scores"), b("kmean"), b("split"), b("norm")),
+           "debug_opq_trace")
+    if detail:
+        for key in ("centred", "proj", "codes", "recon"):
+            out[key] = bulk[key]
+        out["km"], at = [], 0
+        for t in range(T):
+            row = []
+            for m in range(M):
+                sl = slice(at, at + its[t])
+                row.append({"sample": np.arange(ns, dtype=np.int64), "init": bulk["init"][t * M + m],
+                            "labels": bulk["labels"][sl], "scores": bulk["scores"][sl], "mean": bulk["kmean"][sl],
+                            "split": bulk["split"][sl], "norm": bulk["norm"][sl]})
+                at += its[t]
+            out["km"].append(row)
+    return out
+
+
 def kmeans_update(x, k, assign, device=0):
     x = _f32(x)
     assign = np.ascontiguousarray(assign, np.int64)
