@@ -150,6 +150,14 @@ int gb_index_tombstone(gb_index *index, int list, int pos);
 int gb_index_delete(gb_index *index, const int64_t *vids, int64_t n);
 int gb_index_purge(gb_index *index, float threshold, const uint8_t *del_bitmap, int64_t bitmap_bytes, int64_t *dropped);
 int gb_index_dead_counts(gb_index *index, int *out);
+/* Test hook: the list entries of vid as (list << 32 | position), out[2], ~0 for none.  An index with SOAR spilling
+ * (model parameter "soar_lambda" > 0) holds every indexed vid in two lists; a fresh build puts its primary entry in
+ * out[0] and its spilled one in out[1], a loaded index either way round.  An unspilled index leaves out[1] = ~0. */
+int gb_index_vid_slots(gb_index *index, int64_t vid, uint64_t *out);
+/* Test hook: what admission under SetMemoryLimitConfig charges for storing rows up to n_total -- *store_bytes, the raw
+ * store's growth, making room for *rows rows, and *index_bytes, the list entries those rows will take once indexed (two
+ * per row with SOAR spilling). */
+int gb_index_memory_charge(gb_index *index, int64_t n_total, int64_t *store_bytes, int64_t *rows, int64_t *index_bytes);
 /* IndexModel::Dump / Load (index/index_model.h) in gamma's own file formats -- "IvFl" / "IwPQ" header,
  * IndexFlat quantizer, "ilar" inverted lists (index/impl/gamma_index_ivfflat.cc:807-892,
  * gamma_index_ivfpq.cc:1019-1116, index/index_io.cc:108-194): <dir>/<abs_name>/{ivfflat,ivfpq}.index.

@@ -94,6 +94,8 @@ def _declare(l):
     l.gb_index_delete.argtypes = [vp, vp, i64]
     l.gb_index_purge.argtypes = [vp, f32, vp, i64, vp]
     l.gb_index_dead_counts.argtypes = [vp, vp]
+    l.gb_index_vid_slots.argtypes = [vp, i64, vp]
+    l.gb_index_memory_charge.argtypes = [vp, i64, vp, vp, vp]
     l.gb_index_dump.argtypes = [vp, cstr, cstr]
     l.gb_index_compact.argtypes = [vp]
     l.gb_index_mirror_builds.argtypes = [vp]

@@ -624,7 +624,7 @@ int IvfLists::tombstone(int list, int pos, cudaStream_t st) {
   return 0;
 }
 
-int IvfLists::purge(const std::vector<int>& lists, const uint32_t* d_del_bits, cudaStream_t st, Purged* out) {
+int IvfLists::purge(const std::vector<int>& lists, const uint32_t* d_del_bits, cudaStream_t st, Purged* out, int copies) {
   *out = Purged();
   std::vector<int> sel, chunk0(1, 0);
   std::vector<PurgeChunk> chunks;
@@ -681,15 +681,15 @@ int IvfLists::purge(const std::vector<int>& lists, const uint32_t* d_del_bits, c
   const int align = (int)(bits & (~bits + 1));  // lowest set bit: at most 16
   GB_ALLOC(d_nd, void*, nsel, s);
   GB_ALLOC(d_ni, int64_t*, nsel, s);
-  GB_ALLOC(d_newpos, unsigned long long, vid_span, s);
+  GB_ALLOC(d_newpos, unsigned long long, vid_span * copies, s);
   GB_CUDA(cudaMemcpyAsync(d_nd, nd.data(), sizeof(void*) * nsel, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemcpyAsync(d_ni, ni.data(), sizeof(int64_t*) * nsel, cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemsetAsync(d_newpos, 0xFF, (size_t)vid_span * 8, st));
+  GB_CUDA(cudaMemsetAsync(d_newpos, 0xFF, (size_t)vid_span * copies * 8, st));
   GB_CUDA(launch_purge_scatter(dir, d_sel, d_chunks, nchunks, d_del_bits, d_chunk_off, code_bytes_, align, d_nd, d_ni, d_newpos,
-                               vid_min, st));
+                               vid_min, st, copies));
   out->vid_min = vid_min;
-  out->newpos.resize((size_t)vid_span);
-  GB_CUDA(cudaMemcpyAsync(out->newpos.data(), d_newpos, (size_t)vid_span * 8, cudaMemcpyDeviceToHost, st));
+  out->newpos.resize((size_t)vid_span * copies);
+  GB_CUDA(cudaMemcpyAsync(out->newpos.data(), d_newpos, (size_t)vid_span * copies * 8, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));  // the scatter is done (and has not failed) before anything is published
   for (int i = 0; i < nsel; i++) {
     const int l = sel[i];
@@ -849,7 +849,7 @@ void Index::memory_charges(int64_t n_total, std::vector<mem::Charge>* out) {
   charge_index_rows(rows, out);
 }
 void IvfIndex::charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) {
-  out->push_back({device_, rows * (code_bytes() + 8)});
+  out->push_back({device_, rows * (spilled() ? 2 : 1) * (code_bytes() + 8)});  // spilled: two entries per row
 }
 void IVFFlatIndex::charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) {
   IvfIndex::charge_index_rows(rows, out);
@@ -1712,6 +1712,11 @@ int IvfIndex::assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* out, S
   return 0;
 }
 
+int IvfIndex::spill_dev(const float* x, int64_t n, const int32_t* primary, int32_t* out, Scratch& s) {
+  GB_CUDA(launch_soar_spill(x, dpad_, n, d_, d_centroids_, dpad_, nlist_, primary, (float)mp_.soar_lambda, out, s.stream()));
+  return 0;
+}
+
 int IVFFlatIndex::append_batch(const void* xv, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
                                const std::vector<int>& add, Scratch& s) {
   const float* x = static_cast<const float*>(xv);
@@ -1735,12 +1740,19 @@ int IvfIndex::index_batch(const void* x, int64_t n, int64_t vid0, const uint8_t*
   Scratch s(st);
   GB_ALLOC(d_assign, int32_t, n, s);
   if (assign_batch(x, n, &x, d_assign, s)) return -1;
-  std::vector<int32_t> h_list(n), h_pos(n);
+  const bool spill = spilled();
+  std::vector<int32_t> h_list(n), h_pos(n), h_spill(spill ? n : 0), h_spos(spill ? n : 0);
+  if (spill) {  // the second list of every row, from the same rows and centroids as its primary one
+    GB_ALLOC(d_sp, int32_t, n, s);
+    if (spill_dev(static_cast<const float*>(x), n, d_assign, d_sp, s)) return -1;
+    GB_CUDA(cudaMemcpyAsync(h_spill.data(), d_sp, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+  }
   GB_CUDA(cudaMemcpyAsync(h_list.data(), d_assign, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
   std::vector<int> add(nlist_, 0);
   const std::vector<int>& lens = lists_->lens();
   if ((int64_t)vid2pos_.size() < vid0 + n) vid2pos_.resize(vid0 + n, ~(uint64_t)0);
+  if (spill && (int64_t)vid2pos2_.size() < vid0 + n) vid2pos2_.resize(vid0 + n, ~(uint64_t)0);
   for (int64_t i = 0; i < n; i++) {
     int64_t vid = vid0 + i, gvid = global_vid(vid);
     int l = h_list[i];
@@ -1754,15 +1766,44 @@ int IvfIndex::index_batch(const void* x, int64_t n, int64_t vid0, const uint8_t*
     h_pos[i] = lens[l] + add[l]++;  // insertion (vid) order inside the list
     vid2pos_[vid] = ((uint64_t)l << 32) | (uint32_t)h_pos[i];
   }
+  // the spilled entries after the batch's primary ones, in vid order.  A row without a spilled list (|r| = 0, values
+  // not finite, no primary list) takes list gvid % nlist as an unassigned row does, or the next one when that is its
+  // primary list
+  for (int64_t i = 0; spill && i < n; i++) {
+    const int64_t vid = vid0 + i, gvid = global_vid(vid);
+    const int l = h_list[i];
+    int sl = h_spill[i];
+    if (l < 0) {
+      h_spill[i] = -1;
+      h_spos[i] = 0;
+      continue;
+    }
+    if (sl < 0 || sl >= nlist_ || sl == l) {
+      sl = (int)(gvid % nlist_);
+      if (sl == l) sl = (int)((gvid + 1) % nlist_);
+    }
+    h_spill[i] = sl;
+    h_spos[i] = lens[sl] + add[sl]++;
+    vid2pos2_[vid] = ((uint64_t)sl << 32) | (uint32_t)h_spos[i];
+  }
   GB_ALLOC(d_list, int32_t, n, s);
   GB_ALLOC(d_pos, int32_t, n, s);
   GB_CUDA(cudaMemcpyAsync(d_list, h_list.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemcpyAsync(d_pos, h_pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  int32_t *d_slist = nullptr, *d_spos = nullptr;
+  if (spill) {
+    d_slist = s.alloc_n<int32_t>(n);
+    d_spos = s.alloc_n<int32_t>(n);
+    if (!d_slist || !d_spos) return -1;
+    GB_CUDA(cudaMemcpyAsync(d_slist, h_spill.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    GB_CUDA(cudaMemcpyAsync(d_spos, h_spos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  }
   std::unique_lock<std::shared_mutex> lk(mu_);
   drain_searches();  // kernels of earlier searches read lengths and base pointers at run time
   if (lists_->reserve(add, st)) return -1;
   // data first, the new lengths last (realtime_mem_data.cc:292-293)
   if (append_batch(x, n, vid0, d_list, d_pos, add, s)) return -1;
+  if (spill && append_batch(x, n, vid0, d_slist, d_spos, add, s)) return -1;  // codes against the spilled centroids
   if (lists_->commit(add, st)) return -1;
   if (lists_changed(st)) return -1;
   GB_CUDA(cudaStreamSynchronize(st));
@@ -1809,6 +1850,7 @@ int IvfIndex::reset_index() {
   cudaDeviceSynchronize();  // kernels of earlier device-resident searches may still read the lists
   lists_.reset();
   vid2pos_.clear();
+  vid2pos2_.clear();
   del_counted_.clear();
   reset_codec();
   indexed_count_ = 0;
@@ -1823,6 +1865,7 @@ void IvfIndex::clear_lists() {
   drain_searches();
   if (lists_) lists_.reset(new IvfLists(nlist_, code_bytes()));
   vid2pos_.clear();
+  vid2pos2_.clear();
   del_counted_.clear();
   indexed_count_ = 0;
   if (lists_) lists_changed(build_stream_);
@@ -1888,6 +1931,20 @@ int IvfIndex::update_vector(int64_t vid, const void* x) {
   return reindex_vector(vid, x_dev);
 }
 int IvfIndex::reindex_vector(int64_t vid, const void* x_dev) {
+  if (spilled()) {  // both entries tombstoned, then the row goes to its primary and its spilled list again
+    std::unique_lock<std::shared_mutex> lk(mu_);
+    const bool counted = vid < (int64_t)del_counted_.size() && del_counted_[vid];
+    if (counted) del_counted_[vid] = false;
+    for (std::vector<uint64_t>* slots : {&vid2pos_, &vid2pos2_}) {
+      if (vid >= (int64_t)slots->size() || (*slots)[vid] == ~(uint64_t)0) continue;
+      const uint64_t at = (*slots)[vid];
+      if (counted) lists_->add_dead((int)(at >> 32), -1);  // counted as deleted: the tombstone counts it instead
+      if (lists_->tombstone((int)(at >> 32), (int)(uint32_t)at, build_stream_)) return -1;
+      (*slots)[vid] = ~(uint64_t)0;
+    }
+    lk.unlock();
+    return index_batch(x_dev, 1, vid, nullptr);
+  }
   if (vid < (int64_t)vid2pos_.size() && vid2pos_[vid] != ~(uint64_t)0) {
     std::unique_lock<std::shared_mutex> lk(mu_);
     const int l = (int)(vid2pos_[vid] >> 32);
@@ -1900,11 +1957,29 @@ int IvfIndex::reindex_vector(int64_t vid, const void* x_dev) {
   return index_batch(x_dev, 1, vid, nullptr);
 }
 
+int IvfIndex::vid_slots(int64_t vid, uint64_t* out) {
+  std::lock_guard<std::mutex> bg(build_mu_);
+  out[0] = vid >= 0 && vid < (int64_t)vid2pos_.size() ? vid2pos_[vid] : ~(uint64_t)0;
+  out[1] = vid >= 0 && vid < (int64_t)vid2pos2_.size() ? vid2pos2_[vid] : ~(uint64_t)0;
+  return 0;
+}
+
 int IvfIndex::delete_vectors(const int64_t* vids, int64_t n) {
   std::lock_guard<std::mutex> bg(build_mu_);
   if (!lists_) return 0;
   for (int64_t i = 0; i < n; i++) {
     const int64_t vid = vids[i];
+    if (spilled()) {  // a dead entry in each list that holds one
+      const uint64_t a = vid >= 0 && vid < (int64_t)vid2pos_.size() ? vid2pos_[vid] : ~(uint64_t)0;
+      const uint64_t b = vid >= 0 && vid < (int64_t)vid2pos2_.size() ? vid2pos2_[vid] : ~(uint64_t)0;
+      if (a == ~(uint64_t)0 && b == ~(uint64_t)0) continue;
+      if ((int64_t)del_counted_.size() <= vid) del_counted_.resize(std::max(vid2pos_.size(), vid2pos2_.size()), false);
+      if (del_counted_[vid]) continue;
+      del_counted_[vid] = true;
+      if (a != ~(uint64_t)0) lists_->add_dead((int)(a >> 32), 1);
+      if (b != ~(uint64_t)0) lists_->add_dead((int)(b >> 32), 1);
+      continue;
+    }
     if (vid < 0 || vid >= (int64_t)vid2pos_.size() || vid2pos_[vid] == ~(uint64_t)0) continue;
     if (del_counted_.size() < vid2pos_.size()) del_counted_.resize(vid2pos_.size(), false);
     if (del_counted_[vid]) continue;
@@ -1952,8 +2027,40 @@ int IvfIndex::purge_locked(const std::vector<int>& sel, const uint32_t* d_del_bi
   for (int l : sel) purged[l] = 1;
   drain_searches();  // kernels of earlier searches read lengths and base pointers at run time
   IvfLists::Purged pg;
-  if (lists_->purge(sel, d_del_bits, st, &pg)) return -1;
+  if (lists_->purge(sel, d_del_bits, st, &pg, spilled() ? 2 : 1)) return -1;
   if (pg.dropped == 0) return 0;
+  if (spilled()) {
+    // both slots of every vid with an entry in a purged list: the new entry in the same list (a vid's two entries are in
+    // two lists), ~0 if it was dropped
+    const int64_t span = (int64_t)pg.newpos.size() / 2;
+    const int64_t top = std::min<int64_t>((int64_t)vid2pos_.size(), pg.vid_min + span);
+    for (int64_t vid = pg.vid_min; vid < top; vid++) {
+      const uint64_t* np = &pg.newpos[2 * (vid - pg.vid_min)];
+      bool moved = false, left = false;
+      for (std::vector<uint64_t>* slots : {&vid2pos_, &vid2pos2_}) {
+        if (vid >= (int64_t)slots->size()) continue;
+        uint64_t& at = (*slots)[vid];
+        if (at == ~(uint64_t)0) continue;
+        if (!purged[at >> 32]) {
+          left = true;
+          continue;
+        }
+        const uint64_t now = (np[0] >> 32) == (at >> 32) ? np[0] : (np[1] >> 32) == (at >> 32) ? np[1] : ~(uint64_t)0;
+        at = now;
+        moved = true;
+        if (now != ~(uint64_t)0) {
+          left = true;
+          if (vid < (int64_t)del_counted_.size() && del_counted_[vid]) lists_->add_dead((int)(now >> 32), 1);
+        }
+      }
+      if (moved && !left && vid < (int64_t)del_counted_.size()) del_counted_[vid] = false;
+    }
+    if (lists_changed(st)) return -1;
+    GB_CUDA(cudaStreamSynchronize(st));
+    if (dropped) *dropped = pg.dropped;
+    if (lists_->compact_due() && compact_locked()) return -1;
+    return 0;
+  }
   // vid_bucket_no_pos_ of every vid that was in a purged list, from the table the scatter wrote
   const int64_t hi = std::min<int64_t>((int64_t)vid2pos_.size(), pg.vid_min + (int64_t)pg.newpos.size());
   for (int64_t vid = pg.vid_min; vid < hi; vid++) {
@@ -2894,9 +3001,13 @@ int IvfIndex::scan_query_major_dev(const char* kernel, const SearchContext& ctx,
   // rerank", gamma_index_ivfpq_gpu.cc:565): recall_num is checked at the search entry and changes nothing else.
   const bool rerank = ctx.params.recall_num > 0 && !gpu_contract_;
   const int kk = rerank ? std::max(k, ctx.params.recall_num) : k;
-  if (kk > max_kk) {
-    set_last_error(type_ + ": recall_num / topn [" + std::to_string(kk) + "] above " + std::to_string(max_kk) +
-                   " is not supported by this engine at " + limit_at);
+  // Spilled lists (DESIGN.md §8, SOAR spilling): a vid may hold two entries of the probed lists, so the scan selects 2 k' keys and
+  // launch_dedupe_keys keeps each vid's first; the k' vids of best best-copy keys all lie among those 2 k'
+  const bool spill = spilled();
+  const int max_sel = spill ? std::min(max_kk, kDedupeMaxKeys) / 2 : max_kk;
+  if (kk > max_sel) {
+    set_last_error(type_ + ": recall_num / topn [" + std::to_string(kk) + "] above " + std::to_string(max_sel) +
+                   " is not supported by this engine at " + limit_at + (spill ? " with spilled lists" : ""));
     return -1;
   }
   unsigned long long* keys = out_keys;
@@ -2904,26 +3015,36 @@ int IvfIndex::scan_query_major_dev(const char* kernel, const SearchContext& ctx,
     keys = s.alloc_n<unsigned long long>((size_t)nq * kk);
     if (!keys) return -1;
   }
+  const int depth = spill ? 2 * kk : kk;
+  unsigned long long* sel = keys;
+  if (spill) {
+    sel = s.alloc_n<unsigned long long>((size_t)nq * depth);
+    if (!sel) return -1;
+  }
   // the exact re-rank takes its candidates in any order; without it the keys are the result and must be sorted
-  const int rc = prepare(kk, keys, !rerank);
+  const int rc = prepare(depth, sel, !rerank || spill);
   if (rc < 0) return -1;
   if (rc == 1) {
     const int nsm = sm_count(device_);
     const int pg = (int)std::min<int64_t>(32, std::max<int64_t>(1, (int64_t)nprobe * nq / ((int64_t)nsm * 32)));
     const int ngroups = (nprobe + pg - 1) / pg;
-    GB_ALLOC(partial, unsigned long long, (size_t)nq * ngroups * kk, s);
+    GB_ALLOC(partial, unsigned long long, (size_t)nq * ngroups * depth, s);
     last_scan_kernel_ = kernel;
     snprintf(last_scan_info_, sizeof(last_scan_info_), "{\"probes_per_cta\": %d}", pg);
     scan_timer_begin(st);
     stage_begin(kernel, st);
-    GB_CUDA(launch(kk, pg, partial));
+    GB_CUDA(launch(depth, pg, partial));
     stage_end(st);
     scan_timer_end(st);
     if (ngroups > 1) {
-      GB_CUDA(launch_select_keys(partial, (int64_t)ngroups * kk, nq, ngroups * kk, kk, keys, kk, st));
+      GB_CUDA(launch_select_keys(partial, (int64_t)ngroups * depth, nq, ngroups * depth, depth, sel, depth, st));
     } else {
-      GB_CUDA(cudaMemcpyAsync(keys, partial, (size_t)nq * kk * 8, cudaMemcpyDeviceToDevice, st));
+      GB_CUDA(cudaMemcpyAsync(sel, partial, (size_t)nq * depth * 8, cudaMemcpyDeviceToDevice, st));
     }
+  }
+  if (spill) {
+    StageScope stage(this, "dedupe_keys_kernel", st);
+    GB_CUDA(launch_dedupe_keys(sel, depth, nq, depth, kk, keys, kk, st));
   }
   if (rerank && store_->has_shadow()) {
     int* surv = rr_stats_ ? s.alloc_n<int>((size_t)nq) : nullptr;
@@ -3512,6 +3633,12 @@ Index* create_index(const std::string& type, int d, const ModelParams& mp, int d
     return nullptr;
   }
   if (type == "FLAT") return new FlatIndex(d, mp, device, seg_shift);
+  // SOAR (parsed for IVFPQFastScan, IVFRABITQ and VEARCH only): one list leaves no second list to spill into
+  if (mp.soar_lambda > 0 && mp.ncentroids < 2) {
+    set_last_error("soar_lambda needs ncentroids >= 2 (a row spills into a list other than its own), ncentroids = " +
+                   std::to_string(mp.ncentroids));
+    return nullptr;
+  }
   if (type == "IVFFLAT" || type == "GPU_IVFFLAT") {
     // small batches scan query-major (ivfflat_scan_kernel), whose ring, query and k = 4096 queue must fit one CTA's
     // shared memory; refused here rather than as a CUDA error at every such search

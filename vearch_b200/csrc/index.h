@@ -187,12 +187,14 @@ class IvfLists {
   // the device (RealTimeMemData::CompactBucket, realtime_mem_data.cc:94-146).  Survivors keep their order and move to
   // fresh regions, as copy-on-grow does, so a kernel still reading an old region reads valid memory; pointers are
   // published before lengths.  The caller holds the index lock exclusively with earlier searches drained.
-  // newpos[vid - vid_min] = (list << 32 | pos) of every surviving vid, ~0 for vids no longer in these lists.
+  // newpos[vid - vid_min] = (list << 32 | pos) of every surviving vid, ~0 for vids no longer in these lists.  copies = 2
+  // (spilled lists: a vid may have two live entries): two slots per vid, newpos[2 (vid - vid_min) + {0, 1}], in no
+  // particular order; the list part tells the entries apart.
   struct Purged {
     int64_t dropped = 0, vid_min = 0;
     std::vector<uint64_t> newpos;
   };
-  int purge(const std::vector<int>& lists, const uint32_t* d_del_bits, cudaStream_t st, Purged* out);
+  int purge(const std::vector<int>& lists, const uint32_t* d_del_bits, cudaStream_t st, Purged* out, int copies = 1);
 
  private:
   void* slab_alloc(size_t bytes);
@@ -237,6 +239,9 @@ struct ModelParams {  // index/impl/gamma_index_ivfpq.h:1031-1257, gamma_index_i
   std::string metric_unknown;
   double ns_threshold = 0.2;  // VEARCH noise-shaping threshold (VearchModelParams); NaN: no noise shaping
   bool reordering = false;    // VEARCH exact re-rank of the k' best codes
+  // SOAR spilling (IVFPQFastScan, IVFRABITQ, VEARCH; DESIGN.md §8, SOAR spilling): > 0 stores every row in a second, spilled list
+  // chosen with this lambda; 0 = off.  The other types ignore it.
+  double soar_lambda = 0;
 };
 
 // gamma's two GPU index types (index/impl/gpu/): GPU_IVFPQ is an IVFPQIndex and GPU_IVFFLAT an IVFFlatIndex, created
@@ -607,6 +612,10 @@ class IvfIndex : public Index {
   int reset_index() override;
   int64_t index_mem_bytes() const override;
   int nlist() const { return nlist_; }
+  // SOAR spilling on (ModelParams::soar_lambda > 0): every indexed row has a second entry in its spilled list
+  bool spilled() const { return mp_.soar_lambda > 0; }
+  // test hook: vid's list entries as (list << 32 | pos), ~0 = none; a fresh build puts the primary entry first
+  int vid_slots(int64_t vid, uint64_t* out);
   virtual int code_bytes() const = 0;  // bytes per list entry
   void charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) override;  // a list entry and its id
   // parity hooks: exchange index state with the oracle
@@ -695,6 +704,8 @@ class IvfIndex : public Index {
   cudaError_t group_pairs_by_list(const int32_t* probe_ids, int64_t npairs, int nseg, int group, const LmGrouping& g,
                                   cudaStream_t st);
   int assign_dev(const float* x, int64_t ldx, int64_t n, int32_t* assign_dev_out, Scratch& s);
+  // each row's spilled list (launch_soar_spill) given its primary list, -1 for the fallback rule of index_batch
+  int spill_dev(const float* x, int64_t n, const int32_t* primary, int32_t* out, Scratch& s);
   // the rows of a batch as the codec takes them (*xc) and each row's nearest list (out): fp32 rows (stride dpad) through
   // transform_dev and assign_dev; BINARYIVF: the packed rows as they are, by Hamming distance
   virtual int assign_batch(const void* x, int64_t n, const void** xc, int32_t* out, Scratch& s);
@@ -732,7 +743,9 @@ class IvfIndex : public Index {
   virtual int centroids_changed(cudaStream_t st) { (void)st; return 0; }
   std::unique_ptr<IvfLists> lists_;
   std::vector<uint64_t> vid2pos_;  // vid -> (list << 32 | pos), ~0 = not in a list (vid_bucket_no_pos_)
-  std::vector<bool> del_counted_;  // vid's entry is counted dead by delete_vectors (so it is counted once)
+  // spilled: vid's other entry, as vid2pos_ (~0 = none).  The two slots are equal: neither is known as the primary one.
+  std::vector<uint64_t> vid2pos2_;
+  std::vector<bool> del_counted_;  // vid's entries are counted dead by delete_vectors (so they are counted once)
 };
 
 // GammaIVFFlatIndex (index/impl/gamma_index_ivfflat.{h,cc}): the lists hold the raw fp32 rows.  type: "IVFFLAT", or

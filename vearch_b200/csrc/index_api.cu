@@ -2,6 +2,7 @@
 #include <strings.h>
 
 #include <algorithm>
+#include <cmath>
 #include <vector>
 
 #include "../../include/gamma_b200_index.h"
@@ -23,6 +24,21 @@ namespace gb {
 // gamma_index_ivfpq.h:1031-1257)
 // VearchModelParams::Parse (gamma_index_vearch.cc:40-126): ncentroids and nsubvector are required, ns_threshold < 0 means
 // no noise shaping, metric_type defaults to InnerProduct; thread_num has no effect here
+// "soar_lambda" of the types whose lists may spill (IVFPQFastScan, IVFRABITQ, VEARCH): absent or 0 = off, > 0 and finite =
+// every row also goes to a SOAR-chosen second list (DESIGN.md §8, SOAR spilling); anything else is refused
+static bool parse_soar_lambda(const JsonValue& jv, ModelParams* mp, std::string* err) {
+  const JsonValue* v = jv.get("soar_lambda");
+  if (!v) return true;
+  if (v->type != JsonValue::Number || !(v->num >= 0) || !std::isfinite(v->num)) {
+    char buf[64];
+    snprintf(buf, sizeof(buf), "%g", v->type == JsonValue::Number ? v->num : std::nan(""));
+    *err = std::string("invalid soar_lambda = ") + (v->type == JsonValue::Number ? buf : "(not a number)");
+    return false;
+  }
+  mp->soar_lambda = v->num;
+  return true;
+}
+
 static bool parse_vearch_params(const std::string& text, ModelParams* mp, std::string* err) {
   JsonValue jv;
   if (!JsonParser::parse(text, &jv) || jv.type != JsonValue::Object) {
@@ -64,7 +80,7 @@ static bool parse_vearch_params(const std::string& text, ModelParams* mp, std::s
   if (jv.get_int("training_threshold", &v) && v > 0) mp->training_threshold = v;
   std::string stt;
   if (jv.get_string("store_type", &stt)) mp->host_store = !strcasecmp("RocksDB", stt.c_str());
-  return true;
+  return parse_soar_lambda(jv, mp, err);
 }
 
 bool parse_model_params(const std::string& text, const std::string& type, ModelParams* mp, std::string* err) {
@@ -169,6 +185,7 @@ bool parse_model_params(const std::string& text, const std::string& type, ModelP
     }
     mp->metric = !strcasecmp("L2", mt.c_str()) ? kMetricL2 : kMetricIP;
   }
+  if (type == "IVFPQFastScan" || type == "IVFRABITQ") return parse_soar_lambda(jv, mp, err);
   return true;
 }
 
@@ -652,6 +669,23 @@ int gb_index_purge(gb_index* index, float threshold, const uint8_t* del_bitmap, 
     return -1;
   }
   return index->impl->purge_lists(threshold, del_bitmap, bitmap_bytes, dropped);
+}
+int gb_index_memory_charge(gb_index* index, int64_t n_total, int64_t* store_bytes, int64_t* rows, int64_t* index_bytes) {
+  IDX_OR_FAIL(index);
+  if (!store_bytes || !rows || !index_bytes) return -1;
+  // what admission under the memory limit charges (Index::memory_charges): the store's growth, and the index entries of
+  // the rows it makes room for
+  *store_bytes = index->impl->store().growth_bytes(n_total, rows);
+  std::vector<mem::Charge> c;
+  index->impl->charge_index_rows(*rows, &c);
+  *index_bytes = 0;
+  for (const mem::Charge& e : c) *index_bytes += e.bytes;
+  return 0;
+}
+int gb_index_vid_slots(gb_index* index, int64_t vid, uint64_t* out) {
+  IVF_OR_FAIL(ivf, index);
+  if (!out) return -1;
+  return ivf->vid_slots(vid, out);
 }
 int gb_index_dead_counts(gb_index* index, int* out) {
   if (!out) return -1;

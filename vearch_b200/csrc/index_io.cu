@@ -30,6 +30,9 @@
 //   "GbVR" gb_vearch.index    : u64 code_size, i32 nsubvector, i32 nblocks, f64 ns_threshold (NaN: none), u8 reordering,
 //                               u64 16*d, fp32 block codebooks [16 d] (each block's centres in their trained order)
 //   "GbBI" gb_binaryivf.index : u64 code_size (d / 8), u64 nlist*code_size, packed centroids [nlist][d / 8]
+// An index with SOAR spilling (soar_lambda > 0, DESIGN.md §8) writes the same file under the variant fourcc "GsFS" /
+// "GsRQ" / "GsVR" (for "GbFS" / "GbRQ" / "GbVR") with f64 soar_lambda right after the codec block; its lists hold both
+// entries of every spilled row, two live entries per vid in two different lists.
 // d is in bits for BINARYIVF, whose coarse-quantiser block holds the float k-means centroids (metric L2).  A file is
 // refused unless d, nlist, metric and every codec parameter match the table; the index is then left untrained.
 #include <errno.h>
@@ -105,13 +108,16 @@ int fail(const std::string& msg) {
 // IVF-Flat rows are padded to a multiple of 4 floats here; gamma's are not
 GammaFileFormat IVFFlatIndex::gamma_format() const { return {"ivfflat.index", fourcc("IvFl"), (uint64_t)d_ * 4, true}; }
 GammaFileFormat IVFPQIndex::gamma_format() const { return {"ivfpq.index", fourcc("IwPQ"), (uint64_t)code_bytes(), false}; }
+// a spilled index (soar_lambda > 0) writes the variant fourcc ("Gs" for "Gb") and its lambda after the codec block
 GammaFileFormat IVFPQFastScanIndex::gamma_format() const {
-  return {"gb_ivfpqfs.index", fourcc("GbFS"), (uint64_t)code_bytes(), true};
+  return {"gb_ivfpqfs.index", spilled() ? fourcc("GsFS") : fourcc("GbFS"), (uint64_t)code_bytes(), true};
 }
 GammaFileFormat RaBitQIndex::gamma_format() const {
-  return {"gb_ivfrabitq.index", fourcc("GbRQ"), (uint64_t)code_bytes(), true};
+  return {"gb_ivfrabitq.index", spilled() ? fourcc("GsRQ") : fourcc("GbRQ"), (uint64_t)code_bytes(), true};
 }
-GammaFileFormat VearchIndex::gamma_format() const { return {"gb_vearch.index", fourcc("GbVR"), (uint64_t)code_bytes(), true}; }
+GammaFileFormat VearchIndex::gamma_format() const {
+  return {"gb_vearch.index", spilled() ? fourcc("GsVR") : fourcc("GbVR"), (uint64_t)code_bytes(), true};
+}
 GammaFileFormat BinaryIvfIndex::gamma_format() const {
   return {"gb_binaryivf.index", fourcc("GbBI"), (uint64_t)code_bytes(), true};
 }
@@ -152,6 +158,7 @@ int IvfIndex::capture_head(int64_t indexed, GammaImage* img) {
   ok = ok && wr<uint64_t>(f, (uint64_t)cent.size()) && wr_bytes(f, cent.data(), cent.size() * 4);  // WRITEXBVECTOR
   ok = ok && wr<uint8_t>(f, 0) && wr<uint64_t>(f, 0);                                              // direct map: none
   ok = ok && dump_gamma_extra(f) == 0;
+  if (spilled()) ok = ok && wr<double>(f, mp_.soar_lambda);
   ok = fclose(f) == 0 && ok;
   if (ok) img->head.assign(buf, len);
   free(buf);
@@ -367,6 +374,13 @@ int IvfIndex::load_gamma_part(const std::string& dir, const std::string& abs_nam
   if (dm_type != 0 || n != 0) return fail("direct maps are not supported");  // gamma never maintains one
   if (set_centroids(cent.data(), nlist_)) return -1;
   if (load_gamma_extra(f)) return -1;
+  if (spilled()) {
+    double lambda = 0;
+    if (!rd(f, &lambda)) return fail("truncated soar_lambda in " + path);
+    if (lambda != mp_.soar_lambda)
+      return fail("index file soar_lambda " + std::to_string(lambda) + " differs from the table's " +
+                  std::to_string(mp_.soar_lambda));
+  }
   // ReadInvertedLists (index_io.cc:143-194)
   uint32_t lt = 0;
   uint64_t nb = 0, cb = 0, ns = 0;
@@ -407,7 +421,7 @@ int IvfIndex::load_gamma_part(const std::string& dir, const std::string& abs_nam
   }
   std::vector<uint8_t> codes, padded;
   int64_t live = 0, max_vid = -1;
-  std::vector<uint64_t> v2p;  // vid_bucket_no_pos_, installed only if the whole file loads
+  std::vector<uint64_t> v2p, v2p2;  // vid_bucket_no_pos_ (spilled: and the second entries), installed only if the whole file loads
   std::vector<int> dead(nlist_, 0);
   const size_t my_cb = (size_t)code_bytes();
   for (int l = 0; l < nlist_; l++) {
@@ -444,6 +458,13 @@ int IvfIndex::load_gamma_part(const std::string& dir, const std::string& abs_nam
       live++;
       max_vid = std::max(max_vid, id);
       if ((size_t)id >= v2p.size()) v2p.resize(std::max<size_t>((size_t)id + 1, v2p.size() * 2), ~(uint64_t)0);
+      if (spilled() && v2p[id] != ~(uint64_t)0) {  // the vid's other live entry
+        if ((size_t)id >= v2p2.size()) v2p2.resize(std::max<size_t>((size_t)id + 1, v2p2.size() * 2), ~(uint64_t)0);
+        if (v2p2[id] != ~(uint64_t)0) return fail("vid " + std::to_string(id) + " has more than two live entries in " + path);
+        if ((v2p[id] >> 32) == (uint64_t)l) return fail("vid " + std::to_string(id) + " has two live entries in list " + std::to_string(l) + " of " + path);
+        v2p2[id] = (uint64_t)l << 32 | (uint64_t)pos;
+        continue;
+      }
       v2p[id] = (uint64_t)l << 32 | (uint64_t)pos;
     }
   }
@@ -463,6 +484,7 @@ int IvfIndex::load_gamma_part(const std::string& dir, const std::string& abs_nam
     std::unique_lock<std::shared_mutex> lk(mu_);
     if (lists_->commit(add, st)) return -1;
     vid2pos_.swap(v2p);
+    vid2pos2_.swap(v2p2);
     for (int l = 0; l < nlist_; l++) lists_->add_dead(l, dead[l]);
     if (lists_changed(st)) return -1;  // IVF-Flat on a host store: the row pointers into the loaded lists
     GB_CUDA(cudaStreamSynchronize(st));

@@ -366,11 +366,25 @@ cudaError_t launch_purge_count(ListDirectory dir, const int* sel_list, const int
                                int* sel_live, unsigned long long* vid_range, cudaStream_t st);
 // live entry with rank r of sel_list[s]: code -> dst_data[s] + r code_bytes, id -> dst_ids[s][r], and
 // newpos[vid - vid_min] = list << 32 | r (the caller pre-fills newpos with ~0, so a dropped vid reads ~0).  align: the
-// widest power of two <= 16 that divides code_bytes and every source and destination base.
+// widest power of two <= 16 that divides code_bytes and every source and destination base.  copies = 2 (spilled lists,
+// where a vid may have two live entries): newpos holds two slots per vid, [2 (vid - vid_min) + {0, 1}], filled in
+// whichever order the entries are met
 cudaError_t launch_purge_scatter(ListDirectory dir, const int* sel_list, const PurgeChunk* chunks, int nchunks,
                                  const uint32_t* del_bits, const int* chunk_off, int code_bytes, int align,
                                  void* const* dst_data, int64_t* const* dst_ids, unsigned long long* newpos,
-                                 int64_t vid_min, cudaStream_t st);
+                                 int64_t vid_min, cudaStream_t st, int copies = 1);
+
+// ---- SOAR spilling (kernels_soar.cu, DESIGN.md §8, SOAR spilling) -------------------------------------------
+// out[i] = the spilled list of row i (rows x, ldx floats apart, d dims) whose primary list is primary[i]: the list
+// c' != primary[i] of least |x - c'|^2 + lambda <r, x - c'>^2 / |r|^2 (r = x - c_primary), the lower id among equal
+// losses; -1 when primary[i] is no list, |r|^2 is 0 or not finite, or no loss is finite
+cudaError_t launch_soar_spill(const float* x, int64_t ldx, int64_t n, int d, const float* centroids, int64_t ldc, int nlist,
+                              const int32_t* primary, float lambda, int32_t* out, cudaStream_t st);
+// Per row of m sorted keys (ld apart): the first k whose vid (low 32 bits) has not occurred earlier in the row, in key
+// order, sentinel padded; m <= kDedupeMaxKeys
+constexpr int kDedupeMaxKeys = 4096;
+cudaError_t launch_dedupe_keys(const unsigned long long* keys, int64_t ld, int nrows, int m, int k, unsigned long long* out,
+                               int64_t out_stride, cudaStream_t st);
 // List pack (the capture of a backup or dump, stage.h): n entries of one list from its slab region into a stage, in the
 // index file's order.  Each code keeps the first dst_cb of its src_cb bytes (IVF-Flat rows drop their padding); the
 // ids are copied as stored, tombstone bits included, to dst_ids, which may sit at any byte offset.  A list is cut into

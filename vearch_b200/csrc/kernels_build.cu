@@ -348,7 +348,7 @@ __global__ void __launch_bounds__(256)
     purge_scatter_kernel(ListDirectory dir, const int* __restrict__ sel_list, const PurgeChunk* __restrict__ chunks,
                          const uint32_t* __restrict__ del_bits, const int* __restrict__ chunk_off, int code_bytes,
                          void* const* __restrict__ dst_data, int64_t* const* __restrict__ dst_ids,
-                         unsigned long long* __restrict__ newpos, int64_t vid_min) {
+                         unsigned long long* __restrict__ newpos, int64_t vid_min, int copies) {
   __shared__ int s_src[kPurgeChunk];
   __shared__ int s_warp[8];
   const PurgeChunk c = chunks[blockIdx.x];
@@ -377,7 +377,13 @@ __global__ void __launch_bounds__(256)
       const int r = nlive + before + __popc(m & ((1u << lane) - 1u));
       s_src[r] = p;
       out_ids[off + r] = id;
-      newpos[id - vid_min] = ((unsigned long long)list << 32) | (unsigned)(off + r);
+      const unsigned long long np = ((unsigned long long)list << 32) | (unsigned)(off + r);
+      if (copies == 1) {
+        newpos[id - vid_min] = np;
+      } else {  // the vid's first live entry met takes the first slot, its other one the second
+        unsigned long long* slot = newpos + 2 * (id - vid_min);
+        if (atomicCAS(slot, ~0ull, np) != ~0ull) slot[1] = np;
+      }
     }
     nlive += tot;
     __syncthreads();
@@ -411,12 +417,13 @@ cudaError_t launch_purge_count(ListDirectory dir, const int* sel_list, const int
 cudaError_t launch_purge_scatter(ListDirectory dir, const int* sel_list, const PurgeChunk* chunks, int nchunks,
                                  const uint32_t* del_bits, const int* chunk_off, int code_bytes, int align,
                                  void* const* dst_data, int64_t* const* dst_ids, unsigned long long* newpos,
-                                 int64_t vid_min, cudaStream_t st) {
+                                 int64_t vid_min, cudaStream_t st, int copies) {
   if (nchunks <= 0) return cudaSuccess;
   if (code_bytes <= 0 || code_bytes > kPurgeMaxCodeBytes || align <= 0 || code_bytes % align) return cudaErrorInvalidValue;
+  if (copies != 1 && copies != 2) return cudaErrorInvalidValue;
 #define GB_PURGE_SCATTER(V)                                                                                          \
   purge_scatter_kernel<V><<<nchunks, 256, 0, st>>>(dir, sel_list, chunks, del_bits, chunk_off, code_bytes, dst_data, \
-                                                   dst_ids, newpos, vid_min)
+                                                   dst_ids, newpos, vid_min, copies)
   switch (align) {
     case 16: GB_PURGE_SCATTER(uint4); break;
     case 8: GB_PURGE_SCATTER(uint2); break;

@@ -412,6 +412,21 @@ class GammaIndex:
                "purge")
         return int(n[0])
 
+    def vid_slots(self, vid):
+        """The list entries of vid as [(list, position), ...]: two for an index with SOAR spilling ("soar_lambda" > 0),
+        one otherwise, none for a vid in no list.  A fresh build lists the primary entry first."""
+        out = np.zeros(2, np.uint64)
+        _check(_lib.lib().gb_index_vid_slots(self._h, int(vid), _ptr(out)), "vid_slots")
+        return [(int(v) >> 32, int(v) & 0xFFFFFFFF) for v in out if int(v) != 2**64 - 1]
+
+    def memory_charge(self, n_total):
+        """What admission under the memory limit charges for storing rows up to n_total: (store growth bytes, rows that
+        growth makes room for, index bytes of those rows once indexed)."""
+        out = np.zeros(3, np.int64)
+        _check(_lib.lib().gb_index_memory_charge(self._h, int(n_total), _ptr(out[0:]), _ptr(out[1:]), _ptr(out[2:])),
+               "memory_charge")
+        return int(out[0]), int(out[1]), int(out[2])
+
     def dead_counts(self):
         """Dead entries counted per list (updates' tombstones + delete_vectors) since the list's last purge."""
         out = np.zeros(self.nlist, np.int32)
