@@ -250,7 +250,8 @@ int gb_debug_kmeans_trace(int device, const float *x, int64_t n, int d, int k, i
 /* One OPQ training run (the rotation "opq": {"nsubvector": M} learns in front of IVFPQ) over the n x d rows x, for
  * niter rounds, traced (a debug surface for the tests; DESIGN.md §5, OPQ bar).  n_s = min(n, 65536) rows are trained
  * on; T = niter.  Always written: sample [n_s], mean [d], r0 [d][d] (fp64 start), rf [T][d][d] (the fp32 rotation of
- * each round), xty [T][d][d] (X^T Y read back), r [T][d][d] (fp64 rotation each round solves for).  With detail set
+ * each round), xty [T][d][d] (X^T Y read back), r [T][d][d] (fp64 rotation each round solves for), sweeps [T] (the
+ * Jacobi sweeps of each round's SVD), solve_ms [T] (device time of each round's SVD and R = V U^T).  With detail set
  * also: centred [n_s][d], proj [T][n_s][d], codes [T][n_s][M], recon [T][n_s][d], and per round and subspace (round
  * major) the subspace k-means of gb_debug_kmeans_trace (k = 256, width d / M, no sampling below 256 000 rows; I
  * iterations: 40 in round 0, 4 after it): km_init [256][d / M], km_labels and km_scores [I][n_s], km_mean, km_split
@@ -258,7 +259,7 @@ int gb_debug_kmeans_trace(int device, const float *x, int64_t n, int d, int k, i
 int gb_debug_opq_trace(int device, const float *x, int64_t n, int d, int M, int niter, int detail, int64_t *sample,
                        float *mean, float *centred, double *r0, float *rf, float *proj, uint8_t *codes, float *recon,
                        float *xty, double *r, float *km_init, int32_t *km_labels, float *km_scores, float *km_mean,
-                       float *km_split, float *km_norm);
+                       float *km_split, float *km_norm, int32_t *sweeps, float *solve_ms);
 /* centroid update only: centroids[c] = mean of x[assign == c] in point order */
 int gb_kmeans_update(int device, const float *x, int64_t n, int d, int k, const int64_t *assign, float *centroids);
 /* router merge (internal/client/client.go:1530-1609) on device memory: dis/ids are

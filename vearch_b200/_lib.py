@@ -127,7 +127,7 @@ def _declare(l):
     l.gb_index_vearch_lut.argtypes = [vp, i32, vp, vp, vp]
     l.gb_kmeans.argtypes = [i32, vp, i64, i32, i32, i32, i64, i32, i32, vp, vp]
     l.gb_debug_kmeans_trace.argtypes = [i32, vp, i64, i32, i32, i32, i64, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
-    l.gb_debug_opq_trace.argtypes = [i32, vp, i64, i32, i32, i32, i32] + [vp] * 16
+    l.gb_debug_opq_trace.argtypes = [i32, vp, i64, i32, i32, i32, i32] + [vp] * 18
     l.gb_kmeans_update.argtypes = [i32, vp, i64, i32, i32, vp, vp]
     l.gb_device_pool_usage.argtypes = [i32, i32, C.POINTER(i64), C.POINTER(i64)]
     l.gb_memory_ledger.argtypes = [i32, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64)]

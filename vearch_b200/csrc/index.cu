@@ -11,7 +11,6 @@
 #include <random>
 
 #include "common.cuh"
-#include "jacobi_svd.h"
 #include "mem_ledger.h"
 
 namespace gb {
@@ -2691,13 +2690,30 @@ int opq_train_device(const float* xt, int64_t n_in, int d, int dpad, int Mo, int
     }
   }
   if (trace) trace->r0 = R;
-  std::vector<float> Rf((size_t)d * d), hx((size_t)d * dpad);
-  std::vector<double> a, U, V;
+  {
+    std::vector<float> Rf(R.begin(), R.end());
+    GB_CUDA(upload_rows_padded(d_opq, Rf.data(), d, d, dpad, st));
+  }
+  // every later rotation is solved on the device and written to d_opq as float (kernels_opq.cu); X^T Y and R come back
+  // to the host only for a trace
+  void* ws = s.alloc(opq_procrustes_ws_bytes(d));
+  double* r64 = trace ? s.alloc_n<double>((size_t)d * d) : nullptr;
+  if (!ws || (trace && !r64)) return -1;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  struct EventsGuard {
+    cudaEvent_t* e;
+    ~EventsGuard() {
+      for (int i = 0; i < 2; i++)
+        if (e[i]) cudaEventDestroy(e[i]);
+    }
+  } ev_guard{ev};
+  if (trace) {
+    GB_CUDA(cudaEventCreate(&ev[0]));
+    GB_CUDA(cudaEventCreate(&ev[1]));
+  }
   const int niter_pq_0 = 40, niter_pq = 4;
   for (int it = 0; it < niter; it++) {
-    for (size_t i = 0; i < R.size(); i++) Rf[i] = (float)R[i];
-    if (trace) trace->rf.insert(trace->rf.end(), Rf.begin(), Rf.end());
-    GB_CUDA(upload_rows_padded(d_opq, Rf.data(), d, d, dpad, st));
+    if (trace) GB_CUDA(trace_rows<float>(d_opq, dpad, d, d, trace->rf, st));
     GB_CUDA(cudaMemsetAsync(xproj, 0, (size_t)n * dpad * 4, st));
     GB_CUDA(launch_dist_matrix(xc, dpad, (int)n, d_opq, dpad, d, dpad, kMetricIP, xproj, dpad, st));
     const bool detail = trace && trace->detail;
@@ -2720,31 +2736,26 @@ int opq_train_device(const float* xt, int64_t n_in, int d, int dpad, int Mo, int
     GB_CUDA(launch_pq_encode(xproj, dpad, n, nullptr, 0, nullptr, pqc, Mo, dso, codes, st));
     GB_CUDA(launch_pq_decode(codes, n, pqc, Mo, dso, recon, dpad, st));
     GB_CUDA(launch_transpose(recon, dpad, n, d, rT, ldn, st));
-    GB_CUDA(launch_dist_matrix(xT, ldn, d, rT, ldn, d, (int)ldn, kMetricIP, xxr, dpad, st));
-    GB_CUDA(cudaMemcpyAsync(hx.data(), xxr, (size_t)d * dpad * 4, cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
+    GB_CUDA(launch_dist_matrix(xT, ldn, d, rT, ldn, d, (int)ldn, kMetricIP, xxr, dpad, st));  // X^T Y, d x d
     if (detail) {
       GB_CUDA(trace_rows<uint8_t>(codes, Mo, n, Mo, trace->codes, st));
       GB_CUDA(trace_rows<float>(recon, dpad, n, d, trace->recon, st));
     }
-    a.assign((size_t)d * d, 0.0);  // X^T Y, d x d
-    for (int i = 0; i < d; i++)
-      for (int j = 0; j < d; j++) a[(size_t)i * d + j] = hx[(size_t)i * dpad + j];
-    if (trace)
-      for (int i = 0; i < d; i++)
-        trace->xty.insert(trace->xty.end(), hx.begin() + (size_t)i * dpad, hx.begin() + (size_t)i * dpad + d);
-    jacobi_svd(a, d, d, &U, &V);
-    // R^T = U V^T  =>  R[i][j] = sum_k V[i][k] U[j][k]
-    for (int i = 0; i < d; i++)
-      for (int j = 0; j < d; j++) {
-        double acc = 0;
-        for (int kk = 0; kk < d; kk++) acc += V[(size_t)i * d + kk] * U[(size_t)j * d + kk];
-        R[(size_t)i * d + j] = acc;
-      }
-    if (trace) trace->r.insert(trace->r.end(), R.begin(), R.end());
+    if (trace) {
+      GB_CUDA(trace_rows<float>(xxr, dpad, d, d, trace->xty, st));
+      GB_CUDA(cudaEventRecord(ev[0], st));
+    }
+    int sweeps = 0;
+    GB_CUDA(opq_procrustes_device(xxr, dpad, d, ws, d_opq, dpad, r64, &sweeps, st));
+    if (trace) {
+      GB_CUDA(cudaEventRecord(ev[1], st));
+      GB_CUDA(trace_rows<double>(r64, d, d, d, trace->r, st));
+      float ms = 0;
+      GB_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+      trace->sweeps.push_back(sweeps);
+      trace->solve_ms.push_back(ms);
+    }
   }
-  for (size_t i = 0; i < R.size(); i++) Rf[i] = (float)R[i];
-  GB_CUDA(upload_rows_padded(d_opq, Rf.data(), d, d, dpad, st));
   GB_CUDA(cudaStreamSynchronize(st));
   return 0;
 }

@@ -562,6 +562,8 @@ struct OpqTrace {
   std::vector<float> xty;        // [T][d][d] X^T Y as read back
   std::vector<double> r;         // [T][d][d] the rotation the round's Procrustes solution gives
   std::vector<KMeansTrace> km;   // [T][M] each subspace's k-means
+  std::vector<int32_t> sweeps;   // [T] the Jacobi sweeps of the round's SVD
+  std::vector<float> solve_ms;   // [T] device time of the round's SVD and R = V U^T (CUDA events)
 };
 // OPQ rotation (faiss OPQMatrix restated) learnt from the n rows of xt (stride dpad) in niter rounds; the final d x d
 // rotation is written to d_opq (row stride dpad).  trace: nullptr on every production path

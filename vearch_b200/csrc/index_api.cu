@@ -891,7 +891,7 @@ int gb_debug_kmeans_trace(int device, const float* x, int64_t n, int d, int k, i
 int gb_debug_opq_trace(int device, const float* x, int64_t n, int d, int M, int niter, int detail, int64_t* sample,
                        float* mean, float* centred, double* r0, float* rf, float* proj, uint8_t* codes, float* recon,
                        float* xty, double* r, float* km_init, int32_t* km_labels, float* km_scores, float* km_mean,
-                       float* km_split, float* km_norm) {
+                       float* km_split, float* km_norm, int32_t* sweeps, float* solve_ms) {
   if (M <= 0 || d % M != 0 || niter < 1 || n <= 0) {
     set_last_error("opq trace: bad shape");
     return -1;
@@ -923,6 +923,8 @@ int gb_debug_opq_trace(int device, const float* x, int64_t n, int d, int M, int 
   std::copy(t.rf.begin(), t.rf.end(), rf);
   std::copy(t.xty.begin(), t.xty.end(), xty);
   std::copy(t.r.begin(), t.r.end(), r);
+  std::copy(t.sweeps.begin(), t.sweeps.end(), sweeps);
+  std::copy(t.solve_ms.begin(), t.solve_ms.end(), solve_ms);
   if (!t.detail) return 0;
   std::copy(t.centred.begin(), t.centred.end(), centred);
   std::copy(t.proj.begin(), t.proj.end(), proj);

@@ -165,6 +165,13 @@ cudaError_t launch_transpose(const float* x, int64_t ldx, int64_t n, int d, floa
 // recon[i][m * dsub + j] = pq[m][codes[i][m]][j]
 cudaError_t launch_pq_decode(const uint8_t* codes, int64_t n, const float* pq_centroids, int M, int dsub, float* recon,
                              int64_t ldr, cudaStream_t st);
+// The rotation of one OPQ round (kernels_opq.cu): R = V U^T for xty = X^T Y = U S V^T (d x d fp32, row stride ldx),
+// the SVD a one-sided Jacobi in fp64 with jacobi_svd.h's rules.  float(R) goes to r32 (row stride ld32, columns >= d
+// untouched); R itself to r64 (d x d) when it is not null.  ws: opq_procrustes_ws_bytes(d) bytes of device memory.
+// Synchronises st once, to read which singular values vanished; *sweeps (when not null): the Jacobi sweeps run.
+size_t opq_procrustes_ws_bytes(int d);
+cudaError_t opq_procrustes_device(const float* xty, int64_t ldx, int d, void* ws, float* r32, int64_t ld32,
+                                  double* r64, int* sweeps, cudaStream_t st);
 
 // ---- K4/K5: IVF-PQ look-up tables + ADC scan --------------------------------------------
 // ip[q][m][c] = <x_q|m, pq_m[c]>   (pq.compute_inner_prod_table); ksub = 2^nbits centroids per sub-quantiser

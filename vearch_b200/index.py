@@ -719,14 +719,15 @@ def debug_opq_trace(x, M, niter=3, detail=True, device=0):
     """One OPQ training run (the rotation "opq": {"nsubvector": M} learns), niter rounds, traced: a dict of numpy
     arrays.  sample [n_s]: the rows trained on; mean [d]; r0 [d, d] float64: the random orthonormal start; rf
     [niter, d, d]: the float32 rotation of each round; xty [niter, d, d]: X^T Y as the device formed it; r [niter, d, d]
-    float64: the rotation each round solves for.  With detail: centred [n_s, d]; proj, recon [niter, n_s, d]; codes
+    float64: the rotation each round solves for; sweeps [niter]: the Jacobi sweeps of each round's SVD; solve_ms
+    [niter]: the device time of each round's SVD and R = V U^T (CUDA events).  With detail: centred [n_s, d]; proj, recon [niter, n_s, d]; codes
     [niter, n_s, M]; km [niter][M]: each subspace's k-means trace, as debug_kmeans_trace gives it."""
     x = _f32(x)
     n, d = x.shape
     ns, ds, T = min(n, OPQ_MAX_TRAIN), d // M, niter
     out = {"sample": np.empty(ns, np.int64), "mean": np.empty(d, np.float32), "r0": np.empty((d, d), np.float64),
            "rf": np.empty((T, d, d), np.float32), "xty": np.empty((T, d, d), np.float32),
-           "r": np.empty((T, d, d), np.float64)}
+           "r": np.empty((T, d, d), np.float64), "sweeps": np.empty(T, np.int32), "solve_ms": np.empty(T, np.float32)}
     its = [opq_kmeans_iters(t) for t in range(T)]
     tot = sum(its) * M
     bulk = dict(centred=np.empty((ns, d), np.float32), proj=np.empty((T, ns, d), np.float32),
@@ -738,7 +739,8 @@ def debug_opq_trace(x, M, niter=3, detail=True, device=0):
     _check(_lib.lib().gb_debug_opq_trace(device, _ptr(x), n, d, M, niter, int(detail), _ptr(out["sample"]),
                                          _ptr(out["mean"]), b("centred"), _ptr(out["r0"]), _ptr(out["rf"]), b("proj"),
                                          b("codes"), b("recon"), _ptr(out["xty"]), _ptr(out["r"]), b("init"),
-                                         b("labels"), b("scores"), b("kmean"), b("split"), b("norm")),
+                                         b("labels"), b("scores"), b("kmean"), b("split"), b("norm"),
+                                         _ptr(out["sweeps"]), _ptr(out["solve_ms"])),
            "debug_opq_trace")
     if detail:
         for key in ("centred", "proj", "codes", "recon"):
