@@ -66,6 +66,7 @@ struct PtShared {
   uint64_t code_full[PT_CS], code_empty[PT_CS];
   uint64_t b_full[2], b_empty[2], a_full[2], a_empty[2], acc_empty[2];
   alignas(16) float ne[2][PT_N];  // |r_e|^2 of the tile's entries, +inf = can never be returned
+  alignas(16) float ne_min[2][PT_N / 32];  // min of ne over each decode warp's 32 entries (columns 32 g .. 32 g + 31)
   // candidate queue: the epilogue warps append (query, probe, position) records with shared-memory atomics and move on;
   // the drain warp turns them into the global per-query lists.  A global atomicAdd-with-return costs ~1 us of latency:
   // issued from the epilogue it stalled the whole pipeline as soon as a loose bound let a percent of the entries through.
@@ -523,29 +524,53 @@ __global__ void __launch_bounds__(PT_NT, 1)
         wg_wait<0>();
         wg_fence_acc(acc);
         mbar_arrive(&sh.b_empty[b]);
-        // biased, the accumulators' bits are floats without a conversion (PairMeta).  (Starting the MMAs from the bias
-        // instead makes ptxas serialise every wgmma of the kernel, C7520.)
-#pragma unroll
-        for (int u = 0; u < 2; u++)
-#pragma unroll
-          for (int k = 0; k < 64; k++) acc[u][k] += kAccBias;
         if (i == ntiles - 1) mbar_arrive(&sh.a_empty[ab]);
-        // Fast path: min over the tile of v = c * ne - (bias + acc) per pair, on the fragments themselves.  A warp where
-        // some pair has a candidate redoes the test per entry and pushes the hits (pt_push_frag_hits).
-        float mn[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
+        // Group screen: per pair and group of 32 columns (one decode warp's entries), lb = c * min ne - (bias + max acc)
+        // with the same fma as the per-entry test.  Its exact argument is <= every entry's (ne >= min ne, c > 0,
+        // acc <= max acc, and the biased float grows with acc), and correctly rounded fma is monotone, so lb <= v for
+        // every entry of the group: a pair with some v <= thr has lb <= thr.  One integer max per element instead of an
+        // add, an fma and a min; the per-entry test below runs only in warps the screen did not clear.
+        const float4 nm4 = *reinterpret_cast<const float4*>(sh.ne_min[b]);
+        const float nmin[4] = {nm4.x, nm4.y, nm4.z, nm4.w};
+        bool maybe = false;
 #pragma unroll
-        for (int j = 0; j < PT_N / 8; j++) {
-          const float2 n2 = *reinterpret_cast<const float2*>(&sh.ne[b][8 * j + 2 * (t & 3)]);
+        for (int f4 = 0; f4 < 4; f4++) {
+          float lb = INFINITY;
 #pragma unroll
-          for (int f4 = 0; f4 < 4; f4++) {
-            const uint32_t* a2 = &acc[f4 >> 1][4 * j + 2 * (f4 & 1)];
-            mn[f4] = fminf(mn[f4], fminf(fmaf(n2.x, fc[f4], -__uint_as_float(a2[0])), fmaf(n2.y, fc[f4], -__uint_as_float(a2[1]))));
+          for (int g = 0; g < PT_N / 32; g++) {
+            int mx = (int)acc[f4 >> 1][16 * g + 2 * (f4 & 1)];
+#pragma unroll
+            for (int j = 4 * g; j < 4 * g + 4; j++)
+#pragma unroll
+              for (int e = 0; e < 2; e++) mx = max(mx, (int)acc[f4 >> 1][4 * j + 2 * (f4 & 1) + e]);
+            lb = fminf(lb, fmaf(nmin[g], fc[f4], -__uint_as_float((uint32_t)mx + kAccBias)));
           }
+          maybe |= lb <= fthr[f4];
         }
-        bool hit = false;
+        if (__any_sync(0xffffffffu, maybe)) {
+          // biased, the accumulators' bits are floats without a conversion (PairMeta).  (Starting the MMAs from the bias
+          // instead makes ptxas serialise every wgmma of the kernel, C7520.)
 #pragma unroll
-        for (int f4 = 0; f4 < 4; f4++) hit |= mn[f4] <= fthr[f4];
-        if (__any_sync(0xffffffffu, hit)) pt_push_frag_hits(acc, sh.ne[b], fthr, fc, gm, (uint32_t)(tl.row0 + i * PT_N), &sh);
+          for (int u = 0; u < 2; u++)
+#pragma unroll
+            for (int k = 0; k < 64; k++) acc[u][k] += kAccBias;
+          // min over the tile of v = c * ne - (bias + acc) per pair, on the fragments themselves.  A warp where some pair
+          // has a candidate redoes the test per entry and pushes the hits (pt_push_frag_hits).
+          float mn[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
+#pragma unroll
+          for (int j = 0; j < PT_N / 8; j++) {
+            const float2 n2 = *reinterpret_cast<const float2*>(&sh.ne[b][8 * j + 2 * (t & 3)]);
+#pragma unroll
+            for (int f4 = 0; f4 < 4; f4++) {
+              const uint32_t* a2 = &acc[f4 >> 1][4 * j + 2 * (f4 & 1)];
+              mn[f4] = fminf(mn[f4], fminf(fmaf(n2.x, fc[f4], -__uint_as_float(a2[0])), fmaf(n2.y, fc[f4], -__uint_as_float(a2[1]))));
+            }
+          }
+          bool hit = false;
+#pragma unroll
+          for (int f4 = 0; f4 < 4; f4++) hit |= mn[f4] <= fthr[f4];
+          if (__any_sync(0xffffffffu, hit)) pt_push_frag_hits(acc, sh.ne[b], fthr, fc, gm, (uint32_t)(tl.row0 + i * PT_N), &sh);
+        }
         mbar_arrive(&sh.acc_empty[b]);
       }
       an++;
@@ -623,7 +648,12 @@ __global__ void __launch_bounds__(PT_NT, 1)
         }
         // ne[b] is read by the epilogue of tile bn - 2: wait until it has released the buffer
         mbar_wait(&sh.acc_empty[b], ((bn >> 1) & 1) ^ 1);
-        sh.ne[b][e] = valid ? nsum : INFINITY;
+        const float ne_e = valid ? nsum : INFINITY;
+        sh.ne[b][e] = ne_e;
+        float nmin = ne_e;  // the group screen's min ne over this warp's 32 entries (fminf: a NaN never wins)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) nmin = fminf(nmin, __shfl_xor_sync(0xffffffffu, nmin, o));
+        if ((e & 31) == 0) sh.ne_min[b][e >> 5] = nmin;
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> tensor-core proxy
         mbar_arrive(&sh.b_full[b]);
       }
