@@ -274,6 +274,21 @@ int gb_merge_partition_keys_device(int device, const unsigned long long *keys_de
 int gb_debug_dist_matrix(int device, const float *x, int n, const float *c, int m, int d, int metric, int use_tc,
                          float *out);
 
+/* The exact re-rank over the index's HBM rows, for tests: nq queries [nq][d], each with ncand candidate vids
+ * cand[nq][ncand] (-1: no candidate, at any position), re-ranked to k by the two-pass kernel (two_pass != 0) or the
+ * one-pass kernel under the score window of gb_index_search.  The bitmaps (gb_index_search's) screen the candidates as
+ * the list scans do before a re-rank: a deleted or filtered-out vid is no candidate.  Results out_dis / out_ids
+ * [nq][k].  Two-pass only: out_survivors[nq], the candidates whose fp32 rows were read, and per candidate [nq][ncand] its pass-1 interval
+ * [out_lo, out_hi] as scores and out_state: 0 bounded, 1 bounded but withheld from the k-th bound (the interval
+ * crosses the score window), 2 unbounded (lo, hi NaN), 3 dead (no candidate; lo, hi NaN). */
+int gb_debug_rerank(gb_index *index, int nq, const float *xq, int ncand, const int64_t *cand, int k,
+                    const uint8_t *del_bitmap, const uint8_t *filter_bitmap, int64_t bitmap_bits, float min_score,
+                    float max_score, int two_pass, float *out_dis, int64_t *out_ids, int *out_survivors, float *out_lo,
+                    float *out_hi, int *out_state);
+/* the raw store's int8 shadow rows [start, start + n), *row_bytes = round_up(dpad, 16) + 16 bytes each: the int8
+ * values, then float {s, e, nrm, 0}.  out == NULL: only *row_bytes. */
+int gb_debug_shadow_rows(gb_index *index, int64_t start, int64_t n, uint8_t *out, int64_t *row_bytes);
+
 /* the device's default memory pool, which every search's scratch comes from: bytes in use and the high-water mark
  * since the last reset (after the device's pending work); reset_peak != 0 then restarts the mark at the current use */
 int gb_device_pool_usage(int device, int reset_peak, int64_t *used, int64_t *peak);

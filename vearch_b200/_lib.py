@@ -64,6 +64,8 @@ def _declare(l):
     l.gb_index_set_rerank_stats.restype = None
     l.gb_index_set_rerank_stats.argtypes = [vp, i32]
     l.gb_index_rerank_survivors.argtypes = [vp, C.POINTER(C.c_void_p), C.POINTER(i64)]
+    l.gb_debug_rerank.argtypes = [vp, i32, vp, i32, vp, i32, vp, vp, i64, f32, f32, i32, vp, vp, vp, vp, vp, vp]
+    l.gb_debug_shadow_rows.argtypes = [vp, i64, i64, vp, C.POINTER(i64)]
     l.gb_index_set_scan_timing.restype = None
     l.gb_index_set_scan_timing.argtypes = [vp, i32]
     l.gb_index_last_scan_ms.restype = f32

@@ -1278,6 +1278,100 @@ int Index::search_direct(const SearchContext& ctx, int nq, const void* x, int k,
   return download_results(keys, nq, k, search_metric(ctx), out_dis, out_ids, s);
 }
 
+int Index::debug_rerank(const SearchContext& ctx, int nq, const float* xq, int ncand, const int64_t* cand, int k,
+                        bool two_pass, float* out_dis, int64_t* out_ids, int* out_surv, float* out_lo, float* out_hi,
+                        int* out_state) {
+  if (nq <= 0) return 0;
+  if (store_->on_host() || store_->row_bytes() != 4 * d_ || (two_pass && !store_->has_shadow())) {
+    set_last_error("debug_rerank: needs fp32 rows in HBM (and their shadow for the two-pass kernel)");
+    return -1;
+  }
+  if (ncand <= 0 || ncand > 8192 || k <= 0 || k > ncand) {
+    set_last_error("debug_rerank: needs 1 <= k <= ncand <= 8192");
+    return -1;
+  }
+  cudaSetDevice(device_);
+  Scratch s(thread_stream(device_));
+  cudaStream_t st = s.stream();
+  const void* dq = upload_queries(nq, xq, s);
+  if (!dq) return -1;
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  const int64_t n = store_->size();
+  // the re-rank kernels take candidates the list scans have already screened with the bitmaps: a vid they exclude
+  // (deleted; or not allowed, ids past the filter bitmap included) is no candidate
+  auto bit = [&](const uint8_t* b, int64_t v) { return v < ctx.bitmap_bits && ((b[v >> 3] >> (v & 7)) & 1); };
+  std::vector<unsigned long long> h((size_t)nq * ncand);
+  for (size_t i = 0; i < h.size(); i++) {
+    const int64_t v = cand[i];
+    if (v >= n) {
+      set_last_error("debug_rerank: candidate vid past the store");
+      return -1;
+    }
+    const bool out = v < 0 || (ctx.del_bitmap && bit(ctx.del_bitmap, v)) || (ctx.filter_bitmap && !bit(ctx.filter_bitmap, v));
+    h[i] = out ? kKeySentinel : (unsigned long long)v;
+  }
+  const FilterArgs f{nullptr, nullptr, ctx.min_score, ctx.max_score};
+  const int metric = mp_.metric;
+  GB_ALLOC(keys, unsigned long long, h.size(), s);
+  GB_ALLOC(out_keys, unsigned long long, (size_t)nq * k, s);
+  GB_CUDA(cudaMemcpyAsync(keys, h.data(), h.size() * 8, cudaMemcpyHostToDevice, st));
+  const float* x = static_cast<const float*>(dq);
+  if (!two_pass) {
+    GB_CUDA(launch_rerank(keys, ncand, nq, x, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_, false, k, metric,
+                          f, out_keys, st));
+    return download_results(out_keys, nq, k, metric, out_dis, out_ids, s);
+  }
+  GB_ALLOC(surv, int, (size_t)nq, s);
+  GB_ALLOC(iv, uint4, h.size(), s);
+  GB_CUDA(launch_rerank_prefilter(keys, ncand, nq, x, dpad_, dpad_, store_->d_segs(), store_->seg_shift(), dpad_,
+                                  store_->shadow_segs(), store_->shadow_stride(), k, metric, f, out_keys, surv, st, iv));
+  std::vector<uint4> hv(h.size());
+  GB_CUDA(cudaMemcpyAsync(hv.data(), iv, hv.size() * sizeof(uint4), cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaMemcpyAsync(out_surv, surv, (size_t)nq * sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (download_results(out_keys, nq, k, metric, out_dis, out_ids, s)) return -1;
+  // the ordinals pass 1 ranks by must be the ones of the interval's ends (the better end for lo, the worse for hi)
+  for (size_t i = 0; i < hv.size(); i++) {
+    const uint4 v = hv[i];
+    float flo, fhi;
+    memcpy(&flo, &v.z, 4);
+    memcpy(&fhi, &v.w, 4);
+    const float best = metric == kMetricL2 ? flo : fhi, worst = metric == kMetricL2 ? fhi : flo;
+    const bool bounded = flo == flo && fhi == fhi;
+    int state;
+    bool ok;
+    if (v.x == 0xFFFFFFFFu) {
+      state = kRrDead, ok = v.y == 0xFFFFFFFFu && !bounded && h[i] == kKeySentinel;
+    } else if (!bounded) {
+      state = kRrUnbounded, ok = v.x == 0 && v.y == 0xFFFFFFFFu;
+    } else {
+      state = v.y == 0xFFFFFFFFu ? kRrWithheld : kRrBounded;
+      ok = v.x == score2ord(best, metric) && (state == kRrWithheld || v.y == score2ord(worst, metric));
+    }
+    if (!ok) {
+      set_last_error("debug_rerank: candidate " + std::to_string(i) + ": pass-1 ordinals disagree with its interval");
+      return -1;
+    }
+    out_lo[i] = flo, out_hi[i] = fhi, out_state[i] = state;
+  }
+  return 0;
+}
+
+int Index::debug_shadow_rows(int64_t start, int64_t n, void* out, int64_t* row_bytes) {
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  if (!store_->has_shadow()) {
+    set_last_error("debug_shadow_rows: the raw store has no shadow");
+    return -1;
+  }
+  *row_bytes = store_->shadow_stride();
+  if (!out) return 0;
+  cudaSetDevice(device_);
+  if (store_->get_shadow_rows(start, n, out)) {
+    set_last_error("debug_shadow_rows: rows out of range");
+    return -1;
+  }
+  return 0;
+}
+
 cudaError_t Index::flat_tile(const void* xq, int nq, const void* rows, int m, int metric, float* scores, int64_t ldo,
                              cudaStream_t st) {
   last_scan_kernel_ = "dist_tile_kernel+select_rows_kernel";

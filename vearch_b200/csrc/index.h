@@ -111,6 +111,10 @@ class RawStore {
   bool has_shadow() const { return shadow_ != nullptr; }
   const unsigned char* const* shadow_segs() const { return shadow_->d_segs_; }
   int64_t shadow_stride() const { return shadow_->stride_; }
+  // shadow rows [start, start + n), packed, into host memory (tests)
+  int get_shadow_rows(int64_t start, int64_t n, void* out) const {
+    return shadow_ ? shadow_->get_rows_host(start, n, out) : -1;
+  }
 
  private:
   int encode_shadow(int64_t si, int64_t off, int64_t cnt, cudaStream_t st);
@@ -383,6 +387,15 @@ class Index {
     std::lock_guard<std::mutex> g(ev_mu_);
     return std::move(rr_survivors_);
   }
+  // Tests of the exact re-rank over this index's HBM rows (gb_debug_rerank): the caller's nq x ncand candidate vids
+  // (-1: none, anywhere) re-ranked by the two-pass kernel (two_pass) or the one-pass kernel, keys decoded into
+  // out_dis / out_ids [nq][k]; two-pass only: survivor counts [nq] and each candidate's pass-1 interval as scores
+  // out_lo / out_hi [nq][ncand] (NaN where there is none) and its state (kRrBounded, ...)
+  enum { kRrBounded = 0, kRrWithheld = 1, kRrUnbounded = 2, kRrDead = 3 };
+  int debug_rerank(const SearchContext& ctx, int nq, const float* xq, int ncand, const int64_t* cand, int k, bool two_pass,
+                   float* out_dis, int64_t* out_ids, int* out_surv, float* out_lo, float* out_hi, int* out_state);
+  // shadow rows [start, start + n) of the raw store, (round_up(dpad, 16) + 16) bytes each (gb_debug_shadow_rows)
+  int debug_shadow_rows(int64_t start, int64_t n, void* out, int64_t* row_bytes);
 
  protected:
   // Device queries, here and below: nq rows store().stride() bytes apart, zero padded (dpad floats; BINARYIVF: words).

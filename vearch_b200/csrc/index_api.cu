@@ -486,6 +486,25 @@ int gb_index_rerank_survivors(gb_index* index, int** out, int64_t* n) {
   return 0;
 }
 
+int gb_debug_rerank(gb_index* index, int nq, const float* xq, int ncand, const int64_t* cand, int k,
+                    const uint8_t* del_bitmap, const uint8_t* filter_bitmap, int64_t bitmap_bits, float min_score,
+                    float max_score, int two_pass, float* out_dis, int64_t* out_ids, int* out_survivors, float* out_lo,
+                    float* out_hi, int* out_state) {
+  IDX_OR_FAIL(index);
+  SearchContext ctx;
+  if (fill_ctx(&ctx, nullptr, 0, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score)) return -1;
+  if (two_pass && !(out_survivors && out_lo && out_hi && out_state)) {
+    set_last_error("debug_rerank: the two-pass kernel needs every output");
+    return -1;
+  }
+  return index->impl->debug_rerank(ctx, nq, xq, ncand, cand, k, two_pass != 0, out_dis, out_ids, out_survivors, out_lo,
+                                   out_hi, out_state);
+}
+int gb_debug_shadow_rows(gb_index* index, int64_t start, int64_t n, uint8_t* out, int64_t* row_bytes) {
+  IDX_OR_FAIL(index);
+  return index->impl->debug_shadow_rows(start, n, out, row_bytes);
+}
+
 void gb_index_set_scan_timing(gb_index* index, int on) {
   if (index && index->impl) index->impl->set_time_scan(on != 0);
 }

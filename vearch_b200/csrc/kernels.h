@@ -249,11 +249,14 @@ cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq
 // The same re-rank in two passes (rows in HBM with an int8 shadow, RawStore): candidates are bounded from their shadow
 // rows (shadow_segs, the same segments as raw_segments, shadow_stride = round_up(d, 16) + 16 bytes apart) and only
 // those that can still reach the top k have their fp32 rows read and scored.  The output keys equal launch_rerank's.
-// survivors (nullable): per query, the candidates whose fp32 row was read.
+// survivors (nullable): per query, the candidates whose fp32 row was read.  intervals (nullable, tests only):
+// [nq][ncand] pass-1 results {lo, hi, flo, fhi}: the two ordinals pass 1 keeps (kOrdDead / 0 markers included) and the
+// interval's fp32 ends as float bits (NaN for a dead or unbounded candidate).
 cudaError_t launch_rerank_prefilter(const unsigned long long* cand_keys, int ncand, int nq, const float* xq, int64_t ldq,
                                     int d, const float* const* raw_segments, int seg_shift, int64_t ld_raw,
                                     const unsigned char* const* shadow_segs, int64_t shadow_stride, int k, int metric,
-                                    FilterArgs f, unsigned long long* out_keys, int* survivors, cudaStream_t st);
+                                    FilterArgs f, unsigned long long* out_keys, int* survivors, cudaStream_t st,
+                                    uint4* intervals = nullptr);
 // n fp32 rows (cols values, ld floats apart) -> their shadow rows, out_stride = round_up(cols, 16) + 16 bytes apart:
 // int8 qy = rn(y / s), s = max|y| / 127, zero padded, then float4 {s, e >= |y - s qy|, nrm >= |s qy|, 0}; a row with a
 // zero or non-finite scale gets {0, inf, inf, 0}

@@ -378,13 +378,15 @@ __device__ __forceinline__ float rs_qy(uint32_t w_biased, int b) {
   return __uint_as_float(__byte_perm(w_biased, 0x4B000000u, 0x7540u + b)) - 8388736.0f;
 }
 
-template <int METRIC>
+// INTERVALS: write each candidate's pass-1 result to `intervals` (tests); the search instantiates it off
+template <int METRIC, bool INTERVALS>
 __global__ void __launch_bounds__(RR_NT)
     rerank_prefilter_kernel(const unsigned long long* __restrict__ cand_keys, int ncand, int NP,
                             const float* __restrict__ xq, int64_t ldq, int d, const float* const* __restrict__ raw_segments,
                             int seg_shift, int64_t ld_raw, const unsigned char* const* __restrict__ shadow_segs,
                             int64_t shadow_stride, int cols16, int k, FilterArgs f,
-                            unsigned long long* __restrict__ out_keys, int* __restrict__ survivors) {
+                            unsigned long long* __restrict__ out_keys, int* __restrict__ survivors,
+                            uint4* __restrict__ intervals) {
   extern __shared__ __align__(16) unsigned char rr_smem[];
   unsigned long long* buf = reinterpret_cast<unsigned long long*>(rr_smem);  // [NP] survivors' keys
   float* qs = reinterpret_cast<float*>(buf + NP);                              // [cols16], zero padded
@@ -476,6 +478,7 @@ __global__ void __launch_bounds__(RR_NT)
     const int j = j0 + sub * 4 + g;
     if (sub < RS_U && j < ncand) {
       uint32_t jlo = kOrdDead, jhi = kOrdDead;
+      float flo = __int_as_float(0x7FC00000), fhi = flo;
       if (live) {
         const double st = a, s = m.x, e = m.y, nrm = m.z;
         double slo, shi, mag;
@@ -503,7 +506,7 @@ __global__ void __launch_bounds__(RR_NT)
         }
         // every partial sum of either evaluation stays below 2^126: no overflow; NaN or inf anywhere: unbounded
         if (mag <= 0x1p126) {
-          const float flo = __double2float_rd(slo), fhi = __double2float_ru(shi);
+          flo = __double2float_rd(slo), fhi = __double2float_ru(shi);
           jlo = score2ord<METRIC>(METRIC == kMetricL2 ? flo : fhi);
           if (flo >= f.min_score && fhi <= f.max_score) jhi = score2ord<METRIC>(METRIC == kMetricL2 ? fhi : flo);
         } else {
@@ -512,6 +515,8 @@ __global__ void __launch_bounds__(RR_NT)
       }
       lo[j] = jlo;
       hi[j] = jhi;
+      if (INTERVALS)
+        intervals[(int64_t)q * ncand + j] = make_uint4(jlo, jhi, __float_as_uint(flo), __float_as_uint(fhi));
     }
   }
   __syncthreads();
@@ -727,6 +732,17 @@ cudaError_t launch_ivfpq_packed_scan(const float* ip_table, int nq, const int32_
   return launch_list_scan<IvfpqPackedCodec, kMetricIP, 0>(c, nq, a, st);
 }
 
+// A launch's dynamic shared memory past 48 KiB, together with the kernel's static shared memory (the two-pass
+// kernel's radix-select histogram), needs the kernel's opt-in: without it a launch at, e.g., d = 4096 and 2048
+// candidates (exactly 48 KiB dynamic) is refused
+template <class K>
+static cudaError_t rr_opt_in_smem(K kern, size_t smem) {
+  cudaFuncAttributes fa;
+  if (cudaError_t e = cudaFuncGetAttributes(&fa, kern)) return e;
+  if (smem + fa.sharedSizeBytes <= 48 * 1024) return cudaSuccess;
+  return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+}
+
 cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq, const float* xq, int64_t ldq, int d,
                           const float* const* raw_segments, int seg_shift, int64_t ld_raw, bool host_rows, int k,
                           int metric, FilterArgs f, unsigned long long* out_keys, cudaStream_t st) {
@@ -735,10 +751,7 @@ cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq
   int NP = next_pow2(ncand < 2 ? 2 : ncand);  // >= 16 bytes of keys: the query row behind them is read as float4
   size_t smem = (size_t)NP * 8 + (size_t)d * 4;
   auto kern = host_rows ? rerank_kernel<8> : rerank_kernel<4>;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-  }
+  if (cudaError_t e = rr_opt_in_smem(kern, smem)) return e;
   kern<<<nq, RR_NT, smem, st>>>(cand_keys, ncand, NP, xq, ldq, d, raw_segments, seg_shift, ld_raw, k, metric, f,
                                 out_keys);
   note_launch();
@@ -748,20 +761,21 @@ cudaError_t launch_rerank(const unsigned long long* cand_keys, int ncand, int nq
 cudaError_t launch_rerank_prefilter(const unsigned long long* cand_keys, int ncand, int nq, const float* xq, int64_t ldq,
                                     int d, const float* const* raw_segments, int seg_shift, int64_t ld_raw,
                                     const unsigned char* const* shadow_segs, int64_t shadow_stride, int k, int metric,
-                                    FilterArgs f, unsigned long long* out_keys, int* survivors, cudaStream_t st) {
+                                    FilterArgs f, unsigned long long* out_keys, int* survivors, cudaStream_t st,
+                                    uint4* intervals) {
   if (nq <= 0) return cudaSuccess;
   const int cols16 = (d + 15) & ~15;
   if (ncand <= 0 || ncand > 8192 || k <= 0 || k > ncand || (d & 3) || shadow_stride != cols16 + 16)
     return cudaErrorInvalidValue;
   const int NP = next_pow2(ncand < 2 ? 2 : ncand);
   const size_t smem = (size_t)NP * 8 + (size_t)cols16 * 4 + (size_t)NP * 8;
-  auto kern = metric == kMetricL2 ? rerank_prefilter_kernel<kMetricL2> : rerank_prefilter_kernel<kMetricIP>;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-  }
+  auto kern = metric == kMetricL2 ? (intervals ? rerank_prefilter_kernel<kMetricL2, true>
+                                               : rerank_prefilter_kernel<kMetricL2, false>)
+                                  : (intervals ? rerank_prefilter_kernel<kMetricIP, true>
+                                               : rerank_prefilter_kernel<kMetricIP, false>);
+  if (cudaError_t e = rr_opt_in_smem(kern, smem)) return e;
   kern<<<nq, RR_NT, smem, st>>>(cand_keys, ncand, NP, xq, ldq, d, raw_segments, seg_shift, ld_raw, shadow_segs,
-                                shadow_stride, cols16, k, f, out_keys, survivors);
+                                shadow_stride, cols16, k, f, out_keys, survivors, intervals);
   note_launch();
   return cudaGetLastError();
 }

@@ -259,6 +259,42 @@ class GammaIndex:
         C.CDLL(None).free(C.c_void_p(p.value))
         return out
 
+    RR_BOUNDED, RR_WITHHELD, RR_UNBOUNDED, RR_DEAD = 0, 1, 2, 3  # debug_rerank's per-candidate states
+
+    def debug_rerank(self, x, cand, k, two_pass=True, del_bitmap=None, filter_bitmap=None, min_score=-FLT_MAX,
+                     max_score=FLT_MAX):
+        """The exact re-rank of caller-given candidates (int64 vids [nq, ncand], -1: none, anywhere) over this index's
+        HBM rows, by the two-pass kernel or the one-pass kernel.  The bitmaps screen the candidates as the list scans do
+        before a re-rank (a deleted or filtered-out vid is no candidate).  Returns a dict: dis, ids [nq, k]; two-pass also
+        surv [nq] (candidates whose fp32 rows were read) and per candidate lo, hi [nq, ncand] float32 (its pass-1
+        interval as scores, NaN where there is none) and state (RR_BOUNDED; RR_WITHHELD: bounded, but the interval
+        crosses the score window, so it does not set the k-th bound; RR_UNBOUNDED; RR_DEAD: no candidate)."""
+        x = _f32(x)
+        cand = np.ascontiguousarray(cand, np.int64)
+        nq, ncand = cand.shape
+        assert x.shape == (nq, self.d)
+        out = {"dis": np.empty((nq, k), np.float32), "ids": np.empty((nq, k), np.int64)}
+        if two_pass:
+            out.update(surv=np.empty(nq, np.int32), lo=np.empty((nq, ncand), np.float32),
+                       hi=np.empty((nq, ncand), np.float32), state=np.empty((nq, ncand), np.int32))
+        db, fb = _bitmap(del_bitmap), _bitmap(filter_bitmap)
+        bits = max([b.size * 8 for b in (db, fb) if b is not None], default=0)
+        _check(_lib.lib().gb_debug_rerank(self._h, nq, _ptr(x), ncand, _ptr(cand), k, _ptr(db), _ptr(fb), bits,
+                                          C.c_float(min_score), C.c_float(max_score), int(two_pass), _ptr(out["dis"]),
+                                          _ptr(out["ids"]), _ptr(out.get("surv")), _ptr(out.get("lo")),
+                                          _ptr(out.get("hi")), _ptr(out.get("state"))), "debug_rerank")
+        return out
+
+    def debug_shadow_rows(self, start, n):
+        """The raw store's int8 shadow rows [start, start + n): (qy int8 [n, cols16], s, e, nrm float32 [n])."""
+        rb = C.c_int64()
+        _check(_lib.lib().gb_debug_shadow_rows(self._h, start, n, None, C.byref(rb)), "debug_shadow_rows")
+        raw = np.empty((n, rb.value), np.uint8)
+        _check(_lib.lib().gb_debug_shadow_rows(self._h, start, n, _ptr(raw), C.byref(rb)), "debug_shadow_rows")
+        cols16 = rb.value - 16
+        meta = raw[:, cols16:].copy().view(np.float32)
+        return raw[:, :cols16].view(np.int8), meta[:, 0].copy(), meta[:, 1].copy(), meta[:, 2].copy()
+
     def set_scan_timing(self, on):
         _lib.lib().gb_index_set_scan_timing(self._h, int(on))
 
