@@ -1674,7 +1674,7 @@ int kmeans_device(const float* x_in, int64_t ldx_in, int64_t n_in, int d, int k,
 
 // ------------------------------------------------------------------------------------------
 IvfIndex::IvfIndex(const std::string& type, int d, const ModelParams& mp, int device, int seg_shift, int row_bytes)
-    : Index(type, d, mp, device, seg_shift, row_bytes), nlist_(mp.ncentroids) {
+    : Index(type, d, mp, device, seg_shift, row_bytes), nlist_(mp.ncentroids), slots_(spilled() ? 2 : 1) {
   mem::dev_malloc(&d_centroids_, (size_t)nlist_ * dpad_ * 4);
   cudaMemset(d_centroids_, 0, (size_t)nlist_ * dpad_ * 4);
   const int64_t ctiles = (nlist_ + 127) / 128;
@@ -1831,21 +1831,19 @@ int IvfIndex::assign_batch(const void* x, int64_t n, const void** xc, int32_t* o
 int IvfIndex::index_batch(const void* x, int64_t n, int64_t vid0, const uint8_t* del_bitmap) {
   cudaStream_t st = build_stream_;
   Scratch s(st);
-  GB_ALLOC(d_assign, int32_t, n, s);
-  if (assign_batch(x, n, &x, d_assign, s)) return -1;
-  const bool spill = spilled();
-  std::vector<int32_t> h_list(n), h_pos(n), h_spill(spill ? n : 0), h_spos(spill ? n : 0);
-  if (spill) {  // the second list of every row, from the same rows and centroids as its primary one
-    GB_ALLOC(d_sp, int32_t, n, s);
-    if (spill_dev(static_cast<const float*>(x), n, d_assign, d_sp, s)) return -1;
-    GB_CUDA(cudaMemcpyAsync(h_spill.data(), d_sp, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-  }
-  GB_CUDA(cudaMemcpyAsync(h_list.data(), d_assign, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+  const int C = copies();
+  // [copies][n]: each row's primary list and position, then (spilled) its spilled ones
+  GB_ALLOC(d_list, int32_t, n * C, s);
+  GB_ALLOC(d_pos, int32_t, n * C, s);
+  if (assign_batch(x, n, &x, d_list, s)) return -1;
+  // the second list of every row, from the same rows and centroids as its primary one
+  if (C > 1 && spill_dev(static_cast<const float*>(x), n, d_list, d_list + n, s)) return -1;
+  std::vector<int32_t> h_list(n * C), h_pos(n * C);
+  GB_CUDA(cudaMemcpyAsync(h_list.data(), d_list, (size_t)n * C * 4, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
   std::vector<int> add(nlist_, 0);
   const std::vector<int>& lens = lists_->lens();
-  if ((int64_t)vid2pos_.size() < vid0 + n) vid2pos_.resize(vid0 + n, ~(uint64_t)0);
-  if (spill && (int64_t)vid2pos2_.size() < vid0 + n) vid2pos2_.resize(vid0 + n, ~(uint64_t)0);
+  slots_.grow(vid0 + n);
   for (int64_t i = 0; i < n; i++) {
     int64_t vid = vid0 + i, gvid = global_vid(vid);
     int l = h_list[i];
@@ -1857,46 +1855,36 @@ int IvfIndex::index_batch(const void* x, int64_t n, int64_t vid0, const uint8_t*
     if (l < 0 || l >= nlist_) l = (int)(gvid % nlist_);  // ivfflat.cc:443-446
     h_list[i] = l;
     h_pos[i] = lens[l] + add[l]++;  // insertion (vid) order inside the list
-    vid2pos_[vid] = ((uint64_t)l << 32) | (uint32_t)h_pos[i];
+    slots_.at(vid)[0] = ((uint64_t)l << 32) | (uint32_t)h_pos[i];
   }
   // the spilled entries after the batch's primary ones, in vid order.  A row without a spilled list (|r| = 0, values
   // not finite, no primary list) takes list gvid % nlist as an unassigned row does, or the next one when that is its
   // primary list
-  for (int64_t i = 0; spill && i < n; i++) {
+  for (int64_t i = 0; C > 1 && i < n; i++) {
     const int64_t vid = vid0 + i, gvid = global_vid(vid);
     const int l = h_list[i];
-    int sl = h_spill[i];
+    int sl = h_list[n + i];
     if (l < 0) {
-      h_spill[i] = -1;
-      h_spos[i] = 0;
+      h_list[n + i] = -1;
+      h_pos[n + i] = 0;
       continue;
     }
     if (sl < 0 || sl >= nlist_ || sl == l) {
       sl = (int)(gvid % nlist_);
       if (sl == l) sl = (int)((gvid + 1) % nlist_);
     }
-    h_spill[i] = sl;
-    h_spos[i] = lens[sl] + add[sl]++;
-    vid2pos2_[vid] = ((uint64_t)sl << 32) | (uint32_t)h_spos[i];
+    h_list[n + i] = sl;
+    h_pos[n + i] = lens[sl] + add[sl]++;
+    slots_.at(vid)[1] = ((uint64_t)sl << 32) | (uint32_t)h_pos[n + i];
   }
-  GB_ALLOC(d_list, int32_t, n, s);
-  GB_ALLOC(d_pos, int32_t, n, s);
-  GB_CUDA(cudaMemcpyAsync(d_list, h_list.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemcpyAsync(d_pos, h_pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  int32_t *d_slist = nullptr, *d_spos = nullptr;
-  if (spill) {
-    d_slist = s.alloc_n<int32_t>(n);
-    d_spos = s.alloc_n<int32_t>(n);
-    if (!d_slist || !d_spos) return -1;
-    GB_CUDA(cudaMemcpyAsync(d_slist, h_spill.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-    GB_CUDA(cudaMemcpyAsync(d_spos, h_spos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  }
+  GB_CUDA(cudaMemcpyAsync(d_list, h_list.data(), (size_t)n * C * 4, cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaMemcpyAsync(d_pos, h_pos.data(), (size_t)n * C * 4, cudaMemcpyHostToDevice, st));
   std::unique_lock<std::shared_mutex> lk(mu_);
   drain_searches();  // kernels of earlier searches read lengths and base pointers at run time
   if (lists_->reserve(add, st)) return -1;
-  // data first, the new lengths last (realtime_mem_data.cc:292-293)
-  if (append_batch(x, n, vid0, d_list, d_pos, add, s)) return -1;
-  if (spill && append_batch(x, n, vid0, d_slist, d_spos, add, s)) return -1;  // codes against the spilled centroids
+  // data first, the new lengths last (realtime_mem_data.cc:292-293); spilled entries are coded against their own lists
+  for (int c = 0; c < C; c++)
+    if (append_batch(x, n, vid0, d_list + (int64_t)c * n, d_pos + (int64_t)c * n, add, s)) return -1;
   if (lists_->commit(add, st)) return -1;
   if (lists_changed(st)) return -1;
   GB_CUDA(cudaStreamSynchronize(st));
@@ -1942,9 +1930,7 @@ int IvfIndex::reset_index() {
   std::unique_lock<std::shared_mutex> lk(mu_);
   cudaDeviceSynchronize();  // kernels of earlier device-resident searches may still read the lists
   lists_.reset();
-  vid2pos_.clear();
-  vid2pos2_.clear();
-  del_counted_.clear();
+  slots_.clear();
   reset_codec();
   indexed_count_ = 0;
   trained_ = false;
@@ -1957,9 +1943,7 @@ void IvfIndex::clear_lists() {
   std::unique_lock<std::shared_mutex> lk(mu_);
   drain_searches();
   if (lists_) lists_.reset(new IvfLists(nlist_, code_bytes()));
-  vid2pos_.clear();
-  vid2pos2_.clear();
-  del_counted_.clear();
+  slots_.clear();
   indexed_count_ = 0;
   if (lists_) lists_changed(build_stream_);
   cudaStreamSynchronize(build_stream_);
@@ -1989,7 +1973,7 @@ int IvfIndex::compact_locked() {
 int IVFFlatIndex::lists_changed(cudaStream_t st) {
   if (!rescore_from_lists() || !lists_) return 0;
   drain_searches();  // no kernel of an earlier search reads the table while it is rewritten or freed
-  const int64_t need = (int64_t)vid2pos_.size();
+  const int64_t need = slots_.size();
   if (need > rowptr_cap_) {
     const int64_t cap = std::max<int64_t>(need, rowptr_cap_ + rowptr_cap_ / 2);
     const float** p = nullptr;
@@ -2024,36 +2008,25 @@ int IvfIndex::update_vector(int64_t vid, const void* x) {
   return reindex_vector(vid, x_dev);
 }
 int IvfIndex::reindex_vector(int64_t vid, const void* x_dev) {
-  if (spilled()) {  // both entries tombstoned, then the row goes to its primary and its spilled list again
+  if (vid >= 0 && vid < slots_.size()) {  // every entry tombstoned, then the row goes to its lists again
     std::unique_lock<std::shared_mutex> lk(mu_);
-    const bool counted = vid < (int64_t)del_counted_.size() && del_counted_[vid];
-    if (counted) del_counted_[vid] = false;
-    for (std::vector<uint64_t>* slots : {&vid2pos_, &vid2pos2_}) {
-      if (vid >= (int64_t)slots->size() || (*slots)[vid] == ~(uint64_t)0) continue;
-      const uint64_t at = (*slots)[vid];
-      if (counted) lists_->add_dead((int)(at >> 32), -1);  // counted as deleted: the tombstone counts it instead
-      if (lists_->tombstone((int)(at >> 32), (int)(uint32_t)at, build_stream_)) return -1;
-      (*slots)[vid] = ~(uint64_t)0;
+    const bool counted = slots_.counted[vid];
+    slots_.counted[vid] = false;
+    uint64_t* at = slots_.at(vid);
+    for (int c = 0; c < copies(); c++) {
+      if (at[c] == VidSlots::kNone) continue;
+      const int l = (int)(at[c] >> 32);
+      if (counted) lists_->add_dead(l, -1);  // counted as deleted: the tombstone counts it instead
+      if (lists_->tombstone(l, (int)(uint32_t)at[c], build_stream_)) return -1;
+      at[c] = VidSlots::kNone;
     }
-    lk.unlock();
-    return index_batch(x_dev, 1, vid, nullptr);
-  }
-  if (vid < (int64_t)vid2pos_.size() && vid2pos_[vid] != ~(uint64_t)0) {
-    std::unique_lock<std::shared_mutex> lk(mu_);
-    const int l = (int)(vid2pos_[vid] >> 32);
-    if (vid < (int64_t)del_counted_.size() && del_counted_[vid]) {  // counted as deleted: the tombstone counts it instead
-      del_counted_[vid] = false;
-      lists_->add_dead(l, -1);
-    }
-    if (lists_->tombstone(l, (int)(uint32_t)vid2pos_[vid], build_stream_)) return -1;
   }
   return index_batch(x_dev, 1, vid, nullptr);
 }
 
 int IvfIndex::vid_slots(int64_t vid, uint64_t* out) {
   std::lock_guard<std::mutex> bg(build_mu_);
-  out[0] = vid >= 0 && vid < (int64_t)vid2pos_.size() ? vid2pos_[vid] : ~(uint64_t)0;
-  out[1] = vid >= 0 && vid < (int64_t)vid2pos2_.size() ? vid2pos2_[vid] : ~(uint64_t)0;
+  for (int c = 0; c < 2; c++) out[c] = slots_.get(vid, c);
   return 0;
 }
 
@@ -2062,22 +2035,13 @@ int IvfIndex::delete_vectors(const int64_t* vids, int64_t n) {
   if (!lists_) return 0;
   for (int64_t i = 0; i < n; i++) {
     const int64_t vid = vids[i];
-    if (spilled()) {  // a dead entry in each list that holds one
-      const uint64_t a = vid >= 0 && vid < (int64_t)vid2pos_.size() ? vid2pos_[vid] : ~(uint64_t)0;
-      const uint64_t b = vid >= 0 && vid < (int64_t)vid2pos2_.size() ? vid2pos2_[vid] : ~(uint64_t)0;
-      if (a == ~(uint64_t)0 && b == ~(uint64_t)0) continue;
-      if ((int64_t)del_counted_.size() <= vid) del_counted_.resize(std::max(vid2pos_.size(), vid2pos2_.size()), false);
-      if (del_counted_[vid]) continue;
-      del_counted_[vid] = true;
-      if (a != ~(uint64_t)0) lists_->add_dead((int)(a >> 32), 1);
-      if (b != ~(uint64_t)0) lists_->add_dead((int)(b >> 32), 1);
-      continue;
+    if (vid < 0 || vid >= slots_.size() || slots_.counted[vid]) continue;
+    for (int c = 0; c < copies(); c++) {  // a dead entry in each list that holds one (realtime_mem_data.cc:194)
+      const uint64_t at = slots_.at(vid)[c];
+      if (at == VidSlots::kNone) continue;
+      lists_->add_dead((int)(at >> 32), 1);
+      slots_.counted[vid] = true;
     }
-    if (vid < 0 || vid >= (int64_t)vid2pos_.size() || vid2pos_[vid] == ~(uint64_t)0) continue;
-    if (del_counted_.size() < vid2pos_.size()) del_counted_.resize(vid2pos_.size(), false);
-    if (del_counted_[vid]) continue;
-    del_counted_[vid] = true;
-    lists_->add_dead((int)(vid2pos_[vid] >> 32), 1);  // realtime_mem_data.cc:194
   }
   return 0;
 }
@@ -2120,53 +2084,34 @@ int IvfIndex::purge_locked(const std::vector<int>& sel, const uint32_t* d_del_bi
   for (int l : sel) purged[l] = 1;
   drain_searches();  // kernels of earlier searches read lengths and base pointers at run time
   IvfLists::Purged pg;
-  if (lists_->purge(sel, d_del_bits, st, &pg, spilled() ? 2 : 1)) return -1;
+  const int C = copies();
+  if (lists_->purge(sel, d_del_bits, st, &pg, C)) return -1;
   if (pg.dropped == 0) return 0;
-  if (spilled()) {
-    // both slots of every vid with an entry in a purged list: the new entry in the same list (a vid's two entries are in
-    // two lists), ~0 if it was dropped
-    const int64_t span = (int64_t)pg.newpos.size() / 2;
-    const int64_t top = std::min<int64_t>((int64_t)vid2pos_.size(), pg.vid_min + span);
-    for (int64_t vid = pg.vid_min; vid < top; vid++) {
-      const uint64_t* np = &pg.newpos[2 * (vid - pg.vid_min)];
-      bool moved = false, left = false;
-      for (std::vector<uint64_t>* slots : {&vid2pos_, &vid2pos2_}) {
-        if (vid >= (int64_t)slots->size()) continue;
-        uint64_t& at = (*slots)[vid];
-        if (at == ~(uint64_t)0) continue;
-        if (!purged[at >> 32]) {
-          left = true;
-          continue;
-        }
-        const uint64_t now = (np[0] >> 32) == (at >> 32) ? np[0] : (np[1] >> 32) == (at >> 32) ? np[1] : ~(uint64_t)0;
-        at = now;
-        moved = true;
-        if (now != ~(uint64_t)0) {
-          left = true;
-          if (vid < (int64_t)del_counted_.size() && del_counted_[vid]) lists_->add_dead((int)(now >> 32), 1);
-        }
+  // every slot in a purged list, from the table the scatter wrote: the vid's new entry in the same list (a vid's entries
+  // are in distinct lists), ~0 if it was dropped
+  const int64_t top = std::min<int64_t>(slots_.size(), pg.vid_min + (int64_t)pg.newpos.size() / C);
+  for (int64_t vid = pg.vid_min; vid < top; vid++) {
+    const uint64_t* np = &pg.newpos[(size_t)(vid - pg.vid_min) * C];
+    uint64_t* at = slots_.at(vid);
+    bool moved = false, left = false;
+    for (int c = 0; c < C; c++) {
+      if (at[c] == VidSlots::kNone) continue;
+      const uint64_t l = at[c] >> 32;
+      if (!purged[l]) {
+        left = true;
+        continue;
       }
-      if (moved && !left && vid < (int64_t)del_counted_.size()) del_counted_[vid] = false;
+      uint64_t now = VidSlots::kNone;
+      for (int j = 0; j < C && now == VidSlots::kNone; j++)
+        if ((np[j] >> 32) == l) now = np[j];
+      at[c] = now;
+      moved = true;
+      if (now != VidSlots::kNone) {
+        left = true;
+        if (slots_.counted[vid]) lists_->add_dead((int)l, 1);  // deleted, but not in this bitmap: still there, still counted
+      }
     }
-    if (lists_changed(st)) return -1;
-    GB_CUDA(cudaStreamSynchronize(st));
-    if (dropped) *dropped = pg.dropped;
-    if (lists_->compact_due() && compact_locked()) return -1;
-    return 0;
-  }
-  // vid_bucket_no_pos_ of every vid that was in a purged list, from the table the scatter wrote
-  const int64_t hi = std::min<int64_t>((int64_t)vid2pos_.size(), pg.vid_min + (int64_t)pg.newpos.size());
-  for (int64_t vid = pg.vid_min; vid < hi; vid++) {
-    const uint64_t old = vid2pos_[vid];
-    if (old == ~(uint64_t)0 || !purged[old >> 32]) continue;
-    const uint64_t now = pg.newpos[vid - pg.vid_min];
-    vid2pos_[vid] = now;
-    if (vid < (int64_t)del_counted_.size() && del_counted_[vid]) {
-      if (now == ~(uint64_t)0)
-        del_counted_[vid] = false;
-      else
-        lists_->add_dead((int)(now >> 32), 1);  // deleted, but not in this bitmap: still there, still counted
-    }
+    if (moved && !left) slots_.counted[vid] = false;
   }
   if (lists_changed(st)) return -1;
   GB_CUDA(cudaStreamSynchronize(st));

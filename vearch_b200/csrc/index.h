@@ -757,10 +757,32 @@ class IvfIndex : public Index {
   // after every change of d_centroids_ (the end of rebuild_centroid_tiles), with mu_ held exclusively, ordered on st
   virtual int centroids_changed(cudaStream_t st) { (void)st; return 0; }
   std::unique_ptr<IvfLists> lists_;
-  std::vector<uint64_t> vid2pos_;  // vid -> (list << 32 | pos), ~0 = not in a list (vid_bucket_no_pos_)
-  // spilled: vid's other entry, as vid2pos_ (~0 = none).  The two slots are equal: neither is known as the primary one.
-  std::vector<uint64_t> vid2pos2_;
-  std::vector<bool> del_counted_;  // vid's entries are counted dead by delete_vectors (so they are counted once)
+  // vid_bucket_no_pos_: each vid's `copies` list entries as (list << 32 | pos), kNone = none.  copies is 2 for a spilled
+  // index (slot 0 the primary entry, slot 1 the spilled one), 1 otherwise; counted: delete_vectors counted the vid's
+  // entries dead (so they are counted once)
+  struct VidSlots {
+    static constexpr uint64_t kNone = ~(uint64_t)0;
+    int copies;
+    std::vector<uint64_t> pos;  // [vid][copies]
+    std::vector<bool> counted;
+    explicit VidSlots(int copies) : copies(copies) {}
+    int64_t size() const { return (int64_t)counted.size(); }
+    void grow(int64_t n) {
+      if (n <= size()) return;
+      pos.resize((size_t)n * copies, kNone);
+      counted.resize((size_t)n, false);
+    }
+    uint64_t* at(int64_t vid) { return &pos[(size_t)vid * copies]; }  // 0 <= vid < size()
+    uint64_t get(int64_t vid, int c) const {
+      return vid >= 0 && vid < size() && c < copies ? pos[(size_t)vid * copies + c] : kNone;
+    }
+    void clear() {
+      pos.clear();
+      counted.clear();
+    }
+  };
+  VidSlots slots_;
+  int copies() const { return slots_.copies; }
 };
 
 // GammaIVFFlatIndex (index/impl/gamma_index_ivfflat.{h,cc}): the lists hold the raw fp32 rows.  type: "IVFFLAT", or

@@ -421,7 +421,7 @@ int IvfIndex::load_gamma_part(const std::string& dir, const std::string& abs_nam
   }
   std::vector<uint8_t> codes, padded;
   int64_t live = 0, max_vid = -1;
-  std::vector<uint64_t> v2p, v2p2;  // vid_bucket_no_pos_ (spilled: and the second entries), installed only if the whole file loads
+  VidSlots v2p(copies());  // installed only if the whole file loads
   std::vector<int> dead(nlist_, 0);
   const size_t my_cb = (size_t)code_bytes();
   for (int l = 0; l < nlist_; l++) {
@@ -457,15 +457,15 @@ int IvfIndex::load_gamma_part(const std::string& dir, const std::string& abs_nam
       }
       live++;
       max_vid = std::max(max_vid, id);
-      if ((size_t)id >= v2p.size()) v2p.resize(std::max<size_t>((size_t)id + 1, v2p.size() * 2), ~(uint64_t)0);
-      if (spilled() && v2p[id] != ~(uint64_t)0) {  // the vid's other live entry
-        if ((size_t)id >= v2p2.size()) v2p2.resize(std::max<size_t>((size_t)id + 1, v2p2.size() * 2), ~(uint64_t)0);
-        if (v2p2[id] != ~(uint64_t)0) return fail("vid " + std::to_string(id) + " has more than two live entries in " + path);
-        if ((v2p[id] >> 32) == (uint64_t)l) return fail("vid " + std::to_string(id) + " has two live entries in list " + std::to_string(l) + " of " + path);
-        v2p2[id] = (uint64_t)l << 32 | (uint64_t)pos;
-        continue;
-      }
-      v2p[id] = (uint64_t)l << 32 | (uint64_t)pos;
+      if (id >= v2p.size()) v2p.grow(std::max(id + 1, v2p.size() * 2));
+      // the vid's live entries in file order fill its slots; an unspilled vid's later entry replaces the earlier one
+      uint64_t* at = v2p.at(id);
+      int c = 0;
+      while (c + 1 < copies() && at[c] != VidSlots::kNone) c++;
+      if (c > 0 && at[c] != VidSlots::kNone) return fail("vid " + std::to_string(id) + " has more than two live entries in " + path);
+      for (int j = 0; j < c; j++)
+        if ((at[j] >> 32) == (uint64_t)l) return fail("vid " + std::to_string(id) + " has two live entries in list " + std::to_string(l) + " of " + path);
+      at[c] = (uint64_t)l << 32 | (uint64_t)pos;
     }
   }
   int64_t indexed = live;  // IwPQ: ReadInvertedLists' running count (total - tombstones)
@@ -483,8 +483,7 @@ int IvfIndex::load_gamma_part(const std::string& dir, const std::string& abs_nam
   {  // publish: nothing above this point changed what a search can see
     std::unique_lock<std::shared_mutex> lk(mu_);
     if (lists_->commit(add, st)) return -1;
-    vid2pos_.swap(v2p);
-    vid2pos2_.swap(v2p2);
+    std::swap(slots_, v2p);
     for (int l = 0; l < nlist_; l++) lists_->add_dead(l, dead[l]);
     if (lists_changed(st)) return -1;  // IVF-Flat on a host store: the row pointers into the loaded lists
     GB_CUDA(cudaStreamSynchronize(st));
