@@ -176,6 +176,29 @@ int gb_index_mirror_builds(gb_index *index);
  * x - s_l and y - s_l.  s_l = round(c_l / g_l) * g_l with g_l the largest power of two <= rho_l / sqrt(d) and rho_l half
  * the distance from centroid c_l to its nearest other centroid; s_l = c_l when rho_l = 0 */
 int gb_index_get_list_shifts(gb_index *index, float *out);
+/* Test hooks over the caches the list-major scans keep beside the lists (DESIGN.md section 3, cache freshness).  None
+ * changes index state: each holds the index locks shared and writes only scratch and the caller's buffers.  They take an
+ * unsharded index or a shard handle (gb_index_shard).
+ * gb_debug_mirror (IVFFLAT, GPU_IVFFLAT): list `list`'s first ceil(len / 128) tensor-core mirror tiles, *tile_floats
+ * floats each (the hi then the lo operand of 128 rows), into tiles, and their 128 row norms each into norms, from the
+ * live mirror; gb_debug_mirror_rebuilt: the same tiles as a build from the lists into scratch writes them, the live
+ * mirror left as it is.  *ntiles = tiles written (at most max_tiles; none when tiles is NULL, or the live mirror does
+ * not exist); *state (both) bit 0: the live mirror is current, bit 1: it is disabled (HBM too full).
+ * gb_debug_rowptr_rows (IVFFLAT on a "RocksDB" store, or a shard of GPU_IVFFLAT): the rows the winner re-score's
+ * row-pointer table points at for vids [v0, v0 + n) (a shard's local vids), rows [n][d]; state[i] 0: an entry of a
+ * list, 1: null, 2: points at no list entry (row zeroed where state != 0).
+ * gb_debug_pq_norms (IVFPQ at 8 bits): list `list`'s cached |r_e|^2 segment (live, the first min(*len, cached length)
+ * entries) and the same segment recomputed from the lists and codebook into scratch (recomputed, *len entries; *len =
+ * the list's length); *current: the cache's key matches the lists and the codebook.  live / recomputed may be NULL.
+ * gb_debug_pq_tables (IVFPQ at 8 bits): the tensor-core filter's int8 codebook cb8 [M][256][dsub] and cbnrm
+ * [M * 256 + 4]: |pq[m][c]|^2, then R^2, sb, D and one unused float. */
+int gb_debug_mirror(gb_index *index, int list, int64_t max_tiles, float *tiles, float *norms, int64_t *ntiles,
+                    int64_t *tile_floats, int *state);
+int gb_debug_mirror_rebuilt(gb_index *index, int list, int64_t max_tiles, float *tiles, float *norms, int64_t *ntiles,
+                            int64_t *tile_floats, int *state);
+int gb_debug_rowptr_rows(gb_index *index, int64_t v0, int64_t n, float *rows, int *state);
+int gb_debug_pq_norms(gb_index *index, int list, float *live, float *recomputed, int64_t *len, int *current);
+int gb_debug_pq_tables(gb_index *index, int8_t *cb8, float *cbnrm);
 /* test hook (IVF types): the kernel(s) of the last coarse search: "coarse_topk_kernel" (fused), or the score matrix of
  * "dist_tc_kernel+select_rows_kernel" (>= 32 queries) or "dist_tile_kernel+select_rows_kernel" (exact) */
 const char *gb_index_last_coarse_kernel(gb_index *index);

@@ -102,6 +102,11 @@ def _declare(l):
     l.gb_index_compact.argtypes = [vp]
     l.gb_index_mirror_builds.argtypes = [vp]
     l.gb_index_get_list_shifts.argtypes = [vp, vp]
+    l.gb_debug_mirror.argtypes = [vp, i32, i64, vp, vp, vp, vp, vp]
+    l.gb_debug_mirror_rebuilt.argtypes = [vp, i32, i64, vp, vp, vp, vp, vp]
+    l.gb_debug_rowptr_rows.argtypes = [vp, i64, i64, vp, vp]
+    l.gb_debug_pq_norms.argtypes = [vp, i32, vp, vp, vp, vp]
+    l.gb_debug_pq_tables.argtypes = [vp, vp, vp]
     l.gb_index_last_coarse_kernel.argtypes = [vp]
     l.gb_index_last_coarse_kernel.restype = cstr
     l.gb_index_load.argtypes = [vp, cstr, cstr, vp]

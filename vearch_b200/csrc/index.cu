@@ -735,6 +735,19 @@ int IvfLists::download_list(int l, std::vector<uint8_t>* codes, std::vector<int6
   }
   return 0;
 }
+bool IvfLists::locate(const void* p, int* list, int* pos) const {
+  const char* c = static_cast<const char*>(p);
+  for (int l = 0; l < nlist_; l++) {
+    const char* b = static_cast<const char*>(h_data_[l]);
+    if (!b || c < b) continue;
+    const int64_t off = c - b;
+    if (off >= (int64_t)h_len_[l] * code_bytes_ || off % code_bytes_) continue;
+    *list = l;
+    *pos = (int)(off / code_bytes_);
+    return true;
+  }
+  return false;
+}
 
 // ------------------------------------------------------------------------------------------
 namespace {
@@ -2206,7 +2219,7 @@ int IVFFlatIndex::mirror_append(const float* x, int64_t n, const int32_t* d_list
   if (!mirror_.base || mirror_.disabled || mirror_.lens.size() != (size_t)nlist_) return 0;
   std::vector<int> lens = lists_->lens();  // lengths BEFORE this batch is committed
   for (int l = 0; l < nlist_; l++) {
-    if (mirror_.lens[l] != lens[l] || mirror_.content_gen != lists_->content_gen() ||
+    if (mirror_.lens[l] != lens[l] || mirror_.lists_uid != lists_->uid() || mirror_.content_gen != lists_->content_gen() ||
         (int64_t)lens[l] + add[l] > (int64_t)mirror_.list_tiles[l] * 128) {
       mirror_.lens.clear();  // stale: outgrown, purged or out of step; rebuilt by the next list-major search
       return 0;
@@ -2271,6 +2284,7 @@ int IVFFlatIndex::ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStr
         GB_CUDA(cudaStreamSynchronize(st));  // tile0 is a stack vector; other streams may use the mirror next
         mirror_.tiles = tiles;
         mirror_.lens = lens;
+        mirror_.lists_uid = lists_->uid();
         mirror_.content_gen = lists_->content_gen();
         mirror_.builds++;
       }
@@ -2279,6 +2293,85 @@ int IVFFlatIndex::ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStr
   lk.lock();
   if (mirror_.disabled) return 1;
   return mirror_current() ? 0 : 1;
+}
+
+// Test hooks.  They change nothing a search or a mutation reads: the index locks are held shared, the rebuild goes to
+// scratch on a stream of its own.
+int IVFFlatIndex::debug_mirror(int l, bool rebuilt, int64_t max_tiles, float* tiles, float* norms, int64_t* ntiles,
+                               int64_t* tile_floats, int* state) {
+  if (l < 0 || l >= nlist_) {
+    set_last_error("debug_mirror: no such list");
+    return -1;
+  }
+  cudaSetDevice(device_);
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  std::shared_lock<std::shared_mutex> ml(mirror_rw_);
+  const int k16 = (int)round_up(dpad_, 16);
+  const int64_t tf = tc_mirror_tile_floats(k16);
+  *tile_floats = tf;
+  *ntiles = 0;
+  *state = (mirror_.disabled ? kMirrorDisabled : 0) | (lists_ && mirror_current() ? kMirrorCurrent : 0);
+  if (!lists_ || !tiles || !norms) return 0;
+  const std::vector<int>& lens = lists_->lens();
+  int64_t nt = std::min<int64_t>((lens[l] + 127) / 128, max_tiles);
+  if (nt <= 0) return 0;
+  if (!rebuilt) {
+    if (!mirror_.base || mirror_.list_tiles.size() != (size_t)nlist_) return 0;
+    int64_t t0 = 0;
+    for (int j = 0; j < l; j++) t0 += mirror_.list_tiles[j];
+    nt = std::min<int64_t>(nt, mirror_.list_tiles[l]);
+    GB_CUDA(cudaMemcpy(tiles, mirror_.base + t0 * tf, (size_t)(nt * tf) * 4, cudaMemcpyDeviceToHost));
+    GB_CUDA(cudaMemcpy(norms, mirror_.norms + t0 * 128, (size_t)nt * 128 * 4, cudaMemcpyDeviceToHost));
+    *ntiles = nt;
+    return 0;
+  }
+  std::vector<int64_t> tile0(nlist_ + 1, 0);  // no slack: every list's tiles end at its last row's
+  for (int j = 0; j < nlist_; j++) tile0[j + 1] = tile0[j] + (lens[j] + 127) / 128;
+  cudaStream_t st;
+  GB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  auto build = [&]() -> int {
+    Scratch s(st);
+    GB_ALLOC(d_tile0, int64_t, nlist_ + 1, s);
+    GB_ALLOC(mt, float, (size_t)(tile0[nlist_] * tf), s);
+    GB_ALLOC(mn, float, (size_t)tile0[nlist_] * 128, s);
+    GB_CUDA(cudaMemcpyAsync(d_tile0, tile0.data(), sizeof(int64_t) * (nlist_ + 1), cudaMemcpyHostToDevice, st));
+    GB_CUDA(launch_tc_mirror_build(lists_->directory(), dpad_, k16, d_tile0, tile0[nlist_], d_shifts_, mt, mn, st));
+    GB_CUDA(cudaMemcpyAsync(tiles, mt + tile0[l] * tf, (size_t)(nt * tf) * 4, cudaMemcpyDeviceToHost, st));
+    GB_CUDA(cudaMemcpyAsync(norms, mn + tile0[l] * 128, (size_t)nt * 128 * 4, cudaMemcpyDeviceToHost, st));
+    GB_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  };
+  const int rc = build();
+  cudaStreamSynchronize(st);
+  cudaStreamDestroy(st);
+  if (!rc) *ntiles = nt;
+  return rc;
+}
+
+int IVFFlatIndex::debug_rowptr_rows(int64_t v0, int64_t n, float* rows, int* state) {
+  cudaSetDevice(device_);
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  if (!rescore_from_lists() || !lists_) {
+    set_last_error("debug_rowptr_rows: no row-pointer table (an HBM store of an unsharded index, or untrained)");
+    return -1;
+  }
+  if (v0 < 0 || n < 0) {
+    set_last_error("debug_rowptr_rows: negative range");
+    return -1;
+  }
+  std::vector<const float*> p((size_t)n, nullptr);
+  const int64_t have = std::max<int64_t>(0, std::min<int64_t>(n, rowptr_cap_ - v0));
+  if (have > 0) GB_CUDA(cudaMemcpy(p.data(), d_rowptr_ + v0, (size_t)have * sizeof(float*), cudaMemcpyDeviceToHost));
+  for (int64_t i = 0; i < n; i++) {
+    float* row = rows + i * d_;
+    int l = 0, pos = 0;
+    state[i] = !p[i] ? kRowNull : lists_->locate(p[i], &l, &pos) ? kRowLive : kRowStray;
+    if (state[i] == kRowLive)  // only a pointer at an entry of the lists is read
+      GB_CUDA(cudaMemcpy(row, p[i], (size_t)d_ * 4, cudaMemcpyDeviceToHost));
+    else
+      std::fill(row, row + d_, 0.f);
+  }
+  return 0;
 }
 
 int IVFFlatIndex::scan_listmajor_dev(const FilterArgs& f, int metric, int nq, const float* xq, int k,
@@ -2835,6 +2928,11 @@ int IVFPQIndex::codebook_changed(cudaStream_t st) {
   GB_CUDA(launch_pq_precompute_table(d_centroids_, dpad_, nlist_, d_pq_, M_, dsub_, d_table_, st, ksub_));
   return 0;
 }
+int IVFPQIndex::centroids_changed(cudaStream_t st) {
+  if (!d_table_) return 0;  // no codebook yet: codebook_changed builds the table once there is one
+  GB_CUDA(launch_pq_precompute_table(d_centroids_, dpad_, nlist_, d_pq_, M_, dsub_, d_table_, st, ksub_));
+  return 0;
+}
 int IVFPQIndex::get_precomputed_table(float* host) const {
   if (!d_table_) {
     set_last_error("no precomputed table (IP metric or untrained)");
@@ -2912,6 +3010,62 @@ int IVFPQIndex::ensure_pq_norms(cudaStream_t st) {
   pqn_.lists_uid = lists_->uid();
   pqn_.content_gen = lists_->content_gen();
   pqn_.pq_gen = pq_gen_;
+  return 0;
+}
+
+// Test hooks: the index locks held shared, the recomputation in scratch on a stream of its own
+int IVFPQIndex::debug_pq_norms(int l, float* live, float* recomputed, int64_t* len, int* current) {
+  if (l < 0 || l >= nlist_) {
+    set_last_error("debug_pq_norms: no such list");
+    return -1;
+  }
+  cudaSetDevice(device_);
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  std::lock_guard<std::mutex> g(pqn_mu_);
+  if (!lists_ || !d_cbnrm_) {
+    set_last_error("debug_pq_norms: no tensor-core filter tables (untrained, or codes below 8 bits)");
+    return -1;
+  }
+  const std::vector<int>& lens = lists_->lens();
+  *len = lens[l];
+  *current = pqn_.base && pqn_.lists_uid == lists_->uid() && pqn_.content_gen == lists_->content_gen() &&
+             pqn_.pq_gen == pq_gen_ && pqn_.lens == lens;
+  if (live && pqn_.base && pqn_.lens.size() == (size_t)nlist_) {
+    int64_t o = 0;
+    for (int j = 0; j < l; j++) o += round_up(pqn_.lens[j], 32);
+    const int n = std::min(lens[l], pqn_.lens[l]);
+    if (n > 0) GB_CUDA(cudaMemcpy(live, pqn_.base + o, (size_t)n * 4, cudaMemcpyDeviceToHost));
+  }
+  if (!recomputed || lens[l] == 0) return 0;
+  std::vector<int64_t> off((size_t)nlist_ + 1, 0);
+  for (int j = 0; j < nlist_; j++) off[j + 1] = off[j] + round_up(lens[j], 32);
+  cudaStream_t st;
+  GB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  auto recompute = [&]() -> int {
+    Scratch s(st);
+    GB_ALLOC(d_off, int64_t, nlist_ + 1, s);
+    GB_ALLOC(out, float, (size_t)off[nlist_], s);
+    GB_CUDA(cudaMemcpyAsync(d_off, off.data(), sizeof(int64_t) * (nlist_ + 1), cudaMemcpyHostToDevice, st));
+    GB_CUDA(launch_pq_entry_norms(lists_->directory(), nlist_, lists_->max_len(), M_, d_cbnrm_, d_off, out, st));
+    GB_CUDA(cudaMemcpyAsync(recomputed, out + off[l], (size_t)lens[l] * 4, cudaMemcpyDeviceToHost, st));
+    GB_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  };
+  const int rc = recompute();
+  cudaStreamSynchronize(st);
+  cudaStreamDestroy(st);
+  return rc;
+}
+
+int IVFPQIndex::debug_pq_tables(int8_t* cb8, float* cbnrm) {
+  cudaSetDevice(device_);
+  std::shared_lock<std::shared_mutex> lk(mu_);
+  if (!d_cb8_ || !d_cbnrm_) {
+    set_last_error("debug_pq_tables: no tensor-core filter tables (untrained, or codes below 8 bits)");
+    return -1;
+  }
+  GB_CUDA(cudaMemcpy(cb8, d_cb8_, (size_t)M_ * 256 * dsub_, cudaMemcpyDeviceToHost));
+  GB_CUDA(cudaMemcpy(cbnrm, d_cbnrm_, ((size_t)M_ * 256 + 4) * 4, cudaMemcpyDeviceToHost));
   return 0;
 }
 

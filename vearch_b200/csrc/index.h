@@ -163,6 +163,9 @@ class IvfLists {
   int tombstone(int list, int pos, cudaStream_t st);
   // host copies for parity tests
   int download_list(int l, std::vector<uint8_t>* codes, std::vector<int64_t>* ids) const;
+  // test hook: the list and position of the entry (below its list's length) whose code starts at device address p;
+  // false if no entry's does
+  bool locate(const void* p, int* list, int* pos) const;
   // a capture (stage.h): every list in the index file's order, each its codes cut to file_cb bytes then its ids, takes
   // pack_bytes(file_cb) bytes; pack_chunks appends the chunks that copy them to dst (launch_list_pack)
   int64_t pack_bytes(int file_cb) const;
@@ -796,6 +799,18 @@ class IVFFlatIndex : public IvfIndex {
   void charge_index_rows(int64_t rows, std::vector<mem::Charge>* out) override;  // and its mirror row, while kept
   int mirror_builds() const { return mirror_.builds; }  // test hook
   int get_list_shifts(float* host) const;               // test hook: d_shifts_ as [nlist][d] (L2 indexes only)
+  // Test hooks; they hold mu_ (and mirror_rw_) shared and write only scratch and the caller's buffers.
+  // debug_mirror: list l's first ceil(len / 128) mirror tiles (hi and lo, *tile_floats floats each) and their 128 row
+  // norms each, as the live mirror holds them or (rebuilt) as launch_tc_mirror_build writes them from the lists into
+  // scratch; *ntiles = the tiles written (at most max_tiles; tiles == nullptr: none), *state = kMirrorCurrent |
+  // kMirrorDisabled bits of the live mirror
+  enum { kMirrorCurrent = 1, kMirrorDisabled = 2 };
+  int debug_mirror(int l, bool rebuilt, int64_t max_tiles, float* tiles, float* norms, int64_t* ntiles,
+                   int64_t* tile_floats, int* state);
+  // debug_rowptr_rows: the rows the winner re-score's row-pointer table holds for vids [v0, v0 + n), into rows [n][d];
+  // state[i] = kRowLive (an entry of a list, below its length), kRowNull or kRowStray (points at no such entry; row zeroed)
+  enum { kRowLive = 0, kRowNull = 1, kRowStray = 2 };
+  int debug_rowptr_rows(int64_t v0, int64_t n, float* rows, int* state);
 
  protected:
   GammaFileFormat gamma_format() const override;
@@ -833,6 +848,7 @@ class IVFFlatIndex : public IvfIndex {
     int64_t* d_tile0 = nullptr;
     int64_t tiles = 0, cap_tiles = 0;
     std::vector<int> lens;        // rows mirrored per list
+    uint64_t lists_uid = 0;       // IvfLists::uid() of the list set mirrored: a Load may refill new lists to the old lengths
     uint64_t content_gen = 0;     // IvfLists::content_gen() they were mirrored at: a purge moves rows inside lists
     std::vector<int> list_tiles;  // tiles reserved per list (a little slack, so appends go in place)
     bool disabled = false;
@@ -845,7 +861,8 @@ class IVFFlatIndex : public IvfIndex {
   std::shared_mutex mirror_rw_;  // taken after mu_
   int ensure_mirror(std::shared_lock<std::shared_mutex>& lk, cudaStream_t st);  // 0 = usable and current
   bool mirror_current() const {
-    return mirror_.base && mirror_.lens == lists_->lens() && mirror_.content_gen == lists_->content_gen();
+    return mirror_.base && mirror_.lists_uid == lists_->uid() && mirror_.lens == lists_->lens() &&
+           mirror_.content_gen == lists_->content_gen();
   }
 };
 
@@ -906,6 +923,7 @@ class IVFPQIndex : public IvfPqBase {
   cudaError_t encode_dev(const float* x, int64_t n, const int32_t* lists, uint8_t* codes, cudaStream_t st) override;
   int train_extra(const float* xtrain, int64_t n, Scratch& s) override;
   int codebook_changed(cudaStream_t st) override;
+  int centroids_changed(cudaStream_t st) override;  // the L2 table holds <c_l, pq>: it follows the centroids too
   // list-major scan through the tensor-core filter (kernels_pqtc.cu); 1 = not applicable
   int scan_listmajor_pq(const FilterArgs& f, int metric, int nq, const float* xq, int kk, float* ip,
                         const int32_t* probe_ids, const float* coarse_dis, int nprobe, unsigned long long* adc_out,
@@ -936,6 +954,12 @@ class IVFPQIndex : public IvfPqBase {
   bool opq_trained_ = false;
 
  public:
+  // Test hooks; they hold mu_ shared and write only scratch and the caller's buffers.  debug_pq_norms: list l's |r_e|^2
+  // segment as the cache holds it (live; its first min(*len, cached length) entries) and as launch_pq_entry_norms
+  // recomputes it from the lists into scratch (recomputed, *len entries, *len = the list's length); *current = the
+  // cache's key matches the lists and the codebook.  debug_pq_tables: d_cb8_ [M][256][dsub] and d_cbnrm_ [M * 256 + 4]
+  int debug_pq_norms(int l, float* live, float* recomputed, int64_t* len, int* current);
+  int debug_pq_tables(int8_t* cb8, float* cbnrm);
   bool has_opq() const { return d_opq_ != nullptr; }
   int set_opq(const float* host_A);        // d x d row-major; marks the rotation trained
   int get_opq(float* host_A) const;

@@ -598,6 +598,36 @@ int gb_index_get_list_shifts(gb_index* index, float* out) {
   STATE_OR_FAIL(IVFFlatIndex, ivf, index, "IVFFLAT");
   return ivf->get_list_shifts(out);
 }
+// the cache hooks read one index's own structures: a sharded index answers through its shard handles
+static int debug_mirror(gb_index* index, int list, bool rebuilt, int64_t max_tiles, float* tiles, float* norms,
+                        int64_t* ntiles, int64_t* tile_floats, int* state) {
+  AS_OR_FAIL(IVFFlatIndex, ivf, index, "IVFFLAT (or a shard of a sharded GPU_IVFFLAT)");
+  if (!ntiles || !tile_floats || !state) return -1;
+  return ivf->debug_mirror(list, rebuilt, max_tiles, tiles, norms, ntiles, tile_floats, state);
+}
+int gb_debug_mirror(gb_index* index, int list, int64_t max_tiles, float* tiles, float* norms, int64_t* ntiles,
+                    int64_t* tile_floats, int* state) {
+  return debug_mirror(index, list, false, max_tiles, tiles, norms, ntiles, tile_floats, state);
+}
+int gb_debug_mirror_rebuilt(gb_index* index, int list, int64_t max_tiles, float* tiles, float* norms, int64_t* ntiles,
+                            int64_t* tile_floats, int* state) {
+  return debug_mirror(index, list, true, max_tiles, tiles, norms, ntiles, tile_floats, state);
+}
+int gb_debug_rowptr_rows(gb_index* index, int64_t v0, int64_t n, float* rows, int* state) {
+  AS_OR_FAIL(IVFFlatIndex, ivf, index, "IVFFLAT (or a shard of a sharded GPU_IVFFLAT)");
+  if (n > 0 && (!rows || !state)) return -1;
+  return ivf->debug_rowptr_rows(v0, n, rows, state);
+}
+int gb_debug_pq_norms(gb_index* index, int list, float* live, float* recomputed, int64_t* len, int* current) {
+  AS_OR_FAIL(IVFPQIndex, pq, index, "IVFPQ (or a shard of a sharded GPU_IVFPQ)");
+  if (!len || !current) return -1;
+  return pq->debug_pq_norms(list, live, recomputed, len, current);
+}
+int gb_debug_pq_tables(gb_index* index, int8_t* cb8, float* cbnrm) {
+  AS_OR_FAIL(IVFPQIndex, pq, index, "IVFPQ (or a shard of a sharded GPU_IVFPQ)");
+  if (!cb8 || !cbnrm) return -1;
+  return pq->debug_pq_tables(cb8, cbnrm);
+}
 const char* gb_index_last_coarse_kernel(gb_index* index) {
   IvfIndex* ivf = state_of<IvfIndex>(index);
   return ivf ? ivf->last_coarse_kernel() : "";

@@ -405,6 +405,56 @@ class GammaIndex:
         _check(_lib.lib().gb_index_get_list_shifts(self._h, _ptr(out)), "get_list_shifts")
         return out
 
+    MIRROR_CURRENT, MIRROR_DISABLED = 1, 2  # debug_mirror's state bits
+    ROW_LIVE, ROW_NULL, ROW_STRAY = 0, 1, 2  # debug_rowptr_rows' per-vid states
+
+    def _debug_mirror(self, fn, l):
+        nt, tf, st = C.c_int64(), C.c_int64(), C.c_int32()
+        _check(fn(self._h, int(l), 0, None, None, C.byref(nt), C.byref(tf), C.byref(st)), "debug_mirror")
+        want = (self.list_len(l) + 127) // 128
+        tiles, norms = np.zeros((want, tf.value), np.float32), np.zeros((want, 128), np.float32)
+        _check(fn(self._h, int(l), want, _ptr(tiles), _ptr(norms), C.byref(nt), C.byref(tf), C.byref(st)), "debug_mirror")
+        return {"tiles": tiles[:nt.value], "norms": norms[:nt.value], "current": bool(st.value & self.MIRROR_CURRENT),
+                "disabled": bool(st.value & self.MIRROR_DISABLED)}
+
+    def debug_mirror(self, l):
+        """IVFFLAT (or a shard of GPU_IVFFLAT): list l's first ceil(len / 128) tiles of the live tensor-core mirror, as a
+        dict: tiles [n, 2 * 128 * k16] float32 (hi then lo operand), norms [n, 128], and whether the mirror is current
+        and whether it is disabled.  n is 0 when no mirror exists."""
+        return self._debug_mirror(_lib.lib().gb_debug_mirror, l)
+
+    def debug_mirror_rebuilt(self, l):
+        """The same tiles as a build of the mirror from the current lists writes them (into scratch; the live mirror is
+        left as it is)."""
+        return self._debug_mirror(_lib.lib().gb_debug_mirror_rebuilt, l)
+
+    def debug_rowptr_rows(self, v0, n):
+        """IVFFLAT on a "RocksDB" store (or a shard of GPU_IVFFLAT, local vids): the rows the winner re-score's row
+        pointers give vids [v0, v0 + n), and per vid ROW_LIVE (a list entry), ROW_NULL or ROW_STRAY (no list entry; row
+        zero).  Returns (rows [n, d] float32, state [n] int32)."""
+        rows, state = np.zeros((n, self.d), np.float32), np.zeros(n, np.int32)
+        _check(_lib.lib().gb_debug_rowptr_rows(self._h, int(v0), int(n), _ptr(rows), _ptr(state)), "debug_rowptr_rows")
+        return rows, state
+
+    def debug_pq_norms(self, l):
+        """IVFPQ at 8 bits: list l's cached |r_e|^2 segment and the same segment recomputed from the lists, as
+        (live float32 [<= len], recomputed float32 [len], current: whether the cache's key matches)."""
+        n, cur = C.c_int64(), C.c_int32()
+        _check(_lib.lib().gb_debug_pq_norms(self._h, int(l), None, None, C.byref(n), C.byref(cur)), "debug_pq_norms")
+        live, rec = np.zeros(n.value, np.float32), np.zeros(n.value, np.float32)
+        _check(_lib.lib().gb_debug_pq_norms(self._h, int(l), _ptr(live), _ptr(rec), C.byref(n), C.byref(cur)),
+               "debug_pq_norms")
+        return live, rec, bool(cur.value)
+
+    def debug_pq_tables(self):
+        """IVFPQ at 8 bits: the tensor-core filter's tables, (int8 codebook [M, 256, dsub], cbnrm float32 [M * 256 + 4]:
+        |pq[m][c]|^2, then R^2, sb, D and one unused float)."""
+        m = self.pq_m
+        cb8 = np.zeros((m, 256, self.d // m), np.int8)
+        nrm = np.zeros(m * 256 + 4, np.float32)
+        _check(_lib.lib().gb_debug_pq_tables(self._h, _ptr(cb8), _ptr(nrm)), "debug_pq_tables")
+        return cb8, nrm
+
     def compact(self):
         _check(_lib.lib().gb_index_compact(self._h), "compact")
 
