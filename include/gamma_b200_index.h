@@ -100,6 +100,31 @@ int gb_index_search_device_filtered(gb_index *index, int nq, const float *x_dev,
                                     const char *retrieval_params_json, int brute_force, const uint8_t *del_bits_dev,
                                     const uint8_t *filter_bits_dev, int64_t bitmap_bits, float min_score,
                                     float max_score, float *out_scores_dev, int64_t *out_ids_dev, void *stream);
+/* Cancellation (RequestContext::is_killed; DESIGN.md section 8, cancellation).  A token is one cancel word in pinned host
+ * memory that every device reads; it only ever goes from unset to set.  A search given a token polls it in its scan and
+ * re-rank kernels and its host loops, stops early once it is set, and returns -2 when it was set at any time before
+ * the search's final synchronise (gb_index_search_device_cancellable: before it returns; a token set later leaves the
+ * outputs undefined).  NULL = never cancelled; an unset token changes no result.  A token may serve one search at a
+ * time; free it after that search has returned.  create: NULL on failure (gb_last_error). */
+typedef struct gb_cancel_token gb_cancel_token;
+gb_cancel_token *gb_cancel_token_create(void);
+void gb_cancel_token_set(gb_cancel_token *token);
+int gb_cancel_token_is_set(gb_cancel_token *token);
+void gb_cancel_token_free(gb_cancel_token *token);
+/* gb_index_search with the enable_realtime tail (search_unindexed_tail, as gb_index_search_binary) and a cancel token */
+int gb_index_search_cancellable(gb_index *index, int nq, const float *x, int k, const char *retrieval_params_json,
+                                int brute_force, const uint8_t *del_bitmap, const uint8_t *filter_bitmap,
+                                int64_t bitmap_bits, float min_score, float max_score, int search_unindexed_tail,
+                                gb_cancel_token *cancel, float *out_scores, int64_t *out_ids);
+int gb_index_search_device_cancellable(gb_index *index, int nq, const float *x_dev, int64_t ld, int k,
+                                       const char *retrieval_params_json, int brute_force, gb_cancel_token *cancel,
+                                       float *out_scores_dev, int64_t *out_ids_dev, void *stream);
+/* Test hooks.  cancel_stats: {"kernel": CTAs that skipped their work, ...} for every kernel that polls, on `device`,
+ * since the last call (which clears them); *json_out is malloc'd, the caller frees it.  cancel_register: the kill
+ * registry behind SetKillStatus with `token` in place of a running search's word (op 1 register under (request_id,
+ * partition_id), op 0 remove); no device is involved. */
+int gb_debug_cancel_stats(int device, char **json_out, int *out_len);
+int gb_debug_cancel_register(const char *request_id, int partition_id, gb_cancel_token *token, int op);
 /* {"stage": ms, ...}: device time per stage of the searches run since the last call with timing enabled
  * (CUDA events on the launching stream); *json_out is malloc'd, the caller frees it */
 int gb_index_stage_times(gb_index *index, char **json_out, int *out_len);
@@ -222,6 +247,10 @@ int gb_index_get_binary(gb_index *index, int64_t start, int64_t n, uint8_t *out)
 int gb_index_search_binary(gb_index *index, int nq, const uint8_t *x, int k, const char *retrieval_params_json,
                            int brute_force, const uint8_t *del_bitmap, const uint8_t *filter_bitmap, int64_t bitmap_bits,
                            float min_score, float max_score, int search_unindexed_tail, float *out_scores, int64_t *out_ids);
+int gb_index_search_binary_cancellable(gb_index *index, int nq, const uint8_t *x, int k, const char *retrieval_params_json,
+                                       int brute_force, const uint8_t *del_bitmap, const uint8_t *filter_bitmap,
+                                       int64_t bitmap_bits, float min_score, float max_score, int search_unindexed_tail,
+                                       gb_cancel_token *cancel, float *out_scores, int64_t *out_ids);
 int gb_index_set_binary_centroids(gb_index *index, const uint8_t *centroids, int nlist);
 int gb_index_get_binary_centroids(gb_index *index, uint8_t *centroids);
 /* the float centroids of the +-1 k-means the packed centroids were taken from: nlist x d floats */

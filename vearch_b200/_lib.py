@@ -57,6 +57,17 @@ def _declare(l):
     l.gb_index_mem_bytes.argtypes = [vp, i32]
     l.gb_index_search.argtypes = [vp, i32, vp, i32, cstr, i32, vp, vp, i64, f32, f32, vp, vp]
     l.gb_index_search_device.argtypes = [vp, i32, vp, i64, i32, cstr, i32, vp, vp, vp]
+    l.gb_index_search_cancellable.argtypes = [vp, i32, vp, i32, cstr, i32, vp, vp, i64, f32, f32, i32, vp, vp, vp]
+    l.gb_index_search_device_cancellable.argtypes = [vp, i32, vp, i64, i32, cstr, i32, vp, vp, vp, vp]
+    l.gb_cancel_token_create.restype = vp
+    l.gb_cancel_token_create.argtypes = []
+    l.gb_cancel_token_set.restype = None
+    l.gb_cancel_token_set.argtypes = [vp]
+    l.gb_cancel_token_is_set.argtypes = [vp]
+    l.gb_cancel_token_free.restype = None
+    l.gb_cancel_token_free.argtypes = [vp]
+    l.gb_debug_cancel_stats.argtypes = [i32, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]
+    l.gb_debug_cancel_register.argtypes = [cstr, i32, vp, i32]
     l.gb_index_search_device_keys.argtypes = [vp, i32, vp, i64, i32, cstr, i32, vp, vp, vp, vp]
     l.gb_index_search_device_filtered.argtypes = [vp, i32, vp, i64, i32, cstr, i32, vp, vp, i64, f32, f32, vp, vp, vp]
     l.gb_index_stage_times.argtypes = [vp, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]
@@ -117,6 +128,7 @@ def _declare(l):
     l.gb_index_update_binary.argtypes = [vp, i64, vp]
     l.gb_index_get_binary.argtypes = [vp, i64, i64, vp]
     l.gb_index_search_binary.argtypes = [vp, i32, vp, i32, cstr, i32, vp, vp, i64, f32, f32, i32, vp, vp]
+    l.gb_index_search_binary_cancellable.argtypes = [vp, i32, vp, i32, cstr, i32, vp, vp, i64, f32, f32, i32, vp, vp, vp]
     l.gb_index_set_binary_centroids.argtypes = [vp, vp, i32]
     l.gb_index_get_binary_centroids.argtypes = [vp, vp]
     l.gb_index_get_real_centroids.argtypes = [vp, vp]

@@ -81,6 +81,51 @@ __device__ __forceinline__ bool ctx_is_valid(const uint32_t* del_bits, const uin
   return true;
 }
 
+// ---- cancellation (DESIGN.md section 8) ---------------------------------------------------
+// Every translation unit has its own copy of the skip counters (no relocatable device code); each registers a reader
+// with register_cancel_skips when the library loads.
+namespace {
+__device__ unsigned long long g_cancel_skips[kCancelSites];
+cudaError_t take_cancel_skips_tu(int device, unsigned long long* acc) {
+  unsigned long long h[kCancelSites];
+  cudaError_t e = cudaSetDevice(device);
+  if (e == cudaSuccess) e = cudaMemcpyFromSymbol(h, g_cancel_skips, sizeof(h));
+  if (e == cudaErrorInvalidSymbol) {  // no kernel of this unit polls: the compiler dropped its counters
+    cudaGetLastError();
+    return cudaSuccess;
+  }
+  if (e != cudaSuccess) return e;
+  for (int i = 0; i < kCancelSites; i++) acc[i] += h[i];
+  const unsigned long long z[kCancelSites] = {};
+  return cudaMemcpyToSymbol(g_cancel_skips, z, sizeof(z));
+}
+[[maybe_unused]] const int g_cancel_skips_reader = register_cancel_skips(&take_cancel_skips_tu);
+}  // namespace
+
+// The CTA-wide poll of a cancel word (CancelPoll), called by every thread of the CTA at a work-unit boundary, before
+// any mbarrier is initialised: one thread reads `seen` and, in one CTA of kCancelPollStride, the host word itself
+// (system scope: the host sets it while the kernel runs; reads of one host address from every CTA would queue on
+// PCIe), the barrier hands its answer to the whole CTA, and a CTA that is to skip counts itself once in its kernel's
+// counter.  A null word costs one uniform branch and no barrier.
+__device__ __forceinline__ bool cta_cancelled(CancelPoll c, int site) {
+  if (c.word == nullptr) return false;
+  const bool first = threadIdx.x == 0 && threadIdx.y == 0 && threadIdx.z == 0;
+  int set = 0;
+  if (first) {
+    uint32_t v;
+    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(c.seen) : "memory");
+    const unsigned b = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
+    if (v == 0 && b % kCancelPollStride == 0) {
+      asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(c.word) : "memory");
+      if (v) asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(c.seen), "r"(1u) : "memory");
+    }
+    set = v != 0;
+  }
+  set = __syncthreads_or(set);
+  if (set && first) atomicAdd(&g_cancel_skips[site], 1ull);
+  return set != 0;
+}
+
 // ---- shared-memory helpers ---------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 

@@ -164,15 +164,56 @@ bool SearchRequestPB::parse(const uint8_t* data, size_t len) {
 }
 
 // ---- kill switch ---------------------------------------------------------------------------
+// g_killed: the kills recorded (checked before and after a search); g_inflight: the cancel word of every running search
+// by (request id, partition id), which SetKill sets so the search's kernels and host loops stop early (DESIGN.md
+// section 8, cancellation).  A word only ever goes from 0 to 1 while its search runs: ClearKill does not reset it.
 static std::mutex g_kill_mu;
 static std::map<std::pair<std::string, int>, int> g_killed;
+static std::multimap<std::pair<std::string, int>, CancelWord*> g_inflight;
+static std::vector<CancelWord*> g_idle_words;  // words of finished searches, reset to 0, for the next ones
 void Engine::SetKill(const std::string& request_id, int partition_id, int reason) {
   std::lock_guard<std::mutex> g(g_kill_mu);
   g_killed[{request_id, partition_id}] = reason;
+  auto r = g_inflight.equal_range({request_id, partition_id});
+  for (auto it = r.first; it != r.second; ++it) cancel_set(it->second->w);
 }
 void Engine::ClearKill(const std::string& request_id, int partition_id) {
   std::lock_guard<std::mutex> g(g_kill_mu);
   g_killed.erase({request_id, partition_id});
+}
+void Engine::RegisterCancel(const std::string& request_id, int partition_id, CancelWord* c) {
+  std::lock_guard<std::mutex> g(g_kill_mu);
+  g_inflight.insert({{request_id, partition_id}, c});
+  if (g_killed.count({request_id, partition_id})) cancel_set(c->w);
+}
+void Engine::UnregisterCancel(const std::string& request_id, int partition_id, CancelWord* c) {
+  std::lock_guard<std::mutex> g(g_kill_mu);
+  auto r = g_inflight.equal_range({request_id, partition_id});
+  for (auto it = r.first; it != r.second; ++it)
+    if (it->second == c) {
+      g_inflight.erase(it);
+      return;
+    }
+}
+Engine::KillScope::KillScope(const std::string& request_id, int partition_id) : rid(request_id), pid(partition_id) {
+  if (request_id.empty()) return;  // a request without an id cannot be killed (IsKilled)
+  {
+    std::lock_guard<std::mutex> g(g_kill_mu);
+    if (!g_idle_words.empty()) {
+      c = g_idle_words.back();
+      g_idle_words.pop_back();
+    }
+  }
+  if (!c) c = cancel_word_create();
+  if (!c) return;  // no word: the search runs to its end, and the kill is still seen after it
+  RegisterCancel(rid, pid, c);
+}
+Engine::KillScope::~KillScope() {
+  if (!c) return;
+  UnregisterCancel(rid, pid, c);
+  *c->w = 0;  // the search has returned: nothing reads the word until the next search takes it
+  std::lock_guard<std::mutex> g(g_kill_mu);
+  g_idle_words.push_back(c);
 }
 bool Engine::IsKilled(const std::string& request_id, int partition_id) {
   if (request_id.empty()) return false;
@@ -842,7 +883,9 @@ Status Engine::Search(const SearchRequestPB& req, std::string* pb_out) {
   int n = (int)(vq.value.size() / qbytes);
   if (n <= 0) return Status::Make(kInvalidArgument, "Search n shouldn't less than 0!");
   if (IsKilled(req.request_id, req.partition_id)) return Status::Make(kMemoryExceeded, "");
+  KillScope kill(req.request_id, req.partition_id);
   SearchContext ctx;
+  ctx.cancel = kill.word();
   std::string err;
   if (!parse_retrieval_params(req.index_params, &ctx.params, &err)) return Status::Make(kInvalidArgument, err);
   ctx.params.brute_force = brute != 0;
@@ -1002,7 +1045,9 @@ Status Engine::SearchMulti(const SearchRequestPB& req, std::string* pb_out) {
     return Status::Make(kIndexError, space_name_ + " index not trained, brute_force_search is 0, max_docid_ = " +
                                          std::to_string(max_docid_) + ", threshold = 100");
   if (IsKilled(req.request_id, req.partition_id)) return Status::Make(kMemoryExceeded, "");
+  KillScope kill(req.request_id, req.partition_id);
   SearchContext base;
+  base.cancel = kill.word();
   if (!parse_retrieval_params(req.index_params, &base.params, &err)) return Status::Make(kInvalidArgument, err);
   base.params.brute_force = brute != 0;
   base.search_unindexed_tail = enable_realtime_;

@@ -167,6 +167,19 @@ class Engine {
   static void SetKill(const std::string& request_id, int partition_id, int reason);
   static void ClearKill(const std::string& request_id, int partition_id);
   static bool IsKilled(const std::string& request_id, int partition_id);
+  // the registry of running searches' cancel words (SetKill sets the words registered under its pair)
+  static void RegisterCancel(const std::string& request_id, int partition_id, CancelWord* c);
+  static void UnregisterCancel(const std::string& request_id, int partition_id, CancelWord* c);
+  // a search's cancel word, registered for its lifetime (none for a request without an id); taken from a pool of
+  // words of finished searches
+  struct KillScope {
+    std::string rid;
+    int pid;
+    CancelWord* c = nullptr;
+    KillScope(const std::string& request_id, int partition_id);
+    ~KillScope();
+    const uint32_t* word() const { return c && c->device_readable ? c->w : nullptr; }
+  };
 
  private:
   int flush_pending_locked();

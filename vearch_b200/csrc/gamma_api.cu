@@ -280,6 +280,17 @@ static std::string to_hex(const std::string& s) {
 
 extern "C" {
 
+// the kill registry (SetKillStatus) with a caller's token in place of a running search's word: op 1 registers it under
+// (request_id, partition_id), op 0 removes it
+int gb_debug_cancel_register(const char* request_id, int partition_id, gb_cancel_token* token, int op) {
+  if (!request_id || !token) return -1;
+  if (op)
+    Engine::RegisterCancel(request_id, partition_id, token->c);
+  else
+    Engine::UnregisterCancel(request_id, partition_id, token->c);
+  return 0;
+}
+
 // admission controller introspection: op 0 = threshold, 1 = in-flight count, 2 = set threshold to `value`
 // (<= 0 restores the system-derived one), 3 = Acquire(value) -> 1 admitted / 0 refused, 4 = Release(value)
 int gb_debug_concurrency(int op, int value) {

@@ -1090,6 +1090,7 @@ int Index::search_keys(const SearchContext& ctx, int nq, const void* xq, int k, 
   cudaStream_t st = s.stream();
   FilterArgs f;
   if (upload_bitmaps(ctx, &f, s)) return -1;
+  if (cancel_poll_init(ctx.cancel, &f, s)) return -1;
   const int metric = search_metric(ctx);
   GB_ALLOC(keys, unsigned long long, (size_t)nq * k, s);
   *out_keys = keys;
@@ -1102,7 +1103,7 @@ int Index::search_keys(const SearchContext& ctx, int nq, const void* xq, int k, 
     // enable_realtime (vector_manager.cc:854-889, 971-1053): vectors stored but not yet indexed are
     // searched brute-force (the reference's MemoryBuffer FLAT index) and merged by score
     const int64_t tail0 = indexed_count_, tail1 = store_->size();
-    if (rc == 0 && ctx.search_unindexed_tail && tail1 > tail0) {
+    if (rc == 0 && ctx.search_unindexed_tail && tail1 > tail0 && !cancel_is_set(ctx.cancel)) {
       GB_ALLOC(both, unsigned long long, (size_t)nq * 2 * k, s);
       GB_CUDA(cudaMemcpy2DAsync(both, (size_t)2 * k * 8, keys, (size_t)k * 8, (size_t)k * 8, nq,
                                 cudaMemcpyDeviceToDevice, st));
@@ -1153,7 +1154,8 @@ int Index::search_device(const SearchContext& ctx, int nq, const float* x_dev, i
   if (out_keys_dev) GB_CUDA(cudaMemcpyAsync(out_keys_dev, keys, (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, st));
   if (out_dis_dev && out_ids_dev)
     GB_CUDA(launch_decode_keys(keys, k, nq, k, search_metric(ctx), out_dis_dev, out_ids_dev, 0, st));
-  return 0;
+  // asynchronous: a word set after this point leaves the outputs undefined, and its setter knows not to read them
+  return cancel_is_set(ctx.cancel) ? -2 : 0;
 }
 
 static bool coalesce_enabled() {
@@ -1207,8 +1209,14 @@ void Index::coalesce_loop() {
     for (CoReq* r : batch) total += r->nq;
     const int k = batch[0]->k;
     int rc;
+    // every member keeps its own cancel word; the batch runs unless all of them are already set, and a member whose
+    // word is set by the end of the batch returns -2 while the others take their results
+    bool all_cancelled = true;
+    for (CoReq* r : batch) all_cancelled = all_cancelled && cancel_is_set(r->ctx->cancel);
     if (batch.size() == 1) {
       rc = search_direct(*batch[0]->ctx, batch[0]->nq, batch[0]->x, k, batch[0]->out_dis, batch[0]->out_ids);
+    } else if (all_cancelled) {
+      rc = -2;
     } else {
       const size_t rb = store_->row_bytes();
       xs.resize((size_t)total * rb);
@@ -1219,7 +1227,9 @@ void Index::coalesce_loop() {
         memcpy(xs.data() + o * rb, r->x, (size_t)r->nq * rb);
         o += r->nq;
       }
-      rc = search_direct(*batch[0]->ctx, total, xs.data(), k, dd.data(), ii.data());
+      SearchContext bctx = *batch[0]->ctx;
+      bctx.cancel = nullptr;
+      rc = search_direct(bctx, total, xs.data(), k, dd.data(), ii.data());
       o = 0;
       for (CoReq* r : batch) {
         if (rc == 0) {
@@ -1233,8 +1243,8 @@ void Index::coalesce_loop() {
     {
       std::lock_guard<std::mutex> lk(co_mu_);
       for (CoReq* r : batch) {
-        r->rc = rc;
-        r->err = err;
+        r->rc = rc == 0 && cancel_is_set(r->ctx->cancel) ? -2 : rc;
+        r->err = r->rc == -2 ? "" : err;
         r->done = true;
       }
     }
@@ -1277,6 +1287,51 @@ int Index::search(const SearchContext& ctx, int nq, const void* x, int k, float*
   return req.rc;
 }
 
+CancelWord* cancel_word_create() {
+  auto* c = new CancelWord;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    cudaGetLastError();
+    c->w = static_cast<uint32_t*>(calloc(1, sizeof(uint32_t)));
+  } else {
+    void* p = nullptr;
+    const cudaError_t e = cudaHostAlloc(&p, sizeof(uint32_t), cudaHostAllocMapped | cudaHostAllocPortable);
+    if (e != cudaSuccess) {
+      set_last_error(std::string("cancel token: ") + cudaGetErrorString(e));
+      delete c;
+      return nullptr;
+    }
+    c->w = static_cast<uint32_t*>(p);
+    c->device_readable = true;
+    *c->w = 0;
+  }
+  if (!c->w) {
+    set_last_error("cancel token: out of host memory");
+    delete c;
+    return nullptr;
+  }
+  return c;
+}
+
+int cancel_poll_init(const uint32_t* word, FilterArgs* f, Scratch& s) {
+  f->cancel = CancelPoll{};
+  if (!word) return 0;
+  uint32_t* seen = s.alloc_n<uint32_t>(1);
+  if (!seen) return -1;
+  GB_CUDA(cudaMemsetAsync(seen, 0, sizeof(uint32_t), s.stream()));
+  f->cancel = CancelPoll{word, seen};
+  return 0;
+}
+
+void cancel_word_free(CancelWord* c) {
+  if (!c) return;
+  if (c->device_readable)
+    cudaFreeHost(c->w);
+  else
+    free(c->w);
+  delete c;
+}
+
 int Index::search_direct(const SearchContext& ctx, int nq, const void* x, int k, float* out_dis, int64_t* out_ids) {
   if (nq <= 0) return 0;
   cudaSetDevice(device_);
@@ -1288,7 +1343,9 @@ int Index::search_direct(const SearchContext& ctx, int nq, const void* x, int k,
     std::shared_lock<std::shared_mutex> lk(mu_);
     if (int rc = search_keys(ctx, nq, xq, k, &keys, s)) return rc;
   }
-  return download_results(keys, nq, k, search_metric(ctx), out_dis, out_ids, s);
+  if (download_results(keys, nq, k, search_metric(ctx), out_dis, out_ids, s)) return -1;
+  // after the final synchronise: the outcome does not depend on whether any kernel saw the word
+  return cancel_is_set(ctx.cancel) ? -2 : 0;
 }
 
 int Index::debug_rerank(const SearchContext& ctx, int nq, const float* xq, int ncand, const int64_t* cand, int k,
@@ -1386,10 +1443,10 @@ int Index::debug_shadow_rows(int64_t start, int64_t n, void* out, int64_t* row_b
 }
 
 cudaError_t Index::flat_tile(const void* xq, int nq, const void* rows, int m, int metric, float* scores, int64_t ldo,
-                             cudaStream_t st) {
+                             cudaStream_t st, CancelPoll cancel) {
   last_scan_kernel_ = "dist_tile_kernel+select_rows_kernel";
   return launch_dist_matrix(static_cast<const float*>(xq), dpad_, nq, static_cast<const float*>(rows), dpad_, m, dpad_, metric,
-                            scores, ldo, st);
+                            scores, ldo, st, cancel);
 }
 
 // GammaFLATIndex::Search (gamma_index_flat.cc:130-370): every stored row, filters before top-k.
@@ -1450,6 +1507,7 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
     for (int p0 = 0; p0 < nq; p0 += PB) {  // one block unless the partials need more: the rows stream once per block
       const int pb = std::min(PB, nq - p0);
       for (int c = 0; c < nch; c++, copies++) {
+        if (copies > 0 && cancel_is_set(f.cancel.word)) break;  // the first chunk is enqueued: its kernels poll the word
         const int b = copies & 1;
         GB_CUDA(cudaStreamWaitEvent(cl.cs, cl.reusable[b], 0));
         GB_CUDA(cudaMemcpyAsync(stage[b], chunks[c].base, (size_t)chunks[c].cnt * ld, cudaMemcpyHostToDevice, cl.cs));
@@ -1457,7 +1515,7 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
         GB_CUDA(cudaStreamWaitEvent(st, cl.copied[b], 0));
         for (int q0 = 0; q0 < pb; q0 += QB) {
           int qb = std::min(QB, pb - q0);
-          GB_CUDA(flat_tile(xq + (p0 + q0) * ld, qb, stage[b], chunks[c].cnt, metric, scores, ldo, st));
+          GB_CUDA(flat_tile(xq + (p0 + q0) * ld, qb, stage[b], chunks[c].cnt, metric, scores, ldo, st, f.cancel));
           GB_CUDA(launch_select_scores(scores, ldo, qb, chunks[c].cnt, chunks[c].id0, k, metric, f,
                                        (nch > 1 ? partial + (int64_t)q0 * nch * k : out_keys + (int64_t)(p0 + q0) * k) +
                                            (int64_t)c * k,
@@ -1465,6 +1523,7 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
         }
         GB_CUDA(cudaEventRecord(cl.reusable[b], st));
       }
+      if (cancel_is_set(f.cancel.word)) break;
       if (nch > 1) GB_CUDA(launch_select_keys(partial, (int64_t)nch * k, pb, nch * k, k, out_keys + (int64_t)p0 * k, k, st));
     }
     scan_timer_end(st);
@@ -1476,13 +1535,15 @@ int Index::flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int me
     for (int q0 = 0; q0 < pb; q0 += QB) {
       int qb = std::min(QB, pb - q0);
       for (int c = 0; c < nch; c++) {
-        GB_CUDA(flat_tile(xq + (p0 + q0) * ld, qb, chunks[c].base, chunks[c].cnt, metric, scores, ldo, st));
+        if ((p0 > 0 || q0 > 0 || c > 0) && cancel_is_set(f.cancel.word)) break;
+        GB_CUDA(flat_tile(xq + (p0 + q0) * ld, qb, chunks[c].base, chunks[c].cnt, metric, scores, ldo, st, f.cancel));
         GB_CUDA(launch_select_scores(scores, ldo, qb, chunks[c].cnt, chunks[c].id0, k, metric, f,
                                      (nch > 1 ? partial + (int64_t)q0 * nch * k : out_keys + (int64_t)(p0 + q0) * k) +
                                          (int64_t)c * k,
                                      (int64_t)nch * k, st));
       }
     }
+    if (cancel_is_set(f.cancel.word)) break;
     if (nch > 1) GB_CUDA(launch_select_keys(partial, (int64_t)nch * k, pb, nch * k, k, out_keys + (int64_t)p0 * k, k, st));
   }
   scan_timer_end(st);
@@ -2523,6 +2584,7 @@ int IvfIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int
   const int nprobe = resolve_nprobe(ctx);
   const int64_t ld = store_->stride();
   for (int q0 = 0; q0 < nq; q0 += kQueryBlock) {
+    if (q0 > 0 && cancel_is_set(ctx.cancel)) break;  // the blocks enqueued so far finish; their kernels poll the word
     int qb = std::min(kQueryBlock, nq - q0);
     Scratch sb(s.stream());
     GB_ALLOC(probe_ids, int32_t, (size_t)qb * nprobe, sb);
@@ -3462,13 +3524,13 @@ int BinaryIvfIndex::append_batch(const void* x, int64_t n, int64_t vid0, const i
 
 // launch_hamming_tile, in launches of at most kHammingTileMaxQueries queries
 cudaError_t BinaryIvfIndex::flat_tile(const void* xq, int nq, const void* rows, int m, int metric, float* scores, int64_t ldo,
-                                      cudaStream_t st) {
+                                      cudaStream_t st, CancelPoll cancel) {
   (void)metric;
   last_scan_kernel_ = "hamming_tile_kernel+select_rows_kernel";
   for (int q0 = 0; q0 < nq; q0 += kHammingTileMaxQueries) {
     const cudaError_t e = launch_hamming_tile(static_cast<const uint32_t*>(xq) + q0 * ldw_, ldw_,
                                               std::min(kHammingTileMaxQueries, nq - q0), static_cast<const uint32_t*>(rows),
-                                              ldw_, m, (cb_ + 3) / 4, scores + q0 * ldo, ldo, st);
+                                              ldw_, m, (cb_ + 3) / 4, scores + q0 * ldo, ldo, st, cancel);
     if (e != cudaSuccess) return e;
   }
   return cudaSuccess;

@@ -280,7 +280,24 @@ struct SearchContext {  // RetrievalContext / SearchCondition (common/gamma_comm
   float min_score = -3.4028235e38f, max_score = 3.4028235e38f;
   bool search_unindexed_tail = false;  // table.enable_realtime: brute-force the not-yet-indexed vectors too
   RetrievalParams params;
+  // the search's cancel word (FilterArgs::cancel): mapped, portable pinned host memory that goes from 0 to 1 at most
+  // once.  A search whose word is set before its final synchronise returns -2; nullptr: never cancelled
+  const uint32_t* cancel = nullptr;
 };
+// the host side of a cancel word: the host loops of a search stop enqueuing launches once it is set
+inline bool cancel_is_set(const uint32_t* w) { return w && __atomic_load_n(w, __ATOMIC_RELAXED) != 0; }
+inline void cancel_set(uint32_t* w) { __atomic_store_n(w, 1u, __ATOMIC_RELAXED); }
+// One cancel word (gb_cancel_token): pinned host memory mapped into every device's address space (cudaHostAllocMapped |
+// cudaHostAllocPortable), so a kernel of any shard reads the word the host sets.  Without any CUDA device (host-only
+// uses of the engine's kill registry) the word is plain host memory, and no search accepts it (device_readable false).
+struct CancelWord {
+  uint32_t* w = nullptr;
+  bool device_readable = false;
+};
+CancelWord* cancel_word_create();  // nullptr on failure (last_error set)
+// f->cancel for the search's word (nullable): the word and a zeroed `seen` flag in s, on s's device
+int cancel_poll_init(const uint32_t* word, FilterArgs* f, Scratch& s);
+void cancel_word_free(CancelWord* c);
 
 class Index {
  public:
@@ -416,9 +433,9 @@ class Index {
   int flat_search_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, int k,
                       int64_t nrows, unsigned long long* out_keys, Scratch& s, int64_t row_begin = 0);
   // flat_search_dev's distance tile: scores [nq][ldo] of queries xq against m device rows (both store().stride() bytes
-  // apart), exact; names the scan's kernels in last_scan_kernel_
+  // apart), exact; names the scan's kernels in last_scan_kernel_; cancel: the search's cancel word (nullable)
   virtual cudaError_t flat_tile(const void* xq, int nq, const void* rows, int m, int metric, float* scores, int64_t ldo,
-                                cudaStream_t st);
+                                cudaStream_t st, CancelPoll cancel);
   virtual int search_keys_dev(const SearchContext& ctx, const FilterArgs& f, int metric, int nq, const void* xq, int k,
                               unsigned long long* out_keys, Scratch& s) = 0;
   int upload_bitmaps(const SearchContext& ctx, FilterArgs* f, Scratch& s);
@@ -1030,7 +1047,7 @@ class BinaryIvfIndex : public IvfIndex {
   // Hamming distances rank like L2, whatever metric_type the retrieval parameters carry
   int search_metric(const SearchContext& ctx) const override { (void)ctx; return kMetricL2; }
   cudaError_t flat_tile(const void* xq, int nq, const void* rows, int m, int metric, float* scores, int64_t ldo,
-                        cudaStream_t st) override;
+                        cudaStream_t st, CancelPoll cancel) override;
   int coarse_dev(int nq, const void* xq, int nprobe, int metric, int32_t* probe_ids, float* coarse_dis, Scratch& s) override;
   int assign_batch(const void* x, int64_t n, const void** xc, int32_t* out, Scratch& s) override;
   int append_batch(const void* x, int64_t n, int64_t vid0, const int32_t* d_list, const int32_t* d_pos,
@@ -1206,3 +1223,8 @@ int merge_partition_keys_device(const unsigned long long* keys, int nparts, int 
                                 int64_t* out_ids, cudaStream_t st);
 
 }  // namespace gb
+
+// the C-ABI handle of a cancel word (include/gamma_b200_index.h)
+struct gb_cancel_token {
+  gb::CancelWord* c;
+};

@@ -230,6 +230,17 @@ static int fill_ctx(SearchContext* ctx, const char* rp_json, int brute_force, co
   return 0;
 }
 
+// a search's cancel token (nullable): only a word every device can read
+static int set_cancel(SearchContext* ctx, gb_cancel_token* t) {
+  if (!t) return 0;
+  if (!t->c->device_readable) {
+    set_last_error("cancel token: made without a CUDA device, no kernel can read it");
+    return -1;
+  }
+  ctx->cancel = t->c->w;
+  return 0;
+}
+
 #define IDX_OR_FAIL(idx)                 \
   if (!(idx) || !(idx)->impl) {          \
     set_last_error("null index handle"); \
@@ -402,23 +413,72 @@ int64_t gb_index_mem_bytes(gb_index* index, int which) {
 int gb_index_search(gb_index* index, int nq, const float* x, int k, const char* retrieval_params_json, int brute_force,
                     const uint8_t* del_bitmap, const uint8_t* filter_bitmap, int64_t bitmap_bits, float min_score,
                     float max_score, float* out_scores, int64_t* out_ids) {
+  return gb_index_search_cancellable(index, nq, x, k, retrieval_params_json, brute_force, del_bitmap, filter_bitmap,
+                                     bitmap_bits, min_score, max_score, 0, nullptr, out_scores, out_ids);
+}
+
+int gb_index_search_cancellable(gb_index* index, int nq, const float* x, int k, const char* retrieval_params_json,
+                                int brute_force, const uint8_t* del_bitmap, const uint8_t* filter_bitmap,
+                                int64_t bitmap_bits, float min_score, float max_score, int search_unindexed_tail,
+                                gb_cancel_token* cancel, float* out_scores, int64_t* out_ids) {
   IDX_OR_FAIL(index);
   if (packed_binary(index)) return -1;
   SearchContext ctx;
   if (fill_ctx(&ctx, retrieval_params_json, brute_force, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score))
     return -1;
+  ctx.search_unindexed_tail = search_unindexed_tail != 0;
+  if (set_cancel(&ctx, cancel)) return -1;
   return index->impl->search(ctx, nq, x, k, out_scores, out_ids);
 }
 
 int gb_index_search_device(gb_index* index, int nq, const float* x_dev, int64_t ld, int k,
                            const char* retrieval_params_json, int brute_force, float* out_scores_dev,
                            int64_t* out_ids_dev, void* stream) {
+  return gb_index_search_device_cancellable(index, nq, x_dev, ld, k, retrieval_params_json, brute_force, nullptr,
+                                            out_scores_dev, out_ids_dev, stream);
+}
+
+int gb_index_search_device_cancellable(gb_index* index, int nq, const float* x_dev, int64_t ld, int k,
+                                       const char* retrieval_params_json, int brute_force, gb_cancel_token* cancel,
+                                       float* out_scores_dev, int64_t* out_ids_dev, void* stream) {
   IDX_OR_FAIL(index);
   if (packed_binary(index)) return -1;
   SearchContext ctx;
   if (fill_ctx(&ctx, retrieval_params_json, brute_force, nullptr, nullptr, 0, -3.4028235e38f, 3.4028235e38f)) return -1;
+  if (set_cancel(&ctx, cancel)) return -1;
   return index->impl->search_device(ctx, nq, x_dev, ld, k, out_scores_dev, out_ids_dev,
                                     static_cast<cudaStream_t>(stream));
+}
+
+gb_cancel_token* gb_cancel_token_create(void) {
+  CancelWord* c = cancel_word_create();
+  return c ? new gb_cancel_token{c} : nullptr;
+}
+void gb_cancel_token_set(gb_cancel_token* t) {
+  if (t) cancel_set(t->c->w);
+}
+int gb_cancel_token_is_set(gb_cancel_token* t) { return t && cancel_is_set(t->c->w) ? 1 : 0; }
+void gb_cancel_token_free(gb_cancel_token* t) {
+  if (!t) return;
+  cancel_word_free(t->c);
+  delete t;
+}
+
+int gb_debug_cancel_stats(int device, char** json_out, int* out_len) {
+  unsigned long long acc[kCancelSites] = {};
+  if (cudaError_t e = cancel_skips_take(device, acc)) {
+    set_last_error(std::string("cancel stats: ") + cudaGetErrorString(e));
+    return -1;
+  }
+  std::string js = "{";
+  for (int i = 0; i < kCancelSites; i++)
+    js += std::string(i ? ", \"" : "\"") + cancel_site_name(i) + "\": " + std::to_string(acc[i]);
+  js += "}";
+  *json_out = static_cast<char*>(malloc(js.size() + 1));
+  if (!*json_out) return -1;
+  memcpy(*json_out, js.c_str(), js.size() + 1);
+  *out_len = (int)js.size();
+  return 0;
 }
 
 int gb_index_search_device_filtered(gb_index* index, int nq, const float* x_dev, int64_t ld, int k,
@@ -788,11 +848,20 @@ int gb_index_get_binary(gb_index* index, int64_t start, int64_t n, uint8_t* out)
 int gb_index_search_binary(gb_index* index, int nq, const uint8_t* x, int k, const char* retrieval_params_json,
                            int brute_force, const uint8_t* del_bitmap, const uint8_t* filter_bitmap, int64_t bitmap_bits,
                            float min_score, float max_score, int search_unindexed_tail, float* out_scores, int64_t* out_ids) {
+  return gb_index_search_binary_cancellable(index, nq, x, k, retrieval_params_json, brute_force, del_bitmap, filter_bitmap,
+                                            bitmap_bits, min_score, max_score, search_unindexed_tail, nullptr, out_scores,
+                                            out_ids);
+}
+int gb_index_search_binary_cancellable(gb_index* index, int nq, const uint8_t* x, int k, const char* retrieval_params_json,
+                                       int brute_force, const uint8_t* del_bitmap, const uint8_t* filter_bitmap,
+                                       int64_t bitmap_bits, float min_score, float max_score, int search_unindexed_tail,
+                                       gb_cancel_token* cancel, float* out_scores, int64_t* out_ids) {
   BIN_OR_FAIL(b, index);
   SearchContext ctx;
   if (fill_ctx(&ctx, retrieval_params_json, brute_force, del_bitmap, filter_bitmap, bitmap_bits, min_score, max_score))
     return -1;
   ctx.search_unindexed_tail = search_unindexed_tail != 0;
+  if (set_cancel(&ctx, cancel)) return -1;
   return b->search(ctx, nq, x, k, out_scores, out_ids);
 }
 int gb_index_set_binary_centroids(gb_index* index, const uint8_t* centroids, int nlist) {

@@ -473,7 +473,8 @@ int ShardedIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f,
   int rc = 0;
   if (cudaEventRecord(ln->start, pst) != cudaSuccess) rc = -1;
   int touched = 0;  // shards whose stream waited on `start`: each records done[i] after whatever it enqueued
-  for (int i = 0; i < S && rc == 0; i++) {
+  // a cancelled search enqueues no further shard; the shards already enqueued poll the word in their kernels
+  for (int i = 0; i < S && rc == 0 && !(i > 0 && cancel_is_set(f.cancel.word)); i++) {
     IvfIndex* sh = shards_[i].get();
     const int dev = devices_[i];
     cudaStream_t sst = ln->st[i];
@@ -484,6 +485,8 @@ int ShardedIndex::search_keys_dev(const SearchContext& ctx, const FilterArgs& f,
     if (e == cudaSuccess) touched++;
     const void* xq_i = xq;
     FilterArgs fi = f;
+    // the shard's own `seen` flag, on its device
+    if (e == cudaSuccess && cancel_poll_init(f.cancel.word, &fi, ss)) e = cudaErrorMemoryAllocation;
     fi.del_bits = split[0] ? split[0] + (size_t)i * words : nullptr;
     fi.filter_bits = split[1] ? split[1] + (size_t)i * words : nullptr;
     if (dev != device_ && e == cudaSuccess) {  // the queries and this shard's bitmaps on its device

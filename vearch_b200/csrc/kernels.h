@@ -14,16 +14,52 @@ constexpr int kMetricL2 = 1;
 void note_launch(int n = 1);
 long long launch_count();
 
+// A search's cancel word as its kernels poll it (DESIGN.md section 8, cancellation).  word: mapped host memory that only
+// ever goes from 0 to 1 (RequestContext::is_killed); seen: 4 bytes of device memory, zeroed when the search starts, on
+// the device the kernel runs on.  Every CTA reads `seen`; one CTA in kCancelPollStride also reads `word` and, finding it
+// set, sets `seen`, so most CTAs never cross PCIe.  Every CTA that skips has found `seen` or `word` set and leaves
+// `seen` set, so the kernels after it in stream order skip too.  word == nullptr: never cancelled.
+struct CancelPoll {
+  const uint32_t* word = nullptr;
+  uint32_t* seen = nullptr;
+};
+constexpr int kCancelPollStride = 32;
+
 struct FilterArgs {            // RetrievalContext (index/index_model.h:86-110)
   const uint32_t* del_bits;    // bit set => docid deleted            (nullable)
   const uint32_t* filter_bits; // bit set => docid passes the filter  (nullable = no filter)
   float min_score, max_score;  // IsSimilarScoreValid window
+  // the search's cancel word: a CTA of a polling kernel that finds it set leaves its outputs unwritten
+  CancelPoll cancel;
 };
+
+// Kernels that poll the cancel word; a CTA that skips its work adds 1 to its kernel's counter (device memory, per
+// device).  cancel_skips_take adds the counters of `device` to acc[kCancelSites] and clears them.
+enum CancelSite {
+  kCsDistTile,        // dist_tile_kernel (FLAT distance tiles)
+  kCsSelectRows,      // select_rows_kernel (FLAT selection; scored inputs only)
+  kCsHammingTile,     // hamming_tile_kernel (BINARYIVF brute force)
+  kCsIvfflatScan,     // ivfflat_scan_kernel (IVF-Flat query-major)
+  kCsIvfflatScanWarp, // ivfflat_scan_warp_kernel (IVF-Flat query-major, short rows)
+  kCsListmajorTma,    // ivf_listmajor_tma_kernel
+  kCsListmajorPipe,   // ivf_listmajor_pipe_kernel
+  kCsSegSelect,       // seg_select_kernel (IVF-Flat list-major, large k)
+  kCsListScan,        // list_scan_kernel (IVF-PQ, IVFPQFastScan, IVFRABITQ, VEARCH, BINARYIVF query-major)
+  kCsPqtcScan,        // pqtc_scan_kernel
+  kCsPqRescore,       // pq_rescore_kernel
+  kCsRerank,          // rerank_kernel
+  kCsRerankPrefilter, // rerank_prefilter_kernel
+  kCancelSites
+};
+const char* cancel_site_name(int site);
+int register_cancel_skips(cudaError_t (*take)(int device, unsigned long long* acc));
+cudaError_t cancel_skips_take(int device, unsigned long long* acc);
 
 // ---- K1/K2/K6/K8: tiled exact distance kernel ------------------------------------------
 // out[i][j] = |X_i - C_j|^2 (L2) or <X_i, C_j> (IP), i<n, j<m.  d multiple of 4.
+// cancel: the search's cancel word, polled by every CTA (none by default)
 cudaError_t launch_dist_matrix(const float* X, int64_t ldx, int n, const float* C, int64_t ldc, int m, int d,
-                               int metric, float* out, int64_t ldo, cudaStream_t st);
+                               int metric, float* out, int64_t ldo, cudaStream_t st, CancelPoll cancel = {});
 // best[i] = min over j of key(score(X_i,C_j), j + col_base) via atomicMin; caller pre-fills
 // best with 0xFF.. .  Lowest j wins ties (faiss IndexFlat::assign, "first minimum wins").
 cudaError_t launch_dist_argmin(const float* X, int64_t ldx, int n, const float* C, int64_t ldc, int m, int d,
@@ -283,7 +319,7 @@ cudaError_t launch_ivfpqfs_scan(const uint8_t* lut8, const float* ab, int nq, co
 // integers as fp32.  Used for every query x rows job: coarse search (rows = centroids), add-time assignment, brute force.
 constexpr int kHammingTileMaxQueries = 65535 * 16;  // queries of one launch: grid.y of 16-query tiles
 cudaError_t launch_hamming_tile(const uint32_t* Q, int64_t ldq, int nq, const uint32_t* R, int64_t ldr, int m, int words,
-                                float* out, int64_t ldo, cudaStream_t st);
+                                float* out, int64_t ldo, cudaStream_t st, CancelPoll cancel = {});
 // faiss binary_to_real / real_to_binary: bit j of a packed row (byte j >> 3, bit j & 7) <-> +1 / -1 (a float > 0 is 1)
 cudaError_t launch_binary_to_real(const uint8_t* x, int64_t ldx, int64_t n, int d, float* out, int64_t ldo, cudaStream_t st);
 cudaError_t launch_real_to_binary(const float* x, int64_t ldx, int64_t n, int d, uint8_t* out, int64_t ldo, cudaStream_t st);

@@ -18,7 +18,8 @@ constexpr int HT_MAXW = 64;   // words of a query chunk in shared memory (256 by
 // each row word is loaded once and XORed with every query of the tile.
 __global__ void __launch_bounds__(HT_ROWS)
     hamming_tile_kernel(const uint32_t* __restrict__ Q, int64_t ldq, int nq, const uint32_t* __restrict__ R, int64_t ldr,
-                        int m, int W, float* __restrict__ out, int64_t ldo) {
+                        int m, int W, float* __restrict__ out, int64_t ldo, CancelPoll cancel) {
+  if (cta_cancelled(cancel, kCsHammingTile)) return;
   __shared__ uint32_t qs[HT_QB][HT_MAXW];
   const int q0 = blockIdx.y * HT_QB;
   const int nqb = min(HT_QB, nq - q0);
@@ -133,12 +134,12 @@ int64_t blocks_of(int64_t n, int nt) { return (n + nt - 1) / nt; }
 }  // namespace
 
 cudaError_t launch_hamming_tile(const uint32_t* Q, int64_t ldq, int nq, const uint32_t* R, int64_t ldr, int m, int words,
-                                float* out, int64_t ldo, cudaStream_t st) {
+                                float* out, int64_t ldo, cudaStream_t st, CancelPoll cancel) {
   if (nq <= 0 || m <= 0) return cudaSuccess;
   static_assert(kHammingTileMaxQueries == 65535 * HT_QB, "one launch: at most 65535 query tiles");
   if (words <= 0 || nq > kHammingTileMaxQueries) return cudaErrorInvalidValue;
   dim3 grid((unsigned)blocks_of(m, HT_ROWS), (unsigned)blocks_of(nq, HT_QB));
-  hamming_tile_kernel<<<grid, HT_ROWS, 0, st>>>(Q, ldq, nq, R, ldr, m, words, out, ldo);
+  hamming_tile_kernel<<<grid, HT_ROWS, 0, st>>>(Q, ldq, nq, R, ldr, m, words, out, ldo, cancel);
   note_launch();
   return cudaGetLastError();
 }

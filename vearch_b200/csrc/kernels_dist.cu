@@ -13,12 +13,38 @@
 #include "kernels.h"
 
 #include <atomic>
+#include <mutex>
+#include <vector>
 
 namespace gb {
 
 static std::atomic<long long> g_launches{0};
 void note_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 long long launch_count() { return g_launches.load(std::memory_order_relaxed); }
+
+const char* cancel_site_name(int site) {
+  static const char* const names[kCancelSites] = {
+      "dist_tile_kernel",         "select_rows_kernel",        "hamming_tile_kernel", "ivfflat_scan_kernel", "ivfflat_scan_warp_kernel",
+      "ivf_listmajor_tma_kernel", "ivf_listmajor_pipe_kernel", "seg_select_kernel",   "list_scan_kernel",
+      "pqtc_scan_kernel",         "pq_rescore_kernel",         "rerank_kernel",       "rerank_prefilter_kernel"};
+  return site >= 0 && site < kCancelSites ? names[site] : "";
+}
+// readers of every translation unit's skip counters; filled by static initialisers while the library loads
+static std::vector<cudaError_t (*)(int, unsigned long long*)>& cancel_readers() {
+  static std::vector<cudaError_t (*)(int, unsigned long long*)> v;
+  return v;
+}
+int register_cancel_skips(cudaError_t (*take)(int device, unsigned long long* acc)) {
+  cancel_readers().push_back(take);
+  return (int)cancel_readers().size();
+}
+cudaError_t cancel_skips_take(int device, unsigned long long* acc) {
+  static std::mutex mu;
+  std::lock_guard<std::mutex> g(mu);
+  for (auto take : cancel_readers())
+    if (cudaError_t e = take(device, acc)) return e;
+  return cudaSuccess;
+}
 
 namespace {
 
@@ -29,7 +55,8 @@ template <int METRIC, int EPI>
 __global__ void __launch_bounds__(NT)
     dist_tile_kernel(const float* __restrict__ X, int64_t ldx, int n, const float* __restrict__ C, int64_t ldc, int m,
                      int d, float* __restrict__ out, int64_t ldo, unsigned long long* __restrict__ best,
-                     int col_base) {
+                     int col_base, CancelPoll cancel) {
+  if (EPI == EPI_WRITE && cta_cancelled(cancel, kCsDistTile)) return;  // the arg-min epilogue serves training only
   __shared__ __align__(16) float Xs[BK][BM + 4];
   __shared__ __align__(16) float Cs[BK][BN + 4];
   const int tid = threadIdx.x;
@@ -144,11 +171,12 @@ __global__ void pad_rows_kernel(const float* __restrict__ src, int64_t n, int d,
 
 template <int METRIC, int EPI>
 cudaError_t launch_tile(const float* X, int64_t ldx, int n, const float* C, int64_t ldc, int m, int d, float* out,
-                        int64_t ldo, unsigned long long* best, int col_base, cudaStream_t st) {
+                        int64_t ldo, unsigned long long* best, int col_base, cudaStream_t st,
+                        CancelPoll cancel = {}) {
   if (n <= 0 || m <= 0) return cudaSuccess;
   dim3 grid((m + BN - 1) / BN, (n + BM - 1) / BM);
   if (grid.y > 65535) return cudaErrorInvalidValue;
-  dist_tile_kernel<METRIC, EPI><<<grid, NT, 0, st>>>(X, ldx, n, C, ldc, m, d, out, ldo, best, col_base);
+  dist_tile_kernel<METRIC, EPI><<<grid, NT, 0, st>>>(X, ldx, n, C, ldc, m, d, out, ldo, best, col_base, cancel);
   note_launch();
   return cudaGetLastError();
 }
@@ -156,7 +184,7 @@ cudaError_t launch_tile(const float* X, int64_t ldx, int n, const float* C, int6
 }  // namespace
 
 cudaError_t launch_dist_matrix(const float* X, int64_t ldx, int n, const float* C, int64_t ldc, int m, int d,
-                               int metric, float* out, int64_t ldo, cudaStream_t st) {
+                               int metric, float* out, int64_t ldo, cudaStream_t st, CancelPoll cancel) {
   if ((d & 3) || (ldx & 3) || (ldc & 3)) return cudaErrorInvalidValue;
   // keep grid.y under 65535 rows of tiles
   const int max_rows = 65535 * BM;
@@ -164,9 +192,9 @@ cudaError_t launch_dist_matrix(const float* X, int64_t ldx, int n, const float* 
     int nr = n - r0 < max_rows ? n - r0 : max_rows;
     cudaError_t e = metric == kMetricL2
                         ? launch_tile<kMetricL2, EPI_WRITE>(X + (int64_t)r0 * ldx, ldx, nr, C, ldc, m, d,
-                                                            out + (int64_t)r0 * ldo, ldo, nullptr, 0, st)
+                                                            out + (int64_t)r0 * ldo, ldo, nullptr, 0, st, cancel)
                         : launch_tile<kMetricIP, EPI_WRITE>(X + (int64_t)r0 * ldx, ldx, nr, C, ldc, m, d,
-                                                            out + (int64_t)r0 * ldo, ldo, nullptr, 0, st);
+                                                            out + (int64_t)r0 * ldo, ldo, nullptr, 0, st, cancel);
     if (e != cudaSuccess) return e;
   }
   return cudaSuccess;

@@ -62,6 +62,7 @@ __global__ void __launch_bounds__(IVF_NT)
     ivfflat_scan_kernel(const float* __restrict__ xq, int64_t ldq, int d, const int32_t* __restrict__ probe_ids,
                         int nprobe, int nsplit, ListDirectory dir, IvfGeom g, int nst, int k, int KP, int SORTN,
                         FilterArgs f, unsigned long long* __restrict__ partial) {
+  if (cta_cancelled(f.cancel, kCsIvfflatScan)) return;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* stages = reinterpret_cast<float*>(smem_raw);
   float* qs = reinterpret_cast<float*>(smem_raw + (size_t)nst * g.stage_bytes);
@@ -229,6 +230,7 @@ __global__ void __launch_bounds__(IVF_NT)
     ivfflat_scan_warp_kernel(const float* __restrict__ xq, int64_t ldq, const int32_t* __restrict__ probe_ids,
                              int nprobe, int nsplit, int pg, ListDirectory dir, int R, int nst, int k, int KP, int SORTNW,
                              FilterArgs f, unsigned long long* __restrict__ partial) {
+  if (cta_cancelled(f.cancel, kCsIvfflatScanWarp)) return;
   constexpr int S = LPR * J;
   constexpr int RPW = 32 / LPR;  // rows per warp round
   constexpr int ROW_BYTES = S * 16;

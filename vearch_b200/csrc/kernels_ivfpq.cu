@@ -268,6 +268,7 @@ __global__ void __launch_bounds__(RR_NT)
     rerank_kernel(const unsigned long long* __restrict__ cand_keys, int ncand, int NP, const float* __restrict__ xq,
                   int64_t ldq, int d, const float* const* __restrict__ raw_segments, int seg_shift, int64_t ld_raw,
                   int k, int metric, FilterArgs f, unsigned long long* __restrict__ out_keys) {
+  if (cta_cancelled(f.cancel, kCsRerank)) return;  // before any candidate's row is read (DESIGN.md section 8)
   extern __shared__ __align__(16) unsigned char rr_smem[];
   unsigned long long* buf = reinterpret_cast<unsigned long long*>(rr_smem);  // [NP]
   float* qs = reinterpret_cast<float*>(buf + NP);                              // [d]
@@ -387,6 +388,7 @@ __global__ void __launch_bounds__(RR_NT)
                             int64_t shadow_stride, int cols16, int k, FilterArgs f,
                             unsigned long long* __restrict__ out_keys, int* __restrict__ survivors,
                             uint4* __restrict__ intervals) {
+  if (cta_cancelled(f.cancel, kCsRerankPrefilter)) return;
   extern __shared__ __align__(16) unsigned char rr_smem[];
   unsigned long long* buf = reinterpret_cast<unsigned long long*>(rr_smem);  // [NP] survivors' keys
   float* qs = reinterpret_cast<float*>(buf + NP);                              // [cols16], zero padded

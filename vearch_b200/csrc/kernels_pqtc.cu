@@ -453,6 +453,9 @@ __global__ void __launch_bounds__(PT_NT, 1)
   unsigned char* b_buf = a_buf + 4 * TILE;
   unsigned char* code_buf = b_buf + 2 * TILE;
 
+  // once per CTA, before the barriers and the warp roles: the roles walk the items on their own, so none may leave
+  // the schedule part way
+  if (cta_cancelled(f.cancel, kCsPqtcScan)) return;
   const int tid = threadIdx.x, warp = tid >> 5;
   const int64_t n_items = totals[1];
 
@@ -742,6 +745,7 @@ __global__ void __launch_bounds__(RS_NT)
                       const int* __restrict__ cand_cnt, const unsigned long long* __restrict__ cand, int cap,
                       const unsigned long long* __restrict__ keys_a, int64_t keys_a_stride, int kprime, int NP,
                       const int* __restrict__ row_limit, FilterArgs f, int sorted_out, unsigned long long* __restrict__ out) {
+  if (cta_cancelled(f.cancel, kCsPqRescore)) return;
   extern __shared__ __align__(16) unsigned char rs_smem[];
   unsigned long long* buf = reinterpret_cast<unsigned long long*>(rs_smem);  // [NP]
   float* ips = reinterpret_cast<float*>(buf + NP);                            // [M][256]

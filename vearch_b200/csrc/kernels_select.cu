@@ -25,6 +25,7 @@ template <bool KEYS_IN>
 __global__ void __launch_bounds__(SEL_NT)
     select_rows_kernel(const void* __restrict__ in, int64_t ld, int m, int64_t id_base, int k, int KP, int SORTN,
                        int metric, FilterArgs f, unsigned long long* __restrict__ out_keys, int64_t out_stride) {
+  if (cta_cancelled(f.cancel, kCsSelectRows)) return;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned long long* buf = reinterpret_cast<unsigned long long*>(smem_raw);
   __shared__ int s_cnt;

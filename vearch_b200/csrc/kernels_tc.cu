@@ -423,6 +423,7 @@ __global__ void __launch_bounds__(LW_NT, 1)
   extern __shared__ __align__(1024) unsigned char smem[];  // [ring][slabs][key sets: k * 1 KiB]
   __shared__ LwShared sh;
   if ((int64_t)blockIdx.x >= totals[1]) return;
+  if (cta_cancelled(f.cancel, kCsListmajorPipe)) return;
   const int tid = threadIdx.x, warp = tid >> 5;
   const LmTile t = items[blockIdx.x];
   const int row_end = t.row0 + t.nrows;
@@ -611,6 +612,7 @@ __global__ void __launch_bounds__(LT_NT, 1)
   extern __shared__ __align__(1024) unsigned char smem[];
   __shared__ LtShared sh;
   if ((int64_t)blockIdx.x >= totals[1]) return;
+  if (cta_cancelled(f.cancel, kCsListmajorTma)) return;
   constexpr int NST = LT_STAGES;
   constexpr int STAGE = TC_STAGE_BYTES;
   const int tid = threadIdx.x, warp = tid >> 5;
@@ -1160,6 +1162,7 @@ __global__ void __launch_bounds__(SEG_NT)
     seg_select_kernel(const float* __restrict__ scores, const int64_t* __restrict__ seg_off,
                       const int32_t* __restrict__ probe_ids, int nprobe, ListDirectory dir, int k, int KP, int SORTN,
                       FilterArgs f, unsigned long long* __restrict__ out_keys) {
+  if (cta_cancelled(f.cancel, kCsSegSelect)) return;
   extern __shared__ __align__(16) unsigned char sel_smem[];
   unsigned long long* buf = reinterpret_cast<unsigned long long*>(sel_smem);
   __shared__ int s_cnt;

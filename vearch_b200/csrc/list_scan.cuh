@@ -176,6 +176,7 @@ __global__ void __launch_bounds__(LS_NT, Codec::kMinCtasPerSm)
   // flag-gated launch (safety net of the tensor-core filter, kernels_pqtc.cu): only queries whose candidate list
   // overflowed are scanned
   if (gate_cnt && gate_cnt[q] <= gate_cap) return;
+  if (cta_cancelled(f.cancel, kCsListScan)) return;
   unsigned long long* out = partial + ((int64_t)q * gridDim.x + grp) * k;
   const int p0 = grp * pg;
   const int np = min(pg, nprobe - p0);

@@ -22,9 +22,61 @@ class GammaError(RuntimeError):
     pass
 
 
+class SearchKilled(GammaError):
+    """A search whose cancel token was set before it finished (the C-ABI's -2)."""
+
+
 def _check(rc, what):
+    if rc == -2:
+        raise SearchKilled(f"{what} killed")
     if rc != 0:
         raise GammaError(f"{what} failed (rc={rc}): {_lib.last_error()}")
+
+
+class CancelToken:
+    """One cancel word of a search (gb_cancel_token): set() stops the searches given it early, and they raise
+    SearchKilled.  It only ever goes from unset to set; one search at a time may hold it."""
+
+    def __init__(self):
+        self._h = _lib.lib().gb_cancel_token_create()
+        if not self._h:
+            raise GammaError(f"cancel token: {_lib.last_error()}")
+
+    def set(self):
+        _lib.lib().gb_cancel_token_set(self._h)
+
+    def is_set(self):
+        return bool(_lib.lib().gb_cancel_token_is_set(self._h))
+
+    def close(self):
+        if self._h:
+            _lib.lib().gb_cancel_token_free(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _token(cancel):
+    return None if cancel is None else C.c_void_p(cancel._h)
+
+
+def debug_cancel_stats(device=0):
+    """{kernel: CTAs that skipped their work on a set cancel word} on `device` since the last call, which clears them"""
+    p, n = C.c_void_p(), C.c_int()
+    _check(_lib.lib().gb_debug_cancel_stats(device, C.byref(p), C.byref(n)), "debug_cancel_stats")
+    js = C.string_at(p.value, n.value).decode()
+    C.CDLL(None).free(C.c_void_p(p.value))
+    return json.loads(js)
+
+
+def debug_cancel_register(request_id, partition_id, token, register=True):
+    """the kill registry behind SetKillStatus, with `token` standing in for a running search's cancel word"""
+    _check(_lib.lib().gb_debug_cancel_register(request_id.encode(), partition_id, C.c_void_p(token._h), int(register)),
+           "debug_cancel_register")
 
 
 def _f32(a):
@@ -167,8 +219,10 @@ class GammaIndex:
 
     # ---- search -------------------------------------------------------------------------
     def search(self, x, k, params=None, brute_force=False, del_bitmap=None, filter_bitmap=None, min_score=-FLT_MAX,
-               max_score=FLT_MAX):
-        """IndexModel::Search. Returns (scores[nq,k] float32, ids[nq,k] int64)."""
+               max_score=FLT_MAX, cancel=None, search_unindexed_tail=False):
+        """IndexModel::Search. Returns (scores[nq,k] float32, ids[nq,k] int64).  cancel: a CancelToken; the search
+        raises SearchKilled when it was set before the search finished.  search_unindexed_tail: enable_realtime's
+        brute-force pass over the stored rows not yet indexed."""
         x = _f32(x)
         assert x.ndim == 2 and x.shape[1] == self.d
         nq = x.shape[0]
@@ -180,16 +234,23 @@ class GammaIndex:
         for b in (db, fb):
             if b is not None:
                 bits = max(bits, b.size * 8)
-        rc = _lib.lib().gb_index_search(self._h, nq, _ptr(x), k, pj, int(brute_force), _ptr(db), _ptr(fb), bits,
-                                        C.c_float(min_score), C.c_float(max_score), _ptr(dis), _ptr(ids))
+        if cancel is None and not search_unindexed_tail:
+            rc = _lib.lib().gb_index_search(self._h, nq, _ptr(x), k, pj, int(brute_force), _ptr(db), _ptr(fb), bits,
+                                            C.c_float(min_score), C.c_float(max_score), _ptr(dis), _ptr(ids))
+        else:
+            rc = _lib.lib().gb_index_search_cancellable(self._h, nq, _ptr(x), k, pj, int(brute_force), _ptr(db), _ptr(fb),
+                                                        bits, C.c_float(min_score), C.c_float(max_score),
+                                                        int(search_unindexed_tail), _token(cancel), _ptr(dis), _ptr(ids))
         _check(rc, "search")
         return dis, ids
 
     def search_device(self, x, k, params=None, brute_force=False, out=None, del_bitmap=None, filter_bitmap=None,
-                      min_score=-FLT_MAX, max_score=FLT_MAX):
+                      min_score=-FLT_MAX, max_score=FLT_MAX, cancel=None):
         """Queries and results stay in HBM (torch CUDA tensors); asynchronous on torch's current stream.
         del_bitmap / filter_bitmap: CUDA uint8 tensors of one length on the index's device in search()'s layout
-        (LSB-first, bit set => deleted / allowed, ids past the bitmap neither), read on that stream."""
+        (LSB-first, bit set => deleted / allowed, ids past the bitmap neither), read on that stream.  cancel: a
+        CancelToken (without bitmaps or a score window); SearchKilled when it was set by the time the search was
+        enqueued, and the outputs are undefined when it is set later."""
         import torch
         assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1
         nq = x.shape[0]
@@ -198,6 +259,14 @@ class GammaIndex:
                    torch.empty((nq, k), dtype=torch.int64, device=x.device))
         pj = json.dumps(params).encode() if params else b""
         st = torch.cuda.current_stream(x.device).cuda_stream
+        if cancel is not None:
+            assert del_bitmap is None and filter_bitmap is None and min_score == -FLT_MAX and max_score == FLT_MAX
+            rc = _lib.lib().gb_index_search_device_cancellable(self._h, nq, C.c_void_p(x.data_ptr()), x.stride(0), k, pj,
+                                                               int(brute_force), _token(cancel),
+                                                               C.c_void_p(out[0].data_ptr()),
+                                                               C.c_void_p(out[1].data_ptr()), C.c_void_p(st))
+            _check(rc, "search_device")
+            return out
         if del_bitmap is None and filter_bitmap is None and min_score == -FLT_MAX and max_score == FLT_MAX:
             rc = _lib.lib().gb_index_search_device(self._h, nq, C.c_void_p(x.data_ptr()), x.stride(0), k, pj,
                                                    int(brute_force), C.c_void_p(out[0].data_ptr()),
@@ -600,7 +669,7 @@ class BinaryIVFIndex(GammaIndex):
         return self.get_vectors(vid, 1)[0]
 
     def search(self, x, k, params=None, brute_force=False, del_bitmap=None, filter_bitmap=None, min_score=-FLT_MAX,
-               max_score=FLT_MAX, search_unindexed_tail=False):
+               max_score=FLT_MAX, search_unindexed_tail=False, cancel=None):
         x = self._rows(x)
         nq = x.shape[0]
         dis = np.empty((nq, k), np.float32)
@@ -608,9 +677,10 @@ class BinaryIVFIndex(GammaIndex):
         pj = json.dumps(params).encode() if params else b""
         db, fb = _bitmap(del_bitmap), _bitmap(filter_bitmap)
         bits = max([b.size * 8 for b in (db, fb) if b is not None], default=0)
-        rc = _lib.lib().gb_index_search_binary(self._h, nq, _ptr(x), k, pj, int(brute_force), _ptr(db), _ptr(fb), bits,
-                                               C.c_float(min_score), C.c_float(max_score), int(search_unindexed_tail),
-                                               _ptr(dis), _ptr(ids))
+        rc = _lib.lib().gb_index_search_binary_cancellable(self._h, nq, _ptr(x), k, pj, int(brute_force), _ptr(db),
+                                                           _ptr(fb), bits, C.c_float(min_score), C.c_float(max_score),
+                                                           int(search_unindexed_tail), _token(cancel), _ptr(dis),
+                                                           _ptr(ids))
         _check(rc, "search_binary")
         return dis, ids
 
